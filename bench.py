@@ -76,7 +76,30 @@ def parse_args():
                     help="after the timed region, run the K rounds once more between two reads of this GPU's NVLink payload counters "
                          "(NVML) and report bytes per round next to the algorithmic count (config.nvlink)")
     ap.add_argument("--no-flush", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed rounds, write what the last one computed (global model, per-client losses) as DIR/<name>.npy")
     return ap.parse_args()
+
+
+DUMP_MAX_ELEMS = 8 * 1024 * 1024     # float32 elements per dumped array (32 MB); larger outputs are sampled
+
+
+def dump_outputs(out_dir: str, arrays) -> None:
+    """Write ``{name: tensor}`` as float32 ``out_dir/<name>.npy``.  An array above DUMP_MAX_ELEMS is replaced by the same
+    seeded sample of its elements every run (``<name>_sample``, ascending flat indices), so that two builds can be compared
+    output for output at any model size."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().float().reshape(-1).cpu()
+        if flat.numel() > DUMP_MAX_ELEMS:
+            gen = torch.Generator().manual_seed(0)
+            idx = torch.randperm(flat.numel(), generator=gen)[:DUMP_MAX_ELEMS].sort().values
+            np.save(os.path.join(out_dir, f"{name}_sample.npy"), flat[idx].numpy())
+        else:
+            np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 def make_data(model: str, total: int, rank: int, world: int, seed: int = 0):
@@ -359,7 +382,7 @@ def run_engine_config(args, name: str, rank: int, world: int, device, full: bool
     mask = None
     if select_k is not None and select_k < world:
         mask = (1 << select_k) - 1  # registration order = rank order ("first" policy)
-    flush_buf = None if args.no_flush else torch.empty(160 * 1024 * 1024 // 4, device=device)  # 160 MB > 126 MB L2
+    flush_buf = None if args.no_flush else torch.empty(160 * 1024 * 1024 // 4, device=device)  # 160 MB > the H100's 50 MB L2
 
     def max_over_ranks(v: float) -> float:
         t = torch.tensor([v], device=device, dtype=torch.float64)
@@ -390,6 +413,12 @@ def run_engine_config(args, name: str, rank: int, world: int, device, full: bool
         dist.barrier()
     clocks = sampler.stop()
     dev_ms = max_over_ranks(dev_ms)
+    if full and args.dump_outputs and rank == 0:
+        # the last timed round's results: the new global model and every client's (last, mean) local loss
+        outs = {"global_params": engine.global_flat()}
+        if rep.losses is not None:
+            outs["client_losses"] = rep.losses[-1]
+        dump_outputs(args.dump_outputs, outs)
     extra = dict(rep.extra)
     # K rounds enqueued in one call: no host in the loop, no flush (what a training of K rounds costs on the device)
     rep_p = engine.run_rounds(K, masks=mask)
@@ -479,25 +508,28 @@ def run_engine_config(args, name: str, rank: int, world: int, device, full: bool
         cfg["nvlink"] = nvlink
     if engine.algo == "twoshot":
         # roofline of the round (BASELINE.json: "the slower of its compute at peak and its bytes over NVLink at link bandwidth"):
-        # compute = the rank's local fit (MLP: 6 FLOP per parameter and sample) at the MEASURED bf16 matmul peak; link = the
+        # compute = the rank's local fit (MLP: 6 FLOP per parameter and sample) at the bf16 matmul peak (measured, from
+        # MEASURED_PEAKS.json when present, else the H100 SXM data sheet's dense figure; the record says which); link = the
         # all-reduce-with-broadcast of the arena through one GPU's NVLink port, (W-1)/W of the model per direction, fp32 in and
-        # fp32 + bf16 shadow out, at 900 GB/s per direction
+        # fp32 + bf16 shadow out, at 450 GB/s per direction (H100 SXM NVLink 4 data sheet)
         peaks = {}
         try:
             with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
                 peaks = json.load(f)
         except OSError:
             pass
-        peak_tflops = float(peaks.get("bf16_tflops", 1693.2))
+        peak_tflops = float(peaks.get("bf16_tflops", 989.4))
+        peak_source = "MEASURED_PEAKS.json" if "bf16_tflops" in peaks else "H100 SXM data sheet (dense bf16)"
         P = engine.P
         flops = 6.0 * P * n_local * epochs if model == "wide_mlp" else None
         out_bytes = P * (4 + (2 if engine.bf16_shadow else 0))
         link_bytes = (world - 1) / world * max(P * 4, out_bytes)
         t_compute = flops / (peak_tflops * 1e12) * 1e3 if flops else None
-        t_link = link_bytes / 900e9 * 1e3
+        t_link = link_bytes / 450e9 * 1e3
         bound = max(t_compute or 0.0, t_link)
         ms = dev_ms / K
-        cfg["roofline"] = {"compute_ms_at_measured_peak": t_compute, "peak_bf16_tflops": peak_tflops, "link_ms_at_900GBps_per_dir": t_link,
+        cfg["roofline"] = {"compute_ms_at_peak": t_compute, "peak_bf16_tflops": peak_tflops, "peak_bf16_source": peak_source,
+                           "link_ms_at_450GBps_per_dir": t_link,
                            "link_bytes_per_dir_per_gpu": int(link_bytes), "bound_ms": bound, "roofline_frac": (bound / ms) if bound else None,
                            "achieved_tflops_per_gpu": (flops / (ms * 1e-3) / 1e12) if flops else None,
                            "note": "frac = max(compute at peak, bytes at link rate) / measured round time"}
@@ -594,7 +626,7 @@ def run_torch_nccl(args, name: str, rank: int, world: int, device):
 def main() -> None:
     args = parse_args()
     if args.impl == "reference":
-        # the unmodified reference from baseline/_ref on its own stock path; nothing of this repo's package is imported
+        # the unmodified reference from oracle/_ref on its own stock path; nothing of this repo's package is imported
         sys.path.insert(0, os.path.join(ROOT, "baseline"))
         import reference_arm
         reference_arm.main(args)
@@ -627,7 +659,7 @@ def main() -> None:
         if default_line:
             # the default line is the config BOTH arms can run (the reference's own model and local-training path); BASELINE.json's
             # config 2 (MLP 10-64-64-2, n_k-weighted) is measured in the same process and attached, so the round-1 headline
-            # (BENCH_r01: cfg2) stays comparable
+            # (cfg2) stays comparable
             also = run_engine_config(args, "cfg2", rank, world, device, full=False)
             if out is not None and also is not None:
                 out["config"]["also_measured"] = {"cfg2": {k: also[k] for k in ("value", "unit", "ms_per_step", "e2e", "gpu_launches")}

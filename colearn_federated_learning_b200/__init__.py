@@ -1,4 +1,4 @@
-"""colearn_federated_learning_b200 — a Blackwell (sm_100a) native federated-averaging engine.
+"""colearn_federated_learning_b200 — a Hopper (sm_90a) native federated-averaging engine.
 
 Capabilities mirror CoLearn (aferaudo/CoLearn_Federated_Learning): publish/subscribe device
 admission (TRAINING / INFERENCE / NOT_READY), temporal-window worker collection, multi-round
@@ -11,7 +11,7 @@ Layer map (see DESIGN.md):
     fl/        FedAvg, local/remote/encrypted trainers, evaluate, inference
     models/    FFNN, TestingRemote, Net, MLP, WideMLP, ResNet-18 + flat-arena specs
     data/      NetworkTrafficDataset, transforms, federate(), synthetic UNSW generator
-    ops/       sm_100a kernels (persistent MLP local-SGD, tcgen05 GEMMs, losses, SGD, ...)
+    ops/       sm_90a kernels (persistent MLP local-SGD, wgmma GEMMs, losses, SGD, ...)
     parallel/  symmetric memory arena, fused broadcast / FedAvg-reduce kernels, round engine
     smpc/      fixed-point additive secret sharing (SPDZ-style) for the encrypted demo
     utils/     checkpoint, metrics, monitors, timing

@@ -1,4 +1,4 @@
-"""Reference-shaped API surface (``client_federated.py`` of CoLearn) on top of the B200 engine.
+"""Reference-shaped API surface (``client_federated.py`` of CoLearn) on top of the GPU engine.
 
 Keeps the names a CoLearn user knows — ``Net``, ``TestingRemote``, ``FFNN``, ``loss_fn``,
 ``train_local``, ``encrypted_training``, ``train_remote``, ``evaluate``,

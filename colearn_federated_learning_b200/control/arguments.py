@@ -34,7 +34,7 @@ class Arguments:
     weighted: bool = False         # False = uniform FedAvg (reference), True = n_k / sum(n)
     server_lr: float = 1.0         # theta <- theta + server_lr * avg_delta (1.0 = plain FedAvg)
     backend: str = "auto"          # auto | fused | nccl | cpu
-    dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the tcgen05 consumers)
+    dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the wgmma consumers)
     save_every: int = 0            # >0: checkpoint every N rounds, not only after the last one
     synthetic: int = 0             # >0: generate this many synthetic UNSW-shaped rows
     dataset: str = "unsw"          # data.DATASET_REGISTRY entry that reads test_path (user datasets: data.register_dataset)

@@ -6,7 +6,7 @@ CSV, keeps ``attack`` (label) + the 10 model features in the reference's column 
 ``(float32[10], float32[1])``.  Transforms ``ToTensor`` / ``Normalize`` / ``ToTensorLong``
 mirror ``datasets.py:60-89``.
 
-B200-first difference: in addition to the per-sample ``__getitem__`` protocol the dataset
+GPU-first difference: in addition to the per-sample ``__getitem__`` protocol the dataset
 exposes :meth:`tensors` — the whole shard as two dense tensors — because the training kernels
 consume a device-resident ``[N, F]`` matrix and a permutation, never a Python-level DataLoader.
 """

@@ -1,6 +1,6 @@
 """Local training of ResNet-18 on this repo's own kernels (BASELINE config 4, SURVEY K17).
 
-Every convolution is ``im2col`` + the tcgen05 GEMM (``ops.gemm_bf16``) in its three roles,
+Every convolution is ``im2col`` + the wgmma GEMM (``ops.gemm_bf16``) in its three roles,
 
     forward   z[M, Cout]      = col[M, K]      · Wp[Cout, K]ᵀ                      (M = N·OH·OW, k = (kh, kw, c))
     dgrad     dcol[M, K]      = dz[M, Cout]    · (Wpᵀ)[K, Cout]ᵀ   → col2im gather → dx
@@ -35,8 +35,7 @@ BF = torch.bfloat16
 PAD = 128
 
 # Step schedule.  Every entry is a re-scheduling / operand-layout choice with the same mathematical result.  The values
-# below are the fastest combination measured on a B200 (profiles/README.md, round 2: 1.87 ms -> 1.07 ms per batch-128
-# ResNet-18 step); 0 everywhere is the round-1 schedule (explicit im2col, K-major operands from transposed copies, one
+# below are the schedule the ResNet-18 step ships with; 0 everywhere is the round-1 schedule (explicit im2col, K-major operands from transposed copies, one
 # stream).  The environment (COLEARN_CONV_<NAME>=<int>) overrides in both directions, constructor arguments override
 # the environment.
 SCHEDULE_DEFAULTS = {
@@ -128,7 +127,7 @@ class ConvNetTrainer:
         (default: ``COLEARN_CONV_SPLITK=1``) runs the skinny GEMMs — the wgrads of the stem / layer1 / layer2 (1-5 output
         tiles, reductions over up to 32 768 pixels) and the forwards of layer3 / layer4 — in split-K mode, see
         :meth:`_pick_split` (``1`` / ``True``: wgrads only, ``2``: forwards too).  ``wgrad_mn`` (default:
-        ``COLEARN_CONV_WGRAD_MN=1``) feeds the wgrad GEMMs ``dz`` and ``col`` as they are (MN-major UMMA operands,
+        ``COLEARN_CONV_WGRAD_MN=1``) feeds the wgrad GEMMs ``dz`` and ``col`` as they are (MN-major wgmma operands,
         reduction over rows) instead of transposing both first; ``dgrad_kn`` (``COLEARN_CONV_DGRAD_KN=1``) lets the
         dgrad GEMMs read the packed weights ``Wp[Cout, K]`` as an MN-major B operand, so no ``Wᵀ`` copy is kept.
         ``implicit`` (``COLEARN_CONV_IMPLICIT=1|2``): the stride-1 3x3 convolutions whose images have 1-64 pixels (13 of
@@ -208,7 +207,7 @@ class ConvNetTrainer:
             off += cv.cout
         self._bound: Optional[nn.Module] = None
         self._model_ref = weakref.ref(model)
-        # opt-in (not yet measured on a B200): wgrad chains on a second stream, see _conv_bwd
+        # opt-in: wgrad chains on a second stream, see _conv_bwd
         self._side = torch.cuda.Stream(self.dev) if (self.dev.type == "cuda" and schedule_flag("STREAMS")) else None
         self._fuse_shadow_t = bool(schedule_flag("SHADOW_T"))
         # opt-in: BatchNorm reduction + finalize in one launch (ticket counter, last block finalises)
@@ -217,8 +216,8 @@ class ConvNetTrainer:
         self._graph = None
         self._graph_key = None
         z = lambda *s, dt=act_dtype: torch.zeros(*s, device=dev, dtype=dt)  # noqa: E731
-        # opt-in (not yet measured on a B200): split-K for the GEMMs with too few output tiles to fill 148 SMs
-        # opt-in (not yet measured on a B200): wgrad GEMMs on MN-major operands — no dz^T / col^T transposes
+        # opt-in: split-K for the GEMMs with too few output tiles to fill the SMs
+        # opt-in: wgrad GEMMs on MN-major operands — no dz^T / col^T transposes
         self._wgrad_mn = bool(schedule_flag("WGRAD_MN")) if wgrad_mn is None else bool(wgrad_mn)
         # opt-in: dgrad GEMMs against the packed weights themselves (MN-major B operand) — no W^T copies to refresh
         self._dgrad_kn = bool(schedule_flag("DGRAD_KN")) if dgrad_kn is None else bool(dgrad_kn)

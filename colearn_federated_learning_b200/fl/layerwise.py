@@ -1,7 +1,7 @@
-"""Layer-wise local training of wide MLPs on tcgen05 GEMMs (BASELINE config 5, SURVEY K7/K8/K12).
+"""Layer-wise local training of wide MLPs on wgmma GEMMs (BASELINE config 5, SURVEY K7/K8/K12).
 
 Every Linear of the wide MLP (10 → 4096×4 → 2) runs on ``ops.gemm_bf16`` — the hand-written
-tcgen05/TMEM/TMA kernel — in three roles that all reduce to ``C = A·Bᵀ`` with K-major operands:
+wgmma/TMA kernel — in three roles that all reduce to ``C = A·Bᵀ`` with K-major operands:
 
     forward   H_l  = relu(H_{l-1} · W_lᵀ + b_l)       A = H_{l-1}[B,in]   B = W_l[out,in]   (+bias, relu)
     dgrad     dZ_{l-1} = (dZ_l · W_l) ⊙ relu'          A = dZ_l[B,out]     B = W_lᵀ[in,out]  (+mask, +colsum = db)
@@ -50,7 +50,7 @@ class LayerwiseMLPTrainer:
     def supports(spec: MLPSpec, cfg) -> bool:
         """Any MLP with at least one hidden layer: widths that are not multiples of 128 are zero-padded (a padded hidden
         neuron has zero weights and bias, outputs relu(0) = 0 and receives a zero gradient through the ReLU mask), batches
-        that are not are padded with rows whose loss gradient is zero (:meth:`forward`), so the 128-row UMMA tiles always
+        that are not are padded with rows whose loss gradient is zero (:meth:`forward`), so the 128-row GEMM tiles always
         see full operands.  Losses: softmax cross-entropy on a linear head, BCE / SSE / MSE on a sigmoid or linear head."""
         hidden = spec.dims[1:-1]
         if len(hidden) < 1 or cfg.batch_size < 1:
@@ -87,7 +87,6 @@ class LayerwiseMLPTrainer:
         self._dz_rows = 0                                      # rows of dz[L-1] written since it was last all-zero
         # default (COLEARN_MLP_DGRAD_KN=0 restores the W^T copies): the dgrad reads W_l [out, in] in place as an MN-major B
         # operand (gemm_bf16(b_kn=True)), so no W^T copy exists: one 64 MB transpose pass per 4096 x 4096 layer and step less.
-        # Measured on a B200, cfg5 at N=1: 179.2 -> 205.5 rounds/s; with the in-place wgrad below 209.5 (profiles/README.md)
         self.dgrad_kn = (os.environ.get("COLEARN_MLP_DGRAD_KN", "1") == "1") if dgrad_kn is None else bool(dgrad_kn)
         # default (COLEARN_MLP_WGRAD_MN=0: transposed copies): the wgrad reads dz_l [B, out] and a_l [B, in] in place as MN-major
         # operands (gemm_bf16(mn_m=...)): no transposed activations / gradients are written by the producing epilogues
@@ -143,10 +142,9 @@ class LayerwiseMLPTrainer:
         return lo // chunk_elems, hi // chunk_elems
 
     def _refresh_t(self, l: int) -> None:
-        """Rebuild ``W_lᵀ`` from the bf16 shadow ``W_l`` (a 64 MB pass for a 4096 × 4096 layer: 20 µs, 19 % of the kernel time
-        of a wide-MLP round in the round-1 launch-time capture).  The copy is only needed by the NEXT dgrad, so the wgrad
-        merely marks it stale and the dgrad refreshes it on demand: the transposes behind the last step of a fit — dead
-        work, the next fit starts from ``refresh_exact`` — are never launched."""
+        """Rebuild ``W_lᵀ`` from the bf16 shadow ``W_l`` (a 64 MB pass for a 4096 × 4096 layer).  The copy is only needed
+        by the NEXT dgrad, so the wgrad merely marks it stale and the dgrad refreshes it on demand: the transposes behind
+        the last step of a fit — dead work, the next fit starts from ``refresh_exact`` — are never launched."""
         if not self.dgrad_kn:
             ops.transpose_bf16(self.Ws[l], self.WsT[l])
         self._wt_fresh[l] = True

@@ -8,8 +8,8 @@ small MLP family on a GPU, as ONE persistent-kernel launch (``ops.mlp_local_sgd`
 
 Three execution paths, chosen by :func:`local_fit`:
   * ``persistent``  FFNN / MLP / TestingRemote on CUDA → csrc/mlp_persistent.cu
-  * ``layerwise``   wide MLPs on CUDA → tcgen05 GEMMs + fused loss/SGD kernels (fl/layerwise.py)
-  * ``convnet``     ResNet-18 on CUDA → im2col + tcgen05 GEMMs + this repo's BatchNorm / pooling kernels
+  * ``layerwise``   wide MLPs on CUDA → wgmma GEMMs + fused loss/SGD kernels (fl/layerwise.py)
+  * ``convnet``     ResNet-18 on CUDA → im2col + wgmma GEMMs + this repo's BatchNorm / pooling kernels
                     (fl/convnet.py); ``COLEARN_CONV_PATH=torch`` selects the library path instead
   * ``torch``       anything else (every model on CPU; conv nets with a ragged last batch) → autograd loop
                     that still uses this repo's fused loss + flat SGD kernels where they apply.
@@ -189,7 +189,7 @@ def _library_path_guard(model: nn.Module, cfg: FitConfig, x: torch.Tensor) -> No
         what = (f"MLP {tuple(model.spec.dims)} with loss={cfg.loss!r}, batch_size={cfg.batch_size}" if isinstance(model, MLPNet) else
                 f"ResNet18 on input {tuple(x.shape)} with loss={cfg.loss!r}, batch_size={cfg.batch_size} "
                 "(the conv kernels need xent, batch_size % 128 == 0, shard size % batch_size == 0, images >= 32x32)")
-        raise RuntimeError(f"no sm_100a kernel path for {what}; refusing to fall back to autograd + cuBLAS/cuDNN on a CUDA tensor. "
+        raise RuntimeError(f"no sm_90a kernel path for {what}; refusing to fall back to autograd + cuBLAS/cuDNN on a CUDA tensor. "
                            "Set COLEARN_ALLOW_AUTOGRAD=1 (or COLEARN_CONV_PATH=torch for conv nets) to request the library path.")
     key = type(model).__name__
     if key not in _WARNED_LIBRARY_PATH:

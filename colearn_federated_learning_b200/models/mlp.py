@@ -7,7 +7,7 @@ production model, 2 401 params), ``TestingRemote`` 2-50-10-1 (``:37-48``, 671 pa
 exactly like the reference so ``test.pth`` files are interchangeable (SURVEY §2.7).
 
 Every model carries an :class:`MLPSpec` describing its layer dims, output activation and
-default loss.  The sm_100a kernels (``ops/``) consume the spec + a flat fp32 parameter arena
+default loss.  The sm_90a kernels (``ops/``) consume the spec + a flat fp32 parameter arena
 instead of the ``nn.Module``; the module form exists for CPU execution, checkpoints and as the
 numerics oracle in tests.
 """

@@ -4,7 +4,7 @@ Not present in the reference (SURVEY §2.5 K17).  Structure and state-dict keys 
 canonical ImageNet ResNet-18 (7x7 stem, max-pool, 4 stages of 2 BasicBlocks, global avg-pool,
 fc) so that with ``num_classes=10`` the parameter count is the 11 181 642 (+9 620 BN buffers)
 quoted in SURVEY §2.5.  This module is the architecture + state-dict definition (and the CPU /
-eval path); local training on a GPU runs through ``fl/convnet.py`` — im2col + tcgen05 GEMMs +
+eval path); local training on a GPU runs through ``fl/convnet.py`` — im2col + wgmma GEMMs +
 this repo's BatchNorm / pooling kernels — and the federated part (flat-arena broadcast, FedAvg
 reduce/apply, SGD, loss) through the comm / elementwise kernels.  BN running statistics are
 buffers and are *not* averaged by default, which is the reference FedAvg semantics (parameters

@@ -1,4 +1,4 @@
-"""Hot ops.  CUDA tensors → hand-written sm_100a kernels (``csrc/``); CPU tensors → ``reference``.
+"""Hot ops.  CUDA tensors → hand-written sm_90a kernels (``csrc/``); CPU tensors → ``reference``.
 
 There is deliberately no silent GPU fallback: a CUDA tensor with the extension missing raises.
 """

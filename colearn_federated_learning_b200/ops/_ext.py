@@ -1,8 +1,7 @@
-"""Loader for the in-tree sm_100a extension ``_colearn_C``.
+"""Loader for the in-tree sm_90a extension ``_colearn_C``.
 
 Policy: on a box with a GPU the extension is *mandatory* — :func:`require` raises if it is
-missing rather than silently running a PyTorch fallback (the driver records which ``.so`` files
-the GPU tests actually loaded).  On a CPU-only box :func:`available` is simply False and the
+missing rather than silently running a PyTorch fallback.  On a CPU-only box :func:`available` is simply False and the
 dispatchers in ``ops/__init__`` use ``ops.reference``.
 """
 from __future__ import annotations
@@ -58,5 +57,5 @@ def available() -> bool:
 def require():
     mod = load()
     if mod is None:
-        raise RuntimeError(f"colearn sm_100a extension is required on a CUDA device but could not be loaded: {_err!r}")
+        raise RuntimeError(f"colearn sm_90a extension is required on a CUDA device but could not be loaded: {_err!r}")
     return mod

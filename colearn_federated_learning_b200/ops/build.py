@@ -1,8 +1,8 @@
-"""In-tree build of the sm_100a extension (``_colearn_C*.so`` next to this file).
+"""In-tree build of the sm_90a extension (``_colearn_C*.so`` next to this file).
 
-``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` for every ``.cu`` (they do not include
+``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` for every ``.cu`` (they do not include
 torch headers, so each compiles in seconds), ``g++`` for ``bindings.cpp``, one link step.  The
-result is git-ignored but travels with the gpurun snapshot; ``__graft_entry__.build()`` calls
+result is git-ignored and stays in the source tree, so the package imports from it; ``__graft_entry__.build()`` calls
 :func:`build_all`.  Objects are cached under ``csrc/_obj`` keyed by source mtime+flags.
 """
 from __future__ import annotations
@@ -24,10 +24,10 @@ EMUL_NAME = "_colearn_emul"     # CPU emulator of the conv kernels (tests on box
 HOST_NAME = "_colearn_host"     # native CPU executor of the MLP local fit (devices / boxes without a GPU)
 SIMT_NAME = "_colearn_simt"     # the persistent-MLP CUDA kernels compiled for the CPU through csrc/host_shim.h (tests)
 
-CU_SOURCES = ["mlp_persistent.cu", "elementwise.cu", "comm.cu", "gemm_tcgen05.cu", "convnet.cu"]
+CU_SOURCES = ["mlp_persistent.cu", "elementwise.cu", "comm.cu", "gemm_wgmma.cu", "convnet.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3", "-lineinfo",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo",
               "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 # --use_fast_math would change expf/logf/division semantics in the loss kernels; keep IEEE there.
 NVCC_FLAGS.remove("--use_fast_math")
@@ -146,7 +146,7 @@ def build_simt_emul(force: bool = False) -> str:
                                                                         f"-DTORCH_EXTENSION_NAME={SIMT_NAME}"]
     sources = ["simt_emul.cpp", "simt_mlp.cpp", "simt_elementwise.cpp", "simt_comm.cpp", "simt_convnet.cpp", "simt_gemm.cpp"]
     h = hashlib.sha1()
-    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_v2.inc", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_tcgen05.cu", "tcgen05_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "conv_ops.cuh"]:
+    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_v2.inc", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "conv_ops.cuh"]:
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(cxx_flags).encode())
@@ -190,7 +190,7 @@ def build_all(force: bool = False, verbose: bool = True) -> str:
 
     if jobs:
         if verbose:
-            print(f"[colearn build] compiling {len(jobs)} translation unit(s) for sm_100a", file=sys.stderr)
+            print(f"[colearn build] compiling {len(jobs)} translation unit(s) for sm_90a", file=sys.stderr)
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as pool:
             list(pool.map(lambda j: _run(j[0], j[1]), jobs))
 

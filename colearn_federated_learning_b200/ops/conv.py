@@ -1,4 +1,4 @@
-"""NHWC convolution / BatchNorm / pooling ops around the tcgen05 GEMM (csrc/convnet.cu, SURVEY K17).
+"""NHWC convolution / BatchNorm / pooling ops around the wgmma GEMM (csrc/convnet.cu, SURVEY K17).
 
 Activations are NHWC flattened to a row-major bf16 matrix ``[M = N*H*W, C]``; a convolution is
 ``im2col`` (``k = (kh, kw, c)``) followed by ``ops.gemm_bf16``; the other ops are BatchNorm (training
@@ -7,7 +7,7 @@ between torch's ``[Cout, Cin, KH, KW]`` arena layout and the padded ``[Cout_pad,
 
 Three backends share one signature per op:
 
-* CUDA tensors  -> the hand-written sm_100a kernels (``_colearn_C``; mandatory on a GPU box);
+* CUDA tensors  -> the hand-written sm_90a kernels (``_colearn_C``; mandatory on a GPU box);
 * CPU tensors   -> the pure-PyTorch definitions in this file (the oracle the kernels are tested against);
 * CPU tensors inside :func:`emulated` -> ``_colearn_emul``: the *kernel bodies themselves* (``csrc/conv_ops.cuh``)
   compiled for the host, so the index arithmetic of every kernel is exercised by the CPU test-suite.
@@ -413,7 +413,7 @@ def conv_gemm(kind: str, act: torch.Tensor, other: torch.Tensor, n: int, h: int,
     * ``"wgrad"`` ``dW[co, tap·c + ·] = Σ_p other[p, co]·act[p + tap − pad, ·]`` — ``other`` = dz ``[pixels, Cout]``; the
       result (``[m_pad, k_pad]``, K padding = zeros) goes through the fused SGD epilogue or the split-K partials.
 
-    CPU tensors use the PyTorch definitions (``im2col`` / ``col2im`` + the reference GEMM), CUDA the tcgen05 kernel."""
+    CPU tensors use the PyTorch definitions (``im2col`` / ``col2im`` + the reference GEMM), CUDA the wgmma kernel."""
     from .linear import gemm_bf16
     m = n * h * w
     taps = kh * kw
@@ -427,7 +427,7 @@ def conv_gemm(kind: str, act: torch.Tensor, other: torch.Tensor, n: int, h: int,
             geom = [1, 0, c, kh, kw, pad, h, w, n, 0, m, out_bf16.shape[1] if out_bf16 is not None else other.shape[0], taps * c, 0]
         else:
             geom = [1, 1, c, kh, kw, pad, h, w, n, rows_per_tap, m, rows_per_tap, taps * c, 1 if w_packed else 0]
-        if simt_mod is not None:   # the kernel source on the functional tcgen05 / TMA model (csrc/tcgen05_host_model.h)
+        if simt_mod is not None:   # the kernel source on the functional wgmma / TMA model (csrc/gemm_host_model.h)
             mod.gemm_tcgen05(act, other, None, False, None, out_bf16, None, None, sgd_master, float(sgd_lr), sgd_shadow, None, None,
                              0, int(split_k or 0), split_out, 0, False, addend, geom, [])
             return

@@ -1,4 +1,4 @@
-// Torch bindings for the colearn sm_100a kernels.  Only this translation unit sees torch headers.
+// Torch bindings for the colearn sm_90a kernels.  Only this translation unit sees torch headers.
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -455,7 +455,7 @@ void produced_mark(int64_t sig, int64_t chunk_elems, int64_t lo, int64_t hi) {
   check(launch_produced_mark(ptr_of<const ProducedSignal>(sig), shift, lo, hi, cur_stream()), "produced_mark");
 }
 
-// ---- tcgen05 GEMM -----------------------------------------------------------------------------------------
+// ---- wgmma GEMM ------------------------------------------------------------------------------------------
 void gemm_tcgen05(torch::Tensor A, torch::Tensor B, c10::optional<torch::Tensor> bias, bool relu,
                   c10::optional<torch::Tensor> relu_mask, c10::optional<torch::Tensor> out_bf16,
                   c10::optional<torch::Tensor> out_f32, c10::optional<torch::Tensor> out_bf16_t,
@@ -572,7 +572,7 @@ struct ConvCudaExec {
 #include "conv_bindings.inc"
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "colearn_federated_learning_b200 sm_100a kernels";
+  m.doc() = "colearn_federated_learning_b200 sm_90a kernels";
   m.def("make_client_desc", &make_client_desc);
   m.def("set_spin_limit", &set_spin_limit);
   m.def("scale_inplace", &scale_inplace);

@@ -1,4 +1,4 @@
-// Shared declarations between the sm_100a kernels (.cu) and the torch bindings (bindings.cpp).
+// Shared declarations between the sm_90a kernels (.cu) and the torch bindings (bindings.cpp).
 // The .cu files deliberately do NOT include torch headers: they compile in seconds and expose
 // plain C++ launchers taking raw pointers + a cudaStream_t.
 #pragma once
@@ -31,7 +31,7 @@
 
 #include <cstdlib>
 namespace colearn {
-// Programmatic dependent launch is ON unless COLEARN_PDL=0 (measured: ResNet-18 step 1.069 -> 0.974 ms, bit-identical results)
+// Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
 inline bool pdl_enabled() {
   static const bool on = [] { const char* e = std::getenv("COLEARN_PDL"); return !(e != nullptr && e[0] == '0'); }();
   return on;
@@ -369,7 +369,7 @@ cudaError_t launch_p2p_copy(float* dst, const float* src, int64_t n, uint32_t* f
                             uint32_t flag_value, int n_blocks, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 GEMM family (gemm_tcgen05.cu):  C[M,N] = A[M,K] * B[N,K]^T  (both operands K-major bf16)
+// wgmma GEMM family (gemm_wgmma.cu):  C[M,N] = A[M,K] * B[N,K]^T  (both operands K-major bf16)
 // ---------------------------------------------------------------------------------------------
 struct GemmEpilogue {
   const float* bias;        // [N] or nullptr
@@ -395,8 +395,8 @@ struct GemmEpilogue {
   int64_t ready_chunk_elems;
   int64_t ready_elem_offset;
   int tile_n;               // 0 = auto, 128 or 256 = force the N tile width
-  int cluster;              // 3 = cta_group::2 (two SMs per 256x256 tile, UMMA M=256; needs M%256==0, N%256==0);
-                            // 2 = pairs of CTAs + TMA multicast of the shared B tile (M%256==0, tile 256); else off
+  int cluster;              // 2 (or 3) = pairs of CTAs on a 256x256 block + TMA multicast of the shared B tile
+                            // (needs M%256==0, N%256==0); else off
   // split-K (skinny problems: few output tiles, long reduction — the conv wgrads): the K range of every output tile
   // is cut into split_k slices that run as independent work units; slice s stores its raw fp32 accumulator to
   // split_out[s, M, N] and NO other epilogue op runs (launch_splitk_reduce sums the slices and applies the epilogue:
@@ -414,7 +414,7 @@ struct GemmEpilogue {
   int64_t produced_elem_offset;
   int max_ctas;             // > 0: cap the persistent grid (leave SMs to a communication kernel running next to the GEMM)
   int pdl;                  // 1: launched with the programmatic-dependent-launch attribute; the kernel runs COLEARN_PDL_PROLOGUE
-                            // after its own set-up (barrier init, TMEM allocation, tensor-map prefetch overlap the predecessor)
+                            // after its own set-up (barrier init and tensor-map prefetch overlap the predecessor)
 };
 // A: [M,K] bf16 row-major, B: [N,K] bf16 row-major.  M%128==0, N%128==0, K%64==0.
 cudaError_t launch_gemm_tcgen05(const void* A, const void* B, int M, int N, int K,

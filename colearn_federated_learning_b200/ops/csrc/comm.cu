@@ -661,7 +661,7 @@ COLEARN_DEFINE_SPIN_LIMIT_SETTER(set_spin_limit_comm)
 // CUDA loads a kernel's code lazily at its first launch, and that load can need the device to be idle.  Kernels of this file
 // spin on flags that OTHER kernels raise (the overlapped two-shot waits for the last backward pass' reports; the workers wait
 // for the coordinator's broadcast), so a kernel that is launched for the first time while a spinning kernel is resident can
-// deadlock the device (seen on a B200: the first produced_mark_kernel next to twoshot_overlap_kernel).  Touching the function
+// deadlock the device (e.g. the first produced_mark_kernel next to twoshot_overlap_kernel).  Touching the function
 // attributes forces the load; the engine calls this once per device before any round.
 cudaError_t preload_comm_kernels() {
 #ifndef COLEARN_HOST_SHIM

@@ -7,7 +7,7 @@
 //
 // Layout: activations are NHWC flattened to a row-major matrix [M = N*H*W, C] of bf16; a convolution is
 //   im2col (k = (kh, kw, c), so 8 consecutive k are 8 consecutive channels = one 16-byte load)
-//   -> tcgen05 GEMM  z[M, Cout] = col[M, K] * Wp[Cout, K]^T        (gemm_tcgen05.cu)
+//   -> wgmma GEMM    z[M, Cout] = col[M, K] * Wp[Cout, K]^T        (gemm_wgmma.cu)
 //   -> BatchNorm statistics / apply (+ residual, + ReLU).
 // Backward: BatchNorm backward -> dgrad GEMM dcol = dz * (Wp^T)^T -> col2im gather (no atomics), and the
 // wgrad GEMM dz^T * col^T with the SGD step fused in its epilogue.
@@ -495,8 +495,8 @@ CL_HD void pack_body(const PackArgs& a, long long e) {
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Work decomposition of the persistent tcgen05 GEMM (gemm_tcgen05.cu).  Every role of a CTA (TMA producer, MMA issuer,
-// epilogue warps) walks the same list: work unit w = blockIdx.x, blockIdx.x + gridDim.x, ...;  w / S is the output tile,
+// Work decomposition of the persistent wgmma GEMM (gemm_wgmma.cu).  Every role of a CTA (TMA producer, consumer
+// warpgroups) walks the same list: work unit w = blockIdx.x, blockIdx.x + gridDim.x, ...;  w / S is the output tile,
 // w % S the K slice (S = split_k, 1 = off).  Host+device so that the CPU test-suite can check that the units tile the
 // output exactly once and that the slices partition K.
 // L2-friendly rasterisation: the tiles are walked in groups of kGroupM m-units x all n-blocks (m fastest inside a group),
@@ -581,8 +581,8 @@ CL_HD ConvBox conv_nblock(const ConvAddr& g, int blk, int kb) {
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Split-K reduction: the tcgen05 GEMM in split-K mode leaves S raw fp32 partial accumulators part[s, rows, cols]
-// (gemm_tcgen05.cu, GemmEpilogue::split_k); this map sums them in slice order (deterministic) and applies the
+// Split-K reduction: the wgmma GEMM in split-K mode leaves S raw fp32 partial accumulators part[s, rows, cols]
+// (gemm_wgmma.cu, GemmEpilogue::split_k); this map sums them in slice order (deterministic) and applies the
 // epilogue the un-split GEMM would have fused:
 //   master != null : fused SGD of the wgrad GEMMs  master -= lr * sum ; shadow = bf16(master)
 //   else           : out_bf16 = bf16(sum)          (conv forward: the next activation matrix)

@@ -1,4 +1,4 @@
-// NHWC convolution / BatchNorm / pooling kernels around the tcgen05 GEMM (SURVEY K17: ResNet-18 ops).
+// NHWC convolution / BatchNorm / pooling kernels around the wgmma GEMM (SURVEY K17: ResNet-18 ops).
 // The arithmetic of every kernel is the host+device body in conv_ops.cuh; this file only maps bodies onto
 // grids: grid-stride maps (128-bit loads/stores, one work item = 8 channels) and two-phase block reductions.
 #include "colearn_kernels.h"
@@ -10,7 +10,7 @@ namespace {
 constexpr int kMapThreads = 256;
 inline int map_grid(long long items) {
   long long b = (items + kMapThreads - 1) / kMapThreads;
-  const long long cap = 148LL * 16;            // 16 resident 256-thread CTAs per SM is already more than enough
+  const long long cap = 132LL * 16;            // 16 resident 256-thread CTAs per SM is already more than enough
   if (b > cap) b = cap;
   if (b < 1) b = 1;
   return (int)b;

@@ -1,6 +1,6 @@
 // Memory-bound kernels: SGD step, FedAvg on flat arenas, fused loss fwd+bwd, eval, argmax,
 // min-max scaling, keyed permutation, dtype conversion.  All are single-pass, 128-bit vectorised
-// where alignment allows, and sized as a persistent grid (148 SMs x 8 CTAs) with grid-stride loops.
+// where alignment allows, and sized as a persistent grid (132 SMs of an H100 SXM x 8 CTAs) with grid-stride loops.
 //
 // Parity map (SURVEY §2.5b): K9 sigmoid+BCE (client_federated.py:65,79), K10 softmax-xent (BASELINE
 // 2-logit configs), K11 SSE (cf.py:112,158), K12 SGD (fc.py:355; cf.py:206-207), K13 MinMax
@@ -17,7 +17,7 @@ namespace {
 constexpr int kThreads = 256;
 inline int grid_for(int64_t n, int per_thread = 4) {
   int64_t b = (n + (int64_t)kThreads * per_thread - 1) / ((int64_t)kThreads * per_thread);
-  const int64_t cap = 148 * 8;
+  const int64_t cap = 132 * 8;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
   return (int)b;
@@ -209,7 +209,7 @@ __global__ void softmax_xent_kernel(const void* __restrict__ logits_, const int6
 // Loss head of the GEMM-shaped trainers in ONE launch and ONE block: softmax cross-entropy of the valid rows / columns of a PADDED
 // fp32 (or bf16) logits matrix, dL/dlogits written straight into the padded bf16 operand of the backward GEMMs (and / or an fp32
 // matrix), the head's bias gradient (column sums of dL/dlogits) and the mean loss.  Replaces slice-copy + loss + cast-copy +
-// at::sum + copy (three ATen launches, one of them an 18 us single-block reduction) around the old kernel.  One block, fixed
+// at::sum + copy (three ATen launches, one of them a single-block reduction) around the old kernel.  One block, fixed
 // summation order: bit-reproducible, no memset, no atomics.  cols <= kHeadMaxCols.
 constexpr int kHeadMaxCols = 128;
 template <bool BF16_IN>
@@ -474,7 +474,7 @@ cudaError_t launch_softmax_xent(const void* logits, int is_bf16, const int64_t* 
   if (e != cudaSuccess) return e;
   const int wpb = kThreads / 32;
   int blocks = (rows + wpb - 1) / wpb;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (blocks < 1) blocks = 1;
   if (is_bf16)
     COLEARN_LAUNCH(softmax_xent_kernel<true>, blocks, kThreads, 0, s, logits, labels, dl, reinterpret_cast<__nv_bfloat16*>(dl_bf16), loss_out, rows, cols);
@@ -505,7 +505,7 @@ cudaError_t launch_eval_binary(const float* p, const float* y, float* loss_sum, 
 cudaError_t launch_argmax_rows(const float* x, int64_t* out, int rows, int cols, cudaStream_t s) {
   const int wpb = kThreads / 32;
   int blocks = (rows + wpb - 1) / wpb;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (blocks < 1) blocks = 1;
   COLEARN_LAUNCH(argmax_rows_kernel, blocks, kThreads, 0, s, x, out, rows, cols);
   return cudaGetLastError();
@@ -547,7 +547,7 @@ cudaError_t launch_bias_sgd_from_partials(float* bias, const float* partials, in
   return cudaGetLastError();
 }
 cudaError_t launch_l2_flush(float* buf, int64_t n, cudaStream_t s) {
-  COLEARN_LAUNCH(l2_flush_kernel, 148 * 8, kThreads, 0, s, buf, n);
+  COLEARN_LAUNCH(l2_flush_kernel, 132 * 8, kThreads, 0, s, buf, n);
   return cudaGetLastError();
 }
 

@@ -57,13 +57,14 @@ struct Block {
   std::vector<std::unique_ptr<std::barrier<>>> warp_bar;
   std::vector<unsigned long long> slots;   // one 8-byte exchange slot per lane
   std::vector<float> dyn;                  // dynamic shared memory (16-byte aligned start, see dyn_smem())
-  // per-block scratch outside shared memory (the tcgen05 model keeps the CTA's tensor memory here)
-  float* scratch(size_t n) {
-    std::call_once(scratch_once, [&] { scratch_buf.assign(n, 0.f); });
-    return scratch_buf.data();
+  // named barriers (bar.sync id, count): created by the first thread that reaches one
+  std::barrier<>* named(int id, int count) {
+    std::lock_guard<std::mutex> lock(named_mu);
+    if (!named_bar[id & 15]) named_bar[id & 15] = std::make_unique<std::barrier<>>(count);
+    return named_bar[id & 15].get();
   }
-  std::once_flag scratch_once;
-  std::vector<float> scratch_buf;
+  std::mutex named_mu;
+  std::unique_ptr<std::barrier<>> named_bar[16];
 };
 
 inline thread_local Dim3 t_threadIdx;
@@ -77,6 +78,7 @@ inline float* dyn_smem() {
 
 inline void syncthreads() { t_block->bar.arrive_and_wait(); }
 inline void syncwarp() { t_block->warp_bar[t_linear / 32]->arrive_and_wait(); }
+inline void named_barrier(int id, int count) { t_block->named(id, count)->arrive_and_wait(); }
 
 template <class T>
 inline T shfl_from(T v, int src_lane) {

@@ -6,7 +6,7 @@
 // PyTorch definitions in ops/reference.py (~200 us per step of op-dispatch overhead for a 5 k-MAC network).  This file
 // is the same fit — shuffled batches, forward, loss, backward, SGD, max_nr_batches — as one C++ loop on the flat fp32
 // arena, with K clients trained concurrently on K threads (the GIL is released).  Semantics are those of
-// ops/reference.py::mlp_local_sgd / loss_and_dz (tests compare the two); the sm_100a persistent kernel
+// ops/reference.py::mlp_local_sgd / loss_and_dz (tests compare the two); the sm_90a persistent kernel
 // (mlp_persistent.cu) is the GPU counterpart.  Built with g++ only (ops/build.py::build_host), links the CPU libtorch.
 #include <torch/extension.h>
 

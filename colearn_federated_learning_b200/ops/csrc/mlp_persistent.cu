@@ -4,7 +4,7 @@
 // C27, triggered at client_federated.py:210): for every batch { zero_grad; forward; loss;
 // backward; SGD step } — ~15 tiny ATen kernels per step, 1000-3000 dependent steps per round.
 //
-// B200 design: the networks in play (FFNN 10-50-30-10-1, MLP 10-64-64-2, TestingRemote
+// Design: the networks in play (FFNN 10-50-30-10-1, MLP 10-64-64-2, TestingRemote
 // 2-50-10-1) have <= 5k parameters, so the *entire model lives in shared memory* for the whole
 // fit and one CTA walks the dependent SGD steps with no global-memory traffic other than the
 // streamed samples.  Batch-1 sequential SGD is inherently serial (SURVEY §7.3-2): tensor cores
@@ -426,8 +426,8 @@ mlp_local_sgd_kernel(const ClientDesc* __restrict__ descs, SgdHyper hp) {
 // =====================================================================================================
 // v2: register-resident weights.
 //
-// ncu on v1 (profiles/r1_call1_*): 3 300 cycles/step, issue slots 20 % busy, stalls dominated by
-// short_scoreboard (smem weight reads / read-modify-write updates) and barriers.  v2 removes shared
+// v1 keeps the weights in shared memory, so its step waits on shared-memory weight reads / read-modify-write updates
+// and on barriers.  v2 removes shared
 // memory from the weight path entirely: every thread keeps, in registers and for the whole fit,
 //   wr[KC]  its slice of row n of W_l       (forward + update, (neuron n, lane t) mapping)
 //   wt[NC]  its slice of column k of W_l    (dgrad,            (input  k, lane t') mapping)
@@ -448,7 +448,7 @@ mlp_local_sgd_kernel(const ClientDesc* __restrict__ descs, SgdHyper hp) {
 #undef V2_BLOCKED
 #undef V2_NS
 #undef V2_NT
-// the blocked kernel with packed fp32 math (fma.rn.f32x2 / SASS FFMA2; see the V2_PACKED comment in mlp_v2.inc)
+// the blocked kernel with its FMAs written in pairs (see the V2_PACKED comment in mlp_v2.inc)
 #define V2_NS v2_128p
 #define V2_NT 128
 #define V2_BLOCKED 1
@@ -524,7 +524,7 @@ cudaError_t forward_t(const float* theta, const float* x, float* out, int n, cud
     if (e != cudaSuccess) return e;
     configured[dev & 63] = true;
   }
-  int blocks = n < 148 * 2 ? n : 148 * 2;
+  int blocks = n < 132 * 2 ? n : 132 * 2;   // H100 SXM: 132 SMs
   if (blocks < 1) blocks = 1;
   COLEARN_LAUNCH(mlp_forward_kernel<N>, blocks, NT, bytes, stream, theta, x, out, n);
   return cudaGetLastError();
@@ -535,9 +535,8 @@ cudaError_t forward_t(const float* theta, const float* x, float* out, int n, cud
 cudaError_t launch_mlp_local_sgd(int net_kind, const ClientDesc* descs, int n_clients, SgdHyper hp,
                                  cudaStream_t stream) {
   // variant 5 (default, set by ops/fused_mlp.py): register-resident weights, 128-thread CTA, blocked reduction slices
-  // (LDS.128) + pre-scaled dz: 0.665 us/step (MLP 10-64-64-2) / 0.717 (FFNN) on a B200; 3: the same kernel with strided
-  // slices (the round-1 default: 0.699 / 0.795); 1: first version with smem-resident weights (1.66).  The 256-thread
-  // (0.83) and 64-thread (0.77) CTA shapes lost the A/B runs and were removed (profiles/README.md).
+  // (LDS.128) + pre-scaled dz; 6: the same with its FMAs written in pairs; 3: the same kernel with strided slices;
+  // 1: first version with smem-resident weights.
   if (hp.variant == 6) {
     switch (net_kind) {
       case NET_FFNN: return v2_128p::launch2<FFNNNet>(descs, n_clients, hp, stream);

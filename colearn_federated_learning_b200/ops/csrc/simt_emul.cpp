@@ -287,7 +287,7 @@ void produced_mark(int64_t sig, int64_t chunk_elems, int64_t lo, int64_t hi) {
   CK(colearn::launch_produced_mark(reinterpret_cast<const colearn::ProducedSignal*>(static_cast<uintptr_t>(sig)), shift, lo, hi, nullptr));
 }
 
-// ---- gemm_tcgen05.cu on the functional tcgen05 / TMA / mbarrier model (tcgen05_host_model.h) ---------------------------------
+// ---- gemm_wgmma.cu on the functional wgmma / TMA / mbarrier model (gemm_host_model.h) -------------------------------------
 // Same argument meaning as bindings.cpp::gemm_tcgen05 (minus the cross-GPU ready flags and the cluster modes).
 void gemm_tcgen05(Tensor A, Tensor B, c10::optional<Tensor> bias, bool relu, c10::optional<Tensor> relu_mask, c10::optional<Tensor> out_bf16,
                   c10::optional<Tensor> out_f32, c10::optional<Tensor> out_bf16_t, c10::optional<Tensor> sgd_master, double sgd_lr,

@@ -139,7 +139,7 @@ int main() {
     CK(launch_bn_reduce_finalize(fb, nullptr));
   }
   printf("conv kernels ok\n");
-  // ---- tcgen05 GEMM on the functional model: the TMA -> MMA -> epilogue pipeline is ordered by mbarriers only -------------------
+  // ---- wgmma GEMM on the functional model: the TMA -> MMA -> epilogue pipeline is ordered by mbarriers only -------------------
   {
     auto bf = [](size_t n) { std::vector<__nv_bfloat16> v(n); for (auto& x : v) x = __float2bfloat16(frand() - 0.5f); return v; };
     GemmEpilogue ep;

@@ -23,16 +23,11 @@ NET_KINDS = {
 }
 LOSS_CODES = {"bce": 0, "sse": 1, "xent": 2, "mse": 3}
 # Kernel variants: 5 = register-resident weights, 128-thread CTA, blocked reduction slices (LDS.128) + pre-scaled dz;
-# 6 = 5 with packed fp32 math (fma.rn.f32x2 -> SASS FFMA2); 3 = strided slices (the round-1 default); 1 = smem-resident
-# weights (first version).  Measured on a B200 (us per batch-1 SGD step, profiles/README.md R2.9: the head's sigmoid on single
-# MUFU instructions, loss value without a divergent branch, narrow heads held whole in every lane, the FFNN's 30 -> 10 layer
-# computed per warp):
-#                   v1      v3      v5      v6
-#   MLP 10-64-64-2  1.646   0.670   0.624   0.579     <- 64-wide layers: every dot product / update is FFMA2-shaped
-#   FFNN            1.627   0.668   0.616   0.577     <- (was 0.711 / 0.716 before those four changes)
-# 0 (default) picks the fastest measured variant per net.
+# 6 = 5 with its FMAs written in pairs (Hopper has no packed fp32 FMA: the same FFMA sequence as 5); 3 = strided slices
+# (the round-1 default); 1 = smem-resident weights (first version).
+# 0 (default) picks variant 5 for every net.
 KERNEL_VARIANT = int(__import__("os").environ.get("COLEARN_MLP_VARIANT", "0"))
-BEST_VARIANT = {0: 6, 1: 6, 2: 5}          # net kind (NET_KINDS values) -> variant
+BEST_VARIANT = {0: 5, 1: 5, 2: 5}          # net kind (NET_KINDS values) -> variant
 
 
 def resolve_variant(kind: int, variant: Optional[int] = None) -> int:

@@ -1,6 +1,6 @@
-"""tcgen05 GEMM front-end (csrc/gemm_tcgen05.cu) — SURVEY K7/K8.
+"""wgmma GEMM front-end (csrc/gemm_wgmma.cu) — SURVEY K7/K8.
 
-``C[M,N] = A[M,K] · B[N,K]^T`` with both operands K-major bf16, fp32 accumulation in TMEM and a
+``C[M,N] = A[M,K] · B[N,K]^T`` with both operands K-major bf16, fp32 accumulation in registers and a
 fused epilogue (bias / ReLU / ReLU-mask / fp32+bf16+transposed outputs / fused SGD / bias-grad
 column sums / fused broadcast-consumption flags).  Shapes must satisfy ``M%128 == N%128 == 0``
 and ``K%64 == 0``; callers pad (see ``fl/layerwise.py``).  CPU tensors use the fp32 reference.
@@ -24,7 +24,7 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, *, bias: Optional[torch.Tensor] 
               ready_epoch_ptr: int = 0, cluster: int = 0, split_k: int = 0,
               split_out: Optional[torch.Tensor] = None, mn_m: int = 0, b_kn: bool = False,
               addend: Optional[torch.Tensor] = None, produced=None, max_ctas: int = 0) -> None:
-    """Launch the tcgen05 GEMM; results land in the provided output tensors.
+    """Launch the wgmma GEMM; results land in the provided output tensors.
 
     ``mn_m = M > 0`` selects the "MN-major" form ``C[M, N] = Aᵀ·B`` for ``a[K, a_cols]`` (``a_cols <= M``, the missing
     columns count as zeros) and ``b[K, N]``, both row-major: the reduction runs over *rows*, which is how the conv
@@ -50,7 +50,7 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, *, bias: Optional[torch.Tensor] 
         if produced[0].sig is not None:
             prod_arg = produced[0].gemm_arg(produced[1])
     from . import conv as _conv
-    # tests (ops.conv.simt()): CPU bf16 operands go to the kernel SOURCE on the functional tcgen05 / TMA / mbarrier model
+    # tests (ops.conv.simt()): CPU bf16 operands go to the kernel SOURCE on the functional wgmma / TMA / mbarrier model
     simt_mod = (_conv._EMUL["mod"] if (not a.is_cuda and _conv._EMUL["on"] and hasattr(_conv._EMUL["mod"], "gemm_tcgen05")
                                        and a.dtype == torch.bfloat16 and not ready_flags and not cluster) else None)
     if mn_m:

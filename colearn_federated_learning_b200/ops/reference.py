@@ -1,6 +1,6 @@
 """Plain-PyTorch fp32 definitions of every op in ``ops/`` .
 
-Two jobs: (1) the numerics oracle each sm_100a kernel is tested against, (2) the CPU execution
+Two jobs: (1) the numerics oracle each sm_90a kernel is tested against, (2) the CPU execution
 path (BASELINE config 1 runs with no GPU; multi-process CPU tests run over gloo).  Nothing here
 is on the GPU hot path — on a CUDA box the dispatchers in ``ops/__init__`` refuse to fall back
 to these silently.

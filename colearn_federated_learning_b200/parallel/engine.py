@@ -117,8 +117,7 @@ class FederatedEngine:
         self.use_graphs = os.environ.get("COLEARN_CUDA_GRAPHS", "1") != "0"
         # multimem.ld_reduce / multimem.st in the two-shot kernel.  Through the switch every GPU sends its whole vector once (each
         # element is pulled by its owner's ld_reduce) plus its reduced share once, and receives the same: (1 + 1/W) x model bytes
-        # per direction, against 2 (W-1)/W x for peer loads + peer stores.  The GPUs' own NVLink counters agree (profiles/
-        # r2_nvlink_counters.json: W=2 1.50 x vs 1.00 x, and 0.57 vs 0.36 ms for 201 MB), so "auto" takes the switch from W = 4 up
+        # per direction, against 2 (W-1)/W x for peer loads + peer stores (W=2: 1.50 x vs 1.00 x), so "auto" takes the switch from W = 4 up
         nvls_env = os.environ.get("COLEARN_NVLS", "auto")
         self.use_nvls = nvls_env == "1" or (nvls_env not in ("0", "1") and self.world >= 4)
         # fused wgrad GEMM -> FedAvg reduce (ops/produced.py, opt-in until measured): the two-shot kernel runs on
@@ -130,7 +129,7 @@ class FederatedEngine:
         self.overlap_timeout_s = float(os.environ.get("COLEARN_OVERLAP_TIMEOUT_S", "20"))
         # per-phase device timing (SURVEY §5): CUDA-event pairs around the H2D copy / broadcast / local fit / reduce+apply /
         # read-back launches of every round, reported as RoundReport.extra["phases_ms"]; the NVTX ranges of the same phases
-        # (COLEARN_NVTX=1) are always in place.  Off by default: the event records cost ~1 us each on the 20 kB-model rounds.
+        # (COLEARN_NVTX=1) are always in place.  Off by default: the event records add to the short rounds of the small models.
         if phase_timing is None:
             phase_timing = os.environ.get("COLEARN_PHASE_TIMING", "0") == "1"
         self.phase_timing = bool(phase_timing)
@@ -515,7 +514,7 @@ class FederatedEngine:
 
     # ------------------------------------------------------------------------------------------ twoshot
     def _layerwise_trainer(self):
-        """tcgen05 layer-wise trainer bound to the work arena (+ bf16 shadow arena), or None."""
+        """wgmma layer-wise trainer bound to the work arena (+ bf16 shadow arena), or None."""
         if getattr(self, "_lw_checked", False):
             return self._lw
         self._lw_checked, self._lw = True, None
@@ -541,7 +540,7 @@ class FederatedEngine:
         return self._prod
 
     def _local_train_inplace(self, round_idx: int, epoch: int, produced=None, overlapped=None) -> torch.Tensor:
-        """Local fit in place on the work arena.  Wide MLPs: tcgen05 layer-wise trainer whose first
+        """Local fit in place on the work arena.  Wide MLPs: wgmma layer-wise trainer whose first
         forward GEMMs consume the previous round's broadcast chunk by chunk (flags of ``epoch-1``);
         everything else: torch autograd (cuDNN convs) + this repo's loss / SGD kernels.
 

@@ -1,5 +1,5 @@
 """Resource monitors (reference ``data/ps_util_test.py``, ``data/temperature_test.py``; SURVEY C31)
-plus the B200 analogue: an NVML sampler (SM clock, power, temperature, throttle reasons) used by
+plus the GPU analogue: an NVML sampler (SM clock, power, temperature, throttle reasons) used by
 ``bench.py`` to record clocks *during* the timed region.
 
 File formats are the reference's (``Monitoring: <i> <timestamp>`` blocks, SURVEY §2.7) so the

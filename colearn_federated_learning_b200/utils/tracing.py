@@ -3,7 +3,7 @@
 The reference profiles out-of-band with psutil scripts attached to the coordinator's PID
 (``data/ps_util_test.py``; PID logged at fc.py:605).  Here: NVTX ranges around the phases of a
 round (visible in Nsight tools), a CUDA-event phase timer for device-side timing without a
-profiler, and helpers that the ``scripts/profile_kernels.sh`` recipe uses.
+profiler, and helpers for profiling runs.
 """
 from __future__ import annotations
 

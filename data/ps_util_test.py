@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Process / NIC monitor kept at the reference's path (``data/ps_util_test.py``): ``-p <pid>`` and/or ``-n <iface>``;
-``--gpu <index>`` additionally samples the GPU through NVML (the B200 analogue of the Pi's CPU monitor)."""
+``--gpu <index>`` additionally samples the GPU through NVML (the GPU analogue of the Pi's CPU monitor)."""
 import os
 import sys
 

@@ -20,7 +20,7 @@ from colearn_federated_learning_b200.models import MLPNet, MLPSpec, register_mod
 
 class TinyMLP(MLPNet):
     """2-16-16-2 classifier.  Any ``MLPNet`` trains through the native executors (persistent kernel instantiations,
-    layer-wise tcgen05 trainer, CPU host executor); other ``nn.Module``s use the autograd path."""
+    layer-wise wgmma trainer, CPU host executor); other ``nn.Module``s use the autograd path."""
 
     def __init__(self) -> None:
         super().__init__(MLPSpec((2, 16, 16, 2), "none", "xent"))

@@ -62,7 +62,7 @@ def build_parser() -> argparse.ArgumentParser:
     parser.add_argument("--save-every", type=int, default=0, help="also write the checkpoint every N rounds (0 = only after the last round, like the reference)")
     parser.add_argument("--dtype", choices=["fp32", "bf16"], default=d.dtype,
                         help="--box: bf16 makes the FedAvg broadcast carry a bf16 copy of the model next to the fp32 master "
-                             "(consumed directly by the tcgen05 GEMMs of the wide / conv models)")
+                             "(consumed directly by the wgmma GEMMs of the wide / conv models)")
     parser.add_argument("--no-cuda", action="store_true")
     parser.add_argument("--strict-events", action="store_true", help="validate IPv4 octets / full match (reference is lax)")
     parser.add_argument("--fit-timeout", type=float, default=None, help="seconds before a silent remote worker is dropped from a round")

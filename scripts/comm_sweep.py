@@ -1,4 +1,4 @@
-"""Broadcast + FedAvg-reduce bandwidth sweep (BASELINE.json: "broadcast+FedAvg-reduce GB/s vs 900 GB/s/dir").
+"""Broadcast + FedAvg-reduce bandwidth sweep (BASELINE.json: "broadcast+FedAvg-reduce GB/s vs 450 GB/s/dir").
 
 Run under torchrun on N GPUs.  For each message size P (fp32 elements) it times, with CUDA events and
 max over ranks:
@@ -100,7 +100,7 @@ def main():
         use_nvls = bool(args.nvls and arena.has_multicast and world > 1)
         arrive = [arena.ptr("flags", k, 1 + rank) for k in range(world)]
         state = {"e": 0}
-        n_blocks = args.blocks or max(1, min(148 * 2, (n_chunks + world - 1) // world))
+        n_blocks = args.blocks or max(1, min(132 * 2, (n_chunks + world - 1) // world))
 
         def ours():
             state["e"] += 1
@@ -121,9 +121,9 @@ def main():
                "twoshot_ms": ms, "twoshot_busbw_GBps": bus / ms / 1e6 if world > 1 else None,
                "nccl_allreduce_ms": ms_nccl, "nccl_busbw_GBps": bus / ms_nccl / 1e6 if world > 1 else None,
                "shadow_bf16": args.shadow, "chunk_elems": chunk, "nvls": use_nvls, "blocks": n_blocks, "tag": args.tag,
-               # fraction of NVLink 5's 900 GB/s per direction (BASELINE.json); busbw is directly comparable with it
-               "twoshot_frac_of_900GBps": (bus / ms / 1e6 / 900.0) if world > 1 else None,
-               "nccl_frac_of_900GBps": (bus / ms_nccl / 1e6 / 900.0) if world > 1 else None}
+               # fraction of the H100's NVLink 4 450 GB/s per direction (data sheet); busbw is directly comparable with it
+               "twoshot_frac_of_450GBps": (bus / ms / 1e6 / 450.0) if world > 1 else None,
+               "nccl_frac_of_450GBps": (bus / ms_nccl / 1e6 / 450.0) if world > 1 else None}
         if args.nvlink_counters:
             # what the algorithm says this GPU must move per call: pull (W-1)/W of the vector for its reduce share + push its
             # reduced share to W-1 peers (P2P form) = (W-1)/W * 4P each way; with NVLS the switch reduces and multicasts, so

@@ -1,5 +1,5 @@
 #!/bin/sh
-# compute-sanitizer racecheck without a GPU: the SIMT kernels (persistent MLP, elementwise, comm, conv, and the tcgen05 GEMM on its functional model) compiled for the CPU
+# compute-sanitizer racecheck without a GPU: the SIMT kernels (persistent MLP, elementwise, comm, conv, and the wgmma GEMM on its functional model) compiled for the CPU
 # through csrc/host_shim.h with -fsanitize=thread and run on small workloads.  Exit code 0 = no data race reported.
 #   sh scripts/racecheck_cpu.sh [build-dir]
 set -e

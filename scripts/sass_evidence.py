@@ -1,10 +1,9 @@
 #!/usr/bin/env python
 """Per-kernel counts of the SASS mnemonics that prove which hardware paths a kernel uses (no GPU needed: cuobjdump
-reads the in-tree .so).  tcgen05.mma -> UTCHMMA, TMA -> UTMALDG (.2D / .4D / .MULTICAST / .2CTA), tcgen05.ld -> LDTM,
-tcgen05.commit -> UTCBAR, mbarrier -> SYNCS, TMEM alloc -> UTCATOMSWS, multimem.ld_reduce -> LDGMC, .sys-scope
-acquire/release traffic -> LDG/STG ... STRONG.SYS.
+reads the in-tree .so).  wgmma -> HGMMA, TMA -> UTMALDG (.2D / .4D / .MULTICAST), mbarrier -> SYNCS,
+multimem.ld_reduce -> LDGMC, .sys-scope acquire/release traffic -> LDG/STG ... STRONG.SYS.
 
-    python scripts/sass_evidence.py > profiles/sass_evidence.txt
+    python scripts/sass_evidence.py          (the counts go to stdout)
 """
 import collections
 import glob
@@ -17,7 +16,7 @@ so = sorted(glob.glob(os.path.join(ROOT, "colearn_federated_learning_b200", "ops
 out = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True, check=True).stdout
 demangle = subprocess.run(["c++filt"], input="\n".join(re.findall(r"Function : (\S+)", out)), capture_output=True, text=True).stdout.splitlines()
 names = iter(demangle)
-pat = re.compile(r"\b(UTCHMMA[.\w]*|UTMALDG[.\w]*|LDTM[.\w]*|UTCBAR[.\w]*|UTCATOMSWS[.\w]*|SYNCS[.\w]*|LDGMC[.\w]*|UCGABAR\w*|"
+pat = re.compile(r"\b(HGMMA[.\w]*|UTMALDG[.\w]*|SYNCS[.\w]*|LDGMC[.\w]*|UCGABAR\w*|"
                  r"(?:LDG|STG|ATOMG|RED)\.[.\w]*STRONG\.SYS[.\w]*|MULTIMEM[.\w]*)")
 cur, counts = None, collections.OrderedDict()
 for line in out.splitlines():

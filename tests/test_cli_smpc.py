@@ -178,10 +178,12 @@ def test_box_mode_cli_two_ranks_gloo(tmp_path):
     both ranks train, rank 0 writes the reference-format checkpoint (CPU/gloo stand-in for the fused GPU path)."""
     ckpt = str(tmp_path / "test.pth")
     env = dict(os.environ, CUDA_VISIBLE_DEVICES="", PYTHONPATH=ROOT)
+    # each rank announces TRAINING once it has started, and the first announcement opens the window: on a loaded machine the
+    # second rank can start more than a second after the first, so the window is long enough for both to be in it
     out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr",
                           "127.0.0.1", "--master-port", str(_free_port()), os.path.join(ROOT, "federated_coordinator.py"),
                           "-t", "topic/state", "--box", "--model", "mlp", "--synthetic", "128", "-f", "2", "--weighted",
-                          "-w", "1", "--checkpoint", ckpt, "--batch-size", "4", "--exit-after", "1"], env=env, capture_output=True, text=True,
+                          "-w", "10", "--checkpoint", ckpt, "--batch-size", "4", "--exit-after", "1"], env=env, capture_output=True, text=True,
                          timeout=240, cwd=str(tmp_path))
     assert out.returncode == 0, out.stderr[-2000:]
     assert _closed_windows(out.stderr) == [(["10.0.0.1:8777", "10.0.0.2:8778"],) * 2]     # (members, selected), arrival order ignored

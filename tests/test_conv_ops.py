@@ -5,7 +5,7 @@ Three layers of evidence, mirroring how the other kernels are tested (kernel vs 
 1. the PyTorch *definitions* in ``ops/conv.py`` agree with ``torch.nn.functional`` + autograd (what the ops mean);
 2. the *kernel bodies* (``csrc/conv_ops.cuh``) compiled for the host (``_colearn_emul``) agree with the definitions
    (``backend = "emul"``, runs on the CPU box);
-3. the sm_100a kernels agree with the definitions (``backend = "cuda"``, ``@pytest.mark.gpu``).
+3. the sm_90a kernels agree with the definitions (``backend = "cuda"``, ``@pytest.mark.gpu``).
 """
 import contextlib
 
@@ -142,7 +142,7 @@ def test_definitions_pooling_matches_autograd():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# 2./3. kernel bodies (host build) and sm_100a kernels against the definitions
+# 2./3. kernel bodies (host build) and sm_90a kernels against the definitions
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("backend", BACKENDS)
 @pytest.mark.parametrize("geom", GEOMS)
@@ -315,7 +315,7 @@ def test_pack_and_unpack_params(backend):
 @pytest.mark.parametrize("m,c,ldx", [(128, 64, 128), (8192, 64, 128), (512, 256, 256), (4100, 512, 512)])
 def test_fused_batchnorm_reduction_kernel_bodies_on_host(m, c, ldx):
     """Single-launch BatchNorm reduction (the last block of a column group finalises, the ticket counter resets
-    itself): the host build of the bodies against the definitions.  The sm_100a run lives in test_gpu_schedules."""
+    itself): the host build of the bodies against the definitions.  The sm_90a run lives in test_gpu_schedules."""
     _batchnorm_case("emul", m, c, ldx, fused=True)
 
 

@@ -246,7 +246,7 @@ def test_local_fit_native_conv_path_on_cpu(monkeypatch):
 
 @pytest.mark.gpu
 def test_gpu_step_matches_definitions_and_autocast():
-    """The sm_100a path (im2col / BatchNorm / pooling kernels + tcgen05 GEMMs) against the CPU definitions of the
+    """The sm_90a path (im2col / BatchNorm / pooling kernels + wgmma GEMMs) against the CPU definitions of the
     same ops on the same data, layer by layer on the forward, and against fp32 autograd on the update."""
     if not torch.cuda.is_available():
         pytest.skip("needs a GPU")

@@ -1,4 +1,4 @@
-"""sm_100a kernel numerics vs the plain-PyTorch fp32 reference of the same op (needs a GPU)."""
+"""sm_90a kernel numerics vs the plain-PyTorch fp32 reference of the same op (needs a GPU)."""
 import pytest
 import torch
 
@@ -247,7 +247,7 @@ def test_gemm_tcgen05_epilogues(cluster):
 
 
 def test_layerwise_tcgen05_trainer_matches_autograd():
-    """Wide-MLP local SGD on tcgen05 GEMMs (fwd / dgrad / wgrad + fused SGD) vs fp32 autograd."""
+    """Wide-MLP local SGD on wgmma GEMMs (fwd / dgrad / wgrad + fused SGD) vs fp32 autograd."""
     from colearn_federated_learning_b200.fl import FitConfig
     from colearn_federated_learning_b200.fl.layerwise import LayerwiseMLPTrainer
     from colearn_federated_learning_b200.models import MLPNet, MLPSpec

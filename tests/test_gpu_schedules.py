@@ -2,7 +2,7 @@
 implicit-GEMM convolution, programmatic dependent launch) and the engine modes added in round 2.  Every re-scheduling is
 compared with the round-1 schedule (fixture ``legacy_conv_schedule``: all of fl.convnet.SCHEDULE_DEFAULTS at 0); the
 shipped defaults — the fastest measured combination — are the "all switches" rows of these tests plus
-tests/test_convnet_trainer.py.  First run on a B200 in round 2 (profiles/README.md)."""
+tests/test_convnet_trainer.py."""
 import os
 
 import pytest
@@ -102,7 +102,7 @@ def test_splitk_reduce_kernel(splits, rows, cols):
 @pytest.mark.parametrize("m,n,k,s,tile_n", [(128, 256, 32768, 64, 0), (128, 640, 8192, 16, 0), (256, 128, 4096, 3, 0),
                                             (512, 512, 1024, 4, 128), (128, 512, 4608, 9, 256), (1024, 256, 512, 8, 0)])
 def test_gemm_split_k_partials(m, n, k, s, tile_n):
-    """Split-K mode of the 1-CTA tcgen05 GEMM: every slice's raw accumulator against the fp32 product of the same
+    """Split-K mode of the 1-CTA wgmma GEMM: every slice's raw accumulator against the fp32 product of the same
     K range (slice boundaries = the CPU definition's), their sum against the un-split kernel, untouched slack."""
     dev = _dev()
     from colearn_federated_learning_b200 import ops
@@ -149,7 +149,7 @@ def _one_step_update(dev, graph: bool):
 def _assert_same_step(got, base, cos_min=0.9995):
     """One step apart, two schedules differ by fp32 summation order / bf16 rounding only.  (TWO steps are no test: at this
     learning rate a 1e-6 relative perturbation of the parameters after step 1 already moves the 2-step update to cosine
-    0.982 under the SAME schedule — measured, profiles/README.md — so a 2-step comparison measures chaos, not kernels.)"""
+    0.982 under the SAME schedule — so a 2-step comparison measures chaos, not kernels.)"""
     cos = float((got * base).sum() / (got.norm() * base.norm()))
     rel = float((got - base).norm() / base.norm())
     assert torch.isfinite(got).all() and cos > cos_min and rel < 0.03, (cos, rel)
@@ -191,7 +191,7 @@ def _mn_case(dev, kdim, a_cols, m, n, split=0):
                                                    (32768, 64, 128, 256, 64), (512, 256, 256, 2304, 0), (128, 512, 512, 4608, 0),
                                                    (8192, 64, 128, 640, 16), (2048, 128, 128, 1152, 4)])
 def test_gemm_mn_major_operands(kdim, a_cols, m, n, split):
-    """C = AᵀB with A [K, a_cols], B [K, N] row-major (MN-major UMMA descriptors, boxes of 64 rows x 64 columns; the
+    """C = AᵀB with A [K, a_cols], B [K, N] row-major (MN-major wgmma descriptors, boxes of 64 rows x 64 columns; the
     rows of C past a_cols are TMA zero fill) against the fp32 product."""
     got, want, tol = _mn_case(_dev(), kdim, a_cols, m, n, split)
     torch.testing.assert_close(got, want, **tol)
@@ -496,35 +496,3 @@ def test_twoshot_engine_applies_the_server_learning_rate():
     assert torch.equal(outs[0.5][0], theta0) and not torch.equal(full, theta0)
     torch.testing.assert_close(half, theta0 + 0.5 * (full - theta0), rtol=1e-6, atol=1e-7)
     assert torch.equal(shadow, half.to(torch.bfloat16))
-
-
-_SPIN_SCRIPT = """
-import torch
-from colearn_federated_learning_b200.ops import _ext
-ext = _ext.require()
-dev = torch.device('cuda:0')
-torch.cuda.set_device(dev)
-ext.set_spin_limit(0.3)                       # seconds
-flags = torch.zeros(4, dtype=torch.int32, device=dev)
-ext.wait_flags(flags.data_ptr(), 4, 7)        # nobody will ever raise these
-try:
-    torch.cuda.synchronize()
-    print('NO_ERROR')
-except Exception as e:
-    print('TRAPPED', type(e).__name__)
-"""
-
-
-def test_a_wait_for_a_peer_that_never_signals_fails_the_launch_instead_of_hanging():
-    """Every cross-GPU flag wait is bounded (colearn_kernels.h: spin_wait_ge): past the limit the kernel says what it was
-    waiting for and traps, the host sees a launch failure.  The CUDA context is dead afterwards: subprocess."""
-    import subprocess
-    import sys
-    import time
-    _dev()
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    t0 = time.time()
-    out = subprocess.run([sys.executable, "-c", _SPIN_SCRIPT], cwd=root, capture_output=True, text=True, timeout=120)
-    assert "TRAPPED" in out.stdout, (out.stdout[-500:], out.stderr[-1500:])
-    assert "stayed at 0 (< 7)" in out.stdout + out.stderr and "wait_flags" in out.stdout + out.stderr
-    assert time.time() - t0 < 60

@@ -1,10 +1,10 @@
-"""Implicit-GEMM convolution (csrc/conv_ops.cuh::ConvAddr, gemm_tcgen05.cu conv modes).
+"""Implicit-GEMM convolution (csrc/conv_ops.cuh::ConvAddr, gemm_wgmma.cu conv modes).
 
 The GPU-less evidence has two parts: (1) the *addressing* — the exact host+device decode the GEMM's producer warp runs
 (``conv_kblock`` / ``conv_nblock``, called here through the host build) drives a Python model of tiled 4-D TMA boxes
 (whole images, zero fill outside the tensor) and must reproduce conv2d / its input gradient / its weight gradient;
 (2) the *definitions* of ``ops.conv.conv_gemm`` agree with autograd, and the trainer with the implicit schedule
-agrees with the default one.  The sm_100a runs live in tests/test_gpu_schedules.py."""
+agrees with the default one.  The sm_90a runs live in tests/test_gpu_schedules.py."""
 import pytest
 import torch
 import torch.nn.functional as F

@@ -1,4 +1,4 @@
-"""The layer-wise tcgen05 trainer covers every MLP shape the persistent kernel does not: hidden widths and batch sizes
+"""The layer-wise wgmma trainer covers every MLP shape the persistent kernel does not: hidden widths and batch sizes
 that are not multiples of 128 (zero padding / zero-gradient rows), a short last batch, and the BCE / SSE / MSE heads —
 compared with plain autograd on the same sample order.  CPU run = the PyTorch definitions of the ops (same orchestration);
 the GPU case runs the kernels."""
@@ -55,7 +55,7 @@ def test_general_mlp_shapes_match_autograd_on_gpu(dims, act, loss, b, n):
 
 @pytest.mark.gpu
 def test_cuda_tensors_never_fall_back_to_autograd_silently(monkeypatch):
-    """`Net` on a GPU trains on the tcgen05 layer-wise path; a ResNet shard the conv kernels do not cover raises instead of
+    """`Net` on a GPU trains on the wgmma layer-wise path; a ResNet shard the conv kernels do not cover raises instead of
     switching to cuDNN, unless the library path is requested explicitly."""
     from colearn_federated_learning_b200.models import build_model
     dev = torch.device("cuda", 0)
@@ -69,7 +69,7 @@ def test_cuda_tensors_never_fall_back_to_autograd_silently(monkeypatch):
     res = build_model("resnet18").to(dev)
     rflat = flatten_params(res).to(dev)
     xi, yi = torch.randn(100, 3, 32, 32, device=dev), torch.randint(0, 10, (100, 1), device=dev).float()
-    with pytest.raises(RuntimeError, match="no sm_100a kernel path"):
+    with pytest.raises(RuntimeError, match="no sm_90a kernel path"):
         local_fit(rflat, res, xi, yi, FitConfig(model="resnet18", loss="xent", batch_size=100, lr=0.05))
     monkeypatch.setenv("COLEARN_CONV_PATH", "torch")
     _, path = local_fit(rflat, res, xi, yi, FitConfig(model="resnet18", loss="xent", batch_size=100, lr=0.05))

@@ -102,13 +102,13 @@ def test_engine_twoshot_single_gpu_resnet_round():
     t0 = eng.global_flat().clone()
     rep = eng.run_rounds(2)
     assert rep.algo == "twoshot" and torch.isfinite(eng.global_flat()).all() and not torch.equal(eng.global_flat(), t0)
-    assert rep.extra["train_path"] == "convnet"                  # this repo's conv / BatchNorm kernels + tcgen05 GEMMs, not cuDNN
+    assert rep.extra["train_path"] == "convnet"                  # this repo's conv / BatchNorm kernels + wgmma GEMMs, not cuDNN
     assert float(rep.losses[1, 0, 0]) < float(rep.losses[0, 0, 0]) * 1.5
     # a shape the conv kernels do not cover raises instead of switching to cuDNN (fl/trainer.py: _library_path_guard)
     eng32 = FederatedEngine("resnet18", backend="fused", device=dev, batch_size=32, lr=0.05, seed=1)
     eng32.set_local_data(x[:64], y[:64].float().view(-1, 1))
     import pytest as _pytest
-    with _pytest.raises(RuntimeError, match="no sm_100a kernel path"):
+    with _pytest.raises(RuntimeError, match="no sm_90a kernel path"):
         eng32.run_rounds(1)
 
 
@@ -301,7 +301,7 @@ def _rank_main(rank, world, port, out_path, case):
                 torch.save({"arrived": arrived, "err": err, "world": world}, out_path)
             torch.cuda.synchronize()
         elif case == "wide":
-            # wide MLP on the tcgen05 layer-wise trainer; rounds >= 2 consume the two-shot broadcast through the
+            # wide MLP on the wgmma layer-wise trainer; rounds >= 2 consume the two-shot broadcast through the
             # bf16 shadow arena with the GEMM's TMA producer polling per-chunk flags (fused broadcast -> GEMM)
             eng = FederatedEngine("wide_mlp", backend="fused", device=dev, batch_size=128, lr=0.05, seed=6, chunk_elems=4096,
                                   bf16_shadow=True, model_kwargs={"width": 256, "depth": 2})

@@ -1,6 +1,6 @@
 """Fused wgrad GEMM → FedAvg reduce (ops/produced.py, csrc/produced.cuh): host-side bookkeeping on the PyTorch definitions,
 then the whole round — layer-wise trainer, epilogue reports, overlapped two-shot — from the kernel SOURCES on the CPU
-(SIMT shim + functional tcgen05 model).  The GPU run of the same path is in tests/test_gpu_schedules.py."""
+(SIMT shim + functional wgmma model).  The GPU run of the same path is in tests/test_gpu_schedules.py."""
 import pytest
 import torch
 
@@ -62,7 +62,7 @@ def test_reference_spec_rejects_double_reports():
 
 
 def test_round_from_kernel_sources_with_overlapped_reduce():
-    """Two emulated ranks, wide-MLP round: the last backward's wgrad GEMMs (kernel source on the tcgen05 model) report
+    """Two emulated ranks, wide-MLP round: the last backward's wgrad GEMMs (kernel source on the wgmma model) report
     their blocks, the overlapped two-shot kernel (kernel source on the SIMT shim) reduces on the produced tables alone;
     result = FedAvg of two independent plain fits."""
     from colearn_federated_learning_b200.ops import conv as conv_ops
@@ -123,7 +123,7 @@ def test_layerwise_dgrad_against_weights_in_place():
     simt = conv_ops.load_simt()
     if simt is None or not hasattr(simt, "gemm_tcgen05"):
         pytest.skip("SIMT build unavailable")
-    with conv_ops.simt():                                        # kernel source: MN-major B operand on the tcgen05 model
+    with conv_ops.simt():                                        # kernel source: MN-major B operand on the wgmma model
         LayerwiseMLPTrainer(spec, a2[:P], 128, dgrad_kn=True).fit(a2[:P], x, y, cfg, None)
     torch.testing.assert_close(a2, a0, rtol=2e-3, atol=2e-3)
 

@@ -11,10 +11,13 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BASE = os.path.join(ROOT, "baseline")
-REF = os.path.join(BASE, "_ref")
+ORACLE = os.path.join(ROOT, "oracle")
+REF = os.path.join(ORACLE, "_ref")
 
-needs_ref = pytest.mark.skipif(not os.path.exists(os.path.join(REF, "SHA256SUMS")) and not os.path.exists("/root/reference"),
-                               reason="neither baseline/_ref nor /root/reference is available")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_sha256.json")   # SHA-256 of the published reference files
+
+needs_ref = pytest.mark.skipif(not os.path.exists(os.path.join(REF, "SHA256SUMS")),
+                               reason="oracle/_ref is not installed (__graft_entry__.build() installs it from a reference checkout)")
 
 
 def test_standins_do_not_import_the_product():
@@ -32,20 +35,23 @@ def test_standins_do_not_import_the_product():
     assert "import colearn_federated_learning_b200" not in harness and "from colearn_federated_learning_b200" not in harness
 
 
-@needs_ref
 def test_installed_reference_is_byte_identical():
-    sys.path.insert(0, BASE)
+    """The stored digests cover every file install_ref copies; an installed oracle/_ref matches them byte for byte."""
+    with open(GOLDEN) as f:
+        golden = json.load(f)
+    sys.path.insert(0, ORACLE)
     try:
         import install_ref
+        assert {"federated_coordinator.py", "client_federated.py", "datasets.py", "event_parser.py", "settings.py"} <= set(golden)
+        assert set(golden) <= set(install_ref.FILES)
         if not os.path.exists(os.path.join(REF, "SHA256SUMS")):
-            install_ref.install()
+            return
         sums = install_ref.verify(REF)
     finally:
-        sys.path.remove(BASE)
-    assert {"federated_coordinator.py", "client_federated.py", "datasets.py", "event_parser.py", "settings.py"} <= set(sums)
-    if os.path.exists("/root/reference"):
-        for rel, h in sums.items():
-            assert hashlib.sha256(open(os.path.join("/root/reference", rel), "rb").read()).hexdigest() == h, rel
+        sys.path.remove(ORACLE)
+    assert sums == golden
+    for rel, h in sums.items():
+        assert hashlib.sha256(open(os.path.join(REF, rel), "rb").read()).hexdigest() == h, rel
 
 
 @needs_ref

@@ -1,6 +1,6 @@
-"""The built extension really contains the Blackwell instructions the design claims (checked from the cubin with
-cuobjdump — no GPU needed): tcgen05.mma -> UTCHMMA, TMA -> UTMALDG (2-D, 4-D, multicast, cta_group::2), tcgen05.ld ->
-LDTM, tcgen05.commit -> UTCBAR, mbarrier -> SYNCS, multimem.ld_reduce -> LDGMC, .sys-scope release/acquire flags."""
+"""The built extension really contains the Hopper instructions the design claims (checked from the cubin with
+cuobjdump — no GPU needed): wgmma -> HGMMA, TMA -> UTMALDG (2-D, 4-D, multicast), mbarrier -> SYNCS, multimem.ld_reduce ->
+LDGMC, .sys-scope release/acquire flags."""
 import glob
 import os
 import re
@@ -28,7 +28,7 @@ def sass():
             per_kernel[cur] = []
         elif cur is not None:
             per_kernel[cur].append(line)
-    assert "sm_100a" in out.stdout or "SM100" in out.stdout.upper() or per_kernel
+    assert "sm_90a" in out.stdout or "SM90" in out.stdout.upper() or per_kernel
     return {k: "\n".join(v) for k, v in per_kernel.items()}
 
 
@@ -36,16 +36,16 @@ def _kernels(sass, needle):
     return {k: v for k, v in sass.items() if needle in k}
 
 
-def test_gemm_kernels_use_tcgen05_tmem_and_tma(sass):
-    gemms = _kernels(sass, "gemm_tcgen05_kernel")
+def test_gemm_kernels_use_wgmma_and_tma(sass):
+    gemms = _kernels(sass, "gemm_wgmma_kernel")
     assert len(gemms) >= 6                                     # K-major x3 tiles (+cluster), MN-major, mixed, 128x64
     for name, text in gemms.items():
-        for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "UTCBAR", "SYNCS"):
+        for mnemonic in ("HGMMA", "UTMALDG", "SYNCS"):
             assert mnemonic in text, (name, mnemonic)
     # implicit-GEMM convolution: 4-D activation boxes in the 1-CTA instantiations
     assert sum("UTMALDG.4D" in t for t in gemms.values()) >= 5
-    two_sm = _kernels(sass, "gemm_tcgen05_2sm_kernel")
-    assert len(two_sm) == 1 and "UTCHMMA.2CTA" in next(iter(two_sm.values())) and "UTMALDG.2D.2CTA" in next(iter(two_sm.values()))
+    # the cluster pair multicasts its shared B tile
+    assert any("MULTICAST" in t.upper() for t in gemms.values())
 
 
 def test_comm_kernels_use_multimem_and_system_scope_flags(sass):
@@ -64,7 +64,7 @@ def test_round2_paths_compile_to_the_instructions_their_docs_claim(sass):
     with_pdl = [k for k, v in conv.items() if "ACQBULK" in v and "PREEXIT" in v]
     without = [k for k, v in conv.items() if "ACQBULK" not in v and "PREEXIT" not in v]
     assert len(with_pdl) == len(without) == 13, (len(with_pdl), len(without))
-    for text in {**_kernels(sass, "gemm_tcgen05_kernel"), **_kernels(sass, "gemm_tcgen05_2sm_kernel")}.values():
+    for text in _kernels(sass, "gemm_wgmma_kernel").values():
         assert "ACQBULK" in text and "PREEXIT" in text          # behind `if (ep.pdl)`, after the kernel's own set-up
     # fused wgrad -> FedAvg reduce: the overlapped two-shot polls .sys-scope flags and shares the reduce body
     overlap = next(iter(_kernels(sass, "twoshot_overlap_kernel").values()))
@@ -75,10 +75,9 @@ def test_round2_paths_compile_to_the_instructions_their_docs_claim(sass):
     v3 = {k: v for k, v in _kernels(sass, "mlp_local_sgd_kernel_v2").items() if "6v2_128" in k and "Li64ELi64" in k}
     assert len(v5) == 2 and all(t.count("LDS.128") >= 16 for t in v5.values())
     assert len(v3) == 2 and all("LDS.128" not in t for t in v3.values())
-    # variant 6 (default for the 10-64-64-2 MLP): packed fp32 math — FFMA2 carries the dot products and rank-1 updates
+    # variant 6: the paired form of variant 5 is built too (Hopper has no packed fp32 FMA, so it issues plain FFMA)
     v6 = {k: v for k, v in _kernels(sass, "mlp_local_sgd_kernel_v2").items() if "7v2_128p" in k and "Li64ELi64" in k}
-    assert len(v6) == 2 and max(t.count("FFMA2") for t in v6.values()) >= 60 and all("FFMA2" in t for t in v6.values())
-    assert all("FFMA2" not in t for t in v5.values())
+    assert len(v6) == 2 and all("FFMA" in t for t in v6.values())
     # bounded flag waits: the spin helper reads the nanosecond timer; the comm kernels carry the trap of spin_wait_failed
     star = next(iter(_kernels(sass, "star_round_kernel").values()))
     assert "GLOBALTIMER" in star.upper() or "SR_GLOBALTIMER" in star.upper()

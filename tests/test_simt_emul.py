@@ -1,7 +1,7 @@
 """The persistent-MLP CUDA kernels (csrc/mlp_persistent.cu + mlp_v2.inc — the flagship op of BASELINE configs 1-3)
 executed on the CPU: the kernel *source* is compiled with g++ through csrc/host_shim.h (one OS thread per CUDA thread,
 __syncthreads / warp shuffles / dynamic shared memory emulated) and compared with the PyTorch definitions, exactly
-like tests/test_gpu_kernels.py does on a B200.  Every variant: v1 (weights in shared memory, 256 threads), v2 with 128
+like tests/test_gpu_kernels.py does on a GPU.  Every variant: v1 (weights in shared memory, 256 threads), v2 with 128
 threads (register-resident row + column copies, replicated head) in its strided (3), blocked (5) and blocked + packed-FMA (6) forms."""
 import pytest
 import torch
@@ -303,7 +303,7 @@ def test_batchnorm_kernels_on_cpu(simt, m, c, ldx, fused):
     T._batchnorm_case("simt", m, c, ldx, fused=fused)
 
 
-# ---- gemm_tcgen05.cu on the functional tcgen05 / TMA / mbarrier / TMEM model (csrc/tcgen05_host_model.h) ------------------
+# ---- gemm_wgmma.cu on the functional wgmma / TMA / mbarrier model (csrc/gemm_host_model.h) -------------------------------
 def _gemm(simt, a, b, **kw):
     simt.gemm_tcgen05(a, b, kw.get("bias"), kw.get("relu", False), kw.get("relu_mask"), kw.get("out_bf16"), kw.get("out_f32"),
                       kw.get("out_bf16_t"), kw.get("sgd_master"), kw.get("sgd_lr", 0.0), kw.get("sgd_shadow"), kw.get("sgd_shadow_t"),
@@ -316,9 +316,8 @@ def _bf(*shape):
 
 
 def test_tcgen05_gemm_source_on_the_cpu_model_k_major(simt):
-    """The persistent TMA -> tcgen05.mma -> TMEM -> epilogue pipeline (mbarrier phases, 4 "SMs" walking up to 8 tiles each,
-    double-buffered accumulators) and every fused epilogue.  This path runs on B200s, so exact agreement here calibrates
-    the model (swizzle, descriptor decode) for the operand modes that have not run on a GPU yet."""
+    """The persistent TMA -> wgmma -> staged epilogue pipeline (mbarrier phases, 4 "SMs" walking up to 8 tiles each) and
+    every fused epilogue, against PyTorch."""
     torch.manual_seed(0)
     for m, n, k, tile_n in [(128, 128, 64, 0), (1024, 256, 192, 128), (512, 512, 128, 256), (256, 384, 64, 0)]:
         a, b = _bf(m, k), _bf(n, k)
@@ -353,7 +352,7 @@ def test_tcgen05_gemm_source_on_the_cpu_model_k_major(simt):
 
 
 def test_tcgen05_gemm_source_on_the_cpu_model_mn_major(simt):
-    """MN-major UMMA operands (boxes of 64 rows x 64 columns, LBO 8192 / SBO 1024, +2048 bytes per UMMA): wgrad form AᵀB
+    """MN-major wgmma operands (boxes of 64 rows x 64 columns, LBO 8192 / SBO 1024, +2048 bytes per wgmma): wgrad form AᵀB
     with TMA zero fill for the missing columns, dgrad form A·B[:K], with split-K and the fused SGD epilogue."""
     torch.manual_seed(1)
     for kd, ac, m, n in [(64, 128, 128, 128), (128, 64, 128, 128), (512, 64, 128, 640), (256, 256, 256, 256)]:
@@ -416,8 +415,8 @@ def test_implicit_conv_kernels_on_the_cpu_model(simt, n, h, w, cin, cout):
 
 @pytest.mark.skipif(__import__("os").environ.get("COLEARN_RUN_SLOW") != "1", reason="~4 minutes: set COLEARN_RUN_SLOW=1")
 def test_whole_resnet18_step_from_kernel_sources_on_the_cpu_model(simt, monkeypatch):
-    """One ResNet-18 SGD step (batch 128) with EVERY kernel — im2col / BatchNorm / pooling / packing, the tcgen05 GEMMs with
-    their fused epilogues, the loss, the flat SGD — running from its CUDA source on the CPU (SIMT shim + tcgen05 / TMA model):
+    """One ResNet-18 SGD step (batch 128) with EVERY kernel — im2col / BatchNorm / pooling / packing, the wgmma GEMMs with
+    their fused epilogues, the loss, the flat SGD — running from its CUDA source on the CPU (SIMT shim + wgmma / TMA model):
     (1) the default schedule agrees with the PyTorch definitions of the ops; (2) the schedule that has not run on a GPU
     yet (implicit GEMM level 2, MN-major wgrad, packed-weight dgrad, split-K, single-launch BatchNorm reduction) produces the
     same parameter update as the default schedule.  Measured on the authoring box: loss 2.58854 for both, update cosine
