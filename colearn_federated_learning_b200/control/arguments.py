@@ -33,6 +33,11 @@ class Arguments:
     loss: str = "auto"             # auto | bce | sse | xent
     weighted: bool = False         # False = uniform FedAvg (reference), True = n_k / sum(n)
     server_lr: float = 1.0         # theta <- theta + server_lr * avg_delta (1.0 = plain FedAvg)
+    server_opt: str = "sgd"        # server optimizer: sgd (plain FedAvg) | avgm | adagrad | adam | yogi (fl/server_opt.py);
+                                   # the CLI's --server-lr defaults to 0.01 for the adaptive kinds, 1.0 otherwise
+    server_beta1: float = 0.9
+    server_beta2: float = 0.99
+    server_tau: float = 1e-3
     backend: str = "auto"          # auto | fused | nccl | cpu
     dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the wgmma consumers)
     save_every: int = 0            # >0: checkpoint every N rounds, not only after the last one
@@ -40,6 +45,11 @@ class Arguments:
     dataset: str = "unsw"          # data.DATASET_REGISTRY entry that reads test_path (user datasets: data.register_dataset)
     n_train_items_enc: int = 1000  # fc.py:432
     precision_fractional: int = 3  # fc.py:433
+
+    def server_optimizer(self):
+        """The :class:`fl.server_opt.ServerOpt` these arguments describe (``server_lr`` is its learning rate)."""
+        from ..fl.server_opt import ServerOpt
+        return ServerOpt(self.server_opt, lr=self.server_lr, beta1=self.server_beta1, beta2=self.server_beta2, tau=self.server_tau)
 
     def set_federated_batches(self, batches: int) -> None:
         self.federate_after_n_batches = batches

@@ -86,6 +86,9 @@ class Coordinator(BusClient):
         self.trainings_done = 0
         self._in_flight: Dict[str, Any] = {}      # id -> handle of the devices a running training is using
         self._withdrawn: set = set()              # ids that sent NOT_READY while their fit was in flight
+        # server optimizer moments (--server-opt other than sgd): carried from round to round and from window to window for the
+        # Coordinator's lifetime, reset when the model's parameter count changes; never written to the checkpoint
+        self._server_opt_state = None
 
         self.windower = TemporalWindow(self.registry, window, self._start_training, timer_factory,
                                        lower_bound=0, rearm_if_pending=rearm_if_pending)
@@ -310,7 +313,7 @@ class Coordinator(BusClient):
             live = [i for i, c in enumerate(counts) if c > 0]
             if live:
                 w = normalized_weights([counts[i] for i in live] if self.args.weighted else None, len(live), device=self.device)
-                ops.fedavg_apply(theta, flats[live].contiguous(), w, self.args.server_lr)
+                self._server_update(theta, flats[live].contiguous(), w)
             for wid, l in zip(fed.workers, losses):
                 self.metrics.worker_loss(wid, l)
                 result["losses"][wid] = l
@@ -430,7 +433,7 @@ class Coordinator(BusClient):
                 stacked = torch.stack(flats).to(self.device)
                 w = normalized_weights(counts if self.args.weighted else None, len(flats), device=self.device)
                 th = theta.to(self.device)
-                ops.fedavg_apply(th, stacked, w, self.args.server_lr)
+                self._server_update(th, stacked, w)
                 theta = th.cpu()
                 self._average_buffers(model, [getattr(alive.get(wid), "last_buffers", None) for wid in ids], w.cpu())
             # traffic of this round: model + fit config towards the devices, trained model + loss back (paper §4.3)
@@ -441,6 +444,22 @@ class Coordinator(BusClient):
             if not alive:
                 break
         return theta
+
+    def _server_update(self, theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor) -> None:
+        """FedAvg of ``models`` into ``theta`` in place, followed by the server optimizer step of ``--server-opt``."""
+        if self.args.server_opt == "sgd":
+            ops.fedavg_apply(theta, models, weights, self.args.server_lr)
+            return
+        opt = self.args.server_optimizer()
+        st = self._server_opt_state
+        if st is None or st.opt != opt or st.numel != theta.numel():
+            if st is not None and st.numel != theta.numel():
+                log.info("Server optimizer state reset: the model has %d parameters, the state %d", theta.numel(), st.numel)
+            st = self._server_opt_state = opt.init_state(theta.numel(), theta.device)
+        if st.m.device != theta.device:
+            st.m = st.m.to(theta.device)
+            st.v = st.v.to(theta.device) if st.v is not None else None
+        ops.fedavg_apply(theta, models, weights, opt=st)
 
     @staticmethod
     def _average_buffers(model, buffers, weights) -> None:

@@ -35,8 +35,20 @@ def fedavg_flat(models: torch.Tensor, weights: torch.Tensor) -> torch.Tensor:
     return reference.fedavg_flat(models, weights)
 
 
-def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor, server_lr: float = 1.0) -> torch.Tensor:
-    """``theta += server_lr * (sum_k w_k models[k] - theta)`` in place (reduce + scale + apply fused)."""
+def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor, server_lr: float = 1.0, opt=None) -> torch.Tensor:
+    """``theta += server_lr * (sum_k w_k models[k] - theta)`` in place (reduce + scale + apply fused).
+
+    ``opt``: a :class:`fl.server_opt.ServerOptState` — the average is followed by that server optimizer's step (FedAvgM /
+    FedAdagrad / FedAdam / FedYogi) in the same kernel, with the optimizer's own ``lr``; its moments are updated in place."""
+    if opt is not None:
+        if float(server_lr) != 1.0:
+            raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
+        if _cuda(theta):
+            _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(opt.lr),
+                                        opt.code, opt.hyper, opt.m, opt.v)
+            return theta
+        b1, b2, tau = opt.hyper
+        return reference.server_opt_apply(theta, models, weights, opt.kind, opt.lr, opt.m, opt.v, b1, b2, tau)
     if _cuda(theta):
         _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(server_lr))
         return theta

@@ -105,12 +105,44 @@ void sgd_step(torch::Tensor p, torch::Tensor g, double lr) {
     TORCH_CHECK(false, "grad dtype must be float32 or bfloat16");
 }
 
-void fedavg_apply(torch::Tensor theta, torch::Tensor slots, torch::Tensor weights, double server_lr) {
+// Server optimizer of the FedAvg kernels (server_opt.cuh): kind 0 = plain FedAvg with server_lr (the launch the caller made
+// before optimizers existed); otherwise hyper = [beta1, beta2, tau] and m / v point to the moment buffers (v: adaptive kinds).
+static ServerOptArgs server_opt_args(int64_t kind, double lr, const std::vector<double>& hyper, int64_t m, int64_t v) {
+  ServerOptArgs o;
+  std::memset(&o, 0, sizeof(o));
+  o.kind = (int)kind;
+  o.lr = (float)lr;
+  if (kind != SOPT_SGD) {
+    TORCH_CHECK(hyper.size() == 3, "server optimizer: hyper = [beta1, beta2, tau]");
+    o.beta1 = (float)hyper[0];
+    o.beta2 = (float)hyper[1];
+    o.tau = (float)hyper[2];
+    o.m = ptr_of<float>(m);
+    o.v = ptr_of<float>(v);
+  }
+  TORCH_CHECK(server_opt_args_ok(o), "server optimizer: unknown kind ", kind, ", or a moment buffer missing / not 16-byte aligned");
+  return o;
+}
+
+void fedavg_apply(torch::Tensor theta, torch::Tensor slots, torch::Tensor weights, double server_lr, int64_t opt_kind,
+                  std::vector<double> opt_hyper, c10::optional<torch::Tensor> m, c10::optional<torch::Tensor> v) {
   CHECK_CUDA_F32(theta); CHECK_CUDA_F32(slots); CHECK_CUDA_F32(weights);
   TORCH_CHECK(slots.dim() == 2 && slots.size(1) >= theta.numel() && weights.numel() == slots.size(0), "shapes");
   c10::cuda::CUDAGuard guard(theta.device());
-  check(launch_fedavg_apply(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(),
-                            (int)slots.size(0), (float)server_lr, theta.numel(), cur_stream()), "fedavg_apply");
+  if (opt_kind == SOPT_SGD) {
+    check(launch_fedavg_apply(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(),
+                              (int)slots.size(0), (float)server_lr, theta.numel(), cur_stream()), "fedavg_apply");
+    return;
+  }
+  auto state = [&](const c10::optional<torch::Tensor>& t, const char* name) -> int64_t {
+    if (!t.has_value()) return 0;
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() >= theta.numel() &&
+                t->device() == theta.device(), name, ": contiguous CUDA float32 with one element per parameter, on theta's device");
+    return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
+  };
+  const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
+  check(launch_fedavg_apply_opt(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(),
+                                (int)slots.size(0), o, theta.numel(), cur_stream()), "fedavg_apply (server optimizer)");
 }
 torch::Tensor fedavg_flat(torch::Tensor slots, torch::Tensor weights) {
   CHECK_CUDA_F32(slots); CHECK_CUDA_F32(weights);
@@ -289,7 +321,8 @@ void l2_flush(torch::Tensor buf) {
 void star_round(int64_t theta, int64_t slots, int64_t slot_stride, int64_t arrive_flags, int64_t arrive_epoch,
                 std::vector<int64_t> peer_inbox, std::vector<int64_t> peer_bcast_flag, int64_t bcast_epoch,
                 int64_t mc_inbox, int64_t select_mask, double server_lr, int64_t n, bool do_reduce, bool do_bcast,
-                int64_t grid_counter, int64_t n_blocks, double timeout_ms, std::vector<double> weights, int64_t decision) {
+                int64_t grid_counter, int64_t n_blocks, double timeout_ms, std::vector<double> weights, int64_t decision,
+                int64_t opt_kind, std::vector<double> opt_hyper, int64_t opt_m, int64_t opt_v) {
   StarRoundArgs a;
   std::memset(&a, 0, sizeof(a));
   a.theta = ptr_of<float>(theta);
@@ -315,6 +348,7 @@ void star_round(int64_t theta, int64_t slots, int64_t slot_stride, int64_t arriv
   for (size_t k = 0; k < weights.size() && k < 16; ++k) a.weights[k] = (float)weights[k];
   a.decision = ptr_of<uint32_t>(decision);
   TORCH_CHECK(a.timeout_ns == 0 || a.decision != nullptr, "a deadline needs the decision scratch buffer");
+  a.opt = server_opt_args(opt_kind, server_lr, opt_hyper, opt_m, opt_v);
   check(launch_star_round(a, (int)n_blocks, cur_stream()), "star_round");
 }
 
@@ -356,9 +390,12 @@ void twoshot_fedavg(std::vector<int64_t> work, std::vector<int64_t> shadow, std:
                     int64_t arrive_flags, int64_t weights, int64_t theta_prev, int64_t epoch, int64_t select_mask,
                     double server_lr, int64_t n, int64_t chunk_elems, int64_t rank, int64_t n_blocks,
                     std::vector<int64_t> peer_arrive, bool wait_all, int64_t mc_work, int64_t mc_shadow, int64_t produced,
-                    double produced_timeout_s) {
+                    double produced_timeout_s, int64_t opt_kind, std::vector<double> opt_hyper, int64_t opt_m, int64_t opt_v) {
   TwoShotArgs a = make_twoshot_args(work, shadow, chunk_flags, arrive_flags, weights, theta_prev, epoch, select_mask, server_lr, n,
                                     chunk_elems, rank, peer_arrive, wait_all, mc_work, mc_shadow, produced, produced_timeout_s);
+  a.opt = server_opt_args(opt_kind, server_lr, opt_hyper, opt_m, opt_v);
+  TORCH_CHECK(a.opt.kind == SOPT_SGD || (a.theta_prev != nullptr && a.mc_work == nullptr),
+              "twoshot_fedavg: a server optimizer needs theta_prev and the P2P path (no multicast)");
   check(launch_twoshot_fedavg(a, (int)n_blocks, cur_stream()), "twoshot_fedavg");
 }
 
@@ -571,6 +608,8 @@ struct ConvCudaExec {
 
 #include "conv_bindings.inc"
 
+namespace py = pybind11;
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "colearn_federated_learning_b200 sm_90a kernels";
   m.def("make_client_desc", &make_client_desc);
@@ -582,7 +621,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mlp_smem_bytes", &mlp_smem_bytes);
   m.def("mlp_forward", &mlp_forward);
   m.def("sgd_step", &sgd_step);
-  m.def("fedavg_apply", &fedavg_apply);
+  // trailing server-optimizer arguments (server_opt.cuh) default to plain FedAvg: the shorter positional calls keep working
+  m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("weights"), py::arg("server_lr"), py::arg("opt_kind") = 0,
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);
@@ -600,8 +641,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("float_precision", &float_precision);
   m.def("ring_matmul", &ring_matmul);
   m.def("transpose_bf16", &transpose_bf16);
-  m.def("star_round", &star_round);
-  m.def("twoshot_fedavg", &twoshot_fedavg);
+  m.def("star_round", &star_round, py::arg("theta"), py::arg("slots"), py::arg("slot_stride"), py::arg("arrive_flags"), py::arg("arrive_epoch"),
+        py::arg("peer_inbox"), py::arg("peer_bcast_flag"), py::arg("bcast_epoch"), py::arg("mc_inbox"), py::arg("select_mask"),
+        py::arg("server_lr"), py::arg("n"), py::arg("do_reduce"), py::arg("do_bcast"), py::arg("grid_counter"), py::arg("n_blocks"),
+        py::arg("timeout_ms"), py::arg("weights"), py::arg("decision"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
+        py::arg("opt_m") = 0, py::arg("opt_v") = 0);
+  m.def("twoshot_fedavg", &twoshot_fedavg, py::arg("work"), py::arg("shadow"), py::arg("chunk_flags"), py::arg("arrive_flags"), py::arg("weights"),
+        py::arg("theta_prev"), py::arg("epoch"), py::arg("select_mask"), py::arg("server_lr"), py::arg("n"), py::arg("chunk_elems"),
+        py::arg("rank"), py::arg("n_blocks"), py::arg("peer_arrive"), py::arg("wait_all"), py::arg("mc_work"), py::arg("mc_shadow"),
+        py::arg("produced"), py::arg("produced_timeout_s"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
+        py::arg("opt_m") = 0, py::arg("opt_v") = 0);
   m.def("twoshot_fedavg_deadline", &twoshot_fedavg_deadline);
   m.def("twoshot_resync", &twoshot_resync);
   m.def("produced_signal_pack", &produced_signal_pack);

@@ -30,6 +30,16 @@
 #endif
 
 #include <cstdlib>
+
+// functions shared by the kernels and host code (Feistel bijection, server optimizer step)
+#if defined(__CUDACC__) && !defined(COLEARN_HOST_SHIM)
+#define COLEARN_HD __host__ __device__ __forceinline__
+#else
+#define COLEARN_HD inline
+#endif
+// per-element server optimizer step (FedAvgM / FedAdagrad / FedAdam / FedYogi) shared by the FedAvg kernels
+#include "server_opt.cuh"
+
 namespace colearn {
 // Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
 inline bool pdl_enabled() {
@@ -115,11 +125,7 @@ cudaError_t set_spin_limit_gemm(unsigned long long ns);
 // with cycle walking.  Shared by feistel_perm_kernel (tabulates whole rows) and the persistent MLP kernel's gather
 // (computes the index of the sample it is about to prefetch), so both produce the same order for the same (seed, row).
 // ---------------------------------------------------------------------------------------------
-#if defined(__CUDACC__) && !defined(COLEARN_HOST_SHIM)
-#define COLEARN_HD __host__ __device__ __forceinline__
-#else
-#define COLEARN_HD inline
-#endif
+// (COLEARN_HD: defined above)
 // The network is UNBALANCED when the index needs an odd number of bits (left half lb = bits / 2, right half rb = bits - lb;
 // a round maps (l, r) -> (r, l ^ F(r)), so the two widths swap every round and are back after the 4th): the domain is
 // exactly 2^bits < 2 n, i.e. no rejections at all for a power-of-two n and fewer than one per index otherwise.
@@ -218,6 +224,10 @@ cudaError_t launch_sgd_step_bf16grad(float* param, const void* grad_bf16, float 
 cudaError_t launch_fedavg_apply(float* theta, const float* slots, int64_t slot_stride,
                                 const float* weights, int k, float server_lr, int64_t n,
                                 cudaStream_t s);
+// same average a = sum_k w[k] * slots[k], then the server optimizer step of server_opt.cuh (opt.kind 0: launch_fedavg_apply
+// with opt.lr); opt.m / opt.v hold n floats each
+cudaError_t launch_fedavg_apply_opt(float* theta, const float* slots, int64_t slot_stride, const float* weights, int k,
+                                    const ServerOptArgs& opt, int64_t n, cudaStream_t s);
 // out = sum_k w[k] * slots[k]
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride,
                                const float* weights, int k, int64_t n, cudaStream_t s);
@@ -301,6 +311,10 @@ struct StarRoundArgs {
   unsigned long long timeout_ns;
   float weights[16];
   uint32_t* decision;
+  // server optimizer (server_opt.cuh): kind 0 = theta += server_lr (a - theta), today's kernel; otherwise opt.m / opt.v are
+  // the coordinator's local [n] moment buffers and the step runs where the reduce does (do_reduce), never for a round in which
+  // nobody arrived
+  ServerOptArgs opt;
 };
 cudaError_t launch_star_round(const StarRoundArgs& a, int n_blocks, cudaStream_t s);
 
@@ -317,7 +331,7 @@ struct TwoShotArgs {
   uint32_t* chunk_flags[16];    // per-rank [n_chunks] ready flags (peer pointers)
   const uint32_t* arrive_flags; // local [world]: rank k finished local training (value >= epoch)
   const float* weights;         // local device [world]: normalised FedAvg weights
-  float* theta_prev;            // local previous global model (needed iff server_lr != 1) or null
+  float* theta_prev;            // local previous global model (needed iff server_lr != 1 or a server optimizer) or null
   uint32_t epoch;
   uint32_t select_mask;
   float server_lr;
@@ -343,6 +357,10 @@ struct TwoShotArgs {
   uint32_t* decision[16];       // per-rank ring of 8 x {epoch, mask} words (peer pointers)
   float* global_copy[16];       // per-rank second fp32 arena (peer pointers) or nullptr
   const float* true_weights;    // local device [world]: the FedAvg weights to renormalise over the arrived set
+  // server optimizer (server_opt.cuh): kind 0 = theta_prev + server_lr (a - theta_prev), today's kernel.  Otherwise theta_prev
+  // is required, opt.m / opt.v are this rank's local [n] buffers and only the chunks it owns (c % world) are read or written:
+  // the moments are sharded like the work.  Not with deadline_ns (ownership follows the arrived set) nor with mc_work (NVLS)
+  ServerOptArgs opt;
 };
 cudaError_t launch_twoshot_fedavg(const TwoShotArgs& a, int n_blocks, cudaStream_t s);
 // deadline mode, start of a round: if this rank was NOT in the arrived mask of `prev_epoch`, its work arena (and bf16 shadow) is

@@ -16,6 +16,8 @@
 //       the server update, pushes the new slice into every peer's fp32 arena AND its bf16 shadow
 //       (fp32->bf16 conversion fused into the broadcast), raising per-chunk ready flags that the
 //       next round's first consumer GEMM polls from its TMA producer warp (fused broadcast->GEMM).
+//   Both apply plain FedAvg with a server learning rate, or (template flag OPT) a FedOpt server optimizer step of
+//   server_opt.cuh (FedAvgM / FedAdagrad / FedAdam / FedYogi) in the same pass.
 //
 // Memory model: data stores are weak; a CTA finishes with __threadfence_system() and the flag is
 // written with st.release.sys; consumers spin with ld.acquire.sys (and add fence.proxy.async before
@@ -105,6 +107,8 @@ __device__ __forceinline__ uint2 pack_bf16x4(const float4& v) {
 }
 
 // -------------------------------------------------------------------------------------------------
+// OPT = false: theta += server_lr (a - theta) (StarRoundArgs::opt.kind == 0); true: the server optimizer step of server_opt.cuh
+template <bool OPT>
 __global__ void __launch_bounds__(256)
 star_round_kernel(StarRoundArgs a) {
   const int tid = threadIdx.x;
@@ -171,8 +175,12 @@ star_round_kernel(StarRoundArgs a) {
       }
       if (mask == 0u) acc = t;   // nobody arrived: keep theta
       else if (renorm != 1.f) { acc.x *= renorm; acc.y *= renorm; acc.z *= renorm; acc.w *= renorm; }
-      t.x = fmaf(a.server_lr, acc.x - t.x, t.x); t.y = fmaf(a.server_lr, acc.y - t.y, t.y);
-      t.z = fmaf(a.server_lr, acc.z - t.z, t.z); t.w = fmaf(a.server_lr, acc.w - t.w, t.w);
+      if constexpr (OPT) {
+        if (mask != 0u) t = server_opt_step4(a.opt, j, t, acc);     // (nobody arrived: theta and the moments stay)
+      } else {
+        t.x = fmaf(a.server_lr, acc.x - t.x, t.x); t.y = fmaf(a.server_lr, acc.y - t.y, t.y);
+        t.z = fmaf(a.server_lr, acc.z - t.z, t.z); t.w = fmaf(a.server_lr, acc.w - t.w, t.w);
+      }
       theta4[j] = t;
     }
     if (a.do_bcast) {
@@ -192,7 +200,11 @@ star_round_kernel(StarRoundArgs a) {
       for (int k = 0; k < a.world; ++k)
         if ((mask >> k) & 1u) acc += __ldcg(a.slots + k * a.slot_stride + j);
       acc = (mask == 0u) ? t : acc * renorm;
-      t = fmaf(a.server_lr, acc - t, t);
+      if constexpr (OPT) {
+        if (mask != 0u) t = server_opt_step(a.opt, j, t, acc);
+      } else {
+        t = fmaf(a.server_lr, acc - t, t);
+      }
       a.theta[j] = t;
     }
     if (a.do_bcast)
@@ -222,7 +234,9 @@ star_round_kernel(StarRoundArgs a) {
 // belongs to rank (c % world) (interleaved ownership keeps every rank's NVLink ports busy for the
 // whole kernel and lets early layers become ready first on every peer).  A CTA processes whole
 // chunks so that it can publish the chunk's ready flag by itself.
-// one owned chunk: pull it from every selected rank, apply, push it to every rank (fp32 + bf16), publish its flag
+// one owned chunk: pull it from every selected rank, apply, push it to every rank (fp32 + bf16), publish its flag.
+// OPT: the server optimizer step (server_opt.cuh) on theta_prev with this rank's moment shards a.opt.m / a.opt.v, P2P path only
+template <bool OPT>
 __device__ __forceinline__ void twoshot_chunk(const TwoShotArgs& a, const int64_t c, const float* sw, const int tid,
                                               const uint32_t mask, const bool use_mc) {
   const int64_t lo = c * a.chunk_elems;
@@ -279,7 +293,19 @@ __device__ __forceinline__ void twoshot_chunk(const TwoShotArgs& a, const int64_
         }
       }
     }
-    if (a.theta_prev != nullptr) {
+    if constexpr (OPT) {
+      // theta_prev is required with an optimizer (launch_twoshot_fedavg); the owner keeps the moments of its chunks
+      float4 t = reinterpret_cast<float4*>(a.theta_prev)[e4a];
+      t = server_opt_step4(a.opt, e4a, t, acca);
+      reinterpret_cast<float4*>(a.theta_prev)[e4a] = t;
+      acca = t;
+      if (has_b) {
+        float4 u = reinterpret_cast<float4*>(a.theta_prev)[e4b];
+        u = server_opt_step4(a.opt, e4b, u, accb);
+        reinterpret_cast<float4*>(a.theta_prev)[e4b] = u;
+        accb = u;
+      }
+    } else if (a.theta_prev != nullptr) {
       float4 t = reinterpret_cast<float4*>(a.theta_prev)[e4a];
       t.x = fmaf(a.server_lr, acca.x - t.x, t.x); t.y = fmaf(a.server_lr, acca.y - t.y, t.y);
       t.z = fmaf(a.server_lr, acca.z - t.z, t.z); t.w = fmaf(a.server_lr, acca.w - t.w, t.w);
@@ -317,6 +343,7 @@ __device__ __forceinline__ void twoshot_chunk(const TwoShotArgs& a, const int64_
   __syncthreads();
 }
 
+template <bool OPT>
 __global__ void __launch_bounds__(512)
 twoshot_fedavg_kernel(TwoShotArgs a) {
   const int tid = threadIdx.x;
@@ -382,12 +409,12 @@ twoshot_fedavg_kernel(TwoShotArgs a) {
   const int n_own = __popc(owners);
   const bool i_own = (owners >> a.rank) & 1u;
   const int my_idx = __popc(owners & ((1u << a.rank) - 1u));
-  const bool use_mc = a.mc_work != nullptr && (a.deadline_ns == 0 || mask == full);
+  const bool use_mc = !OPT && a.mc_work != nullptr && (a.deadline_ns == 0 || mask == full);
   if (i_own && mask != 0u) {
     for (int64_t oc = blockIdx.x; ; oc += gridDim.x) {
       const int64_t c = my_idx + oc * n_own;
       if (c >= n_chunks) break;
-      twoshot_chunk(a, c, sw, tid, mask, use_mc);
+      twoshot_chunk<OPT>(a, c, sw, tid, mask, use_mc);
     }
   } else if (mask == 0u && a.rank == 0) {
     // nobody arrived in time: the model stays as it is; the coordinator still publishes the chunk flags so that nobody waits
@@ -421,6 +448,7 @@ twoshot_resync_kernel(const uint32_t* ring, uint32_t prev_epoch, int rank, float
 // Chunks are taken in whatever order the producers of all selected ranks finish them (the backward pass finalises the
 // last layers first): each CTA sweeps its owned chunks, newest-first, and processes those whose produced epochs have
 // arrived from every selected rank.
+template <bool OPT>
 __global__ void __launch_bounds__(512)
 twoshot_overlap_kernel(TwoShotArgs a) {
   const int tid = threadIdx.x;
@@ -449,7 +477,7 @@ twoshot_overlap_kernel(TwoShotArgs a) {
         const int ready = s_ready;
         __syncthreads();
         if (!ready) continue;
-        twoshot_chunk(a, c, sw, tid, a.select_mask, a.mc_work != nullptr);
+        twoshot_chunk<OPT>(a, c, sw, tid, a.select_mask, !OPT && a.mc_work != nullptr);
         if (tid == 0) s_done[i >> 6] |= 1ull << (i & 63);
         __syncthreads();
         --left;
@@ -576,20 +604,34 @@ p2p_copy_kernel(float* __restrict__ dst, const float* __restrict__ src, int64_t 
 }  // namespace
 
 cudaError_t launch_star_round(const StarRoundArgs& a, int n_blocks, cudaStream_t s) {
-  if (a.world > 16) return cudaErrorInvalidValue;
+  if (a.world > 16 || !server_opt_args_ok(a.opt)) return cudaErrorInvalidValue;
   if (n_blocks < 1) n_blocks = 1;
-  COLEARN_LAUNCH(star_round_kernel, n_blocks, 256, 0, s, a);
+  if (a.opt.kind != SOPT_SGD) {
+    COLEARN_LAUNCH(star_round_kernel<true>, n_blocks, 256, 0, s, a);
+    return cudaGetLastError();
+  }
+  COLEARN_LAUNCH(star_round_kernel<false>, n_blocks, 256, 0, s, a);
   return cudaGetLastError();
 }
 
 cudaError_t launch_twoshot_fedavg(const TwoShotArgs& a, int n_blocks, cudaStream_t s) {
   if (a.world > 8 || (a.n & 3) || (a.chunk_elems & 3)) return cudaErrorInvalidValue;
   if (n_blocks < 1) n_blocks = 1;
-  if (a.produced != nullptr) {
-    COLEARN_LAUNCH(twoshot_overlap_kernel, n_blocks, 512, 0, s, a);
+  if (a.opt.kind != SOPT_SGD) {
+    // the moments are sharded by the fixed ownership c % world: no deadline (ownership follows the arrived set), no NVLS
+    if (!server_opt_args_ok(a.opt) || a.theta_prev == nullptr || a.deadline_ns != 0 || a.mc_work != nullptr) return cudaErrorInvalidValue;
+    if (a.produced != nullptr) {
+      COLEARN_LAUNCH(twoshot_overlap_kernel<true>, n_blocks, 512, 0, s, a);
+      return cudaGetLastError();
+    }
+    COLEARN_LAUNCH(twoshot_fedavg_kernel<true>, n_blocks, 512, 0, s, a);
     return cudaGetLastError();
   }
-  COLEARN_LAUNCH(twoshot_fedavg_kernel, n_blocks, 512, 0, s, a);
+  if (a.produced != nullptr) {
+    COLEARN_LAUNCH(twoshot_overlap_kernel<false>, n_blocks, 512, 0, s, a);
+    return cudaGetLastError();
+  }
+  COLEARN_LAUNCH(twoshot_fedavg_kernel<false>, n_blocks, 512, 0, s, a);
   return cudaGetLastError();
 }
 
@@ -666,7 +708,8 @@ COLEARN_DEFINE_SPIN_LIMIT_SETTER(set_spin_limit_comm)
 cudaError_t preload_comm_kernels() {
 #ifndef COLEARN_HOST_SHIM
   cudaFuncAttributes attr;
-  const void* kernels[] = {(const void*)star_round_kernel, (const void*)twoshot_fedavg_kernel, (const void*)twoshot_overlap_kernel,
+  const void* kernels[] = {(const void*)star_round_kernel<false>, (const void*)star_round_kernel<true>, (const void*)twoshot_fedavg_kernel<false>,
+                           (const void*)twoshot_fedavg_kernel<true>, (const void*)twoshot_overlap_kernel<false>, (const void*)twoshot_overlap_kernel<true>,
                            (const void*)produced_mark_kernel, (const void*)twoshot_resync_kernel, (const void*)reduce_push_kernel, (const void*)set_flag_kernel,
                            (const void*)signal_peers_kernel, (const void*)wait_flag_kernel, (const void*)wait_flags_kernel,
                            (const void*)wait_flags_dev_kernel, (const void*)p2p_copy_kernel};

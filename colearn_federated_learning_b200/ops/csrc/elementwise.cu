@@ -139,6 +139,41 @@ __global__ void fedavg_kernel(float* __restrict__ theta, const float* __restrict
   }
 }
 
+// FedAvg average (same weights, same summation order as fedavg_kernel) followed by a server optimizer step (server_opt.cuh)
+// on theta with the moments opt.m[n] / opt.v[n]: Coordinator-side FedAvgM / FedAdagrad / FedAdam / FedYogi in one pass
+__global__ void fedavg_opt_kernel(float* __restrict__ theta, const float* __restrict__ slots, int64_t slot_stride,
+                                  const float* __restrict__ weights, int k, ServerOptArgs opt, int64_t n) {
+  constexpr int kSw = 256;
+  __shared__ float sw[kSw];
+  for (int c = threadIdx.x; c < k && c < kSw; c += blockDim.x) sw[c] = weights[c];
+  __syncthreads();
+  auto wt = [&](int c) -> float { return c < kSw ? sw[c] : __ldg(weights + c); };
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool aligned = (((uintptr_t)theta | (uintptr_t)slots | (uintptr_t)opt.m | (uintptr_t)opt.v) & 15) == 0 && (slot_stride & 3) == 0;
+  int64_t scalar_from = 0;
+  if (aligned) {
+    const int64_t n4 = n >> 2;
+    for (int64_t j = i0; j < n4; j += stride) {
+      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int c = 0; c < k; ++c) {
+        const float4 v = __ldcs(reinterpret_cast<const float4*>(slots + c * slot_stride) + j);
+        const float w = wt(c);
+        acc.x = fmaf(w, v.x, acc.x); acc.y = fmaf(w, v.y, acc.y);
+        acc.z = fmaf(w, v.z, acc.z); acc.w = fmaf(w, v.w, acc.w);
+      }
+      float4* t4 = reinterpret_cast<float4*>(theta) + j;
+      *t4 = server_opt_step4(opt, j, *t4, acc);
+    }
+    scalar_from = n4 << 2;
+  }
+  for (int64_t j = scalar_from + i0; j < n; j += stride) {
+    float acc = 0.f;
+    for (int c = 0; c < k; ++c) acc = fmaf(wt(c), slots[c * slot_stride + j], acc);
+    theta[j] = server_opt_step(opt, j, theta[j], acc);
+  }
+}
+
 // ---- losses ---------------------------------------------------------------------------------------
 __global__ void sigmoid_bce_kernel(const float* __restrict__ z, const float* __restrict__ y,
                                    float* __restrict__ dz, float* __restrict__ loss_out, int64_t n) {
@@ -448,6 +483,13 @@ cudaError_t launch_fedavg_apply(float* theta, const float* slots, int64_t slot_s
                                 int k, float server_lr, int64_t n, cudaStream_t s) {
   if (k < 1) return cudaErrorInvalidValue;
   COLEARN_LAUNCH(fedavg_kernel<true>, grid_for(n), kThreads, 0, s, theta, slots, slot_stride, weights, k, server_lr, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_fedavg_apply_opt(float* theta, const float* slots, int64_t slot_stride, const float* weights, int k,
+                                    const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
+  if (k < 1 || !server_opt_args_ok(opt)) return cudaErrorInvalidValue;
+  if (opt.kind == SOPT_SGD) return launch_fedavg_apply(theta, slots, slot_stride, weights, k, opt.lr, n, s);
+  COLEARN_LAUNCH(fedavg_opt_kernel, grid_for(n), kThreads, 0, s, theta, slots, slot_stride, weights, k, opt, n);
   return cudaGetLastError();
 }
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride, const float* weights,

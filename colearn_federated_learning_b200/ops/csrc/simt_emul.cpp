@@ -95,10 +95,33 @@ Tensor mlp_forward(int64_t net_kind, Tensor theta, Tensor x, int64_t d_out) {
 float* fmut(Tensor& t, const char* name) { return const_cast<float*>(fptr(t, name)); }
 
 void sgd_step(Tensor p, Tensor g, double lr) { CK(colearn::launch_sgd_step(fmut(p, "p"), fptr(g, "g"), (float)lr, p.numel(), nullptr)); }
-void fedavg_apply(Tensor theta, Tensor slots, Tensor w, double server_lr) {
+// server optimizer (server_opt.cuh): kind 0 = plain server_lr; hyper = [beta1, beta2, tau]; m / v: CPU fp32 moment buffers of n floats
+colearn::ServerOptArgs server_opt_args(int64_t kind, double lr, const std::vector<double>& hyper, c10::optional<Tensor>& m,
+                                       c10::optional<Tensor>& v, int64_t n) {
+  colearn::ServerOptArgs o;
+  memset(&o, 0, sizeof(o));
+  o.kind = (int)kind;
+  o.lr = (float)lr;
+  if (kind != colearn::SOPT_SGD) {
+    TORCH_CHECK(hyper.size() == 3, "hyper = [beta1, beta2, tau]");
+    o.beta1 = (float)hyper[0]; o.beta2 = (float)hyper[1]; o.tau = (float)hyper[2];
+    if (m.has_value()) { TORCH_CHECK(m->numel() >= n, "m size"); o.m = fmut(*m, "m"); }
+    if (v.has_value()) { TORCH_CHECK(v->numel() >= n, "v size"); o.v = fmut(*v, "v"); }
+  }
+  TORCH_CHECK(colearn::server_opt_args_ok(o), "server optimizer: unknown kind or a moment buffer missing / misaligned");
+  return o;
+}
+void fedavg_apply(Tensor theta, Tensor slots, Tensor w, double server_lr, int64_t opt_kind, std::vector<double> opt_hyper,
+                  c10::optional<Tensor> m, c10::optional<Tensor> v) {
   TORCH_CHECK(slots.dim() == 2 && slots.size(1) == theta.numel() && w.numel() == slots.size(0), "slots [K, P], weights [K]");
-  CK(colearn::launch_fedavg_apply(fmut(theta, "theta"), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0),
-                                  (float)server_lr, theta.numel(), nullptr));
+  if (opt_kind == colearn::SOPT_SGD) {
+    CK(colearn::launch_fedavg_apply(fmut(theta, "theta"), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0),
+                                    (float)server_lr, theta.numel(), nullptr));
+    return;
+  }
+  const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, theta.numel());
+  CK(colearn::launch_fedavg_apply_opt(fmut(theta, "theta"), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0), o,
+                                      theta.numel(), nullptr));
 }
 Tensor fedavg_flat(Tensor slots, Tensor w) {
   Tensor out = torch::zeros({slots.size(1)}, torch::kFloat);
@@ -172,7 +195,8 @@ Tensor ring_matmul(Tensor a, Tensor b) {
 // rank k's inbox), bcast flags int32 [W].  Returns the arrived mask (deadline mode) or the select mask.
 int64_t star_round(Tensor theta, Tensor slots, Tensor arrive, int64_t arrive_epoch, Tensor inboxes, Tensor bcast_flags, int64_t bcast_epoch,
                    int64_t select_mask, double server_lr, bool do_reduce, bool do_bcast, int64_t n_blocks, double timeout_ms,
-                   std::vector<double> weights) {
+                   std::vector<double> weights, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<Tensor> m,
+                   c10::optional<Tensor> v) {
   const int W = (int)slots.size(0);
   colearn::StarRoundArgs a;
   memset(&a, 0, sizeof(a));
@@ -197,6 +221,7 @@ int64_t star_round(Tensor theta, Tensor slots, Tensor arrive, int64_t arrive_epo
   a.grid_counter = &counter;
   a.timeout_ns = (unsigned long long)(timeout_ms * 1e6);
   a.decision = decision;
+  a.opt = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, a.n);
   {
     py::gil_scoped_release nogil;
     CK(colearn::launch_star_round(a, (int)n_blocks, nullptr));
@@ -208,7 +233,8 @@ int64_t star_round(Tensor theta, Tensor slots, Tensor arrive, int64_t arrive_epo
 // int32 [W, n_chunks]; `arrive` (this rank's int32 [W]) must already carry `epoch` for every selected rank.
 void twoshot_fedavg(int64_t rank, Tensor works, c10::optional<Tensor> shadows, Tensor chunk_flags, Tensor arrive, Tensor weights,
                     c10::optional<Tensor> theta_prev, int64_t epoch, int64_t select_mask, double server_lr, int64_t chunk_elems, int64_t n_blocks,
-                    c10::optional<Tensor> produced, double produced_timeout_s) {
+                    c10::optional<Tensor> produced, double produced_timeout_s, int64_t opt_kind, std::vector<double> opt_hyper,
+                    c10::optional<Tensor> m, c10::optional<Tensor> v) {
   const int W = (int)works.size(0);
   colearn::TwoShotArgs a;
   memset(&a, 0, sizeof(a));
@@ -232,6 +258,8 @@ void twoshot_fedavg(int64_t rank, Tensor works, c10::optional<Tensor> shadows, T
     a.produced = reinterpret_cast<const uint32_t*>(produced->data_ptr<int>()) + rank * W * produced->size(2);
     a.produced_timeout_ns = produced_timeout_s > 0 ? (unsigned long long)(produced_timeout_s * 1e9) : 0ull;
   }
+  a.opt = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, a.n);     // this rank's moment buffers (it touches the chunks it owns)
+  TORCH_CHECK(a.opt.kind == colearn::SOPT_SGD || a.theta_prev != nullptr, "a server optimizer needs theta_prev");
   {
     py::gil_scoped_release nogil;
     CK(colearn::launch_twoshot_fedavg(a, (int)n_blocks, nullptr));
@@ -384,7 +412,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mlp_forward", &mlp_forward);
   m.def("mlp_net_params", [](int64_t kind) { return (int64_t)colearn::mlp_net_num_params((int)kind); });
   m.def("sgd_step", &sgd_step);
-  m.def("fedavg_apply", &fedavg_apply);
+  // trailing server-optimizer arguments default to plain FedAvg (the shorter positional calls keep working)
+  m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("w"), py::arg("server_lr"), py::arg("opt_kind") = 0,
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);
@@ -396,8 +426,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("feistel_permutation", &feistel_permutation);
   m.def("transpose_bf16", &transpose_bf16);
   m.def("ring_matmul", &ring_matmul);
-  m.def("star_round", &star_round);
-  m.def("twoshot_fedavg", &twoshot_fedavg);
+  m.def("star_round", &star_round, py::arg("theta"), py::arg("slots"), py::arg("arrive"), py::arg("arrive_epoch"), py::arg("inboxes"),
+        py::arg("bcast_flags"), py::arg("bcast_epoch"), py::arg("select_mask"), py::arg("server_lr"), py::arg("do_reduce"), py::arg("do_bcast"),
+        py::arg("n_blocks"), py::arg("timeout_ms"), py::arg("weights"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
+        py::arg("m") = py::none(), py::arg("v") = py::none());
+  m.def("twoshot_fedavg", &twoshot_fedavg, py::arg("rank"), py::arg("works"), py::arg("shadows"), py::arg("chunk_flags"), py::arg("arrive"),
+        py::arg("weights"), py::arg("theta_prev"), py::arg("epoch"), py::arg("select_mask"), py::arg("server_lr"), py::arg("chunk_elems"),
+        py::arg("n_blocks"), py::arg("produced"), py::arg("produced_timeout_s"), py::arg("opt_kind") = 0,
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
   m.def("twoshot_fedavg_deadline", &twoshot_fedavg_deadline);
   m.def("twoshot_resync", &twoshot_resync);
   m.def("produced_signal_pack", &produced_signal_pack);

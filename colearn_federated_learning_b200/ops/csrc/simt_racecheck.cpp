@@ -97,6 +97,11 @@ int main() {
     a.bcast_epoch = 6; a.select_mask = 7; a.world = W; a.server_lr = 1.f; a.n = P; a.do_reduce = 1; a.do_bcast = 1;
     a.grid_counter = &counter; a.timeout_ns = 5000000ull; a.decision = decision.data();
     CK(launch_star_round(a, 3, nullptr));
+    // the same round with a server optimizer (FedAdam): moments read and written next to theta, float4 body + scalar tail
+    std::vector<float> m(P, 0.f), v(P, 1e-6f);
+    a.opt.kind = SOPT_ADAM; a.opt.lr = 0.01f; a.opt.beta1 = 0.9f; a.opt.beta2 = 0.99f; a.opt.tau = 1e-3f;
+    a.opt.m = m.data(); a.opt.v = v.data(); a.arrive_epoch = 5; a.bcast_epoch = 7;
+    CK(launch_star_round(a, 3, nullptr));
     const int64_t n = 4 * 200, chunk = 64;
     std::vector<float> works = randv((size_t)W * n), weights(W, 1.f / W);
     std::vector<uint32_t> cflags((size_t)W * ((n + chunk - 1) / chunk), 0), arr(W, 2);
@@ -106,6 +111,18 @@ int main() {
       for (int k = 0; k < W; ++k) { t.work[k] = works.data() + (size_t)k * n; t.chunk_flags[k] = cflags.data() + (size_t)k * ((n + chunk - 1) / chunk); }
       t.arrive_flags = arr.data(); t.weights = weights.data(); t.epoch = 2; t.select_mask = 7; t.server_lr = 1.f; t.n = n; t.chunk_elems = chunk;
       t.world = W; t.rank = r;
+      CK(launch_twoshot_fedavg(t, 2, nullptr));
+    }
+    // two-shot with FedAdam: every rank keeps theta_prev and the moments of the chunks it owns
+    std::vector<float> prevs = randv((size_t)W * n), ms((size_t)W * n, 0.f), vs((size_t)W * n, 1e-6f);
+    for (int r = 0; r < W; ++r) {
+      TwoShotArgs t;
+      memset(&t, 0, sizeof(t));
+      for (int k = 0; k < W; ++k) { t.work[k] = works.data() + (size_t)k * n; t.chunk_flags[k] = cflags.data() + (size_t)k * ((n + chunk - 1) / chunk); }
+      t.arrive_flags = arr.data(); t.weights = weights.data(); t.epoch = 2; t.select_mask = 7; t.server_lr = 0.01f; t.n = n; t.chunk_elems = chunk;
+      t.world = W; t.rank = r; t.theta_prev = prevs.data() + (size_t)r * n;
+      t.opt.kind = SOPT_ADAM; t.opt.lr = 0.01f; t.opt.beta1 = 0.9f; t.opt.beta2 = 0.99f; t.opt.tau = 1e-3f;
+      t.opt.m = ms.data() + (size_t)r * n; t.opt.v = vs.data() + (size_t)r * n;
       CK(launch_twoshot_fedavg(t, 2, nullptr));
     }
     std::vector<float> dst(P), lsrc = randv(2 * W), ldst(2);

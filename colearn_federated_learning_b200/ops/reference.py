@@ -188,6 +188,35 @@ def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tenso
     return theta.add_(server_lr * (avg - theta))
 
 
+def server_opt_step(theta: torch.Tensor, avg: torch.Tensor, kind: str, lr: float, m=None, v=None, beta1: float = 0.9,
+                    beta2: float = 0.99, tau: float = 1e-3) -> torch.Tensor:
+    """One server optimizer step towards the FedAvg average ``avg`` (``fl/server_opt.py`` has the table), in place on
+    ``theta`` and the moments ``m`` / ``v``.  ``sgd`` is exactly :func:`fedavg_apply`'s update."""
+    d = avg - theta
+    if kind == "sgd":
+        return theta.add_(lr * d)
+    if kind == "avgm":
+        m.mul_(beta1).add_(d)
+        return theta.add_(lr * m)
+    m.mul_(beta1).add_((1.0 - beta1) * d)
+    d2 = d * d
+    if kind == "adagrad":
+        v.add_(d2)
+    elif kind == "adam":
+        v.mul_(beta2).add_((1.0 - beta2) * d2)
+    elif kind == "yogi":
+        v.sub_((1.0 - beta2) * d2 * torch.sign(v - d2))
+    else:
+        raise ValueError(f"unknown server optimizer {kind!r}")
+    return theta.add_(lr * m / (v.sqrt() + tau))
+
+
+def server_opt_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor, kind: str, lr: float, m=None, v=None,
+                     beta1: float = 0.9, beta2: float = 0.99, tau: float = 1e-3) -> torch.Tensor:
+    """``avg = sum_k w_k models[k]`` then :func:`server_opt_step` (the oracle of the fused kernels)."""
+    return server_opt_step(theta, fedavg_flat(models, weights), kind, lr, m, v, beta1, beta2, tau)
+
+
 def linear_bias_relu(x, w, b, relu=True):
     y = x.float() @ w.float().t() + b.float()
     return torch.relu(y) if relu else y

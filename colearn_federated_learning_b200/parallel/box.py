@@ -373,9 +373,11 @@ class BoxService:
         if self.rounds > 1 and max_batches < 0:
             max_batches = ROUND_MODE_BATCHES          # fc.py:533-535
         on_gpu = backend != "cpu" and device.type == "cuda"
+        sgd = getattr(args, "server_opt", "sgd") == "sgd"        # plain FedAvg: server_lr as before; else the ServerOpt carries it
         self.engine = FederatedEngine(args.model, backend=backend, device=device, batch_size=args.batch_size, lr=args.lr,
                                       local_epochs=args.epochs, max_batches=max_batches, loss=args.loss, weighted=args.weighted,
-                                      server_lr=args.server_lr, seed=args.seed,
+                                      server_lr=args.server_lr if sgd else 1.0, seed=args.seed,
+                                      server_opt=None if sgd else args.server_optimizer(),
                                       bf16_shadow=on_gpu and getattr(args, "dtype", "fp32") == "bf16",
                                       clients_per_rank=getattr(cli, "clients_per_gpu", 1) if on_gpu else 1,
                                       round_deadline_ms=float(getattr(cli, "round_deadline_ms", 0.0) or 0.0))

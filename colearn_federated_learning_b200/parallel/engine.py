@@ -34,6 +34,7 @@ import torch.nn as nn
 
 from .. import ops
 from ..fl.fedavg import normalized_weights
+from ..fl.server_opt import ServerOpt, resolve_server_opt
 from ..fl.trainer import FitConfig, local_fit, resolve_loss
 from ..models import MLPNet, build_model, flatten_params, num_params, state_dict_from_flat
 from ..utils.checkpoint import save_state_dict
@@ -68,7 +69,7 @@ class FederatedEngine:
                  shuffle: bool = True, chunk_elems: int = 0, bf16_shadow: bool = False,
                  round_deadline_ms: float = 0.0, clients_per_rank: int = 1,
                  model_kwargs: Optional[Dict[str, Any]] = None, overlap_reduce: Optional[bool] = None,
-                 phase_timing: Optional[bool] = None) -> None:
+                 phase_timing: Optional[bool] = None, server_opt: Optional[ServerOpt] = None) -> None:
         self.rank = dist.get_rank(group) if _dist_ready() else 0
         self.world = dist.get_world_size(group) if _dist_ready() else 1
         self.group = group
@@ -93,7 +94,9 @@ class FederatedEngine:
         self.cfg = FitConfig(model=model, loss=resolve_loss(model, loss), batch_size=batch_size, epochs=local_epochs,
                              max_nr_batches=max_batches, lr=lr, shuffle=shuffle, seed=seed)
         self.weighted = weighted
-        self.server_lr = server_lr
+        # server optimizer (fl/server_opt.py): plain FedAvg with server_lr unless a ServerOpt is given (it carries its own lr)
+        self.server_opt = resolve_server_opt(server_opt, server_lr)
+        self.server_lr = self.server_opt.lr
         self.seed = seed
         persistent = self.spec is not None and ops.net_kind_for(self.spec.dims, self.spec.out_activation) is not None
         if algo == "auto":
@@ -101,6 +104,11 @@ class FederatedEngine:
         if algo == "star" and backend == "fused" and not persistent:
             raise ValueError(f"algo 'star' needs a persistent-kernel model, got {model}")
         self.algo = algo
+        if algo == "twoshot" and round_deadline_ms > 0 and self.server_opt.kind != "sgd":
+            raise ValueError(f"server_opt={self.server_opt.kind!r} cannot run on the two-shot path with a round deadline: the "
+                             "optimizer moments are sharded by chunk owner, and with a deadline chunk ownership moves with the set "
+                             "of ranks that arrived, so a moment would land on a rank that does not hold it; use server_opt 'sgd' "
+                             "or no deadline")
         if not chunk_elems:
             # flag/work granularity of the two-shot kernel: >= ~2 CTAs per SM worth of chunks per rank
             target = max(1, self.P4 // (self.world * 296))
@@ -145,6 +153,11 @@ class FederatedEngine:
         else:
             self.theta = flatten_params(self.model).to(self.device)
         self.model.to(self.device)
+        # moments of the server optimizer: the coordinator's on the star / CPU paths; on the two-shot path every rank holds a
+        # P4-sized buffer of which it reads and writes only the chunks it owns (c % world), next to its theta_prev
+        self.opt_state = None
+        if self.server_opt.kind != "sgd" and (self.rank == self.coord or (backend == "fused" and self.algo == "twoshot")):
+            self.opt_state = self.server_opt.init_state(self.P4 if backend == "fused" else self.P, self.device)
 
     # ------------------------------------------------------------------------------------------
     def _init_fused(self) -> None:
@@ -214,6 +227,21 @@ class FederatedEngine:
             self.counts = [int(c) for c in gathered]
         else:
             self.counts = [self.n_local]
+
+    def server_state(self) -> Dict[str, Optional[torch.Tensor]]:
+        """This rank's server optimizer moments ``{"m", "v"}`` (first P elements; None where the kind or the rank has none).
+        Two-shot path: only the chunks this rank owns are ever updated."""
+        st = self.opt_state
+        if st is None:
+            return {"m": None, "v": None}
+        return {"m": st.m[: self.P], "v": st.v[: self.P] if st.v is not None else None}
+
+    def _opt_args(self) -> Tuple[int, List[float], int, int]:
+        """Trailing server-optimizer arguments of the star / two-shot bindings: (kind code, [beta1, beta2, tau], m, v)."""
+        st = self.opt_state
+        if st is None:
+            return 0, [], 0, 0
+        return st.code, st.hyper, st.m.data_ptr(), st.v.data_ptr() if st.v is not None else 0
 
     def load_global(self, flat: torch.Tensor) -> None:
         self.theta[: self.P].copy_(flat.to(self.device).float().reshape(-1)[: self.P])
@@ -323,7 +351,16 @@ class FederatedEngine:
             contrib = local * w
         if _dist_ready() and W > 1:
             dist.reduce(contrib, dst=self.coord, group=self.group)                       # K2 + K3, library form
-        expected = theta0 + self.server_lr * (contrib - theta0)
+        if self.opt_state is None:
+            expected = theta0 + self.server_lr * (contrib - theta0)
+        else:
+            # the optimizer step on a copy of the coordinator's moments (the fused round below updates the real ones)
+            expected = theta0.clone()
+            if r == self.coord and mask != 0:
+                st, P = self.opt_state, self.P
+                b1, b2, tau = st.hyper
+                ops.reference.server_opt_step(expected, contrib, st.kind, st.lr, st.m[:P].clone(),
+                                              st.v[:P].clone() if st.v is not None else None, b1, b2, tau)
         rep = self.run_rounds(1, masks=mask)
         got = self.theta[: self.P]
         out: Dict[str, Any] = {"algo": self.algo, "provider": rep.extra.get("provider"), "multicast": rep.extra.get("multicast"),
@@ -429,16 +466,20 @@ class FederatedEngine:
             ring_ev = self._ring_ev
             self.loss_history: List[torch.Tensor] = []
 
+        opt_kind, opt_hyper, opt_m, opt_v = self._opt_args()
+
         def star(do_reduce: bool, do_bcast: bool, mask_reduce: int, mask_bcast: int, arrive_epoch: int, bcast_epoch: int):
             wts = [float(v) for v in self._round_weights(mask_reduce)] if do_reduce else [0.0] * W
             # reduce over the workers of the finished round, broadcast to those of the next one
             if do_reduce and do_bcast and mask_reduce != mask_bcast:
                 ext.star_round(self.theta.data_ptr(), arena.ptr("slots"), P4, arena.ptr("flags", None, 1), arrive_epoch,
                                inbox_ptrs, bflag_ptrs, bcast_epoch, 0, mask_reduce, self.server_lr, P4, True, False,
-                               self.grid_counter.data_ptr(), n_blocks, self.round_deadline_ms, wts, self.decision.data_ptr())
+                               self.grid_counter.data_ptr(), n_blocks, self.round_deadline_ms, wts, self.decision.data_ptr(),
+                               opt_kind, opt_hyper, opt_m, opt_v)
                 ext.star_round(self.theta.data_ptr(), arena.ptr("slots"), P4, arena.ptr("flags", None, 1), arrive_epoch,
                                inbox_ptrs, bflag_ptrs, bcast_epoch, arena.mc_ptr("inbox"),
-                               mask_bcast, self.server_lr, P4, False, True, self.grid_counter.data_ptr(), n_blocks, 0.0, wts, 0)
+                               mask_bcast, self.server_lr, P4, False, True, self.grid_counter.data_ptr(), n_blocks, 0.0, wts, 0,
+                               opt_kind, opt_hyper, opt_m, opt_v)
                 return 2
             mask = mask_reduce if do_reduce else mask_bcast
             # NVLS broadcast also for a subset: multimem.st lands in every rank's inbox (one egress copy, the switch replicates);
@@ -447,7 +488,7 @@ class FederatedEngine:
             ext.star_round(self.theta.data_ptr(), arena.ptr("slots"), P4, arena.ptr("flags", None, 1), arrive_epoch,
                            inbox_ptrs, bflag_ptrs, bcast_epoch, mc, mask, self.server_lr, P4, do_reduce, do_bcast,
                            self.grid_counter.data_ptr(), n_blocks, self.round_deadline_ms if do_reduce else 0.0, wts,
-                           self.decision.data_ptr())
+                           self.decision.data_ptr(), opt_kind, opt_hyper, opt_m, opt_v)
             return 1
 
         self._phases_begin()
@@ -510,7 +551,8 @@ class FederatedEngine:
         return RoundReport(rounds, W, "fused", "star", ev0.elapsed_time(ev1), losses_log, launches,
                            bytes_bcast=4 * self.P * sum(nsel), bytes_reduce=4 * self.P * sum(nsel),
                            extra={"provider": arena.provider, "multicast": arena.has_multicast, "phases_ms": phases,
-                                  "arrived_masks": arrived_log.tolist() if (is_coord and self.round_deadline_ms > 0) else None})
+                                  "arrived_masks": arrived_log.tolist() if (is_coord and self.round_deadline_ms > 0) else None,
+                                  "server_opt": self.server_opt.kind})
 
     # ------------------------------------------------------------------------------------------ twoshot
     def _layerwise_trainer(self):
@@ -608,10 +650,12 @@ class FederatedEngine:
         if deadline:
             assert self.coord == 0, "the two-shot deadline protocol takes rank 0 as the coordinator"
             decision_ptrs, global_ptrs = arena.peer_ptrs("decision"), arena.peer_ptrs("global")
-        use_prev = abs(self.server_lr - 1.0) > 1e-12
+        use_prev = abs(self.server_lr - 1.0) > 1e-12 or self.opt_state is not None
+        opt_kind, opt_hyper, opt_m, opt_v = self._opt_args()
         if use_prev and getattr(self, "theta_prev", None) is None:
-            # server_lr != 1: theta <- theta + lr_s (sum_k w_k theta_k - theta) needs the model the round started from, and the
-            # ranks train IN PLACE on the arena — every rank keeps a copy (one local P-element pass per round)
+            # server_lr != 1 or a server optimizer: theta <- theta + lr_s (sum_k w_k theta_k - theta) (or the optimizer step) needs
+            # the model the round started from, and the ranks train IN PLACE on the arena — every rank keeps a copy (one local
+            # P-element pass per round)
             self.theta_prev = torch.empty(P4, device=dev)
         work_ptrs = arena.peer_ptrs("work")
         shadow_ptrs = arena.peer_ptrs("shadow") if self.bf16_shadow else []
@@ -679,7 +723,7 @@ class FederatedEngine:
                                    arrive_ptrs if not produced_ptr else [], need_wait,
                                    arena.mc_ptr("work") if nvls else 0,
                                    arena.mc_ptr("shadow") if (nvls and self.bf16_shadow) else 0,
-                                   produced_ptr, self.overlap_timeout_s if produced_ptr else 0.0)
+                                   produced_ptr, self.overlap_timeout_s if produced_ptr else 0.0, opt_kind, opt_hyper, opt_m, opt_v)
 
             # fused wgrad -> FedAvg reduce: every rank trains this round, so every rank's last backward reports its chunks
             prod = self._produced_spec() if (masks[i] == full and not prescale and not deadline) else None
@@ -731,7 +775,7 @@ class FederatedEngine:
                            bytes_bcast=4 * self.P * sum(nsel), bytes_reduce=4 * self.P * sum(nsel),
                            extra={"provider": arena.provider, "train_path": getattr(self, "_last_path", None), "phases_ms": phases,
                                   "n_chunks": self.n_chunks, "nvls": getattr(self, "_last_nvls", False),
-                                  "arrived_masks": getattr(self, "_arrived_masks", None)})
+                                  "arrived_masks": getattr(self, "_arrived_masks", None), "server_opt": self.server_opt.kind})
 
     # ------------------------------------------------------------------------------------------ cpu / gloo
     def _run_cpu(self, rounds: int, masks: List[int]) -> RoundReport:
@@ -757,10 +801,15 @@ class FederatedEngine:
                     dist.reduce(contrib, dst=self.coord, group=self.group)                 # K2 + K3
                     dist.reduce(lvec, dst=self.coord, group=self.group)
                 if r == self.coord:
-                    self.theta.add_(self.server_lr * (contrib - self.theta))
+                    st = self.opt_state
+                    if st is None:
+                        self.theta.add_(self.server_lr * (contrib - self.theta))
+                    elif masks[i] != 0:                  # (nobody selected: theta and the moments stay)
+                        b1, b2, tau = st.hyper
+                        ops.reference.server_opt_step(self.theta, contrib, st.kind, st.lr, st.m, st.v, b1, b2, tau)
                     losses_log[i] = lvec
         self.rounds_done += rounds
         nsel = [bin(m).count("1") for m in masks]
         return RoundReport(rounds, W, "cpu", "gloo", (time.perf_counter() - t0) * 1e3, losses_log, 0,
                            bytes_bcast=4 * self.P * sum(nsel), bytes_reduce=4 * self.P * sum(nsel),
-                           extra={"phases_ms": self._phases_end()})
+                           extra={"phases_ms": self._phases_end(), "server_opt": self.server_opt.kind})

@@ -46,7 +46,14 @@ def build_parser() -> argparse.ArgumentParser:
     parser.add_argument("--local-epochs", type=int, default=d.epochs)
     parser.add_argument("--max-batches", type=int, default=d.federate_after_n_batches, help="local SGD steps per round (-1 = full epoch; rounds>1 default to 1000)")
     parser.add_argument("--lr", type=float, default=d.lr)
-    parser.add_argument("--server-lr", type=float, default=d.server_lr)
+    parser.add_argument("--server-lr", type=float, default=None,
+                        help="server learning rate (default: 1.0 for --server-opt sgd / avgm, 0.01 for adagrad / adam / yogi)")
+    parser.add_argument("--server-opt", choices=["sgd", "avgm", "adagrad", "adam", "yogi"], default=d.server_opt,
+                        help="server optimizer on top of the FedAvg average: sgd = plain FedAvg, avgm = server momentum, "
+                             "adagrad / adam / yogi = adaptive (Reddi et al. 2021); its state is not checkpointed")
+    parser.add_argument("--server-beta1", type=float, default=d.server_beta1, help="first-moment decay of --server-opt, in [0, 1)")
+    parser.add_argument("--server-beta2", type=float, default=d.server_beta2, help="second-moment decay of adam / yogi, in [0, 1)")
+    parser.add_argument("--server-tau", type=float, default=d.server_tau, help="adaptivity of adagrad / adam / yogi (> 0)")
     parser.add_argument("--seed", type=int, default=d.seed)
     parser.add_argument("--log-interval", type=int, default=d.log_interval)
     parser.add_argument("--test-path", type=str, default=d.test_path, help="CSV used by local/encrypted mode and evaluation")
@@ -100,7 +107,14 @@ def build_parser() -> argparse.ArgumentParser:
 def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a = Arguments()
     a.model, a.loss, a.batch_size, a.epochs = ns.model, ns.loss, ns.batch_size, ns.local_epochs
-    a.federate_after_n_batches, a.lr, a.server_lr, a.seed = ns.max_batches, ns.lr, ns.server_lr, ns.seed
+    a.federate_after_n_batches, a.lr, a.seed = ns.max_batches, ns.lr, ns.seed
+    from colearn_federated_learning_b200.fl.server_opt import default_server_lr
+    a.server_opt = getattr(ns, "server_opt", "sgd")
+    a.server_lr = ns.server_lr if ns.server_lr is not None else default_server_lr(a.server_opt)
+    a.server_beta1 = getattr(ns, "server_beta1", a.server_beta1)
+    a.server_beta2 = getattr(ns, "server_beta2", a.server_beta2)
+    a.server_tau = getattr(ns, "server_tau", a.server_tau)
+    a.server_optimizer()              # rejects a beta outside [0, 1) / tau <= 0 before anything starts
     a.log_interval, a.test_path, a.synthetic, a.weighted = ns.log_interval, ns.test_path, ns.synthetic, ns.weighted
     a.no_cuda, a.backend = ns.no_cuda, ns.backend
     if getattr(ns, "enc_items", None):
@@ -181,7 +195,13 @@ def parse_cli(argv=None) -> argparse.Namespace:
     if known.plugin:
         from colearn_federated_learning_b200.models import load_plugins
         load_plugins(known.plugin)
-    return build_parser().parse_args(argv)
+    parser = build_parser()
+    ns = parser.parse_args(argv)
+    try:
+        arguments_from_cli(ns)           # the server optimizer settings (beta in [0, 1), tau > 0)
+    except ValueError as e:
+        parser.error(str(e))
+    return ns
 
 
 if __name__ == "__main__":
