@@ -38,6 +38,8 @@ class Arguments:
     server_beta1: float = 0.9
     server_beta2: float = 0.99
     server_tau: float = 1e-3
+    aggregator: str = "mean"       # mean (weighted FedAvg) | median | trimmed_mean (fl/aggregate.py; unweighted, Byzantine-robust)
+    trim_fraction: float = 0.1     # trimmed_mean: fraction of the values dropped at each end, in [0, 0.5)
     backend: str = "auto"          # auto | fused | nccl | cpu
     dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the wgmma consumers)
     save_every: int = 0            # >0: checkpoint every N rounds, not only after the last one
@@ -50,6 +52,14 @@ class Arguments:
         """The :class:`fl.server_opt.ServerOpt` these arguments describe (``server_lr`` is its learning rate)."""
         from ..fl.server_opt import ServerOpt
         return ServerOpt(self.server_opt, lr=self.server_lr, beta1=self.server_beta1, beta2=self.server_beta2, tau=self.server_tau)
+
+    def client_aggregator(self):
+        """The :class:`fl.aggregate.Aggregator` these arguments describe; a robust kind refuses ``weighted`` (it is unweighted)."""
+        from ..fl.aggregate import Aggregator
+        agg = Aggregator(self.aggregator, self.trim_fraction)
+        if agg.robust and self.weighted:
+            raise ValueError(f"--weighted does not apply to aggregator {self.aggregator!r}: the median / trimmed mean are unweighted")
+        return agg
 
     def set_federated_batches(self, batches: int) -> None:
         self.federate_after_n_batches = batches

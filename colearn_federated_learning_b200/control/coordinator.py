@@ -446,9 +446,11 @@ class Coordinator(BusClient):
         return theta
 
     def _server_update(self, theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor) -> None:
-        """FedAvg of ``models`` into ``theta`` in place, followed by the server optimizer step of ``--server-opt``."""
+        """FedAvg of ``models`` into ``theta`` in place (or their median / trimmed mean, ``--aggregator``), followed by the
+        server optimizer step of ``--server-opt``."""
+        agg = self.args.client_aggregator()
         if self.args.server_opt == "sgd":
-            ops.fedavg_apply(theta, models, weights, self.args.server_lr)
+            ops.fedavg_apply(theta, models, weights, self.args.server_lr, aggregator=agg)
             return
         opt = self.args.server_optimizer()
         st = self._server_opt_state
@@ -459,13 +461,14 @@ class Coordinator(BusClient):
         if st.m.device != theta.device:
             st.m = st.m.to(theta.device)
             st.v = st.v.to(theta.device) if st.v is not None else None
-        ops.fedavg_apply(theta, models, weights, opt=st)
+        ops.fedavg_apply(theta, models, weights, opt=st, aggregator=agg)
 
     @staticmethod
     def _average_buffers(model, buffers, weights) -> None:
         """BatchNorm models in remote mode: the devices return their running statistics next to the parameters; the global
         model gets their FedAvg-weighted mean (PySyft's federated_avg averages parameters only — with it the reference could
-        not train a BatchNorm model remotely at all; documented in docs/PARITY.md)."""
+        not train a BatchNorm model remotely at all; documented in docs/PARITY.md).  They keep this mean under a robust
+        ``--aggregator`` too: only the parameters get the median / trimmed mean."""
         mine = [b for b in model.buffers() if b.is_floating_point()]
         total = sum(b.numel() for b in mine)
         if not mine or any(b is None or b.numel() != total or not bool(torch.isfinite(b).all()) for b in buffers):

@@ -35,24 +35,34 @@ def fedavg_flat(models: torch.Tensor, weights: torch.Tensor) -> torch.Tensor:
     return reference.fedavg_flat(models, weights)
 
 
-def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor, server_lr: float = 1.0, opt=None) -> torch.Tensor:
+def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor, server_lr: float = 1.0, opt=None,
+                 aggregator=None) -> torch.Tensor:
     """``theta += server_lr * (sum_k w_k models[k] - theta)`` in place (reduce + scale + apply fused).
 
     ``opt``: a :class:`fl.server_opt.ServerOptState` — the average is followed by that server optimizer's step (FedAvgM /
-    FedAdagrad / FedAdam / FedYogi) in the same kernel, with the optimizer's own ``lr``; its moments are updated in place."""
+    FedAdagrad / FedAdam / FedYogi) in the same kernel, with the optimizer's own ``lr``; its moments are updated in place.
+
+    ``aggregator``: a robust :class:`fl.aggregate.Aggregator` (``median`` / ``trimmed_mean``) replaces the weighted sum by
+    the coordinate-wise median / trimmed mean of the K models in the same kernel (``weights`` are then not used)."""
+    robust = aggregator is not None and aggregator.robust
     if opt is not None:
         if float(server_lr) != 1.0:
             raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
         if _cuda(theta):
+            ext_args = (aggregator.code, aggregator.trim) if robust else ()
             _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(opt.lr),
-                                        opt.code, opt.hyper, opt.m, opt.v)
+                                        opt.code, opt.hyper, opt.m, opt.v, *ext_args)
             return theta
         b1, b2, tau = opt.hyper
-        return reference.server_opt_apply(theta, models, weights, opt.kind, opt.lr, opt.m, opt.v, b1, b2, tau)
+        return reference.server_opt_apply(theta, models, weights, opt.kind, opt.lr, opt.m, opt.v, b1, b2, tau, aggregator=aggregator)
     if _cuda(theta):
+        if robust:
+            _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(server_lr),
+                                        0, [], None, None, aggregator.code, aggregator.trim)
+            return theta
         _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(server_lr))
         return theta
-    return reference.fedavg_apply(theta, models, weights, server_lr)
+    return reference.fedavg_apply(theta, models, weights, server_lr, aggregator=aggregator)
 
 
 def sigmoid_bce(z: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:

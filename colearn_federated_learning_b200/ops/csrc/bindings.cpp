@@ -124,12 +124,23 @@ static ServerOptArgs server_opt_args(int64_t kind, double lr, const std::vector<
   return o;
 }
 
+// Aggregator of the FedAvg kernels (robust_agg.cuh): kind 0 = the weighted mean; 1 = median, 2 = trimmed mean (trim per end)
+static AggArgs agg_args(int64_t kind, double trim) {
+  AggArgs g;
+  std::memset(&g, 0, sizeof(g));
+  g.kind = (int)kind;
+  g.trim = (float)trim;
+  TORCH_CHECK(agg_args_ok(g), "aggregator: unknown kind ", kind, " or trim fraction ", trim, " outside [0, 0.5)");
+  return g;
+}
+
 void fedavg_apply(torch::Tensor theta, torch::Tensor slots, torch::Tensor weights, double server_lr, int64_t opt_kind,
-                  std::vector<double> opt_hyper, c10::optional<torch::Tensor> m, c10::optional<torch::Tensor> v) {
+                  std::vector<double> opt_hyper, c10::optional<torch::Tensor> m, c10::optional<torch::Tensor> v, int64_t agg_kind,
+                  double trim) {
   CHECK_CUDA_F32(theta); CHECK_CUDA_F32(slots); CHECK_CUDA_F32(weights);
   TORCH_CHECK(slots.dim() == 2 && slots.size(1) >= theta.numel() && weights.numel() == slots.size(0), "shapes");
   c10::cuda::CUDAGuard guard(theta.device());
-  if (opt_kind == SOPT_SGD) {
+  if (opt_kind == SOPT_SGD && agg_kind == AGG_MEAN) {
     check(launch_fedavg_apply(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(),
                               (int)slots.size(0), (float)server_lr, theta.numel(), cur_stream()), "fedavg_apply");
     return;
@@ -141,6 +152,12 @@ void fedavg_apply(torch::Tensor theta, torch::Tensor slots, torch::Tensor weight
     return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
   };
   const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
+  if (agg_kind != AGG_MEAN) {
+    // robust aggregate (unweighted: `weights` is not read), then the plain step or the server optimizer step
+    check(launch_fedavg_apply_robust(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), (int)slots.size(0),
+                                     agg_args(agg_kind, trim), o, theta.numel(), cur_stream()), "fedavg_apply (robust aggregator)");
+    return;
+  }
   check(launch_fedavg_apply_opt(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(),
                                 (int)slots.size(0), o, theta.numel(), cur_stream()), "fedavg_apply (server optimizer)");
 }
@@ -322,7 +339,7 @@ void star_round(int64_t theta, int64_t slots, int64_t slot_stride, int64_t arriv
                 std::vector<int64_t> peer_inbox, std::vector<int64_t> peer_bcast_flag, int64_t bcast_epoch,
                 int64_t mc_inbox, int64_t select_mask, double server_lr, int64_t n, bool do_reduce, bool do_bcast,
                 int64_t grid_counter, int64_t n_blocks, double timeout_ms, std::vector<double> weights, int64_t decision,
-                int64_t opt_kind, std::vector<double> opt_hyper, int64_t opt_m, int64_t opt_v) {
+                int64_t opt_kind, std::vector<double> opt_hyper, int64_t opt_m, int64_t opt_v, int64_t agg_kind, double trim) {
   StarRoundArgs a;
   std::memset(&a, 0, sizeof(a));
   a.theta = ptr_of<float>(theta);
@@ -349,6 +366,7 @@ void star_round(int64_t theta, int64_t slots, int64_t slot_stride, int64_t arriv
   a.decision = ptr_of<uint32_t>(decision);
   TORCH_CHECK(a.timeout_ns == 0 || a.decision != nullptr, "a deadline needs the decision scratch buffer");
   a.opt = server_opt_args(opt_kind, server_lr, opt_hyper, opt_m, opt_v);
+  a.agg = agg_args(agg_kind, trim);
   check(launch_star_round(a, (int)n_blocks, cur_stream()), "star_round");
 }
 
@@ -390,12 +408,15 @@ void twoshot_fedavg(std::vector<int64_t> work, std::vector<int64_t> shadow, std:
                     int64_t arrive_flags, int64_t weights, int64_t theta_prev, int64_t epoch, int64_t select_mask,
                     double server_lr, int64_t n, int64_t chunk_elems, int64_t rank, int64_t n_blocks,
                     std::vector<int64_t> peer_arrive, bool wait_all, int64_t mc_work, int64_t mc_shadow, int64_t produced,
-                    double produced_timeout_s, int64_t opt_kind, std::vector<double> opt_hyper, int64_t opt_m, int64_t opt_v) {
+                    double produced_timeout_s, int64_t opt_kind, std::vector<double> opt_hyper, int64_t opt_m, int64_t opt_v,
+                    int64_t agg_kind, double trim) {
   TwoShotArgs a = make_twoshot_args(work, shadow, chunk_flags, arrive_flags, weights, theta_prev, epoch, select_mask, server_lr, n,
                                     chunk_elems, rank, peer_arrive, wait_all, mc_work, mc_shadow, produced, produced_timeout_s);
   a.opt = server_opt_args(opt_kind, server_lr, opt_hyper, opt_m, opt_v);
   TORCH_CHECK(a.opt.kind == SOPT_SGD || (a.theta_prev != nullptr && a.mc_work == nullptr),
               "twoshot_fedavg: a server optimizer needs theta_prev and the P2P path (no multicast)");
+  a.agg = agg_args(agg_kind, trim);
+  TORCH_CHECK(a.agg.kind == AGG_MEAN || a.mc_work == nullptr, "twoshot_fedavg: a robust aggregator needs the P2P path (no multicast)");
   check(launch_twoshot_fedavg(a, (int)n_blocks, cur_stream()), "twoshot_fedavg");
 }
 
@@ -405,7 +426,8 @@ void twoshot_fedavg_deadline(std::vector<int64_t> work, std::vector<int64_t> sha
                              int64_t arrive_flags, int64_t weights, int64_t theta_prev, int64_t epoch, int64_t select_mask,
                              double server_lr, int64_t n, int64_t chunk_elems, int64_t rank, int64_t n_blocks,
                              std::vector<int64_t> peer_arrive, bool wait_all, int64_t mc_work, int64_t mc_shadow,
-                             double deadline_ms, std::vector<int64_t> decision, std::vector<int64_t> global_copy) {
+                             double deadline_ms, std::vector<int64_t> decision, std::vector<int64_t> global_copy, int64_t agg_kind,
+                             double trim) {
   TwoShotArgs a = make_twoshot_args(work, shadow, chunk_flags, arrive_flags, weights, theta_prev, epoch, select_mask, server_lr, n,
                                     chunk_elems, rank, peer_arrive, wait_all, mc_work, mc_shadow, 0, 0.0);
   TORCH_CHECK(deadline_ms > 0 && decision.size() == work.size() && global_copy.size() == work.size(),
@@ -416,6 +438,8 @@ void twoshot_fedavg_deadline(std::vector<int64_t> work, std::vector<int64_t> sha
     a.decision[k] = ptr_of<uint32_t>(decision[k]);
     a.global_copy[k] = ptr_of<float>(global_copy[k]);
   }
+  a.agg = agg_args(agg_kind, trim);
+  TORCH_CHECK(a.agg.kind == AGG_MEAN || a.mc_work == nullptr, "twoshot_fedavg: a robust aggregator needs the P2P path (no multicast)");
   check(launch_twoshot_fedavg(a, (int)n_blocks, cur_stream()), "twoshot_fedavg (deadline)");
 }
 
@@ -622,8 +646,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mlp_forward", &mlp_forward);
   m.def("sgd_step", &sgd_step);
   // trailing server-optimizer arguments (server_opt.cuh) default to plain FedAvg: the shorter positional calls keep working
+  // trailing aggregator arguments (robust_agg.cuh) default to the weighted mean
   m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("weights"), py::arg("server_lr"), py::arg("opt_kind") = 0,
-        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
+        py::arg("trim") = 0.0);
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);
@@ -645,13 +671,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("peer_inbox"), py::arg("peer_bcast_flag"), py::arg("bcast_epoch"), py::arg("mc_inbox"), py::arg("select_mask"),
         py::arg("server_lr"), py::arg("n"), py::arg("do_reduce"), py::arg("do_bcast"), py::arg("grid_counter"), py::arg("n_blocks"),
         py::arg("timeout_ms"), py::arg("weights"), py::arg("decision"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
-        py::arg("opt_m") = 0, py::arg("opt_v") = 0);
+        py::arg("opt_m") = 0, py::arg("opt_v") = 0, py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
   m.def("twoshot_fedavg", &twoshot_fedavg, py::arg("work"), py::arg("shadow"), py::arg("chunk_flags"), py::arg("arrive_flags"), py::arg("weights"),
         py::arg("theta_prev"), py::arg("epoch"), py::arg("select_mask"), py::arg("server_lr"), py::arg("n"), py::arg("chunk_elems"),
         py::arg("rank"), py::arg("n_blocks"), py::arg("peer_arrive"), py::arg("wait_all"), py::arg("mc_work"), py::arg("mc_shadow"),
         py::arg("produced"), py::arg("produced_timeout_s"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
-        py::arg("opt_m") = 0, py::arg("opt_v") = 0);
-  m.def("twoshot_fedavg_deadline", &twoshot_fedavg_deadline);
+        py::arg("opt_m") = 0, py::arg("opt_v") = 0, py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
+  m.def("twoshot_fedavg_deadline", &twoshot_fedavg_deadline, py::arg("work"), py::arg("shadow"), py::arg("chunk_flags"), py::arg("arrive_flags"),
+        py::arg("weights"), py::arg("theta_prev"), py::arg("epoch"), py::arg("select_mask"), py::arg("server_lr"), py::arg("n"),
+        py::arg("chunk_elems"), py::arg("rank"), py::arg("n_blocks"), py::arg("peer_arrive"), py::arg("wait_all"), py::arg("mc_work"),
+        py::arg("mc_shadow"), py::arg("deadline_ms"), py::arg("decision"), py::arg("global_copy"), py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
   m.def("twoshot_resync", &twoshot_resync);
   m.def("produced_signal_pack", &produced_signal_pack);
   m.def("produced_mark", &produced_mark);

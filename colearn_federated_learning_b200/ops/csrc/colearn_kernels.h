@@ -31,7 +31,7 @@
 
 #include <cstdlib>
 
-// functions shared by the kernels and host code (Feistel bijection, server optimizer step)
+// functions shared by the kernels and host code (Feistel bijection, server optimizer step, robust aggregation)
 #if defined(__CUDACC__) && !defined(COLEARN_HOST_SHIM)
 #define COLEARN_HD __host__ __device__ __forceinline__
 #else
@@ -39,6 +39,8 @@
 #endif
 // per-element server optimizer step (FedAvgM / FedAdagrad / FedAdam / FedYogi) shared by the FedAvg kernels
 #include "server_opt.cuh"
+// per-element coordinate-wise median / trimmed mean shared by the FedAvg kernels
+#include "robust_agg.cuh"
 
 namespace colearn {
 // Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
@@ -228,6 +230,10 @@ cudaError_t launch_fedavg_apply(float* theta, const float* slots, int64_t slot_s
 // with opt.lr); opt.m / opt.v hold n floats each
 cudaError_t launch_fedavg_apply_opt(float* theta, const float* slots, int64_t slot_stride, const float* weights, int k,
                                     const ServerOptArgs& opt, int64_t n, cudaStream_t s);
+// robust aggregate a of robust_agg.cuh over the k slots (agg.kind != AGG_MEAN; no weights), then theta += opt.lr (a - theta)
+// (opt.kind 0) or the server optimizer step; any k >= 1
+cudaError_t launch_fedavg_apply_robust(float* theta, const float* slots, int64_t slot_stride, int k, const AggArgs& agg,
+                                       const ServerOptArgs& opt, int64_t n, cudaStream_t s);
 // out = sum_k w[k] * slots[k]
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride,
                                const float* weights, int k, int64_t n, cudaStream_t s);
@@ -315,6 +321,9 @@ struct StarRoundArgs {
   // the coordinator's local [n] moment buffers and the step runs where the reduce does (do_reduce), never for a round in which
   // nobody arrived
   ServerOptArgs opt;
+  // aggregator (robust_agg.cuh): kind 0 = the weighted sum above; otherwise the slots hold the raw models theta_k (producers push
+  // them unscaled), weights and renormalisation do not apply and a is the median / trimmed mean over the arrived slots
+  AggArgs agg;
 };
 cudaError_t launch_star_round(const StarRoundArgs& a, int n_blocks, cudaStream_t s);
 
@@ -361,6 +370,9 @@ struct TwoShotArgs {
   // is required, opt.m / opt.v are this rank's local [n] buffers and only the chunks it owns (c % world) are read or written:
   // the moments are sharded like the work.  Not with deadline_ns (ownership follows the arrived set) nor with mc_work (NVLS)
   ServerOptArgs opt;
+  // aggregator (robust_agg.cuh): kind 0 = the weighted sum; otherwise the median / trimmed mean of the selected (deadline: arrived)
+  // ranks' values, unweighted, on the P2P path only (not with mc_work: the switch can only sum)
+  AggArgs agg;
 };
 cudaError_t launch_twoshot_fedavg(const TwoShotArgs& a, int n_blocks, cudaStream_t s);
 // deadline mode, start of a round: if this rank was NOT in the arrived mask of `prev_epoch`, its work arena (and bf16 shadow) is

@@ -17,7 +17,8 @@
 //       (fp32->bf16 conversion fused into the broadcast), raising per-chunk ready flags that the
 //       next round's first consumer GEMM polls from its TMA producer warp (fused broadcast->GEMM).
 //   Both apply plain FedAvg with a server learning rate, or (template flag OPT) a FedOpt server optimizer step of
-//   server_opt.cuh (FedAvgM / FedAdagrad / FedAdam / FedYogi) in the same pass.
+//   server_opt.cuh (FedAvgM / FedAdagrad / FedAdam / FedYogi) in the same pass.  With the template flag ROBUST the average
+//   is the coordinate-wise median / trimmed mean of robust_agg.cuh instead of the weighted sum (unweighted, P2P only).
 //
 // Memory model: data stores are weak; a CTA finishes with __threadfence_system() and the flag is
 // written with st.release.sys; consumers spin with ld.acquire.sys (and add fence.proxy.async before
@@ -107,8 +108,9 @@ __device__ __forceinline__ uint2 pack_bf16x4(const float4& v) {
 }
 
 // -------------------------------------------------------------------------------------------------
-// OPT = false: theta += server_lr (a - theta) (StarRoundArgs::opt.kind == 0); true: the server optimizer step of server_opt.cuh
-template <bool OPT>
+// OPT = false: theta += server_lr (a - theta) (StarRoundArgs::opt.kind == 0); true: the server optimizer step of server_opt.cuh.
+// ROBUST = false: a = sum of the (pre-weighted) slots; true: a = robust_agg.cuh over the raw slots of the arrived workers
+template <bool OPT, bool ROBUST>
 __global__ void __launch_bounds__(256)
 star_round_kernel(StarRoundArgs a) {
   const int tid = threadIdx.x;
@@ -168,13 +170,32 @@ star_round_kernel(StarRoundArgs a) {
     float4 t = theta4[j];
     if (a.do_reduce) {
       float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int k = 0; k < a.world; ++k) {
-        if (!((mask >> k) & 1u)) continue;
-        const float4 v = __ldcg(reinterpret_cast<const float4*>(a.slots + k * a.slot_stride) + j);
-        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+      if constexpr (ROBUST) {
+        // the raw models of the arrived workers (slots k >= world do not exist), unweighted
+        const uint32_t live = mask & ((1u << a.world) - 1u);
+        const int n_live = __popc(live), b_trim = agg_trim_count(a.agg, n_live);
+        float x[16], y[16], z[16], w[16];
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+          float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+          if ((live >> k) & 1u) v = __ldcg(reinterpret_cast<const float4*>(a.slots + k * a.slot_stride) + j);
+          x[k] = v.x; y[k] = v.y; z[k] = v.z; w[k] = v.w;
+        }
+        if (live == 0u) {
+          acc = t;   // nobody arrived: keep theta
+        } else {
+          acc.x = agg_robust<16>(x, live, n_live, b_trim); acc.y = agg_robust<16>(y, live, n_live, b_trim);
+          acc.z = agg_robust<16>(z, live, n_live, b_trim); acc.w = agg_robust<16>(w, live, n_live, b_trim);
+        }
+      } else {
+        for (int k = 0; k < a.world; ++k) {
+          if (!((mask >> k) & 1u)) continue;
+          const float4 v = __ldcg(reinterpret_cast<const float4*>(a.slots + k * a.slot_stride) + j);
+          acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+        }
+        if (mask == 0u) acc = t;   // nobody arrived: keep theta
+        else if (renorm != 1.f) { acc.x *= renorm; acc.y *= renorm; acc.z *= renorm; acc.w *= renorm; }
       }
-      if (mask == 0u) acc = t;   // nobody arrived: keep theta
-      else if (renorm != 1.f) { acc.x *= renorm; acc.y *= renorm; acc.z *= renorm; acc.w *= renorm; }
       if constexpr (OPT) {
         if (mask != 0u) t = server_opt_step4(a.opt, j, t, acc);     // (nobody arrived: theta and the moments stay)
       } else {
@@ -197,9 +218,18 @@ star_round_kernel(StarRoundArgs a) {
     float t = a.theta[j];
     if (a.do_reduce) {
       float acc = 0.f;
-      for (int k = 0; k < a.world; ++k)
-        if ((mask >> k) & 1u) acc += __ldcg(a.slots + k * a.slot_stride + j);
-      acc = (mask == 0u) ? t : acc * renorm;
+      if constexpr (ROBUST) {
+        const uint32_t live = mask & ((1u << a.world) - 1u);
+        const int n_live = __popc(live), b_trim = agg_trim_count(a.agg, n_live);
+        float v[16];
+#pragma unroll
+        for (int k = 0; k < 16; ++k) v[k] = ((live >> k) & 1u) ? __ldcg(a.slots + k * a.slot_stride + j) : 0.f;
+        acc = (live == 0u) ? t : agg_robust<16>(v, live, n_live, b_trim);
+      } else {
+        for (int k = 0; k < a.world; ++k)
+          if ((mask >> k) & 1u) acc += __ldcg(a.slots + k * a.slot_stride + j);
+        acc = (mask == 0u) ? t : acc * renorm;
+      }
       if constexpr (OPT) {
         if (mask != 0u) t = server_opt_step(a.opt, j, t, acc);
       } else {
@@ -229,14 +259,28 @@ star_round_kernel(StarRoundArgs a) {
   }
 }
 
+// robust_agg.cuh on each component of the float4 values v[k] of the ranks k in `valid` (the two-shot owner's registers; the
+// other entries were never loaded and are not read)
+__device__ __forceinline__ float4 agg_robust4(const float4 (&v)[8], uint32_t valid, int n, int b) {
+  float x[8], y[8], z[8], w[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const float4 u = ((valid >> k) & 1u) ? v[k] : make_float4(0.f, 0.f, 0.f, 0.f);
+    x[k] = u.x; y[k] = u.y; z[k] = u.z; w[k] = u.w;
+  }
+  return make_float4(agg_robust<8>(x, valid, n, b), agg_robust<8>(y, valid, n, b), agg_robust<8>(z, valid, n, b),
+                     agg_robust<8>(w, valid, n, b));
+}
+
 // -------------------------------------------------------------------------------------------------
 // Two-shot FedAvg.  Work decomposition: the arena is cut into chunks of chunk_elems floats; chunk c
 // belongs to rank (c % world) (interleaved ownership keeps every rank's NVLink ports busy for the
 // whole kernel and lets early layers become ready first on every peer).  A CTA processes whole
 // chunks so that it can publish the chunk's ready flag by itself.
 // one owned chunk: pull it from every selected rank, apply, push it to every rank (fp32 + bf16), publish its flag.
-// OPT: the server optimizer step (server_opt.cuh) on theta_prev with this rank's moment shards a.opt.m / a.opt.v, P2P path only
-template <bool OPT>
+// OPT: the server optimizer step (server_opt.cuh) on theta_prev with this rank's moment shards a.opt.m / a.opt.v, P2P path only.
+// ROBUST: the median / trimmed mean of robust_agg.cuh over the ranks in `mask` instead of the weighted sum, P2P path only
+template <bool OPT, bool ROBUST>
 __device__ __forceinline__ void twoshot_chunk(const TwoShotArgs& a, const int64_t c, const float* sw, const int tid,
                                               const uint32_t mask, const bool use_mc) {
   const int64_t lo = c * a.chunk_elems;
@@ -281,15 +325,23 @@ __device__ __forceinline__ void twoshot_chunk(const TwoShotArgs& a, const int64_
       }
     }
     float4 acca = make_float4(0.f, 0.f, 0.f, 0.f), accb = make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (ROBUST) {
+      // the ranks that contribute, unweighted
+      const uint32_t live = mask & ((1u << a.world) - 1u);
+      const int n_live = __popc(live), b_trim = agg_trim_count(a.agg, n_live);
+      acca = agg_robust4(va, live, n_live, b_trim);
+      if (has_b) accb = agg_robust4(vb, live, n_live, b_trim);
+    } else {
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      if (k < a.world && ((mask >> k) & 1u)) {
-        const float w = sw[k];
-        acca.x = fmaf(w, va[k].x, acca.x); acca.y = fmaf(w, va[k].y, acca.y);
-        acca.z = fmaf(w, va[k].z, acca.z); acca.w = fmaf(w, va[k].w, acca.w);
-        if (has_b) {
-          accb.x = fmaf(w, vb[k].x, accb.x); accb.y = fmaf(w, vb[k].y, accb.y);
-          accb.z = fmaf(w, vb[k].z, accb.z); accb.w = fmaf(w, vb[k].w, accb.w);
+      for (int k = 0; k < 8; ++k) {
+        if (k < a.world && ((mask >> k) & 1u)) {
+          const float w = sw[k];
+          acca.x = fmaf(w, va[k].x, acca.x); acca.y = fmaf(w, va[k].y, acca.y);
+          acca.z = fmaf(w, va[k].z, acca.z); acca.w = fmaf(w, va[k].w, acca.w);
+          if (has_b) {
+            accb.x = fmaf(w, vb[k].x, accb.x); accb.y = fmaf(w, vb[k].y, accb.y);
+            accb.z = fmaf(w, vb[k].z, accb.z); accb.w = fmaf(w, vb[k].w, accb.w);
+          }
         }
       }
     }
@@ -343,8 +395,10 @@ __device__ __forceinline__ void twoshot_chunk(const TwoShotArgs& a, const int64_
   __syncthreads();
 }
 
-template <bool OPT>
-__global__ void __launch_bounds__(512)
+// ROBUST instances run 256-thread CTAs (launch_twoshot_fedavg): the rank count over the owner's 2 x 8 float4 registers does
+// not fit the 128 registers a 512-thread CTA leaves a thread without spilling
+template <bool OPT, bool ROBUST>
+__global__ void __launch_bounds__(ROBUST ? 256 : 512)
 twoshot_fedavg_kernel(TwoShotArgs a) {
   const int tid = threadIdx.x;
   __shared__ float sw[16];
@@ -409,12 +463,12 @@ twoshot_fedavg_kernel(TwoShotArgs a) {
   const int n_own = __popc(owners);
   const bool i_own = (owners >> a.rank) & 1u;
   const int my_idx = __popc(owners & ((1u << a.rank) - 1u));
-  const bool use_mc = !OPT && a.mc_work != nullptr && (a.deadline_ns == 0 || mask == full);
+  const bool use_mc = !OPT && !ROBUST && a.mc_work != nullptr && (a.deadline_ns == 0 || mask == full);
   if (i_own && mask != 0u) {
     for (int64_t oc = blockIdx.x; ; oc += gridDim.x) {
       const int64_t c = my_idx + oc * n_own;
       if (c >= n_chunks) break;
-      twoshot_chunk<OPT>(a, c, sw, tid, mask, use_mc);
+      twoshot_chunk<OPT, ROBUST>(a, c, sw, tid, mask, use_mc);
     }
   } else if (mask == 0u && a.rank == 0) {
     // nobody arrived in time: the model stays as it is; the coordinator still publishes the chunk flags so that nobody waits
@@ -448,8 +502,8 @@ twoshot_resync_kernel(const uint32_t* ring, uint32_t prev_epoch, int rank, float
 // Chunks are taken in whatever order the producers of all selected ranks finish them (the backward pass finalises the
 // last layers first): each CTA sweeps its owned chunks, newest-first, and processes those whose produced epochs have
 // arrived from every selected rank.
-template <bool OPT>
-__global__ void __launch_bounds__(512)
+template <bool OPT, bool ROBUST>
+__global__ void __launch_bounds__(ROBUST ? 256 : 512)
 twoshot_overlap_kernel(TwoShotArgs a) {
   const int tid = threadIdx.x;
   __shared__ float sw[16];
@@ -477,7 +531,7 @@ twoshot_overlap_kernel(TwoShotArgs a) {
         const int ready = s_ready;
         __syncthreads();
         if (!ready) continue;
-        twoshot_chunk<OPT>(a, c, sw, tid, a.select_mask, !OPT && a.mc_work != nullptr);
+        twoshot_chunk<OPT, ROBUST>(a, c, sw, tid, a.select_mask, !OPT && !ROBUST && a.mc_work != nullptr);
         if (tid == 0) s_done[i >> 6] |= 1ull << (i & 63);
         __syncthreads();
         --left;
@@ -603,35 +657,47 @@ p2p_copy_kernel(float* __restrict__ dst, const float* __restrict__ src, int64_t 
 
 }  // namespace
 
+// (the plain FedAvg instances are referenced last: the cubin then lists them first for each kernel)
 cudaError_t launch_star_round(const StarRoundArgs& a, int n_blocks, cudaStream_t s) {
-  if (a.world > 16 || !server_opt_args_ok(a.opt)) return cudaErrorInvalidValue;
+  if (a.world > 16 || !server_opt_args_ok(a.opt) || !agg_args_ok(a.agg)) return cudaErrorInvalidValue;
   if (n_blocks < 1) n_blocks = 1;
-  if (a.opt.kind != SOPT_SGD) {
-    COLEARN_LAUNCH(star_round_kernel<true>, n_blocks, 256, 0, s, a);
-    return cudaGetLastError();
+  const bool opt = a.opt.kind != SOPT_SGD, robust = a.agg.kind != AGG_MEAN;
+  if (robust && opt) {
+    COLEARN_LAUNCH((star_round_kernel<true, true>), n_blocks, 256, 0, s, a);
+  } else if (robust) {
+    COLEARN_LAUNCH((star_round_kernel<false, true>), n_blocks, 256, 0, s, a);
+  } else if (opt) {
+    COLEARN_LAUNCH((star_round_kernel<true, false>), n_blocks, 256, 0, s, a);
+  } else {
+    COLEARN_LAUNCH((star_round_kernel<false, false>), n_blocks, 256, 0, s, a);
   }
-  COLEARN_LAUNCH(star_round_kernel<false>, n_blocks, 256, 0, s, a);
   return cudaGetLastError();
 }
 
 cudaError_t launch_twoshot_fedavg(const TwoShotArgs& a, int n_blocks, cudaStream_t s) {
   if (a.world > 8 || (a.n & 3) || (a.chunk_elems & 3)) return cudaErrorInvalidValue;
   if (n_blocks < 1) n_blocks = 1;
-  if (a.opt.kind != SOPT_SGD) {
+  const bool opt = a.opt.kind != SOPT_SGD, robust = a.agg.kind != AGG_MEAN;
+  if (opt) {
     // the moments are sharded by the fixed ownership c % world: no deadline (ownership follows the arrived set), no NVLS
     if (!server_opt_args_ok(a.opt) || a.theta_prev == nullptr || a.deadline_ns != 0 || a.mc_work != nullptr) return cudaErrorInvalidValue;
-    if (a.produced != nullptr) {
-      COLEARN_LAUNCH(twoshot_overlap_kernel<true>, n_blocks, 512, 0, s, a);
-      return cudaGetLastError();
-    }
-    COLEARN_LAUNCH(twoshot_fedavg_kernel<true>, n_blocks, 512, 0, s, a);
-    return cudaGetLastError();
   }
-  if (a.produced != nullptr) {
-    COLEARN_LAUNCH(twoshot_overlap_kernel<false>, n_blocks, 512, 0, s, a);
-    return cudaGetLastError();
+  // robust: the switch of the NVLS path can only sum; a deadline is fine (a robust aggregate keeps no per-rank state)
+  if (robust && (!agg_args_ok(a.agg) || a.mc_work != nullptr)) return cudaErrorInvalidValue;
+  const bool overlap = a.produced != nullptr;
+  if (robust && opt) {
+    if (overlap) COLEARN_LAUNCH((twoshot_overlap_kernel<true, true>), n_blocks, 256, 0, s, a);
+    else COLEARN_LAUNCH((twoshot_fedavg_kernel<true, true>), n_blocks, 256, 0, s, a);
+  } else if (robust) {
+    if (overlap) COLEARN_LAUNCH((twoshot_overlap_kernel<false, true>), n_blocks, 256, 0, s, a);
+    else COLEARN_LAUNCH((twoshot_fedavg_kernel<false, true>), n_blocks, 256, 0, s, a);
+  } else if (opt) {
+    if (overlap) COLEARN_LAUNCH((twoshot_overlap_kernel<true, false>), n_blocks, 512, 0, s, a);
+    else COLEARN_LAUNCH((twoshot_fedavg_kernel<true, false>), n_blocks, 512, 0, s, a);
+  } else {
+    if (overlap) COLEARN_LAUNCH((twoshot_overlap_kernel<false, false>), n_blocks, 512, 0, s, a);
+    else COLEARN_LAUNCH((twoshot_fedavg_kernel<false, false>), n_blocks, 512, 0, s, a);
   }
-  COLEARN_LAUNCH(twoshot_fedavg_kernel<false>, n_blocks, 512, 0, s, a);
   return cudaGetLastError();
 }
 
@@ -708,8 +774,12 @@ COLEARN_DEFINE_SPIN_LIMIT_SETTER(set_spin_limit_comm)
 cudaError_t preload_comm_kernels() {
 #ifndef COLEARN_HOST_SHIM
   cudaFuncAttributes attr;
-  const void* kernels[] = {(const void*)star_round_kernel<false>, (const void*)star_round_kernel<true>, (const void*)twoshot_fedavg_kernel<false>,
-                           (const void*)twoshot_fedavg_kernel<true>, (const void*)twoshot_overlap_kernel<false>, (const void*)twoshot_overlap_kernel<true>,
+  const void* kernels[] = {(const void*)star_round_kernel<false, false>, (const void*)star_round_kernel<true, false>,
+                           (const void*)star_round_kernel<false, true>, (const void*)star_round_kernel<true, true>,
+                           (const void*)twoshot_fedavg_kernel<false, false>, (const void*)twoshot_fedavg_kernel<true, false>,
+                           (const void*)twoshot_fedavg_kernel<false, true>, (const void*)twoshot_fedavg_kernel<true, true>,
+                           (const void*)twoshot_overlap_kernel<false, false>, (const void*)twoshot_overlap_kernel<true, false>,
+                           (const void*)twoshot_overlap_kernel<false, true>, (const void*)twoshot_overlap_kernel<true, true>,
                            (const void*)produced_mark_kernel, (const void*)twoshot_resync_kernel, (const void*)reduce_push_kernel, (const void*)set_flag_kernel,
                            (const void*)signal_peers_kernel, (const void*)wait_flag_kernel, (const void*)wait_flags_kernel,
                            (const void*)wait_flags_dev_kernel, (const void*)p2p_copy_kernel};

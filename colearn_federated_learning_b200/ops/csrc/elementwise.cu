@@ -174,6 +174,33 @@ __global__ void fedavg_opt_kernel(float* __restrict__ theta, const float* __rest
   }
 }
 
+// Byzantine-robust aggregate (robust_agg.cuh: coordinate-wise median / trimmed mean over all k slots, unweighted) followed by
+// theta += opt.lr (a - theta) (opt.kind 0) or a server optimizer step (server_opt.cuh).  One element per thread.
+// KMAX > 0: register path for k <= KMAX, the k values and their keys stay in registers and the rank count is KMAX x KMAX
+// unrolled compares; KMAX = 0: any k, tiles of 32 values in registers, the rank count rereads the values through L1 / L2
+// (k ceil(k / 32) loads per element).
+template <int KMAX>
+__global__ void __launch_bounds__(256)
+fedavg_robust_kernel(float* __restrict__ theta, const float* __restrict__ slots, int64_t slot_stride, int k, AggArgs agg,
+                     ServerOptArgs opt, int64_t n) {
+  const int b = agg_trim_count(agg, k);
+  const uint32_t valid = k >= 32 ? 0xffffffffu : (1u << k) - 1u;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
+    float a;
+    if constexpr (KMAX > 0) {
+      float v[KMAX];
+#pragma unroll
+      for (int c = 0; c < KMAX; ++c) v[c] = c < k ? __ldcs(slots + c * slot_stride + j) : 0.f;
+      a = agg_robust<KMAX>(v, valid, k, b);
+    } else {
+      a = agg_robust_tiled<32>([&](int c) { return __ldg(slots + c * slot_stride + j); }, k, b);
+    }
+    const float t = theta[j];
+    theta[j] = (opt.kind == SOPT_SGD) ? fmaf(opt.lr, a - t, t) : server_opt_step(opt, j, t, a);
+  }
+}
+
 // ---- losses ---------------------------------------------------------------------------------------
 __global__ void sigmoid_bce_kernel(const float* __restrict__ z, const float* __restrict__ y,
                                    float* __restrict__ dz, float* __restrict__ loss_out, int64_t n) {
@@ -490,6 +517,24 @@ cudaError_t launch_fedavg_apply_opt(float* theta, const float* slots, int64_t sl
   if (k < 1 || !server_opt_args_ok(opt)) return cudaErrorInvalidValue;
   if (opt.kind == SOPT_SGD) return launch_fedavg_apply(theta, slots, slot_stride, weights, k, opt.lr, n, s);
   COLEARN_LAUNCH(fedavg_opt_kernel, grid_for(n), kThreads, 0, s, theta, slots, slot_stride, weights, k, opt, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_fedavg_apply_robust(float* theta, const float* slots, int64_t slot_stride, int k, const AggArgs& agg,
+                                       const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
+  if (k < 1 || agg.kind == AGG_MEAN || !agg_args_ok(agg) || !server_opt_args_ok(opt)) return cudaErrorInvalidValue;
+  const int grid = grid_for(n, 1);
+  // the register path costs KMAX^2 compares per element whatever k is: take the smallest that holds k
+  if (k <= 4) {
+    COLEARN_LAUNCH(fedavg_robust_kernel<4>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
+  } else if (k <= 8) {
+    COLEARN_LAUNCH(fedavg_robust_kernel<8>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
+  } else if (k <= 16) {
+    COLEARN_LAUNCH(fedavg_robust_kernel<16>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
+  } else if (k <= 32) {
+    COLEARN_LAUNCH(fedavg_robust_kernel<32>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
+  } else {
+    COLEARN_LAUNCH(fedavg_robust_kernel<0>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
+  }
   return cudaGetLastError();
 }
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride, const float* weights,

@@ -111,9 +111,24 @@ colearn::ServerOptArgs server_opt_args(int64_t kind, double lr, const std::vecto
   TORCH_CHECK(colearn::server_opt_args_ok(o), "server optimizer: unknown kind or a moment buffer missing / misaligned");
   return o;
 }
+// aggregator (robust_agg.cuh): kind 0 = weighted mean; 1 = median, 2 = trimmed mean with `trim` per end
+colearn::AggArgs agg_args(int64_t kind, double trim) {
+  colearn::AggArgs g;
+  memset(&g, 0, sizeof(g));
+  g.kind = (int)kind;
+  g.trim = (float)trim;
+  TORCH_CHECK(colearn::agg_args_ok(g), "aggregator: unknown kind ", kind, " or trim fraction ", trim, " outside [0, 0.5)");
+  return g;
+}
 void fedavg_apply(Tensor theta, Tensor slots, Tensor w, double server_lr, int64_t opt_kind, std::vector<double> opt_hyper,
-                  c10::optional<Tensor> m, c10::optional<Tensor> v) {
+                  c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind, double trim) {
   TORCH_CHECK(slots.dim() == 2 && slots.size(1) == theta.numel() && w.numel() == slots.size(0), "slots [K, P], weights [K]");
+  if (agg_kind != colearn::AGG_MEAN) {
+    const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, theta.numel());
+    CK(colearn::launch_fedavg_apply_robust(fmut(theta, "theta"), fptr(slots, "slots"), slots.size(1), (int)slots.size(0),
+                                           agg_args(agg_kind, trim), o, theta.numel(), nullptr));
+    return;
+  }
   if (opt_kind == colearn::SOPT_SGD) {
     CK(colearn::launch_fedavg_apply(fmut(theta, "theta"), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0),
                                     (float)server_lr, theta.numel(), nullptr));
@@ -196,7 +211,7 @@ Tensor ring_matmul(Tensor a, Tensor b) {
 int64_t star_round(Tensor theta, Tensor slots, Tensor arrive, int64_t arrive_epoch, Tensor inboxes, Tensor bcast_flags, int64_t bcast_epoch,
                    int64_t select_mask, double server_lr, bool do_reduce, bool do_bcast, int64_t n_blocks, double timeout_ms,
                    std::vector<double> weights, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<Tensor> m,
-                   c10::optional<Tensor> v) {
+                   c10::optional<Tensor> v, int64_t agg_kind, double trim) {
   const int W = (int)slots.size(0);
   colearn::StarRoundArgs a;
   memset(&a, 0, sizeof(a));
@@ -222,6 +237,7 @@ int64_t star_round(Tensor theta, Tensor slots, Tensor arrive, int64_t arrive_epo
   a.timeout_ns = (unsigned long long)(timeout_ms * 1e6);
   a.decision = decision;
   a.opt = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, a.n);
+  a.agg = agg_args(agg_kind, trim);
   {
     py::gil_scoped_release nogil;
     CK(colearn::launch_star_round(a, (int)n_blocks, nullptr));
@@ -234,7 +250,7 @@ int64_t star_round(Tensor theta, Tensor slots, Tensor arrive, int64_t arrive_epo
 void twoshot_fedavg(int64_t rank, Tensor works, c10::optional<Tensor> shadows, Tensor chunk_flags, Tensor arrive, Tensor weights,
                     c10::optional<Tensor> theta_prev, int64_t epoch, int64_t select_mask, double server_lr, int64_t chunk_elems, int64_t n_blocks,
                     c10::optional<Tensor> produced, double produced_timeout_s, int64_t opt_kind, std::vector<double> opt_hyper,
-                    c10::optional<Tensor> m, c10::optional<Tensor> v) {
+                    c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind, double trim) {
   const int W = (int)works.size(0);
   colearn::TwoShotArgs a;
   memset(&a, 0, sizeof(a));
@@ -260,6 +276,7 @@ void twoshot_fedavg(int64_t rank, Tensor works, c10::optional<Tensor> shadows, T
   }
   a.opt = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, a.n);     // this rank's moment buffers (it touches the chunks it owns)
   TORCH_CHECK(a.opt.kind == colearn::SOPT_SGD || a.theta_prev != nullptr, "a server optimizer needs theta_prev");
+  a.agg = agg_args(agg_kind, trim);
   {
     py::gil_scoped_release nogil;
     CK(colearn::launch_twoshot_fedavg(a, (int)n_blocks, nullptr));
@@ -268,7 +285,8 @@ void twoshot_fedavg(int64_t rank, Tensor works, c10::optional<Tensor> shadows, T
 
 // deadline mode of one emulated rank: decisions int32 [W, 16] (row k = rank k's ring), globals [W, n] (second arenas)
 void twoshot_fedavg_deadline(int64_t rank, Tensor works, Tensor globals, Tensor chunk_flags, Tensor arrive, Tensor weights, int64_t epoch,
-                             int64_t select_mask, int64_t chunk_elems, int64_t n_blocks, double deadline_ms, Tensor decisions) {
+                             int64_t select_mask, int64_t chunk_elems, int64_t n_blocks, double deadline_ms, Tensor decisions,
+                             int64_t agg_kind, double trim) {
   const int W = (int)works.size(0);
   colearn::TwoShotArgs a;
   memset(&a, 0, sizeof(a));
@@ -289,6 +307,7 @@ void twoshot_fedavg_deadline(int64_t rank, Tensor works, Tensor globals, Tensor 
   a.rank = (int)rank;
   a.wait_all = 0;      // (the emulated ranks run one after the other: nobody may wait for a later rank's chunks)
   a.deadline_ns = (unsigned long long)(deadline_ms * 1e6);
+  a.agg = agg_args(agg_kind, trim);
   py::gil_scoped_release nogil;
   CK(colearn::launch_twoshot_fedavg(a, (int)n_blocks, nullptr));
 }
@@ -414,7 +433,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sgd_step", &sgd_step);
   // trailing server-optimizer arguments default to plain FedAvg (the shorter positional calls keep working)
   m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("w"), py::arg("server_lr"), py::arg("opt_kind") = 0,
-        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
+        py::arg("trim") = 0.0);
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);
@@ -429,12 +449,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("star_round", &star_round, py::arg("theta"), py::arg("slots"), py::arg("arrive"), py::arg("arrive_epoch"), py::arg("inboxes"),
         py::arg("bcast_flags"), py::arg("bcast_epoch"), py::arg("select_mask"), py::arg("server_lr"), py::arg("do_reduce"), py::arg("do_bcast"),
         py::arg("n_blocks"), py::arg("timeout_ms"), py::arg("weights"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
-        py::arg("m") = py::none(), py::arg("v") = py::none());
+        py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
   m.def("twoshot_fedavg", &twoshot_fedavg, py::arg("rank"), py::arg("works"), py::arg("shadows"), py::arg("chunk_flags"), py::arg("arrive"),
         py::arg("weights"), py::arg("theta_prev"), py::arg("epoch"), py::arg("select_mask"), py::arg("server_lr"), py::arg("chunk_elems"),
         py::arg("n_blocks"), py::arg("produced"), py::arg("produced_timeout_s"), py::arg("opt_kind") = 0,
-        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
-  m.def("twoshot_fedavg_deadline", &twoshot_fedavg_deadline);
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
+        py::arg("trim") = 0.0);
+  m.def("twoshot_fedavg_deadline", &twoshot_fedavg_deadline, py::arg("rank"), py::arg("works"), py::arg("globals"), py::arg("chunk_flags"),
+        py::arg("arrive"), py::arg("weights"), py::arg("epoch"), py::arg("select_mask"), py::arg("chunk_elems"), py::arg("n_blocks"),
+        py::arg("deadline_ms"), py::arg("decisions"), py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
   m.def("twoshot_resync", &twoshot_resync);
   m.def("produced_signal_pack", &produced_signal_pack);
   m.def("produced_mark", &produced_mark);

@@ -102,6 +102,11 @@ int main() {
     a.opt.kind = SOPT_ADAM; a.opt.lr = 0.01f; a.opt.beta1 = 0.9f; a.opt.beta2 = 0.99f; a.opt.tau = 1e-3f;
     a.opt.m = m.data(); a.opt.v = v.data(); a.arrive_epoch = 5; a.bcast_epoch = 7;
     CK(launch_star_round(a, 3, nullptr));
+    // the same round with a robust aggregator (median of the raw slots, register rank count), float4 body + scalar tail
+    memset(&a.opt, 0, sizeof(a.opt));
+    a.agg.kind = AGG_MEDIAN; a.bcast_epoch = 8;
+    CK(launch_star_round(a, 3, nullptr));
+    memset(&a.agg, 0, sizeof(a.agg));
     const int64_t n = 4 * 200, chunk = 64;
     std::vector<float> works = randv((size_t)W * n), weights(W, 1.f / W);
     std::vector<uint32_t> cflags((size_t)W * ((n + chunk - 1) / chunk), 0), arr(W, 2);
@@ -123,6 +128,16 @@ int main() {
       t.world = W; t.rank = r; t.theta_prev = prevs.data() + (size_t)r * n;
       t.opt.kind = SOPT_ADAM; t.opt.lr = 0.01f; t.opt.beta1 = 0.9f; t.opt.beta2 = 0.99f; t.opt.tau = 1e-3f;
       t.opt.m = ms.data() + (size_t)r * n; t.opt.v = vs.data() + (size_t)r * n;
+      CK(launch_twoshot_fedavg(t, 2, nullptr));
+    }
+    // two-shot with a trimmed mean: the owner ranks its peers' values in registers (P2P path)
+    for (int r = 0; r < W; ++r) {
+      TwoShotArgs t;
+      memset(&t, 0, sizeof(t));
+      for (int k = 0; k < W; ++k) { t.work[k] = works.data() + (size_t)k * n; t.chunk_flags[k] = cflags.data() + (size_t)k * ((n + chunk - 1) / chunk); }
+      t.arrive_flags = arr.data(); t.weights = weights.data(); t.epoch = 2; t.select_mask = 7; t.server_lr = 1.f; t.n = n; t.chunk_elems = chunk;
+      t.world = W; t.rank = r;
+      t.agg.kind = AGG_TRIMMED_MEAN; t.agg.trim = 0.34f;
       CK(launch_twoshot_fedavg(t, 2, nullptr));
     }
     std::vector<float> dst(P), lsrc = randv(2 * W), ldst(2);

@@ -12,8 +12,9 @@ backward; SGD step; if ++it >= max_nr_batches >= 0: stop`` and return the last l
 from __future__ import annotations
 
 import math
-from typing import List, Sequence, Tuple
+from typing import List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 LOSSES = ("bce", "sse", "xent", "mse")
@@ -181,10 +182,49 @@ def fedavg_flat(models: torch.Tensor, weights: torch.Tensor) -> torch.Tensor:
     return (weights.view(-1, 1).to(models.dtype) * models).sum(0)
 
 
+def agg_trim_count(kind: str, beta: float, n: int) -> int:
+    """Values dropped at each end of ``n`` sorted ones (``fl/aggregate.py``); ``beta * n`` is formed in float32."""
+    half = (n - 1) // 2
+    if kind == "median":
+        return half
+    if kind == "trimmed_mean":
+        return min(int(math.floor(np.float32(beta) * np.float32(n))), half)
+    raise ValueError(f"not a robust aggregator: {kind!r}")
+
+
+def robust_aggregate(models: torch.Tensor, mask: Optional[int] = None, kind: str = "median", beta: float = 0.0) -> torch.Tensor:
+    """Coordinate-wise median / trimmed mean of the rows ``k`` of ``models [K, P]`` set in the bitmask ``mask`` (all rows if
+    None), the definition the kernels (``ops/csrc/robust_agg.cuh``) match bit for bit: int32 keys of the IEEE total order, rank
+    = #smaller keys + #equal keys in earlier rows, a sequential float32 sum of the kept rows in row order, one division.
+    Returns ``[P]``; no row selected is an error (the caller keeps theta)."""
+    rows = [k for k in range(models.shape[0]) if mask is None or (mask >> k) & 1]
+    n = len(rows)
+    if n == 0:
+        raise ValueError("robust_aggregate: no model contributes")
+    v = models[rows].float().contiguous()
+    bits = v.view(torch.int32)
+    key = bits ^ ((bits >> 31) & 0x7FFFFFFF)
+    b = agg_trim_count(kind, beta, n)
+    acc = torch.zeros(v.shape[1], dtype=torch.float32, device=v.device)
+    for k in range(n):
+        rank = (key < key[k]).sum(0) + (key[:k] == key[k]).sum(0)
+        acc = acc + torch.where((rank >= b) & (rank < n - b), v[k], torch.zeros_like(v[k]))
+    return acc / torch.full_like(acc, float(n - 2 * b))
+
+
+def aggregate(models: torch.Tensor, weights: torch.Tensor, aggregator=None) -> torch.Tensor:
+    """The average the server steps towards: :func:`fedavg_flat` (``aggregator`` None or ``mean``) or
+    :func:`robust_aggregate` over all rows (unweighted)."""
+    if aggregator is None or not aggregator.robust:
+        return fedavg_flat(models, weights)
+    return robust_aggregate(models, None, aggregator.kind, aggregator.trim)
+
+
 def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor,
-                 server_lr: float = 1.0) -> torch.Tensor:
-    """``theta <- theta + server_lr * (sum_k w_k models[k] - theta)`` (weights sum to 1)."""
-    avg = fedavg_flat(models, weights)
+                 server_lr: float = 1.0, aggregator=None) -> torch.Tensor:
+    """``theta <- theta + server_lr * (sum_k w_k models[k] - theta)`` (weights sum to 1).  ``aggregator``: a robust
+    :class:`fl.aggregate.Aggregator` replaces the weighted sum by its unweighted aggregate."""
+    avg = aggregate(models, weights, aggregator)
     return theta.add_(server_lr * (avg - theta))
 
 
@@ -212,9 +252,10 @@ def server_opt_step(theta: torch.Tensor, avg: torch.Tensor, kind: str, lr: float
 
 
 def server_opt_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor, kind: str, lr: float, m=None, v=None,
-                     beta1: float = 0.9, beta2: float = 0.99, tau: float = 1e-3) -> torch.Tensor:
-    """``avg = sum_k w_k models[k]`` then :func:`server_opt_step` (the oracle of the fused kernels)."""
-    return server_opt_step(theta, fedavg_flat(models, weights), kind, lr, m, v, beta1, beta2, tau)
+                     beta1: float = 0.9, beta2: float = 0.99, tau: float = 1e-3, aggregator=None) -> torch.Tensor:
+    """``avg = sum_k w_k models[k]`` (or the robust aggregate of ``aggregator``) then :func:`server_opt_step` (the oracle of
+    the fused kernels)."""
+    return server_opt_step(theta, aggregate(models, weights, aggregator), kind, lr, m, v, beta1, beta2, tau)
 
 
 def linear_bias_relu(x, w, b, relu=True):

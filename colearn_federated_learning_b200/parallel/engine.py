@@ -33,6 +33,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from .. import ops
+from ..fl.aggregate import Aggregator
 from ..fl.fedavg import normalized_weights
 from ..fl.server_opt import ServerOpt, resolve_server_opt
 from ..fl.trainer import FitConfig, local_fit, resolve_loss
@@ -69,7 +70,12 @@ class FederatedEngine:
                  shuffle: bool = True, chunk_elems: int = 0, bf16_shadow: bool = False,
                  round_deadline_ms: float = 0.0, clients_per_rank: int = 1,
                  model_kwargs: Optional[Dict[str, Any]] = None, overlap_reduce: Optional[bool] = None,
-                 phase_timing: Optional[bool] = None, server_opt: Optional[ServerOpt] = None) -> None:
+                 phase_timing: Optional[bool] = None, server_opt: Optional[ServerOpt] = None,
+                 aggregator: Optional[Aggregator] = None) -> None:
+        """``aggregator``: how the client models become the average the server steps towards (``fl/aggregate.py``):
+        the weighted FedAvg mean (default) or the coordinate-wise ``median`` / ``trimmed_mean``.  The robust kinds are
+        unweighted, so ``weighted`` does not apply to them; they need one client per rank (``clients_per_rank == 1``) and take
+        the P2P path of the two-shot kernel (no NVLS)."""
         self.rank = dist.get_rank(group) if _dist_ready() else 0
         self.world = dist.get_world_size(group) if _dist_ready() else 1
         self.group = group
@@ -122,6 +128,11 @@ class FederatedEngine:
         self.round_deadline_ms = float(round_deadline_ms)
         # many virtual clients (federated devices) per GPU: one CTA each, summed locally before the NVLink push
         self.clients_per_rank = max(1, int(clients_per_rank))
+        self.aggregator = aggregator if aggregator is not None else Aggregator()
+        if self.aggregator.robust and self.clients_per_rank > 1:
+            raise ValueError(f"aggregator={self.aggregator.kind!r} needs clients_per_rank=1: with several clients per rank the "
+                             "rank sums its clients' models before the coordinator sees them, so there is no per-client value "
+                             "left to take the median / trimmed mean of")
         self.use_graphs = os.environ.get("COLEARN_CUDA_GRAPHS", "1") != "0"
         # multimem.ld_reduce / multimem.st in the two-shot kernel.  Through the switch every GPU sends its whole vector once (each
         # element is pulled by its owner's ld_reduce) plus its reduced share once, and receives the same: (1 + 1/W) x model bytes
@@ -243,6 +254,24 @@ class FederatedEngine:
             return 0, [], 0, 0
         return st.code, st.hyper, st.m.data_ptr(), st.v.data_ptr() if st.v is not None else 0
 
+    def _agg_args(self) -> Tuple[int, float]:
+        """Trailing aggregator arguments of the star / two-shot bindings: (kind code, trim fraction)."""
+        return self.aggregator.code, self.aggregator.trim
+
+    def _robust_average(self, local: torch.Tensor, mask: int) -> Optional[torch.Tensor]:
+        """Library form of the robust aggregate: every rank's model is gathered to the coordinator (a robust aggregate is not
+        a sum, so ``dist.reduce`` cannot form it), which returns ``robust_aggregate`` over the selected ranks (None elsewhere
+        and when nobody is selected)."""
+        W, r = self.world, self.rank
+        rows = [torch.empty_like(local) for _ in range(W)] if r == self.coord else None
+        if _dist_ready() and W > 1:
+            dist.gather(local, rows, dst=self.coord, group=self.group)
+        elif rows is not None:
+            rows[0] = local
+        if r != self.coord or mask == 0:
+            return None
+        return ops.reference.robust_aggregate(torch.stack(rows), mask, self.aggregator.kind, self.aggregator.trim)
+
     def load_global(self, flat: torch.Tensor) -> None:
         self.theta[: self.P].copy_(flat.to(self.device).float().reshape(-1)[: self.P])
 
@@ -261,9 +290,13 @@ class FederatedEngine:
 
     # ------------------------------------------------------------------------------------------
     def _round_weights(self, mask: int) -> List[float]:
+        """Per-rank scale of the round's contributions: the normalised FedAvg weights, or 1 for every selected rank with a
+        robust aggregator (the slots then hold the raw models)."""
         sel = [k for k in range(self.world) if (mask >> k) & 1]
         if not sel:
             return [0.0] * self.world
+        if self.aggregator.robust:
+            return [1.0 if (mask >> k) & 1 else 0.0 for k in range(self.world)]
         w = normalized_weights([self.counts[k] for k in sel] if self.weighted else None, len(sel))
         out = [0.0] * self.world
         for k, v in zip(sel, w.tolist()):
@@ -349,7 +382,10 @@ class FederatedEngine:
             ops.mlp_local_sgd(local, self.spec.dims, self.x, self.y, perm, cfg.batch_size, cfg.lr, cfg.epochs, cfg.max_nr_batches,
                               cfg.loss, self.spec.out_activation)
             contrib = local * w
-        if _dist_ready() and W > 1:
+        if self.aggregator.robust:
+            avg = self._robust_average(contrib, mask)                                     # K2 + K3, library form (gather)
+            contrib = avg if avg is not None else theta0
+        elif _dist_ready() and W > 1:
             dist.reduce(contrib, dst=self.coord, group=self.group)                       # K2 + K3, library form
         if self.opt_state is None:
             expected = theta0 + self.server_lr * (contrib - theta0)
@@ -467,6 +503,7 @@ class FederatedEngine:
             self.loss_history: List[torch.Tensor] = []
 
         opt_kind, opt_hyper, opt_m, opt_v = self._opt_args()
+        agg_kind, agg_trim = self._agg_args()
 
         def star(do_reduce: bool, do_bcast: bool, mask_reduce: int, mask_bcast: int, arrive_epoch: int, bcast_epoch: int):
             wts = [float(v) for v in self._round_weights(mask_reduce)] if do_reduce else [0.0] * W
@@ -475,11 +512,11 @@ class FederatedEngine:
                 ext.star_round(self.theta.data_ptr(), arena.ptr("slots"), P4, arena.ptr("flags", None, 1), arrive_epoch,
                                inbox_ptrs, bflag_ptrs, bcast_epoch, 0, mask_reduce, self.server_lr, P4, True, False,
                                self.grid_counter.data_ptr(), n_blocks, self.round_deadline_ms, wts, self.decision.data_ptr(),
-                               opt_kind, opt_hyper, opt_m, opt_v)
+                               opt_kind, opt_hyper, opt_m, opt_v, agg_kind, agg_trim)
                 ext.star_round(self.theta.data_ptr(), arena.ptr("slots"), P4, arena.ptr("flags", None, 1), arrive_epoch,
                                inbox_ptrs, bflag_ptrs, bcast_epoch, arena.mc_ptr("inbox"),
                                mask_bcast, self.server_lr, P4, False, True, self.grid_counter.data_ptr(), n_blocks, 0.0, wts, 0,
-                               opt_kind, opt_hyper, opt_m, opt_v)
+                               opt_kind, opt_hyper, opt_m, opt_v, agg_kind, agg_trim)
                 return 2
             mask = mask_reduce if do_reduce else mask_bcast
             # NVLS broadcast also for a subset: multimem.st lands in every rank's inbox (one egress copy, the switch replicates);
@@ -488,7 +525,7 @@ class FederatedEngine:
             ext.star_round(self.theta.data_ptr(), arena.ptr("slots"), P4, arena.ptr("flags", None, 1), arrive_epoch,
                            inbox_ptrs, bflag_ptrs, bcast_epoch, mc, mask, self.server_lr, P4, do_reduce, do_bcast,
                            self.grid_counter.data_ptr(), n_blocks, self.round_deadline_ms if do_reduce else 0.0, wts,
-                           self.decision.data_ptr(), opt_kind, opt_hyper, opt_m, opt_v)
+                           self.decision.data_ptr(), opt_kind, opt_hyper, opt_m, opt_v, agg_kind, agg_trim)
             return 1
 
         self._phases_begin()
@@ -552,7 +589,7 @@ class FederatedEngine:
                            bytes_bcast=4 * self.P * sum(nsel), bytes_reduce=4 * self.P * sum(nsel),
                            extra={"provider": arena.provider, "multicast": arena.has_multicast, "phases_ms": phases,
                                   "arrived_masks": arrived_log.tolist() if (is_coord and self.round_deadline_ms > 0) else None,
-                                  "server_opt": self.server_opt.kind})
+                                  "server_opt": self.server_opt.kind, "aggregator": self.aggregator.kind})
 
     # ------------------------------------------------------------------------------------------ twoshot
     def _layerwise_trainer(self):
@@ -652,6 +689,7 @@ class FederatedEngine:
             decision_ptrs, global_ptrs = arena.peer_ptrs("decision"), arena.peer_ptrs("global")
         use_prev = abs(self.server_lr - 1.0) > 1e-12 or self.opt_state is not None
         opt_kind, opt_hyper, opt_m, opt_v = self._opt_args()
+        agg_kind, agg_trim = self._agg_args()
         if use_prev and getattr(self, "theta_prev", None) is None:
             # server_lr != 1 or a server optimizer: theta <- theta + lr_s (sum_k w_k theta_k - theta) (or the optimizer step) needs
             # the model the round started from, and the ranks train IN PLACE on the arena — every rank keeps a copy (one local
@@ -696,7 +734,8 @@ class FederatedEngine:
             #   uniform weights over all ranks   -> reduce as is, scale the sum by 1/W in the kernel
             #   n_k weights and / or a subset    -> every rank first scales its own arena by its weight (0 when it was not
             #                                       selected: it presents zeros), the kernel sums with weight 1 over ALL ranks
-            nvls = self.use_nvls and arena.has_multicast and W > 1 and not use_prev and bool(sel_w)
+            # (a robust aggregate is not a sum: the switch cannot form it, the P2P path does)
+            nvls = self.use_nvls and arena.has_multicast and W > 1 and not use_prev and bool(sel_w) and not self.aggregator.robust
             prescale = nvls and (masks[i] != full or max(sel_w) - min(sel_w) >= 1e-7)
             if deadline and prescale:          # (a dropped rank's pre-scaled arena could not be renormalised away inside the switch)
                 nvls = prescale = False
@@ -715,7 +754,7 @@ class FederatedEngine:
                                                 self.chunk_elems, r, blocks, arrive_ptrs, need_wait,
                                                 arena.mc_ptr("work") if nvls else 0,
                                                 arena.mc_ptr("shadow") if (nvls and self.bf16_shadow) else 0,
-                                                self.round_deadline_ms, decision_ptrs, global_ptrs)
+                                                self.round_deadline_ms, decision_ptrs, global_ptrs, agg_kind, agg_trim)
                     return
                 ext.twoshot_fedavg(work_ptrs, shadow_ptrs, cflag_ptrs, arena.ptr("flags", None, 1), self.weights_dev.data_ptr(),
                                    self.theta_prev.data_ptr() if use_prev else 0, e, full if prescale else masks[i], self.server_lr, P4,
@@ -723,7 +762,8 @@ class FederatedEngine:
                                    arrive_ptrs if not produced_ptr else [], need_wait,
                                    arena.mc_ptr("work") if nvls else 0,
                                    arena.mc_ptr("shadow") if (nvls and self.bf16_shadow) else 0,
-                                   produced_ptr, self.overlap_timeout_s if produced_ptr else 0.0, opt_kind, opt_hyper, opt_m, opt_v)
+                                   produced_ptr, self.overlap_timeout_s if produced_ptr else 0.0, opt_kind, opt_hyper, opt_m, opt_v,
+                                   agg_kind, agg_trim)
 
             # fused wgrad -> FedAvg reduce: every rank trains this round, so every rank's last backward reports its chunks
             prod = self._produced_spec() if (masks[i] == full and not prescale and not deadline) else None
@@ -775,7 +815,8 @@ class FederatedEngine:
                            bytes_bcast=4 * self.P * sum(nsel), bytes_reduce=4 * self.P * sum(nsel),
                            extra={"provider": arena.provider, "train_path": getattr(self, "_last_path", None), "phases_ms": phases,
                                   "n_chunks": self.n_chunks, "nvls": getattr(self, "_last_nvls", False),
-                                  "arrived_masks": getattr(self, "_arrived_masks", None), "server_opt": self.server_opt.kind})
+                                  "arrived_masks": getattr(self, "_arrived_masks", None), "server_opt": self.server_opt.kind,
+                                  "aggregator": self.aggregator.kind})
 
     # ------------------------------------------------------------------------------------------ cpu / gloo
     def _run_cpu(self, rounds: int, masks: List[int]) -> RoundReport:
@@ -797,8 +838,13 @@ class FederatedEngine:
             lvec = torch.zeros(W, 2)
             lvec[r, 0] = float(loss)
             with self._phase("reduce_apply"):
+                robust = self.aggregator.robust
+                if robust:
+                    avg = self._robust_average(local, masks[i])                           # K2 + K3 (gather)
+                    contrib = avg if avg is not None else self.theta                       # (nobody selected: theta stays)
                 if _dist_ready() and W > 1:
-                    dist.reduce(contrib, dst=self.coord, group=self.group)                 # K2 + K3
+                    if not robust:
+                        dist.reduce(contrib, dst=self.coord, group=self.group)             # K2 + K3
                     dist.reduce(lvec, dst=self.coord, group=self.group)
                 if r == self.coord:
                     st = self.opt_state
@@ -812,4 +858,5 @@ class FederatedEngine:
         nsel = [bin(m).count("1") for m in masks]
         return RoundReport(rounds, W, "cpu", "gloo", (time.perf_counter() - t0) * 1e3, losses_log, 0,
                            bytes_bcast=4 * self.P * sum(nsel), bytes_reduce=4 * self.P * sum(nsel),
-                           extra={"phases_ms": self._phases_end(), "server_opt": self.server_opt.kind})
+                           extra={"phases_ms": self._phases_end(), "server_opt": self.server_opt.kind,
+                                  "aggregator": self.aggregator.kind})

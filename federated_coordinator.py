@@ -54,6 +54,11 @@ def build_parser() -> argparse.ArgumentParser:
     parser.add_argument("--server-beta1", type=float, default=d.server_beta1, help="first-moment decay of --server-opt, in [0, 1)")
     parser.add_argument("--server-beta2", type=float, default=d.server_beta2, help="second-moment decay of adam / yogi, in [0, 1)")
     parser.add_argument("--server-tau", type=float, default=d.server_tau, help="adaptivity of adagrad / adam / yogi (> 0)")
+    parser.add_argument("--aggregator", choices=["mean", "median", "trimmed_mean"], default=d.aggregator,
+                        help="how the client models are combined: mean = (weighted) FedAvg; median / trimmed_mean = coordinate-wise, "
+                             "unweighted, robust to a minority of bad clients (not with --weighted)")
+    parser.add_argument("--trim-fraction", type=float, default=d.trim_fraction,
+                        help="trimmed_mean: fraction of the values dropped at each end of every parameter, in [0, 0.5)")
     parser.add_argument("--seed", type=int, default=d.seed)
     parser.add_argument("--log-interval", type=int, default=d.log_interval)
     parser.add_argument("--test-path", type=str, default=d.test_path, help="CSV used by local/encrypted mode and evaluation")
@@ -116,6 +121,9 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.server_tau = getattr(ns, "server_tau", a.server_tau)
     a.server_optimizer()              # rejects a beta outside [0, 1) / tau <= 0 before anything starts
     a.log_interval, a.test_path, a.synthetic, a.weighted = ns.log_interval, ns.test_path, ns.synthetic, ns.weighted
+    a.aggregator = getattr(ns, "aggregator", a.aggregator)
+    a.trim_fraction = getattr(ns, "trim_fraction", a.trim_fraction)
+    a.client_aggregator()             # rejects a trim fraction outside [0, 0.5) and --weighted with a robust kind
     a.no_cuda, a.backend = ns.no_cuda, ns.backend
     if getattr(ns, "enc_items", None):
         a.n_train_items_enc = int(ns.enc_items)
@@ -198,7 +206,7 @@ def parse_cli(argv=None) -> argparse.Namespace:
     parser = build_parser()
     ns = parser.parse_args(argv)
     try:
-        arguments_from_cli(ns)           # the server optimizer settings (beta in [0, 1), tau > 0)
+        arguments_from_cli(ns)           # the server optimizer and aggregator settings (beta in [0, 1), tau > 0, trim in [0, 0.5))
     except ValueError as e:
         parser.error(str(e))
     return ns
