@@ -40,6 +40,7 @@ class Arguments:
     server_tau: float = 1e-3
     aggregator: str = "mean"       # mean (weighted FedAvg) | median | trimmed_mean (fl/aggregate.py; unweighted, Byzantine-robust)
     trim_fraction: float = 0.1     # trimmed_mean: fraction of the values dropped at each end, in [0, 0.5)
+    uplink: str = "fp32"           # what a device sends back after a fit: fp32 (its model) | int8 | int4 (its quantized delta, fl/uplink.py)
     backend: str = "auto"          # auto | fused | nccl | cpu
     dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the wgmma consumers)
     save_every: int = 0            # >0: checkpoint every N rounds, not only after the last one
@@ -60,6 +61,11 @@ class Arguments:
         if agg.robust and self.weighted:
             raise ValueError(f"--weighted does not apply to aggregator {self.aggregator!r}: the median / trimmed mean are unweighted")
         return agg
+
+    def uplink_codec(self):
+        """The :class:`fl.uplink.UplinkCodec` of the devices' replies."""
+        from ..fl.uplink import UplinkCodec
+        return UplinkCodec(self.uplink)
 
     def set_federated_batches(self, batches: int) -> None:
         self.federate_after_n_batches = batches

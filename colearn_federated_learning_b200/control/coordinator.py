@@ -23,6 +23,7 @@ import time
 from collections import OrderedDict
 from typing import Any, Dict, List, Optional
 
+import numpy as np
 import torch
 
 from .. import ops, settings
@@ -30,6 +31,7 @@ from ..data import federate, synthetic_for_model, BaseDataset
 from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
 from ..fl.evaluate import evaluate
+from ..fl.uplink import UplinkCodec, uplink_key
 from ..models import MLPNet, build_model, flatten_params, unflatten_params
 from ..utils.checkpoint import DEFAULT_PATH, checkpoint_compatible, load_or_init, save_model
 from ..utils.metrics import RoundLogger
@@ -307,13 +309,21 @@ class Coordinator(BusClient):
         log.info("Start training")
         self.metrics.start_training(cfg.max_nr_batches)
         result: Dict[str, Any] = {"workers": list(to_train.keys()), "losses": {}, "rounds": self.enabled_round}
+        codec = self.args.uplink_codec()
+        result["uplink"] = codec.kind
         for r in range(self.enabled_round):
             t0 = time.time()
             flats, losses, counts = train_virtual_workers(theta, model, fed, cfg, r)
             live = [i for i, c in enumerate(counts) if c > 0]
             if live:
                 w = normalized_weights([counts[i] for i in live] if self.args.weighted else None, len(live), device=self.device)
-                self._server_update(theta, flats[live].contiguous(), w)
+                if codec.quantized:
+                    # every worker's delta through the uplink codec (one batched encode), as a device would send it
+                    keys = [uplink_key(fed.workers[i], cfg.seed + r) for i in live]
+                    payload, scales = ops.encode_delta(flats[live], theta, codec, keys)
+                    self._server_update(theta, None, w, uplink=(payload, scales, codec))
+                else:
+                    self._server_update(theta, flats[live].contiguous(), w)
             for wid, l in zip(fed.workers, losses):
                 self.metrics.worker_loss(wid, l)
                 result["losses"][wid] = l
@@ -391,7 +401,10 @@ class Coordinator(BusClient):
 
     async def _remote_rounds(self, alive, to_train, theta, cfg, loop, pool, model, result) -> torch.Tensor:
         """The round loop of ``training_remote`` (fc.py:540-568): fan the fit RPC out to every live device, FedAvg what came
-        back, repeat.  Returns the final global parameters."""
+        back, repeat.  Returns the final global parameters.  With a quantized ``--uplink-codec`` the devices send their deltas
+        (fl/uplink.py), each reply is checked by :func:`check_quantized_reply` and the decode runs inside the FedAvg kernel."""
+        codec = self.args.uplink_codec()
+        result["uplink"] = codec.kind
         for r in range(self.enabled_round):
             log.info("\n\n#### ROUND {} #####".format(r))
             t0 = time.time()
@@ -399,6 +412,10 @@ class Coordinator(BusClient):
 
             async def one(wid: str, worker: RemoteWorkerClient):
                 try:
+                    if codec.quantized:
+                        fut = loop.run_in_executor(pool, lambda: worker.fit_quantized(theta, rcfg, codec, timeout=self.fit_timeout))
+                        update, loss, n = await fut
+                        return wid, check_quantized_reply(update, codec, theta.numel()), loss, n
                     fut = loop.run_in_executor(pool, lambda: worker.fit(theta, rcfg, timeout=self.fit_timeout))
                     flat, loss, n = await fut
                     # a device's reply is untrusted input: a wrong-length or non-finite model would poison (or abort) the
@@ -430,10 +447,13 @@ class Coordinator(BusClient):
                     result["dropped"].append(wid)
                     alive.pop(wid, None)
             if flats:
-                stacked = torch.stack(flats).to(self.device)
                 w = normalized_weights(counts if self.args.weighted else None, len(flats), device=self.device)
                 th = theta.to(self.device)
-                self._server_update(th, stacked, w)
+                if codec.quantized:
+                    uplink = (torch.stack([p for p, _ in flats]).to(self.device), torch.stack([s for _, s in flats]).to(self.device), codec)
+                    self._server_update(th, None, w, uplink=uplink)
+                else:
+                    self._server_update(th, torch.stack(flats).to(self.device), w)
                 theta = th.cpu()
                 self._average_buffers(model, [getattr(alive.get(wid), "last_buffers", None) for wid in ids], w.cpu())
             # traffic of this round: model + fit config towards the devices, trained model + loss back (paper §4.3)
@@ -445,12 +465,18 @@ class Coordinator(BusClient):
                 break
         return theta
 
-    def _server_update(self, theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor) -> None:
+    def _server_update(self, theta: torch.Tensor, models: Optional[torch.Tensor], weights: torch.Tensor, uplink=None) -> None:
         """FedAvg of ``models`` into ``theta`` in place (or their median / trimmed mean, ``--aggregator``), followed by the
-        server optimizer step of ``--server-opt``."""
+        server optimizer step of ``--server-opt``.  ``uplink = (payload, scales, codec)``: the clients' quantized deltas
+        instead of their models (``ops.fedavg_apply_quantized``; ``models`` is not used)."""
         agg = self.args.client_aggregator()
+        if uplink is None:
+            apply = lambda **kw: ops.fedavg_apply(theta, models, weights, **kw)  # noqa: E731
+        else:
+            payload, scales, codec = uplink
+            apply = lambda **kw: ops.fedavg_apply_quantized(theta, payload, scales, weights, codec, **kw)  # noqa: E731
         if self.args.server_opt == "sgd":
-            ops.fedavg_apply(theta, models, weights, self.args.server_lr, aggregator=agg)
+            apply(server_lr=self.args.server_lr, aggregator=agg)
             return
         opt = self.args.server_optimizer()
         st = self._server_opt_state
@@ -461,7 +487,7 @@ class Coordinator(BusClient):
         if st.m.device != theta.device:
             st.m = st.m.to(theta.device)
             st.v = st.v.to(theta.device) if st.v is not None else None
-        ops.fedavg_apply(theta, models, weights, opt=st, aggregator=agg)
+        apply(opt=st, aggregator=agg)
 
     @staticmethod
     def _average_buffers(model, buffers, weights) -> None:
@@ -496,6 +522,23 @@ class Coordinator(BusClient):
         finally:
             self.known_workers.pop(worker.id, None)
             worker.close()
+
+
+def check_quantized_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
+    """``(payload uint8 [codec.payload_bytes(p)], scales fp32 [codec.scale_count(p)])`` of a device's quantized reply, or
+    ValueError.  A reply is untrusted input: it must echo the codec asked for, carry exactly the bytes the codec defines for
+    ``p`` parameters, and only finite scales with ``|step| <= codec.max_scale`` (no decoded value can overflow)."""
+    if update.get("uplink") != codec.kind:
+        raise ValueError(f"uplink {update.get('uplink')!r} returned, {codec.kind!r} asked for")
+    payload, scales = update.get("payload"), update.get("scales")
+    if not isinstance(payload, bytes) or len(payload) != codec.payload_bytes(p):
+        raise ValueError(f"payload of {len(payload) if isinstance(payload, bytes) else None} bytes, expected {codec.payload_bytes(p)}")
+    if not isinstance(scales, bytes) or len(scales) != 4 * codec.scale_count(p):
+        raise ValueError(f"{len(scales) // 4 if isinstance(scales, bytes) else None} scales, expected {codec.scale_count(p)}")
+    s = torch.from_numpy(np.frombuffer(scales, dtype="<f4").copy())
+    if not bool(torch.isfinite(s).all()) or float(s.abs().max()) > codec.max_scale:
+        raise ValueError("non-finite or oversize block scale returned")
+    return torch.from_numpy(np.frombuffer(payload, dtype=np.uint8).copy()), s
 
 
 # --------------------------------------------------------------------------------------------------

@@ -30,6 +30,7 @@ import torch
 from ..data import dataset_tensors
 from ..fl.trainer import FitConfig, local_fit
 from ..fl.evaluate import predict as predict_fn
+from ..fl.uplink import UplinkCodec, uplink_key
 from ..models import build_model, num_params
 
 log = logging.getLogger(__name__)
@@ -181,6 +182,8 @@ class WorkerServer:
         if op == "fit":
             cfg = FitConfig.from_dict(req["config"])
             x, y = self.datasets[req.get("dataset_key", "training")]
+            # "uplink": send the quantized delta instead of the model (fl/uplink.py); absent = the fp32 model
+            codec = UplinkCodec(req.get("uplink", "fp32"))
             with self._work_lock:
                 model, flat, err = self._model_and_arena(cfg.model, req["params"])
                 if err:
@@ -188,12 +191,19 @@ class WorkerServer:
                 spec = getattr(model, "spec", None)
                 if spec is not None and not spec.flatten_input and x.shape[1] != spec.dims[0]:
                     return {"ok": False, "error": f"dataset has {x.shape[1]} features, {cfg.model} wants {spec.dims[0]}"}
+                received = flat.clone() if codec.quantized else None      # the theta the coordinator decodes against
                 from ..utils.threads import small_model_threads
                 with small_model_threads(flat.numel(), flat.device):   # tiny models on a CPU device: no OpenMP fork/join
                     loss, path = local_fit(flat, model, x, y, cfg, round_idx=self._round)
                 self._round += 1
                 self.fits_served += 1
-                reply = {"ok": True, "params": _to_bytes(flat), "loss": float(loss), "n": int(x.shape[0]), "path": path}
+                if codec.quantized:
+                    from .. import ops
+                    payload, scales = ops.encode_delta(flat.unsqueeze(0), received, codec, [uplink_key(self.id, cfg.seed)])
+                    reply = {"ok": True, "uplink": codec.kind, "payload": payload.cpu().numpy().tobytes(), "scales": _to_bytes(scales),
+                             "loss": float(loss), "n": int(x.shape[0]), "path": path}
+                else:
+                    reply = {"ok": True, "params": _to_bytes(flat), "loss": float(loss), "n": int(x.shape[0]), "path": path}
                 # floating-point buffers the fit updated on this device (BatchNorm running statistics): the flat arena holds
                 # named_parameters only, so without them the coordinator would save trained weights next to the INITIAL running
                 # stats and every eval-mode use of the checkpoint would be meaningless (FFNN / MLPs have none: nothing is sent)
@@ -292,6 +302,16 @@ class RemoteWorkerClient:
                            "dataset_key": dataset_key}, timeout=timeout)
         self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None     # BatchNorm statistics, if any
         return _from_bytes(resp["params"]), float(resp["loss"]), int(resp["n"])
+
+    def fit_quantized(self, flat: torch.Tensor, cfg: FitConfig, codec: UplinkCodec, dataset_key: str = "training",
+                      timeout: Optional[float] = None) -> Tuple[Dict[str, Any], float, int]:
+        """:meth:`fit` asking the device for its quantized delta (``codec``): returns the reply's ``{"uplink", "payload",
+        "scales"}`` unchecked (it is untrusted input: the coordinator validates it), the loss and the sample count."""
+        resp = self._call({"op": "fit", "config": cfg.to_dict(), "params": _to_bytes(flat), "dataset_key": dataset_key,
+                           "uplink": codec.kind}, timeout=timeout)
+        self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None
+        update = {"uplink": resp.get("uplink"), "payload": resp.get("payload"), "scales": resp.get("scales")}
+        return update, float(resp["loss"]), int(resp["n"])
 
     def search(self, tag: str) -> int:
         return int(self._call({"op": "search", "tag": tag}).get("count", 0))

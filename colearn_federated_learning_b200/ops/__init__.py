@@ -65,6 +65,65 @@ def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tenso
     return reference.fedavg_apply(theta, models, weights, server_lr, aggregator=aggregator)
 
 
+def _keys_i32(keys, device) -> torch.Tensor:
+    """uint32 keys as the int32 tensor (same bits) the kernels take"""
+    k = torch.tensor([int(x) & 0xFFFFFFFF for x in keys], dtype=torch.int64)
+    return torch.where(k >= 1 << 31, k - (1 << 32), k).to(torch.int32).to(device)
+
+
+def encode_delta(models: torch.Tensor, theta: torch.Tensor, codec, keys) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Quantize the deltas ``models [K, P] - theta [P]`` with the :class:`fl.uplink.UplinkCodec` ``codec`` (int8 / int4)
+    and the uint32 rounding ``keys`` (one per row): ``(payload uint8 [K, codec.payload_bytes(P)], scales fp32 [K,
+    codec.scale_count(P)])``.  CUDA tensors: ``quantize_delta_kernel`` in one launch (the payload is a view of rows padded
+    to 16 bytes); CPU tensors: ``reference.encode_delta``."""
+    if not codec.quantized:
+        raise ValueError("encode_delta needs an int8 / int4 codec")
+    models = models.reshape(len(keys), -1)
+    if _cuda(models):
+        payload, scales = _ext.require().quantize_delta(models.float().contiguous(), theta.float().contiguous().view(-1),
+                                                        _keys_i32(keys, models.device), codec.bits)
+        return payload[:, :codec.payload_bytes(theta.numel())], scales
+    return reference.encode_delta(models, theta, codec.bits, keys)
+
+
+def _aligned_rows(payload: torch.Tensor) -> torch.Tensor:
+    """the payload with 16-byte aligned rows (the kernels load 8 / 4 bytes per lane): as is when it already has them"""
+    if payload.stride(1) == 1 and payload.stride(0) % 16 == 0 and payload.data_ptr() % 16 == 0:
+        return payload
+    row = (payload.shape[1] + 15) // 16 * 16
+    out = torch.zeros(payload.shape[0], row, dtype=torch.uint8, device=payload.device)
+    out[:, :payload.shape[1]].copy_(payload)
+    return out
+
+
+def fedavg_apply_quantized(theta: torch.Tensor, payload: torch.Tensor, scales: torch.Tensor, weights: torch.Tensor, codec,
+                           server_lr: float = 1.0, opt=None, aggregator=None) -> torch.Tensor:
+    """:func:`fedavg_apply` on quantized deltas (``encode_delta``'s output, or the same bytes from the wire): ``a = theta +
+    sum_k w_k d^_k`` (or ``theta +`` the robust aggregate of the decoded deltas) and the server step towards ``a``, decode
+    fused into the reduce (``fedavg_q_kernel`` / ``fedavg_q_robust_kernel``).  ``opt`` / ``aggregator`` as in
+    :func:`fedavg_apply`.  CPU tensors: ``reference.fedavg_apply_quantized``."""
+    if not codec.quantized:
+        raise ValueError("fedavg_apply_quantized needs an int8 / int4 codec")
+    robust = aggregator is not None and aggregator.robust
+    if opt is not None and float(server_lr) != 1.0:
+        raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
+    if _cuda(theta):
+        dev = theta.device
+        if weights is None:                        # (a robust aggregator does not read them)
+            weights = torch.full((payload.shape[0],), 1.0 / payload.shape[0])
+        args = [theta, _aligned_rows(payload.to(dev)), scales.to(dev, torch.float32).contiguous(),
+                weights.to(dev, torch.float32).contiguous(), codec.bits]
+        if opt is not None:
+            args += [float(opt.lr), opt.code, opt.hyper, opt.m, opt.v]
+        else:
+            args += [float(server_lr), 0, [], None, None]
+        if robust:
+            args += [aggregator.code, aggregator.trim]
+        _ext.require().fedavg_apply_quantized(*args)
+        return theta
+    return reference.fedavg_apply_quantized(theta, payload, scales, weights, codec.bits, server_lr, opt=opt, aggregator=aggregator)
+
+
 def sigmoid_bce(z: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """(mean BCE(sigmoid(z), y), dL/dz) in one pass (SURVEY K9)."""
     if _cuda(z):

@@ -161,6 +161,55 @@ void fedavg_apply(torch::Tensor theta, torch::Tensor slots, torch::Tensor weight
   check(launch_fedavg_apply_opt(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(),
                                 (int)slots.size(0), o, theta.numel(), cur_stream()), "fedavg_apply (server optimizer)");
 }
+// ---- uplink codec (uplink_quant.cuh) ------------------------------------------------------------------------------------------
+// (payload uint8 [K, row_bytes], scales fp32 [K, ceil(P / 256)]) of models [K, P] - theta [P] with keys int32 [K] (uint32 bits);
+// row_bytes = the packed codes (P bytes for bits 8, ceil(P / 2) for bits 4) rounded up to 16 bytes
+std::vector<torch::Tensor> quantize_delta(torch::Tensor models, torch::Tensor theta, torch::Tensor keys, int64_t bits) {
+  CHECK_CUDA_F32(models); CHECK_CUDA_F32(theta);
+  TORCH_CHECK(models.dim() == 2 && models.size(1) == theta.numel() && models.device() == theta.device(), "models [K, P], theta [P], one device");
+  TORCH_CHECK(keys.is_cuda() && keys.scalar_type() == at::kInt && keys.is_contiguous() && keys.numel() == models.size(0) &&
+              keys.device() == theta.device(), "keys: CUDA int32 [K] on theta's device");
+  TORCH_CHECK(bits == 8 || bits == 4, "bits must be 8 or 4");
+  c10::cuda::CUDAGuard guard(theta.device());
+  const int64_t k = models.size(0), n = theta.numel();
+  const int64_t row = ((bits == 8 ? n : (n + 1) / 2) + 15) / 16 * 16;
+  auto payload = torch::empty({k, row}, models.options().dtype(at::kByte));
+  auto scales = torch::empty({k, (n + kUqBlock - 1) / kUqBlock}, models.options());
+  check(launch_quantize_delta(models.data_ptr<float>(), models.stride(0), theta.data_ptr<float>(),
+                              reinterpret_cast<const uint32_t*>(keys.data_ptr<int>()), (int)k, (int)bits, payload.data_ptr<uint8_t>(), row,
+                              scales.data_ptr<float>(), n, cur_stream()), "quantize_delta");
+  return {payload, scales};
+}
+
+// theta += step towards theta + aggregate of the K decoded deltas (payload uint8 [K, >= packed codes] with 16-byte aligned rows,
+// scales fp32 [K, ceil(P / 256)]); the server optimizer / aggregator arguments as in fedavg_apply
+void fedavg_apply_quantized(torch::Tensor theta, torch::Tensor payload, torch::Tensor scales, torch::Tensor weights, int64_t bits,
+                            double server_lr, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<torch::Tensor> m,
+                            c10::optional<torch::Tensor> v, int64_t agg_kind, double trim) {
+  CHECK_CUDA_F32(theta); CHECK_CUDA_F32(scales); CHECK_CUDA_F32(weights);
+  const int64_t n = theta.numel(), k = payload.size(0);
+  TORCH_CHECK(payload.is_cuda() && payload.scalar_type() == at::kByte && payload.dim() == 2 && payload.stride(1) == 1 &&
+              payload.device() == theta.device(), "payload: CUDA uint8 [K, row_bytes] on theta's device");
+  TORCH_CHECK(scales.dim() == 2 && scales.size(0) == k && scales.size(1) == (n + kUqBlock - 1) / kUqBlock && weights.numel() == k &&
+              scales.device() == theta.device() && weights.device() == theta.device(), "scales [K, ceil(P / 256)], weights [K]");
+  c10::cuda::CUDAGuard guard(theta.device());
+  auto state = [&](const c10::optional<torch::Tensor>& t, const char* name) -> int64_t {
+    if (!t.has_value()) return 0;
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() >= n &&
+                t->device() == theta.device(), name, ": contiguous CUDA float32 with one element per parameter, on theta's device");
+    return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
+  };
+  const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
+  const uint8_t* p = payload.data_ptr<uint8_t>();
+  if (agg_kind != AGG_MEAN) {
+    check(launch_fedavg_apply_quantized_robust(theta.data_ptr<float>(), p, payload.stride(0), scales.data_ptr<float>(), (int)k, (int)bits,
+                                               agg_args(agg_kind, trim), o, n, cur_stream()), "fedavg_apply_quantized (robust aggregator)");
+    return;
+  }
+  check(launch_fedavg_apply_quantized(theta.data_ptr<float>(), p, payload.stride(0), scales.data_ptr<float>(), weights.data_ptr<float>(),
+                                      (int)k, (int)bits, o, n, cur_stream()), "fedavg_apply_quantized");
+}
+
 torch::Tensor fedavg_flat(torch::Tensor slots, torch::Tensor weights) {
   CHECK_CUDA_F32(slots); CHECK_CUDA_F32(weights);
   TORCH_CHECK(slots.dim() == 2 && weights.numel() == slots.size(0), "shapes");
@@ -650,6 +699,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("weights"), py::arg("server_lr"), py::arg("opt_kind") = 0,
         py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
         py::arg("trim") = 0.0);
+  m.def("quantize_delta", &quantize_delta);
+  m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("weights"),
+        py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
+        py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);

@@ -41,6 +41,8 @@
 #include "server_opt.cuh"
 // per-element coordinate-wise median / trimmed mean shared by the FedAvg kernels
 #include "robust_agg.cuh"
+// int8 / int4 stochastic codec of the client deltas (uplink compression) shared by the encode and the quantized FedAvg kernels
+#include "uplink_quant.cuh"
 
 namespace colearn {
 // Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
@@ -234,6 +236,18 @@ cudaError_t launch_fedavg_apply_opt(float* theta, const float* slots, int64_t sl
 // (opt.kind 0) or the server optimizer step; any k >= 1
 cudaError_t launch_fedavg_apply_robust(float* theta, const float* slots, int64_t slot_stride, int k, const AggArgs& agg,
                                        const ServerOptArgs& opt, int64_t n, cudaStream_t s);
+// Uplink codec (uplink_quant.cuh), bits = 8 or 4.  Encode: row k of payload [k, row_bytes] / scales [k, ceil(n / 256)] holds
+// the codes / block steps of models[k] - theta, rounded with keys[k]; row_bytes is a multiple of 16 and covers the packed
+// codes (n bytes for int8, ceil(n / 2) for int4); n < 2^31.
+cudaError_t launch_quantize_delta(const float* models, int64_t model_stride, const float* theta, const uint32_t* keys, int k, int bits,
+                                  uint8_t* payload, int64_t row_bytes, float* scales, int64_t n, cudaStream_t s);
+// a = theta + sum_k w[k] * decode(payload[k], scales[k]) (fmaf in slot order), then theta += opt.lr (a - theta) (opt.kind 0) or
+// the server optimizer step; payload 16-byte aligned, row_bytes a multiple of 16
+cudaError_t launch_fedavg_apply_quantized(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales,
+                                          const float* weights, int k, int bits, const ServerOptArgs& opt, int64_t n, cudaStream_t s);
+// a = theta + robust aggregate (robust_agg.cuh) of the k decoded deltas, then the step as above (agg.kind != AGG_MEAN)
+cudaError_t launch_fedavg_apply_quantized_robust(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, int k,
+                                                 int bits, const AggArgs& agg, const ServerOptArgs& opt, int64_t n, cudaStream_t s);
 // out = sum_k w[k] * slots[k]
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride,
                                const float* weights, int k, int64_t n, cudaStream_t s);

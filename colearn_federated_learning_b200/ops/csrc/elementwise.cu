@@ -174,15 +174,47 @@ __global__ void fedavg_opt_kernel(float* __restrict__ theta, const float* __rest
   }
 }
 
+// Slot loaders of the robust FedAvg body.  stream(c, j) / cached(c, j): value j of slot c, read once (register path) or
+// reread through L1 / L2 (general path); average(a, t): the a the server step moves towards, from the aggregate of the slots.
+// fp32 slots hold the client models themselves.
+struct F32Slots {
+  const float* p;
+  int64_t stride;
+  __device__ __forceinline__ float stream(int c, int64_t j) const { return __ldcs(p + c * stride + j); }
+  __device__ __forceinline__ float cached(int c, int64_t j) const { return __ldg(p + c * stride + j); }
+  __device__ __forceinline__ float average(float a, float) const { return a; }
+};
+// Quantized slots (uplink_quant.cuh) hold the clients' deltas: value j is decoded from its code and its block's step (one
+// broadcast load per warp: the 32 elements of a warp lie in one block), and a = theta + aggregate of the decoded deltas
+// (theta + x is monotone in x: the robust aggregate of the decoded models up to the final add).
+template <int BITS>
+struct QSlots {
+  const uint8_t* payload;
+  int64_t row_bytes;
+  const float* scales;
+  int64_t nblk;
+  __device__ __forceinline__ float cached(int c, int64_t j) const {
+    const float step = __ldg(scales + c * nblk + (j >> 8));
+    int q;
+    if constexpr (BITS == 8) {
+      q = (int)(int8_t)__ldg(payload + c * row_bytes + j);
+    } else {
+      q = uq_nibble(__ldg(payload + c * row_bytes + (j >> 1)), (int)(j & 1));
+    }
+    return uq_decode(q, step);
+  }
+  __device__ __forceinline__ float stream(int c, int64_t j) const { return cached(c, j); }
+  __device__ __forceinline__ float average(float a, float t) const { return t + a; }
+};
+
 // Byzantine-robust aggregate (robust_agg.cuh: coordinate-wise median / trimmed mean over all k slots, unweighted) followed by
 // theta += opt.lr (a - theta) (opt.kind 0) or a server optimizer step (server_opt.cuh).  One element per thread.
 // KMAX > 0: register path for k <= KMAX, the k values and their keys stay in registers and the rank count is KMAX x KMAX
 // unrolled compares; KMAX = 0: any k, tiles of 32 values in registers, the rank count rereads the values through L1 / L2
 // (k ceil(k / 32) loads per element).
-template <int KMAX>
-__global__ void __launch_bounds__(256)
-fedavg_robust_kernel(float* __restrict__ theta, const float* __restrict__ slots, int64_t slot_stride, int k, AggArgs agg,
-                     ServerOptArgs opt, int64_t n) {
+template <int KMAX, class Slots>
+__device__ __forceinline__ void fedavg_robust_body(float* __restrict__ theta, const Slots& slots, int k, const AggArgs& agg,
+                                                   const ServerOptArgs& opt, int64_t n) {
   const int b = agg_trim_count(agg, k);
   const uint32_t valid = k >= 32 ? 0xffffffffu : (1u << k) - 1u;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -191,14 +223,171 @@ fedavg_robust_kernel(float* __restrict__ theta, const float* __restrict__ slots,
     if constexpr (KMAX > 0) {
       float v[KMAX];
 #pragma unroll
-      for (int c = 0; c < KMAX; ++c) v[c] = c < k ? __ldcs(slots + c * slot_stride + j) : 0.f;
+      for (int c = 0; c < KMAX; ++c) v[c] = c < k ? slots.stream(c, j) : 0.f;
       a = agg_robust<KMAX>(v, valid, k, b);
     } else {
-      a = agg_robust_tiled<32>([&](int c) { return __ldg(slots + c * slot_stride + j); }, k, b);
+      a = agg_robust_tiled<32>([&](int c) { return slots.cached(c, j); }, k, b);
     }
     const float t = theta[j];
+    a = slots.average(a, t);
     theta[j] = (opt.kind == SOPT_SGD) ? fmaf(opt.lr, a - t, t) : server_opt_step(opt, j, t, a);
   }
+}
+
+template <int KMAX>
+__global__ void __launch_bounds__(256)
+fedavg_robust_kernel(float* __restrict__ theta, const float* __restrict__ slots, int64_t slot_stride, int k, AggArgs agg,
+                     ServerOptArgs opt, int64_t n) {
+  fedavg_robust_body<KMAX>(theta, F32Slots{slots, slot_stride}, k, agg, opt, n);
+}
+
+// ---- uplink codec (uplink_quant.cuh) ----------------------------------------------------------------------------------------
+// Encode: one warp per (row, 256-element block); lane l holds elements 8 l .. 8 l + 7 of the block (two 16-byte loads of the
+// model and of theta when rows are 16-byte aligned, scalar loads with the same bits otherwise), the warp takes the block
+// max with shuffles, every lane stores its 8 codes in one 8-byte (int8) or 4-byte (int4) store and lane 0 the block's step.
+// Elements past n encode as 0 (the int4 pad nibble).  Single pass.
+template <int BITS>
+__global__ void __launch_bounds__(256)
+quantize_delta_kernel(const float* __restrict__ models, int64_t model_stride, const float* __restrict__ theta,
+                      const uint32_t* __restrict__ keys, int k, uint8_t* __restrict__ payload, int64_t row_bytes,
+                      float* __restrict__ scales, int64_t n) {
+  constexpr int L = UqCodec<BITS>::kLevels;
+  const int lane = threadIdx.x & 31;
+  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t tasks = nblk * k;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const bool vec = (((uintptr_t)models | (uintptr_t)theta) & 15) == 0 && (model_stride & 3) == 0 && (n & 3) == 0;
+  for (int64_t t = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); t < tasks; t += warps) {
+    const int c = (int)(t / nblk);
+    const int64_t blk = t - (int64_t)c * nblk;
+    const int64_t e0 = blk * kUqBlock + lane * 8;
+    const float* row = models + c * model_stride;
+    float d[8];
+    if (vec) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t e = e0 + 4 * h;
+        if (e < n) {
+          const float4 m = __ldcs(reinterpret_cast<const float4*>(row + e));
+          const float4 th = __ldg(reinterpret_cast<const float4*>(theta + e));
+          d[4 * h + 0] = m.x - th.x; d[4 * h + 1] = m.y - th.y; d[4 * h + 2] = m.z - th.z; d[4 * h + 3] = m.w - th.w;
+        } else {
+          d[4 * h + 0] = 0.f; d[4 * h + 1] = 0.f; d[4 * h + 2] = 0.f; d[4 * h + 3] = 0.f;
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) d[i] = (e0 + i < n) ? row[e0 + i] - theta[e0 + i] : 0.f;
+    }
+    uint32_t amax = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const uint32_t a = uq_abs_bits(d[i]);
+      amax = a > amax ? a : amax;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const uint32_t a = __shfl_xor_sync(0xffffffffu, amax, o);
+      amax = a > amax ? a : amax;
+    }
+    float step, inv;
+    uq_block_scale(amax, L, step, inv);
+    const uint32_t key = keys[c];
+    if (e0 < n) {
+      uint8_t* out = payload + c * row_bytes;
+      if constexpr (BITS == 8) {
+        uint2 w = make_uint2(0u, 0u);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          w.x |= ((uint32_t)uq_encode(d[i], inv, key, (uint32_t)(e0 + i), L) & 0xffu) << (8 * i);
+          w.y |= ((uint32_t)uq_encode(d[4 + i], inv, key, (uint32_t)(e0 + 4 + i), L) & 0xffu) << (8 * i);
+        }
+        *reinterpret_cast<uint2*>(out + e0) = w;
+      } else {
+        uint32_t w = 0u;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) w |= ((uint32_t)uq_encode(d[i], inv, key, (uint32_t)(e0 + i), L) & 0xfu) << (4 * i);
+        *reinterpret_cast<uint32_t*>(out + (e0 >> 1)) = w;
+      }
+    }
+    if (lane == 0) scales[c * nblk + blk] = step;
+  }
+}
+
+// Decode + FedAvg reduce + apply, the quantized twin of fedavg_kernel / fedavg_opt_kernel: per element
+// acc = fmaf(w_k, d^_k, acc) in slot order from +0, a = theta + acc, then theta += opt.lr (a - theta) (OPT false) or the server
+// optimizer step (OPT true).  One warp per 256-element block (a slot's step is one broadcast load per warp), 8 elements per
+// lane: one 8-byte (int8) or 4-byte (int4) load per slot and lane.  Weights staged in shared memory as in fedavg_kernel.
+template <int BITS, bool OPT>
+__global__ void __launch_bounds__(256)
+fedavg_q_kernel(float* __restrict__ theta, const uint8_t* __restrict__ payload, int64_t row_bytes, const float* __restrict__ scales,
+                const float* __restrict__ weights, int k, ServerOptArgs opt, int64_t n) {
+  constexpr int kSw = 256;
+  __shared__ float sw[kSw];
+  for (int c = threadIdx.x; c < k && c < kSw; c += blockDim.x) sw[c] = weights[c];
+  __syncthreads();
+  auto wt = [&](int c) -> float { return c < kSw ? sw[c] : __ldg(weights + c); };
+  const int lane = threadIdx.x & 31;
+  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const bool vec = (((uintptr_t)theta | (uintptr_t)opt.m | (uintptr_t)opt.v) & 15) == 0;
+  for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
+    const int64_t e0 = blk * kUqBlock + lane * 8;
+    if (e0 >= n) continue;
+    float acc[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+    const uint8_t* p = payload + (BITS == 8 ? e0 : (e0 >> 1));
+#pragma unroll 4
+    for (int c = 0; c < k; ++c) {
+      const float step = __ldg(scales + c * nblk + blk);
+      const float w = wt(c);
+      if constexpr (BITS == 8) {
+        const uint2 v = __ldcs(reinterpret_cast<const uint2*>(p + c * row_bytes));
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          acc[i] = fmaf(w, uq_decode((int)(int8_t)(v.x >> (8 * i)), step), acc[i]);
+          acc[4 + i] = fmaf(w, uq_decode((int)(int8_t)(v.y >> (8 * i)), step), acc[4 + i]);
+        }
+      } else {
+        const uint32_t v = __ldcs(reinterpret_cast<const unsigned int*>(p + c * row_bytes));
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] = fmaf(w, uq_decode(uq_nibble(v, i), step), acc[i]);
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t e = e0 + 4 * h;
+      if (vec && e + 4 <= n) {
+        float4* t4 = reinterpret_cast<float4*>(theta + e);
+        float4 t = *t4;
+        const float4 a = make_float4(t.x + acc[4 * h], t.y + acc[4 * h + 1], t.z + acc[4 * h + 2], t.w + acc[4 * h + 3]);
+        if constexpr (OPT) {
+          t = server_opt_step4(opt, e >> 2, t, a);
+        } else {
+          t.x = fmaf(opt.lr, a.x - t.x, t.x); t.y = fmaf(opt.lr, a.y - t.y, t.y);
+          t.z = fmaf(opt.lr, a.z - t.z, t.z); t.w = fmaf(opt.lr, a.w - t.w, t.w);
+        }
+        *t4 = t;
+      } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          if (e + i < n) {
+            const float t = theta[e + i], a = t + acc[4 * h + i];
+            theta[e + i] = OPT ? server_opt_step(opt, e + i, t, a) : fmaf(opt.lr, a - t, t);
+          }
+        }
+      }
+    }
+  }
+}
+
+// robust aggregate of the decoded deltas: the body of fedavg_robust_kernel with the decoding loader
+template <int KMAX, int BITS>
+__global__ void __launch_bounds__(256)
+fedavg_q_robust_kernel(float* __restrict__ theta, const uint8_t* __restrict__ payload, int64_t row_bytes, const float* __restrict__ scales,
+                       int k, AggArgs agg, ServerOptArgs opt, int64_t n) {
+  fedavg_robust_body<KMAX>(theta, QSlots<BITS>{payload, row_bytes, scales, (n + kUqBlock - 1) / kUqBlock}, k, agg, opt, n);
 }
 
 // ---- losses ---------------------------------------------------------------------------------------
@@ -536,6 +725,76 @@ cudaError_t launch_fedavg_apply_robust(float* theta, const float* slots, int64_t
     COLEARN_LAUNCH(fedavg_robust_kernel<0>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
   }
   return cudaGetLastError();
+}
+namespace {
+// one warp per 256-element block (of one row): 8 warps per CTA, at most the persistent grid
+inline int grid_for_warps(int64_t warp_tasks) {
+  int64_t b = (warp_tasks + kThreads / 32 - 1) / (kThreads / 32);
+  if (b > 132 * 8) b = 132 * 8;
+  return (int)(b < 1 ? 1 : b);
+}
+// kernel pointers: launched through COLEARN_LAUNCH like a kernel name (template argument lists would split the macro's arguments)
+template <int BITS>
+inline cudaError_t launch_quantize_delta_t(const float* models, int64_t model_stride, const float* theta, const uint32_t* keys, int k,
+                                           uint8_t* payload, int64_t row_bytes, float* scales, int64_t n, cudaStream_t s) {
+  auto kernel = quantize_delta_kernel<BITS>;
+  COLEARN_LAUNCH(kernel, grid_for_warps(k * ((n + kUqBlock - 1) / kUqBlock)), kThreads, 0, s, models, model_stride, theta, keys, k, payload,
+                 row_bytes, scales, n);
+  return cudaGetLastError();
+}
+template <int BITS>
+inline cudaError_t launch_fedavg_q_t(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, const float* weights,
+                                     int k, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
+  const int grid = grid_for_warps((n + kUqBlock - 1) / kUqBlock);
+  if (opt.kind == SOPT_SGD) {
+    auto kernel = fedavg_q_kernel<BITS, false>;
+    COLEARN_LAUNCH(kernel, grid, kThreads, 0, s, theta, payload, row_bytes, scales, weights, k, opt, n);
+  } else {
+    auto kernel = fedavg_q_kernel<BITS, true>;
+    COLEARN_LAUNCH(kernel, grid, kThreads, 0, s, theta, payload, row_bytes, scales, weights, k, opt, n);
+  }
+  return cudaGetLastError();
+}
+template <int BITS>
+inline cudaError_t launch_fedavg_q_robust_t(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, int k,
+                                            const AggArgs& agg, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
+  const int grid = grid_for(n, 1);
+  void (*kernel)(float*, const uint8_t*, int64_t, const float*, int, AggArgs, ServerOptArgs, int64_t);
+  // as launch_fedavg_apply_robust: the smallest register path that holds k, the general path above 32
+  if (k <= 4) kernel = fedavg_q_robust_kernel<4, BITS>;
+  else if (k <= 8) kernel = fedavg_q_robust_kernel<8, BITS>;
+  else if (k <= 16) kernel = fedavg_q_robust_kernel<16, BITS>;
+  else if (k <= 32) kernel = fedavg_q_robust_kernel<32, BITS>;
+  else kernel = fedavg_q_robust_kernel<0, BITS>;
+  COLEARN_LAUNCH(kernel, grid, kThreads, 0, s, theta, payload, row_bytes, scales, k, agg, opt, n);
+  return cudaGetLastError();
+}
+inline bool uq_layout_ok(int bits, const uint8_t* payload, int64_t row_bytes, int64_t n) {
+  if (bits != 8 && bits != 4) return false;
+  if (n < 1 || n >= ((int64_t)1 << 31)) return false;            // element indices are hashed as uint32
+  const int64_t need = bits == 8 ? n : (n + 1) / 2;
+  return (row_bytes & 15) == 0 && row_bytes >= need && (reinterpret_cast<uintptr_t>(payload) & 15) == 0;
+}
+}  // namespace
+
+cudaError_t launch_quantize_delta(const float* models, int64_t model_stride, const float* theta, const uint32_t* keys, int k, int bits,
+                                  uint8_t* payload, int64_t row_bytes, float* scales, int64_t n, cudaStream_t s) {
+  if (k < 1 || model_stride < n || !uq_layout_ok(bits, payload, row_bytes, n)) return cudaErrorInvalidValue;
+  return bits == 8 ? launch_quantize_delta_t<8>(models, model_stride, theta, keys, k, payload, row_bytes, scales, n, s)
+                   : launch_quantize_delta_t<4>(models, model_stride, theta, keys, k, payload, row_bytes, scales, n, s);
+}
+cudaError_t launch_fedavg_apply_quantized(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales,
+                                          const float* weights, int k, int bits, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
+  if (k < 1 || !uq_layout_ok(bits, payload, row_bytes, n) || !server_opt_args_ok(opt)) return cudaErrorInvalidValue;
+  return bits == 8 ? launch_fedavg_q_t<8>(theta, payload, row_bytes, scales, weights, k, opt, n, s)
+                   : launch_fedavg_q_t<4>(theta, payload, row_bytes, scales, weights, k, opt, n, s);
+}
+cudaError_t launch_fedavg_apply_quantized_robust(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, int k,
+                                                 int bits, const AggArgs& agg, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
+  if (k < 1 || agg.kind == AGG_MEAN || !agg_args_ok(agg) || !server_opt_args_ok(opt) || !uq_layout_ok(bits, payload, row_bytes, n))
+    return cudaErrorInvalidValue;
+  return bits == 8 ? launch_fedavg_q_robust_t<8>(theta, payload, row_bytes, scales, k, agg, opt, n, s)
+                   : launch_fedavg_q_robust_t<4>(theta, payload, row_bytes, scales, k, agg, opt, n, s);
 }
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride, const float* weights,
                                int k, int64_t n, cudaStream_t s) {

@@ -138,6 +138,36 @@ void fedavg_apply(Tensor theta, Tensor slots, Tensor w, double server_lr, int64_
   CK(colearn::launch_fedavg_apply_opt(fmut(theta, "theta"), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0), o,
                                       theta.numel(), nullptr));
 }
+// uplink codec (uplink_quant.cuh): same shapes and row padding as bindings.cpp::quantize_delta / fedavg_apply_quantized
+std::tuple<Tensor, Tensor> quantize_delta(Tensor models, Tensor theta, Tensor keys, int64_t bits) {
+  TORCH_CHECK(models.dim() == 2 && models.size(1) == theta.numel(), "models [K, P], theta [P]");
+  TORCH_CHECK(!keys.is_cuda() && keys.scalar_type() == at::kInt && keys.is_contiguous() && keys.numel() == models.size(0), "keys int32 [K]");
+  const int64_t k = models.size(0), n = theta.numel();
+  const int64_t row = ((bits == 8 ? n : (n + 1) / 2) + 15) / 16 * 16;
+  Tensor payload = torch::zeros({k, row}, torch::kUInt8), scales = torch::zeros({k, (n + 255) / 256}, torch::kFloat);
+  {
+    py::gil_scoped_release nogil;
+    CK(colearn::launch_quantize_delta(fptr(models, "models"), models.stride(0), fptr(theta, "theta"),
+                                      reinterpret_cast<const uint32_t*>(keys.data_ptr<int>()), (int)k, (int)bits, payload.data_ptr<uint8_t>(), row,
+                                      scales.data_ptr<float>(), n, nullptr));
+  }
+  return {payload, scales};
+}
+void fedavg_apply_quantized(Tensor theta, Tensor payload, Tensor scales, Tensor w, int64_t bits, double server_lr, int64_t opt_kind,
+                            std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind, double trim) {
+  TORCH_CHECK(!payload.is_cuda() && payload.scalar_type() == at::kByte && payload.dim() == 2 && payload.stride(1) == 1, "payload uint8 [K, row]");
+  const int64_t k = payload.size(0), n = theta.numel();
+  TORCH_CHECK(scales.size(0) == k && scales.size(1) == (n + 255) / 256 && w.numel() == k, "scales [K, ceil(P / 256)], weights [K]");
+  const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, n);
+  py::gil_scoped_release nogil;
+  if (agg_kind != colearn::AGG_MEAN) {
+    CK(colearn::launch_fedavg_apply_quantized_robust(fmut(theta, "theta"), payload.data_ptr<uint8_t>(), payload.stride(0), fptr(scales, "scales"),
+                                                     (int)k, (int)bits, agg_args(agg_kind, trim), o, n, nullptr));
+    return;
+  }
+  CK(colearn::launch_fedavg_apply_quantized(fmut(theta, "theta"), payload.data_ptr<uint8_t>(), payload.stride(0), fptr(scales, "scales"),
+                                            fptr(w, "w"), (int)k, (int)bits, o, n, nullptr));
+}
 Tensor fedavg_flat(Tensor slots, Tensor w) {
   Tensor out = torch::zeros({slots.size(1)}, torch::kFloat);
   CK(colearn::launch_fedavg_flat(out.data_ptr<float>(), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0), slots.size(1), nullptr));
@@ -435,6 +465,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("w"), py::arg("server_lr"), py::arg("opt_kind") = 0,
         py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
         py::arg("trim") = 0.0);
+  m.def("quantize_delta", &quantize_delta);
+  m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("w"),
+        py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
+        py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);

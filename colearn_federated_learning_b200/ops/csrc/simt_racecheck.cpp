@@ -82,6 +82,21 @@ int main() {
     CK(launch_transpose_bf16(tin.data(), tout.data(), 70, 45, nullptr));
     std::vector<long long> A(9 * 20, 3), B(20 * 13, 5), C(9 * 13);
     CK(launch_ring_matmul(A.data(), B.data(), C.data(), 9, 20, 13, nullptr));
+    // uplink codec: encode 3 rows (warp max by shuffles), then the fused decode + FedAvg (weights in shared memory) and its
+    // robust twin, int8 and int4, with a partial last block
+    const int64_t qn = 1000, qrow = 1008;
+    std::vector<float> qtheta = randv(qn), qmodels = randv(3 * qn), qscales(3 * 4), qw(3, 1.f / 3);
+    std::vector<uint32_t> qkeys = {1u, 2u, 3u};
+    alignas(16) static uint8_t qpayload[3 * 1008];
+    for (int bits : {8, 4}) {
+      CK(launch_quantize_delta(qmodels.data(), qn, qtheta.data(), qkeys.data(), 3, bits, qpayload, qrow, qscales.data(), qn, nullptr));
+      ServerOptArgs qo;
+      memset(&qo, 0, sizeof(qo));
+      qo.lr = 1.f;
+      CK(launch_fedavg_apply_quantized(qtheta.data(), qpayload, qrow, qscales.data(), qw.data(), 3, bits, qo, qn, nullptr));
+      AggArgs qa{AGG_MEDIAN, 0.f};
+      CK(launch_fedavg_apply_quantized_robust(qtheta.data(), qpayload, qrow, qscales.data(), 3, bits, qa, qo, qn, nullptr));
+    }
   }
   printf("elementwise kernels ok\n");
   // ---- comm: star round (with deadline) and two-shot on 3 emulated ranks, reduce_push -------------------------------------------

@@ -258,6 +258,104 @@ def server_opt_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.T
     return server_opt_step(theta, aggregate(models, weights, aggregator), kind, lr, m, v, beta1, beta2, tau)
 
 
+# ------------------------------------------------------------------------------------------------
+# uplink codec (ops/csrc/uplink_quant.cuh; fl/uplink.py)
+# ------------------------------------------------------------------------------------------------
+UQ_BLOCK = 256
+_UQ_LEVELS = {8: 127, 4: 7}
+
+
+def _fmix32(h: np.ndarray) -> np.ndarray:
+    """MurmurHash3 finalizer on uint32 arrays (wrap-around arithmetic)."""
+    h = h ^ (h >> np.uint32(16))
+    h = h * np.uint32(0x85EBCA6B)
+    h = h ^ (h >> np.uint32(13))
+    h = h * np.uint32(0xC2B2AE35)
+    return h ^ (h >> np.uint32(16))
+
+
+def uplink_uniform(keys, n: int) -> np.ndarray:
+    """float32 ``[K, n]``: r_j = (fmix32(key ^ (j * 0x9E3779B9)) >> 8) * 2^-24 for the elements j < n of every key."""
+    keys = np.asarray(keys, dtype=np.int64).astype(np.uint32).reshape(-1, 1)
+    with np.errstate(over="ignore"):
+        j = np.arange(n, dtype=np.uint32) * np.uint32(0x9E3779B9)
+        h = _fmix32(keys ^ j[None, :])
+    return (h >> np.uint32(8)).astype(np.float32) * np.float32(2.0 ** -24)
+
+
+def encode_delta(models: torch.Tensor, theta: torch.Tensor, bits: int, keys) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The int8 / int4 codes of ``models [K, P] - theta [P]`` rounded with the uint32 ``keys [K]``: ``(payload uint8 [K,
+    payload bytes], scales float32 [K, ceil(P / 256)])`` in the wire layout (two's complement bytes, or nibbles with element
+    2i in the low nibble of byte i).  Vectorised numpy; bit for bit what ``quantize_delta_kernel`` writes."""
+    L = _UQ_LEVELS[bits]
+    m = models.detach().to("cpu", torch.float32).reshape(len(keys), -1).numpy()
+    t = theta.detach().to("cpu", torch.float32).reshape(-1).numpy()
+    K, P = m.shape
+    if P >= 1 << 31:
+        raise ValueError("the codec indexes elements as uint32: P must be below 2^31")
+    nblk = (P + UQ_BLOCK - 1) // UQ_BLOCK
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
+        d = np.zeros((K, nblk * UQ_BLOCK), dtype=np.float32)
+        d[:, :P] = m - t[None, :]
+        db = d.reshape(K, nblk, UQ_BLOCK)
+        sbits = (db.view(np.uint32) & np.uint32(0x7FFFFFFF)).max(axis=2)
+        nonfinite = sbits >= np.uint32(0x7F800000)
+        s = sbits.view(np.float32)
+        inv = np.float32(L) / s
+        zero = ~nonfinite & ~(inv <= np.finfo(np.float32).max)
+        step = s / np.float32(L)
+        dead = nonfinite | zero
+        step = np.where(zero, np.float32(0.0), step)
+        step = np.where(nonfinite, np.array(0x7FC00000, dtype=np.uint32).view(np.float32), step).astype(np.float32)
+        inv = np.where(dead, np.float32(0.0), inv).astype(np.float32)
+        u = (db * inv[:, :, None]).reshape(K, -1)
+        f = np.floor(u)
+        r = uplink_uniform(keys, nblk * UQ_BLOCK)
+        q = f + (r < (u - f)).astype(np.float32)
+        q = np.where(np.repeat(dead, UQ_BLOCK, axis=1), np.float32(0.0), q)
+        q = np.clip(q, -L, L).astype(np.int8)[:, :P]
+    if bits == 8:
+        payload = q.view(np.uint8)
+    else:
+        nib = (q.astype(np.uint8) & np.uint8(0xF))
+        if P % 2:
+            nib = np.concatenate([nib, np.zeros((K, 1), dtype=np.uint8)], axis=1)
+        payload = nib[:, 0::2] | (nib[:, 1::2] << np.uint8(4))
+    return torch.from_numpy(np.ascontiguousarray(payload)), torch.from_numpy(np.ascontiguousarray(step))
+
+
+def decode_codes(payload: torch.Tensor, bits: int, n: int) -> torch.Tensor:
+    """int32 codes ``[K, n]`` of a payload in the wire layout (rows may carry trailing padding)."""
+    b = payload.detach().to("cpu").numpy().astype(np.uint8)
+    if bits == 8:
+        q = b[:, :n].view(np.int8).astype(np.int32)
+    else:
+        b = b[:, :(n + 1) // 2]
+        nib = np.stack([b & np.uint8(0xF), b >> np.uint8(4)], axis=2).reshape(b.shape[0], -1)[:, :n].astype(np.int32)
+        q = np.where(nib >= 8, nib - 16, nib)
+    return torch.from_numpy(np.ascontiguousarray(q))
+
+
+def decode_delta(payload: torch.Tensor, scales: torch.Tensor, bits: int, n: int) -> torch.Tensor:
+    """float32 deltas ``[K, n]``: d^_j = (float)q_j * step of j's block."""
+    q = decode_codes(payload, bits, n).float()
+    step = scales.detach().to("cpu", torch.float32).repeat_interleave(UQ_BLOCK, dim=1)[:, :n]
+    return q * step
+
+
+def fedavg_apply_quantized(theta: torch.Tensor, payload: torch.Tensor, scales: torch.Tensor, weights: torch.Tensor, bits: int,
+                           server_lr: float = 1.0, opt=None, aggregator=None) -> torch.Tensor:
+    """``a = theta + aggregate(decoded deltas)`` (the weighted sum, or the robust aggregate of ``aggregator``), then
+    ``theta += server_lr (a - theta)`` or the server optimizer step of ``opt`` (a ``ServerOptState``), in place."""
+    deltas = decode_delta(payload, scales, bits, theta.numel()).to(theta.device)
+    w = weights.to(theta.device, torch.float32) if weights is not None else None
+    avg = theta + aggregate(deltas, w, aggregator)
+    if opt is None:
+        return theta.add_(server_lr * (avg - theta))
+    b1, b2, tau = opt.hyper
+    return server_opt_step(theta, avg, opt.kind, opt.lr, opt.m, opt.v, b1, b2, tau)
+
+
 def linear_bias_relu(x, w, b, relu=True):
     y = x.float() @ w.float().t() + b.float()
     return torch.relu(y) if relu else y

@@ -59,6 +59,10 @@ def build_parser() -> argparse.ArgumentParser:
                              "unweighted, robust to a minority of bad clients (not with --weighted)")
     parser.add_argument("--trim-fraction", type=float, default=d.trim_fraction,
                         help="trimmed_mean: fraction of the values dropped at each end of every parameter, in [0, 0.5)")
+    parser.add_argument("--uplink-codec", choices=["fp32", "int8", "int4"], default=d.uplink,
+                        help="what a device sends back after a fit: fp32 = its model; int8 / int4 = its delta to the received model, "
+                             "stochastically quantized with one scale per 256 parameters (~3.9x / ~7.5x fewer bytes); "
+                             "local and remote mode only (not with --box or -e)")
     parser.add_argument("--seed", type=int, default=d.seed)
     parser.add_argument("--log-interval", type=int, default=d.log_interval)
     parser.add_argument("--test-path", type=str, default=d.test_path, help="CSV used by local/encrypted mode and evaluation")
@@ -124,6 +128,8 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.aggregator = getattr(ns, "aggregator", a.aggregator)
     a.trim_fraction = getattr(ns, "trim_fraction", a.trim_fraction)
     a.client_aggregator()             # rejects a trim fraction outside [0, 0.5) and --weighted with a robust kind
+    a.uplink = getattr(ns, "uplink_codec", a.uplink)
+    a.uplink_codec()
     a.no_cuda, a.backend = ns.no_cuda, ns.backend
     if getattr(ns, "enc_items", None):
         a.n_train_items_enc = int(ns.enc_items)
@@ -209,6 +215,9 @@ def parse_cli(argv=None) -> argparse.Namespace:
         arguments_from_cli(ns)           # the server optimizer and aggregator settings (beta in [0, 1), tau > 0, trim in [0, 0.5))
     except ValueError as e:
         parser.error(str(e))
+    if ns.uplink_codec != "fp32" and (ns.box or ns.encryption):
+        parser.error(f"--uplink-codec {ns.uplink_codec} applies to the local and remote modes only: --box trains on the GPUs of one "
+                     "box (fp32 models over NVLink) and -e exchanges secret shares")
     return ns
 
 
