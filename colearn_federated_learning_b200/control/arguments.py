@@ -40,7 +40,9 @@ class Arguments:
     server_tau: float = 1e-3
     aggregator: str = "mean"       # mean (weighted FedAvg) | median | trimmed_mean (fl/aggregate.py; unweighted, Byzantine-robust)
     trim_fraction: float = 0.1     # trimmed_mean: fraction of the values dropped at each end, in [0, 0.5)
-    uplink: str = "fp32"           # what a device sends back after a fit: fp32 (its model) | int8 | int4 (its quantized delta, fl/uplink.py)
+    uplink: str = "fp32"           # what a device sends back after a fit: fp32 (its model) | int8 | int4 (its quantized delta) |
+                                   # topk (the largest entries of its delta, with error feedback; fl/uplink.py)
+    uplink_topk: int = 8           # topk: entries kept per block of 256 parameters, in 1..32
     backend: str = "auto"          # auto | fused | nccl | cpu
     dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the wgmma consumers)
     save_every: int = 0            # >0: checkpoint every N rounds, not only after the last one
@@ -63,9 +65,13 @@ class Arguments:
         return agg
 
     def uplink_codec(self):
-        """The :class:`fl.uplink.UplinkCodec` of the devices' replies."""
+        """The :class:`fl.uplink.UplinkCodec` of the devices' replies; topk refuses a robust aggregator (a coordinate-wise
+        median of sparse deltas is 0 wherever fewer than half the devices sent that coordinate)."""
         from ..fl.uplink import UplinkCodec
-        return UplinkCodec(self.uplink)
+        codec = UplinkCodec(self.uplink, k=self.uplink_topk)
+        if codec.sparse and self.client_aggregator().robust:
+            raise ValueError(f"--uplink-codec topk does not combine with --aggregator {self.aggregator}: only the mean of sparse deltas keeps the update")
+        return codec
 
     def set_federated_batches(self, batches: int) -> None:
         self.federate_after_n_batches = batches

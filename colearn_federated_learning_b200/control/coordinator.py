@@ -311,6 +311,8 @@ class Coordinator(BusClient):
         result: Dict[str, Any] = {"workers": list(to_train.keys()), "losses": {}, "rounds": self.enabled_round}
         codec = self.args.uplink_codec()
         result["uplink"] = codec.kind
+        # topk: every device's error-feedback residual, zero at the start of the training (memory only, not checkpointed)
+        residual = torch.zeros(len(fed.workers), theta.numel(), device=self.device) if codec.sparse else None
         for r in range(self.enabled_round):
             t0 = time.time()
             flats, losses, counts = train_virtual_workers(theta, model, fed, cfg, r)
@@ -322,6 +324,14 @@ class Coordinator(BusClient):
                     keys = [uplink_key(fed.workers[i], cfg.seed + r) for i in live]
                     payload, scales = ops.encode_delta(flats[live], theta, codec, keys)
                     self._server_update(theta, None, w, uplink=(payload, scales, codec))
+                elif codec.sparse:
+                    # the live workers' deltas plus residuals through the top-k encode (one batched launch); a worker that
+                    # did not train this round keeps its residual
+                    res = residual if len(live) == len(fed.workers) else residual[live]
+                    indices, values = ops.encode_topk_delta(flats[live], theta, res, codec)
+                    if res is not residual:
+                        residual[live] = res
+                    self._server_update(theta, None, w, uplink=(indices, values, codec))
                 else:
                     self._server_update(theta, flats[live].contiguous(), w)
             for wid, l in zip(fed.workers, losses):
@@ -402,7 +412,9 @@ class Coordinator(BusClient):
     async def _remote_rounds(self, alive, to_train, theta, cfg, loop, pool, model, result) -> torch.Tensor:
         """The round loop of ``training_remote`` (fc.py:540-568): fan the fit RPC out to every live device, FedAvg what came
         back, repeat.  Returns the final global parameters.  With a quantized ``--uplink-codec`` the devices send their deltas
-        (fl/uplink.py), each reply is checked by :func:`check_quantized_reply` and the decode runs inside the FedAvg kernel."""
+        (fl/uplink.py), each reply is checked by :func:`check_quantized_reply` and the decode runs inside the FedAvg kernel;
+        with ``topk`` they send sparse deltas with error feedback (the first round resets their residuals), checked by
+        :func:`check_topk_reply`."""
         codec = self.args.uplink_codec()
         result["uplink"] = codec.kind
         for r in range(self.enabled_round):
@@ -416,6 +428,10 @@ class Coordinator(BusClient):
                         fut = loop.run_in_executor(pool, lambda: worker.fit_quantized(theta, rcfg, codec, timeout=self.fit_timeout))
                         update, loss, n = await fut
                         return wid, check_quantized_reply(update, codec, theta.numel()), loss, n
+                    if codec.sparse:
+                        fut = loop.run_in_executor(pool, lambda: worker.fit_topk(theta, rcfg, codec, ef_reset=r == 0, timeout=self.fit_timeout))
+                        update, loss, n = await fut
+                        return wid, check_topk_reply(update, codec, theta.numel()), loss, n
                     fut = loop.run_in_executor(pool, lambda: worker.fit(theta, rcfg, timeout=self.fit_timeout))
                     flat, loss, n = await fut
                     # a device's reply is untrusted input: a wrong-length or non-finite model would poison (or abort) the
@@ -449,7 +465,7 @@ class Coordinator(BusClient):
             if flats:
                 w = normalized_weights(counts if self.args.weighted else None, len(flats), device=self.device)
                 th = theta.to(self.device)
-                if codec.quantized:
+                if codec.quantized or codec.sparse:
                     uplink = (torch.stack([p for p, _ in flats]).to(self.device), torch.stack([s for _, s in flats]).to(self.device), codec)
                     self._server_update(th, None, w, uplink=uplink)
                 else:
@@ -468,10 +484,14 @@ class Coordinator(BusClient):
     def _server_update(self, theta: torch.Tensor, models: Optional[torch.Tensor], weights: torch.Tensor, uplink=None) -> None:
         """FedAvg of ``models`` into ``theta`` in place (or their median / trimmed mean, ``--aggregator``), followed by the
         server optimizer step of ``--server-opt``.  ``uplink = (payload, scales, codec)``: the clients' quantized deltas
-        instead of their models (``ops.fedavg_apply_quantized``; ``models`` is not used)."""
+        instead of their models (``ops.fedavg_apply_quantized``; ``models`` is not used); ``(indices, values, codec)`` with a
+        topk codec: their sparse deltas (``ops.fedavg_apply_topk``)."""
         agg = self.args.client_aggregator()
         if uplink is None:
             apply = lambda **kw: ops.fedavg_apply(theta, models, weights, **kw)  # noqa: E731
+        elif uplink[2].sparse:
+            indices, values, codec = uplink
+            apply = lambda **kw: ops.fedavg_apply_topk(theta, indices, values, weights, codec, **kw)  # noqa: E731
         else:
             payload, scales, codec = uplink
             apply = lambda **kw: ops.fedavg_apply_quantized(theta, payload, scales, weights, codec, **kw)  # noqa: E731
@@ -539,6 +559,31 @@ def check_quantized_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
     if not bool(torch.isfinite(s).all()) or float(s.abs().max()) > codec.max_scale:
         raise ValueError("non-finite or oversize block scale returned")
     return torch.from_numpy(np.frombuffer(payload, dtype=np.uint8).copy()), s
+
+
+def check_topk_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
+    """``(indices uint8 [codec.entries(p)], values fp32 [codec.entries(p)])`` of a device's top-k reply, or ValueError.  A
+    reply is untrusted input: it must echo the codec and ``k`` asked for, carry exactly ``codec.entries(p)`` offsets and
+    values, offsets strictly ascending inside each block and below the block's length (so the decode sees each coordinate
+    at most once per device), and only finite values."""
+    if update.get("uplink") != codec.kind or type(update.get("topk")) is not int or update.get("topk") != codec.k:
+        raise ValueError(f"uplink {update.get('uplink')!r} / topk {update.get('topk')!r} returned, {codec.kind!r} / {codec.k} asked for")
+    e = codec.entries(p)
+    indices, values = update.get("indices"), update.get("values")
+    if not isinstance(indices, bytes) or len(indices) != e:
+        raise ValueError(f"{len(indices) if isinstance(indices, bytes) else None} offsets returned, expected {e}")
+    if not isinstance(values, bytes) or len(values) != 4 * e:
+        raise ValueError(f"{len(values) // 4 if isinstance(values, bytes) else None} values returned, expected {e}")
+    idx = np.frombuffer(indices, dtype=np.uint8).astype(np.int64)
+    blk = np.arange(e) // codec.k
+    if (idx >= np.minimum(codec.BLOCK, p - blk * codec.BLOCK)).any():
+        raise ValueError("offset past the end of its block returned")
+    if ((idx[1:] <= idx[:-1]) & (blk[1:] == blk[:-1])).any():
+        raise ValueError("offsets not strictly ascending inside a block returned")
+    v = torch.from_numpy(np.frombuffer(values, dtype="<f4").copy())
+    if not bool(torch.isfinite(v).all()):
+        raise ValueError("non-finite value returned")
+    return torch.from_numpy(idx.astype(np.uint8)), v
 
 
 # --------------------------------------------------------------------------------------------------

@@ -120,6 +120,8 @@ class WorkerServer:
         # one model instance + one flat arena per architecture, reused across fits: the trainers behind local_fit
         # (layer-wise MLP, conv net) cache their buffers / CUDA graphs per (model, arena)
         self._models: Dict[str, Tuple[torch.nn.Module, torch.Tensor]] = {}
+        # topk uplink: the error-feedback residual [1, P] per architecture, on this device (memory only, like the arenas)
+        self._residuals: Dict[str, torch.Tensor] = {}
         self._work_lock = threading.Lock()   # fits / predictions share those buffers: one at a time
         outer = self
 
@@ -182,8 +184,10 @@ class WorkerServer:
         if op == "fit":
             cfg = FitConfig.from_dict(req["config"])
             x, y = self.datasets[req.get("dataset_key", "training")]
-            # "uplink": send the quantized delta instead of the model (fl/uplink.py); absent = the fp32 model
-            codec = UplinkCodec(req.get("uplink", "fp32"))
+            # "uplink": send the quantized or top-k delta instead of the model (fl/uplink.py); absent = the fp32 model.
+            # topk carries "topk" (k in 1..32, anything else is refused before the fit) and "ef_reset" (zero the residual)
+            kind = req.get("uplink", "fp32")
+            codec = UplinkCodec(kind, k=req.get("topk")) if kind == "topk" else UplinkCodec(kind)
             with self._work_lock:
                 model, flat, err = self._model_and_arena(cfg.model, req["params"])
                 if err:
@@ -191,7 +195,7 @@ class WorkerServer:
                 spec = getattr(model, "spec", None)
                 if spec is not None and not spec.flatten_input and x.shape[1] != spec.dims[0]:
                     return {"ok": False, "error": f"dataset has {x.shape[1]} features, {cfg.model} wants {spec.dims[0]}"}
-                received = flat.clone() if codec.quantized else None      # the theta the coordinator decodes against
+                received = flat.clone() if codec.quantized or codec.sparse else None   # the theta the coordinator decodes against
                 from ..utils.threads import small_model_threads
                 with small_model_threads(flat.numel(), flat.device):   # tiny models on a CPU device: no OpenMP fork/join
                     loss, path = local_fit(flat, model, x, y, cfg, round_idx=self._round)
@@ -202,6 +206,14 @@ class WorkerServer:
                     payload, scales = ops.encode_delta(flat.unsqueeze(0), received, codec, [uplink_key(self.id, cfg.seed)])
                     reply = {"ok": True, "uplink": codec.kind, "payload": payload.cpu().numpy().tobytes(), "scales": _to_bytes(scales),
                              "loss": float(loss), "n": int(x.shape[0]), "path": path}
+                elif codec.sparse:
+                    from .. import ops
+                    res = self._residuals.get(cfg.model)
+                    if req.get("ef_reset") or res is None or res.numel() != flat.numel() or res.device != flat.device:
+                        res = self._residuals[cfg.model] = torch.zeros(1, flat.numel(), device=flat.device)
+                    indices, values = ops.encode_topk_delta(flat.unsqueeze(0), received, res, codec)
+                    reply = {"ok": True, "uplink": codec.kind, "topk": codec.k, "indices": indices.cpu().numpy().tobytes(),
+                             "values": _to_bytes(values), "loss": float(loss), "n": int(x.shape[0]), "path": path}
                 else:
                     reply = {"ok": True, "params": _to_bytes(flat), "loss": float(loss), "n": int(x.shape[0]), "path": path}
                 # floating-point buffers the fit updated on this device (BatchNorm running statistics): the flat arena holds
@@ -311,6 +323,17 @@ class RemoteWorkerClient:
                            "uplink": codec.kind}, timeout=timeout)
         self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None
         update = {"uplink": resp.get("uplink"), "payload": resp.get("payload"), "scales": resp.get("scales")}
+        return update, float(resp["loss"]), int(resp["n"])
+
+    def fit_topk(self, flat: torch.Tensor, cfg: FitConfig, codec: UplinkCodec, ef_reset: bool, dataset_key: str = "training",
+                 timeout: Optional[float] = None) -> Tuple[Dict[str, Any], float, int]:
+        """:meth:`fit` asking the device for the top-k entries of its delta plus residual (``codec``), after zeroing that
+        residual if ``ef_reset``: returns the reply's ``{"uplink", "topk", "indices", "values"}`` unchecked (it is untrusted
+        input: the coordinator validates it), the loss and the sample count."""
+        resp = self._call({"op": "fit", "config": cfg.to_dict(), "params": _to_bytes(flat), "dataset_key": dataset_key,
+                           "uplink": codec.kind, "topk": codec.k, "ef_reset": bool(ef_reset)}, timeout=timeout)
+        self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None
+        update = {k: resp.get(k) for k in ("uplink", "topk", "indices", "values")}
         return update, float(resp["loss"]), int(resp["n"])
 
     def search(self, tag: str) -> int:

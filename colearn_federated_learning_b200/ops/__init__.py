@@ -124,6 +124,48 @@ def fedavg_apply_quantized(theta: torch.Tensor, payload: torch.Tensor, scales: t
     return reference.fedavg_apply_quantized(theta, payload, scales, weights, codec.bits, server_lr, opt=opt, aggregator=aggregator)
 
 
+def encode_topk_delta(models: torch.Tensor, theta: torch.Tensor, residual: torch.Tensor, codec) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Top-``codec.k`` sparsification with error feedback of ``v = (models [K, P] - theta [P]) + residual [K, P]``:
+    ``(indices uint8 [K, E], values fp32 [K, E])`` with ``E = codec.entries(P)``, and ``residual`` (fp32, contiguous)
+    overwritten in place with what was not sent.  CUDA tensors: ``topk_delta_kernel`` in one launch; CPU tensors:
+    ``reference.encode_topk_delta``."""
+    if not codec.sparse:
+        raise ValueError("encode_topk_delta needs a topk codec")
+    if residual.dtype != torch.float32 or not residual.is_contiguous() or residual.dim() != 2:
+        raise ValueError("residual must be a contiguous float32 [K, P] tensor (it is updated in place)")
+    models = models.reshape(residual.shape)
+    if _cuda(models):
+        idx, val = _ext.require().topk_delta(models.float().contiguous(), theta.float().contiguous().view(-1), residual, codec.k)
+        return idx, val
+    return reference.encode_topk_delta(models, theta, residual, codec.k)
+
+
+def fedavg_apply_topk(theta: torch.Tensor, indices: torch.Tensor, values: torch.Tensor, weights: torch.Tensor, codec,
+                      server_lr: float = 1.0, opt=None, aggregator=None) -> torch.Tensor:
+    """:func:`fedavg_apply` on top-k sparse deltas (``encode_topk_delta``'s output, or the same bytes from the wire): ``a =
+    theta + sum_k w_k d_k`` and the server step towards ``a`` (``server_lr``, or the server optimizer ``opt`` as in
+    :func:`fedavg_apply`), decode fused into the reduce (``fedavg_topk_kernel``).  A robust ``aggregator`` is refused: a
+    coordinate-wise median of k/256-sparse deltas is 0 wherever fewer than half the devices sent that coordinate, so it
+    would throw the update away.  CPU tensors: ``reference.fedavg_apply_topk``."""
+    if not codec.sparse:
+        raise ValueError("fedavg_apply_topk needs a topk codec")
+    if aggregator is not None and aggregator.robust:
+        raise ValueError(f"aggregator {aggregator.kind!r} does not apply to top-k sparse deltas: only the (weighted) mean does")
+    if opt is not None and float(server_lr) != 1.0:
+        raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
+    if _cuda(theta):
+        dev = theta.device
+        args = [theta, indices.to(dev, torch.uint8).contiguous(), values.to(dev, torch.float32).contiguous(),
+                weights.to(dev, torch.float32).contiguous(), codec.k]
+        if opt is not None:
+            args += [float(opt.lr), opt.code, opt.hyper, opt.m, opt.v]
+        else:
+            args += [float(server_lr)]
+        _ext.require().fedavg_apply_topk(*args)
+        return theta
+    return reference.fedavg_apply_topk(theta, indices, values, weights, codec.k, server_lr, opt=opt)
+
+
 def sigmoid_bce(z: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """(mean BCE(sigmoid(z), y), dL/dz) in one pass (SURVEY K9)."""
     if _cuda(z):

@@ -210,6 +210,47 @@ void fedavg_apply_quantized(torch::Tensor theta, torch::Tensor payload, torch::T
                                       (int)k, (int)bits, o, n, cur_stream()), "fedavg_apply_quantized");
 }
 
+// ---- top-k uplink with error feedback (uplink_topk.cuh) -----------------------------------------------------------------------
+// (indices uint8 [K, E], values fp32 [K, E]) of v = (models [K, P] - theta [P]) + residual [K, P], E = ut_entries(P, topk);
+// residual is overwritten with the unsent part of v
+std::vector<torch::Tensor> topk_delta(torch::Tensor models, torch::Tensor theta, torch::Tensor residual, int64_t topk) {
+  CHECK_CUDA_F32(models); CHECK_CUDA_F32(theta); CHECK_CUDA_F32(residual);
+  TORCH_CHECK(models.dim() == 2 && models.size(1) == theta.numel() && residual.sizes() == models.sizes() &&
+              models.device() == theta.device() && residual.device() == theta.device(), "models / residual [K, P], theta [P], one device");
+  TORCH_CHECK(topk >= 1 && topk <= kUtMaxK, "topk must be in 1..32");
+  c10::cuda::CUDAGuard guard(theta.device());
+  const int64_t k = models.size(0), n = theta.numel(), e = ut_entries(n, (int)topk);
+  auto indices = torch::empty({k, e}, models.options().dtype(at::kByte));
+  auto values = torch::empty({k, e}, models.options());
+  check(launch_topk_delta(models.data_ptr<float>(), models.stride(0), theta.data_ptr<float>(), residual.data_ptr<float>(), n, (int)k,
+                          (int)topk, indices.data_ptr<uint8_t>(), values.data_ptr<float>(), e, n, cur_stream()), "topk_delta");
+  return {indices, values};
+}
+
+// theta += step towards theta + the weighted sum of the K sparse deltas (indices uint8 / values fp32 [K, E(P, topk)]); the
+// server optimizer arguments as in fedavg_apply
+void fedavg_apply_topk(torch::Tensor theta, torch::Tensor indices, torch::Tensor values, torch::Tensor weights, int64_t topk,
+                       double server_lr, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<torch::Tensor> m,
+                       c10::optional<torch::Tensor> v) {
+  CHECK_CUDA_F32(theta); CHECK_CUDA_F32(values); CHECK_CUDA_F32(weights);
+  const int64_t n = theta.numel(), k = indices.size(0);
+  TORCH_CHECK(topk >= 1 && topk <= kUtMaxK, "topk must be in 1..32");
+  TORCH_CHECK(indices.is_cuda() && indices.scalar_type() == at::kByte && indices.dim() == 2 && indices.is_contiguous() &&
+              indices.size(1) == ut_entries(n, (int)topk) && values.sizes() == indices.sizes() && weights.numel() == k &&
+              indices.device() == theta.device() && values.device() == theta.device() && weights.device() == theta.device(),
+              "indices / values [K, E(P, topk)], weights [K], on theta's device");
+  c10::cuda::CUDAGuard guard(theta.device());
+  auto state = [&](const c10::optional<torch::Tensor>& t, const char* name) -> int64_t {
+    if (!t.has_value()) return 0;
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() >= n &&
+                t->device() == theta.device(), name, ": contiguous CUDA float32 with one element per parameter, on theta's device");
+    return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
+  };
+  const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
+  check(launch_fedavg_apply_topk(theta.data_ptr<float>(), indices.data_ptr<uint8_t>(), values.data_ptr<float>(), indices.size(1),
+                                 weights.data_ptr<float>(), (int)k, (int)topk, o, n, cur_stream()), "fedavg_apply_topk");
+}
+
 torch::Tensor fedavg_flat(torch::Tensor slots, torch::Tensor weights) {
   CHECK_CUDA_F32(slots); CHECK_CUDA_F32(weights);
   TORCH_CHECK(slots.dim() == 2 && weights.numel() == slots.size(0), "shapes");
@@ -699,6 +740,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("weights"), py::arg("server_lr"), py::arg("opt_kind") = 0,
         py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
         py::arg("trim") = 0.0);
+  m.def("topk_delta", &topk_delta);
+  m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("weights"),
+        py::arg("topk"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
+        py::arg("m") = py::none(), py::arg("v") = py::none());
   m.def("quantize_delta", &quantize_delta);
   m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("weights"),
         py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},

@@ -43,6 +43,8 @@
 #include "robust_agg.cuh"
 // int8 / int4 stochastic codec of the client deltas (uplink compression) shared by the encode and the quantized FedAvg kernels
 #include "uplink_quant.cuh"
+// top-k sparsified uplink with error feedback shared by the encode and the sparse FedAvg kernels
+#include "uplink_topk.cuh"
 
 namespace colearn {
 // Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
@@ -248,6 +250,15 @@ cudaError_t launch_fedavg_apply_quantized(float* theta, const uint8_t* payload, 
 // a = theta + robust aggregate (robust_agg.cuh) of the k decoded deltas, then the step as above (agg.kind != AGG_MEAN)
 cudaError_t launch_fedavg_apply_quantized_robust(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, int k,
                                                  int bits, const AggArgs& agg, const ServerOptArgs& opt, int64_t n, cudaStream_t s);
+// Top-k uplink (uplink_topk.cuh), 1 <= topk <= 32.  Encode: v = (models[r] - theta) + residual[r] for the rows r < rows;
+// row r of indices / values [rows, entries] receives the kept entries of v (entries >= ut_entries(n, topk)), and residual[r]
+// is overwritten with the unsent part of v.
+cudaError_t launch_topk_delta(const float* models, int64_t model_stride, const float* theta, float* residual, int64_t residual_stride,
+                              int rows, int topk, uint8_t* indices, float* values, int64_t entries, int64_t n, cudaStream_t s);
+// a = theta + sum_r w[r] * (entries of row r) (fmaf in slot order, each element from +0), then theta += opt.lr (a - theta)
+// (opt.kind 0) or the server optimizer step; the offsets of a block of a row must be distinct
+cudaError_t launch_fedavg_apply_topk(float* theta, const uint8_t* indices, const float* values, int64_t entries, const float* weights,
+                                     int rows, int topk, const ServerOptArgs& opt, int64_t n, cudaStream_t s);
 // out = sum_k w[k] * slots[k]
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride,
                                const float* weights, int k, int64_t n, cudaStream_t s);

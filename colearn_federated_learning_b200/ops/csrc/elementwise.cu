@@ -390,6 +390,196 @@ fedavg_q_robust_kernel(float* __restrict__ theta, const uint8_t* __restrict__ pa
   fedavg_robust_body<KMAX>(theta, QSlots<BITS>{payload, row_bytes, scales, (n + kUqBlock - 1) / kUqBlock}, k, agg, opt, n);
 }
 
+// ---- top-k uplink with error feedback (uplink_topk.cuh) -----------------------------------------------------------------------
+// exclusive prefix over the lower lanes of x in [0, 15], one ballot per bit
+__device__ __forceinline__ int warp_exclusive_prefix4(int x, uint32_t lower_lanes) {
+  int s = 0;
+#pragma unroll
+  for (int b = 0; b < 4; ++b) s += __popc(__ballot_sync(0xffffffffu, (x >> b) & 1) & lower_lanes) << b;
+  return s;
+}
+
+// Encode: one warp per (row, 256-element block); lane l holds elements 8 l .. 8 l + 7 of the block (16-byte loads of the
+// model, theta and the residual when rows are 16-byte aligned, scalar loads with the same bits otherwise).  The warp finds
+// the k_b-th greatest key T bit by bit from the top (31 rounds of one __reduce_add_sync: the largest T with
+// #{key >= T} >= k_b), keeps every key > T and the lowest-index keys == T up to k_b (a ballot prefix of the per-lane tie
+// counts), and stores the kept entries in index order at the exclusive prefix of the per-lane kept counts.  The residual is
+// written back in place.  Elements past n take key 0: they lose every tie to the block's own elements, and k_b <= m_b.
+__global__ void __launch_bounds__(256)
+topk_delta_kernel(const float* __restrict__ models, int64_t model_stride, const float* __restrict__ theta, float* __restrict__ residual,
+                  int64_t residual_stride, int k, int topk, uint8_t* __restrict__ indices, float* __restrict__ values, int64_t entries,
+                  int64_t n) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t lower_lanes = (1u << lane) - 1u;
+  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t tasks = nblk * k;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const bool vec = (((uintptr_t)models | (uintptr_t)theta | (uintptr_t)residual) & 15) == 0 && (model_stride & 3) == 0 &&
+                   (residual_stride & 3) == 0 && (n & 3) == 0;
+  for (int64_t t = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); t < tasks; t += warps) {
+    const int c = (int)(t / nblk);
+    const int64_t blk = t - (int64_t)c * nblk;
+    const int64_t e0 = blk * kUqBlock + lane * 8;
+    const float* row = models + c * model_stride;
+    float* res = residual + c * residual_stride;
+    float v[8];
+    if (vec) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t e = e0 + 4 * h;
+        if (e < n) {
+          const float4 m = __ldcs(reinterpret_cast<const float4*>(row + e));
+          const float4 th = __ldg(reinterpret_cast<const float4*>(theta + e));
+          const float4 r = *reinterpret_cast<const float4*>(res + e);
+          v[4 * h + 0] = (m.x - th.x) + r.x; v[4 * h + 1] = (m.y - th.y) + r.y;
+          v[4 * h + 2] = (m.z - th.z) + r.z; v[4 * h + 3] = (m.w - th.w) + r.w;
+        } else {
+          v[4 * h + 0] = 0.f; v[4 * h + 1] = 0.f; v[4 * h + 2] = 0.f; v[4 * h + 3] = 0.f;
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] = (e0 + i < n) ? (row[e0 + i] - theta[e0 + i]) + res[e0 + i] : 0.f;
+    }
+    uint32_t key[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) key[i] = (e0 + i < n) ? ut_key(v[i]) : 0u;
+    const int kb = ut_block_k(n, blk, topk);
+    uint32_t thr = 0;
+    for (int b = 30; b >= 0; --b) {                   // keys are below 2^31
+      const uint32_t cand = thr | (1u << b);
+      int cnt = 0;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) cnt += key[i] >= cand ? 1 : 0;
+      if (__reduce_add_sync(0xffffffffu, cnt) >= kb) thr = cand;
+    }
+    int ngt = 0, ntie = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      ngt += key[i] > thr ? 1 : 0;
+      ntie += key[i] == thr ? 1 : 0;
+    }
+    // ties this lane may keep: the kb - #{key > thr} >= 1 lowest-index ties of the block, minus those of the lower lanes
+    const int room = kb - __reduce_add_sync(0xffffffffu, ngt) - warp_exclusive_prefix4(ntie, lower_lanes);
+    // per-element flags, not a bit mask: a `keep |= 1u << i` form of this selection lost element 1's tie on the H100
+    // (sm_90a, CUDA 12.9) while its PTX and the SIMT build were right
+    bool keep[8];
+    int nkeep = 0, seen = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const bool tie = key[i] == thr;
+      keep[i] = key[i] > thr || (tie && seen < room);
+      seen += tie ? 1 : 0;
+      nkeep += keep[i] ? 1 : 0;
+    }
+    const int64_t out = c * entries + blk * topk + warp_exclusive_prefix4(nkeep, lower_lanes);
+    int o = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      if (keep[i]) {
+        indices[out + o] = (uint8_t)(lane * 8 + i);
+        values[out + o] = v[i];
+        ++o;
+      }
+    }
+    float r[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) r[i] = keep[i] ? 0.f : v[i];
+    if (vec) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t e = e0 + 4 * h;
+        if (e < n) *reinterpret_cast<float4*>(res + e) = make_float4(r[4 * h], r[4 * h + 1], r[4 * h + 2], r[4 * h + 3]);
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        if (e0 + i < n) res[e0 + i] = r[i];
+      }
+    }
+  }
+}
+
+// Sparse decode + FedAvg reduce + apply, the top-k twin of fedavg_q_kernel: one warp per 256-element block with a 256-float
+// shared accumulator per warp.  Per slot in slot order, lanes < k_b scatter-fmaf their entry into it (a slot's offsets are
+// distinct, and a __syncwarp separates slots: deterministic); the entries of 8 slots are loaded ahead of their scatters.  Then
+// lane l reads elements 8 l .. 8 l + 7 back, a = theta + acc, and theta += opt.lr (a - theta) (OPT false) or the server
+// optimizer step (OPT true).  A uint8 offset cannot leave the accumulator; offsets past the end of a partial last block land
+// in accumulator cells no lane applies.  Weights staged in shared memory as in fedavg_kernel.
+template <bool OPT>
+__global__ void __launch_bounds__(256)
+fedavg_topk_kernel(float* __restrict__ theta, const uint8_t* __restrict__ indices, const float* __restrict__ values, int64_t entries,
+                   const float* __restrict__ weights, int k, int topk, ServerOptArgs opt, int64_t n) {
+  constexpr int kSw = 256, kAhead = 8;
+  __shared__ float sw[kSw];
+  __shared__ __align__(16) float sacc[kThreads / 32][kUqBlock];
+  for (int c = threadIdx.x; c < k && c < kSw; c += blockDim.x) sw[c] = weights[c];
+  __syncthreads();
+  auto wt = [&](int c) -> float { return c < kSw ? sw[c] : __ldg(weights + c); };
+  const int lane = threadIdx.x & 31;
+  float* acc = sacc[threadIdx.x >> 5];
+  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const bool vec = (((uintptr_t)theta | (uintptr_t)opt.m | (uintptr_t)opt.v) & 15) == 0;
+  for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
+    const int64_t e0 = blk * kUqBlock + lane * 8;
+    const int kb = ut_block_k(n, blk, topk);
+    const bool sends = lane < kb;
+    const int64_t slot0 = blk * topk + lane;
+    *reinterpret_cast<float4*>(acc + lane * 8) = make_float4(0.f, 0.f, 0.f, 0.f);
+    *reinterpret_cast<float4*>(acc + lane * 8 + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+    __syncwarp();
+    for (int c0 = 0; c0 < k; c0 += kAhead) {
+      uint32_t idx[kAhead];
+      float val[kAhead];
+#pragma unroll
+      for (int u = 0; u < kAhead; ++u) {
+        idx[u] = 0;
+        val[u] = 0.f;
+        if (sends && c0 + u < k) {
+          idx[u] = __ldcs(indices + (c0 + u) * entries + slot0);
+          val[u] = __ldcs(values + (c0 + u) * entries + slot0);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < kAhead; ++u) {
+        if (c0 + u < k) {
+          if (sends) acc[idx[u]] = fmaf(wt(c0 + u), val[u], acc[idx[u]]);
+          __syncwarp();
+        }
+      }
+    }
+    if (e0 >= n) continue;
+    float a8[8];
+    const float4 lo = *reinterpret_cast<const float4*>(acc + lane * 8), hi = *reinterpret_cast<const float4*>(acc + lane * 8 + 4);
+    a8[0] = lo.x; a8[1] = lo.y; a8[2] = lo.z; a8[3] = lo.w; a8[4] = hi.x; a8[5] = hi.y; a8[6] = hi.z; a8[7] = hi.w;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t e = e0 + 4 * h;
+      if (vec && e + 4 <= n) {
+        float4* t4 = reinterpret_cast<float4*>(theta + e);
+        float4 t = *t4;
+        const float4 a = make_float4(t.x + a8[4 * h], t.y + a8[4 * h + 1], t.z + a8[4 * h + 2], t.w + a8[4 * h + 3]);
+        if constexpr (OPT) {
+          t = server_opt_step4(opt, e >> 2, t, a);
+        } else {
+          t.x = fmaf(opt.lr, a.x - t.x, t.x); t.y = fmaf(opt.lr, a.y - t.y, t.y);
+          t.z = fmaf(opt.lr, a.z - t.z, t.z); t.w = fmaf(opt.lr, a.w - t.w, t.w);
+        }
+        *t4 = t;
+      } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          if (e + i < n) {
+            const float t = theta[e + i], a = t + a8[4 * h + i];
+            theta[e + i] = OPT ? server_opt_step(opt, e + i, t, a) : fmaf(opt.lr, a - t, t);
+          }
+        }
+      }
+    }
+  }
+}
+
 // ---- losses ---------------------------------------------------------------------------------------
 __global__ void sigmoid_bce_kernel(const float* __restrict__ z, const float* __restrict__ y,
                                    float* __restrict__ dz, float* __restrict__ loss_out, int64_t n) {
@@ -795,6 +985,26 @@ cudaError_t launch_fedavg_apply_quantized_robust(float* theta, const uint8_t* pa
     return cudaErrorInvalidValue;
   return bits == 8 ? launch_fedavg_q_robust_t<8>(theta, payload, row_bytes, scales, k, agg, opt, n, s)
                    : launch_fedavg_q_robust_t<4>(theta, payload, row_bytes, scales, k, agg, opt, n, s);
+}
+cudaError_t launch_topk_delta(const float* models, int64_t model_stride, const float* theta, float* residual, int64_t residual_stride,
+                              int rows, int topk, uint8_t* indices, float* values, int64_t entries, int64_t n, cudaStream_t s) {
+  if (rows < 1 || topk < 1 || topk > kUtMaxK || n < 1 || model_stride < n || residual_stride < n || entries < ut_entries(n, topk))
+    return cudaErrorInvalidValue;
+  COLEARN_LAUNCH(topk_delta_kernel, grid_for_warps(rows * ((n + kUqBlock - 1) / kUqBlock)), kThreads, 0, s, models, model_stride, theta,
+                 residual, residual_stride, rows, topk, indices, values, entries, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_fedavg_apply_topk(float* theta, const uint8_t* indices, const float* values, int64_t entries, const float* weights,
+                                     int rows, int topk, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
+  if (rows < 1 || topk < 1 || topk > kUtMaxK || n < 1 || entries < ut_entries(n, topk) || !server_opt_args_ok(opt))
+    return cudaErrorInvalidValue;
+  const int grid = grid_for_warps((n + kUqBlock - 1) / kUqBlock);
+  if (opt.kind == SOPT_SGD) {
+    COLEARN_LAUNCH(fedavg_topk_kernel<false>, grid, kThreads, 0, s, theta, indices, values, entries, weights, rows, topk, opt, n);
+  } else {
+    COLEARN_LAUNCH(fedavg_topk_kernel<true>, grid, kThreads, 0, s, theta, indices, values, entries, weights, rows, topk, opt, n);
+  }
+  return cudaGetLastError();
 }
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride, const float* weights,
                                int k, int64_t n, cudaStream_t s) {

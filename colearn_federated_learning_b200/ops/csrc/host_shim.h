@@ -186,6 +186,13 @@ inline int __reduce_add_sync(unsigned, int v) {
   for (int i = 0; i < 32; ++i) s += all[i];
   return s;
 }
+inline unsigned __ballot_sync(unsigned, int pred) {
+  int all[32];
+  ::colearn_shim::warp_gather(pred, all);
+  unsigned m = 0;
+  for (int i = 0; i < 32; ++i) m |= (all[i] != 0 ? 1u : 0u) << i;
+  return m;
+}
 template <class T>
 inline T __ldcs(const T* p) { return *p; }
 inline float __uint_as_float(unsigned u) { float f; memcpy(&f, &u, 4); return f; }

@@ -168,6 +168,31 @@ void fedavg_apply_quantized(Tensor theta, Tensor payload, Tensor scales, Tensor 
   CK(colearn::launch_fedavg_apply_quantized(fmut(theta, "theta"), payload.data_ptr<uint8_t>(), payload.stride(0), fptr(scales, "scales"),
                                             fptr(w, "w"), (int)k, (int)bits, o, n, nullptr));
 }
+// top-k uplink (uplink_topk.cuh): same shapes as bindings.cpp::topk_delta / fedavg_apply_topk; residual [K, P] updated in place
+std::tuple<Tensor, Tensor> topk_delta(Tensor models, Tensor theta, Tensor residual, int64_t topk) {
+  TORCH_CHECK(models.dim() == 2 && models.size(1) == theta.numel() && residual.sizes() == models.sizes(), "models / residual [K, P], theta [P]");
+  TORCH_CHECK(topk >= 1 && topk <= colearn::kUtMaxK, "topk must be in 1..32");
+  const int64_t k = models.size(0), n = theta.numel(), e = colearn::ut_entries(n, (int)topk);
+  Tensor indices = torch::zeros({k, e}, torch::kUInt8), values = torch::zeros({k, e}, torch::kFloat);
+  float* res = fmut(residual, "residual");
+  {
+    py::gil_scoped_release nogil;
+    CK(colearn::launch_topk_delta(fptr(models, "models"), models.stride(0), fptr(theta, "theta"), res, n, (int)k, (int)topk,
+                                  indices.data_ptr<uint8_t>(), values.data_ptr<float>(), e, n, nullptr));
+  }
+  return {indices, values};
+}
+void fedavg_apply_topk(Tensor theta, Tensor indices, Tensor values, Tensor w, int64_t topk, double server_lr, int64_t opt_kind,
+                       std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v) {
+  TORCH_CHECK(!indices.is_cuda() && indices.scalar_type() == at::kByte && indices.dim() == 2 && indices.is_contiguous(), "indices uint8 [K, E]");
+  const int64_t k = indices.size(0), n = theta.numel();
+  TORCH_CHECK(topk >= 1 && topk <= colearn::kUtMaxK && indices.size(1) == colearn::ut_entries(n, (int)topk) &&
+              values.sizes() == indices.sizes() && w.numel() == k, "indices / values [K, E(P, topk)], weights [K]");
+  const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, n);
+  py::gil_scoped_release nogil;
+  CK(colearn::launch_fedavg_apply_topk(fmut(theta, "theta"), indices.data_ptr<uint8_t>(), fptr(values, "values"), indices.size(1),
+                                       fptr(w, "w"), (int)k, (int)topk, o, n, nullptr));
+}
 Tensor fedavg_flat(Tensor slots, Tensor w) {
   Tensor out = torch::zeros({slots.size(1)}, torch::kFloat);
   CK(colearn::launch_fedavg_flat(out.data_ptr<float>(), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0), slots.size(1), nullptr));
@@ -465,6 +490,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("w"), py::arg("server_lr"), py::arg("opt_kind") = 0,
         py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
         py::arg("trim") = 0.0);
+  m.def("topk_delta", &topk_delta);
+  m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("w"), py::arg("topk"),
+        py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(),
+        py::arg("v") = py::none());
   m.def("quantize_delta", &quantize_delta);
   m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("w"),
         py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},

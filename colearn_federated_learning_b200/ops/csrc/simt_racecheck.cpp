@@ -97,6 +97,15 @@ int main() {
       AggArgs qa{AGG_MEDIAN, 0.f};
       CK(launch_fedavg_apply_quantized_robust(qtheta.data(), qpayload, qrow, qscales.data(), 3, bits, qa, qo, qn, nullptr));
     }
+    // top-k uplink: encode 3 rows (warp select by reductions and ballots, residual written back), then the sparse decode +
+    // FedAvg (per-warp shared accumulator, one __syncwarp per slot), k = 8, with a partial last block (m_last = 232)
+    std::vector<float> kres(3 * qn, 0.f), kvals(3 * 32);
+    std::vector<uint8_t> kidx(3 * 32);
+    CK(launch_topk_delta(qmodels.data(), qn, qtheta.data(), kres.data(), qn, 3, 8, kidx.data(), kvals.data(), 32, qn, nullptr));
+    ServerOptArgs ko;
+    memset(&ko, 0, sizeof(ko));
+    ko.lr = 1.f;
+    CK(launch_fedavg_apply_topk(qtheta.data(), kidx.data(), kvals.data(), 32, qw.data(), 3, 8, ko, qn, nullptr));
   }
   printf("elementwise kernels ok\n");
   // ---- comm: star round (with deadline) and two-shot on 3 emulated ranks, reduce_push -------------------------------------------

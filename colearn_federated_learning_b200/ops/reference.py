@@ -356,6 +356,72 @@ def fedavg_apply_quantized(theta: torch.Tensor, payload: torch.Tensor, scales: t
     return server_opt_step(theta, avg, opt.kind, opt.lr, opt.m, opt.v, b1, b2, tau)
 
 
+# ------------------------------------------------------------------------------------------------
+# top-k uplink with error feedback (ops/csrc/uplink_topk.cuh; fl/uplink.py)
+# ------------------------------------------------------------------------------------------------
+def topk_entries(p: int, k: int) -> int:
+    """E(P, k) = k (nblk - 1) + min(k, m_last): the entries of one row."""
+    nblk = (p + UQ_BLOCK - 1) // UQ_BLOCK
+    return k * (nblk - 1) + min(k, p - (nblk - 1) * UQ_BLOCK)
+
+
+def topk_keys(v: np.ndarray) -> np.ndarray:
+    """uint32 selection keys of float32 ``v``: the bits of |v|, every NaN mapped to 0x7f800001."""
+    a = v.view(np.uint32) & np.uint32(0x7FFFFFFF)
+    return np.where(a > np.uint32(0x7F800000), np.uint32(0x7F800001), a)
+
+
+def encode_topk_delta(models: torch.Tensor, theta: torch.Tensor, residual: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The top-``k`` entries per 256-element block of ``v = (models [K, P] - theta [P]) + residual [K, P]``: ``(indices
+    uint8 [K, E], values float32 [K, E])`` in the wire layout (offsets ascending inside each block, blocks packed), and
+    ``residual`` overwritten in place with ``v`` minus the sent entries.  Vectorised numpy; bit for bit what
+    ``topk_delta_kernel`` writes (up to NaN payloads, which the GPU makes canonical)."""
+    if not 1 <= k <= 32:
+        raise ValueError(f"topk keeps 1..32 entries per block, not {k}")
+    m = models.detach().to("cpu", torch.float32).reshape(residual.shape).numpy()
+    t = theta.detach().to("cpu", torch.float32).reshape(-1).numpy()
+    e = residual.detach().to("cpu", torch.float32).numpy()
+    K, P = m.shape
+    nblk = (P + UQ_BLOCK - 1) // UQ_BLOCK
+    with np.errstate(over="ignore", invalid="ignore"):
+        v = (m - t[None, :]) + e
+    # composite = key 256 + (255 - offset): unique inside a block, greater = kept first (the lower offset wins a tie);
+    # elements past P get key -1 and are kept only in a last block shorter than k, where they are cut off below
+    key = np.full((K, nblk * UQ_BLOCK), -1, dtype=np.int64)
+    key[:, :P] = topk_keys(v)
+    comp = key.reshape(K, nblk, UQ_BLOCK) * UQ_BLOCK + (UQ_BLOCK - 1 - np.arange(UQ_BLOCK, dtype=np.int64))
+    top = -np.sort(-comp, axis=2)[:, :, :k]
+    off = np.sort((UQ_BLOCK - 1) - (top & (UQ_BLOCK - 1)), axis=2)
+    idx = off.reshape(K, nblk * k)[:, :topk_entries(P, k)]
+    pos = idx + (np.arange(idx.shape[1]) // k * UQ_BLOCK)[None, :]
+    values = np.take_along_axis(v, pos, axis=1)
+    rest = v.copy()
+    np.put_along_axis(rest, pos, np.float32(0.0), axis=1)
+    residual.copy_(torch.from_numpy(rest))
+    return torch.from_numpy(np.ascontiguousarray(idx.astype(np.uint8))), torch.from_numpy(np.ascontiguousarray(values))
+
+
+def decode_topk_delta(indices: torch.Tensor, values: torch.Tensor, k: int, n: int) -> torch.Tensor:
+    """float32 deltas ``[K, n]``: the entries at their positions, zero elsewhere."""
+    idx = indices.detach().to("cpu").numpy().astype(np.int64)
+    pos = idx + (np.arange(idx.shape[1]) // k * UQ_BLOCK)[None, :]
+    out = np.zeros((idx.shape[0], n), dtype=np.float32)
+    np.put_along_axis(out, pos, values.detach().to("cpu", torch.float32).numpy(), axis=1)
+    return torch.from_numpy(out)
+
+
+def fedavg_apply_topk(theta: torch.Tensor, indices: torch.Tensor, values: torch.Tensor, weights: torch.Tensor, k: int,
+                      server_lr: float = 1.0, opt=None) -> torch.Tensor:
+    """``a = theta + sum_k w_k (decoded sparse delta k)``, then ``theta += server_lr (a - theta)`` or the server optimizer
+    step of ``opt`` (a ``ServerOptState``), in place."""
+    deltas = decode_topk_delta(indices, values, k, theta.numel()).to(theta.device)
+    avg = theta + fedavg_flat(deltas, weights.to(theta.device, torch.float32))
+    if opt is None:
+        return theta.add_(server_lr * (avg - theta))
+    b1, b2, tau = opt.hyper
+    return server_opt_step(theta, avg, opt.kind, opt.lr, opt.m, opt.v, b1, b2, tau)
+
+
 def linear_bias_relu(x, w, b, relu=True):
     y = x.float() @ w.float().t() + b.float()
     return torch.relu(y) if relu else y

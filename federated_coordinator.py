@@ -59,10 +59,13 @@ def build_parser() -> argparse.ArgumentParser:
                              "unweighted, robust to a minority of bad clients (not with --weighted)")
     parser.add_argument("--trim-fraction", type=float, default=d.trim_fraction,
                         help="trimmed_mean: fraction of the values dropped at each end of every parameter, in [0, 0.5)")
-    parser.add_argument("--uplink-codec", choices=["fp32", "int8", "int4"], default=d.uplink,
+    parser.add_argument("--uplink-codec", choices=["fp32", "int8", "int4", "topk"], default=d.uplink,
                         help="what a device sends back after a fit: fp32 = its model; int8 / int4 = its delta to the received model, "
-                             "stochastically quantized with one scale per 256 parameters (~3.9x / ~7.5x fewer bytes); "
-                             "local and remote mode only (not with --box or -e)")
+                             "stochastically quantized with one scale per 256 parameters (~3.9x / ~7.5x fewer bytes); topk = the "
+                             "--uplink-topk largest entries of every 256 of its delta plus what it did not send before (error "
+                             "feedback; ~25x fewer bytes at 8); local and remote mode only (not with --box or -e)")
+    parser.add_argument("--uplink-topk", type=int, default=d.uplink_topk,
+                        help="--uplink-codec topk: entries sent per block of 256 parameters, in 1..32 (not with a robust --aggregator)")
     parser.add_argument("--seed", type=int, default=d.seed)
     parser.add_argument("--log-interval", type=int, default=d.log_interval)
     parser.add_argument("--test-path", type=str, default=d.test_path, help="CSV used by local/encrypted mode and evaluation")
@@ -129,7 +132,8 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.trim_fraction = getattr(ns, "trim_fraction", a.trim_fraction)
     a.client_aggregator()             # rejects a trim fraction outside [0, 0.5) and --weighted with a robust kind
     a.uplink = getattr(ns, "uplink_codec", a.uplink)
-    a.uplink_codec()
+    a.uplink_topk = getattr(ns, "uplink_topk", a.uplink_topk)
+    a.uplink_codec()                  # rejects a topk k outside 1..32 and topk with a robust aggregator
     a.no_cuda, a.backend = ns.no_cuda, ns.backend
     if getattr(ns, "enc_items", None):
         a.n_train_items_enc = int(ns.enc_items)
