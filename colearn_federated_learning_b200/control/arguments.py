@@ -43,6 +43,9 @@ class Arguments:
     uplink: str = "fp32"           # what a device sends back after a fit: fp32 (its model) | int8 | int4 (its quantized delta) |
                                    # topk (the largest entries of its delta, with error feedback; fl/uplink.py)
     uplink_topk: int = 8           # topk: entries kept per block of 256 parameters, in 1..32
+    downlink: str = "fp32"         # what the coordinator sends after round 0: fp32 (the model) | int8 | int4 | topk (a compressed
+                                   # delta to the replica the devices keep; needs a delta uplink; fl/uplink.py)
+    downlink_topk: int = 8         # downlink topk: entries sent per block of 256 parameters, in 1..32
     backend: str = "auto"          # auto | fused | nccl | cpu
     dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the wgmma consumers)
     save_every: int = 0            # >0: checkpoint every N rounds, not only after the last one
@@ -71,6 +74,16 @@ class Arguments:
         codec = UplinkCodec(self.uplink, k=self.uplink_topk)
         if codec.sparse and self.client_aggregator().robust:
             raise ValueError(f"--uplink-codec topk does not combine with --aggregator {self.aggregator}: only the mean of sparse deltas keeps the update")
+        return codec
+
+    def downlink_codec(self):
+        """The :class:`fl.uplink.UplinkCodec` of the model sent to the devices; a compressed one needs a delta uplink (int8 /
+        int4 / topk): the devices' deltas are then taken against the replica they trained from."""
+        from ..fl.uplink import UplinkCodec
+        codec = UplinkCodec(self.downlink, k=self.downlink_topk)
+        if codec.kind != "fp32" and self.uplink_codec().kind == "fp32":
+            raise ValueError(f"--downlink-codec {self.downlink} needs --uplink-codec int8, int4 or topk: with fp32 replies the server "
+                             "would have to shift every returned model by theta - replica")
         return codec
 
     def set_federated_batches(self, batches: int) -> None:

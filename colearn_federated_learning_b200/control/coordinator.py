@@ -19,7 +19,9 @@ from __future__ import annotations
 import asyncio
 import logging
 import os
+import secrets
 import time
+import zlib
 from collections import OrderedDict
 from typing import Any, Dict, List, Optional
 
@@ -31,7 +33,8 @@ from ..data import federate, synthetic_for_model, BaseDataset
 from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
 from ..fl.evaluate import evaluate
-from ..fl.uplink import UplinkCodec, uplink_key
+# the reply checks live next to the codec (the workers run them on the downlink wire too) and are exported from here as before
+from ..fl.uplink import UplinkCodec, check_quantized_reply, check_topk_reply, downlink_key, uplink_key  # noqa: F401
 from ..models import MLPNet, build_model, flatten_params, unflatten_params
 from ..utils.checkpoint import DEFAULT_PATH, checkpoint_compatible, load_or_init, save_model
 from ..utils.metrics import RoundLogger
@@ -40,7 +43,7 @@ from .bus import BusClient, InProcessBroker, Message
 from .event_parser import EventParser
 from .selection import (LOWER_BOUND, LOWER_BOUND_ENC, UPPER_BOUND, UPPER_BOUND_ENC, SelectionPolicy)
 from .window import TemporalWindow
-from .workers import RemoteWorkerClient, VirtualWorker
+from .workers import RemoteWorkerClient, VirtualWorker, replica_crc
 
 log = logging.getLogger(__name__)
 
@@ -313,22 +316,29 @@ class Coordinator(BusClient):
         result["uplink"] = codec.kind
         # topk: every device's error-feedback residual, zero at the start of the training (memory only, not checkpointed)
         residual = torch.zeros(len(fed.workers), theta.numel(), device=self.device) if codec.sparse else None
+        # compressed downlink: the workers train from the replica (theta at round 0, then advanced by one encode per round)
+        # and their deltas are taken against it; theta stays the true global model
+        down = self.args.downlink_codec()
+        result["downlink"] = down.kind
+        replica = theta.clone() if down.kind != "fp32" else theta
         for r in range(self.enabled_round):
             t0 = time.time()
-            flats, losses, counts = train_virtual_workers(theta, model, fed, cfg, r)
+            if r > 0 and down.kind != "fp32":
+                ops.encode_downlink(theta, replica, down, downlink_key(cfg.seed + r))
+            flats, losses, counts = train_virtual_workers(replica, model, fed, cfg, r)
             live = [i for i, c in enumerate(counts) if c > 0]
             if live:
                 w = normalized_weights([counts[i] for i in live] if self.args.weighted else None, len(live), device=self.device)
                 if codec.quantized:
                     # every worker's delta through the uplink codec (one batched encode), as a device would send it
                     keys = [uplink_key(fed.workers[i], cfg.seed + r) for i in live]
-                    payload, scales = ops.encode_delta(flats[live], theta, codec, keys)
+                    payload, scales = ops.encode_delta(flats[live], replica, codec, keys)
                     self._server_update(theta, None, w, uplink=(payload, scales, codec))
                 elif codec.sparse:
                     # the live workers' deltas plus residuals through the top-k encode (one batched launch); a worker that
                     # did not train this round keeps its residual
                     res = residual if len(live) == len(fed.workers) else residual[live]
-                    indices, values = ops.encode_topk_delta(flats[live], theta, res, codec)
+                    indices, values = ops.encode_topk_delta(flats[live], replica, res, codec)
                     if res is not residual:
                         residual[live] = res
                     self._server_update(theta, None, w, uplink=(indices, values, codec))
@@ -414,24 +424,40 @@ class Coordinator(BusClient):
         back, repeat.  Returns the final global parameters.  With a quantized ``--uplink-codec`` the devices send their deltas
         (fl/uplink.py), each reply is checked by :func:`check_quantized_reply` and the decode runs inside the FedAvg kernel;
         with ``topk`` they send sparse deltas with error feedback (the first round resets their residuals), checked by
-        :func:`check_topk_reply`."""
+        :func:`check_topk_reply`.  With a compressed ``--downlink-codec`` the rounds after the first send the devices a wire
+        to the replica they keep instead of the model (:meth:`_downlink_fields`), and a device whose replica's crc differs
+        from the coordinator's is dropped."""
         codec = self.args.uplink_codec()
-        result["uplink"] = codec.kind
+        down = self.args.downlink_codec()
+        result["uplink"], result["downlink"] = codec.kind, down.kind
+        # the replica of the model the devices hold, tagged "<nonce>:<round>" (a fresh nonce per training: a device cannot
+        # mistake an earlier training's replica for this one's); memory only
+        replica = theta.to(self.device).clone() if down.kind != "fp32" else None
+        nonce = secrets.token_hex(8)
         for r in range(self.enabled_round):
             log.info("\n\n#### ROUND {} #####".format(r))
             t0 = time.time()
             rcfg = FitConfig(**{**cfg.to_dict(), "seed": cfg.seed + r})
+            downlink = self._downlink_fields(down, theta, replica, nonce, r, rcfg.seed) if replica is not None else None
+            crc = replica_crc(replica) if replica is not None else None
+
+            def same_replica(update):
+                if crc is not None and update.get("replica_crc") != crc:
+                    raise ValueError(f"replica crc {update.get('replica_crc')!r} returned, the coordinator's is {crc}")
+                return update
 
             async def one(wid: str, worker: RemoteWorkerClient):
                 try:
                     if codec.quantized:
-                        fut = loop.run_in_executor(pool, lambda: worker.fit_quantized(theta, rcfg, codec, timeout=self.fit_timeout))
+                        fut = loop.run_in_executor(pool, lambda: worker.fit_quantized(theta, rcfg, codec, timeout=self.fit_timeout,
+                                                                                     downlink=downlink))
                         update, loss, n = await fut
-                        return wid, check_quantized_reply(update, codec, theta.numel()), loss, n
+                        return wid, check_quantized_reply(same_replica(update), codec, theta.numel()), loss, n
                     if codec.sparse:
-                        fut = loop.run_in_executor(pool, lambda: worker.fit_topk(theta, rcfg, codec, ef_reset=r == 0, timeout=self.fit_timeout))
+                        fut = loop.run_in_executor(pool, lambda: worker.fit_topk(theta, rcfg, codec, ef_reset=r == 0, timeout=self.fit_timeout,
+                                                                                downlink=downlink))
                         update, loss, n = await fut
-                        return wid, check_topk_reply(update, codec, theta.numel()), loss, n
+                        return wid, check_topk_reply(same_replica(update), codec, theta.numel()), loss, n
                     fut = loop.run_in_executor(pool, lambda: worker.fit(theta, rcfg, timeout=self.fit_timeout))
                     flat, loss, n = await fut
                     # a device's reply is untrusted input: a wrong-length or non-finite model would poison (or abort) the
@@ -480,6 +506,21 @@ class Coordinator(BusClient):
             if not alive:
                 break
         return theta
+
+    @staticmethod
+    def _downlink_fields(down: UplinkCodec, theta: torch.Tensor, replica: torch.Tensor, nonce: str, r: int, seed: int) -> Dict[str, Any]:
+        """The downlink fields of round ``r``'s fit request, built once for every device.  Round 0: the codec and the replica's
+        tag (the request carries the fp32 model, which becomes the replica).  Later rounds: the wire of ``theta - replica``
+        (rounded with ``downlink_key(seed)``), the tag it applies to and the new tag; ``replica`` advances by the wire."""
+        fields: Dict[str, Any] = {"downlink": down.kind, "downlink_topk": down.k, "replica": f"{nonce}:{r}"}
+        if r == 0:
+            return fields
+        a, b = ops.encode_downlink(theta.to(replica.device), replica, down, downlink_key(seed))
+        fields["replica_base"] = f"{nonce}:{r - 1}"
+        names = ("dpayload", "dscales") if down.quantized else ("dindices", "dvalues")
+        fields[names[0]] = a.cpu().numpy().tobytes()
+        fields[names[1]] = b.cpu().numpy().astype("<f4").tobytes()
+        return fields
 
     def _server_update(self, theta: torch.Tensor, models: Optional[torch.Tensor], weights: torch.Tensor, uplink=None) -> None:
         """FedAvg of ``models`` into ``theta`` in place (or their median / trimmed mean, ``--aggregator``), followed by the
@@ -542,48 +583,6 @@ class Coordinator(BusClient):
         finally:
             self.known_workers.pop(worker.id, None)
             worker.close()
-
-
-def check_quantized_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
-    """``(payload uint8 [codec.payload_bytes(p)], scales fp32 [codec.scale_count(p)])`` of a device's quantized reply, or
-    ValueError.  A reply is untrusted input: it must echo the codec asked for, carry exactly the bytes the codec defines for
-    ``p`` parameters, and only finite scales with ``|step| <= codec.max_scale`` (no decoded value can overflow)."""
-    if update.get("uplink") != codec.kind:
-        raise ValueError(f"uplink {update.get('uplink')!r} returned, {codec.kind!r} asked for")
-    payload, scales = update.get("payload"), update.get("scales")
-    if not isinstance(payload, bytes) or len(payload) != codec.payload_bytes(p):
-        raise ValueError(f"payload of {len(payload) if isinstance(payload, bytes) else None} bytes, expected {codec.payload_bytes(p)}")
-    if not isinstance(scales, bytes) or len(scales) != 4 * codec.scale_count(p):
-        raise ValueError(f"{len(scales) // 4 if isinstance(scales, bytes) else None} scales, expected {codec.scale_count(p)}")
-    s = torch.from_numpy(np.frombuffer(scales, dtype="<f4").copy())
-    if not bool(torch.isfinite(s).all()) or float(s.abs().max()) > codec.max_scale:
-        raise ValueError("non-finite or oversize block scale returned")
-    return torch.from_numpy(np.frombuffer(payload, dtype=np.uint8).copy()), s
-
-
-def check_topk_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
-    """``(indices uint8 [codec.entries(p)], values fp32 [codec.entries(p)])`` of a device's top-k reply, or ValueError.  A
-    reply is untrusted input: it must echo the codec and ``k`` asked for, carry exactly ``codec.entries(p)`` offsets and
-    values, offsets strictly ascending inside each block and below the block's length (so the decode sees each coordinate
-    at most once per device), and only finite values."""
-    if update.get("uplink") != codec.kind or type(update.get("topk")) is not int or update.get("topk") != codec.k:
-        raise ValueError(f"uplink {update.get('uplink')!r} / topk {update.get('topk')!r} returned, {codec.kind!r} / {codec.k} asked for")
-    e = codec.entries(p)
-    indices, values = update.get("indices"), update.get("values")
-    if not isinstance(indices, bytes) or len(indices) != e:
-        raise ValueError(f"{len(indices) if isinstance(indices, bytes) else None} offsets returned, expected {e}")
-    if not isinstance(values, bytes) or len(values) != 4 * e:
-        raise ValueError(f"{len(values) // 4 if isinstance(values, bytes) else None} values returned, expected {e}")
-    idx = np.frombuffer(indices, dtype=np.uint8).astype(np.int64)
-    blk = np.arange(e) // codec.k
-    if (idx >= np.minimum(codec.BLOCK, p - blk * codec.BLOCK)).any():
-        raise ValueError("offset past the end of its block returned")
-    if ((idx[1:] <= idx[:-1]) & (blk[1:] == blk[:-1])).any():
-        raise ValueError("offsets not strictly ascending inside a block returned")
-    v = torch.from_numpy(np.frombuffer(values, dtype="<f4").copy())
-    if not bool(torch.isfinite(v).all()):
-        raise ValueError("non-finite value returned")
-    return torch.from_numpy(idx.astype(np.uint8)), v
 
 
 # --------------------------------------------------------------------------------------------------

@@ -21,6 +21,7 @@ import socket
 import socketserver
 import struct
 import threading
+import zlib
 from typing import Any, Dict, List, Optional, Tuple
 
 import msgpack
@@ -30,7 +31,7 @@ import torch
 from ..data import dataset_tensors
 from ..fl.trainer import FitConfig, local_fit
 from ..fl.evaluate import predict as predict_fn
-from ..fl.uplink import UplinkCodec, uplink_key
+from ..fl.uplink import UplinkCodec, check_quantized_reply, check_topk_reply, uplink_key
 from ..models import build_model, num_params
 
 log = logging.getLogger(__name__)
@@ -103,6 +104,11 @@ def _from_bytes(b: bytes, device=None) -> torch.Tensor:
     return t.to(device) if device is not None else t
 
 
+def replica_crc(replica: torch.Tensor) -> int:
+    """crc32 of a downlink replica's fp32 bytes: a device reports it after every fit, the coordinator compares it with its own"""
+    return zlib.crc32(_to_bytes(replica))
+
+
 # ---------------------------------------------------------------------------------------------
 # device-side runtime
 # ---------------------------------------------------------------------------------------------
@@ -122,6 +128,8 @@ class WorkerServer:
         self._models: Dict[str, Tuple[torch.nn.Module, torch.Tensor]] = {}
         # topk uplink: the error-feedback residual [1, P] per architecture, on this device (memory only, like the arenas)
         self._residuals: Dict[str, torch.Tensor] = {}
+        # compressed downlink: (tag, replica [P]) per architecture, the model as the coordinator last sent it (memory only)
+        self._replicas: Dict[str, Tuple[str, torch.Tensor]] = {}
         self._work_lock = threading.Lock()   # fits / predictions share those buffers: one at a time
         outer = self
 
@@ -188,13 +196,36 @@ class WorkerServer:
             # topk carries "topk" (k in 1..32, anything else is refused before the fit) and "ef_reset" (zero the residual)
             kind = req.get("uplink", "fp32")
             codec = UplinkCodec(kind, k=req.get("topk")) if kind == "topk" else UplinkCodec(kind)
+            # "downlink": the model arrives as a compressed delta to the replica this device keeps (fl/uplink.py); absent = fp32
+            dkind = req.get("downlink", "fp32")
+            down = UplinkCodec(dkind, k=req.get("downlink_topk")) if dkind == "topk" else UplinkCodec(dkind)
+            if down.kind != "fp32" and not isinstance(req.get("replica"), str):
+                return {"ok": False, "error": "a compressed downlink needs the replica's tag"}
             with self._work_lock:
-                model, flat, err = self._model_and_arena(cfg.model, req["params"])
+                if down.kind != "fp32" and "replica_base" in req:
+                    model, flat, err = self._model_and_arena(cfg.model, None)
+                    wire = None if err else self._downlink_wire(req, down, cfg.model, flat.numel())
+                    if isinstance(wire, str):
+                        err = wire
+                elif "params" in req:
+                    model, flat, err = self._model_and_arena(cfg.model, req["params"])
+                else:
+                    err = "fit request without params"
                 if err:
                     return {"ok": False, "error": err}
                 spec = getattr(model, "spec", None)
                 if spec is not None and not spec.flatten_input and x.shape[1] != spec.dims[0]:
                     return {"ok": False, "error": f"dataset has {x.shape[1]} features, {cfg.model} wants {spec.dims[0]}"}
+                replica = None
+                if down.kind != "fp32":
+                    if "replica_base" in req:             # round t >= 1: advance the replica by the wire, train from it
+                        from .. import ops
+                        replica = self._replicas[cfg.model][1]
+                        ops.apply_downlink(replica, wire[0].to(replica.device), wire[1].to(replica.device), down)
+                        flat.copy_(replica)
+                    else:                                 # round 0: the fp32 model is the replica
+                        replica = flat.clone()
+                    self._replicas[cfg.model] = (str(req.get("replica")), replica)
                 received = flat.clone() if codec.quantized or codec.sparse else None   # the theta the coordinator decodes against
                 from ..utils.threads import small_model_threads
                 with small_model_threads(flat.numel(), flat.device):   # tiny models on a CPU device: no OpenMP fork/join
@@ -222,6 +253,8 @@ class WorkerServer:
                 bufs = [b.detach().reshape(-1).float() for b in model.buffers() if b.is_floating_point()]
                 if bufs:
                     reply["buffers"] = _to_bytes(torch.cat(bufs))
+                if replica is not None:
+                    reply["replica_crc"] = replica_crc(replica)
                 return reply
         if op == "predict":
             data = self.tagged.get(req.get("tag", "inference"), [])
@@ -238,12 +271,29 @@ class WorkerServer:
                 return {"ok": True, "pred": pred.reshape(-1).tolist(), "count": len(data)}
         return {"ok": False, "error": f"unknown op {op!r}"}
 
-    def _model_and_arena(self, name: str, params: bytes):
-        """(model, arena holding ``params``, error) — instances are created once per architecture."""
+    def _downlink_wire(self, req: Dict[str, Any], codec: UplinkCodec, model: str, p: int):
+        """The two wire tensors of a round t >= 1 downlink, or the reason it is refused: this device must hold the replica
+        of ``model`` tagged ``replica_base``, and the wire must pass the checks the coordinator runs on replies."""
+        held = self._replicas.get(model)
+        if held is None or held[0] != req.get("replica_base") or held[1].numel() != p:
+            return f"no replica {req.get('replica_base')!r} of {model} on this device (it holds {held[0] if held else None!r})"
+        try:
+            if codec.quantized:
+                return check_quantized_reply({"uplink": codec.kind, "payload": req.get("dpayload"), "scales": req.get("dscales")}, codec, p)
+            return check_topk_reply({"uplink": codec.kind, "topk": codec.k, "indices": req.get("dindices"), "values": req.get("dvalues")},
+                                    codec, p)
+        except ValueError as e:
+            return f"downlink refused: {e}"
+
+    def _model_and_arena(self, name: str, params: Optional[bytes]):
+        """(model, arena holding ``params``, error) — instances are created once per architecture; ``params`` None leaves
+        the arena as it is."""
         if name not in self._models:
             model = build_model(name).to(self.device)
             self._models[name] = (model, torch.empty(num_params(model), device=self.device))
         model, flat = self._models[name]
+        if params is None:
+            return model, flat, None
         incoming = _from_bytes(params)
         if incoming.numel() != flat.numel():
             return None, None, f"param count {incoming.numel()} != {flat.numel()} for {name}"
@@ -315,25 +365,42 @@ class RemoteWorkerClient:
         self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None     # BatchNorm statistics, if any
         return _from_bytes(resp["params"]), float(resp["loss"]), int(resp["n"])
 
+    @staticmethod
+    def _fit_request(flat: torch.Tensor, cfg: FitConfig, dataset_key: str, downlink: Optional[Dict[str, Any]]) -> Dict[str, Any]:
+        """the fit request up to the uplink fields: the fp32 model, unless ``downlink`` (the compressed downlink's fields,
+        :meth:`Coordinator._downlink_fields`) replaces it by a wire to the device's replica"""
+        req: Dict[str, Any] = {"op": "fit", "config": cfg.to_dict()}
+        if downlink is None or "replica_base" not in downlink:
+            req["params"] = _to_bytes(flat)
+        req["dataset_key"] = dataset_key
+        return req
+
     def fit_quantized(self, flat: torch.Tensor, cfg: FitConfig, codec: UplinkCodec, dataset_key: str = "training",
-                      timeout: Optional[float] = None) -> Tuple[Dict[str, Any], float, int]:
+                      timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None) -> Tuple[Dict[str, Any], float, int]:
         """:meth:`fit` asking the device for its quantized delta (``codec``): returns the reply's ``{"uplink", "payload",
-        "scales"}`` unchecked (it is untrusted input: the coordinator validates it), the loss and the sample count."""
-        resp = self._call({"op": "fit", "config": cfg.to_dict(), "params": _to_bytes(flat), "dataset_key": dataset_key,
-                           "uplink": codec.kind}, timeout=timeout)
+        "scales"}`` (and ``"replica_crc"`` with a ``downlink``) unchecked (it is untrusted input: the coordinator validates
+        it), the loss and the sample count."""
+        req = self._fit_request(flat, cfg, dataset_key, downlink)
+        req["uplink"] = codec.kind
+        resp = self._call({**req, **(downlink or {})}, timeout=timeout)
         self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None
         update = {"uplink": resp.get("uplink"), "payload": resp.get("payload"), "scales": resp.get("scales")}
+        if downlink is not None:
+            update["replica_crc"] = resp.get("replica_crc")
         return update, float(resp["loss"]), int(resp["n"])
 
     def fit_topk(self, flat: torch.Tensor, cfg: FitConfig, codec: UplinkCodec, ef_reset: bool, dataset_key: str = "training",
-                 timeout: Optional[float] = None) -> Tuple[Dict[str, Any], float, int]:
+                 timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None) -> Tuple[Dict[str, Any], float, int]:
         """:meth:`fit` asking the device for the top-k entries of its delta plus residual (``codec``), after zeroing that
-        residual if ``ef_reset``: returns the reply's ``{"uplink", "topk", "indices", "values"}`` unchecked (it is untrusted
-        input: the coordinator validates it), the loss and the sample count."""
-        resp = self._call({"op": "fit", "config": cfg.to_dict(), "params": _to_bytes(flat), "dataset_key": dataset_key,
-                           "uplink": codec.kind, "topk": codec.k, "ef_reset": bool(ef_reset)}, timeout=timeout)
+        residual if ``ef_reset``: returns the reply's ``{"uplink", "topk", "indices", "values"}`` (and ``"replica_crc"`` with a
+        ``downlink``) unchecked (it is untrusted input: the coordinator validates it), the loss and the sample count."""
+        req = self._fit_request(flat, cfg, dataset_key, downlink)
+        req.update({"uplink": codec.kind, "topk": codec.k, "ef_reset": bool(ef_reset)})
+        resp = self._call({**req, **(downlink or {})}, timeout=timeout)
         self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None
         update = {k: resp.get(k) for k in ("uplink", "topk", "indices", "values")}
+        if downlink is not None:
+            update["replica_crc"] = resp.get("replica_crc")
         return update, float(resp["loss"]), int(resp["n"])
 
     def search(self, tag: str) -> int:

@@ -27,16 +27,24 @@ dropped, only delayed.  The selection is deterministic (ties go to the lower ind
 are no scales and no keys.  Defined in ``ops/csrc/uplink_topk.cuh``; ``ops.reference.encode_topk_delta`` /
 ``decode_topk_delta`` transcribe it.  The residuals live in memory only, like the server optimizer state.
 
-The coordinator decodes against the ``theta`` it sent; the downlink stays fp32.
+The coordinator decodes against the model it sent.
+
+Downlink: the same codecs compress what the coordinator sends.  Coordinator and devices keep a replica ``r`` of the model
+the devices hold; round 0 of a training sends the global model as fp32 (``r = theta``), every later round encodes ``theta -
+r`` once (int8 / int4 rounded with :func:`downlink_key`, or its top-k entries), broadcasts the same bytes to every device, and
+both sides advance ``r`` by what was sent, bit for bit alike.  Devices train from ``r`` and send their deltas to ``r``; what
+was not delivered yet stays in ``theta - r`` and goes out in later rounds.  Defined in ``ops/csrc/downlink.cuh``;
+``ops.reference.encode_downlink`` / ``apply_downlink`` transcribe it.
 """
 from __future__ import annotations
 
 import math
 import zlib
 from dataclasses import dataclass
-from typing import ClassVar
+from typing import Any, ClassVar, Dict
 
 import numpy as np
+import torch
 
 KINDS = {"fp32": 32, "int8": 8, "int4": 4, "topk": 32}    # bits of one value on the wire
 LEVELS = {"fp32": 0, "int8": 127, "int4": 7, "topk": 0}
@@ -46,6 +54,11 @@ TOPK_MAX = 32                     # entries per 256-element block: one per lane 
 def uplink_key(worker_id: str, seed: int) -> int:
     """The uint32 key of a device's rounding noise for one fit."""
     return zlib.crc32(f"{worker_id}:{int(seed)}".encode())
+
+
+def downlink_key(seed: int) -> int:
+    """The uint32 key of the downlink's rounding noise for the round of ``seed``: one broadcast, so every device shares it."""
+    return zlib.crc32(f"downlink:{int(seed)}".encode())
 
 
 @dataclass(frozen=True)
@@ -113,3 +126,46 @@ class UplinkCodec:
             while not np.isfinite(L * x):
                 x = np.nextafter(x, np.float32(0.0))
         return float(x)
+
+
+# ---- checks of untrusted wire bytes: a device's reply on the coordinator, the coordinator's downlink on a device ----------------
+def check_quantized_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
+    """``(payload uint8 [codec.payload_bytes(p)], scales fp32 [codec.scale_count(p)])`` of a device's quantized reply, or
+    ValueError.  A reply is untrusted input: it must echo the codec asked for, carry exactly the bytes the codec defines for
+    ``p`` parameters, and only finite scales with ``|step| <= codec.max_scale`` (no decoded value can overflow)."""
+    if update.get("uplink") != codec.kind:
+        raise ValueError(f"uplink {update.get('uplink')!r} returned, {codec.kind!r} asked for")
+    payload, scales = update.get("payload"), update.get("scales")
+    if not isinstance(payload, bytes) or len(payload) != codec.payload_bytes(p):
+        raise ValueError(f"payload of {len(payload) if isinstance(payload, bytes) else None} bytes, expected {codec.payload_bytes(p)}")
+    if not isinstance(scales, bytes) or len(scales) != 4 * codec.scale_count(p):
+        raise ValueError(f"{len(scales) // 4 if isinstance(scales, bytes) else None} scales, expected {codec.scale_count(p)}")
+    s = torch.from_numpy(np.frombuffer(scales, dtype="<f4").copy())
+    if not bool(torch.isfinite(s).all()) or float(s.abs().max()) > codec.max_scale:
+        raise ValueError("non-finite or oversize block scale returned")
+    return torch.from_numpy(np.frombuffer(payload, dtype=np.uint8).copy()), s
+
+
+def check_topk_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
+    """``(indices uint8 [codec.entries(p)], values fp32 [codec.entries(p)])`` of a device's top-k reply, or ValueError.  A
+    reply is untrusted input: it must echo the codec and ``k`` asked for, carry exactly ``codec.entries(p)`` offsets and
+    values, offsets strictly ascending inside each block and below the block's length (so the decode sees each coordinate
+    at most once per device), and only finite values."""
+    if update.get("uplink") != codec.kind or type(update.get("topk")) is not int or update.get("topk") != codec.k:
+        raise ValueError(f"uplink {update.get('uplink')!r} / topk {update.get('topk')!r} returned, {codec.kind!r} / {codec.k} asked for")
+    e = codec.entries(p)
+    indices, values = update.get("indices"), update.get("values")
+    if not isinstance(indices, bytes) or len(indices) != e:
+        raise ValueError(f"{len(indices) if isinstance(indices, bytes) else None} offsets returned, expected {e}")
+    if not isinstance(values, bytes) or len(values) != 4 * e:
+        raise ValueError(f"{len(values) // 4 if isinstance(values, bytes) else None} values returned, expected {e}")
+    idx = np.frombuffer(indices, dtype=np.uint8).astype(np.int64)
+    blk = np.arange(e) // codec.k
+    if (idx >= np.minimum(codec.BLOCK, p - blk * codec.BLOCK)).any():
+        raise ValueError("offset past the end of its block returned")
+    if ((idx[1:] <= idx[:-1]) & (blk[1:] == blk[:-1])).any():
+        raise ValueError("offsets not strictly ascending inside a block returned")
+    v = torch.from_numpy(np.frombuffer(values, dtype="<f4").copy())
+    if not bool(torch.isfinite(v).all()):
+        raise ValueError("non-finite value returned")
+    return torch.from_numpy(idx.astype(np.uint8)), v

@@ -166,6 +166,45 @@ def fedavg_apply_topk(theta: torch.Tensor, indices: torch.Tensor, values: torch.
     return reference.fedavg_apply_topk(theta, indices, values, weights, codec.k, server_lr, opt=opt)
 
 
+def encode_downlink(theta: torch.Tensor, replica: torch.Tensor, codec, key: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The coordinator's downlink (``ops/csrc/downlink.cuh``): the wire of ``theta [P] - replica [P]`` with the
+    :class:`fl.uplink.UplinkCodec` ``codec``, and ``replica`` (contiguous fp32) advanced in place by what it carries.  int8 /
+    int4: ``(payload uint8 [codec.payload_bytes(P)], scales fp32 [codec.scale_count(P)])`` rounded with the uint32 ``key``;
+    topk: ``(indices uint8 [E], values fp32 [E])``.  CUDA tensors: ``downlink_quant_kernel`` / ``downlink_topk_kernel`` in one
+    launch; CPU tensors: ``reference.encode_downlink``."""
+    if not (codec.quantized or codec.sparse):
+        raise ValueError("encode_downlink needs an int8 / int4 / topk codec")
+    if replica.dtype != torch.float32 or not replica.is_contiguous() or replica.numel() != theta.numel():
+        raise ValueError("the replica must be a contiguous float32 tensor of theta's size (it is updated in place)")
+    if _cuda(replica):
+        th = theta.to(replica.device, torch.float32).contiguous().view(-1)
+        if codec.quantized:
+            payload, scales = _ext.require().downlink_quant(th, replica.view(-1), int(key) & 0xFFFFFFFF, codec.bits)
+            return payload[:codec.payload_bytes(theta.numel())], scales
+        return tuple(_ext.require().downlink_topk(th, replica.view(-1), codec.k))
+    return reference.encode_downlink(theta, replica, codec, key)
+
+
+def apply_downlink(replica: torch.Tensor, a: torch.Tensor, b: torch.Tensor, codec) -> torch.Tensor:
+    """A device's side of the downlink: ``replica`` (contiguous fp32) advanced in place by a wire ``(a, b)`` that passed the
+    reply checks (``(payload, scales)`` for int8 / int4, ``(indices, values)`` for topk).  CUDA tensors:
+    ``replica_apply_q_kernel`` / ``replica_apply_topk_kernel``; CPU tensors: ``reference.apply_downlink``."""
+    if not (codec.quantized or codec.sparse):
+        raise ValueError("apply_downlink needs an int8 / int4 / topk codec")
+    if replica.dtype != torch.float32 or not replica.is_contiguous():
+        raise ValueError("the replica must be a contiguous float32 tensor (it is updated in place)")
+    if _cuda(replica):
+        dev = replica.device
+        if codec.quantized:
+            payload = _aligned_rows(a.to(dev, torch.uint8).reshape(1, -1)).reshape(-1)
+            _ext.require().replica_apply_quant(replica.view(-1), payload, b.to(dev, torch.float32).contiguous(), codec.bits)
+        else:
+            _ext.require().replica_apply_topk(replica.view(-1), a.to(dev, torch.uint8).contiguous(), b.to(dev, torch.float32).contiguous(),
+                                              codec.k)
+        return replica
+    return reference.apply_downlink(replica, a, b, codec)
+
+
 def sigmoid_bce(z: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """(mean BCE(sigmoid(z), y), dL/dz) in one pass (SURVEY K9)."""
     if _cuda(z):

@@ -251,6 +251,64 @@ void fedavg_apply_topk(torch::Tensor theta, torch::Tensor indices, torch::Tensor
                                  weights.data_ptr<float>(), (int)k, (int)topk, o, n, cur_stream()), "fedavg_apply_topk");
 }
 
+// ---- compressed downlink (downlink.cuh) -----------------------------------------------------------------------------------------
+// (payload uint8 [row_bytes], scales fp32 [ceil(P / 256)]) of theta [P] - replica [P] rounded with key (uint32 bits in an int64),
+// row_bytes as in quantize_delta; replica advanced in place by the decoded codes
+std::vector<torch::Tensor> downlink_quant(torch::Tensor theta, torch::Tensor replica, int64_t key, int64_t bits) {
+  CHECK_CUDA_F32(theta); CHECK_CUDA_F32(replica);
+  TORCH_CHECK(replica.numel() == theta.numel() && replica.device() == theta.device(), "theta / replica [P], one device");
+  TORCH_CHECK(bits == 8 || bits == 4, "bits must be 8 or 4");
+  c10::cuda::CUDAGuard guard(theta.device());
+  const int64_t n = theta.numel();
+  const int64_t row = ((bits == 8 ? n : (n + 1) / 2) + 15) / 16 * 16;
+  auto payload = torch::empty({row}, theta.options().dtype(at::kByte));
+  auto scales = torch::empty({(n + kUqBlock - 1) / kUqBlock}, theta.options());
+  check(launch_downlink_quant(theta.data_ptr<float>(), replica.data_ptr<float>(), (uint32_t)key, (int)bits, payload.data_ptr<uint8_t>(), row,
+                              scales.data_ptr<float>(), n, cur_stream()), "downlink_quant");
+  return {payload, scales};
+}
+
+// (indices uint8 [E], values fp32 [E]) of v = theta [P] - replica [P], E = ut_entries(P, topk); the sent entries added into replica
+std::vector<torch::Tensor> downlink_topk(torch::Tensor theta, torch::Tensor replica, int64_t topk) {
+  CHECK_CUDA_F32(theta); CHECK_CUDA_F32(replica);
+  TORCH_CHECK(replica.numel() == theta.numel() && replica.device() == theta.device(), "theta / replica [P], one device");
+  TORCH_CHECK(topk >= 1 && topk <= kUtMaxK, "topk must be in 1..32");
+  c10::cuda::CUDAGuard guard(theta.device());
+  const int64_t n = theta.numel(), e = ut_entries(n, (int)topk);
+  auto indices = torch::empty({e}, theta.options().dtype(at::kByte));
+  auto values = torch::empty({e}, theta.options());
+  check(launch_downlink_topk(theta.data_ptr<float>(), replica.data_ptr<float>(), (int)topk, indices.data_ptr<uint8_t>(),
+                             values.data_ptr<float>(), n, cur_stream()), "downlink_topk");
+  return {indices, values};
+}
+
+// replica [P] += the decoded int8 / int4 wire (payload uint8, 16-byte aligned, a multiple of 16 bytes covering the codes;
+// scales fp32 [ceil(P / 256)], validated by the caller)
+void replica_apply_quant(torch::Tensor replica, torch::Tensor payload, torch::Tensor scales, int64_t bits) {
+  CHECK_CUDA_F32(replica); CHECK_CUDA_F32(scales);
+  const int64_t n = replica.numel();
+  TORCH_CHECK(payload.is_cuda() && payload.scalar_type() == at::kByte && payload.dim() == 1 && payload.is_contiguous() &&
+              payload.device() == replica.device(), "payload: contiguous CUDA uint8 [row_bytes] on the replica's device");
+  TORCH_CHECK(scales.numel() == (n + kUqBlock - 1) / kUqBlock && scales.device() == replica.device(), "scales [ceil(P / 256)]");
+  c10::cuda::CUDAGuard guard(replica.device());
+  check(launch_replica_apply_quant(replica.data_ptr<float>(), payload.data_ptr<uint8_t>(), payload.numel(), scales.data_ptr<float>(),
+                                   (int)bits, n, cur_stream()), "replica_apply_quant");
+}
+
+// replica [P] += the top-k wire (indices uint8 / values fp32 [E(P, topk)], offsets validated by the caller)
+void replica_apply_topk(torch::Tensor replica, torch::Tensor indices, torch::Tensor values, int64_t topk) {
+  CHECK_CUDA_F32(replica); CHECK_CUDA_F32(values);
+  const int64_t n = replica.numel();
+  TORCH_CHECK(topk >= 1 && topk <= kUtMaxK, "topk must be in 1..32");
+  TORCH_CHECK(indices.is_cuda() && indices.scalar_type() == at::kByte && indices.is_contiguous() &&
+              indices.numel() == ut_entries(n, (int)topk) && values.numel() == indices.numel() &&
+              indices.device() == replica.device() && values.device() == replica.device(),
+              "indices / values [E(P, topk)] on the replica's device");
+  c10::cuda::CUDAGuard guard(replica.device());
+  check(launch_replica_apply_topk(replica.data_ptr<float>(), indices.data_ptr<uint8_t>(), values.data_ptr<float>(), (int)topk, n,
+                                  cur_stream()), "replica_apply_topk");
+}
+
 torch::Tensor fedavg_flat(torch::Tensor slots, torch::Tensor weights) {
   CHECK_CUDA_F32(slots); CHECK_CUDA_F32(weights);
   TORCH_CHECK(slots.dim() == 2 && weights.numel() == slots.size(0), "shapes");
@@ -744,6 +802,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("weights"),
         py::arg("topk"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
         py::arg("m") = py::none(), py::arg("v") = py::none());
+  m.def("downlink_quant", &downlink_quant);
+  m.def("downlink_topk", &downlink_topk);
+  m.def("replica_apply_quant", &replica_apply_quant);
+  m.def("replica_apply_topk", &replica_apply_topk);
   m.def("quantize_delta", &quantize_delta);
   m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("weights"),
         py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},

@@ -45,6 +45,8 @@
 #include "uplink_quant.cuh"
 // top-k sparsified uplink with error feedback shared by the encode and the sparse FedAvg kernels
 #include "uplink_topk.cuh"
+// replica protocol of the compressed downlink (the same two codecs on theta - replica)
+#include "downlink.cuh"
 
 namespace colearn {
 // Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
@@ -259,6 +261,16 @@ cudaError_t launch_topk_delta(const float* models, int64_t model_stride, const f
 // (opt.kind 0) or the server optimizer step; the offsets of a block of a row must be distinct
 cudaError_t launch_fedavg_apply_topk(float* theta, const uint8_t* indices, const float* values, int64_t entries, const float* weights,
                                      int rows, int topk, const ServerOptArgs& opt, int64_t n, cudaStream_t s);
+// Compressed downlink (downlink.cuh), one row.  Coordinator: the int8 / int4 codes (payload, row_bytes as in
+// launch_quantize_delta) and block steps of theta - replica rounded with `key`, or its top-k entries (indices / values
+// [ut_entries(n, topk)]), and replica advanced in place by what was sent.  Device: replica advanced in place by such a wire
+// (already validated: finite steps, offsets inside their block).
+cudaError_t launch_downlink_quant(const float* theta, float* replica, uint32_t key, int bits, uint8_t* payload, int64_t row_bytes,
+                                  float* scales, int64_t n, cudaStream_t s);
+cudaError_t launch_downlink_topk(const float* theta, float* replica, int topk, uint8_t* indices, float* values, int64_t n, cudaStream_t s);
+cudaError_t launch_replica_apply_quant(float* replica, const uint8_t* payload, int64_t row_bytes, const float* scales, int bits,
+                                       int64_t n, cudaStream_t s);
+cudaError_t launch_replica_apply_topk(float* replica, const uint8_t* indices, const float* values, int topk, int64_t n, cudaStream_t s);
 // out = sum_k w[k] * slots[k]
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride,
                                const float* weights, int k, int64_t n, cudaStream_t s);

@@ -399,12 +399,51 @@ __device__ __forceinline__ int warp_exclusive_prefix4(int x, uint32_t lower_lane
   return s;
 }
 
+// The selection of one 256-element block by its warp, lane l holding the keys of elements 8 l .. 8 l + 7: the warp finds the
+// k_b-th greatest key T bit by bit from the top (31 rounds of one __reduce_add_sync: the largest T with #{key >= T} >= k_b),
+// keeps every key > T and the lowest-index keys == T up to k_b (a ballot prefix of the per-lane tie counts).  keep[i] flags
+// this lane's kept elements, `first` is the lane's first entry in the block (the exclusive prefix of the per-lane kept
+// counts), so that the kept entries land in index order.  Keys in and flags out by value: passed by reference, the routine
+// changed the register allocation of topk_delta_kernel.
+struct TopkKeys8 { uint32_t key[8]; };
+struct TopkSel8 { bool keep[8]; int first; };
+__device__ __forceinline__ TopkSel8 warp_topk_select(TopkKeys8 keys, int kb, uint32_t lower_lanes) {
+  const uint32_t* key = keys.key;
+  TopkSel8 sel;
+  uint32_t thr = 0;
+  for (int b = 30; b >= 0; --b) {                   // keys are below 2^31
+    const uint32_t cand = thr | (1u << b);
+    int cnt = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) cnt += key[i] >= cand ? 1 : 0;
+    if (__reduce_add_sync(0xffffffffu, cnt) >= kb) thr = cand;
+  }
+  int ngt = 0, ntie = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    ngt += key[i] > thr ? 1 : 0;
+    ntie += key[i] == thr ? 1 : 0;
+  }
+  // ties this lane may keep: the kb - #{key > thr} >= 1 lowest-index ties of the block, minus those of the lower lanes
+  const int room = kb - __reduce_add_sync(0xffffffffu, ngt) - warp_exclusive_prefix4(ntie, lower_lanes);
+  // per-element flags, not a bit mask: a `keep |= 1u << i` form of this selection lost element 1's tie on the H100
+  // (sm_90a, CUDA 12.9) while its PTX and the SIMT build were right
+  int nkeep = 0, seen = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const bool tie = key[i] == thr;
+    sel.keep[i] = key[i] > thr || (tie && seen < room);
+    seen += tie ? 1 : 0;
+    nkeep += sel.keep[i] ? 1 : 0;
+  }
+  sel.first = warp_exclusive_prefix4(nkeep, lower_lanes);
+  return sel;
+}
+
 // Encode: one warp per (row, 256-element block); lane l holds elements 8 l .. 8 l + 7 of the block (16-byte loads of the
-// model, theta and the residual when rows are 16-byte aligned, scalar loads with the same bits otherwise).  The warp finds
-// the k_b-th greatest key T bit by bit from the top (31 rounds of one __reduce_add_sync: the largest T with
-// #{key >= T} >= k_b), keeps every key > T and the lowest-index keys == T up to k_b (a ballot prefix of the per-lane tie
-// counts), and stores the kept entries in index order at the exclusive prefix of the per-lane kept counts.  The residual is
-// written back in place.  Elements past n take key 0: they lose every tie to the block's own elements, and k_b <= m_b.
+// model, theta and the residual when rows are 16-byte aligned, scalar loads with the same bits otherwise).  warp_topk_select
+// picks the entries, which are stored in index order; the residual is written back in place.  Elements past n take key 0:
+// they lose every tie to the block's own elements, and k_b <= m_b.
 __global__ void __launch_bounds__(256)
 topk_delta_kernel(const float* __restrict__ models, int64_t model_stride, const float* __restrict__ theta, float* __restrict__ residual,
                   int64_t residual_stride, int k, int topk, uint8_t* __restrict__ indices, float* __restrict__ values, int64_t entries,
@@ -441,38 +480,12 @@ topk_delta_kernel(const float* __restrict__ models, int64_t model_stride, const 
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = (e0 + i < n) ? (row[e0 + i] - theta[e0 + i]) + res[e0 + i] : 0.f;
     }
-    uint32_t key[8];
+    TopkKeys8 keys;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) key[i] = (e0 + i < n) ? ut_key(v[i]) : 0u;
-    const int kb = ut_block_k(n, blk, topk);
-    uint32_t thr = 0;
-    for (int b = 30; b >= 0; --b) {                   // keys are below 2^31
-      const uint32_t cand = thr | (1u << b);
-      int cnt = 0;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) cnt += key[i] >= cand ? 1 : 0;
-      if (__reduce_add_sync(0xffffffffu, cnt) >= kb) thr = cand;
-    }
-    int ngt = 0, ntie = 0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      ngt += key[i] > thr ? 1 : 0;
-      ntie += key[i] == thr ? 1 : 0;
-    }
-    // ties this lane may keep: the kb - #{key > thr} >= 1 lowest-index ties of the block, minus those of the lower lanes
-    const int room = kb - __reduce_add_sync(0xffffffffu, ngt) - warp_exclusive_prefix4(ntie, lower_lanes);
-    // per-element flags, not a bit mask: a `keep |= 1u << i` form of this selection lost element 1's tie on the H100
-    // (sm_90a, CUDA 12.9) while its PTX and the SIMT build were right
-    bool keep[8];
-    int nkeep = 0, seen = 0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const bool tie = key[i] == thr;
-      keep[i] = key[i] > thr || (tie && seen < room);
-      seen += tie ? 1 : 0;
-      nkeep += keep[i] ? 1 : 0;
-    }
-    const int64_t out = c * entries + blk * topk + warp_exclusive_prefix4(nkeep, lower_lanes);
+    for (int i = 0; i < 8; ++i) keys.key[i] = (e0 + i < n) ? ut_key(v[i]) : 0u;
+    const TopkSel8 sel = warp_topk_select(keys, ut_block_k(n, blk, topk), lower_lanes);
+    const bool* keep = sel.keep;
+    const int64_t out = c * entries + blk * topk + sel.first;
     int o = 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -577,6 +590,200 @@ fedavg_topk_kernel(float* __restrict__ theta, const uint8_t* __restrict__ indice
         }
       }
     }
+  }
+}
+
+// ---- compressed downlink (downlink.cuh) ---------------------------------------------------------------------------------------
+// lane l's 8 elements 8 l .. 8 l + 7 of theta and of the replica (two 16-byte loads each when vec, scalar loads with the same
+// bits otherwise; 0 past n)
+__device__ __forceinline__ void dl_load8(const float* __restrict__ theta, const float* __restrict__ replica, int64_t e0, int64_t n,
+                                         bool vec, float (&t)[8], float (&r)[8]) {
+  if (vec) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t e = e0 + 4 * h;
+      float4 th = make_float4(0.f, 0.f, 0.f, 0.f), rp = th;
+      if (e < n) {
+        th = __ldg(reinterpret_cast<const float4*>(theta + e));
+        rp = *reinterpret_cast<const float4*>(replica + e);
+      }
+      t[4 * h + 0] = th.x; t[4 * h + 1] = th.y; t[4 * h + 2] = th.z; t[4 * h + 3] = th.w;
+      r[4 * h + 0] = rp.x; r[4 * h + 1] = rp.y; r[4 * h + 2] = rp.z; r[4 * h + 3] = rp.w;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      t[i] = e0 + i < n ? theta[e0 + i] : 0.f;
+      r[i] = e0 + i < n ? replica[e0 + i] : 0.f;
+    }
+  }
+}
+
+// lane l's 8 replica elements back (16-byte stores where the 4 are inside n and vec, scalar stores otherwise)
+__device__ __forceinline__ void dl_store8(float* __restrict__ replica, int64_t e0, int64_t n, bool vec, const float (&r)[8]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t e = e0 + 4 * h;
+    if (vec && e + 4 <= n) {
+      *reinterpret_cast<float4*>(replica + e) = make_float4(r[4 * h], r[4 * h + 1], r[4 * h + 2], r[4 * h + 3]);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if (e + i < n) replica[e + i] = r[4 * h + i];
+      }
+    }
+  }
+}
+
+// Coordinator, int8 / int4: quantize_delta_kernel's shape on d = theta - replica for one row (one warp per 256-element block,
+// block max by shuffles, 8 codes per lane in one store, lane 0 the step), and the replica advanced in the same pass.
+template <int BITS>
+__global__ void __launch_bounds__(256)
+downlink_quant_kernel(const float* __restrict__ theta, float* __restrict__ replica, uint32_t key, uint8_t* __restrict__ payload,
+                      float* __restrict__ scales, int64_t n) {
+  constexpr int L = UqCodec<BITS>::kLevels;
+  const int lane = threadIdx.x & 31;
+  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const bool vec = (((uintptr_t)theta | (uintptr_t)replica) & 15) == 0 && (n & 3) == 0;
+  for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
+    const int64_t e0 = blk * kUqBlock + lane * 8;
+    float t[8], r[8], d[8];
+    dl_load8(theta, replica, e0, n, vec, t, r);
+    uint32_t amax = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      d[i] = t[i] - r[i];
+      const uint32_t a = uq_abs_bits(d[i]);
+      amax = a > amax ? a : amax;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const uint32_t a = __shfl_xor_sync(0xffffffffu, amax, o);
+      amax = a > amax ? a : amax;
+    }
+    float step, inv;
+    uq_block_scale(amax, L, step, inv);
+    if (e0 < n) {
+      int q[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        q[i] = uq_encode(d[i], inv, key, (uint32_t)(e0 + i), L);
+        r[i] = dl_quant_advance(r[i], q[i], step);
+      }
+      if constexpr (BITS == 8) {
+        uint2 w = make_uint2(0u, 0u);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          w.x |= ((uint32_t)q[i] & 0xffu) << (8 * i);
+          w.y |= ((uint32_t)q[4 + i] & 0xffu) << (8 * i);
+        }
+        *reinterpret_cast<uint2*>(payload + e0) = w;
+      } else {
+        uint32_t w = 0u;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) w |= ((uint32_t)q[i] & 0xfu) << (4 * i);
+        *reinterpret_cast<uint32_t*>(payload + (e0 >> 1)) = w;
+      }
+      dl_store8(replica, e0, n, vec, r);
+    }
+    if (lane == 0) scales[blk] = step;
+  }
+}
+
+// Coordinator, topk: the selection of topk_delta_kernel (warp_topk_select) on v = theta - replica with no residual; the kept
+// entries are stored in index order and added into the replica (scalar stores of the kept elements only).
+__global__ void __launch_bounds__(256)
+downlink_topk_kernel(const float* __restrict__ theta, float* __restrict__ replica, int topk, uint8_t* __restrict__ indices,
+                     float* __restrict__ values, int64_t n) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t lower_lanes = (1u << lane) - 1u;
+  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const bool vec = (((uintptr_t)theta | (uintptr_t)replica) & 15) == 0 && (n & 3) == 0;
+  for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
+    const int64_t e0 = blk * kUqBlock + lane * 8;
+    float t[8], r[8], v[8];
+    dl_load8(theta, replica, e0, n, vec, t, r);
+    TopkKeys8 keys;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      v[i] = t[i] - r[i];
+      keys.key[i] = (e0 + i < n) ? ut_key(v[i]) : 0u;
+    }
+    const TopkSel8 sel = warp_topk_select(keys, ut_block_k(n, blk, topk), lower_lanes);
+    const bool* keep = sel.keep;
+    const int64_t out = blk * topk + sel.first;
+    int o = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      if (keep[i]) {
+        indices[out + o] = (uint8_t)(lane * 8 + i);
+        values[out + o] = v[i];
+        replica[e0 + i] = dl_add_rn(r[i], v[i]);
+        ++o;
+      }
+    }
+  }
+}
+
+// Device, int8 / int4: replica += decode(wire), one warp per 256-element block, 8 elements per lane: one 8-byte (int8) or
+// 4-byte (int4) load of codes, 16-byte loads / stores of the replica where aligned.
+template <int BITS>
+__global__ void __launch_bounds__(256)
+replica_apply_q_kernel(float* __restrict__ replica, const uint8_t* __restrict__ payload, const float* __restrict__ scales, int64_t n) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const bool vec = ((uintptr_t)replica & 15) == 0;
+  for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
+    const int64_t e0 = blk * kUqBlock + lane * 8;
+    if (e0 >= n) continue;
+    const float step = __ldg(scales + blk);
+    int q[8];
+    if constexpr (BITS == 8) {
+      const uint2 w = __ldg(reinterpret_cast<const uint2*>(payload + e0));
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        q[i] = (int)(int8_t)(w.x >> (8 * i));
+        q[4 + i] = (int)(int8_t)(w.y >> (8 * i));
+      }
+    } else {
+      const uint32_t w = __ldg(reinterpret_cast<const unsigned int*>(payload + (e0 >> 1)));
+#pragma unroll
+      for (int i = 0; i < 8; ++i) q[i] = uq_nibble(w, i);
+    }
+    float r[8];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t e = e0 + 4 * h;
+      if (vec && e + 4 <= n) {
+        const float4 rp = *reinterpret_cast<const float4*>(replica + e);
+        r[4 * h + 0] = rp.x; r[4 * h + 1] = rp.y; r[4 * h + 2] = rp.z; r[4 * h + 3] = rp.w;
+      } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) r[4 * h + i] = e + i < n ? replica[e + i] : 0.f;
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) r[i] = dl_quant_advance(r[i], q[i], step);
+    dl_store8(replica, e0, n, vec, r);
+  }
+}
+
+// Device, topk: replica[j] += value for every entry, one warp per 256-element block, lane c < k_b taking entry c of the block
+// (a block's offsets are distinct: no two lanes touch one element).  Offsets past n are skipped.
+__global__ void __launch_bounds__(256)
+replica_apply_topk_kernel(float* __restrict__ replica, const uint8_t* __restrict__ indices, const float* __restrict__ values, int topk,
+                          int64_t n) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
+    if (lane >= ut_block_k(n, blk, topk)) continue;
+    const int64_t slot = blk * topk + lane;
+    const int64_t j = blk * kUqBlock + __ldg(indices + slot);
+    if (j < n) replica[j] = dl_add_rn(replica[j], __ldg(values + slot));
   }
 }
 
@@ -1004,6 +1211,32 @@ cudaError_t launch_fedavg_apply_topk(float* theta, const uint8_t* indices, const
   } else {
     COLEARN_LAUNCH(fedavg_topk_kernel<true>, grid, kThreads, 0, s, theta, indices, values, entries, weights, rows, topk, opt, n);
   }
+  return cudaGetLastError();
+}
+cudaError_t launch_downlink_quant(const float* theta, float* replica, uint32_t key, int bits, uint8_t* payload, int64_t row_bytes,
+                                  float* scales, int64_t n, cudaStream_t s) {
+  if (!uq_layout_ok(bits, payload, row_bytes, n)) return cudaErrorInvalidValue;
+  auto kernel = bits == 8 ? downlink_quant_kernel<8> : downlink_quant_kernel<4>;
+  COLEARN_LAUNCH(kernel, grid_for_warps((n + kUqBlock - 1) / kUqBlock), kThreads, 0, s, theta, replica, key, payload, scales, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_downlink_topk(const float* theta, float* replica, int topk, uint8_t* indices, float* values, int64_t n, cudaStream_t s) {
+  if (topk < 1 || topk > kUtMaxK || n < 1) return cudaErrorInvalidValue;
+  COLEARN_LAUNCH(downlink_topk_kernel, grid_for_warps((n + kUqBlock - 1) / kUqBlock), kThreads, 0, s, theta, replica, topk, indices,
+                 values, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_replica_apply_quant(float* replica, const uint8_t* payload, int64_t row_bytes, const float* scales, int bits,
+                                       int64_t n, cudaStream_t s) {
+  if (!uq_layout_ok(bits, payload, row_bytes, n)) return cudaErrorInvalidValue;
+  auto kernel = bits == 8 ? replica_apply_q_kernel<8> : replica_apply_q_kernel<4>;
+  COLEARN_LAUNCH(kernel, grid_for_warps((n + kUqBlock - 1) / kUqBlock), kThreads, 0, s, replica, payload, scales, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_replica_apply_topk(float* replica, const uint8_t* indices, const float* values, int topk, int64_t n, cudaStream_t s) {
+  if (topk < 1 || topk > kUtMaxK || n < 1) return cudaErrorInvalidValue;
+  COLEARN_LAUNCH(replica_apply_topk_kernel, grid_for_warps((n + kUqBlock - 1) / kUqBlock), kThreads, 0, s, replica, indices, values,
+                 topk, n);
   return cudaGetLastError();
 }
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride, const float* weights,

@@ -193,6 +193,50 @@ void fedavg_apply_topk(Tensor theta, Tensor indices, Tensor values, Tensor w, in
   CK(colearn::launch_fedavg_apply_topk(fmut(theta, "theta"), indices.data_ptr<uint8_t>(), fptr(values, "values"), indices.size(1),
                                        fptr(w, "w"), (int)k, (int)topk, o, n, nullptr));
 }
+// compressed downlink (downlink.cuh): same shapes and padding as bindings.cpp::downlink_quant / downlink_topk /
+// replica_apply_quant / replica_apply_topk; the replica [P] is advanced in place
+std::tuple<Tensor, Tensor> downlink_quant(Tensor theta, Tensor replica, int64_t key, int64_t bits) {
+  TORCH_CHECK(replica.numel() == theta.numel(), "theta / replica [P]");
+  const int64_t n = theta.numel();
+  const int64_t row = ((bits == 8 ? n : (n + 1) / 2) + 15) / 16 * 16;
+  Tensor payload = torch::zeros({row}, torch::kUInt8), scales = torch::zeros({(n + 255) / 256}, torch::kFloat);
+  float* r = fmut(replica, "replica");
+  {
+    py::gil_scoped_release nogil;
+    CK(colearn::launch_downlink_quant(fptr(theta, "theta"), r, (uint32_t)key, (int)bits, payload.data_ptr<uint8_t>(), row,
+                                      scales.data_ptr<float>(), n, nullptr));
+  }
+  return {payload, scales};
+}
+std::tuple<Tensor, Tensor> downlink_topk(Tensor theta, Tensor replica, int64_t topk) {
+  TORCH_CHECK(replica.numel() == theta.numel(), "theta / replica [P]");
+  TORCH_CHECK(topk >= 1 && topk <= colearn::kUtMaxK, "topk must be in 1..32");
+  const int64_t n = theta.numel(), e = colearn::ut_entries(n, (int)topk);
+  Tensor indices = torch::zeros({e}, torch::kUInt8), values = torch::zeros({e}, torch::kFloat);
+  float* r = fmut(replica, "replica");
+  {
+    py::gil_scoped_release nogil;
+    CK(colearn::launch_downlink_topk(fptr(theta, "theta"), r, (int)topk, indices.data_ptr<uint8_t>(), values.data_ptr<float>(), n, nullptr));
+  }
+  return {indices, values};
+}
+void replica_apply_quant(Tensor replica, Tensor payload, Tensor scales, int64_t bits) {
+  TORCH_CHECK(!payload.is_cuda() && payload.scalar_type() == at::kByte && payload.dim() == 1 && payload.is_contiguous(), "payload uint8 [row]");
+  const int64_t n = replica.numel();
+  TORCH_CHECK(scales.numel() == (n + 255) / 256, "scales [ceil(P / 256)]");
+  float* r = fmut(replica, "replica");
+  py::gil_scoped_release nogil;
+  CK(colearn::launch_replica_apply_quant(r, payload.data_ptr<uint8_t>(), payload.numel(), fptr(scales, "scales"), (int)bits, n, nullptr));
+}
+void replica_apply_topk(Tensor replica, Tensor indices, Tensor values, int64_t topk) {
+  TORCH_CHECK(!indices.is_cuda() && indices.scalar_type() == at::kByte && indices.is_contiguous(), "indices uint8 [E]");
+  const int64_t n = replica.numel();
+  TORCH_CHECK(topk >= 1 && topk <= colearn::kUtMaxK && indices.numel() == colearn::ut_entries(n, (int)topk) &&
+              values.numel() == indices.numel(), "indices / values [E(P, topk)]");
+  float* r = fmut(replica, "replica");
+  py::gil_scoped_release nogil;
+  CK(colearn::launch_replica_apply_topk(r, indices.data_ptr<uint8_t>(), fptr(values, "values"), (int)topk, n, nullptr));
+}
 Tensor fedavg_flat(Tensor slots, Tensor w) {
   Tensor out = torch::zeros({slots.size(1)}, torch::kFloat);
   CK(colearn::launch_fedavg_flat(out.data_ptr<float>(), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0), slots.size(1), nullptr));
@@ -494,6 +538,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("w"), py::arg("topk"),
         py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(),
         py::arg("v") = py::none());
+  m.def("downlink_quant", &downlink_quant);
+  m.def("downlink_topk", &downlink_topk);
+  m.def("replica_apply_quant", &replica_apply_quant);
+  m.def("replica_apply_topk", &replica_apply_topk);
   m.def("quantize_delta", &quantize_delta);
   m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("w"),
         py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},

@@ -106,6 +106,15 @@ int main() {
     memset(&ko, 0, sizeof(ko));
     ko.lr = 1.f;
     CK(launch_fedavg_apply_topk(qtheta.data(), kidx.data(), kvals.data(), 32, qw.data(), 3, 8, ko, qn, nullptr));
+    // compressed downlink: encode-and-advance of one replica (block max by shuffles / warp select, replica written in place),
+    // then the device-side apply of the same wire to a second replica, int8, int4 and topk k = 8, partial last block
+    std::vector<float> drep(qn, 0.f), dev_rep(qn, 0.f);
+    for (int bits : {8, 4}) {
+      CK(launch_downlink_quant(qtheta.data(), drep.data(), 7u, bits, qpayload, qrow, qscales.data(), qn, nullptr));
+      CK(launch_replica_apply_quant(dev_rep.data(), qpayload, qrow, qscales.data(), bits, qn, nullptr));
+    }
+    CK(launch_downlink_topk(qtheta.data(), drep.data(), 8, kidx.data(), kvals.data(), qn, nullptr));
+    CK(launch_replica_apply_topk(dev_rep.data(), kidx.data(), kvals.data(), 8, qn, nullptr));
   }
   printf("elementwise kernels ok\n");
   // ---- comm: star round (with deadline) and two-shot on 3 emulated ranks, reduce_push -------------------------------------------

@@ -381,10 +381,21 @@ def encode_topk_delta(models: torch.Tensor, theta: torch.Tensor, residual: torch
     m = models.detach().to("cpu", torch.float32).reshape(residual.shape).numpy()
     t = theta.detach().to("cpu", torch.float32).reshape(-1).numpy()
     e = residual.detach().to("cpu", torch.float32).numpy()
-    K, P = m.shape
-    nblk = (P + UQ_BLOCK - 1) // UQ_BLOCK
     with np.errstate(over="ignore", invalid="ignore"):
         v = (m - t[None, :]) + e
+    idx, pos = _topk_select(v, k)
+    values = np.take_along_axis(v, pos, axis=1)
+    rest = v.copy()
+    np.put_along_axis(rest, pos, np.float32(0.0), axis=1)
+    residual.copy_(torch.from_numpy(rest))
+    return torch.from_numpy(np.ascontiguousarray(idx.astype(np.uint8))), torch.from_numpy(np.ascontiguousarray(values))
+
+
+def _topk_select(v: np.ndarray, k: int) -> Tuple[np.ndarray, np.ndarray]:
+    """The wire offsets ``[K, E]`` of the top-``k`` selection of every 256-element block of float32 ``v [K, P]`` and their
+    positions in ``v`` (int64)."""
+    K, P = v.shape
+    nblk = (P + UQ_BLOCK - 1) // UQ_BLOCK
     # composite = key 256 + (255 - offset): unique inside a block, greater = kept first (the lower offset wins a tie);
     # elements past P get key -1 and are kept only in a last block shorter than k, where they are cut off below
     key = np.full((K, nblk * UQ_BLOCK), -1, dtype=np.int64)
@@ -393,12 +404,12 @@ def encode_topk_delta(models: torch.Tensor, theta: torch.Tensor, residual: torch
     top = -np.sort(-comp, axis=2)[:, :, :k]
     off = np.sort((UQ_BLOCK - 1) - (top & (UQ_BLOCK - 1)), axis=2)
     idx = off.reshape(K, nblk * k)[:, :topk_entries(P, k)]
-    pos = idx + (np.arange(idx.shape[1]) // k * UQ_BLOCK)[None, :]
-    values = np.take_along_axis(v, pos, axis=1)
-    rest = v.copy()
-    np.put_along_axis(rest, pos, np.float32(0.0), axis=1)
-    residual.copy_(torch.from_numpy(rest))
-    return torch.from_numpy(np.ascontiguousarray(idx.astype(np.uint8))), torch.from_numpy(np.ascontiguousarray(values))
+    return idx, _topk_positions(idx, k)
+
+
+def _topk_positions(idx: np.ndarray, k: int) -> np.ndarray:
+    """element positions (int64) of the wire offsets ``idx [K, E]``: block ``e // k`` of entry ``e``"""
+    return idx.astype(np.int64) + (np.arange(idx.shape[1]) // k * UQ_BLOCK)[None, :]
 
 
 def decode_topk_delta(indices: torch.Tensor, values: torch.Tensor, k: int, n: int) -> torch.Tensor:
@@ -420,6 +431,57 @@ def fedavg_apply_topk(theta: torch.Tensor, indices: torch.Tensor, values: torch.
         return theta.add_(server_lr * (avg - theta))
     b1, b2, tau = opt.hyper
     return server_opt_step(theta, avg, opt.kind, opt.lr, opt.m, opt.v, b1, b2, tau)
+
+
+# ------------------------------------------------------------------------------------------------
+# compressed downlink (ops/csrc/downlink.cuh; fl/uplink.py)
+# ------------------------------------------------------------------------------------------------
+def _replica_np(replica: torch.Tensor) -> np.ndarray:
+    if replica.dtype != torch.float32 or not replica.is_contiguous():
+        raise ValueError("the replica must be a contiguous float32 tensor (it is updated in place)")
+    return replica.detach().to("cpu").reshape(-1).numpy().copy()
+
+
+def encode_downlink(theta: torch.Tensor, replica: torch.Tensor, codec, key: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The downlink wire of ``theta [P] - replica [P]`` and ``replica`` advanced in place by what it carries: int8 / int4
+    ``(payload uint8 [codec.payload_bytes(P)], scales float32 [codec.scale_count(P)])`` rounded with the uint32 ``key``
+    (``encode_delta``'s codes, then ``r += q step`` in fp32), or topk ``(indices uint8 [E], values float32 [E])`` of ``v =
+    theta - replica`` (``encode_topk_delta``'s selection, then ``r += v`` at the sent entries).  Bit for bit what
+    ``downlink_quant_kernel`` / ``downlink_topk_kernel`` write (up to NaN payloads)."""
+    r = _replica_np(replica)
+    t = theta.detach().to("cpu", torch.float32).reshape(-1)
+    if codec.quantized:
+        payload, scales = encode_delta(t.view(1, -1), torch.from_numpy(r), codec.bits, [key])
+        apply_downlink(replica, payload[0], scales[0], codec)
+        return payload[0], scales[0]
+    if not codec.sparse:
+        raise ValueError("encode_downlink needs an int8 / int4 / topk codec")
+    if not 1 <= codec.k <= 32:
+        raise ValueError(f"topk keeps 1..32 entries per block, not {codec.k}")
+    with np.errstate(over="ignore", invalid="ignore"):
+        v = t.numpy() - r
+    idx, pos = _topk_select(v[None, :], codec.k)
+    values = v[pos[0]]
+    with np.errstate(over="ignore", invalid="ignore"):
+        r[pos[0]] = r[pos[0]] + values
+    replica.copy_(torch.from_numpy(r).view_as(replica))
+    return torch.from_numpy(np.ascontiguousarray(idx[0].astype(np.uint8))), torch.from_numpy(np.ascontiguousarray(values))
+
+
+def apply_downlink(replica: torch.Tensor, a: torch.Tensor, b: torch.Tensor, codec) -> torch.Tensor:
+    """``replica [P]`` advanced in place by a downlink wire: int8 / int4 ``(a, b) = (payload, scales)``, ``r += q step``; topk
+    ``(a, b) = (indices, values)``, ``r += value`` at each entry's position.  Bit for bit what ``replica_apply_q_kernel`` /
+    ``replica_apply_topk_kernel`` write."""
+    r = _replica_np(replica)
+    with np.errstate(over="ignore", invalid="ignore"):
+        if codec.quantized:
+            r = r + decode_delta(a.reshape(1, -1), b.reshape(1, -1), codec.bits, r.size)[0].numpy()
+        elif codec.sparse:
+            pos = _topk_positions(a.detach().to("cpu").numpy().reshape(1, -1), codec.k)[0]
+            r[pos] = r[pos] + b.detach().to("cpu", torch.float32).numpy().reshape(-1)
+        else:
+            raise ValueError("apply_downlink needs an int8 / int4 / topk codec")
+    return replica.copy_(torch.from_numpy(r).view_as(replica))
 
 
 def linear_bias_relu(x, w, b, relu=True):

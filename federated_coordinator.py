@@ -66,6 +66,12 @@ def build_parser() -> argparse.ArgumentParser:
                              "feedback; ~25x fewer bytes at 8); local and remote mode only (not with --box or -e)")
     parser.add_argument("--uplink-topk", type=int, default=d.uplink_topk,
                         help="--uplink-codec topk: entries sent per block of 256 parameters, in 1..32 (not with a robust --aggregator)")
+    parser.add_argument("--downlink-codec", choices=["fp32", "int8", "int4", "topk"], default=d.downlink,
+                        help="what the coordinator sends after the first round of a training: fp32 = the model; int8 / int4 / topk = "
+                             "the same codecs as --uplink-codec applied to the model minus the replica every device keeps, one "
+                             "encode per round for all devices (needs --uplink-codec int8, int4 or topk; not with --box or -e)")
+    parser.add_argument("--downlink-topk", type=int, default=d.downlink_topk,
+                        help="--downlink-codec topk: entries sent per block of 256 parameters, in 1..32")
     parser.add_argument("--seed", type=int, default=d.seed)
     parser.add_argument("--log-interval", type=int, default=d.log_interval)
     parser.add_argument("--test-path", type=str, default=d.test_path, help="CSV used by local/encrypted mode and evaluation")
@@ -134,6 +140,9 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.uplink = getattr(ns, "uplink_codec", a.uplink)
     a.uplink_topk = getattr(ns, "uplink_topk", a.uplink_topk)
     a.uplink_codec()                  # rejects a topk k outside 1..32 and topk with a robust aggregator
+    a.downlink = getattr(ns, "downlink_codec", a.downlink)
+    a.downlink_topk = getattr(ns, "downlink_topk", a.downlink_topk)
+    a.downlink_codec()                # rejects a topk k outside 1..32 and a compressed downlink with an fp32 uplink
     a.no_cuda, a.backend = ns.no_cuda, ns.backend
     if getattr(ns, "enc_items", None):
         a.n_train_items_enc = int(ns.enc_items)
@@ -222,6 +231,9 @@ def parse_cli(argv=None) -> argparse.Namespace:
     if ns.uplink_codec != "fp32" and (ns.box or ns.encryption):
         parser.error(f"--uplink-codec {ns.uplink_codec} applies to the local and remote modes only: --box trains on the GPUs of one "
                      "box (fp32 models over NVLink) and -e exchanges secret shares")
+    if ns.downlink_codec != "fp32" and (ns.box or ns.encryption):
+        parser.error(f"--downlink-codec {ns.downlink_codec} applies to the local and remote modes only: --box broadcasts fp32 models "
+                     "over NVLink and -e exchanges secret shares")
     return ns
 
 
