@@ -3,8 +3,9 @@
 // same bytes to every device, and both sides advance r by what was sent, bit for bit alike.  Whatever has not been delivered
 // yet is theta - r: it stays on the coordinator and goes out in later rounds (error feedback with no residual array).
 // downlink_quant_kernel / downlink_topk_kernel (encode and advance, coordinator) and replica_apply_q_kernel /
-// replica_apply_topk_kernel (advance from the wire, device) in elementwise.cu use these functions; the GPU build and the SIMT
-// CPU build (host_shim.h) both compile them, and ops/reference.py encode_downlink / apply_downlink is the numpy transcription.
+// replica_apply_topk_kernel (advance from the wire, device) in elementwise.cu use these functions, with the per-lane load,
+// block-scale, code and top-k emit steps they share with the uplink kernels there; the GPU build and the SIMT CPU build
+// (host_shim.h) both compile them, and ops/reference.py encode_downlink / apply_downlink is the numpy transcription.
 //
 // The codecs are the uplink's, with the same wire layout:
 //   int8 / int4 (uplink_quant.cuh): the codes and block steps of d = theta - r (one fp32 subtraction) with one key per round

@@ -241,19 +241,161 @@ fedavg_robust_kernel(float* __restrict__ theta, const float* __restrict__ slots,
   fedavg_robust_body<KMAX>(theta, F32Slots{slots, slot_stride}, k, agg, opt, n);
 }
 
+// ---- codec kernels: the per-lane steps they share ------------------------------------------------------------------------------
+// Every codec kernel below runs one warp per 256-element block (kUqBlock) and lane l holds elements e0 .. e0 + 7 of its block,
+// e0 = 256 b + 8 l.  Each kernel decides its own `vec` (its pointers 16-byte aligned, and whatever else it needs); without it
+// the same bits move through scalar accesses.
+
+// the cache hint of a load: plain (data the kernel writes back), streaming __ldcs (read once) or read-only __ldg
+enum LdHint { kLdPlain, kLdStream, kLdReadOnly };
+template <LdHint HINT, class T>
+__device__ __forceinline__ T ld_hint(const T* p) {
+  if constexpr (HINT == kLdStream) return __ldcs(p);
+  else if constexpr (HINT == kLdReadOnly) return __ldg(p);
+  else return *p;
+}
+
+// lane l's elements e0 .. e0 + 7 of p, 0 past n: two 16-byte loads with hint HINT when vec, which must imply n % 4 == 0 (a
+// 4-element group is then wholly inside or past n), plain scalar loads otherwise.  One branch on vec and predicated loads
+// inside it: a branch per group between a 16-byte and scalar loads kept a lane's loads from overlapping (the encoders ran up
+// to a quarter slower on the H100).
+template <LdHint HINT>
+__device__ __forceinline__ void lane_load8(const float* __restrict__ p, int64_t e0, int64_t n, bool vec, float (&x)[8]) {
+  if (vec) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (e0 + 4 * h < n) v = ld_hint<HINT>(reinterpret_cast<const float4*>(p + e0 + 4 * h));
+      x[4 * h + 0] = v.x; x[4 * h + 1] = v.y; x[4 * h + 2] = v.z; x[4 * h + 3] = v.w;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) x[i] = e0 + i < n ? p[e0 + i] : 0.f;
+  }
+}
+
+// lane l's elements e0 .. e0 + 7 of p back, none past n: 16-byte stores of the groups of 4 inside n when vec, scalar stores
+// otherwise (any n)
+__device__ __forceinline__ void lane_store8(float* __restrict__ p, int64_t e0, int64_t n, bool vec, const float (&x)[8]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t e = e0 + 4 * h;
+    if (vec && e + 4 <= n) {
+      *reinterpret_cast<float4*>(p + e) = make_float4(x[4 * h], x[4 * h + 1], x[4 * h + 2], x[4 * h + 3]);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if (e + i < n) p[e + i] = x[4 * h + i];
+      }
+    }
+  }
+}
+
+// the block's step and inverse scale (uq_block_scale) from the lanes' deltas d: the warp max of uq_abs_bits by shuffles
+template <int BITS>
+__device__ __forceinline__ void warp_block_scale(const float (&d)[8], float& step, float& inv) {
+  uint32_t amax = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const uint32_t a = uq_abs_bits(d[i]);
+    amax = a > amax ? a : amax;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const uint32_t a = __shfl_xor_sync(0xffffffffu, amax, o);
+    amax = a > amax ? a : amax;
+  }
+  uq_block_scale(amax, UqCodec<BITS>::kLevels, step, inv);
+}
+
+// lane l's 8 codes into / out of a payload row: one 8-byte (int8) or 4-byte (int4, element 2 i in the low nibble) access
+template <int BITS>
+__device__ __forceinline__ void store_codes8(uint8_t* __restrict__ row, int64_t e0, const int (&q)[8]) {
+  if constexpr (BITS == 8) {
+    uint2 w = make_uint2(0u, 0u);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      w.x |= ((uint32_t)q[i] & 0xffu) << (8 * i);
+      w.y |= ((uint32_t)q[4 + i] & 0xffu) << (8 * i);
+    }
+    *reinterpret_cast<uint2*>(row + e0) = w;
+  } else {
+    uint32_t w = 0u;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) w |= ((uint32_t)q[i] & 0xfu) << (4 * i);
+    *reinterpret_cast<uint32_t*>(row + (e0 >> 1)) = w;
+  }
+}
+template <int BITS, LdHint HINT>
+__device__ __forceinline__ void load_codes8(const uint8_t* __restrict__ row, int64_t e0, int (&q)[8]) {
+  if constexpr (BITS == 8) {
+    const uint2 w = ld_hint<HINT>(reinterpret_cast<const uint2*>(row + e0));
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      q[i] = (int)(int8_t)(w.x >> (8 * i));
+      q[4 + i] = (int)(int8_t)(w.y >> (8 * i));
+    }
+  } else {
+    const uint32_t w = ld_hint<HINT>(reinterpret_cast<const unsigned int*>(row + (e0 >> 1)));
+#pragma unroll
+    for (int i = 0; i < 8; ++i) q[i] = uq_nibble(w, i);
+  }
+}
+
+// The FedAvg weights of the codec apply kernels, as in fedavg_kernel: the first kSw staged in the shared array sw by the whole
+// CTA (the constructor ends in __syncthreads), any beyond read through the read-only cache.
+struct StagedWeights {
+  static constexpr int kSw = 256;
+  const float* sw;
+  const float* weights;
+  __device__ __forceinline__ StagedWeights(float* s, const float* w, int k) : sw(s), weights(w) {
+    for (int c = threadIdx.x; c < k && c < kSw; c += blockDim.x) s[c] = w[c];
+    __syncthreads();
+  }
+  __device__ __forceinline__ float wt(int c) const { return c < kSw ? sw[c] : __ldg(weights + c); }
+};
+
+// theta[e0 .. e0 + 7] (none past n) moved towards a = theta + acc: theta += opt.lr (a - theta) (OPT false) or the server
+// optimizer step (OPT true); 16-byte accesses of theta and the moments per 4 elements inside n when vec
+template <bool OPT>
+__device__ __forceinline__ void apply8(float* __restrict__ theta, int64_t e0, int64_t n, bool vec, const float (&acc)[8],
+                                       const ServerOptArgs& opt) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t e = e0 + 4 * h;
+    if (vec && e + 4 <= n) {
+      float4* t4 = reinterpret_cast<float4*>(theta + e);
+      float4 t = *t4;
+      const float4 a = make_float4(t.x + acc[4 * h], t.y + acc[4 * h + 1], t.z + acc[4 * h + 2], t.w + acc[4 * h + 3]);
+      if constexpr (OPT) {
+        t = server_opt_step4(opt, e >> 2, t, a);
+      } else {
+        t.x = fmaf(opt.lr, a.x - t.x, t.x); t.y = fmaf(opt.lr, a.y - t.y, t.y);
+        t.z = fmaf(opt.lr, a.z - t.z, t.z); t.w = fmaf(opt.lr, a.w - t.w, t.w);
+      }
+      *t4 = t;
+    } else {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if (e + i < n) {
+          const float t = theta[e + i], a = t + acc[4 * h + i];
+          theta[e + i] = OPT ? server_opt_step(opt, e + i, t, a) : fmaf(opt.lr, a - t, t);
+        }
+      }
+    }
+  }
+}
+
 // ---- uplink codec (uplink_quant.cuh) ----------------------------------------------------------------------------------------
-// Encode: one warp per (row, 256-element block); lane l holds elements 8 l .. 8 l + 7 of the block (two 16-byte loads of the
-// model and of theta when rows are 16-byte aligned, scalar loads with the same bits otherwise), the warp takes the block
-// max with shuffles, every lane stores its 8 codes in one 8-byte (int8) or 4-byte (int4) store and lane 0 the block's step.
-// Elements past n encode as 0 (the int4 pad nibble).  Single pass.
+// Encode: one warp per (row, block).  The lanes load the model (streamed) and theta, the warp takes the block's step, every
+// lane stores its 8 codes and lane 0 the step.  Elements past n encode as 0 (the int4 pad nibble).  Single pass.
 template <int BITS>
 __global__ void __launch_bounds__(256)
 quantize_delta_kernel(const float* __restrict__ models, int64_t model_stride, const float* __restrict__ theta,
                       const uint32_t* __restrict__ keys, int k, uint8_t* __restrict__ payload, int64_t row_bytes,
                       float* __restrict__ scales, int64_t n) {
-  constexpr int L = UqCodec<BITS>::kLevels;
   const int lane = threadIdx.x & 31;
-  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t nblk = uq_nblk(n);
   const int64_t tasks = nblk * k;
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const bool vec = (((uintptr_t)models | (uintptr_t)theta) & 15) == 0 && (model_stride & 3) == 0 && (n & 3) == 0;
@@ -261,54 +403,19 @@ quantize_delta_kernel(const float* __restrict__ models, int64_t model_stride, co
     const int c = (int)(t / nblk);
     const int64_t blk = t - (int64_t)c * nblk;
     const int64_t e0 = blk * kUqBlock + lane * 8;
-    const float* row = models + c * model_stride;
-    float d[8];
-    if (vec) {
+    float m[8], th[8], d[8];
+    lane_load8<kLdStream>(models + c * model_stride, e0, n, vec, m);
+    lane_load8<kLdReadOnly>(theta, e0, n, vec, th);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t e = e0 + 4 * h;
-        if (e < n) {
-          const float4 m = __ldcs(reinterpret_cast<const float4*>(row + e));
-          const float4 th = __ldg(reinterpret_cast<const float4*>(theta + e));
-          d[4 * h + 0] = m.x - th.x; d[4 * h + 1] = m.y - th.y; d[4 * h + 2] = m.z - th.z; d[4 * h + 3] = m.w - th.w;
-        } else {
-          d[4 * h + 0] = 0.f; d[4 * h + 1] = 0.f; d[4 * h + 2] = 0.f; d[4 * h + 3] = 0.f;
-        }
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) d[i] = (e0 + i < n) ? row[e0 + i] - theta[e0 + i] : 0.f;
-    }
-    uint32_t amax = 0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const uint32_t a = uq_abs_bits(d[i]);
-      amax = a > amax ? a : amax;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const uint32_t a = __shfl_xor_sync(0xffffffffu, amax, o);
-      amax = a > amax ? a : amax;
-    }
+    for (int i = 0; i < 8; ++i) d[i] = m[i] - th[i];
     float step, inv;
-    uq_block_scale(amax, L, step, inv);
+    warp_block_scale<BITS>(d, step, inv);
     const uint32_t key = keys[c];
     if (e0 < n) {
-      uint8_t* out = payload + c * row_bytes;
-      if constexpr (BITS == 8) {
-        uint2 w = make_uint2(0u, 0u);
+      int q[8];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          w.x |= ((uint32_t)uq_encode(d[i], inv, key, (uint32_t)(e0 + i), L) & 0xffu) << (8 * i);
-          w.y |= ((uint32_t)uq_encode(d[4 + i], inv, key, (uint32_t)(e0 + 4 + i), L) & 0xffu) << (8 * i);
-        }
-        *reinterpret_cast<uint2*>(out + e0) = w;
-      } else {
-        uint32_t w = 0u;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) w |= ((uint32_t)uq_encode(d[i], inv, key, (uint32_t)(e0 + i), L) & 0xfu) << (4 * i);
-        *reinterpret_cast<uint32_t*>(out + (e0 >> 1)) = w;
-      }
+      for (int i = 0; i < 8; ++i) q[i] = uq_encode(d[i], inv, key, (uint32_t)(e0 + i), UqCodec<BITS>::kLevels);
+      store_codes8<BITS>(payload + c * row_bytes, e0, q);
     }
     if (lane == 0) scales[c * nblk + blk] = step;
   }
@@ -316,19 +423,16 @@ quantize_delta_kernel(const float* __restrict__ models, int64_t model_stride, co
 
 // Decode + FedAvg reduce + apply, the quantized twin of fedavg_kernel / fedavg_opt_kernel: per element
 // acc = fmaf(w_k, d^_k, acc) in slot order from +0, a = theta + acc, then theta += opt.lr (a - theta) (OPT false) or the server
-// optimizer step (OPT true).  One warp per 256-element block (a slot's step is one broadcast load per warp), 8 elements per
-// lane: one 8-byte (int8) or 4-byte (int4) load per slot and lane.  Weights staged in shared memory as in fedavg_kernel.
+// optimizer step (OPT true).  One warp per block: a slot's step is one broadcast load per warp, its codes one streamed load per
+// lane.
 template <int BITS, bool OPT>
 __global__ void __launch_bounds__(256)
 fedavg_q_kernel(float* __restrict__ theta, const uint8_t* __restrict__ payload, int64_t row_bytes, const float* __restrict__ scales,
                 const float* __restrict__ weights, int k, ServerOptArgs opt, int64_t n) {
-  constexpr int kSw = 256;
-  __shared__ float sw[kSw];
-  for (int c = threadIdx.x; c < k && c < kSw; c += blockDim.x) sw[c] = weights[c];
-  __syncthreads();
-  auto wt = [&](int c) -> float { return c < kSw ? sw[c] : __ldg(weights + c); };
+  __shared__ float sw[StagedWeights::kSw];
+  const StagedWeights staged(sw, weights, k);
   const int lane = threadIdx.x & 31;
-  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t nblk = uq_nblk(n);
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const bool vec = (((uintptr_t)theta | (uintptr_t)opt.m | (uintptr_t)opt.v) & 15) == 0;
   for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
@@ -337,48 +441,16 @@ fedavg_q_kernel(float* __restrict__ theta, const uint8_t* __restrict__ payload, 
     float acc[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-    const uint8_t* p = payload + (BITS == 8 ? e0 : (e0 >> 1));
 #pragma unroll 4
     for (int c = 0; c < k; ++c) {
       const float step = __ldg(scales + c * nblk + blk);
-      const float w = wt(c);
-      if constexpr (BITS == 8) {
-        const uint2 v = __ldcs(reinterpret_cast<const uint2*>(p + c * row_bytes));
+      const float w = staged.wt(c);
+      int q[8];
+      load_codes8<BITS, kLdStream>(payload + c * row_bytes, e0, q);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          acc[i] = fmaf(w, uq_decode((int)(int8_t)(v.x >> (8 * i)), step), acc[i]);
-          acc[4 + i] = fmaf(w, uq_decode((int)(int8_t)(v.y >> (8 * i)), step), acc[4 + i]);
-        }
-      } else {
-        const uint32_t v = __ldcs(reinterpret_cast<const unsigned int*>(p + c * row_bytes));
-#pragma unroll
-        for (int i = 0; i < 8; ++i) acc[i] = fmaf(w, uq_decode(uq_nibble(v, i), step), acc[i]);
-      }
+      for (int i = 0; i < 8; ++i) acc[i] = fmaf(w, uq_decode(q[i], step), acc[i]);
     }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t e = e0 + 4 * h;
-      if (vec && e + 4 <= n) {
-        float4* t4 = reinterpret_cast<float4*>(theta + e);
-        float4 t = *t4;
-        const float4 a = make_float4(t.x + acc[4 * h], t.y + acc[4 * h + 1], t.z + acc[4 * h + 2], t.w + acc[4 * h + 3]);
-        if constexpr (OPT) {
-          t = server_opt_step4(opt, e >> 2, t, a);
-        } else {
-          t.x = fmaf(opt.lr, a.x - t.x, t.x); t.y = fmaf(opt.lr, a.y - t.y, t.y);
-          t.z = fmaf(opt.lr, a.z - t.z, t.z); t.w = fmaf(opt.lr, a.w - t.w, t.w);
-        }
-        *t4 = t;
-      } else {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          if (e + i < n) {
-            const float t = theta[e + i], a = t + acc[4 * h + i];
-            theta[e + i] = OPT ? server_opt_step(opt, e + i, t, a) : fmaf(opt.lr, a - t, t);
-          }
-        }
-      }
-    }
+    apply8<OPT>(theta, e0, n, vec, acc, opt);
   }
 }
 
@@ -387,7 +459,7 @@ template <int KMAX, int BITS>
 __global__ void __launch_bounds__(256)
 fedavg_q_robust_kernel(float* __restrict__ theta, const uint8_t* __restrict__ payload, int64_t row_bytes, const float* __restrict__ scales,
                        int k, AggArgs agg, ServerOptArgs opt, int64_t n) {
-  fedavg_robust_body<KMAX>(theta, QSlots<BITS>{payload, row_bytes, scales, (n + kUqBlock - 1) / kUqBlock}, k, agg, opt, n);
+  fedavg_robust_body<KMAX>(theta, QSlots<BITS>{payload, row_bytes, scales, uq_nblk(n)}, k, agg, opt, n);
 }
 
 // ---- top-k uplink with error feedback (uplink_topk.cuh) -----------------------------------------------------------------------
@@ -440,17 +512,30 @@ __device__ __forceinline__ TopkSel8 warp_topk_select(TopkKeys8 keys, int kb, uin
   return sel;
 }
 
-// Encode: one warp per (row, 256-element block); lane l holds elements 8 l .. 8 l + 7 of the block (16-byte loads of the
-// model, theta and the residual when rows are 16-byte aligned, scalar loads with the same bits otherwise).  warp_topk_select
-// picks the entries, which are stored in index order; the residual is written back in place.  Elements past n take key 0:
-// they lose every tie to the block's own elements, and k_b <= m_b.
+// a lane's kept entries (offset in the block, value v[i]) in index order from entry `out` + sel.first of the wire
+__device__ __forceinline__ void topk_emit(uint8_t* __restrict__ indices, float* __restrict__ values, int64_t out, int lane,
+                                          const TopkSel8& sel, const float (&v)[8]) {
+  int o = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    if (sel.keep[i]) {
+      indices[out + sel.first + o] = (uint8_t)(lane * 8 + i);
+      values[out + sel.first + o] = v[i];
+      ++o;
+    }
+  }
+}
+
+// Encode: one warp per (row, block).  The lanes load the model (streamed), theta and the residual, warp_topk_select picks the
+// entries, and the residual is written back in place.  Elements past n take key 0: they lose every tie to the block's own
+// elements, and k_b <= m_b.
 __global__ void __launch_bounds__(256)
 topk_delta_kernel(const float* __restrict__ models, int64_t model_stride, const float* __restrict__ theta, float* __restrict__ residual,
                   int64_t residual_stride, int k, int topk, uint8_t* __restrict__ indices, float* __restrict__ values, int64_t entries,
                   int64_t n) {
   const int lane = threadIdx.x & 31;
   const uint32_t lower_lanes = (1u << lane) - 1u;
-  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t nblk = uq_nblk(n);
   const int64_t tasks = nblk * k;
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const bool vec = (((uintptr_t)models | (uintptr_t)theta | (uintptr_t)residual) & 15) == 0 && (model_stride & 3) == 0 &&
@@ -459,57 +544,22 @@ topk_delta_kernel(const float* __restrict__ models, int64_t model_stride, const 
     const int c = (int)(t / nblk);
     const int64_t blk = t - (int64_t)c * nblk;
     const int64_t e0 = blk * kUqBlock + lane * 8;
-    const float* row = models + c * model_stride;
     float* res = residual + c * residual_stride;
-    float v[8];
-    if (vec) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t e = e0 + 4 * h;
-        if (e < n) {
-          const float4 m = __ldcs(reinterpret_cast<const float4*>(row + e));
-          const float4 th = __ldg(reinterpret_cast<const float4*>(theta + e));
-          const float4 r = *reinterpret_cast<const float4*>(res + e);
-          v[4 * h + 0] = (m.x - th.x) + r.x; v[4 * h + 1] = (m.y - th.y) + r.y;
-          v[4 * h + 2] = (m.z - th.z) + r.z; v[4 * h + 3] = (m.w - th.w) + r.w;
-        } else {
-          v[4 * h + 0] = 0.f; v[4 * h + 1] = 0.f; v[4 * h + 2] = 0.f; v[4 * h + 3] = 0.f;
-        }
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = (e0 + i < n) ? (row[e0 + i] - theta[e0 + i]) + res[e0 + i] : 0.f;
-    }
+    float m[8], th[8], v[8];
+    lane_load8<kLdStream>(models + c * model_stride, e0, n, vec, m);
+    lane_load8<kLdReadOnly>(theta, e0, n, vec, th);
+    lane_load8<kLdPlain>(res, e0, n, vec, v);
     TopkKeys8 keys;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) keys.key[i] = (e0 + i < n) ? ut_key(v[i]) : 0u;
-    const TopkSel8 sel = warp_topk_select(keys, ut_block_k(n, blk, topk), lower_lanes);
-    const bool* keep = sel.keep;
-    const int64_t out = c * entries + blk * topk + sel.first;
-    int o = 0;
-#pragma unroll
     for (int i = 0; i < 8; ++i) {
-      if (keep[i]) {
-        indices[out + o] = (uint8_t)(lane * 8 + i);
-        values[out + o] = v[i];
-        ++o;
-      }
+      v[i] = (m[i] - th[i]) + v[i];
+      keys.key[i] = (e0 + i < n) ? ut_key(v[i]) : 0u;
     }
-    float r[8];
+    const TopkSel8 sel = warp_topk_select(keys, ut_block_k(n, blk, topk), lower_lanes);
+    topk_emit(indices, values, c * entries + blk * topk, lane, sel, v);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) r[i] = keep[i] ? 0.f : v[i];
-    if (vec) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t e = e0 + 4 * h;
-        if (e < n) *reinterpret_cast<float4*>(res + e) = make_float4(r[4 * h], r[4 * h + 1], r[4 * h + 2], r[4 * h + 3]);
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        if (e0 + i < n) res[e0 + i] = r[i];
-      }
-    }
+    for (int i = 0; i < 8; ++i) v[i] = sel.keep[i] ? 0.f : v[i];
+    lane_store8(res, e0, n, vec, v);
   }
 }
 
@@ -518,20 +568,18 @@ topk_delta_kernel(const float* __restrict__ models, int64_t model_stride, const 
 // distinct, and a __syncwarp separates slots: deterministic); the entries of 8 slots are loaded ahead of their scatters.  Then
 // lane l reads elements 8 l .. 8 l + 7 back, a = theta + acc, and theta += opt.lr (a - theta) (OPT false) or the server
 // optimizer step (OPT true).  A uint8 offset cannot leave the accumulator; offsets past the end of a partial last block land
-// in accumulator cells no lane applies.  Weights staged in shared memory as in fedavg_kernel.
+// in accumulator cells no lane applies.
 template <bool OPT>
 __global__ void __launch_bounds__(256)
 fedavg_topk_kernel(float* __restrict__ theta, const uint8_t* __restrict__ indices, const float* __restrict__ values, int64_t entries,
                    const float* __restrict__ weights, int k, int topk, ServerOptArgs opt, int64_t n) {
-  constexpr int kSw = 256, kAhead = 8;
-  __shared__ float sw[kSw];
+  constexpr int kAhead = 8;
+  __shared__ float sw[StagedWeights::kSw];
   __shared__ __align__(16) float sacc[kThreads / 32][kUqBlock];
-  for (int c = threadIdx.x; c < k && c < kSw; c += blockDim.x) sw[c] = weights[c];
-  __syncthreads();
-  auto wt = [&](int c) -> float { return c < kSw ? sw[c] : __ldg(weights + c); };
+  const StagedWeights staged(sw, weights, k);
   const int lane = threadIdx.x & 31;
   float* acc = sacc[threadIdx.x >> 5];
-  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t nblk = uq_nblk(n);
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const bool vec = (((uintptr_t)theta | (uintptr_t)opt.m | (uintptr_t)opt.v) & 15) == 0;
   for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
@@ -557,7 +605,7 @@ fedavg_topk_kernel(float* __restrict__ theta, const uint8_t* __restrict__ indice
 #pragma unroll
       for (int u = 0; u < kAhead; ++u) {
         if (c0 + u < k) {
-          if (sends) acc[idx[u]] = fmaf(wt(c0 + u), val[u], acc[idx[u]]);
+          if (sends) acc[idx[u]] = fmaf(staged.wt(c0 + u), val[u], acc[idx[u]]);
           __syncwarp();
         }
       }
@@ -566,145 +614,59 @@ fedavg_topk_kernel(float* __restrict__ theta, const uint8_t* __restrict__ indice
     float a8[8];
     const float4 lo = *reinterpret_cast<const float4*>(acc + lane * 8), hi = *reinterpret_cast<const float4*>(acc + lane * 8 + 4);
     a8[0] = lo.x; a8[1] = lo.y; a8[2] = lo.z; a8[3] = lo.w; a8[4] = hi.x; a8[5] = hi.y; a8[6] = hi.z; a8[7] = hi.w;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t e = e0 + 4 * h;
-      if (vec && e + 4 <= n) {
-        float4* t4 = reinterpret_cast<float4*>(theta + e);
-        float4 t = *t4;
-        const float4 a = make_float4(t.x + a8[4 * h], t.y + a8[4 * h + 1], t.z + a8[4 * h + 2], t.w + a8[4 * h + 3]);
-        if constexpr (OPT) {
-          t = server_opt_step4(opt, e >> 2, t, a);
-        } else {
-          t.x = fmaf(opt.lr, a.x - t.x, t.x); t.y = fmaf(opt.lr, a.y - t.y, t.y);
-          t.z = fmaf(opt.lr, a.z - t.z, t.z); t.w = fmaf(opt.lr, a.w - t.w, t.w);
-        }
-        *t4 = t;
-      } else {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          if (e + i < n) {
-            const float t = theta[e + i], a = t + a8[4 * h + i];
-            theta[e + i] = OPT ? server_opt_step(opt, e + i, t, a) : fmaf(opt.lr, a - t, t);
-          }
-        }
-      }
-    }
+    apply8<OPT>(theta, e0, n, vec, a8, opt);
   }
 }
 
 // ---- compressed downlink (downlink.cuh) ---------------------------------------------------------------------------------------
-// lane l's 8 elements 8 l .. 8 l + 7 of theta and of the replica (two 16-byte loads each when vec, scalar loads with the same
-// bits otherwise; 0 past n)
-__device__ __forceinline__ void dl_load8(const float* __restrict__ theta, const float* __restrict__ replica, int64_t e0, int64_t n,
-                                         bool vec, float (&t)[8], float (&r)[8]) {
-  if (vec) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t e = e0 + 4 * h;
-      float4 th = make_float4(0.f, 0.f, 0.f, 0.f), rp = th;
-      if (e < n) {
-        th = __ldg(reinterpret_cast<const float4*>(theta + e));
-        rp = *reinterpret_cast<const float4*>(replica + e);
-      }
-      t[4 * h + 0] = th.x; t[4 * h + 1] = th.y; t[4 * h + 2] = th.z; t[4 * h + 3] = th.w;
-      r[4 * h + 0] = rp.x; r[4 * h + 1] = rp.y; r[4 * h + 2] = rp.z; r[4 * h + 3] = rp.w;
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      t[i] = e0 + i < n ? theta[e0 + i] : 0.f;
-      r[i] = e0 + i < n ? replica[e0 + i] : 0.f;
-    }
-  }
-}
-
-// lane l's 8 replica elements back (16-byte stores where the 4 are inside n and vec, scalar stores otherwise)
-__device__ __forceinline__ void dl_store8(float* __restrict__ replica, int64_t e0, int64_t n, bool vec, const float (&r)[8]) {
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int64_t e = e0 + 4 * h;
-    if (vec && e + 4 <= n) {
-      *reinterpret_cast<float4*>(replica + e) = make_float4(r[4 * h], r[4 * h + 1], r[4 * h + 2], r[4 * h + 3]);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        if (e + i < n) replica[e + i] = r[4 * h + i];
-      }
-    }
-  }
-}
-
-// Coordinator, int8 / int4: quantize_delta_kernel's shape on d = theta - replica for one row (one warp per 256-element block,
-// block max by shuffles, 8 codes per lane in one store, lane 0 the step), and the replica advanced in the same pass.
+// Coordinator, int8 / int4: quantize_delta_kernel's steps on d = theta - replica for one row, and the replica advanced in the
+// same pass.
 template <int BITS>
 __global__ void __launch_bounds__(256)
 downlink_quant_kernel(const float* __restrict__ theta, float* __restrict__ replica, uint32_t key, uint8_t* __restrict__ payload,
                       float* __restrict__ scales, int64_t n) {
-  constexpr int L = UqCodec<BITS>::kLevels;
   const int lane = threadIdx.x & 31;
-  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t nblk = uq_nblk(n);
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const bool vec = (((uintptr_t)theta | (uintptr_t)replica) & 15) == 0 && (n & 3) == 0;
   for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
     const int64_t e0 = blk * kUqBlock + lane * 8;
     float t[8], r[8], d[8];
-    dl_load8(theta, replica, e0, n, vec, t, r);
-    uint32_t amax = 0;
+    lane_load8<kLdReadOnly>(theta, e0, n, vec, t);
+    lane_load8<kLdPlain>(replica, e0, n, vec, r);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      d[i] = t[i] - r[i];
-      const uint32_t a = uq_abs_bits(d[i]);
-      amax = a > amax ? a : amax;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const uint32_t a = __shfl_xor_sync(0xffffffffu, amax, o);
-      amax = a > amax ? a : amax;
-    }
+    for (int i = 0; i < 8; ++i) d[i] = t[i] - r[i];
     float step, inv;
-    uq_block_scale(amax, L, step, inv);
+    warp_block_scale<BITS>(d, step, inv);
     if (e0 < n) {
       int q[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        q[i] = uq_encode(d[i], inv, key, (uint32_t)(e0 + i), L);
+        q[i] = uq_encode(d[i], inv, key, (uint32_t)(e0 + i), UqCodec<BITS>::kLevels);
         r[i] = dl_quant_advance(r[i], q[i], step);
       }
-      if constexpr (BITS == 8) {
-        uint2 w = make_uint2(0u, 0u);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          w.x |= ((uint32_t)q[i] & 0xffu) << (8 * i);
-          w.y |= ((uint32_t)q[4 + i] & 0xffu) << (8 * i);
-        }
-        *reinterpret_cast<uint2*>(payload + e0) = w;
-      } else {
-        uint32_t w = 0u;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) w |= ((uint32_t)q[i] & 0xfu) << (4 * i);
-        *reinterpret_cast<uint32_t*>(payload + (e0 >> 1)) = w;
-      }
-      dl_store8(replica, e0, n, vec, r);
+      store_codes8<BITS>(payload, e0, q);
+      lane_store8(replica, e0, n, vec, r);
     }
     if (lane == 0) scales[blk] = step;
   }
 }
 
 // Coordinator, topk: the selection of topk_delta_kernel (warp_topk_select) on v = theta - replica with no residual; the kept
-// entries are stored in index order and added into the replica (scalar stores of the kept elements only).
+// entries go to the wire and are added into the replica (scalar stores of the kept elements only).
 __global__ void __launch_bounds__(256)
 downlink_topk_kernel(const float* __restrict__ theta, float* __restrict__ replica, int topk, uint8_t* __restrict__ indices,
                      float* __restrict__ values, int64_t n) {
   const int lane = threadIdx.x & 31;
   const uint32_t lower_lanes = (1u << lane) - 1u;
-  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t nblk = uq_nblk(n);
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const bool vec = (((uintptr_t)theta | (uintptr_t)replica) & 15) == 0 && (n & 3) == 0;
   for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
     const int64_t e0 = blk * kUqBlock + lane * 8;
     float t[8], r[8], v[8];
-    dl_load8(theta, replica, e0, n, vec, t, r);
+    lane_load8<kLdReadOnly>(theta, e0, n, vec, t);
+    lane_load8<kLdPlain>(replica, e0, n, vec, r);
     TopkKeys8 keys;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -712,28 +674,20 @@ downlink_topk_kernel(const float* __restrict__ theta, float* __restrict__ replic
       keys.key[i] = (e0 + i < n) ? ut_key(v[i]) : 0u;
     }
     const TopkSel8 sel = warp_topk_select(keys, ut_block_k(n, blk, topk), lower_lanes);
-    const bool* keep = sel.keep;
-    const int64_t out = blk * topk + sel.first;
-    int o = 0;
+    topk_emit(indices, values, blk * topk, lane, sel, v);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      if (keep[i]) {
-        indices[out + o] = (uint8_t)(lane * 8 + i);
-        values[out + o] = v[i];
-        replica[e0 + i] = dl_add_rn(r[i], v[i]);
-        ++o;
-      }
+      if (sel.keep[i]) replica[e0 + i] = dl_add_rn(r[i], v[i]);
     }
   }
 }
 
-// Device, int8 / int4: replica += decode(wire), one warp per 256-element block, 8 elements per lane: one 8-byte (int8) or
-// 4-byte (int4) load of codes, 16-byte loads / stores of the replica where aligned.
+// Device, int8 / int4: replica += decode(wire), one warp per block.
 template <int BITS>
 __global__ void __launch_bounds__(256)
 replica_apply_q_kernel(float* __restrict__ replica, const uint8_t* __restrict__ payload, const float* __restrict__ scales, int64_t n) {
   const int lane = threadIdx.x & 31;
-  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t nblk = uq_nblk(n);
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const bool vec = ((uintptr_t)replica & 15) == 0;
   for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
@@ -741,18 +695,8 @@ replica_apply_q_kernel(float* __restrict__ replica, const uint8_t* __restrict__ 
     if (e0 >= n) continue;
     const float step = __ldg(scales + blk);
     int q[8];
-    if constexpr (BITS == 8) {
-      const uint2 w = __ldg(reinterpret_cast<const uint2*>(payload + e0));
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        q[i] = (int)(int8_t)(w.x >> (8 * i));
-        q[4 + i] = (int)(int8_t)(w.y >> (8 * i));
-      }
-    } else {
-      const uint32_t w = __ldg(reinterpret_cast<const unsigned int*>(payload + (e0 >> 1)));
-#pragma unroll
-      for (int i = 0; i < 8; ++i) q[i] = uq_nibble(w, i);
-    }
+    load_codes8<BITS, kLdReadOnly>(payload, e0, q);
+    // not lane_load8: this vec allows any n, so the groups of 4 inside n load 16 bytes and a last partial group scalars
     float r[8];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -767,7 +711,7 @@ replica_apply_q_kernel(float* __restrict__ replica, const uint8_t* __restrict__ 
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) r[i] = dl_quant_advance(r[i], q[i], step);
-    dl_store8(replica, e0, n, vec, r);
+    lane_store8(replica, e0, n, vec, r);
   }
 }
 
@@ -777,7 +721,7 @@ __global__ void __launch_bounds__(256)
 replica_apply_topk_kernel(float* __restrict__ replica, const uint8_t* __restrict__ indices, const float* __restrict__ values, int topk,
                           int64_t n) {
   const int lane = threadIdx.x & 31;
-  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t nblk = uq_nblk(n);
   const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
   for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
     if (lane >= ut_block_k(n, blk, topk)) continue;
@@ -1135,14 +1079,14 @@ template <int BITS>
 inline cudaError_t launch_quantize_delta_t(const float* models, int64_t model_stride, const float* theta, const uint32_t* keys, int k,
                                            uint8_t* payload, int64_t row_bytes, float* scales, int64_t n, cudaStream_t s) {
   auto kernel = quantize_delta_kernel<BITS>;
-  COLEARN_LAUNCH(kernel, grid_for_warps(k * ((n + kUqBlock - 1) / kUqBlock)), kThreads, 0, s, models, model_stride, theta, keys, k, payload,
+  COLEARN_LAUNCH(kernel, grid_for_warps(k * uq_nblk(n)), kThreads, 0, s, models, model_stride, theta, keys, k, payload,
                  row_bytes, scales, n);
   return cudaGetLastError();
 }
 template <int BITS>
 inline cudaError_t launch_fedavg_q_t(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, const float* weights,
                                      int k, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
-  const int grid = grid_for_warps((n + kUqBlock - 1) / kUqBlock);
+  const int grid = grid_for_warps(uq_nblk(n));
   if (opt.kind == SOPT_SGD) {
     auto kernel = fedavg_q_kernel<BITS, false>;
     COLEARN_LAUNCH(kernel, grid, kThreads, 0, s, theta, payload, row_bytes, scales, weights, k, opt, n);
@@ -1197,7 +1141,7 @@ cudaError_t launch_topk_delta(const float* models, int64_t model_stride, const f
                               int rows, int topk, uint8_t* indices, float* values, int64_t entries, int64_t n, cudaStream_t s) {
   if (rows < 1 || topk < 1 || topk > kUtMaxK || n < 1 || model_stride < n || residual_stride < n || entries < ut_entries(n, topk))
     return cudaErrorInvalidValue;
-  COLEARN_LAUNCH(topk_delta_kernel, grid_for_warps(rows * ((n + kUqBlock - 1) / kUqBlock)), kThreads, 0, s, models, model_stride, theta,
+  COLEARN_LAUNCH(topk_delta_kernel, grid_for_warps(rows * uq_nblk(n)), kThreads, 0, s, models, model_stride, theta,
                  residual, residual_stride, rows, topk, indices, values, entries, n);
   return cudaGetLastError();
 }
@@ -1205,7 +1149,7 @@ cudaError_t launch_fedavg_apply_topk(float* theta, const uint8_t* indices, const
                                      int rows, int topk, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
   if (rows < 1 || topk < 1 || topk > kUtMaxK || n < 1 || entries < ut_entries(n, topk) || !server_opt_args_ok(opt))
     return cudaErrorInvalidValue;
-  const int grid = grid_for_warps((n + kUqBlock - 1) / kUqBlock);
+  const int grid = grid_for_warps(uq_nblk(n));
   if (opt.kind == SOPT_SGD) {
     COLEARN_LAUNCH(fedavg_topk_kernel<false>, grid, kThreads, 0, s, theta, indices, values, entries, weights, rows, topk, opt, n);
   } else {
@@ -1217,12 +1161,12 @@ cudaError_t launch_downlink_quant(const float* theta, float* replica, uint32_t k
                                   float* scales, int64_t n, cudaStream_t s) {
   if (!uq_layout_ok(bits, payload, row_bytes, n)) return cudaErrorInvalidValue;
   auto kernel = bits == 8 ? downlink_quant_kernel<8> : downlink_quant_kernel<4>;
-  COLEARN_LAUNCH(kernel, grid_for_warps((n + kUqBlock - 1) / kUqBlock), kThreads, 0, s, theta, replica, key, payload, scales, n);
+  COLEARN_LAUNCH(kernel, grid_for_warps(uq_nblk(n)), kThreads, 0, s, theta, replica, key, payload, scales, n);
   return cudaGetLastError();
 }
 cudaError_t launch_downlink_topk(const float* theta, float* replica, int topk, uint8_t* indices, float* values, int64_t n, cudaStream_t s) {
   if (topk < 1 || topk > kUtMaxK || n < 1) return cudaErrorInvalidValue;
-  COLEARN_LAUNCH(downlink_topk_kernel, grid_for_warps((n + kUqBlock - 1) / kUqBlock), kThreads, 0, s, theta, replica, topk, indices,
+  COLEARN_LAUNCH(downlink_topk_kernel, grid_for_warps(uq_nblk(n)), kThreads, 0, s, theta, replica, topk, indices,
                  values, n);
   return cudaGetLastError();
 }
@@ -1230,12 +1174,12 @@ cudaError_t launch_replica_apply_quant(float* replica, const uint8_t* payload, i
                                        int64_t n, cudaStream_t s) {
   if (!uq_layout_ok(bits, payload, row_bytes, n)) return cudaErrorInvalidValue;
   auto kernel = bits == 8 ? replica_apply_q_kernel<8> : replica_apply_q_kernel<4>;
-  COLEARN_LAUNCH(kernel, grid_for_warps((n + kUqBlock - 1) / kUqBlock), kThreads, 0, s, replica, payload, scales, n);
+  COLEARN_LAUNCH(kernel, grid_for_warps(uq_nblk(n)), kThreads, 0, s, replica, payload, scales, n);
   return cudaGetLastError();
 }
 cudaError_t launch_replica_apply_topk(float* replica, const uint8_t* indices, const float* values, int topk, int64_t n, cudaStream_t s) {
   if (topk < 1 || topk > kUtMaxK || n < 1) return cudaErrorInvalidValue;
-  COLEARN_LAUNCH(replica_apply_topk_kernel, grid_for_warps((n + kUqBlock - 1) / kUqBlock), kThreads, 0, s, replica, indices, values,
+  COLEARN_LAUNCH(replica_apply_topk_kernel, grid_for_warps(uq_nblk(n)), kThreads, 0, s, replica, indices, values,
                  topk, n);
   return cudaGetLastError();
 }

@@ -1,8 +1,9 @@
 // Uplink compression of the client updates (QSGD / FedPAQ-style unbiased stochastic quantization): a client sends its delta
 // d = theta_k - theta as int8 or int4 codes with one float32 scale per block of 256 elements, instead of its fp32 model.
 // quantize_delta_kernel (encode) and fedavg_q_kernel / fedavg_q_robust_kernel (decode fused into the FedAvg apply) in
-// elementwise.cu use these functions; the GPU build and the SIMT CPU build (host_shim.h) both compile them, and
-// ops/reference.py encode_delta / decode_delta is the PyTorch transcription.
+// elementwise.cu use these functions, and so do the int8 / int4 downlink kernels (downlink.cuh) and, for uq_nblk, every codec
+// kernel; the GPU build and the SIMT CPU build (host_shim.h) both compile them, and ops/reference.py encode_delta /
+// decode_delta is the PyTorch transcription.
 //
 // Per block of kUqBlock consecutive elements (the last block may be partial), with L = 127 (int8) or 7 (int4):
 //   s    = max |d_j| over the block (as the uint32 max of the bit patterns |d_j|: NaN and Inf sort above every finite value)
@@ -24,6 +25,9 @@
 namespace colearn {
 
 constexpr int kUqBlock = 256;
+
+// blocks of a row of n elements
+COLEARN_HD int64_t uq_nblk(int64_t n) { return (n + kUqBlock - 1) / kUqBlock; }
 
 template <int BITS>
 struct UqCodec {

@@ -2,8 +2,8 @@
 // client keeps the k largest-magnitude entries of every 256-element block of v = d + e (its delta d = theta_k - theta plus the
 // residual e it did not send in earlier rounds), sends them as (uint8 offset, fp32 value) pairs and carries the rest over.
 // topk_delta_kernel (encode) and fedavg_topk_kernel (decode fused into the FedAvg apply) in elementwise.cu use these
-// functions; the GPU build and the SIMT CPU build (host_shim.h) both compile them, and ops/reference.py encode_topk_delta /
-// decode_topk_delta is the numpy transcription.
+// functions, and so do the top-k downlink kernels (downlink.cuh); the GPU build and the SIMT CPU build (host_shim.h) both
+// compile them, and ops/reference.py encode_topk_delta / decode_topk_delta is the numpy transcription.
 //
 // Per element j (fp32, in this order and with no other arithmetic):  d_j = m_j - theta_j,  v_j = d_j + e_j.
 // Blocks are the codec's kUqBlock-element blocks: block b covers [256 b, min(256 b + 256, P)), length m_b; it keeps
@@ -32,7 +32,7 @@ COLEARN_HD uint32_t ut_key(float v) {
 
 // entries of a row of n elements at k per block
 COLEARN_HD int64_t ut_entries(int64_t n, int k) {
-  const int64_t nblk = (n + kUqBlock - 1) / kUqBlock;
+  const int64_t nblk = uq_nblk(n);
   const int64_t last = n - (nblk - 1) * kUqBlock;
   return (int64_t)k * (nblk - 1) + (last < k ? last : k);
 }
