@@ -46,6 +46,9 @@ class Arguments:
     downlink: str = "fp32"         # what the coordinator sends after round 0: fp32 (the model) | int8 | int4 | topk (a compressed
                                    # delta to the replica the devices keep; needs a delta uplink; fl/uplink.py)
     downlink_topk: int = 8         # downlink topk: entries sent per block of 256 parameters, in 1..32
+    secure_agg: bool = False       # remote mode: devices send pairwise-masked fixed-point deltas, the coordinator learns only their
+                                   # sum (fl/secagg.py)
+    secagg_clip: float = 1.0       # secure aggregation: every coordinate of a delta is clipped to [-clip, clip] (finite, > 0)
     backend: str = "auto"          # auto | fused | nccl | cpu
     dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the wgmma consumers)
     save_every: int = 0            # >0: checkpoint every N rounds, not only after the last one
@@ -81,10 +84,25 @@ class Arguments:
         int4 / topk): the devices' deltas are then taken against the replica they trained from."""
         from ..fl.uplink import UplinkCodec
         codec = UplinkCodec(self.downlink, k=self.downlink_topk)
-        if codec.kind != "fp32" and self.uplink_codec().kind == "fp32":
+        if codec.kind != "fp32" and self.uplink_codec().kind == "fp32" and not self.secure_agg:
             raise ValueError(f"--downlink-codec {self.downlink} needs --uplink-codec int8, int4 or topk: with fp32 replies the server "
                              "would have to shift every returned model by theta - replica")
         return codec
+
+    def secagg_clip_value(self) -> float:
+        """The clip of ``secure_agg`` after the checks that do not depend on the mode: the devices send fixed-point deltas
+        whose sum the coordinator learns, so there is no other uplink codec, no robust aggregator and no weighting."""
+        from ..fl.secagg import check_clip
+        clip = check_clip(self.secagg_clip)
+        if not self.secure_agg:
+            return clip
+        if self.uplink != "fp32":
+            raise ValueError(f"--secure-agg does not combine with --uplink-codec {self.uplink}: the masked row is its own encoding")
+        if self.client_aggregator().robust:
+            raise ValueError(f"--secure-agg does not combine with --aggregator {self.aggregator}: only the sum of the updates survives the masks")
+        if self.weighted:
+            raise ValueError("--secure-agg does not combine with --weighted: the masked sum gives the unweighted mean")
+        return clip
 
     def set_federated_batches(self, batches: int) -> None:
         self.federate_after_n_batches = batches

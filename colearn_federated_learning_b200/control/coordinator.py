@@ -33,6 +33,7 @@ from ..data import federate, synthetic_for_model, BaseDataset
 from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
 from ..fl.evaluate import evaluate
+from ..fl.secagg import check_masked_reply, check_unmask_reply, correction_streams, frac_bits, pk_from_bytes, pk_to_bytes
 # the reply checks live next to the codec (the workers run them on the downlink wire too) and are exported from here as before
 from ..fl.uplink import UplinkCodec, check_quantized_reply, check_topk_reply, downlink_key, uplink_key  # noqa: F401
 from ..models import MLPNet, build_model, flatten_params, unflatten_params
@@ -434,6 +435,13 @@ class Coordinator(BusClient):
         # mistake an earlier training's replica for this one's); memory only
         replica = theta.to(self.device).clone() if down.kind != "fp32" else None
         nonce = secrets.token_hex(8)
+        sa = None
+        if self.args.secure_agg:
+            # secure aggregation (fl/secagg.py): key agreement once per training, tagged with its nonce; fewer than two
+            # devices left after it cannot hide one update in a sum
+            sa = await self._secagg_setup(alive, nonce, loop, pool, result)
+            if sa is None:
+                return theta
         for r in range(self.enabled_round):
             log.info("\n\n#### ROUND {} #####".format(r))
             t0 = time.time()
@@ -446,8 +454,16 @@ class Coordinator(BusClient):
                     raise ValueError(f"replica crc {update.get('replica_crc')!r} returned, the coordinator's is {crc}")
                 return update
 
+            u1 = list(alive)                                          # secure aggregation: this round's participants
+
             async def one(wid: str, worker: RemoteWorkerClient):
                 try:
+                    if sa is not None:
+                        fields = {"tag": sa["tag"], "t": r, "u1": u1, "clip": sa["clip"], "frac_bits": sa["frac_bits"]}
+                        fut = loop.run_in_executor(pool, lambda: worker.fit_secagg(theta, rcfg, fields, timeout=self.fit_timeout,
+                                                                                  downlink=downlink))
+                        update, loss, n = await fut
+                        return wid, check_masked_reply(same_replica(update), theta.numel()), loss, n
                     if codec.quantized:
                         fut = loop.run_in_executor(pool, lambda: worker.fit_quantized(theta, rcfg, codec, timeout=self.fit_timeout,
                                                                                      downlink=downlink))
@@ -475,8 +491,6 @@ class Coordinator(BusClient):
             traffic = lambda w: (getattr(w, "bytes_sent", 0), getattr(w, "bytes_received", 0))  # noqa: E731 - any handle type
             sent0 = {wid: traffic(w) for wid, w in alive.items()}
             results = await asyncio.gather(*[one(wid, w) for wid, w in alive.items()])
-            bytes_out = sum(traffic(w)[0] - sent0[wid][0] for wid, w in to_train.items() if wid in sent0)
-            bytes_in = sum(traffic(w)[1] - sent0[wid][1] for wid, w in to_train.items() if wid in sent0)
             flats, counts, ids = [], [], []
             for wid, flat, loss, n in results:
                 if flat is not None:
@@ -488,7 +502,10 @@ class Coordinator(BusClient):
                 else:
                     result["dropped"].append(wid)
                     alive.pop(wid, None)
-            if flats:
+            secagg_rec = {}
+            if sa is not None:
+                theta, secagg_rec = await self._secagg_round(theta, r, u1, ids, flats, alive, sa, loop, pool, result)
+            elif flats:
                 w = normalized_weights(counts if self.args.weighted else None, len(flats), device=self.device)
                 th = theta.to(self.device)
                 if codec.quantized or codec.sparse:
@@ -498,14 +515,87 @@ class Coordinator(BusClient):
                     self._server_update(th, torch.stack(flats).to(self.device), w)
                 theta = th.cpu()
                 self._average_buffers(model, [getattr(alive.get(wid), "last_buffers", None) for wid in ids], w.cpu())
-            # traffic of this round: model + fit config towards the devices, trained model + loss back (paper §4.3)
-            self.metrics.end_round(r, time.time() - t0, selected=ids, n_k=counts, bytes_out=bytes_out, bytes_in=bytes_in)
+            # traffic of this round: model + fit config towards the devices, trained model + loss back (paper §4.3), and the
+            # unmask exchange of secure aggregation
+            bytes_out = sum(traffic(w)[0] - sent0[wid][0] for wid, w in to_train.items() if wid in sent0)
+            bytes_in = sum(traffic(w)[1] - sent0[wid][1] for wid, w in to_train.items() if wid in sent0)
+            self.metrics.end_round(r, time.time() - t0, selected=ids, n_k=counts, bytes_out=bytes_out, bytes_in=bytes_in, **secagg_rec)
             result["bytes_out"] = result.get("bytes_out", 0) + bytes_out
             result["bytes_in"] = result.get("bytes_in", 0) + bytes_in
             self._maybe_checkpoint(model, theta, r, {"workers": list(to_train.keys()), "mode": "remote"})
             if not alive:
                 break
         return theta
+
+    async def _secagg_setup(self, alive, tag: str, loop, pool, result) -> Optional[Dict[str, Any]]:
+        """Secure aggregation's key agreement: every device returns a fresh public key for the training ``tag``, then every
+        device that did gets the key list in setup order and derives its pair seeds.  A device that fails either step leaves
+        the training.  Returns ``{"tag", "order", "clip", "frac_bits"}`` (``frac_bits`` for the devices left, see
+        :func:`fl.secagg.frac_bits`), or None when fewer than two are left."""
+        clip = self.args.secagg_clip_value()
+        traffic = lambda w: (getattr(w, "bytes_sent", 0), getattr(w, "bytes_received", 0))  # noqa: E731
+        before = {wid: traffic(w) for wid, w in alive.items()}
+        handles = dict(alive)
+
+        async def call(wid, fn):
+            try:
+                return wid, await loop.run_in_executor(pool, fn)
+            except Exception as e:  # noqa: BLE001 - a failing device leaves the training, the others go on
+                log.info("Worker %s failed the secure-aggregation setup: %r", wid, e)
+                result["dropped"].append(wid)
+                alive.pop(wid, None)
+                return wid, None
+
+        keys = await asyncio.gather(*[call(wid, lambda w=w: pk_to_bytes(pk_from_bytes(w.secagg_setup(tag, timeout=self.fit_timeout))))
+                                      for wid, w in alive.items()])
+        ids = [wid for wid, pk in keys if pk is not None]
+        pks = [pk for _, pk in keys if pk is not None]
+        await asyncio.gather(*[call(wid, lambda w=alive[wid]: w.secagg_peers(tag, ids, pks, timeout=self.fit_timeout)) for wid in ids])
+        result["secagg_setup_bytes_out"] = sum(traffic(w)[0] - before[wid][0] for wid, w in handles.items())
+        result["secagg_setup_bytes_in"] = sum(traffic(w)[1] - before[wid][1] for wid, w in handles.items())
+        if len(alive) < 2:
+            log.info("Secure aggregation needs at least two devices, %d left after the setup: no rounds", len(alive))
+            return None
+        f = frac_bits(clip, len(alive))
+        result["secagg_frac_bits"] = f
+        return {"tag": tag, "order": list(ids), "clip": clip, "frac_bits": f}
+
+    async def _secagg_round(self, theta, r: int, u1: List[str], ids: List[str], replies, alive, sa, loop, pool, result):
+        """Unmask and apply round ``r`` of secure aggregation.  ``replies``: the checked masked replies of the devices ``ids``
+        (the survivors U2); the others of ``u1`` dropped (D).  Every survivor is asked for its self seed and its pair seeds with
+        the dropped devices; if fewer than two survived or one of them does not answer, the round is abandoned (theta
+        unchanged, a device that did not answer leaves the training).  Returns ``(theta, the round's secagg record)``."""
+        got = dict(zip(ids, replies))
+        survivors = [w for w in u1 if w in got]
+        dropped = [w for w in u1 if w not in got]
+        rec = {"secagg_u2": len(survivors), "secagg_dropped": len(dropped), "secagg_clipped": sum(got[w][1] for w in survivors),
+               "secagg_nonfinite": sum(got[w][2] for w in survivors), "secagg_abandoned": True}
+        if len(survivors) < 2:
+            log.info("Secure aggregation round %d abandoned: %d device(s) survived", r, len(survivors))
+            return theta, rec
+
+        async def ask(wid):
+            try:
+                resp = await loop.run_in_executor(pool, lambda: alive[wid].secagg_unmask(sa["tag"], r, survivors, timeout=self.fit_timeout))
+                return wid, check_unmask_reply(resp, dropped)
+            except Exception as e:  # noqa: BLE001 - a device that does not answer abandons the round
+                log.info("Worker %s failed the unmask of round %d: %r", wid, r, e)
+                return wid, None
+
+        answers = await asyncio.gather(*[ask(w) for w in survivors])
+        failed = [w for w, a in answers if a is None]
+        if failed:
+            log.info("Secure aggregation round %d abandoned: no seeds from %s", r, failed)
+            for w in failed:
+                result["dropped"].append(w)
+                alive.pop(w, None)
+            return theta, rec
+        keys, signs = correction_streams(sa["order"], survivors, dropped, dict(answers))
+        masked = torch.from_numpy(np.stack([got[w][0] for w in survivors]).view(np.int32))
+        th = theta.to(self.device)
+        self._server_update(th, None, None, secagg=(masked.to(self.device), keys, signs, sa["frac_bits"], len(survivors)))
+        rec["secagg_abandoned"] = False
+        return th.cpu(), rec
 
     @staticmethod
     def _downlink_fields(down: UplinkCodec, theta: torch.Tensor, replica: torch.Tensor, nonce: str, r: int, seed: int) -> Dict[str, Any]:
@@ -522,13 +612,17 @@ class Coordinator(BusClient):
         fields[names[1]] = b.cpu().numpy().astype("<f4").tobytes()
         return fields
 
-    def _server_update(self, theta: torch.Tensor, models: Optional[torch.Tensor], weights: torch.Tensor, uplink=None) -> None:
+    def _server_update(self, theta: torch.Tensor, models: Optional[torch.Tensor], weights: torch.Tensor, uplink=None, secagg=None) -> None:
         """FedAvg of ``models`` into ``theta`` in place (or their median / trimmed mean, ``--aggregator``), followed by the
         server optimizer step of ``--server-opt``.  ``uplink = (payload, scales, codec)``: the clients' quantized deltas
         instead of their models (``ops.fedavg_apply_quantized``; ``models`` is not used); ``(indices, values, codec)`` with a
-        topk codec: their sparse deltas (``ops.fedavg_apply_topk``)."""
+        topk codec: their sparse deltas (``ops.fedavg_apply_topk``).  ``secagg = (masked, keys, signs, frac_bits, n)``: the
+        survivors' masked rows and the correction streams of secure aggregation (``ops.fedavg_apply_secagg``)."""
         agg = self.args.client_aggregator()
-        if uplink is None:
+        if secagg is not None:
+            masked, keys, signs, f, n = secagg
+            apply = lambda **kw: ops.fedavg_apply_secagg(theta, masked, keys, signs, f, n, **kw)  # noqa: E731
+        elif uplink is None:
             apply = lambda **kw: ops.fedavg_apply(theta, models, weights, **kw)  # noqa: E731
         elif uplink[2].sparse:
             indices, values, codec = uplink

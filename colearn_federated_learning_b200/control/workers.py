@@ -31,6 +31,7 @@ import torch
 from ..data import dataset_tensors
 from ..fl.trainer import FitConfig, local_fit
 from ..fl.evaluate import predict as predict_fn
+from ..fl.secagg import SecAggDevice
 from ..fl.uplink import UplinkCodec, check_quantized_reply, check_topk_reply, uplink_key
 from ..models import build_model, num_params
 
@@ -131,6 +132,9 @@ class WorkerServer:
         # compressed downlink: (tag, replica [P]) per architecture, the model as the coordinator last sent it (memory only)
         self._replicas: Dict[str, Tuple[str, torch.Tensor]] = {}
         self._work_lock = threading.Lock()   # fits / predictions share those buffers: one at a time
+        # secure aggregation (fl/secagg.py): key pairs, pair seeds and per-round self seeds per training (memory only)
+        self._secagg = SecAggDevice()
+        self._secagg_lock = threading.Lock()
         outer = self
 
         class Handler(socketserver.BaseRequestHandler):
@@ -189,6 +193,19 @@ class WorkerServer:
             return {"ok": True}
         if op == "search":
             return {"ok": True, "count": len(self.tagged.get(req["tag"], []))}
+        if op in ("secagg_setup", "secagg_unmask"):
+            # secure aggregation (fl/secagg.py): "secagg_setup" with a tag returns this device's public key for the training,
+            # with "ids" / "pks" it takes the key list; "secagg_unmask" reveals one round's seeds for the survivors "u2"
+            try:
+                with self._secagg_lock:
+                    if op == "secagg_unmask":
+                        return {"ok": True, **self._secagg.unmask(req.get("tag"), req.get("t"), req.get("u2"))}
+                    if "pks" in req:
+                        self._secagg.learn_peers(req.get("tag"), req.get("ids"), req.get("pks"))
+                        return {"ok": True}
+                    return {"ok": True, "pk": self._secagg.setup(req.get("tag"))}
+            except ValueError as e:
+                return {"ok": False, "error": f"secure aggregation refused: {e}"}
         if op == "fit":
             cfg = FitConfig.from_dict(req["config"])
             x, y = self.datasets[req.get("dataset_key", "training")]
@@ -201,6 +218,10 @@ class WorkerServer:
             down = UplinkCodec(dkind, k=req.get("downlink_topk")) if dkind == "topk" else UplinkCodec(dkind)
             if down.kind != "fp32" and not isinstance(req.get("replica"), str):
                 return {"ok": False, "error": "a compressed downlink needs the replica's tag"}
+            # "secagg": send the masked fixed-point delta (fl/secagg.py) instead of the model; absent = no secure aggregation
+            sa = req.get("secagg")
+            if sa is not None and (not isinstance(sa, dict) or codec.kind != "fp32"):
+                return {"ok": False, "error": "secure aggregation takes a dict of fields and no uplink codec"}
             with self._work_lock:
                 if down.kind != "fp32" and "replica_base" in req:
                     model, flat, err = self._model_and_arena(cfg.model, None)
@@ -216,6 +237,15 @@ class WorkerServer:
                 spec = getattr(model, "spec", None)
                 if spec is not None and not spec.flatten_input and x.shape[1] != spec.dims[0]:
                     return {"ok": False, "error": f"dataset has {x.shape[1]} features, {cfg.model} wants {spec.dims[0]}"}
+                if sa is not None:
+                    if any(b.is_floating_point() for b in model.buffers()):
+                        return {"ok": False, "error": f"secure aggregation refused: {cfg.model}'s floating-point buffers would travel in the clear"}
+                    try:
+                        with self._secagg_lock:
+                            sa_keys, sa_signs = self._secagg.begin_round(sa.get("tag"), sa.get("t"), sa.get("u1"), sa.get("clip"),
+                                                                         sa.get("frac_bits"))
+                    except ValueError as e:
+                        return {"ok": False, "error": f"secure aggregation refused: {e}"}
                 replica = None
                 if down.kind != "fp32":
                     if "replica_base" in req:             # round t >= 1: advance the replica by the wire, train from it
@@ -226,13 +256,19 @@ class WorkerServer:
                     else:                                 # round 0: the fp32 model is the replica
                         replica = flat.clone()
                     self._replicas[cfg.model] = (str(req.get("replica")), replica)
-                received = flat.clone() if codec.quantized or codec.sparse else None   # the theta the coordinator decodes against
+                # the theta the coordinator decodes against
+                received = flat.clone() if codec.quantized or codec.sparse or sa is not None else None
                 from ..utils.threads import small_model_threads
                 with small_model_threads(flat.numel(), flat.device):   # tiny models on a CPU device: no OpenMP fork/join
                     loss, path = local_fit(flat, model, x, y, cfg, round_idx=self._round)
                 self._round += 1
                 self.fits_served += 1
-                if codec.quantized:
+                if sa is not None:
+                    from .. import ops
+                    masked, clipped, nonfinite = ops.secagg_mask(flat, received, sa_keys, sa_signs, sa["clip"], sa["frac_bits"])
+                    reply = {"ok": True, "secagg": "masked", "masked": masked.cpu().numpy().astype("<u4").tobytes(), "clipped": clipped,
+                             "nonfinite": nonfinite, "loss": float(loss), "n": int(x.shape[0]), "path": path}
+                elif codec.quantized:
                     from .. import ops
                     payload, scales = ops.encode_delta(flat.unsqueeze(0), received, codec, [uplink_key(self.id, cfg.seed)])
                     reply = {"ok": True, "uplink": codec.kind, "payload": payload.cpu().numpy().tobytes(), "scales": _to_bytes(scales),
@@ -402,6 +438,34 @@ class RemoteWorkerClient:
         if downlink is not None:
             update["replica_crc"] = resp.get("replica_crc")
         return update, float(resp["loss"]), int(resp["n"])
+
+    def fit_secagg(self, flat: torch.Tensor, cfg: FitConfig, fields: Dict[str, Any], dataset_key: str = "training",
+                   timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None) -> Tuple[Dict[str, Any], float, int]:
+        """:meth:`fit` asking the device for its masked update (secure aggregation, ``fields`` = the round's ``{"tag", "t",
+        "u1", "clip", "frac_bits"}``): returns the reply's ``{"secagg", "masked", "clipped", "nonfinite"}`` (and
+        ``"replica_crc"`` with a ``downlink``) unchecked (it is untrusted input: the coordinator validates it), the loss and the
+        sample count."""
+        req = self._fit_request(flat, cfg, dataset_key, downlink)
+        req["secagg"] = fields
+        resp = self._call({**req, **(downlink or {})}, timeout=timeout)
+        self.last_buffers = None
+        update = {k: resp.get(k) for k in ("secagg", "masked", "clipped", "nonfinite")}
+        if downlink is not None:
+            update["replica_crc"] = resp.get("replica_crc")
+        return update, float(resp["loss"]), int(resp["n"])
+
+    def secagg_setup(self, tag: str, timeout: Optional[float] = None) -> Any:
+        """The device's public key for the training ``tag`` (unchecked bytes)"""
+        return self._call({"op": "secagg_setup", "tag": tag}, timeout=timeout).get("pk")
+
+    def secagg_peers(self, tag: str, ids: List[str], pks: List[bytes], timeout: Optional[float] = None) -> None:
+        """The training's key list in setup order: the device derives its pair seeds"""
+        self._call({"op": "secagg_setup", "tag": tag, "ids": ids, "pks": pks}, timeout=timeout)
+
+    def secagg_unmask(self, tag: str, t: int, survivors: List[str], timeout: Optional[float] = None) -> Dict[str, Any]:
+        """Round ``t``'s seeds for the survivor list: the reply ``{"self_seed", "pair_seeds"}`` unchecked"""
+        resp = self._call({"op": "secagg_unmask", "tag": tag, "t": t, "u2": survivors}, timeout=timeout)
+        return {k: resp.get(k) for k in ("self_seed", "pair_seeds")}
 
     def search(self, tag: str) -> int:
         return int(self._call({"op": "search", "tag": tag}).get("count", 0))

@@ -4,8 +4,10 @@ There is deliberately no silent GPU fallback: a CUDA tensor with the extension m
 """
 from __future__ import annotations
 
+import math
 from typing import Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import reference
@@ -203,6 +205,63 @@ def apply_downlink(replica: torch.Tensor, a: torch.Tensor, b: torch.Tensor, code
                                               codec.k)
         return replica
     return reference.apply_downlink(replica, a, b, codec)
+
+
+def secagg_key_words(keys, device=None) -> torch.Tensor:
+    """int32 ``[S, 8]`` (the little-endian words, as the kernels take them) of ``S`` 32-byte stream keys"""
+    return torch.from_numpy(reference._key_words(keys).view(np.int32).copy()).to(device)
+
+
+def _secagg_streams_args(keys, signs, device):
+    kw = keys.to(device, torch.int32).contiguous() if isinstance(keys, torch.Tensor) else secagg_key_words(keys, device)
+    sg = torch.as_tensor(signs.cpu() if isinstance(signs, torch.Tensor) else list(signs), dtype=torch.int32).reshape(-1)
+    if sg.numel() != kw.shape[0] or not bool(((sg == 1) | (sg == -1)).all()):
+        raise ValueError("one sign (+1 / -1) per stream key")
+    return kw, sg.to(device)
+
+
+def secagg_mask(model: torch.Tensor, theta: torch.Tensor, keys, signs, clip: float, frac_bits: int) -> Tuple[torch.Tensor, int, int]:
+    """A device's masked update for secure aggregation (``ops/csrc/secagg.cuh``, ``fl/secagg.py``): ``(y uint32 [P], clipped,
+    nonfinite)`` with ``y = enc(model - theta) + sum_s signs[s] PRG(keys[s])`` (mod 2^32), ``enc`` the fixed-point code with
+    clip ``clip`` and ``frac_bits`` fraction bits, ``keys`` 32-byte ChaCha20 keys (or their ``[S, 8]`` int32 words) and
+    ``signs`` +1 / -1.  CUDA tensors: ``secagg_mask_kernel`` in one launch; CPU tensors: ``reference.secagg_mask``."""
+    if not (math.isfinite(clip) and clip > 0):
+        raise ValueError(f"the clip must be finite and > 0, not {clip}")
+    if _cuda(theta):
+        kw, sg = _secagg_streams_args(keys, signs, theta.device)
+        out, counts = _ext.require().secagg_mask(model.to(theta.device, torch.float32).contiguous().view(-1),
+                                                 theta.float().contiguous().view(-1), kw, sg, float(clip), int(frac_bits))
+        c = counts.tolist()
+        return out.view(torch.uint32), int(c[0]), int(c[1])
+    return reference.secagg_mask(model, theta, keys, signs, clip, frac_bits)
+
+
+def fedavg_apply_secagg(theta: torch.Tensor, masked: torch.Tensor, keys, signs, frac_bits: int, n: int, server_lr: float = 1.0,
+                        opt=None, aggregator=None) -> torch.Tensor:
+    """Secure aggregation's unmask + decode + FedAvg apply in place: ``z = sum_k masked[k] + sum_s signs[s] PRG(keys[s])``
+    (mod 2^32; the correction streams are the survivors' self masks and the pair masks of the dropped devices, negated),
+    ``mean = (float)(int32)z 2^-frac_bits / n``, ``a = theta + mean``, then ``theta += server_lr (a - theta)`` or the server
+    optimizer step of ``opt`` (as in :func:`fedavg_apply`).  ``masked``: uint32 (or int32 with the same bits) ``[K, P]``.  A
+    robust ``aggregator`` is refused: only a sum survives the masks.  CUDA tensors: ``fedavg_secagg_kernel`` (after
+    ``secagg_streams_kernel`` when the streams are split); CPU tensors: ``reference.fedavg_apply_secagg``."""
+    if aggregator is not None and aggregator.robust:
+        raise ValueError(f"aggregator {aggregator.kind!r} does not apply to secure aggregation: the coordinator only learns the sum")
+    if opt is not None and float(server_lr) != 1.0:
+        raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
+    if int(n) < 1:
+        raise ValueError("the mean needs n >= 1 survivors")
+    if _cuda(theta):
+        dev = theta.device
+        kw, sg = _secagg_streams_args(keys, signs, dev)
+        rows = masked.to(dev).contiguous().view(torch.int32).reshape(-1, theta.numel())
+        args = [theta, rows, kw, sg, int(frac_bits), int(n)]
+        if opt is not None:
+            args += [float(opt.lr), opt.code, opt.hyper, opt.m, opt.v]
+        else:
+            args += [float(server_lr)]
+        _ext.require().fedavg_apply_secagg(*args)
+        return theta
+    return reference.fedavg_apply_secagg(theta, masked, keys, signs, frac_bits, n, server_lr, opt=opt)
 
 
 def sigmoid_bce(z: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:

@@ -309,6 +309,57 @@ void replica_apply_topk(torch::Tensor replica, torch::Tensor indices, torch::Ten
                                   cur_stream()), "replica_apply_topk");
 }
 
+// ---- secure aggregation (secagg.cuh) ------------------------------------------------------------------------------------------
+// keys: int32 [S, 8] (the little-endian words of the 32-byte stream keys), signs: int32 [S]
+static void check_secagg_streams(const torch::Tensor& keys, const torch::Tensor& signs, const torch::Tensor& like) {
+  TORCH_CHECK(keys.is_cuda() && keys.scalar_type() == at::kInt && keys.is_contiguous() && keys.dim() == 2 && keys.size(1) == 8 &&
+              keys.device() == like.device(), "keys: contiguous CUDA int32 [S, 8] on theta's device");
+  TORCH_CHECK(signs.is_cuda() && signs.scalar_type() == at::kInt && signs.is_contiguous() && signs.numel() == keys.size(0) &&
+              signs.device() == like.device(), "signs: contiguous CUDA int32 [S] on theta's device");
+}
+
+// (masked int32 [P] holding the uint32 words, counts int32 [2] = clipped / non-finite) of model [P] - theta [P]
+std::vector<torch::Tensor> secagg_mask(torch::Tensor model, torch::Tensor theta, torch::Tensor keys, torch::Tensor signs, double clip,
+                                       int64_t frac_bits) {
+  CHECK_CUDA_F32(model); CHECK_CUDA_F32(theta);
+  TORCH_CHECK(model.numel() == theta.numel() && model.device() == theta.device(), "model / theta [P], one device");
+  check_secagg_streams(keys, signs, theta);
+  c10::cuda::CUDAGuard guard(theta.device());
+  const int64_t n = theta.numel();
+  auto out = torch::empty({n}, theta.options().dtype(at::kInt));
+  auto counts = torch::empty({2}, theta.options().dtype(at::kInt));
+  check(launch_secagg_mask(model.data_ptr<float>(), theta.data_ptr<float>(), reinterpret_cast<const uint32_t*>(keys.data_ptr<int>()),
+                           signs.data_ptr<int>(), (int)keys.size(0), (float)clip, (int)frac_bits,
+                           reinterpret_cast<uint32_t*>(out.data_ptr<int>()), counts.data_ptr<int>(), n, cur_stream()), "secagg_mask");
+  return {out, counts};
+}
+
+// theta += step towards theta + decode(sum of the K masked rows + the signed streams) / n_mean; masked int32 [K, >= P] (uint32
+// words); the server optimizer arguments as in fedavg_apply
+void fedavg_apply_secagg(torch::Tensor theta, torch::Tensor masked, torch::Tensor keys, torch::Tensor signs, int64_t frac_bits, int64_t n_mean,
+                         double server_lr, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<torch::Tensor> m,
+                         c10::optional<torch::Tensor> v) {
+  CHECK_CUDA_F32(theta);
+  const int64_t n = theta.numel();
+  TORCH_CHECK(masked.is_cuda() && masked.scalar_type() == at::kInt && masked.dim() == 2 && masked.stride(1) == 1 && masked.size(1) >= n &&
+              masked.device() == theta.device(), "masked: CUDA int32 [K, >= P] with unit column stride on theta's device");
+  check_secagg_streams(keys, signs, theta);
+  c10::cuda::CUDAGuard guard(theta.device());
+  auto state = [&](const c10::optional<torch::Tensor>& t, const char* name) -> int64_t {
+    if (!t.has_value()) return 0;
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() >= n &&
+                t->device() == theta.device(), name, ": contiguous CUDA float32 with one element per parameter, on theta's device");
+    return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
+  };
+  const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
+  torch::Tensor work;
+  if (sa_streams_per_task(n, (int)keys.size(0)) > 0) work = torch::empty({n}, theta.options().dtype(at::kInt));
+  check(launch_fedavg_apply_secagg(theta.data_ptr<float>(), reinterpret_cast<const uint32_t*>(masked.data_ptr<int>()), masked.stride(0),
+                                   (int)masked.size(0), reinterpret_cast<const uint32_t*>(keys.data_ptr<int>()), signs.data_ptr<int>(),
+                                   (int)keys.size(0), work.defined() ? reinterpret_cast<uint32_t*>(work.data_ptr<int>()) : nullptr,
+                                   (int)frac_bits, (int)n_mean, o, n, cur_stream()), "fedavg_apply_secagg");
+}
+
 torch::Tensor fedavg_flat(torch::Tensor slots, torch::Tensor weights) {
   CHECK_CUDA_F32(slots); CHECK_CUDA_F32(weights);
   TORCH_CHECK(slots.dim() == 2 && weights.numel() == slots.size(0), "shapes");
@@ -810,6 +861,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("weights"),
         py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
         py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
+  m.def("secagg_mask", &secagg_mask);
+  m.def("fedavg_apply_secagg", &fedavg_apply_secagg, py::arg("theta"), py::arg("masked"), py::arg("keys"), py::arg("signs"),
+        py::arg("frac_bits"), py::arg("n_mean"), py::arg("server_lr"), py::arg("opt_kind") = 0,
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);

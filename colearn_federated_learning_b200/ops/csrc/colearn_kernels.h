@@ -47,6 +47,8 @@
 #include "uplink_topk.cuh"
 // replica protocol of the compressed downlink (the same two codecs on theta - replica)
 #include "downlink.cuh"
+// secure aggregation: ChaCha20 mask streams and the fixed-point codec of the masked updates
+#include "secagg.cuh"
 
 namespace colearn {
 // Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
@@ -271,6 +273,16 @@ cudaError_t launch_downlink_topk(const float* theta, float* replica, int topk, u
 cudaError_t launch_replica_apply_quant(float* replica, const uint8_t* payload, int64_t row_bytes, const float* scales, int bits,
                                        int64_t n, cudaStream_t s);
 cudaError_t launch_replica_apply_topk(float* replica, const uint8_t* indices, const float* values, int topk, int64_t n, cudaStream_t s);
+// Secure aggregation (secagg.cuh), rows of n < 2^36 uint32 words; keys [streams][8] uint32 (16-byte aligned), signs [streams]
+// (< 0 subtracts the stream).  Device: out = enc(model - theta) + sum_s signs[s] PRG(keys[s]) with clip and 2^frac_bits, counts[0]
+// / counts[1] = clipped / non-finite deltas (0 <= frac_bits <= 64).  Coordinator: z = sum of the k rows of masked + the streams,
+// theta moves towards theta + sa_decode(z) / n_mean by opt.lr (opt.kind 0) or the server optimizer step; workspace: n uint32
+// of scratch, needed when sa_streams_per_task(n, streams) > 0.
+cudaError_t launch_secagg_mask(const float* model, const float* theta, const uint32_t* keys, const int* signs, int streams, float clip,
+                               int frac_bits, uint32_t* out, int* counts, int64_t n, cudaStream_t s);
+cudaError_t launch_fedavg_apply_secagg(float* theta, const uint32_t* masked, int64_t row_stride, int k, const uint32_t* keys, const int* signs,
+                                       int streams, uint32_t* workspace, int frac_bits, int n_mean, const ServerOptArgs& opt, int64_t n,
+                                       cudaStream_t s);
 // out = sum_k w[k] * slots[k]
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride,
                                const float* weights, int k, int64_t n, cudaStream_t s);

@@ -731,6 +731,144 @@ replica_apply_topk_kernel(float* __restrict__ replica, const uint8_t* __restrict
   }
 }
 
+// ---- secure aggregation (secagg.cuh) ------------------------------------------------------------------------------------------
+// One thread per ChaCha20 column: column c is elements 16 c .. 16 c + 15, block c of every stream.  The 16 uint32 accumulators
+// and one block of state stay in registers; a stream's key is the same for every thread of a launch at a given step (uniform
+// 16-byte loads through the read-only cache: S can run into the thousands, the keys stay in global memory).
+
+// the 16 words of column e0 of a uint32 row (0 past n): four 16-byte loads when `full`, scalar loads otherwise
+template <LdHint HINT>
+__device__ __forceinline__ void sa_load16(const uint32_t* __restrict__ p, int64_t e0, int64_t n, bool full, uint32_t (&x)[kSaWords]) {
+  if (full) {
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      const uint4 v = ld_hint<HINT>(reinterpret_cast<const uint4*>(p + e0) + h);
+      x[4 * h + 0] = v.x; x[4 * h + 1] = v.y; x[4 * h + 2] = v.z; x[4 * h + 3] = v.w;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < kSaWords; ++i) x[i] = e0 + i < n ? p[e0 + i] : 0u;
+  }
+}
+
+// acc += sum over the streams s0 <= s < s1 of signs[s] PRG(keys[s]), block `col`
+__device__ __forceinline__ void sa_add_streams(uint32_t (&acc)[kSaWords], const uint32_t* __restrict__ keys, const int* __restrict__ signs,
+                                               int s0, int s1, uint32_t col) {
+#pragma unroll 1
+  for (int s = s0; s < s1; ++s) {
+    const uint4 lo = __ldg(reinterpret_cast<const uint4*>(keys + 8 * (int64_t)s));
+    const uint4 hi = __ldg(reinterpret_cast<const uint4*>(keys + 8 * (int64_t)s) + 1);
+    const uint32_t k[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    sa_add_block(acc, k, __ldg(signs + s), col);
+  }
+}
+
+// Device: y = enc(model - theta) + sum_s signs[s] PRG(keys[s]) (mod 2^32), and the counts of clipped / non-finite deltas
+// (counts[0] / counts[1], added to: the launcher zeroes them).
+__global__ void __launch_bounds__(256)
+secagg_mask_kernel(const float* __restrict__ model, const float* __restrict__ theta, const uint32_t* __restrict__ keys,
+                   const int* __restrict__ signs, int streams, float clip, float scale, uint32_t* __restrict__ out, int* __restrict__ counts,
+                   int64_t n) {
+  const int64_t cols = (n + kSaWords - 1) / kSaWords;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const bool vec = (((uintptr_t)model | (uintptr_t)theta | (uintptr_t)out) & 15) == 0;
+  int clipped = 0, nonfinite = 0;
+  for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < cols; c += stride) {
+    const int64_t e0 = c * kSaWords;
+    const bool full = vec && e0 + kSaWords <= n;
+    uint32_t acc[kSaWords];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float m[8], t[8];
+      lane_load8<kLdStream>(model, e0 + 8 * h, n, full, m);
+      lane_load8<kLdReadOnly>(theta, e0 + 8 * h, n, full, t);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[8 * h + i] = sa_encode(m[i] - t[i], clip, scale, clipped, nonfinite);
+    }
+    sa_add_streams(acc, keys, signs, 0, streams, (uint32_t)c);
+    if (full) {
+#pragma unroll
+      for (int h = 0; h < 4; ++h)
+        reinterpret_cast<uint4*>(out + e0)[h] = make_uint4(acc[4 * h], acc[4 * h + 1], acc[4 * h + 2], acc[4 * h + 3]);
+    } else {
+#pragma unroll
+      for (int i = 0; i < kSaWords; ++i) {
+        if (e0 + i < n) out[e0 + i] = acc[i];
+      }
+    }
+  }
+  clipped = __reduce_add_sync(0xffffffffu, clipped);
+  nonfinite = __reduce_add_sync(0xffffffffu, nonfinite);
+  if ((threadIdx.x & 31) == 0) {
+    if (clipped) atomicAdd(counts, clipped);
+    if (nonfinite) atomicAdd(counts + 1, nonfinite);
+  }
+}
+
+// Coordinator, split path (sa_streams_per_task > 0): task t = (chunk, column), per streams of the chunk expanded and added
+// into partial[] (zeroed by the launcher) with atomicAdd.  Consecutive threads take consecutive columns of one chunk: the
+// key loads stay uniform.
+__global__ void __launch_bounds__(256)
+secagg_streams_kernel(const uint32_t* __restrict__ keys, const int* __restrict__ signs, int streams, int per, uint32_t* __restrict__ partial,
+                      int64_t n) {
+  const int64_t cols = (n + kSaWords - 1) / kSaWords;
+  const int64_t tasks = cols * ((streams + per - 1) / per);
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < tasks; t += stride) {
+    const int chunk = (int)(t / cols);
+    const int64_t c = t - (int64_t)chunk * cols, e0 = c * kSaWords;
+    const int s0 = chunk * per, s1 = s0 + per < streams ? s0 + per : streams;
+    uint32_t acc[kSaWords];
+#pragma unroll
+    for (int i = 0; i < kSaWords; ++i) acc[i] = 0u;
+    sa_add_streams(acc, keys, signs, s0, s1, (uint32_t)c);
+#pragma unroll
+    for (int i = 0; i < kSaWords; ++i) {
+      if (e0 + i < n) atomicAdd(partial + e0 + i, acc[i]);
+    }
+  }
+}
+
+// Coordinator: z = sum of the k masked rows + the streams (all of them here when partial is null, else their sum from
+// secagg_streams_kernel), mean = sa_decode(z), a = theta + mean, then theta += opt.lr (a - theta) (OPT false) or the server
+// optimizer step (OPT true) through apply8.
+template <bool OPT>
+__global__ void __launch_bounds__(256)
+fedavg_secagg_kernel(float* __restrict__ theta, const uint32_t* __restrict__ masked, int64_t row_stride, int k, const uint32_t* __restrict__ keys,
+                     const int* __restrict__ signs, int streams, const uint32_t* __restrict__ partial, float inv_scale, float n_mean,
+                     ServerOptArgs opt, int64_t n) {
+  const int64_t cols = (n + kSaWords - 1) / kSaWords;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const bool vec_rows = (((uintptr_t)masked | (uintptr_t)partial) & 15) == 0 && (row_stride & 3) == 0;
+  const bool vec = (((uintptr_t)theta | (uintptr_t)opt.m | (uintptr_t)opt.v) & 15) == 0;
+  for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < cols; c += stride) {
+    const int64_t e0 = c * kSaWords;
+    const bool full = vec_rows && e0 + kSaWords <= n;
+    uint32_t acc[kSaWords];
+    if (partial != nullptr) {
+      sa_load16<kLdStream>(partial, e0, n, full, acc);
+    } else {
+#pragma unroll
+      for (int i = 0; i < kSaWords; ++i) acc[i] = 0u;
+      sa_add_streams(acc, keys, signs, 0, streams, (uint32_t)c);
+    }
+#pragma unroll 1
+    for (int r = 0; r < k; ++r) {
+      uint32_t y[kSaWords];
+      sa_load16<kLdStream>(masked + r * row_stride, e0, n, full, y);
+#pragma unroll
+      for (int i = 0; i < kSaWords; ++i) acc[i] += y[i];
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mean[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) mean[i] = sa_decode(acc[8 * h + i], inv_scale, n_mean);
+      apply8<OPT>(theta, e0 + 8 * h, n, vec, mean, opt);
+    }
+  }
+}
+
 // ---- losses ---------------------------------------------------------------------------------------
 __global__ void sigmoid_bce_kernel(const float* __restrict__ z, const float* __restrict__ y,
                                    float* __restrict__ dz, float* __restrict__ loss_out, int64_t n) {
@@ -1181,6 +1319,44 @@ cudaError_t launch_replica_apply_topk(float* replica, const uint8_t* indices, co
   if (topk < 1 || topk > kUtMaxK || n < 1) return cudaErrorInvalidValue;
   COLEARN_LAUNCH(replica_apply_topk_kernel, grid_for_warps(uq_nblk(n)), kThreads, 0, s, replica, indices, values,
                  topk, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_secagg_mask(const float* model, const float* theta, const uint32_t* keys, const int* signs, int streams, float clip,
+                               int frac_bits, uint32_t* out, int* counts, int64_t n, cudaStream_t s) {
+  if (n < 1 || n >= kSaMaxElems || streams < 0 || !(clip > 0.f) || !(clip < INFINITY) || frac_bits < 0 || frac_bits > 64 ||
+      (reinterpret_cast<uintptr_t>(keys) & 15) != 0)
+    return cudaErrorInvalidValue;
+  cudaError_t e = cudaMemsetAsync(counts, 0, 2 * sizeof(int), s);
+  if (e != cudaSuccess) return e;
+  COLEARN_LAUNCH(secagg_mask_kernel, grid_for((n + kSaWords - 1) / kSaWords, 1), kThreads, 0, s, model, theta, keys, signs, streams, clip,
+                 ldexpf(1.f, frac_bits), out, counts, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_fedavg_apply_secagg(float* theta, const uint32_t* masked, int64_t row_stride, int k, const uint32_t* keys, const int* signs,
+                                       int streams, uint32_t* workspace, int frac_bits, int n_mean, const ServerOptArgs& opt, int64_t n,
+                                       cudaStream_t s) {
+  if (k < 1 || n < 1 || n >= kSaMaxElems || row_stride < n || streams < 0 || n_mean < 1 || frac_bits < 0 || frac_bits > 64 ||
+      (reinterpret_cast<uintptr_t>(keys) & 15) != 0 || !server_opt_args_ok(opt))
+    return cudaErrorInvalidValue;
+  const int64_t cols = (n + kSaWords - 1) / kSaWords;
+  const int per = sa_streams_per_task(n, streams);
+  const uint32_t* partial = nullptr;
+  if (per > 0) {
+    if (workspace == nullptr) return cudaErrorInvalidValue;
+    cudaError_t e = cudaMemsetAsync(workspace, 0, (size_t)n * sizeof(uint32_t), s);
+    if (e != cudaSuccess) return e;
+    COLEARN_LAUNCH(secagg_streams_kernel, grid_for(cols * ((streams + per - 1) / per), 1), kThreads, 0, s, keys, signs, streams, per,
+                   workspace, n);
+    partial = workspace;
+  }
+  const float inv_scale = ldexpf(1.f, -frac_bits), nf = (float)n_mean;
+  if (opt.kind == SOPT_SGD) {
+    COLEARN_LAUNCH(fedavg_secagg_kernel<false>, grid_for(cols, 1), kThreads, 0, s, theta, masked, row_stride, k, keys, signs, streams,
+                   partial, inv_scale, nf, opt, n);
+  } else {
+    COLEARN_LAUNCH(fedavg_secagg_kernel<true>, grid_for(cols, 1), kThreads, 0, s, theta, masked, row_stride, k, keys, signs, streams,
+                   partial, inv_scale, nf, opt, n);
+  }
   return cudaGetLastError();
 }
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride, const float* weights,

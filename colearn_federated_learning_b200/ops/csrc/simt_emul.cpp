@@ -237,6 +237,35 @@ void replica_apply_topk(Tensor replica, Tensor indices, Tensor values, int64_t t
   py::gil_scoped_release nogil;
   CK(colearn::launch_replica_apply_topk(r, indices.data_ptr<uint8_t>(), fptr(values, "values"), (int)topk, n, nullptr));
 }
+// secure aggregation (secagg.cuh): same shapes as bindings.cpp::secagg_mask / fedavg_apply_secagg (uint32 words in int32 tensors)
+std::tuple<Tensor, Tensor> secagg_mask(Tensor model, Tensor theta, Tensor keys, Tensor signs, double clip, int64_t frac_bits) {
+  TORCH_CHECK(model.numel() == theta.numel(), "model / theta [P]");
+  TORCH_CHECK(keys.scalar_type() == at::kInt && keys.is_contiguous() && keys.dim() == 2 && keys.size(1) == 8, "keys int32 [S, 8]");
+  TORCH_CHECK(signs.scalar_type() == at::kInt && signs.is_contiguous() && signs.numel() == keys.size(0), "signs int32 [S]");
+  const int64_t n = theta.numel();
+  Tensor out = torch::zeros({n}, torch::kInt), counts = torch::zeros({2}, torch::kInt);
+  {
+    py::gil_scoped_release nogil;
+    CK(colearn::launch_secagg_mask(fptr(model, "model"), fptr(theta, "theta"), reinterpret_cast<const uint32_t*>(keys.data_ptr<int>()),
+                                   signs.data_ptr<int>(), (int)keys.size(0), (float)clip, (int)frac_bits,
+                                   reinterpret_cast<uint32_t*>(out.data_ptr<int>()), counts.data_ptr<int>(), n, nullptr));
+  }
+  return {out, counts};
+}
+void fedavg_apply_secagg(Tensor theta, Tensor masked, Tensor keys, Tensor signs, int64_t frac_bits, int64_t n_mean, double server_lr,
+                         int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v) {
+  const int64_t n = theta.numel();
+  TORCH_CHECK(masked.scalar_type() == at::kInt && masked.dim() == 2 && masked.stride(1) == 1 && masked.size(1) >= n, "masked int32 [K, >= P]");
+  TORCH_CHECK(keys.scalar_type() == at::kInt && keys.is_contiguous() && keys.dim() == 2 && keys.size(1) == 8, "keys int32 [S, 8]");
+  TORCH_CHECK(signs.scalar_type() == at::kInt && signs.is_contiguous() && signs.numel() == keys.size(0), "signs int32 [S]");
+  const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, n);
+  Tensor work = torch::zeros({n}, torch::kInt);
+  float* t = fmut(theta, "theta");
+  py::gil_scoped_release nogil;
+  CK(colearn::launch_fedavg_apply_secagg(t, reinterpret_cast<const uint32_t*>(masked.data_ptr<int>()), masked.stride(0), (int)masked.size(0),
+                                         reinterpret_cast<const uint32_t*>(keys.data_ptr<int>()), signs.data_ptr<int>(), (int)keys.size(0),
+                                         reinterpret_cast<uint32_t*>(work.data_ptr<int>()), (int)frac_bits, (int)n_mean, o, n, nullptr));
+}
 Tensor fedavg_flat(Tensor slots, Tensor w) {
   Tensor out = torch::zeros({slots.size(1)}, torch::kFloat);
   CK(colearn::launch_fedavg_flat(out.data_ptr<float>(), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0), slots.size(1), nullptr));
@@ -546,6 +575,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("w"),
         py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
         py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
+  m.def("secagg_mask", &secagg_mask);
+  m.def("fedavg_apply_secagg", &fedavg_apply_secagg, py::arg("theta"), py::arg("masked"), py::arg("keys"), py::arg("signs"),
+        py::arg("frac_bits"), py::arg("n_mean"), py::arg("server_lr"), py::arg("opt_kind") = 0,
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);

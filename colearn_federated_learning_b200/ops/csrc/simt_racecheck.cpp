@@ -115,6 +115,21 @@ int main() {
     }
     CK(launch_downlink_topk(qtheta.data(), drep.data(), 8, kidx.data(), kvals.data(), qn, nullptr));
     CK(launch_replica_apply_topk(dev_rep.data(), kidx.data(), kvals.data(), 8, qn, nullptr));
+    // secure aggregation: the mask of one row (counts by warp reductions and atomics, partial last column), then the unmask-apply
+    // on the fused path (few streams) and on the split path (many streams: atomicAdd into the scratch row, then the finalize)
+    alignas(16) static uint32_t skeys[40 * 8];
+    std::vector<int> ssigns(40), scounts(2);
+    for (int i = 0; i < 40 * 8; ++i) skeys[i] = (uint32_t)rand() * 2654435761u;
+    for (int i = 0; i < 40; ++i) ssigns[i] = (i & 1) ? -1 : 1;
+    std::vector<uint32_t> smasked(2 * qn), swork(qn);
+    CK(launch_secagg_mask(qmodels.data(), qtheta.data(), skeys, ssigns.data(), 3, 0.5f, 20, smasked.data(), scounts.data(), qn, nullptr));
+    CK(launch_secagg_mask(qmodels.data() + qn, qtheta.data(), skeys, ssigns.data(), 3, 0.5f, 20, smasked.data() + qn, scounts.data(), qn,
+                          nullptr));
+    ServerOptArgs so;
+    memset(&so, 0, sizeof(so));
+    so.lr = 1.f;
+    CK(launch_fedavg_apply_secagg(qtheta.data(), smasked.data(), qn, 2, skeys, ssigns.data(), 4, swork.data(), 20, 2, so, qn, nullptr));
+    CK(launch_fedavg_apply_secagg(qtheta.data(), smasked.data(), qn, 2, skeys, ssigns.data(), 40, swork.data(), 20, 2, so, qn, nullptr));
   }
   printf("elementwise kernels ok\n");
   // ---- comm: star round (with deadline) and two-shot on 3 emulated ranks, reduce_push -------------------------------------------

@@ -484,6 +484,157 @@ def apply_downlink(replica: torch.Tensor, a: torch.Tensor, b: torch.Tensor, code
     return replica.copy_(torch.from_numpy(r).view_as(replica))
 
 
+# ------------------------------------------------------------------------------------------------
+# secure aggregation (ops/csrc/secagg.cuh; fl/secagg.py)
+# ------------------------------------------------------------------------------------------------
+SA_WORDS = 16
+SA_MAX_ELEMS = 1 << 36
+_SIGMA = (0x61707865, 0x3320646E, 0x79622D32, 0x6B206574)
+_DIAG = ((0, 4, 8, 12), (1, 5, 9, 13), (2, 6, 10, 14), (3, 7, 11, 15), (0, 5, 10, 15), (1, 6, 11, 12), (2, 7, 8, 13), (3, 4, 9, 14))
+
+
+def _rotl(x: np.ndarray, r: int) -> np.ndarray:
+    return (x << np.uint32(r)) | (x >> np.uint32(32 - r))
+
+
+def _chacha(keys: np.ndarray, counters: np.ndarray, nonce=(0, 0, 0)) -> np.ndarray:
+    """uint32 ``[S, N, 16]``: the ChaCha20 blocks (RFC 8439 §2.3) of the keys ``[S, 8]`` at the block counters ``[N]``."""
+    S, N = keys.shape[0], counters.size
+    init = [np.full((S, N), c, dtype=np.uint32) for c in _SIGMA]
+    init += [np.repeat(keys[:, i:i + 1].astype(np.uint32), N, axis=1) for i in range(8)]
+    init += [np.repeat(counters.astype(np.uint32)[None, :], S, axis=0)]
+    init += [np.full((S, N), w, dtype=np.uint32) for w in nonce]
+    x = [w.copy() for w in init]
+    for _ in range(10):
+        for a, b, c, d in _DIAG:
+            x[a] += x[b]; x[d] ^= x[a]; x[d] = _rotl(x[d], 16)   # noqa: E702
+            x[c] += x[d]; x[b] ^= x[c]; x[b] = _rotl(x[b], 12)   # noqa: E702
+            x[a] += x[b]; x[d] ^= x[a]; x[d] = _rotl(x[d], 8)    # noqa: E702
+            x[c] += x[d]; x[b] ^= x[c]; x[b] = _rotl(x[b], 7)    # noqa: E702
+    return np.stack([x[i] + init[i] for i in range(16)], axis=2)
+
+
+def _key_words(keys) -> np.ndarray:
+    """uint32 ``[S, 8]`` of 32-byte keys (bytes), or of an int32 / uint32 ``[S, 8]`` tensor / array of their words"""
+    if isinstance(keys, torch.Tensor):
+        return keys.detach().to("cpu").contiguous().view(torch.int32).numpy().view(np.uint32).reshape(-1, 8)
+    if isinstance(keys, np.ndarray):
+        return keys.view(np.uint32).reshape(-1, 8)
+    keys = list(keys)
+    if any(not isinstance(k, (bytes, bytearray)) or len(k) != 32 for k in keys):
+        raise ValueError("stream keys are 32 bytes each")
+    return np.frombuffer(b"".join(keys), dtype="<u4").astype(np.uint32).reshape(-1, 8)
+
+
+def chacha20_blocks(key: bytes, counter: int, count: int, nonce: bytes = bytes(12)) -> np.ndarray:
+    """uint32 ``[count, 16]``: the ChaCha20 blocks ``counter .. counter + count - 1`` of the 32-byte ``key`` and 12-byte
+    ``nonce`` (RFC 8439 §2.3; serialised little-endian they are the keystream of §2.4)."""
+    n = np.frombuffer(bytes(nonce), dtype="<u4")
+    return _chacha(_key_words([bytes(key)]), np.arange(counter, counter + count, dtype=np.uint64).astype(np.uint32), tuple(int(w) for w in n))[0]
+
+
+def secagg_streams(keys, signs, n: int) -> np.ndarray:
+    """uint32 ``[n]``: ``sum_s signs[s] PRG(keys[s])`` (mod 2^32), element ``e`` of a stream being word ``e mod 16`` of its
+    block ``e / 16`` with nonce 0."""
+    kw = _key_words(keys)
+    sg = np.asarray(signs.cpu() if isinstance(signs, torch.Tensor) else signs, dtype=np.int64).reshape(-1)
+    if sg.size != kw.shape[0] or not np.isin(sg, (-1, 1)).all():
+        raise ValueError("one sign (+1 / -1) per stream key")
+    if n >= SA_MAX_ELEMS:
+        raise ValueError("a stream indexes blocks with one uint32 word: P must be below 2^36")
+    cols = (n + SA_WORDS - 1) // SA_WORDS
+    counters = np.arange(cols, dtype=np.uint64).astype(np.uint32)
+    acc = np.zeros(cols * SA_WORDS, dtype=np.uint32)
+    step = max(1, (1 << 21) // max(1, cols))               # streams per chunk: bounded temporaries
+    for s0 in range(0, kw.shape[0], step):
+        blocks = _chacha(kw[s0:s0 + step], counters).reshape(-1, cols * SA_WORDS)
+        neg = sg[s0:s0 + step] < 0
+        acc += blocks[~neg].sum(axis=0, dtype=np.uint32) - blocks[neg].sum(axis=0, dtype=np.uint32)
+    return acc[:n]
+
+
+def secagg_encode(delta: np.ndarray, clip: float, frac_bits: int) -> Tuple[np.ndarray, int, int]:
+    """``(q uint32 [P], clipped, nonfinite)``: the fixed-point codes of float32 deltas (``sa_encode``)."""
+    d = np.asarray(delta, dtype=np.float32).reshape(-1)
+    c32 = np.float32(clip)
+    with np.errstate(invalid="ignore"):
+        nan, inf = np.isnan(d), np.isinf(d)
+        clipped = int((~nan & ~inf & (np.abs(d) > c32)).sum())
+        c = np.where(nan, np.float32(0.0), np.clip(d, -c32, c32)).astype(np.float32)
+    q = np.rint(c * np.float32(2.0 ** frac_bits)).astype(np.int64).astype(np.int32)
+    return q.view(np.uint32), clipped, int(nan.sum() + inf.sum())
+
+
+def secagg_mask(model: torch.Tensor, theta: torch.Tensor, keys, signs, clip: float, frac_bits: int) -> Tuple[torch.Tensor, int, int]:
+    """A device's masked update: ``(y uint32 [P], clipped, nonfinite)`` with ``y = enc(model - theta) + sum_s signs[s]
+    PRG(keys[s])`` (mod 2^32).  Bit for bit what ``secagg_mask_kernel`` writes."""
+    m = model.detach().to("cpu", torch.float32).reshape(-1).numpy()
+    t = theta.detach().to("cpu", torch.float32).reshape(-1).numpy()
+    with np.errstate(invalid="ignore", over="ignore"):
+        q, clipped, nonfinite = secagg_encode(m - t, clip, frac_bits)
+    return torch.from_numpy(q + secagg_streams(keys, signs, q.size)), clipped, nonfinite
+
+
+def secagg_unmask_sum(masked: torch.Tensor, keys, signs) -> np.ndarray:
+    """uint32 ``[P]``: the sum of the masked rows ``[K, P]`` plus the signed correction streams (mod 2^32)."""
+    y = masked.detach().to("cpu").contiguous().view(torch.int32).numpy().view(np.uint32)
+    y = y.reshape(-1, y.shape[-1])
+    return y.sum(axis=0, dtype=np.uint32) + secagg_streams(keys, signs, y.shape[1])
+
+
+def secagg_decode(z: np.ndarray, frac_bits: int, n: int) -> np.ndarray:
+    """float32 mean of ``n`` survivors whose codes sum to ``z`` (``sa_decode``)."""
+    zf = np.asarray(z, dtype=np.uint32).view(np.int32).astype(np.float32)
+    return (zf * np.float32(2.0 ** -frac_bits)) / np.float32(n)
+
+
+def _fmaf(a, b, c) -> np.ndarray:
+    """float32 fused multiply-add: the float32 product is exact in float64, then one float64 add and the float32 rounding"""
+    return (np.float64(a) * np.float64(b) + np.float64(c)).astype(np.float32)
+
+
+def _server_opt_np(t: np.ndarray, a: np.ndarray, opt, server_lr: float) -> np.ndarray:
+    """``server_opt.cuh``'s step of theta towards ``a`` in float32 numpy with its fmaf; the moments of ``opt`` updated in place"""
+    f = np.float32
+    if opt is None or opt.kind == "sgd":
+        return _fmaf(f(server_lr if opt is None else opt.lr), a - t, t)
+    lr = f(opt.lr)
+    b1, b2, tau = (f(h) for h in opt.hyper)
+    d = a - t
+    m = opt.m.detach().cpu().numpy().astype(np.float32)
+    if opt.kind == "avgm":
+        m = _fmaf(b1, m, d)
+        opt.m.copy_(torch.from_numpy(m))
+        return _fmaf(lr, m, t)
+    m = _fmaf(b1, m, (f(1.0) - b1) * d)
+    v = opt.v.detach().cpu().numpy().astype(np.float32)
+    d2 = d * d
+    if opt.kind == "adagrad":
+        v = _fmaf(d, d, v)
+    elif opt.kind == "adam":
+        v = _fmaf(b2, v, (f(1.0) - b2) * d2)
+    elif opt.kind == "yogi":
+        s = np.where(v > d2, f(1.0), np.where(v < d2, f(-1.0), f(0.0)))
+        v = _fmaf(-(f(1.0) - b2) * s, d2, v)
+    else:
+        raise ValueError(f"unknown server optimizer {opt.kind!r}")
+    opt.m.copy_(torch.from_numpy(m))
+    opt.v.copy_(torch.from_numpy(v))
+    return _fmaf(lr, m / (np.sqrt(v) + tau), t)
+
+
+def fedavg_apply_secagg(theta: torch.Tensor, masked: torch.Tensor, keys, signs, frac_bits: int, n: int, server_lr: float = 1.0,
+                        opt=None) -> torch.Tensor:
+    """``mean = secagg_decode(secagg_unmask_sum(masked, keys, signs))``, ``a = theta + mean``, then ``theta += server_lr (a -
+    theta)`` or the server optimizer step of ``opt`` (a ``ServerOptState``), in place; the float32 roundings of
+    ``fedavg_secagg_kernel`` (fmaf where it has one): bit for bit what it writes."""
+    mean = secagg_decode(secagg_unmask_sum(masked, keys, signs), frac_bits, n)
+    t = theta.detach().to("cpu", torch.float32).reshape(-1).numpy()
+    with np.errstate(over="ignore", invalid="ignore"):
+        out = _server_opt_np(t, t + mean, opt, server_lr)
+    return theta.copy_(torch.from_numpy(out).view_as(theta))
+
+
 def linear_bias_relu(x, w, b, relu=True):
     y = x.float() @ w.float().t() + b.float()
     return torch.relu(y) if relu else y

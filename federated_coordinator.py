@@ -72,6 +72,12 @@ def build_parser() -> argparse.ArgumentParser:
                              "encode per round for all devices (needs --uplink-codec int8, int4 or topk; not with --box or -e)")
     parser.add_argument("--downlink-topk", type=int, default=d.downlink_topk,
                         help="--downlink-codec topk: entries sent per block of 256 parameters, in 1..32")
+    parser.add_argument("--secure-agg", action="store_true",
+                        help="remote mode: secure aggregation (Bonawitz et al. 2017): every device sends its delta as pairwise-masked "
+                             "fixed-point words, the coordinator learns only their sum; devices that drop out before replying are "
+                             "tolerated (not with --uplink-codec, a robust --aggregator, --weighted, --box, -e or local mode)")
+    parser.add_argument("--secagg-clip", type=float, default=d.secagg_clip,
+                        help="--secure-agg: every coordinate of a device's delta is clipped to [-C, C] before the fixed-point code (finite, > 0)")
     parser.add_argument("--seed", type=int, default=d.seed)
     parser.add_argument("--log-interval", type=int, default=d.log_interval)
     parser.add_argument("--test-path", type=str, default=d.test_path, help="CSV used by local/encrypted mode and evaluation")
@@ -142,6 +148,9 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.uplink_codec()                  # rejects a topk k outside 1..32 and topk with a robust aggregator
     a.downlink = getattr(ns, "downlink_codec", a.downlink)
     a.downlink_topk = getattr(ns, "downlink_topk", a.downlink_topk)
+    a.secure_agg = bool(getattr(ns, "secure_agg", False))
+    a.secagg_clip = getattr(ns, "secagg_clip", a.secagg_clip)
+    a.secagg_clip_value()             # rejects a bad clip and --secure-agg with an uplink codec, a robust aggregator or --weighted
     a.downlink_codec()                # rejects a topk k outside 1..32 and a compressed downlink with an fp32 uplink
     a.no_cuda, a.backend = ns.no_cuda, ns.backend
     if getattr(ns, "enc_items", None):
@@ -234,6 +243,14 @@ def parse_cli(argv=None) -> argparse.Namespace:
     if ns.downlink_codec != "fp32" and (ns.box or ns.encryption):
         parser.error(f"--downlink-codec {ns.downlink_codec} applies to the local and remote modes only: --box broadcasts fp32 models "
                      "over NVLink and -e exchanges secret shares")
+    if ns.secure_agg:
+        if ns.box or ns.encryption or not ns.remote:
+            parser.error("--secure-agg applies to remote mode (-r) only: in local mode every update is in the coordinator's process "
+                         "anyway, --box trains on the GPUs of one box and -e exchanges secret shares")
+        from colearn_federated_learning_b200.models import build_model
+        if any(b.is_floating_point() for b in build_model(ns.model).buffers()):
+            parser.error(f"--secure-agg does not apply to --model {ns.model}: its floating-point buffers (BatchNorm running "
+                         "statistics) would travel in the clear")
     return ns
 
 
