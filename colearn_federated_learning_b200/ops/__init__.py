@@ -282,7 +282,10 @@ def sse_loss(out: torch.Tensor, y: torch.Tensor, mean: bool = False) -> Tuple[to
 
 
 def softmax_xent(logits: torch.Tensor, labels: torch.Tensor, bf16_grad: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
-    """(mean softmax cross-entropy, dL/dlogits) in one pass (SURVEY K10)."""
+    """(mean softmax cross-entropy, dL/dlogits) in one pass (SURVEY K10).
+
+    The kernel does not check ``labels``: a row whose label is outside ``[0, cols)`` adds nothing to the loss and gets
+    the plain softmax as its gradient, with no error.  The CPU path raises on it."""
     if _cuda(logits):
         loss, dl = _ext.require().softmax_xent(logits.contiguous(), labels.contiguous().long().view(-1), bool(bf16_grad))
         return loss, dl
@@ -306,11 +309,15 @@ def argmax_rows(x: torch.Tensor) -> torch.Tensor:
 
 
 def minmax_scale(x: torch.Tensor) -> torch.Tensor:
-    """Column-wise scale to [0,1] (SURVEY K13; reference ``MinMaxScaler`` ds.py:31-32)."""
+    """Column-wise scale to [0,1] (SURVEY K13; reference ``MinMaxScaler`` ds.py:31-32): ``(x - lo) / (hi - lo)``, a
+    constant column to 0.  NaN entries are left out of a column's min and max, as sklearn's ``MinMaxScaler`` does, and
+    scale to NaN; on both paths.  ``minmax_scale_kernel`` multiplies by ``1 / (hi - lo)`` where this path divides: the
+    two may differ in the last bit (the kernel's maximum can be 1 - 2^-24)."""
     if _cuda(x):
         return _ext.require().minmax_scale(x.contiguous().float())
-    lo = x.min(0).values
-    rng = x.max(0).values - lo
+    nan = torch.isnan(x)
+    lo = torch.where(nan, torch.inf, x).amin(0)
+    rng = torch.where(nan, -torch.inf, x).amax(0) - lo
     rng = torch.where(rng == 0, torch.ones_like(rng), rng)
     return (x - lo) / rng
 

@@ -870,6 +870,10 @@ fedavg_secagg_kernel(float* __restrict__ theta, const uint32_t* __restrict__ mas
 }
 
 // ---- losses ---------------------------------------------------------------------------------------
+// the -100 floor of a BCE log term, as torch.clamp(min=-100) (and F.binary_cross_entropy) apply it: -inf becomes -100 and
+// NaN stays NaN, so a diverged model reports a NaN loss (fmaxf(NaN, -100) would return -100)
+__device__ __forceinline__ float bce_log_floor(float x) { return x < -100.f ? -100.f : x; }
+
 __global__ void sigmoid_bce_kernel(const float* __restrict__ z, const float* __restrict__ y,
                                    float* __restrict__ dz, float* __restrict__ loss_out, int64_t n) {
   __shared__ float scratch[32];
@@ -879,7 +883,7 @@ __global__ void sigmoid_bce_kernel(const float* __restrict__ z, const float* __r
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const float p = 1.f / (1.f + __expf(-z[i]));
     const float t = y[i];
-    const float lp = fmaxf(__logf(p), -100.f), l1p = fmaxf(log1pf(-p), -100.f);
+    const float lp = bce_log_floor(__logf(p)), l1p = bce_log_floor(log1pf(-p));
     acc -= t * lp + (1.f - t) * l1p;
     if (dz) dz[i] = (p - t) * inv_n;
   }
@@ -1016,7 +1020,7 @@ __global__ void eval_binary_kernel(const float* __restrict__ p, const float* __r
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const float q = p[i], t = y[i];
-    const float lp = fmaxf(__logf(q), -100.f), l1p = fmaxf(log1pf(-q), -100.f);
+    const float lp = bce_log_floor(__logf(q)), l1p = bce_log_floor(log1pf(-q));
     acc -= t * lp + (1.f - t) * l1p;
     ok += (rintf(q) == t) ? 1 : 0;
   }
@@ -1024,6 +1028,12 @@ __global__ void eval_binary_kernel(const float* __restrict__ p, const float* __r
   if (threadIdx.x == 0) atomicAdd(loss_sum, acc);
   ok = __reduce_add_sync(0xffffffffu, ok);
   if ((threadIdx.x & 31) == 0 && ok) atomicAdd(correct, ok);
+}
+
+// torch.argmax order: NaN above every number, the lowest index among equals (among NaNs too, which is what keeps the rule
+// across the lanes of the shuffle merge)
+__device__ __forceinline__ bool argmax_takes(float v, int c, float best, int bi) {
+  return isnan(v) ? (!isnan(best) || c < bi) : (v > best || (v == best && c < bi));
 }
 
 __global__ void argmax_rows_kernel(const float* __restrict__ x, int64_t* __restrict__ out, int rows, int cols) {
@@ -1034,13 +1044,13 @@ __global__ void argmax_rows_kernel(const float* __restrict__ x, int64_t* __restr
     int bi = 0x7fffffff;
     for (int c = lane; c < cols; c += 32) {
       const float v = x[(size_t)r * cols + c];
-      if (v > best || (v == best && c < bi)) { best = v; bi = c; }
+      if (argmax_takes(v, c, best, bi)) { best = v; bi = c; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       const float ov = __shfl_xor_sync(0xffffffffu, best, o);
       const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+      if (argmax_takes(ov, oi, best, bi)) { best = ov; bi = oi; }
     }
     if (lane == 0) out[r] = bi;
   }
