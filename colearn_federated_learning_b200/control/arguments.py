@@ -38,8 +38,12 @@ class Arguments:
     server_beta1: float = 0.9
     server_beta2: float = 0.99
     server_tau: float = 1e-3
-    aggregator: str = "mean"       # mean (weighted FedAvg) | median | trimmed_mean (fl/aggregate.py; unweighted, Byzantine-robust)
+    aggregator: str = "mean"       # mean (weighted FedAvg) | median | trimmed_mean (coordinate-wise, unweighted) | geomed | norm_clip
+                                   # (distance-based, weighted; fl/aggregate.py)
     trim_fraction: float = 0.1     # trimmed_mean: fraction of the values dropped at each end, in [0, 0.5)
+    geomed_iters: int = 3          # geomed: smoothed Weiszfeld steps, in 1..16
+    geomed_eps: float = 1e-6       # geomed: distance floor nu of the weights alpha_k / max(nu, d_k), finite and > 0
+    clip_norm: float = 0.0         # norm_clip: L2 bound tau of every update (finite, > 0; required with norm_clip)
     uplink: str = "fp32"           # what a device sends back after a fit: fp32 (its model) | int8 | int4 (its quantized delta) |
                                    # topk (the largest entries of its delta, with error feedback; fl/uplink.py)
     uplink_topk: int = 8           # topk: entries kept per block of 256 parameters, in 1..32
@@ -63,10 +67,12 @@ class Arguments:
         return ServerOpt(self.server_opt, lr=self.server_lr, beta1=self.server_beta1, beta2=self.server_beta2, tau=self.server_tau)
 
     def client_aggregator(self):
-        """The :class:`fl.aggregate.Aggregator` these arguments describe; a robust kind refuses ``weighted`` (it is unweighted)."""
+        """The :class:`fl.aggregate.Aggregator` these arguments describe; a coordinate-wise kind refuses ``weighted`` (it is
+        unweighted), the distance-based kinds take it."""
         from ..fl.aggregate import Aggregator
-        agg = Aggregator(self.aggregator, self.trim_fraction)
-        if agg.robust and self.weighted:
+        clip = self.clip_norm if self.aggregator == "norm_clip" else None
+        agg = Aggregator(self.aggregator, self.trim_fraction, iters=self.geomed_iters, eps=self.geomed_eps, clip_norm=clip)
+        if agg.coordinate_wise and self.weighted:
             raise ValueError(f"--weighted does not apply to aggregator {self.aggregator!r}: the median / trimmed mean are unweighted")
         return agg
 
@@ -75,8 +81,12 @@ class Arguments:
         median of sparse deltas is 0 wherever fewer than half the devices sent that coordinate)."""
         from ..fl.uplink import UplinkCodec
         codec = UplinkCodec(self.uplink, k=self.uplink_topk)
-        if codec.sparse and self.client_aggregator().robust:
+        agg = self.client_aggregator()
+        if codec.sparse and agg.coordinate_wise:
             raise ValueError(f"--uplink-codec topk does not combine with --aggregator {self.aggregator}: only the mean of sparse deltas keeps the update")
+        if codec.sparse and agg.distance_based:
+            raise ValueError(f"--uplink-codec topk does not combine with --aggregator {self.aggregator}: the distances of sparse "
+                             "deltas would measure which entries the codec kept, not how far a device moved")
         return codec
 
     def downlink_codec(self):
@@ -98,8 +108,12 @@ class Arguments:
             return clip
         if self.uplink != "fp32":
             raise ValueError(f"--secure-agg does not combine with --uplink-codec {self.uplink}: the masked row is its own encoding")
-        if self.client_aggregator().robust:
+        agg = self.client_aggregator()
+        if agg.coordinate_wise:
             raise ValueError(f"--secure-agg does not combine with --aggregator {self.aggregator}: only the sum of the updates survives the masks")
+        if agg.distance_based:
+            raise ValueError(f"--secure-agg does not combine with --aggregator {self.aggregator}: the per-device distances it weighs by "
+                             "are hidden by the masks")
         if self.weighted:
             raise ValueError("--secure-agg does not combine with --weighted: the masked sum gives the unweighted mean")
         return clip

@@ -328,13 +328,14 @@ class Coordinator(BusClient):
                 ops.encode_downlink(theta, replica, down, downlink_key(cfg.seed + r))
             flats, losses, counts = train_virtual_workers(replica, model, fed, cfg, r)
             live = [i for i, c in enumerate(counts) if c > 0]
+            agg_w = None
             if live:
                 w = normalized_weights([counts[i] for i in live] if self.args.weighted else None, len(live), device=self.device)
                 if codec.quantized:
                     # every worker's delta through the uplink codec (one batched encode), as a device would send it
                     keys = [uplink_key(fed.workers[i], cfg.seed + r) for i in live]
                     payload, scales = ops.encode_delta(flats[live], replica, codec, keys)
-                    self._server_update(theta, None, w, uplink=(payload, scales, codec))
+                    agg_w = self._server_update(theta, None, w, uplink=(payload, scales, codec))
                 elif codec.sparse:
                     # the live workers' deltas plus residuals through the top-k encode (one batched launch); a worker that
                     # did not train this round keeps its residual
@@ -344,11 +345,17 @@ class Coordinator(BusClient):
                         residual[live] = res
                     self._server_update(theta, None, w, uplink=(indices, values, codec))
                 else:
-                    self._server_update(theta, flats[live].contiguous(), w)
+                    agg_w = self._server_update(theta, flats[live].contiguous(), w)
             for wid, l in zip(fed.workers, losses):
                 self.metrics.worker_loss(wid, l)
                 result["losses"][wid] = l
-            self.metrics.end_round(r, time.time() - t0, selected=fed.workers, n_k=counts, loss_k=losses)
+            rec = {}
+            if agg_w is not None:
+                # distance-based aggregator: the final weight of every worker in the order of `selected` (0: excluded or not trained)
+                rec["agg_weights"] = [0.0] * len(fed.workers)
+                for j, i in enumerate(live):
+                    rec["agg_weights"][i] = agg_w[j]
+            self.metrics.end_round(r, time.time() - t0, selected=fed.workers, n_k=counts, loss_k=losses, **rec)
             self._maybe_checkpoint(model, theta, r, {"workers": fed.workers, "mode": "local"})
         log.info("End training")
         unflatten_params(model, theta)
@@ -503,6 +510,7 @@ class Coordinator(BusClient):
                     result["dropped"].append(wid)
                     alive.pop(wid, None)
             secagg_rec = {}
+            agg_rec = {}
             if sa is not None:
                 theta, secagg_rec = await self._secagg_round(theta, r, u1, ids, flats, alive, sa, loop, pool, result)
             elif flats:
@@ -510,16 +518,19 @@ class Coordinator(BusClient):
                 th = theta.to(self.device)
                 if codec.quantized or codec.sparse:
                     uplink = (torch.stack([p for p, _ in flats]).to(self.device), torch.stack([s for _, s in flats]).to(self.device), codec)
-                    self._server_update(th, None, w, uplink=uplink)
+                    agg_w = self._server_update(th, None, w, uplink=uplink)
                 else:
-                    self._server_update(th, torch.stack(flats).to(self.device), w)
+                    agg_w = self._server_update(th, torch.stack(flats).to(self.device), w)
+                if agg_w is not None:
+                    agg_rec["agg_weights"] = agg_w       # the final weight of every device in `ids` (distance-based aggregator)
                 theta = th.cpu()
                 self._average_buffers(model, [getattr(alive.get(wid), "last_buffers", None) for wid in ids], w.cpu())
             # traffic of this round: model + fit config towards the devices, trained model + loss back (paper §4.3), and the
             # unmask exchange of secure aggregation
             bytes_out = sum(traffic(w)[0] - sent0[wid][0] for wid, w in to_train.items() if wid in sent0)
             bytes_in = sum(traffic(w)[1] - sent0[wid][1] for wid, w in to_train.items() if wid in sent0)
-            self.metrics.end_round(r, time.time() - t0, selected=ids, n_k=counts, bytes_out=bytes_out, bytes_in=bytes_in, **secagg_rec)
+            self.metrics.end_round(r, time.time() - t0, selected=ids, n_k=counts, bytes_out=bytes_out, bytes_in=bytes_in, **secagg_rec,
+                                   **agg_rec)
             result["bytes_out"] = result.get("bytes_out", 0) + bytes_out
             result["bytes_in"] = result.get("bytes_in", 0) + bytes_in
             self._maybe_checkpoint(model, theta, r, {"workers": list(to_train.keys()), "mode": "remote"})
@@ -612,27 +623,36 @@ class Coordinator(BusClient):
         fields[names[1]] = b.cpu().numpy().astype("<f4").tobytes()
         return fields
 
-    def _server_update(self, theta: torch.Tensor, models: Optional[torch.Tensor], weights: torch.Tensor, uplink=None, secagg=None) -> None:
-        """FedAvg of ``models`` into ``theta`` in place (or their median / trimmed mean, ``--aggregator``), followed by the
-        server optimizer step of ``--server-opt``.  ``uplink = (payload, scales, codec)``: the clients' quantized deltas
-        instead of their models (``ops.fedavg_apply_quantized``; ``models`` is not used); ``(indices, values, codec)`` with a
-        topk codec: their sparse deltas (``ops.fedavg_apply_topk``).  ``secagg = (masked, keys, signs, frac_bits, n)``: the
-        survivors' masked rows and the correction streams of secure aggregation (``ops.fedavg_apply_secagg``)."""
+    def _server_update(self, theta: torch.Tensor, models: Optional[torch.Tensor], weights: torch.Tensor, uplink=None,
+                       secagg=None) -> Optional[List[float]]:
+        """FedAvg of ``models`` into ``theta`` in place (or their median / trimmed mean / geometric median / norm-bounded mean,
+        ``--aggregator``), followed by the server optimizer step of ``--server-opt``.  ``uplink = (payload, scales, codec)``:
+        the clients' quantized deltas instead of their models (``ops.fedavg_apply_quantized``; ``models`` is not used);
+        ``(indices, values, codec)`` with a topk codec: their sparse deltas (``ops.fedavg_apply_topk``).  ``secagg = (masked,
+        keys, signs, frac_bits, n)``: the survivors' masked rows and the correction streams of secure aggregation
+        (``ops.fedavg_apply_secagg``).  Returns the final weight of every row under a distance-based aggregator (0 for a row
+        it excluded), None otherwise."""
         agg = self.args.client_aggregator()
+        agg_w = None
+        extra = {}
+        if agg.distance_based and secagg is None:
+            k = models.shape[0] if uplink is None else uplink[0].shape[0]
+            agg_w = torch.zeros(k, dtype=torch.float32, device=theta.device)
+            extra = {"agg_weights_out": agg_w}
         if secagg is not None:
             masked, keys, signs, f, n = secagg
             apply = lambda **kw: ops.fedavg_apply_secagg(theta, masked, keys, signs, f, n, **kw)  # noqa: E731
         elif uplink is None:
-            apply = lambda **kw: ops.fedavg_apply(theta, models, weights, **kw)  # noqa: E731
+            apply = lambda **kw: ops.fedavg_apply(theta, models, weights, **kw, **extra)  # noqa: E731
         elif uplink[2].sparse:
             indices, values, codec = uplink
             apply = lambda **kw: ops.fedavg_apply_topk(theta, indices, values, weights, codec, **kw)  # noqa: E731
         else:
             payload, scales, codec = uplink
-            apply = lambda **kw: ops.fedavg_apply_quantized(theta, payload, scales, weights, codec, **kw)  # noqa: E731
+            apply = lambda **kw: ops.fedavg_apply_quantized(theta, payload, scales, weights, codec, **kw, **extra)  # noqa: E731
         if self.args.server_opt == "sgd":
             apply(server_lr=self.args.server_lr, aggregator=agg)
-            return
+            return agg_w.cpu().tolist() if agg_w is not None else None
         opt = self.args.server_optimizer()
         st = self._server_opt_state
         if st is None or st.opt != opt or st.numel != theta.numel():
@@ -643,13 +663,14 @@ class Coordinator(BusClient):
             st.m = st.m.to(theta.device)
             st.v = st.v.to(theta.device) if st.v is not None else None
         apply(opt=st, aggregator=agg)
+        return agg_w.cpu().tolist() if agg_w is not None else None
 
     @staticmethod
     def _average_buffers(model, buffers, weights) -> None:
         """BatchNorm models in remote mode: the devices return their running statistics next to the parameters; the global
         model gets their FedAvg-weighted mean (PySyft's federated_avg averages parameters only — with it the reference could
         not train a BatchNorm model remotely at all; documented in docs/PARITY.md).  They keep this mean under a robust
-        ``--aggregator`` too: only the parameters get the median / trimmed mean."""
+        ``--aggregator`` too: only the parameters get the median / trimmed mean / geometric median / norm-bounded mean."""
         mine = [b for b in model.buffers() if b.is_floating_point()]
         total = sum(b.numel() for b in mine)
         if not mine or any(b is None or b.numel() != total or not bool(torch.isfinite(b).all()) for b in buffers):

@@ -37,33 +37,57 @@ def fedavg_flat(models: torch.Tensor, weights: torch.Tensor) -> torch.Tensor:
     return reference.fedavg_flat(models, weights)
 
 
+def _agg_ext_args(aggregator, weights_out: Optional[torch.Tensor], k: int, device) -> tuple:
+    """the trailing aggregator arguments of the fused FedAvg bindings (none for the mean)"""
+    if aggregator is None or not aggregator.robust:
+        return ()
+    if weights_out is not None and aggregator.distance_based:
+        if weights_out.dtype != torch.float32 or not weights_out.is_contiguous() or weights_out.numel() != k or weights_out.device != device:
+            raise ValueError(f"agg_weights_out must be a contiguous float32 tensor of {k} elements on {device}")
+    else:
+        weights_out = None
+    return (aggregator.code, aggregator.trim, aggregator.iters, aggregator.eps, aggregator.clip, weights_out)
+
+
+def _reference_weights_out(rows: torch.Tensor, weights: torch.Tensor, aggregator, start: torch.Tensor, weights_out) -> None:
+    """CPU path: the final per-row weights of a distance-based aggregator into ``weights_out``"""
+    if weights_out is not None and aggregator is not None and aggregator.distance_based:
+        _, w = reference.distance_aggregate(rows, weights, aggregator, start)
+        weights_out.copy_(w)
+
+
 def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor, server_lr: float = 1.0, opt=None,
-                 aggregator=None) -> torch.Tensor:
+                 aggregator=None, agg_weights_out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``theta += server_lr * (sum_k w_k models[k] - theta)`` in place (reduce + scale + apply fused).
 
     ``opt``: a :class:`fl.server_opt.ServerOptState` — the average is followed by that server optimizer's step (FedAvgM /
     FedAdagrad / FedAdam / FedYogi) in the same kernel, with the optimizer's own ``lr``; its moments are updated in place.
 
     ``aggregator``: a robust :class:`fl.aggregate.Aggregator` (``median`` / ``trimmed_mean``) replaces the weighted sum by
-    the coordinate-wise median / trimmed mean of the K models in the same kernel (``weights`` are then not used)."""
+    the coordinate-wise median / trimmed mean of the K models in the same kernel (``weights`` are then not used).  A
+    distance-based one (``geomed`` / ``norm_clip``, ``ops/csrc/distance_agg.cuh``) reweights the models by their L2 distance
+    from theta (``weights`` are its ``alpha``) in 2 L + 1 launches (``norm_clip``: 3), the last one fused with the step;
+    ``agg_weights_out`` (fp32 ``[K]``, optional) then receives every model's final weight, 0 for an excluded one."""
     robust = aggregator is not None and aggregator.robust
     if opt is not None:
         if float(server_lr) != 1.0:
             raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
         if _cuda(theta):
-            ext_args = (aggregator.code, aggregator.trim) if robust else ()
+            ext_args = _agg_ext_args(aggregator, agg_weights_out, models.shape[0], theta.device)
             _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(opt.lr),
                                         opt.code, opt.hyper, opt.m, opt.v, *ext_args)
             return theta
+        _reference_weights_out(models, weights, aggregator, theta, agg_weights_out)
         b1, b2, tau = opt.hyper
         return reference.server_opt_apply(theta, models, weights, opt.kind, opt.lr, opt.m, opt.v, b1, b2, tau, aggregator=aggregator)
     if _cuda(theta):
         if robust:
             _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(server_lr),
-                                        0, [], None, None, aggregator.code, aggregator.trim)
+                                        0, [], None, None, *_agg_ext_args(aggregator, agg_weights_out, models.shape[0], theta.device))
             return theta
         _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(server_lr))
         return theta
+    _reference_weights_out(models, weights, aggregator, theta, agg_weights_out)
     return reference.fedavg_apply(theta, models, weights, server_lr, aggregator=aggregator)
 
 
@@ -99,11 +123,12 @@ def _aligned_rows(payload: torch.Tensor) -> torch.Tensor:
 
 
 def fedavg_apply_quantized(theta: torch.Tensor, payload: torch.Tensor, scales: torch.Tensor, weights: torch.Tensor, codec,
-                           server_lr: float = 1.0, opt=None, aggregator=None) -> torch.Tensor:
+                           server_lr: float = 1.0, opt=None, aggregator=None, agg_weights_out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """:func:`fedavg_apply` on quantized deltas (``encode_delta``'s output, or the same bytes from the wire): ``a = theta +
     sum_k w_k d^_k`` (or ``theta +`` the robust aggregate of the decoded deltas) and the server step towards ``a``, decode
     fused into the reduce (``fedavg_q_kernel`` / ``fedavg_q_robust_kernel``).  ``opt`` / ``aggregator`` as in
-    :func:`fedavg_apply`.  CPU tensors: ``reference.fedavg_apply_quantized``."""
+    :func:`fedavg_apply`; a distance-based ``aggregator`` measures the decoded deltas from 0 (``fedavg_q`` loaders decode
+    inside every pass), ``agg_weights_out`` as in :func:`fedavg_apply`.  CPU tensors: ``reference.fedavg_apply_quantized``."""
     if not codec.quantized:
         raise ValueError("fedavg_apply_quantized needs an int8 / int4 codec")
     robust = aggregator is not None and aggregator.robust
@@ -111,7 +136,7 @@ def fedavg_apply_quantized(theta: torch.Tensor, payload: torch.Tensor, scales: t
         raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
     if _cuda(theta):
         dev = theta.device
-        if weights is None:                        # (a robust aggregator does not read them)
+        if weights is None:                        # (a coordinate-wise aggregator does not read them)
             weights = torch.full((payload.shape[0],), 1.0 / payload.shape[0])
         args = [theta, _aligned_rows(payload.to(dev)), scales.to(dev, torch.float32).contiguous(),
                 weights.to(dev, torch.float32).contiguous(), codec.bits]
@@ -119,10 +144,12 @@ def fedavg_apply_quantized(theta: torch.Tensor, payload: torch.Tensor, scales: t
             args += [float(opt.lr), opt.code, opt.hyper, opt.m, opt.v]
         else:
             args += [float(server_lr), 0, [], None, None]
-        if robust:
-            args += [aggregator.code, aggregator.trim]
+        args += list(_agg_ext_args(aggregator, agg_weights_out, payload.shape[0], dev))
         _ext.require().fedavg_apply_quantized(*args)
         return theta
+    if agg_weights_out is not None and aggregator is not None and aggregator.distance_based:
+        deltas = reference.decode_delta(payload, scales, codec.bits, theta.numel())
+        _reference_weights_out(deltas, weights, aggregator, torch.zeros(theta.numel()), agg_weights_out)
     return reference.fedavg_apply_quantized(theta, payload, scales, weights, codec.bits, server_lr, opt=opt, aggregator=aggregator)
 
 
@@ -151,8 +178,11 @@ def fedavg_apply_topk(theta: torch.Tensor, indices: torch.Tensor, values: torch.
     would throw the update away.  CPU tensors: ``reference.fedavg_apply_topk``."""
     if not codec.sparse:
         raise ValueError("fedavg_apply_topk needs a topk codec")
-    if aggregator is not None and aggregator.robust:
+    if aggregator is not None and aggregator.coordinate_wise:
         raise ValueError(f"aggregator {aggregator.kind!r} does not apply to top-k sparse deltas: only the (weighted) mean does")
+    if aggregator is not None and aggregator.distance_based:
+        raise ValueError(f"aggregator {aggregator.kind!r} does not apply to top-k sparse deltas: their distances would measure which "
+                         "entries the codec kept, not how far the device moved")
     if opt is not None and float(server_lr) != 1.0:
         raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
     if _cuda(theta):
@@ -244,8 +274,11 @@ def fedavg_apply_secagg(theta: torch.Tensor, masked: torch.Tensor, keys, signs, 
     optimizer step of ``opt`` (as in :func:`fedavg_apply`).  ``masked``: uint32 (or int32 with the same bits) ``[K, P]``.  A
     robust ``aggregator`` is refused: only a sum survives the masks.  CUDA tensors: ``fedavg_secagg_kernel`` (after
     ``secagg_streams_kernel`` when the streams are split); CPU tensors: ``reference.fedavg_apply_secagg``."""
-    if aggregator is not None and aggregator.robust:
+    if aggregator is not None and aggregator.coordinate_wise:
         raise ValueError(f"aggregator {aggregator.kind!r} does not apply to secure aggregation: the coordinator only learns the sum")
+    if aggregator is not None and aggregator.distance_based:
+        raise ValueError(f"aggregator {aggregator.kind!r} does not apply to secure aggregation: the masks hide the per-device distances "
+                         "it weighs by")
     if opt is not None and float(server_lr) != 1.0:
         raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
     if int(n) < 1:

@@ -134,9 +134,33 @@ static AggArgs agg_args(int64_t kind, double trim) {
   return g;
 }
 
+// Distance-based aggregator (distance_agg.cuh): kind 3 = geomed (iters, eps), 4 = norm_clip (clip)
+static bool is_dist_agg(int64_t kind) { return kind == DAGG_GEOMED || kind == DAGG_NORM_CLIP; }
+static DistAggArgs dist_agg_args(int64_t kind, int64_t iters, double eps, double clip) {
+  DistAggArgs g;
+  std::memset(&g, 0, sizeof(g));
+  g.kind = (int)kind;
+  g.iters = (int)iters;
+  g.eps = (float)eps;
+  g.clip = (float)clip;
+  TORCH_CHECK(dist_agg_args_ok(g), "aggregator: kind ", kind, " needs iters in 1..", kDaMaxIters, " and a finite eps > 0 (geomed) or a ",
+              "finite clip > 0 (norm_clip); got iters ", iters, ", eps ", eps, ", clip ", clip);
+  return g;
+}
+// the scratch of one distance-based aggregation from the caching allocator on theta's device, and the weights-out pointer
+static torch::Tensor dist_agg_scratch(const torch::Tensor& theta, int64_t k) {
+  return torch::empty({da_scratch_bytes((int)k, theta.numel())}, theta.options().dtype(at::kByte));
+}
+static float* dist_agg_weights_out(const c10::optional<torch::Tensor>& w, const torch::Tensor& theta, int64_t k) {
+  if (!w.has_value()) return nullptr;
+  TORCH_CHECK(w->is_cuda() && w->scalar_type() == at::kFloat && w->is_contiguous() && w->numel() == k && w->device() == theta.device(),
+              "agg_weights_out: contiguous CUDA float32 [K] on theta's device");
+  return w->data_ptr<float>();
+}
+
 void fedavg_apply(torch::Tensor theta, torch::Tensor slots, torch::Tensor weights, double server_lr, int64_t opt_kind,
                   std::vector<double> opt_hyper, c10::optional<torch::Tensor> m, c10::optional<torch::Tensor> v, int64_t agg_kind,
-                  double trim) {
+                  double trim, int64_t iters, double eps, double clip, c10::optional<torch::Tensor> agg_weights_out) {
   CHECK_CUDA_F32(theta); CHECK_CUDA_F32(slots); CHECK_CUDA_F32(weights);
   TORCH_CHECK(slots.dim() == 2 && slots.size(1) >= theta.numel() && weights.numel() == slots.size(0), "shapes");
   c10::cuda::CUDAGuard guard(theta.device());
@@ -152,6 +176,16 @@ void fedavg_apply(torch::Tensor theta, torch::Tensor slots, torch::Tensor weight
     return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
   };
   const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
+  if (is_dist_agg(agg_kind)) {
+    // weighted distance-based aggregate, then the plain step or the server optimizer step
+    const DistAggArgs g = dist_agg_args(agg_kind, iters, eps, clip);
+    const int64_t k = slots.size(0);
+    auto scratch = dist_agg_scratch(theta, k);
+    check(launch_fedavg_apply_distance(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(), (int)k,
+                                       g, o, theta.numel(), scratch.data_ptr(), dist_agg_weights_out(agg_weights_out, theta, k), 0,
+                                       cur_stream()), "fedavg_apply (distance aggregator)");
+    return;
+  }
   if (agg_kind != AGG_MEAN) {
     // robust aggregate (unweighted: `weights` is not read), then the plain step or the server optimizer step
     check(launch_fedavg_apply_robust(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), (int)slots.size(0),
@@ -185,7 +219,8 @@ std::vector<torch::Tensor> quantize_delta(torch::Tensor models, torch::Tensor th
 // scales fp32 [K, ceil(P / 256)]); the server optimizer / aggregator arguments as in fedavg_apply
 void fedavg_apply_quantized(torch::Tensor theta, torch::Tensor payload, torch::Tensor scales, torch::Tensor weights, int64_t bits,
                             double server_lr, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<torch::Tensor> m,
-                            c10::optional<torch::Tensor> v, int64_t agg_kind, double trim) {
+                            c10::optional<torch::Tensor> v, int64_t agg_kind, double trim, int64_t iters, double eps, double clip,
+                            c10::optional<torch::Tensor> agg_weights_out) {
   CHECK_CUDA_F32(theta); CHECK_CUDA_F32(scales); CHECK_CUDA_F32(weights);
   const int64_t n = theta.numel(), k = payload.size(0);
   TORCH_CHECK(payload.is_cuda() && payload.scalar_type() == at::kByte && payload.dim() == 2 && payload.stride(1) == 1 &&
@@ -201,6 +236,14 @@ void fedavg_apply_quantized(torch::Tensor theta, torch::Tensor payload, torch::T
   };
   const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
   const uint8_t* p = payload.data_ptr<uint8_t>();
+  if (is_dist_agg(agg_kind)) {
+    const DistAggArgs g = dist_agg_args(agg_kind, iters, eps, clip);
+    auto scratch = dist_agg_scratch(theta, k);
+    check(launch_fedavg_apply_quantized_distance(theta.data_ptr<float>(), p, payload.stride(0), scales.data_ptr<float>(), weights.data_ptr<float>(),
+                                                 (int)k, (int)bits, g, o, n, scratch.data_ptr(), dist_agg_weights_out(agg_weights_out, theta, k), 0,
+                                                 cur_stream()), "fedavg_apply_quantized (distance aggregator)");
+    return;
+  }
   if (agg_kind != AGG_MEAN) {
     check(launch_fedavg_apply_quantized_robust(theta.data_ptr<float>(), p, payload.stride(0), scales.data_ptr<float>(), (int)k, (int)bits,
                                                agg_args(agg_kind, trim), o, n, cur_stream()), "fedavg_apply_quantized (robust aggregator)");
@@ -845,10 +888,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mlp_forward", &mlp_forward);
   m.def("sgd_step", &sgd_step);
   // trailing server-optimizer arguments (server_opt.cuh) default to plain FedAvg: the shorter positional calls keep working
-  // trailing aggregator arguments (robust_agg.cuh) default to the weighted mean
+  // trailing aggregator arguments (robust_agg.cuh, distance_agg.cuh) default to the weighted mean
   m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("weights"), py::arg("server_lr"), py::arg("opt_kind") = 0,
         py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
-        py::arg("trim") = 0.0);
+        py::arg("trim") = 0.0, py::arg("iters") = 3,
+        py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none());
   m.def("topk_delta", &topk_delta);
   m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("weights"),
         py::arg("topk"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
@@ -860,7 +904,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("quantize_delta", &quantize_delta);
   m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("weights"),
         py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
-        py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
+        py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0, py::arg("iters") = 3, py::arg("eps") = 1e-6,
+        py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none());
   m.def("secagg_mask", &secagg_mask);
   m.def("fedavg_apply_secagg", &fedavg_apply_secagg, py::arg("theta"), py::arg("masked"), py::arg("keys"), py::arg("signs"),
         py::arg("frac_bits"), py::arg("n_mean"), py::arg("server_lr"), py::arg("opt_kind") = 0,

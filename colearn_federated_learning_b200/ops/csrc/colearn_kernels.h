@@ -47,6 +47,8 @@
 #include "uplink_topk.cuh"
 // replica protocol of the compressed downlink (the same two codecs on theta - replica)
 #include "downlink.cuh"
+// weighted distance-based robust aggregation (geometric median, norm-bounded mean) shared by its passes and the reference
+#include "distance_agg.cuh"
 // secure aggregation: ChaCha20 mask streams and the fixed-point codec of the masked updates
 #include "secagg.cuh"
 
@@ -254,6 +256,17 @@ cudaError_t launch_fedavg_apply_quantized(float* theta, const uint8_t* payload, 
 // a = theta + robust aggregate (robust_agg.cuh) of the k decoded deltas, then the step as above (agg.kind != AGG_MEAN)
 cudaError_t launch_fedavg_apply_quantized_robust(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, int k,
                                                  int bits, const AggArgs& agg, const ServerOptArgs& opt, int64_t n, cudaStream_t s);
+// Distance-based robust aggregation (distance_agg.cuh): the weighted geometric median (g.kind DAGG_GEOMED) or norm-bounded mean
+// (DAGG_NORM_CLIP) of k fp32 model rows (start point theta) or k int8 / int4 delta rows (payload / scales as in
+// launch_fedavg_apply_quantized; start point 0, theta added), with the FedAvg weights alpha = weights[k], then theta += opt.lr (a -
+// theta) (opt.kind 0) or the server optimizer step.  scratch: da_scratch_bytes(k, n) bytes, 16-byte aligned; weights_out (may be
+// null): the final weight of every row (0 for an excluded one).  grid <= 0 picks the grid; the result does not depend on it.
+cudaError_t launch_fedavg_apply_distance(float* theta, const float* rows, int64_t row_stride, const float* weights, int k,
+                                         const DistAggArgs& g, const ServerOptArgs& opt, int64_t n, void* scratch, float* weights_out,
+                                         int grid, cudaStream_t s);
+cudaError_t launch_fedavg_apply_quantized_distance(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales,
+                                                   const float* weights, int k, int bits, const DistAggArgs& g, const ServerOptArgs& opt,
+                                                   int64_t n, void* scratch, float* weights_out, int grid, cudaStream_t s);
 // Top-k uplink (uplink_topk.cuh), 1 <= topk <= 32.  Encode: v = (models[r] - theta) + residual[r] for the rows r < rows;
 // row r of indices / values [rows, entries] receives the kept entries of v (entries >= ut_entries(n, topk)), and residual[r]
 // is overwritten with the unsent part of v.

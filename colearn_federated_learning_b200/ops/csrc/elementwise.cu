@@ -462,6 +462,278 @@ fedavg_q_robust_kernel(float* __restrict__ theta, const uint8_t* __restrict__ pa
   fedavg_robust_body<KMAX>(theta, QSlots<BITS>{payload, row_bytes, scales, uq_nblk(n)}, k, agg, opt, n);
 }
 
+// ---- distance-based robust aggregation (distance_agg.cuh) ---------------------------------------------------------------------
+// Every pass walks the fixed 2048-element chunks grid-stride, one chunk per CTA at a time, lane t holding elements
+// 2048 q + 8 t .. + 7 (the codec kernels' warp-per-256-block layout).  Row loaders: load8<HINT>(k, e0, x) = elements e0 .. e0 + 7
+// of row k, 0 past n (e0 < n); kDelta: the rows are deltas (c^0 = 0, theta added at the end) rather than models (c^0 = theta).
+struct F32Rows {
+  static constexpr bool kDelta = false;
+  const float* p;
+  int64_t stride, n;
+  bool vec;
+  template <LdHint HINT>
+  __device__ __forceinline__ void load8(int k, int64_t e0, float (&x)[8]) const { lane_load8<HINT>(p + k * stride, e0, n, vec, x); }
+};
+template <int BITS>
+struct QRows {
+  static constexpr bool kDelta = true;
+  const uint8_t* payload;
+  int64_t row_bytes;
+  const float* scales;
+  int64_t nblk, n;
+  template <LdHint HINT>
+  __device__ __forceinline__ void load8(int k, int64_t e0, float (&x)[8]) const {
+    const float step = __ldg(scales + k * nblk + (e0 >> 8));
+    int q[8];
+    load_codes8<BITS, HINT>(payload + k * row_bytes, e0, q);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) x[i] = e0 + i < n ? uq_decode(q[i], step) : 0.f;   // codes past n are padding
+  }
+};
+
+__device__ __forceinline__ double warp_tree_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// The per-row chunk sums of one CTA: put(r, s) adds row r's lane values over the warp into red[warp][r % 32]; flush writes rows
+// r0 .. r0 + rows - 1 (rows <= 32) as the warp sums added in warp order.  Every thread of the CTA calls both.
+struct DaRowSums {
+  double (*red)[32];
+  __device__ __forceinline__ void put(int r, double s) const {
+    s = warp_tree_f64(s);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5][r & 31] = s;
+  }
+  __device__ __forceinline__ void flush(int r0, int rows, double* __restrict__ partial, int64_t nchunks, int64_t q) const {
+    __syncthreads();
+    if ((int)threadIdx.x < rows) {
+      double t = red[0][threadIdx.x];
+#pragma unroll
+      for (int w = 1; w < kDaThreads / 32; ++w) t += red[w][threadIdx.x];
+      partial[(int64_t)(r0 + threadIdx.x) * nchunks + q] = t;
+    }
+    __syncthreads();
+  }
+};
+
+// lane's start point c^0: theta (models) or 0 (deltas)
+template <class Rows>
+__device__ __forceinline__ void da_start8(const float* __restrict__ theta, int64_t e0, int64_t n, bool vec, float (&c)[8]) {
+  if constexpr (Rows::kDelta) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) c[i] = 0.f;
+  } else {
+    lane_load8<kLdReadOnly>(theta, e0, n, vec, c);
+  }
+}
+
+// Distance pass of the first step: the chunk sums of (x_k - c^0)^2 for every row
+template <class Rows>
+__global__ void __launch_bounds__(kDaThreads)
+dagg_dist_kernel(Rows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
+  __shared__ double red[kDaThreads / 32][32];
+  const DaRowSums sums{red};
+  const int64_t nchunks = da_chunks(n);
+  const bool vec = ((uintptr_t)theta & 15) == 0 && (n & 3) == 0;
+  for (int64_t q = blockIdx.x; q < nchunks; q += gridDim.x) {
+    const int64_t e0 = q * kDaChunk + threadIdx.x * 8;
+    float c[8];
+    da_start8<Rows>(theta, e0, n, vec, c);
+    for (int r0 = 0; r0 < k; r0 += 32) {
+      const int nr = k - r0 < 32 ? k - r0 : 32;
+      for (int r = 0; r < nr; ++r) {
+        float x[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (e0 < n) rows.template load8<kLdStream>(r0 + r, e0, x);
+        sums.put(r, da_lane_sq8(x, c));
+      }
+      sums.flush(r0, nr, sc.partial, nchunks, q);
+    }
+  }
+}
+
+// A geomed step l < L fused with the next distance pass: the lane forms c^l for its 8 elements from the current weights (c^0
+// when no row is left), then the chunk sums of (x_k - c^l)^2, in one read of the rows.  KMAX > 0: k <= KMAX, the rows' 8 values
+// stay in registers between the two loops; KMAX = 0: any k, the second loop rereads them through L1 / L2.
+template <int KMAX, class Rows>
+__global__ void __launch_bounds__(kDaThreads, 1)
+dagg_center_kernel(Rows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
+  __shared__ double red[kDaThreads / 32][32];
+  __shared__ float sw[StagedWeights::kSw];
+  const StagedWeights staged(sw, sc.w, k);
+  const DaRowSums sums{red};
+  const bool live = *sc.live > 0;
+  const int64_t nchunks = da_chunks(n);
+  const bool vec = ((uintptr_t)theta & 15) == 0 && (n & 3) == 0;
+  for (int64_t q = blockIdx.x; q < nchunks; q += gridDim.x) {
+    const int64_t e0 = q * kDaChunk + threadIdx.x * 8;
+    const bool in = e0 < n;
+    float c[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if constexpr (KMAX > 0) {
+      float x[KMAX][8];
+#pragma unroll
+      for (int r = 0; r < KMAX; ++r) {
+        float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (r < k && in) rows.template load8<kLdStream>(r, e0, v);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) x[r][i] = v[i];
+      }
+#pragma unroll
+      for (int r = 0; r < KMAX; ++r) {
+        const float w = r < k ? staged.wt(r) : 0.f;
+        if (w != 0.f) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) c[i] = fmaf(w, x[r][i], c[i]);
+        }
+      }
+      if (!live) da_start8<Rows>(theta, e0, n, vec, c);
+#pragma unroll
+      for (int r = 0; r < KMAX; ++r) {
+        if (r < k) sums.put(r, da_lane_sq8(x[r], c));
+      }
+      sums.flush(0, k, sc.partial, nchunks, q);
+    } else {
+      if (in) {
+        for (int r = 0; r < k; ++r) {
+          const float w = staged.wt(r);
+          if (w != 0.f) {
+            float x[8];
+            rows.template load8<kLdReadOnly>(r, e0, x);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) c[i] = fmaf(w, x[i], c[i]);
+          }
+        }
+      }
+      if (!live) da_start8<Rows>(theta, e0, n, vec, c);
+      for (int r0 = 0; r0 < k; r0 += 32) {
+        const int nr = k - r0 < 32 ? k - r0 : 32;
+        for (int r = 0; r < nr; ++r) {
+          float x[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+          if (in) rows.template load8<kLdReadOnly>(r0 + r, e0, x);
+          sums.put(r, da_lane_sq8(x, c));
+        }
+        sums.flush(r0, nr, sc.partial, nchunks, q);
+      }
+    }
+  }
+}
+
+// Finalisation of one step: CTA r adds row r's chunk sums (distance_agg.cuh order) into d_r; the last CTA to take a ticket
+// forms the raw weights in parallel, their sum in row order (thread 0) and the weights, and leaves the ticket at 0.
+__global__ void __launch_bounds__(kDaThreads)
+dagg_finalize_kernel(DistAggScratch sc, const float* __restrict__ alpha, int k, DistAggArgs g, float* __restrict__ w_out, int64_t nchunks) {
+  __shared__ double red[kDaThreads / 32];
+  __shared__ double s_tot;
+  __shared__ int s_last;
+  const int r = blockIdx.x;
+  double v = 0.0;
+  for (int64_t q = threadIdx.x; q < nchunks; q += kDaThreads) v += __ldcg(sc.partial + (int64_t)r * nchunks + q);
+  v = warp_tree_f64(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = red[0];
+#pragma unroll
+    for (int w = 1; w < kDaThreads / 32; ++w) t += red[w];
+    sc.dist[r] = sqrt(t);
+    __threadfence();                    // d_r visible device-wide before the ticket
+    s_last = atomicAdd(sc.ticket, 1u) == (unsigned)(k - 1) ? 1 : 0;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  for (int i = threadIdx.x; i < k; i += kDaThreads) sc.raw[i] = da_raw(g, alpha[i], __ldcg(sc.dist + i));
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double tot = 0.0;
+    int live = 0;
+    for (int i = 0; i < k; ++i) {
+      tot += sc.raw[i];
+      live += da_kept(__ldcg(sc.dist + i)) ? 1 : 0;
+    }
+    if (!(tot > 0.0)) live = 0;
+    s_tot = tot;
+    *sc.live = live;
+    *sc.ticket = 0u;
+    s_last = live;
+  }
+  __syncthreads();
+  const double tot = s_tot;
+  const bool any = s_last > 0;
+  for (int i = threadIdx.x; i < k; i += kDaThreads) {
+    const float w = any ? da_weight(g, sc.raw[i], __ldcg(sc.dist + i), tot) : 0.f;
+    sc.w[i] = w;
+    if (w_out != nullptr) w_out[i] = w;
+  }
+}
+
+// theta[e0 .. e0 + 7] (t, none past n) moved towards a: theta += opt.lr (a - theta) (OPT false) or the server optimizer step
+// (OPT true); 16-byte accesses of theta and the moments per 4 elements inside n when vec
+template <bool OPT>
+__device__ __forceinline__ void step_to8(float* __restrict__ theta, int64_t e0, int64_t n, bool vec, const float (&t)[8],
+                                         const float (&a)[8], const ServerOptArgs& opt) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t e = e0 + 4 * h;
+    if (vec && e + 4 <= n) {
+      float4 tt = make_float4(t[4 * h], t[4 * h + 1], t[4 * h + 2], t[4 * h + 3]);
+      const float4 aa = make_float4(a[4 * h], a[4 * h + 1], a[4 * h + 2], a[4 * h + 3]);
+      if constexpr (OPT) {
+        tt = server_opt_step4(opt, e >> 2, tt, aa);
+      } else {
+        tt.x = fmaf(opt.lr, aa.x - tt.x, tt.x); tt.y = fmaf(opt.lr, aa.y - tt.y, tt.y);
+        tt.z = fmaf(opt.lr, aa.z - tt.z, tt.z); tt.w = fmaf(opt.lr, aa.w - tt.w, tt.w);
+      }
+      *reinterpret_cast<float4*>(theta + e) = tt;
+    } else {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if (e + i < n) {
+          const float tv = t[4 * h + i], av = a[4 * h + i];
+          theta[e + i] = OPT ? server_opt_step(opt, e + i, tv, av) : fmaf(opt.lr, av - tv, tv);
+        }
+      }
+    }
+  }
+}
+
+// Last pass: the aggregate from the final weights (geomed: c^L, or c^0 when no row is left; norm_clip: c^0 + the clipped sum),
+// theta + it for deltas, and the server step on theta with the moments in place.
+template <class Rows, bool CLIP, bool OPT>
+__global__ void __launch_bounds__(kDaThreads)
+dagg_apply_kernel(Rows rows, float* __restrict__ theta, int k, DistAggScratch sc, ServerOptArgs opt, int64_t n) {
+  __shared__ float sw[StagedWeights::kSw];
+  const StagedWeights staged(sw, sc.w, k);
+  const bool live = *sc.live > 0;
+  const int64_t nchunks = da_chunks(n);
+  const bool vec = (((uintptr_t)theta | (uintptr_t)opt.m | (uintptr_t)opt.v) & 15) == 0 && (n & 3) == 0;
+  for (int64_t q = blockIdx.x; q < nchunks; q += gridDim.x) {
+    const int64_t e0 = q * kDaChunk + threadIdx.x * 8;
+    if (e0 >= n) continue;
+    float t[8], c0[8], acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    lane_load8<kLdPlain>(theta, e0, n, vec, t);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) c0[i] = Rows::kDelta ? 0.f : t[i];
+#pragma unroll 4
+    for (int r = 0; r < k; ++r) {
+      const float w = staged.wt(r);
+      if (w != 0.f) {
+        float x[8];
+        rows.template load8<kLdStream>(r, e0, x);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] = fmaf(w, CLIP ? x[i] - c0[i] : x[i], acc[i]);
+      }
+    }
+    float a[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      a[i] = CLIP ? c0[i] + acc[i] : (live ? acc[i] : c0[i]);
+      if (Rows::kDelta) a[i] = t[i] + a[i];
+    }
+    step_to8<OPT>(theta, e0, n, vec, t, a, opt);
+  }
+}
+
 // ---- top-k uplink with error feedback (uplink_topk.cuh) -----------------------------------------------------------------------
 // exclusive prefix over the lower lanes of x in [0, 15], one ballot per bit
 __device__ __forceinline__ int warp_exclusive_prefix4(int x, uint32_t lower_lanes) {
@@ -1284,6 +1556,67 @@ cudaError_t launch_fedavg_apply_quantized_robust(float* theta, const uint8_t* pa
     return cudaErrorInvalidValue;
   return bits == 8 ? launch_fedavg_q_robust_t<8>(theta, payload, row_bytes, scales, k, agg, opt, n, s)
                    : launch_fedavg_q_robust_t<4>(theta, payload, row_bytes, scales, k, agg, opt, n, s);
+}
+namespace {
+// The passes of one distance-based aggregation: the distance pass, its finalisation, then per geomed step l < L the fused centre
+// + distance pass and its finalisation, and the apply pass: 2 L + 1 launches (norm_clip: 3).  grid <= 0: one CTA per chunk up to
+// the persistent grid.
+template <class Rows, bool CLIP, bool OPT>
+inline void launch_dagg_apply_t(Rows rows, float* theta, int k, const DistAggScratch& sc, const ServerOptArgs& opt, int64_t n, int grid,
+                                cudaStream_t s) {
+  auto kernel = dagg_apply_kernel<Rows, CLIP, OPT>;
+  COLEARN_LAUNCH(kernel, grid, kDaThreads, 0, s, rows, theta, k, sc, opt, n);
+}
+template <class Rows>
+inline cudaError_t launch_dagg_t(const Rows& rows, float* theta, const float* alpha, int k, const DistAggArgs& g, const ServerOptArgs& opt,
+                                 int64_t n, void* scratch, float* w_out, int grid, cudaStream_t s) {
+  const int64_t nchunks = da_chunks(n);
+  if (grid <= 0) grid = (int)(nchunks < 132 * 8 ? nchunks : 132 * 8);
+  const DistAggScratch sc = da_scratch_carve(scratch, k, n);
+  cudaError_t e = cudaMemsetAsync(sc.ticket, 0, sizeof(unsigned), s);
+  if (e != cudaSuccess) return e;
+  {
+    auto kernel = dagg_dist_kernel<Rows>;
+    COLEARN_LAUNCH(kernel, grid, kDaThreads, 0, s, rows, theta, k, sc, n);
+  }
+  COLEARN_LAUNCH(dagg_finalize_kernel, k, kDaThreads, 0, s, sc, alpha, k, g, w_out, nchunks);
+  const int steps = g.kind == DAGG_GEOMED ? g.iters - 1 : 0;
+  for (int l = 0; l < steps; ++l) {
+    void (*kernel)(Rows, const float*, int, DistAggScratch, int64_t);
+    // the register path holds 8 KMAX floats of rows per lane: KMAX 16 is the largest that stays clear of spills
+    if (k <= 4) kernel = dagg_center_kernel<4, Rows>;
+    else if (k <= 8) kernel = dagg_center_kernel<8, Rows>;
+    else if (k <= 16) kernel = dagg_center_kernel<16, Rows>;
+    else kernel = dagg_center_kernel<0, Rows>;
+    COLEARN_LAUNCH(kernel, grid, kDaThreads, 0, s, rows, theta, k, sc, n);
+    COLEARN_LAUNCH(dagg_finalize_kernel, k, kDaThreads, 0, s, sc, alpha, k, g, w_out, nchunks);
+  }
+  const bool clip = g.kind == DAGG_NORM_CLIP, o = opt.kind != SOPT_SGD;
+  if (clip && o) launch_dagg_apply_t<Rows, true, true>(rows, theta, k, sc, opt, n, grid, s);
+  else if (clip) launch_dagg_apply_t<Rows, true, false>(rows, theta, k, sc, opt, n, grid, s);
+  else if (o) launch_dagg_apply_t<Rows, false, true>(rows, theta, k, sc, opt, n, grid, s);
+  else launch_dagg_apply_t<Rows, false, false>(rows, theta, k, sc, opt, n, grid, s);
+  return cudaGetLastError();
+}
+inline bool dagg_ok(int k, const DistAggArgs& g, const ServerOptArgs& opt, int64_t n, const void* scratch) {
+  return k >= 1 && n >= 1 && dist_agg_args_ok(g) && server_opt_args_ok(opt) && scratch != nullptr &&
+         (reinterpret_cast<uintptr_t>(scratch) & 15) == 0;
+}
+}  // namespace
+
+cudaError_t launch_fedavg_apply_distance(float* theta, const float* rows, int64_t row_stride, const float* weights, int k,
+                                         const DistAggArgs& g, const ServerOptArgs& opt, int64_t n, void* scratch, float* weights_out,
+                                         int grid, cudaStream_t s) {
+  if (!dagg_ok(k, g, opt, n, scratch) || row_stride < n) return cudaErrorInvalidValue;
+  const bool vec = ((uintptr_t)rows & 15) == 0 && (row_stride & 3) == 0 && (n & 3) == 0;
+  return launch_dagg_t(F32Rows{rows, row_stride, n, vec}, theta, weights, k, g, opt, n, scratch, weights_out, grid, s);
+}
+cudaError_t launch_fedavg_apply_quantized_distance(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales,
+                                                   const float* weights, int k, int bits, const DistAggArgs& g, const ServerOptArgs& opt,
+                                                   int64_t n, void* scratch, float* weights_out, int grid, cudaStream_t s) {
+  if (!dagg_ok(k, g, opt, n, scratch) || !uq_layout_ok(bits, payload, row_bytes, n)) return cudaErrorInvalidValue;
+  if (bits == 8) return launch_dagg_t(QRows<8>{payload, row_bytes, scales, uq_nblk(n), n}, theta, weights, k, g, opt, n, scratch, weights_out, grid, s);
+  return launch_dagg_t(QRows<4>{payload, row_bytes, scales, uq_nblk(n), n}, theta, weights, k, g, opt, n, scratch, weights_out, grid, s);
 }
 cudaError_t launch_topk_delta(const float* models, int64_t model_stride, const float* theta, float* residual, int64_t residual_stride,
                               int rows, int topk, uint8_t* indices, float* values, int64_t entries, int64_t n, cudaStream_t s) {

@@ -120,8 +120,43 @@ colearn::AggArgs agg_args(int64_t kind, double trim) {
   TORCH_CHECK(colearn::agg_args_ok(g), "aggregator: unknown kind ", kind, " or trim fraction ", trim, " outside [0, 0.5)");
   return g;
 }
+// distance-based aggregator (distance_agg.cuh): kind 3 = geomed (iters, eps), 4 = norm_clip (clip); the scratch, and the
+// weights-out pointer (CPU fp32 [K] or none)
+bool is_dist_agg(int64_t kind) { return kind == colearn::DAGG_GEOMED || kind == colearn::DAGG_NORM_CLIP; }
+colearn::DistAggArgs dist_agg_args(int64_t kind, int64_t iters, double eps, double clip) {
+  colearn::DistAggArgs g;
+  memset(&g, 0, sizeof(g));
+  g.kind = (int)kind;
+  g.iters = (int)iters;
+  g.eps = (float)eps;
+  g.clip = (float)clip;
+  TORCH_CHECK(colearn::dist_agg_args_ok(g), "aggregator: kind ", kind, " with iters ", iters, ", eps ", eps, ", clip ", clip);
+  return g;
+}
+Tensor dist_agg_scratch(int64_t k, int64_t n) { return torch::zeros({colearn::da_scratch_bytes((int)k, n) / 8 + 2}, torch::kDouble); }
+float* dist_agg_weights_out(c10::optional<Tensor>& w, int64_t k) {
+  if (!w.has_value()) return nullptr;
+  TORCH_CHECK(w->numel() == k, "agg_weights_out [K]");
+  return fmut(*w, "agg_weights_out");
+}
 void fedavg_apply(Tensor theta, Tensor slots, Tensor w, double server_lr, int64_t opt_kind, std::vector<double> opt_hyper,
-                  c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind, double trim) {
+                  c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind, double trim, int64_t iters, double eps, double clip,
+                  c10::optional<Tensor> agg_weights_out, int64_t grid) {
+  if (is_dist_agg(agg_kind)) {
+    // (the rows may be a strided view: slot stride = slots.stride(0))
+    TORCH_CHECK(!slots.is_cuda() && slots.scalar_type() == at::kFloat && slots.dim() == 2 && slots.stride(1) == 1 && slots.size(1) >= theta.numel() &&
+                w.numel() == slots.size(0), "slots [K, >= P] (unit inner stride), weights [K]");
+    const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, theta.numel());
+    const int64_t k = slots.size(0);
+    Tensor scratch = dist_agg_scratch(k, theta.numel());
+    float* wo = dist_agg_weights_out(agg_weights_out, k);
+    float* t = fmut(theta, "theta");
+    py::gil_scoped_release nogil;
+    CK(colearn::launch_fedavg_apply_distance(t, slots.data_ptr<float>(), slots.stride(0), fptr(w, "w"), (int)k,
+                                             dist_agg_args(agg_kind, iters, eps, clip), o, theta.numel(), scratch.data_ptr(), wo, (int)grid,
+                                             nullptr));
+    return;
+  }
   TORCH_CHECK(slots.dim() == 2 && slots.size(1) == theta.numel() && w.numel() == slots.size(0), "slots [K, P], weights [K]");
   if (agg_kind != colearn::AGG_MEAN) {
     const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, theta.numel());
@@ -154,11 +189,21 @@ std::tuple<Tensor, Tensor> quantize_delta(Tensor models, Tensor theta, Tensor ke
   return {payload, scales};
 }
 void fedavg_apply_quantized(Tensor theta, Tensor payload, Tensor scales, Tensor w, int64_t bits, double server_lr, int64_t opt_kind,
-                            std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind, double trim) {
+                            std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind, double trim,
+                            int64_t iters, double eps, double clip, c10::optional<Tensor> agg_weights_out, int64_t grid) {
   TORCH_CHECK(!payload.is_cuda() && payload.scalar_type() == at::kByte && payload.dim() == 2 && payload.stride(1) == 1, "payload uint8 [K, row]");
   const int64_t k = payload.size(0), n = theta.numel();
   TORCH_CHECK(scales.size(0) == k && scales.size(1) == (n + 255) / 256 && w.numel() == k, "scales [K, ceil(P / 256)], weights [K]");
   const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, n);
+  if (is_dist_agg(agg_kind)) {
+    Tensor scratch = dist_agg_scratch(k, n);
+    float* wo = dist_agg_weights_out(agg_weights_out, k);
+    const colearn::DistAggArgs g = dist_agg_args(agg_kind, iters, eps, clip);
+    py::gil_scoped_release nogil;
+    CK(colearn::launch_fedavg_apply_quantized_distance(fmut(theta, "theta"), payload.data_ptr<uint8_t>(), payload.stride(0), fptr(scales, "scales"),
+                                                       fptr(w, "w"), (int)k, (int)bits, g, o, n, scratch.data_ptr(), wo, (int)grid, nullptr));
+    return;
+  }
   py::gil_scoped_release nogil;
   if (agg_kind != colearn::AGG_MEAN) {
     CK(colearn::launch_fedavg_apply_quantized_robust(fmut(theta, "theta"), payload.data_ptr<uint8_t>(), payload.stride(0), fptr(scales, "scales"),
@@ -562,7 +607,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // trailing server-optimizer arguments default to plain FedAvg (the shorter positional calls keep working)
   m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("w"), py::arg("server_lr"), py::arg("opt_kind") = 0,
         py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
-        py::arg("trim") = 0.0);
+        py::arg("trim") = 0.0, py::arg("iters") = 3,
+        py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none(), py::arg("grid") = 0);
   m.def("topk_delta", &topk_delta);
   m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("w"), py::arg("topk"),
         py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(),
@@ -574,7 +620,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("quantize_delta", &quantize_delta);
   m.def("fedavg_apply_quantized", &fedavg_apply_quantized, py::arg("theta"), py::arg("payload"), py::arg("scales"), py::arg("w"),
         py::arg("bits"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
-        py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0);
+        py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0, py::arg("iters") = 3,
+        py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none(), py::arg("grid") = 0);
   m.def("secagg_mask", &secagg_mask);
   m.def("fedavg_apply_secagg", &fedavg_apply_secagg, py::arg("theta"), py::arg("masked"), py::arg("keys"), py::arg("signs"),
         py::arg("frac_bits"), py::arg("n_mean"), py::arg("server_lr"), py::arg("opt_kind") = 0,

@@ -130,6 +130,23 @@ int main() {
     so.lr = 1.f;
     CK(launch_fedavg_apply_secagg(qtheta.data(), smasked.data(), qn, 2, skeys, ssigns.data(), 4, swork.data(), 20, 2, so, qn, nullptr));
     CK(launch_fedavg_apply_secagg(qtheta.data(), smasked.data(), qn, 2, skeys, ssigns.data(), 40, swork.data(), 20, 2, so, qn, nullptr));
+    // distance-based aggregation: geomed L = 3 (distance pass, ticket finalisation by the last CTA, two fused centre passes on the
+    // register path and the general one, apply) and norm_clip, fp32 and int8 rows, partial last chunk
+    {
+      const int64_t dn = 2100;
+      std::vector<float> dtheta = randv(dn), drows = randv(40 * dn), dalpha(40, 1.f / 40), dw(40);
+      std::vector<double> dscratch(da_scratch_bytes(40, dn) / 8 + 2);
+      ServerOptArgs dopt;
+      memset(&dopt, 0, sizeof(dopt));
+      dopt.lr = 1.f;
+      for (int dk : {5, 40}) {
+        DistAggArgs geo{DAGG_GEOMED, 3, 1e-6f, 0.f}, clip{DAGG_NORM_CLIP, 1, 0.f, 0.5f};
+        CK(launch_fedavg_apply_distance(dtheta.data(), drows.data(), dn, dalpha.data(), dk, geo, dopt, dn, dscratch.data(), dw.data(), 2, nullptr));
+        CK(launch_fedavg_apply_distance(dtheta.data(), drows.data(), dn, dalpha.data(), dk, clip, dopt, dn, dscratch.data(), dw.data(), 2, nullptr));
+        CK(launch_fedavg_apply_quantized_distance(dtheta.data(), qpayload, qrow, qscales.data(), dalpha.data(), 3, 8, geo, dopt, qn,
+                                                  dscratch.data(), dw.data(), 2, nullptr));
+      }
+    }
   }
   printf("elementwise kernels ok\n");
   // ---- comm: star round (with deadline) and two-shot on 3 emulated ranks, reduce_push -------------------------------------------

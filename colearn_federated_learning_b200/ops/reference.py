@@ -212,11 +212,106 @@ def robust_aggregate(models: torch.Tensor, mask: Optional[int] = None, kind: str
     return acc / torch.full_like(acc, float(n - 2 * b))
 
 
-def aggregate(models: torch.Tensor, weights: torch.Tensor, aggregator=None) -> torch.Tensor:
-    """The average the server steps towards: :func:`fedavg_flat` (``aggregator`` None or ``mean``) or
-    :func:`robust_aggregate` over all rows (unweighted)."""
+DA_CHUNK = 2048      # elements per chunk of the distance sums (ops/csrc/distance_agg.cuh: one CTA x 8 elements per lane)
+DA_THREADS = 256
+
+
+def _da_tree(v: torch.Tensor) -> torch.Tensor:
+    """float64 ``[..., 256]`` lane values -> ``[...]``: the halving tree over the 32 lanes of each warp, then the 8 warp
+    sums in warp order (the in-CTA order of ``distance_agg.cuh``)."""
+    a = v.reshape(*v.shape[:-1], DA_THREADS // 32, 32).clone()
+    o = 16
+    while o:
+        a[..., :o] = a[..., :o] + a[..., o:2 * o]
+        o >>= 1
+    t = a[..., 0, 0]
+    for w in range(1, DA_THREADS // 32):
+        t = t + a[..., w, 0]
+    return t
+
+
+def distance_sq(rows: torch.Tensor, c: torch.Tensor) -> torch.Tensor:
+    """float64 ``[K]``: ``sum_j (rows[k, j] - c[j])^2`` in the order of ``distance_agg.cuh`` (float32 difference, float64
+    squares; a lane's 8 elements in order, the in-CTA tree per 2048-element chunk, the chunks strided over 256 lanes in
+    ascending order, the same tree).  Bit for bit what the kernels compute."""
+    K, P = rows.shape
+    nch = (P + DA_CHUNK - 1) // DA_CHUNK
+    d = torch.zeros(K, nch * DA_CHUNK, dtype=torch.float32)
+    d[:, :P] = rows.float().cpu() - c.float().cpu().view(1, -1)
+    d = d.double().reshape(K, nch, DA_THREADS, 8)
+    lane = torch.zeros(K, nch, DA_THREADS, dtype=torch.float64)
+    for i in range(8):
+        lane = lane + d[..., i] * d[..., i]          # the square of a float32 is exact in float64: = fma(d, d, lane)
+    part = _da_tree(lane)                              # [K, nch]
+    m = (nch + DA_THREADS - 1) // DA_THREADS
+    pad = torch.zeros(K, m * DA_THREADS, dtype=torch.float64)
+    pad[:, :nch] = part
+    pad = pad.reshape(K, m, DA_THREADS)
+    acc = torch.zeros(K, DA_THREADS, dtype=torch.float64)
+    for i in range(m):
+        acc = acc + pad[:, i]
+    return _da_tree(acc)
+
+
+def distance_weights(aggregator, alpha: torch.Tensor, d: torch.Tensor) -> Tuple[torch.Tensor, bool]:
+    """(float32 ``[K]`` weights, any row left) from the distances ``d`` (float64) and the FedAvg weights ``alpha``:
+    ``distance_agg.cuh``'s da_raw / da_weight, the raw weights summed in row order."""
+    a = alpha.detach().float().cpu().double().tolist()
+    dl = d.tolist()
+    kept = [math.isfinite(x) for x in dl]
+    geo = aggregator.kind == "geomed"
+    eps = float(np.float32(aggregator.eps))
+    tau = float(np.float32(aggregator.clip))
+    raw = [(a[k] / max(eps, dl[k]) if geo else a[k]) if kept[k] else 0.0 for k in range(len(dl))]
+    tot = 0.0
+    for r in raw:
+        tot += r
+    live = sum(kept) > 0 and tot > 0.0
+    w = [0.0] * len(dl)
+    if live:
+        for k in range(len(dl)):
+            if kept[k]:
+                w[k] = raw[k] / tot if geo else raw[k] / tot * min(1.0, tau / dl[k] if dl[k] > 0 else math.inf)
+    return torch.tensor(w, dtype=torch.float64).float(), live
+
+
+def _fmaf_rows(w: torch.Tensor, rows: torch.Tensor) -> torch.Tensor:
+    """``sum_k fmaf(w_k, rows[k], acc)`` in row order from +0, rows of weight 0 skipped (float32 multiply and add: within an
+    ulp per step of the kernels' fmaf)."""
+    acc = torch.zeros(rows.shape[1], dtype=torch.float32)
+    for k in range(rows.shape[0]):
+        if float(w[k]) != 0.0:
+            acc = acc + w[k] * rows[k]
+    return acc
+
+
+def distance_aggregate(rows: torch.Tensor, alpha: torch.Tensor, aggregator, start: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The distance-based aggregate of ``ops/csrc/distance_agg.cuh`` (``geomed`` / ``norm_clip``) of ``rows [K, P]`` from
+    the start point ``start [P]`` (theta for models, 0 for deltas) with the FedAvg weights ``alpha [K]``: ``(a [P], final
+    weights float32 [K])``, weight 0 for an excluded row.  With no row left, ``a`` is the start point."""
+    x = rows.detach().float().cpu()
+    c0 = start.detach().float().cpu().reshape(-1)
+    w, live = distance_weights(aggregator, alpha, distance_sq(x, c0).sqrt())
+    if aggregator.kind == "norm_clip":
+        acc = torch.zeros_like(c0)
+        for k in range(x.shape[0]):
+            if float(w[k]) != 0.0:
+                acc = acc + w[k] * (x[k] - c0)
+        return c0 + acc, w
+    for _ in range(aggregator.iters - 1):
+        c = _fmaf_rows(w, x) if live else c0
+        w, live = distance_weights(aggregator, alpha, distance_sq(x, c).sqrt())
+    return (_fmaf_rows(w, x) if live else c0.clone()), w
+
+
+def aggregate(models: torch.Tensor, weights: torch.Tensor, aggregator=None, start: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The average the server steps towards: :func:`fedavg_flat` (``aggregator`` None or ``mean``),
+    :func:`robust_aggregate` over all rows (unweighted) or :func:`distance_aggregate` from ``start``."""
     if aggregator is None or not aggregator.robust:
         return fedavg_flat(models, weights)
+    if aggregator.distance_based:
+        a, _ = distance_aggregate(models, weights, aggregator, start)
+        return a.to(models.device)
     return robust_aggregate(models, None, aggregator.kind, aggregator.trim)
 
 
@@ -224,7 +319,7 @@ def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tenso
                  server_lr: float = 1.0, aggregator=None) -> torch.Tensor:
     """``theta <- theta + server_lr * (sum_k w_k models[k] - theta)`` (weights sum to 1).  ``aggregator``: a robust
     :class:`fl.aggregate.Aggregator` replaces the weighted sum by its unweighted aggregate."""
-    avg = aggregate(models, weights, aggregator)
+    avg = aggregate(models, weights, aggregator, theta)
     return theta.add_(server_lr * (avg - theta))
 
 
@@ -255,7 +350,7 @@ def server_opt_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.T
                      beta1: float = 0.9, beta2: float = 0.99, tau: float = 1e-3, aggregator=None) -> torch.Tensor:
     """``avg = sum_k w_k models[k]`` (or the robust aggregate of ``aggregator``) then :func:`server_opt_step` (the oracle of
     the fused kernels)."""
-    return server_opt_step(theta, aggregate(models, weights, aggregator), kind, lr, m, v, beta1, beta2, tau)
+    return server_opt_step(theta, aggregate(models, weights, aggregator, theta), kind, lr, m, v, beta1, beta2, tau)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -349,7 +444,7 @@ def fedavg_apply_quantized(theta: torch.Tensor, payload: torch.Tensor, scales: t
     ``theta += server_lr (a - theta)`` or the server optimizer step of ``opt`` (a ``ServerOptState``), in place."""
     deltas = decode_delta(payload, scales, bits, theta.numel()).to(theta.device)
     w = weights.to(theta.device, torch.float32) if weights is not None else None
-    avg = theta + aggregate(deltas, w, aggregator)
+    avg = theta + aggregate(deltas, w, aggregator, torch.zeros_like(theta).reshape(-1))
     if opt is None:
         return theta.add_(server_lr * (avg - theta))
     b1, b2, tau = opt.hyper

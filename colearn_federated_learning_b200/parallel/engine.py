@@ -129,6 +129,9 @@ class FederatedEngine:
         # many virtual clients (federated devices) per GPU: one CTA each, summed locally before the NVLink push
         self.clients_per_rank = max(1, int(clients_per_rank))
         self.aggregator = aggregator if aggregator is not None else Aggregator()
+        if self.aggregator.distance_based:
+            raise ValueError(f"aggregator={self.aggregator.kind!r} is not available in the multi-GPU engine (--box): its distances need "
+                             "a reduction across the ranks before every step; use local or remote mode")
         if self.aggregator.robust and self.clients_per_rank > 1:
             raise ValueError(f"aggregator={self.aggregator.kind!r} needs clients_per_rank=1: with several clients per rank the "
                              "rank sums its clients' models before the coordinator sees them, so there is no per-client value "

@@ -54,11 +54,20 @@ def build_parser() -> argparse.ArgumentParser:
     parser.add_argument("--server-beta1", type=float, default=d.server_beta1, help="first-moment decay of --server-opt, in [0, 1)")
     parser.add_argument("--server-beta2", type=float, default=d.server_beta2, help="second-moment decay of adam / yogi, in [0, 1)")
     parser.add_argument("--server-tau", type=float, default=d.server_tau, help="adaptivity of adagrad / adam / yogi (> 0)")
-    parser.add_argument("--aggregator", choices=["mean", "median", "trimmed_mean"], default=d.aggregator,
+    parser.add_argument("--aggregator", choices=["mean", "median", "trimmed_mean", "geomed", "norm_clip"], default=d.aggregator,
                         help="how the client models are combined: mean = (weighted) FedAvg; median / trimmed_mean = coordinate-wise, "
-                             "unweighted, robust to a minority of bad clients (not with --weighted)")
+                             "unweighted, robust to a minority of bad clients (not with --weighted); geomed = weighted geometric "
+                             "median (RFA), norm_clip = weighted mean of the updates clipped to --clip-norm: distance-based, "
+                             "take --weighted (local and remote mode; not with --uplink-codec topk or --secure-agg)")
     parser.add_argument("--trim-fraction", type=float, default=d.trim_fraction,
                         help="trimmed_mean: fraction of the values dropped at each end of every parameter, in [0, 0.5)")
+    parser.add_argument("--geomed-iters", type=int, default=d.geomed_iters,
+                        help="geomed: smoothed Weiszfeld steps from the current model, in 1..16 (each one more read of the replies)")
+    parser.add_argument("--geomed-eps", type=float, default=d.geomed_eps,
+                        help="geomed: floor nu of the distances in the weights alpha_k / max(nu, d_k), finite and > 0")
+    parser.add_argument("--clip-norm", type=float, default=None,
+                        help="norm_clip (required with it): L2 bound tau of every device's update; a device moves the model by at "
+                             "most alpha_k tau")
     parser.add_argument("--uplink-codec", choices=["fp32", "int8", "int4", "topk"], default=d.uplink,
                         help="what a device sends back after a fit: fp32 = its model; int8 / int4 = its delta to the received model, "
                              "stochastically quantized with one scale per 256 parameters (~3.9x / ~7.5x fewer bytes); topk = the "
@@ -142,6 +151,10 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.log_interval, a.test_path, a.synthetic, a.weighted = ns.log_interval, ns.test_path, ns.synthetic, ns.weighted
     a.aggregator = getattr(ns, "aggregator", a.aggregator)
     a.trim_fraction = getattr(ns, "trim_fraction", a.trim_fraction)
+    a.geomed_iters = getattr(ns, "geomed_iters", a.geomed_iters)
+    a.geomed_eps = getattr(ns, "geomed_eps", a.geomed_eps)
+    clip_norm = getattr(ns, "clip_norm", None)
+    a.clip_norm = a.clip_norm if clip_norm is None else clip_norm
     a.client_aggregator()             # rejects a trim fraction outside [0, 0.5) and --weighted with a robust kind
     a.uplink = getattr(ns, "uplink_codec", a.uplink)
     a.uplink_topk = getattr(ns, "uplink_topk", a.uplink_topk)
@@ -243,6 +256,9 @@ def parse_cli(argv=None) -> argparse.Namespace:
     if ns.downlink_codec != "fp32" and (ns.box or ns.encryption):
         parser.error(f"--downlink-codec {ns.downlink_codec} applies to the local and remote modes only: --box broadcasts fp32 models "
                      "over NVLink and -e exchanges secret shares")
+    if ns.aggregator in ("geomed", "norm_clip") and (ns.box or ns.encryption):
+        parser.error(f"--aggregator {ns.aggregator} applies to the local and remote modes only: --box reduces the models across the "
+                     "GPUs in one pass (no per-step distances) and -e exchanges secret shares")
     if ns.secure_agg:
         if ns.box or ns.encryption or not ns.remote:
             parser.error("--secure-agg applies to remote mode (-r) only: in local mode every update is in the coordinator's process "
