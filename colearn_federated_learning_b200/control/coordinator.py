@@ -23,6 +23,7 @@ import secrets
 import time
 import zlib
 from collections import OrderedDict
+from functools import partial
 from typing import Any, Dict, List, Optional
 
 import numpy as np
@@ -34,6 +35,7 @@ from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
 from ..fl.evaluate import evaluate
 from ..fl.secagg import check_masked_reply, check_unmask_reply, correction_streams, frac_bits, pk_from_bytes, pk_to_bytes
+from ..fl.server_opt import server_opt_state
 # the reply checks live next to the codec (the workers run them on the downlink wire too) and are exported from here as before
 from ..fl.uplink import UplinkCodec, check_quantized_reply, check_topk_reply, downlink_key, uplink_key  # noqa: F401
 from ..models import MLPNet, build_model, flatten_params, unflatten_params
@@ -335,7 +337,7 @@ class Coordinator(BusClient):
                     # every worker's delta through the uplink codec (one batched encode), as a device would send it
                     keys = [uplink_key(fed.workers[i], cfg.seed + r) for i in live]
                     payload, scales = ops.encode_delta(flats[live], replica, codec, keys)
-                    agg_w = self._server_update(theta, None, w, uplink=(payload, scales, codec))
+                    agg_w = self._server_update(theta, partial(ops.fedavg_apply_quantized, theta, payload, scales, w, codec), len(live))
                 elif codec.sparse:
                     # the live workers' deltas plus residuals through the top-k encode (one batched launch); a worker that
                     # did not train this round keeps its residual
@@ -343,9 +345,9 @@ class Coordinator(BusClient):
                     indices, values = ops.encode_topk_delta(flats[live], replica, res, codec)
                     if res is not residual:
                         residual[live] = res
-                    self._server_update(theta, None, w, uplink=(indices, values, codec))
+                    self._server_update(theta, partial(ops.fedavg_apply_topk, theta, indices, values, w, codec), len(live))
                 else:
-                    agg_w = self._server_update(theta, flats[live].contiguous(), w)
+                    agg_w = self._server_update(theta, partial(ops.fedavg_apply, theta, flats[live].contiguous(), w), len(live))
             for wid, l in zip(fed.workers, losses):
                 self.metrics.worker_loss(wid, l)
                 result["losses"][wid] = l
@@ -517,10 +519,12 @@ class Coordinator(BusClient):
                 w = normalized_weights(counts if self.args.weighted else None, len(flats), device=self.device)
                 th = theta.to(self.device)
                 if codec.quantized or codec.sparse:
-                    uplink = (torch.stack([p for p, _ in flats]).to(self.device), torch.stack([s for _, s in flats]).to(self.device), codec)
-                    agg_w = self._server_update(th, None, w, uplink=uplink)
+                    # the checked replies' (payload, scales) or (indices, values), one [K, ...] tensor per field
+                    wire = [torch.stack(field).to(self.device) for field in zip(*flats)]
+                    apply = ops.fedavg_apply_topk if codec.sparse else ops.fedavg_apply_quantized
+                    agg_w = self._server_update(th, partial(apply, th, *wire, w, codec), len(flats))
                 else:
-                    agg_w = self._server_update(th, torch.stack(flats).to(self.device), w)
+                    agg_w = self._server_update(th, partial(ops.fedavg_apply, th, torch.stack(flats).to(self.device), w), len(flats))
                 if agg_w is not None:
                     agg_rec["agg_weights"] = agg_w       # the final weight of every device in `ids` (distance-based aggregator)
                 theta = th.cpu()
@@ -604,7 +608,8 @@ class Coordinator(BusClient):
         keys, signs = correction_streams(sa["order"], survivors, dropped, dict(answers))
         masked = torch.from_numpy(np.stack([got[w][0] for w in survivors]).view(np.int32))
         th = theta.to(self.device)
-        self._server_update(th, None, None, secagg=(masked.to(self.device), keys, signs, sa["frac_bits"], len(survivors)))
+        self._server_update(th, partial(ops.fedavg_apply_secagg, th, masked.to(self.device), keys, signs, sa["frac_bits"], len(survivors)),
+                            len(survivors))
         rec["secagg_abandoned"] = False
         return th.cpu(), rec
 
@@ -623,47 +628,22 @@ class Coordinator(BusClient):
         fields[names[1]] = b.cpu().numpy().astype("<f4").tobytes()
         return fields
 
-    def _server_update(self, theta: torch.Tensor, models: Optional[torch.Tensor], weights: torch.Tensor, uplink=None,
-                       secagg=None) -> Optional[List[float]]:
-        """FedAvg of ``models`` into ``theta`` in place (or their median / trimmed mean / geometric median / norm-bounded mean,
-        ``--aggregator``), followed by the server optimizer step of ``--server-opt``.  ``uplink = (payload, scales, codec)``:
-        the clients' quantized deltas instead of their models (``ops.fedavg_apply_quantized``; ``models`` is not used);
-        ``(indices, values, codec)`` with a topk codec: their sparse deltas (``ops.fedavg_apply_topk``).  ``secagg = (masked,
-        keys, signs, frac_bits, n)``: the survivors' masked rows and the correction streams of secure aggregation
-        (``ops.fedavg_apply_secagg``).  Returns the final weight of every row under a distance-based aggregator (0 for a row
-        it excluded), None otherwise."""
+    def _server_update(self, theta: torch.Tensor, apply, k: int) -> Optional[List[float]]:
+        """One server step on ``theta`` in place: ``apply`` is a fused FedAvg apply of :mod:`ops` bound to theta and the round's
+        ``k`` rows (``partial(ops.fedavg_apply_quantized, theta, payload, scales, w, codec)`` and the like); it gets the
+        aggregate of ``--aggregator`` (mean, median / trimmed mean, geometric median / norm-bounded mean) and the step of
+        ``--server-opt``.  Returns the final weight of every row under a distance-based aggregator (0 for a row it excluded),
+        None otherwise."""
         agg = self.args.client_aggregator()
-        agg_w = None
-        extra = {}
-        if agg.distance_based and secagg is None:
-            k = models.shape[0] if uplink is None else uplink[0].shape[0]
-            agg_w = torch.zeros(k, dtype=torch.float32, device=theta.device)
-            extra = {"agg_weights_out": agg_w}
-        if secagg is not None:
-            masked, keys, signs, f, n = secagg
-            apply = lambda **kw: ops.fedavg_apply_secagg(theta, masked, keys, signs, f, n, **kw)  # noqa: E731
-        elif uplink is None:
-            apply = lambda **kw: ops.fedavg_apply(theta, models, weights, **kw, **extra)  # noqa: E731
-        elif uplink[2].sparse:
-            indices, values, codec = uplink
-            apply = lambda **kw: ops.fedavg_apply_topk(theta, indices, values, weights, codec, **kw)  # noqa: E731
-        else:
-            payload, scales, codec = uplink
-            apply = lambda **kw: ops.fedavg_apply_quantized(theta, payload, scales, weights, codec, **kw, **extra)  # noqa: E731
+        kw: Dict[str, Any] = {"aggregator": agg}
+        if agg.distance_based:
+            kw["agg_weights_out"] = torch.zeros(k, dtype=torch.float32, device=theta.device)
         if self.args.server_opt == "sgd":
-            apply(server_lr=self.args.server_lr, aggregator=agg)
-            return agg_w.cpu().tolist() if agg_w is not None else None
-        opt = self.args.server_optimizer()
-        st = self._server_opt_state
-        if st is None or st.opt != opt or st.numel != theta.numel():
-            if st is not None and st.numel != theta.numel():
-                log.info("Server optimizer state reset: the model has %d parameters, the state %d", theta.numel(), st.numel)
-            st = self._server_opt_state = opt.init_state(theta.numel(), theta.device)
-        if st.m.device != theta.device:
-            st.m = st.m.to(theta.device)
-            st.v = st.v.to(theta.device) if st.v is not None else None
-        apply(opt=st, aggregator=agg)
-        return agg_w.cpu().tolist() if agg_w is not None else None
+            kw["server_lr"] = self.args.server_lr
+        else:
+            kw["opt"] = self._server_opt_state = server_opt_state(self._server_opt_state, self.args.server_optimizer(), theta)
+        apply(**kw)
+        return kw["agg_weights_out"].cpu().tolist() if agg.distance_based else None
 
     @staticmethod
     def _average_buffers(model, buffers, weights) -> None:

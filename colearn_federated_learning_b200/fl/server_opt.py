@@ -22,11 +22,14 @@ The moments live in memory only: a checkpoint holds the model, and a restart beg
 """
 from __future__ import annotations
 
+import logging
 import math
 from dataclasses import dataclass
 from typing import List, Optional
 
 import torch
+
+log = logging.getLogger(__name__)
 
 KINDS = {"sgd": 0, "avgm": 1, "adagrad": 2, "adam": 3, "yogi": 4}   # codes of ServerOptKind (server_opt.cuh)
 ADAPTIVE = ("adagrad", "adam", "yogi")
@@ -121,3 +124,16 @@ def resolve_server_opt(server_opt: Optional[ServerOpt], server_lr: float) -> Ser
         raise ValueError(f"server_lr={server_lr} given next to server_opt={server_opt.kind!r}, which carries its own lr "
                          f"({server_opt.lr}); set ServerOpt(lr=...) only")
     return server_opt
+
+
+def server_opt_state(state: Optional[ServerOptState], opt: ServerOpt, theta: torch.Tensor) -> ServerOptState:
+    """The state ``opt`` steps ``theta`` with from one round to the next: ``state`` when it belongs to ``opt`` and to a model
+    of theta's size, its moments moved to theta's device; otherwise fresh moments (a changed model size is logged)."""
+    if state is None or state.opt != opt or state.numel != theta.numel():
+        if state is not None and state.numel != theta.numel():
+            log.info("Server optimizer state reset: the model has %d parameters, the state %d", theta.numel(), state.numel)
+        return opt.init_state(theta.numel(), theta.device)
+    if state.m.device != theta.device:
+        state.m = state.m.to(theta.device)
+        state.v = state.v.to(theta.device) if state.v is not None else None
+    return state

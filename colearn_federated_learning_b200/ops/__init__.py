@@ -37,23 +37,44 @@ def fedavg_flat(models: torch.Tensor, weights: torch.Tensor) -> torch.Tensor:
     return reference.fedavg_flat(models, weights)
 
 
-def _agg_ext_args(aggregator, weights_out: Optional[torch.Tensor], k: int, device) -> tuple:
-    """the trailing aggregator arguments of the fused FedAvg bindings (none for the mean)"""
-    if aggregator is None or not aggregator.robust:
-        return ()
-    if weights_out is not None and aggregator.distance_based:
-        if weights_out.dtype != torch.float32 or not weights_out.is_contiguous() or weights_out.numel() != k or weights_out.device != device:
-            raise ValueError(f"agg_weights_out must be a contiguous float32 tensor of {k} elements on {device}")
-    else:
-        weights_out = None
-    return (aggregator.code, aggregator.trim, aggregator.iters, aggregator.eps, aggregator.clip, weights_out)
+# The aggregators a row format refuses, by family, and why (launch_fedavg_apply refuses the same ones)
+_REFUSED = {
+    "topk": {"coordinate_wise": "top-k sparse deltas: only the (weighted) mean does",
+             "distance_based": "top-k sparse deltas: their distances would measure which entries the codec kept, not how far the device "
+                               "moved"},
+    "secagg": {"coordinate_wise": "secure aggregation: the coordinator only learns the sum",
+               "distance_based": "secure aggregation: the masks hide the per-device distances it weighs by"},
+}
 
 
-def _reference_weights_out(rows: torch.Tensor, weights: torch.Tensor, aggregator, start: torch.Tensor, weights_out) -> None:
-    """CPU path: the final per-row weights of a distance-based aggregator into ``weights_out``"""
-    if weights_out is not None and aggregator is not None and aggregator.distance_based:
-        _, w = reference.distance_aggregate(rows, weights, aggregator, start)
-        weights_out.copy_(w)
+def _fused_apply(fmt: str, theta: torch.Tensor, k: int, server_lr: float, opt, aggregator, agg_weights_out: Optional[torch.Tensor],
+                 launch, reference_apply, distance_rows=None) -> torch.Tensor:
+    """What the fused FedAvg applies share, for ``k`` client rows of format ``fmt`` (a key of ``_REFUSED``, or any other name
+    for a format that admits every aggregator).  CUDA: ``launch(*tail)`` calls the format's binding with its leading
+    arguments followed by the trailing block built here (server step, aggregator, ``agg_weights_out``).  CPU:
+    ``agg_weights_out`` of a distance-based aggregator from ``distance_rows() = (rows, weights, start)``, then
+    ``reference_apply()``."""
+    robust = aggregator is not None and aggregator.robust
+    if robust:
+        for family, reason in _REFUSED.get(fmt, {}).items():
+            if getattr(aggregator, family):
+                raise ValueError(f"aggregator {aggregator.kind!r} does not apply to {reason}")
+    if opt is not None and float(server_lr) != 1.0:
+        raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
+    weights_out = agg_weights_out if robust and aggregator.distance_based else None
+    if _cuda(theta):
+        tail = [float(opt.lr), opt.code, opt.hyper, opt.m, opt.v] if opt is not None else [float(server_lr), 0, [], None, None]
+        if robust:
+            w = weights_out
+            if w is not None and (w.dtype != torch.float32 or not w.is_contiguous() or w.numel() != k or w.device != theta.device):
+                raise ValueError(f"agg_weights_out must be a contiguous float32 tensor of {k} elements on {theta.device}")
+            tail += [aggregator.code, aggregator.trim, aggregator.iters, aggregator.eps, aggregator.clip, w]
+        launch(*tail)
+        return theta
+    if weights_out is not None:
+        rows, weights, start = distance_rows()
+        weights_out.copy_(reference.distance_aggregate(rows, weights, aggregator, start)[1])
+    return reference_apply()
 
 
 def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tensor, server_lr: float = 1.0, opt=None,
@@ -68,27 +89,17 @@ def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tenso
     distance-based one (``geomed`` / ``norm_clip``, ``ops/csrc/distance_agg.cuh``) reweights the models by their L2 distance
     from theta (``weights`` are its ``alpha``) in 2 L + 1 launches (``norm_clip``: 3), the last one fused with the step;
     ``agg_weights_out`` (fp32 ``[K]``, optional) then receives every model's final weight, 0 for an excluded one."""
-    robust = aggregator is not None and aggregator.robust
-    if opt is not None:
-        if float(server_lr) != 1.0:
-            raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
-        if _cuda(theta):
-            ext_args = _agg_ext_args(aggregator, agg_weights_out, models.shape[0], theta.device)
-            _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(opt.lr),
-                                        opt.code, opt.hyper, opt.m, opt.v, *ext_args)
-            return theta
-        _reference_weights_out(models, weights, aggregator, theta, agg_weights_out)
+    def launch(*tail):
+        _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), *tail)
+
+    def reference_apply():
+        if opt is None:
+            return reference.fedavg_apply(theta, models, weights, server_lr, aggregator=aggregator)
         b1, b2, tau = opt.hyper
         return reference.server_opt_apply(theta, models, weights, opt.kind, opt.lr, opt.m, opt.v, b1, b2, tau, aggregator=aggregator)
-    if _cuda(theta):
-        if robust:
-            _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(server_lr),
-                                        0, [], None, None, *_agg_ext_args(aggregator, agg_weights_out, models.shape[0], theta.device))
-            return theta
-        _ext.require().fedavg_apply(theta, models.contiguous(), weights.to(theta.device, torch.float32).contiguous(), float(server_lr))
-        return theta
-    _reference_weights_out(models, weights, aggregator, theta, agg_weights_out)
-    return reference.fedavg_apply(theta, models, weights, server_lr, aggregator=aggregator)
+
+    return _fused_apply("fp32", theta, models.shape[0], server_lr, opt, aggregator, agg_weights_out, launch, reference_apply,
+                        lambda: (models, weights, theta))
 
 
 def _keys_i32(keys, device) -> torch.Tensor:
@@ -131,26 +142,18 @@ def fedavg_apply_quantized(theta: torch.Tensor, payload: torch.Tensor, scales: t
     inside every pass), ``agg_weights_out`` as in :func:`fedavg_apply`.  CPU tensors: ``reference.fedavg_apply_quantized``."""
     if not codec.quantized:
         raise ValueError("fedavg_apply_quantized needs an int8 / int4 codec")
-    robust = aggregator is not None and aggregator.robust
-    if opt is not None and float(server_lr) != 1.0:
-        raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
-    if _cuda(theta):
+    k = payload.shape[0]
+
+    def launch(*tail):
         dev = theta.device
-        if weights is None:                        # (a coordinate-wise aggregator does not read them)
-            weights = torch.full((payload.shape[0],), 1.0 / payload.shape[0])
-        args = [theta, _aligned_rows(payload.to(dev)), scales.to(dev, torch.float32).contiguous(),
-                weights.to(dev, torch.float32).contiguous(), codec.bits]
-        if opt is not None:
-            args += [float(opt.lr), opt.code, opt.hyper, opt.m, opt.v]
-        else:
-            args += [float(server_lr), 0, [], None, None]
-        args += list(_agg_ext_args(aggregator, agg_weights_out, payload.shape[0], dev))
-        _ext.require().fedavg_apply_quantized(*args)
-        return theta
-    if agg_weights_out is not None and aggregator is not None and aggregator.distance_based:
-        deltas = reference.decode_delta(payload, scales, codec.bits, theta.numel())
-        _reference_weights_out(deltas, weights, aggregator, torch.zeros(theta.numel()), agg_weights_out)
-    return reference.fedavg_apply_quantized(theta, payload, scales, weights, codec.bits, server_lr, opt=opt, aggregator=aggregator)
+        w = weights if weights is not None else torch.full((k,), 1.0 / k)   # (a coordinate-wise aggregator does not read them)
+        _ext.require().fedavg_apply_quantized(theta, _aligned_rows(payload.to(dev)), scales.to(dev, torch.float32).contiguous(),
+                                              w.to(dev, torch.float32).contiguous(), codec.bits, *tail)
+
+    return _fused_apply(
+        codec.kind, theta, k, server_lr, opt, aggregator, agg_weights_out, launch,
+        lambda: reference.fedavg_apply_quantized(theta, payload, scales, weights, codec.bits, server_lr, opt=opt, aggregator=aggregator),
+        lambda: (reference.decode_delta(payload, scales, codec.bits, theta.numel()), weights, torch.zeros(theta.numel())))
 
 
 def encode_topk_delta(models: torch.Tensor, theta: torch.Tensor, residual: torch.Tensor, codec) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -178,24 +181,14 @@ def fedavg_apply_topk(theta: torch.Tensor, indices: torch.Tensor, values: torch.
     would throw the update away.  CPU tensors: ``reference.fedavg_apply_topk``."""
     if not codec.sparse:
         raise ValueError("fedavg_apply_topk needs a topk codec")
-    if aggregator is not None and aggregator.coordinate_wise:
-        raise ValueError(f"aggregator {aggregator.kind!r} does not apply to top-k sparse deltas: only the (weighted) mean does")
-    if aggregator is not None and aggregator.distance_based:
-        raise ValueError(f"aggregator {aggregator.kind!r} does not apply to top-k sparse deltas: their distances would measure which "
-                         "entries the codec kept, not how far the device moved")
-    if opt is not None and float(server_lr) != 1.0:
-        raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
-    if _cuda(theta):
+
+    def launch(*tail):
         dev = theta.device
-        args = [theta, indices.to(dev, torch.uint8).contiguous(), values.to(dev, torch.float32).contiguous(),
-                weights.to(dev, torch.float32).contiguous(), codec.k]
-        if opt is not None:
-            args += [float(opt.lr), opt.code, opt.hyper, opt.m, opt.v]
-        else:
-            args += [float(server_lr)]
-        _ext.require().fedavg_apply_topk(*args)
-        return theta
-    return reference.fedavg_apply_topk(theta, indices, values, weights, codec.k, server_lr, opt=opt)
+        _ext.require().fedavg_apply_topk(theta, indices.to(dev, torch.uint8).contiguous(), values.to(dev, torch.float32).contiguous(),
+                                         weights.to(dev, torch.float32).contiguous(), codec.k, *tail)
+
+    return _fused_apply("topk", theta, indices.shape[0], server_lr, opt, aggregator, None, launch,
+                        lambda: reference.fedavg_apply_topk(theta, indices, values, weights, codec.k, server_lr, opt=opt))
 
 
 def encode_downlink(theta: torch.Tensor, replica: torch.Tensor, codec, key: int) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -274,27 +267,17 @@ def fedavg_apply_secagg(theta: torch.Tensor, masked: torch.Tensor, keys, signs, 
     optimizer step of ``opt`` (as in :func:`fedavg_apply`).  ``masked``: uint32 (or int32 with the same bits) ``[K, P]``.  A
     robust ``aggregator`` is refused: only a sum survives the masks.  CUDA tensors: ``fedavg_secagg_kernel`` (after
     ``secagg_streams_kernel`` when the streams are split); CPU tensors: ``reference.fedavg_apply_secagg``."""
-    if aggregator is not None and aggregator.coordinate_wise:
-        raise ValueError(f"aggregator {aggregator.kind!r} does not apply to secure aggregation: the coordinator only learns the sum")
-    if aggregator is not None and aggregator.distance_based:
-        raise ValueError(f"aggregator {aggregator.kind!r} does not apply to secure aggregation: the masks hide the per-device distances "
-                         "it weighs by")
-    if opt is not None and float(server_lr) != 1.0:
-        raise ValueError(f"server_lr={server_lr} given next to a server optimizer that carries its own lr ({opt.lr})")
     if int(n) < 1:
         raise ValueError("the mean needs n >= 1 survivors")
-    if _cuda(theta):
+
+    def launch(*tail):
         dev = theta.device
         kw, sg = _secagg_streams_args(keys, signs, dev)
         rows = masked.to(dev).contiguous().view(torch.int32).reshape(-1, theta.numel())
-        args = [theta, rows, kw, sg, int(frac_bits), int(n)]
-        if opt is not None:
-            args += [float(opt.lr), opt.code, opt.hyper, opt.m, opt.v]
-        else:
-            args += [float(server_lr)]
-        _ext.require().fedavg_apply_secagg(*args)
-        return theta
-    return reference.fedavg_apply_secagg(theta, masked, keys, signs, frac_bits, n, server_lr, opt=opt)
+        _ext.require().fedavg_apply_secagg(theta, rows, kw, sg, int(frac_bits), int(n), *tail)
+
+    return _fused_apply("secagg", theta, masked.shape[0], server_lr, opt, aggregator, None, launch,
+                        lambda: reference.fedavg_apply_secagg(theta, masked, keys, signs, frac_bits, n, server_lr, opt=opt))
 
 
 def sigmoid_bce(z: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:

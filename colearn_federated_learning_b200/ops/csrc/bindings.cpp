@@ -134,66 +134,57 @@ static AggArgs agg_args(int64_t kind, double trim) {
   return g;
 }
 
-// Distance-based aggregator (distance_agg.cuh): kind 3 = geomed (iters, eps), 4 = norm_clip (clip)
-static bool is_dist_agg(int64_t kind) { return kind == DAGG_GEOMED || kind == DAGG_NORM_CLIP; }
-static DistAggArgs dist_agg_args(int64_t kind, int64_t iters, double eps, double clip) {
-  DistAggArgs g;
-  std::memset(&g, 0, sizeof(g));
-  g.kind = (int)kind;
-  g.iters = (int)iters;
-  g.eps = (float)eps;
-  g.clip = (float)clip;
-  TORCH_CHECK(dist_agg_args_ok(g), "aggregator: kind ", kind, " needs iters in 1..", kDaMaxIters, " and a finite eps > 0 (geomed) or a ",
-              "finite clip > 0 (norm_clip); got iters ", iters, ", eps ", eps, ", clip ", clip);
-  return g;
+// The trailing block of every fused FedAvg apply binding (launch_fedavg_apply): the server optimizer with its moment buffers, the
+// aggregator (kind 0 = the weighted mean, 1 = median, 2 = trimmed mean with trim per end, 3 = geomed with iters / eps, 4 =
+// norm_clip with clip), agg_weights_out (CUDA fp32 [K], distance-based kinds) and the work buffer from the caching allocator on
+// theta's device.  The launcher validates the aggregator and decides which ones the rows admit.
+static void fedavg_apply_rows(torch::Tensor& theta, const ClientRows& rows, double server_lr, int64_t opt_kind,
+                              const std::vector<double>& opt_hyper, const c10::optional<torch::Tensor>& m,
+                              const c10::optional<torch::Tensor>& v, int64_t agg_kind, double trim, int64_t iters, double eps, double clip,
+                              const c10::optional<torch::Tensor>& agg_weights_out, const char* what) {
+  const int64_t n = theta.numel();
+  auto state = [&](const c10::optional<torch::Tensor>& t, const char* name) -> int64_t {
+    if (!t.has_value()) return 0;
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() >= n &&
+                t->device() == theta.device(), name, ": contiguous CUDA float32 with one element per parameter, on theta's device");
+    return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
+  };
+  const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
+  const AggregatorArgs g{(int)agg_kind, (float)trim, (int)iters, (float)eps, (float)clip};
+  ApplyWork w{nullptr, nullptr, 0};
+  if (agg_weights_out.has_value()) {
+    const torch::Tensor& t = *agg_weights_out;
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() == rows.k && t.device() == theta.device(),
+                "agg_weights_out: contiguous CUDA float32 [K] on theta's device");
+    w.weights_out = t.data_ptr<float>();
+  }
+  torch::Tensor scratch;
+  if (const size_t bytes = fedavg_apply_work_bytes(rows, g, n)) {
+    scratch = torch::empty({(int64_t)bytes}, theta.options().dtype(at::kByte));
+    w.scratch = scratch.data_ptr();
+  }
+  check(launch_fedavg_apply(theta.data_ptr<float>(), rows, g, o, n, w, cur_stream()), what);
 }
-// the scratch of one distance-based aggregation from the caching allocator on theta's device, and the weights-out pointer
-static torch::Tensor dist_agg_scratch(const torch::Tensor& theta, int64_t k) {
-  return torch::empty({da_scratch_bytes((int)k, theta.numel())}, theta.options().dtype(at::kByte));
-}
-static float* dist_agg_weights_out(const c10::optional<torch::Tensor>& w, const torch::Tensor& theta, int64_t k) {
-  if (!w.has_value()) return nullptr;
-  TORCH_CHECK(w->is_cuda() && w->scalar_type() == at::kFloat && w->is_contiguous() && w->numel() == k && w->device() == theta.device(),
-              "agg_weights_out: contiguous CUDA float32 [K] on theta's device");
-  return w->data_ptr<float>();
+static ClientRows client_rows(int format, int64_t k, int64_t stride, const float* weights) {
+  ClientRows r{};
+  r.format = format;
+  r.k = (int)k;
+  r.stride = stride;
+  r.weights = weights;
+  return r;
 }
 
+// theta += step towards the aggregate of the K models (slots fp32 [K, >= P]): the server optimizer / aggregator arguments as in
+// fedavg_apply_rows; the weights are not read by the coordinate-wise kinds
 void fedavg_apply(torch::Tensor theta, torch::Tensor slots, torch::Tensor weights, double server_lr, int64_t opt_kind,
                   std::vector<double> opt_hyper, c10::optional<torch::Tensor> m, c10::optional<torch::Tensor> v, int64_t agg_kind,
                   double trim, int64_t iters, double eps, double clip, c10::optional<torch::Tensor> agg_weights_out) {
   CHECK_CUDA_F32(theta); CHECK_CUDA_F32(slots); CHECK_CUDA_F32(weights);
   TORCH_CHECK(slots.dim() == 2 && slots.size(1) >= theta.numel() && weights.numel() == slots.size(0), "shapes");
   c10::cuda::CUDAGuard guard(theta.device());
-  if (opt_kind == SOPT_SGD && agg_kind == AGG_MEAN) {
-    check(launch_fedavg_apply(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(),
-                              (int)slots.size(0), (float)server_lr, theta.numel(), cur_stream()), "fedavg_apply");
-    return;
-  }
-  auto state = [&](const c10::optional<torch::Tensor>& t, const char* name) -> int64_t {
-    if (!t.has_value()) return 0;
-    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() >= theta.numel() &&
-                t->device() == theta.device(), name, ": contiguous CUDA float32 with one element per parameter, on theta's device");
-    return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
-  };
-  const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
-  if (is_dist_agg(agg_kind)) {
-    // weighted distance-based aggregate, then the plain step or the server optimizer step
-    const DistAggArgs g = dist_agg_args(agg_kind, iters, eps, clip);
-    const int64_t k = slots.size(0);
-    auto scratch = dist_agg_scratch(theta, k);
-    check(launch_fedavg_apply_distance(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(), (int)k,
-                                       g, o, theta.numel(), scratch.data_ptr(), dist_agg_weights_out(agg_weights_out, theta, k), 0,
-                                       cur_stream()), "fedavg_apply (distance aggregator)");
-    return;
-  }
-  if (agg_kind != AGG_MEAN) {
-    // robust aggregate (unweighted: `weights` is not read), then the plain step or the server optimizer step
-    check(launch_fedavg_apply_robust(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), (int)slots.size(0),
-                                     agg_args(agg_kind, trim), o, theta.numel(), cur_stream()), "fedavg_apply (robust aggregator)");
-    return;
-  }
-  check(launch_fedavg_apply_opt(theta.data_ptr<float>(), slots.data_ptr<float>(), slots.stride(0), weights.data_ptr<float>(),
-                                (int)slots.size(0), o, theta.numel(), cur_stream()), "fedavg_apply (server optimizer)");
+  ClientRows r = client_rows(ROWS_F32, slots.size(0), slots.stride(0), weights.data_ptr<float>());
+  r.models = slots.data_ptr<float>();
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, "fedavg_apply");
 }
 // ---- uplink codec (uplink_quant.cuh) ------------------------------------------------------------------------------------------
 // (payload uint8 [K, row_bytes], scales fp32 [K, ceil(P / 256)]) of models [K, P] - theta [P] with keys int32 [K] (uint32 bits);
@@ -216,7 +207,7 @@ std::vector<torch::Tensor> quantize_delta(torch::Tensor models, torch::Tensor th
 }
 
 // theta += step towards theta + aggregate of the K decoded deltas (payload uint8 [K, >= packed codes] with 16-byte aligned rows,
-// scales fp32 [K, ceil(P / 256)]); the server optimizer / aggregator arguments as in fedavg_apply
+// scales fp32 [K, ceil(P / 256)]); the server optimizer / aggregator arguments as in fedavg_apply_rows
 void fedavg_apply_quantized(torch::Tensor theta, torch::Tensor payload, torch::Tensor scales, torch::Tensor weights, int64_t bits,
                             double server_lr, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<torch::Tensor> m,
                             c10::optional<torch::Tensor> v, int64_t agg_kind, double trim, int64_t iters, double eps, double clip,
@@ -227,30 +218,13 @@ void fedavg_apply_quantized(torch::Tensor theta, torch::Tensor payload, torch::T
               payload.device() == theta.device(), "payload: CUDA uint8 [K, row_bytes] on theta's device");
   TORCH_CHECK(scales.dim() == 2 && scales.size(0) == k && scales.size(1) == (n + kUqBlock - 1) / kUqBlock && weights.numel() == k &&
               scales.device() == theta.device() && weights.device() == theta.device(), "scales [K, ceil(P / 256)], weights [K]");
+  TORCH_CHECK(bits == 8 || bits == 4, "bits must be 8 or 4");
   c10::cuda::CUDAGuard guard(theta.device());
-  auto state = [&](const c10::optional<torch::Tensor>& t, const char* name) -> int64_t {
-    if (!t.has_value()) return 0;
-    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() >= n &&
-                t->device() == theta.device(), name, ": contiguous CUDA float32 with one element per parameter, on theta's device");
-    return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
-  };
-  const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
-  const uint8_t* p = payload.data_ptr<uint8_t>();
-  if (is_dist_agg(agg_kind)) {
-    const DistAggArgs g = dist_agg_args(agg_kind, iters, eps, clip);
-    auto scratch = dist_agg_scratch(theta, k);
-    check(launch_fedavg_apply_quantized_distance(theta.data_ptr<float>(), p, payload.stride(0), scales.data_ptr<float>(), weights.data_ptr<float>(),
-                                                 (int)k, (int)bits, g, o, n, scratch.data_ptr(), dist_agg_weights_out(agg_weights_out, theta, k), 0,
-                                                 cur_stream()), "fedavg_apply_quantized (distance aggregator)");
-    return;
-  }
-  if (agg_kind != AGG_MEAN) {
-    check(launch_fedavg_apply_quantized_robust(theta.data_ptr<float>(), p, payload.stride(0), scales.data_ptr<float>(), (int)k, (int)bits,
-                                               agg_args(agg_kind, trim), o, n, cur_stream()), "fedavg_apply_quantized (robust aggregator)");
-    return;
-  }
-  check(launch_fedavg_apply_quantized(theta.data_ptr<float>(), p, payload.stride(0), scales.data_ptr<float>(), weights.data_ptr<float>(),
-                                      (int)k, (int)bits, o, n, cur_stream()), "fedavg_apply_quantized");
+  ClientRows r = client_rows(bits == 8 ? ROWS_INT8 : ROWS_INT4, k, payload.stride(0), weights.data_ptr<float>());
+  r.payload = payload.data_ptr<uint8_t>();
+  r.scales = scales.data_ptr<float>();
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out,
+                    "fedavg_apply_quantized");
 }
 
 // ---- top-k uplink with error feedback (uplink_topk.cuh) -----------------------------------------------------------------------
@@ -271,10 +245,11 @@ std::vector<torch::Tensor> topk_delta(torch::Tensor models, torch::Tensor theta,
 }
 
 // theta += step towards theta + the weighted sum of the K sparse deltas (indices uint8 / values fp32 [K, E(P, topk)]); the
-// server optimizer arguments as in fedavg_apply
+// server optimizer / aggregator arguments as in fedavg_apply_rows (the rows admit only the mean)
 void fedavg_apply_topk(torch::Tensor theta, torch::Tensor indices, torch::Tensor values, torch::Tensor weights, int64_t topk,
                        double server_lr, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<torch::Tensor> m,
-                       c10::optional<torch::Tensor> v) {
+                       c10::optional<torch::Tensor> v, int64_t agg_kind, double trim, int64_t iters, double eps, double clip,
+                       c10::optional<torch::Tensor> agg_weights_out) {
   CHECK_CUDA_F32(theta); CHECK_CUDA_F32(values); CHECK_CUDA_F32(weights);
   const int64_t n = theta.numel(), k = indices.size(0);
   TORCH_CHECK(topk >= 1 && topk <= kUtMaxK, "topk must be in 1..32");
@@ -283,15 +258,11 @@ void fedavg_apply_topk(torch::Tensor theta, torch::Tensor indices, torch::Tensor
               indices.device() == theta.device() && values.device() == theta.device() && weights.device() == theta.device(),
               "indices / values [K, E(P, topk)], weights [K], on theta's device");
   c10::cuda::CUDAGuard guard(theta.device());
-  auto state = [&](const c10::optional<torch::Tensor>& t, const char* name) -> int64_t {
-    if (!t.has_value()) return 0;
-    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() >= n &&
-                t->device() == theta.device(), name, ": contiguous CUDA float32 with one element per parameter, on theta's device");
-    return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
-  };
-  const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
-  check(launch_fedavg_apply_topk(theta.data_ptr<float>(), indices.data_ptr<uint8_t>(), values.data_ptr<float>(), indices.size(1),
-                                 weights.data_ptr<float>(), (int)k, (int)topk, o, n, cur_stream()), "fedavg_apply_topk");
+  ClientRows r = client_rows(ROWS_TOPK, k, indices.size(1), weights.data_ptr<float>());
+  r.indices = indices.data_ptr<uint8_t>();
+  r.values = values.data_ptr<float>();
+  r.topk = (int)topk;
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, "fedavg_apply_topk");
 }
 
 // ---- compressed downlink (downlink.cuh) -----------------------------------------------------------------------------------------
@@ -378,29 +349,25 @@ std::vector<torch::Tensor> secagg_mask(torch::Tensor model, torch::Tensor theta,
 }
 
 // theta += step towards theta + decode(sum of the K masked rows + the signed streams) / n_mean; masked int32 [K, >= P] (uint32
-// words); the server optimizer arguments as in fedavg_apply
+// words); the server optimizer / aggregator arguments as in fedavg_apply_rows (the rows admit only the mean)
 void fedavg_apply_secagg(torch::Tensor theta, torch::Tensor masked, torch::Tensor keys, torch::Tensor signs, int64_t frac_bits, int64_t n_mean,
                          double server_lr, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<torch::Tensor> m,
-                         c10::optional<torch::Tensor> v) {
+                         c10::optional<torch::Tensor> v, int64_t agg_kind, double trim, int64_t iters, double eps, double clip,
+                         c10::optional<torch::Tensor> agg_weights_out) {
   CHECK_CUDA_F32(theta);
   const int64_t n = theta.numel();
   TORCH_CHECK(masked.is_cuda() && masked.scalar_type() == at::kInt && masked.dim() == 2 && masked.stride(1) == 1 && masked.size(1) >= n &&
               masked.device() == theta.device(), "masked: CUDA int32 [K, >= P] with unit column stride on theta's device");
   check_secagg_streams(keys, signs, theta);
   c10::cuda::CUDAGuard guard(theta.device());
-  auto state = [&](const c10::optional<torch::Tensor>& t, const char* name) -> int64_t {
-    if (!t.has_value()) return 0;
-    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() >= n &&
-                t->device() == theta.device(), name, ": contiguous CUDA float32 with one element per parameter, on theta's device");
-    return (int64_t)reinterpret_cast<uintptr_t>(t->data_ptr<float>());
-  };
-  const ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, state(m, "m"), state(v, "v"));
-  torch::Tensor work;
-  if (sa_streams_per_task(n, (int)keys.size(0)) > 0) work = torch::empty({n}, theta.options().dtype(at::kInt));
-  check(launch_fedavg_apply_secagg(theta.data_ptr<float>(), reinterpret_cast<const uint32_t*>(masked.data_ptr<int>()), masked.stride(0),
-                                   (int)masked.size(0), reinterpret_cast<const uint32_t*>(keys.data_ptr<int>()), signs.data_ptr<int>(),
-                                   (int)keys.size(0), work.defined() ? reinterpret_cast<uint32_t*>(work.data_ptr<int>()) : nullptr,
-                                   (int)frac_bits, (int)n_mean, o, n, cur_stream()), "fedavg_apply_secagg");
+  ClientRows r = client_rows(ROWS_SECAGG, masked.size(0), masked.stride(0), nullptr);
+  r.masked = reinterpret_cast<const uint32_t*>(masked.data_ptr<int>());
+  r.keys = reinterpret_cast<const uint32_t*>(keys.data_ptr<int>());
+  r.signs = signs.data_ptr<int>();
+  r.streams = (int)keys.size(0);
+  r.frac_bits = (int)frac_bits;
+  r.n_mean = (int)n_mean;
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, "fedavg_apply_secagg");
 }
 
 torch::Tensor fedavg_flat(torch::Tensor slots, torch::Tensor weights) {
@@ -896,7 +863,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("topk_delta", &topk_delta);
   m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("weights"),
         py::arg("topk"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
-        py::arg("m") = py::none(), py::arg("v") = py::none());
+        py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0, py::arg("iters") = 3,
+        py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none());
   m.def("downlink_quant", &downlink_quant);
   m.def("downlink_topk", &downlink_topk);
   m.def("replica_apply_quant", &replica_apply_quant);
@@ -909,7 +877,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("secagg_mask", &secagg_mask);
   m.def("fedavg_apply_secagg", &fedavg_apply_secagg, py::arg("theta"), py::arg("masked"), py::arg("keys"), py::arg("signs"),
         py::arg("frac_bits"), py::arg("n_mean"), py::arg("server_lr"), py::arg("opt_kind") = 0,
-        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
+        py::arg("trim") = 0.0, py::arg("iters") = 3, py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none());
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);

@@ -232,50 +232,68 @@ cudaError_t launch_sgd_step(float* param, const float* grad, float lr, int64_t n
 cudaError_t launch_scale_inplace(float* p, float scale, int64_t n, cudaStream_t s);   // p *= scale
 cudaError_t launch_sgd_step_bf16grad(float* param, const void* grad_bf16, float lr, int64_t n,
                                      cudaStream_t s);
-// theta <- theta + server_lr * (sum_k w[k] * slots[k*stride .. ] - theta)   (weights sum to 1)
-cudaError_t launch_fedavg_apply(float* theta, const float* slots, int64_t slot_stride,
-                                const float* weights, int k, float server_lr, int64_t n,
-                                cudaStream_t s);
-// same average a = sum_k w[k] * slots[k], then the server optimizer step of server_opt.cuh (opt.kind 0: launch_fedavg_apply
-// with opt.lr); opt.m / opt.v hold n floats each
-cudaError_t launch_fedavg_apply_opt(float* theta, const float* slots, int64_t slot_stride, const float* weights, int k,
-                                    const ServerOptArgs& opt, int64_t n, cudaStream_t s);
-// robust aggregate a of robust_agg.cuh over the k slots (agg.kind != AGG_MEAN; no weights), then theta += opt.lr (a - theta)
-// (opt.kind 0) or the server optimizer step; any k >= 1
-cudaError_t launch_fedavg_apply_robust(float* theta, const float* slots, int64_t slot_stride, int k, const AggArgs& agg,
-                                       const ServerOptArgs& opt, int64_t n, cudaStream_t s);
+// The fused FedAvg apply: theta <- step(theta, aggregate of the k client rows), one launch (the distance-based kinds: 2 L + 1,
+// norm_clip 3).  The rows come in one of five formats:
+//   ROWS_F32     models [k][stride] fp32: a = sum_k w[k] models[k] (the mean), or the aggregate of the models
+//   ROWS_INT8/4  deltas through the uplink codec (uplink_quant.cuh): payload [k][stride bytes], 16-byte aligned, stride a multiple
+//                of 16 covering the packed codes; scales [k][ceil(n / 256)]; a = theta + aggregate of the decoded deltas (the mean:
+//                fmaf in slot order)
+//   ROWS_TOPK    top-k deltas (uplink_topk.cuh): indices / values [k][stride = entries >= ut_entries(n, topk)], 1 <= topk <= 32,
+//                the offsets of a block of a row distinct; a = theta + sum_r w[r] (entries of row r) (fmaf in slot order, each
+//                element from +0)
+//   ROWS_SECAGG  secure aggregation (secagg.cuh), n < 2^36: masked [k][stride] uint32 words, keys [streams][8] uint32 (16-byte
+//                aligned), signs [streams] (< 0 subtracts the stream); z = sum of the k rows + the streams, a = theta +
+//                sa_decode(z) / n_mean with 2^frac_bits (0 <= frac_bits <= 64)
+enum RowFormat : int { ROWS_F32 = 0, ROWS_INT8 = 1, ROWS_INT4 = 2, ROWS_TOPK = 3, ROWS_SECAGG = 4 };
+struct ClientRows {
+  int format;                // RowFormat
+  int k;                     // rows, >= 1
+  int64_t stride;            // row stride, in elements of the format's row array (bytes of payload, entries of a top-k row)
+  const float* weights;      // [k] FedAvg weights of the mean and the distance-based kinds (alpha); secure aggregation: none
+  const float* models;       // ROWS_F32
+  const uint8_t* payload;    // ROWS_INT8 / ROWS_INT4
+  const float* scales;
+  const uint8_t* indices;    // ROWS_TOPK
+  const float* values;
+  int topk;
+  const uint32_t* masked;    // ROWS_SECAGG
+  const uint32_t* keys;
+  const int* signs;
+  int streams, frac_bits, n_mean;
+};
+// The aggregator: kind AGG_MEAN (the weighted mean), AGG_MEDIAN / AGG_TRIMMED_MEAN (robust_agg.cuh: coordinate-wise,
+// unweighted, any k) or DAGG_GEOMED / DAGG_NORM_CLIP (distance_agg.cuh: the rows weighted by their L2 distance from a centre,
+// start point theta for fp32 models and 0 for deltas).  Top-k and secure-aggregation rows admit only the mean.
+struct AggregatorArgs {
+  int kind;
+  float trim;      // trimmed mean: fraction trimmed at each end, in [0, 0.5)
+  int iters;       // geomed: L in 1..16
+  float eps;       // geomed: finite and > 0
+  float clip;      // norm_clip: finite and > 0
+};
+// What one apply may need besides its rows.  scratch: fedavg_apply_work_bytes(rows, agg, n) bytes, 16-byte aligned, no state
+// between calls (null when that is 0); weights_out (distance-based, may be null): the final weight of every row (0 for an
+// excluded one); grid (distance-based): <= 0 picks the grid, the result does not depend on it.
+struct ApplyWork {
+  void* scratch;
+  float* weights_out;
+  int grid;
+};
+// The step: theta += opt.lr (a - theta) (opt.kind 0) or the server optimizer step of server_opt.cuh (opt.m / opt.v hold n floats
+// each).  cudaErrorInvalidValue for a layout, aggregator or optimizer the rows do not admit.
+cudaError_t launch_fedavg_apply(float* theta, const ClientRows& rows, const AggregatorArgs& agg, const ServerOptArgs& opt, int64_t n,
+                                const ApplyWork& work, cudaStream_t s);
+size_t fedavg_apply_work_bytes(const ClientRows& rows, const AggregatorArgs& agg, int64_t n);
 // Uplink codec (uplink_quant.cuh), bits = 8 or 4.  Encode: row k of payload [k, row_bytes] / scales [k, ceil(n / 256)] holds
 // the codes / block steps of models[k] - theta, rounded with keys[k]; row_bytes is a multiple of 16 and covers the packed
 // codes (n bytes for int8, ceil(n / 2) for int4); n < 2^31.
 cudaError_t launch_quantize_delta(const float* models, int64_t model_stride, const float* theta, const uint32_t* keys, int k, int bits,
                                   uint8_t* payload, int64_t row_bytes, float* scales, int64_t n, cudaStream_t s);
-// a = theta + sum_k w[k] * decode(payload[k], scales[k]) (fmaf in slot order), then theta += opt.lr (a - theta) (opt.kind 0) or
-// the server optimizer step; payload 16-byte aligned, row_bytes a multiple of 16
-cudaError_t launch_fedavg_apply_quantized(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales,
-                                          const float* weights, int k, int bits, const ServerOptArgs& opt, int64_t n, cudaStream_t s);
-// a = theta + robust aggregate (robust_agg.cuh) of the k decoded deltas, then the step as above (agg.kind != AGG_MEAN)
-cudaError_t launch_fedavg_apply_quantized_robust(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, int k,
-                                                 int bits, const AggArgs& agg, const ServerOptArgs& opt, int64_t n, cudaStream_t s);
-// Distance-based robust aggregation (distance_agg.cuh): the weighted geometric median (g.kind DAGG_GEOMED) or norm-bounded mean
-// (DAGG_NORM_CLIP) of k fp32 model rows (start point theta) or k int8 / int4 delta rows (payload / scales as in
-// launch_fedavg_apply_quantized; start point 0, theta added), with the FedAvg weights alpha = weights[k], then theta += opt.lr (a -
-// theta) (opt.kind 0) or the server optimizer step.  scratch: da_scratch_bytes(k, n) bytes, 16-byte aligned; weights_out (may be
-// null): the final weight of every row (0 for an excluded one).  grid <= 0 picks the grid; the result does not depend on it.
-cudaError_t launch_fedavg_apply_distance(float* theta, const float* rows, int64_t row_stride, const float* weights, int k,
-                                         const DistAggArgs& g, const ServerOptArgs& opt, int64_t n, void* scratch, float* weights_out,
-                                         int grid, cudaStream_t s);
-cudaError_t launch_fedavg_apply_quantized_distance(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales,
-                                                   const float* weights, int k, int bits, const DistAggArgs& g, const ServerOptArgs& opt,
-                                                   int64_t n, void* scratch, float* weights_out, int grid, cudaStream_t s);
 // Top-k uplink (uplink_topk.cuh), 1 <= topk <= 32.  Encode: v = (models[r] - theta) + residual[r] for the rows r < rows;
 // row r of indices / values [rows, entries] receives the kept entries of v (entries >= ut_entries(n, topk)), and residual[r]
 // is overwritten with the unsent part of v.
 cudaError_t launch_topk_delta(const float* models, int64_t model_stride, const float* theta, float* residual, int64_t residual_stride,
                               int rows, int topk, uint8_t* indices, float* values, int64_t entries, int64_t n, cudaStream_t s);
-// a = theta + sum_r w[r] * (entries of row r) (fmaf in slot order, each element from +0), then theta += opt.lr (a - theta)
-// (opt.kind 0) or the server optimizer step; the offsets of a block of a row must be distinct
-cudaError_t launch_fedavg_apply_topk(float* theta, const uint8_t* indices, const float* values, int64_t entries, const float* weights,
-                                     int rows, int topk, const ServerOptArgs& opt, int64_t n, cudaStream_t s);
 // Compressed downlink (downlink.cuh), one row.  Coordinator: the int8 / int4 codes (payload, row_bytes as in
 // launch_quantize_delta) and block steps of theta - replica rounded with `key`, or its top-k entries (indices / values
 // [ut_entries(n, topk)]), and replica advanced in place by what was sent.  Device: replica advanced in place by such a wire
@@ -286,16 +304,11 @@ cudaError_t launch_downlink_topk(const float* theta, float* replica, int topk, u
 cudaError_t launch_replica_apply_quant(float* replica, const uint8_t* payload, int64_t row_bytes, const float* scales, int bits,
                                        int64_t n, cudaStream_t s);
 cudaError_t launch_replica_apply_topk(float* replica, const uint8_t* indices, const float* values, int topk, int64_t n, cudaStream_t s);
-// Secure aggregation (secagg.cuh), rows of n < 2^36 uint32 words; keys [streams][8] uint32 (16-byte aligned), signs [streams]
-// (< 0 subtracts the stream).  Device: out = enc(model - theta) + sum_s signs[s] PRG(keys[s]) with clip and 2^frac_bits, counts[0]
-// / counts[1] = clipped / non-finite deltas (0 <= frac_bits <= 64).  Coordinator: z = sum of the k rows of masked + the streams,
-// theta moves towards theta + sa_decode(z) / n_mean by opt.lr (opt.kind 0) or the server optimizer step; workspace: n uint32
-// of scratch, needed when sa_streams_per_task(n, streams) > 0.
+// Secure aggregation (secagg.cuh), a device's row of n < 2^36 uint32 words; keys and signs as in ClientRows:
+// out = enc(model - theta) + sum_s signs[s] PRG(keys[s]) with clip and 2^frac_bits, counts[0] / counts[1] = clipped / non-finite
+// deltas (0 <= frac_bits <= 64).  The coordinator's side is launch_fedavg_apply with ROWS_SECAGG.
 cudaError_t launch_secagg_mask(const float* model, const float* theta, const uint32_t* keys, const int* signs, int streams, float clip,
                                int frac_bits, uint32_t* out, int* counts, int64_t n, cudaStream_t s);
-cudaError_t launch_fedavg_apply_secagg(float* theta, const uint32_t* masked, int64_t row_stride, int k, const uint32_t* keys, const int* signs,
-                                       int streams, uint32_t* workspace, int frac_bits, int n_mean, const ServerOptArgs& opt, int64_t n,
-                                       cudaStream_t s);
 // out = sum_k w[k] * slots[k]
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride,
                                const float* weights, int k, int64_t n, cudaStream_t s);

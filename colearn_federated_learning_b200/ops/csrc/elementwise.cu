@@ -11,6 +11,8 @@
 #include <cuda_bf16.h>
 #include <math.h>
 
+#include <type_traits>
+
 namespace colearn {
 namespace {
 
@@ -1456,37 +1458,6 @@ cudaError_t launch_sgd_step_bf16grad(float* p, const void* g, float lr, int64_t 
   COLEARN_LAUNCH(sgd_step_bf16grad_kernel, grid_for(n), kThreads, 0, s, p, reinterpret_cast<const __nv_bfloat16*>(g), lr, n);
   return cudaGetLastError();
 }
-cudaError_t launch_fedavg_apply(float* theta, const float* slots, int64_t slot_stride, const float* weights,
-                                int k, float server_lr, int64_t n, cudaStream_t s) {
-  if (k < 1) return cudaErrorInvalidValue;
-  COLEARN_LAUNCH(fedavg_kernel<true>, grid_for(n), kThreads, 0, s, theta, slots, slot_stride, weights, k, server_lr, n);
-  return cudaGetLastError();
-}
-cudaError_t launch_fedavg_apply_opt(float* theta, const float* slots, int64_t slot_stride, const float* weights, int k,
-                                    const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
-  if (k < 1 || !server_opt_args_ok(opt)) return cudaErrorInvalidValue;
-  if (opt.kind == SOPT_SGD) return launch_fedavg_apply(theta, slots, slot_stride, weights, k, opt.lr, n, s);
-  COLEARN_LAUNCH(fedavg_opt_kernel, grid_for(n), kThreads, 0, s, theta, slots, slot_stride, weights, k, opt, n);
-  return cudaGetLastError();
-}
-cudaError_t launch_fedavg_apply_robust(float* theta, const float* slots, int64_t slot_stride, int k, const AggArgs& agg,
-                                       const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
-  if (k < 1 || agg.kind == AGG_MEAN || !agg_args_ok(agg) || !server_opt_args_ok(opt)) return cudaErrorInvalidValue;
-  const int grid = grid_for(n, 1);
-  // the register path costs KMAX^2 compares per element whatever k is: take the smallest that holds k
-  if (k <= 4) {
-    COLEARN_LAUNCH(fedavg_robust_kernel<4>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
-  } else if (k <= 8) {
-    COLEARN_LAUNCH(fedavg_robust_kernel<8>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
-  } else if (k <= 16) {
-    COLEARN_LAUNCH(fedavg_robust_kernel<16>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
-  } else if (k <= 32) {
-    COLEARN_LAUNCH(fedavg_robust_kernel<32>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
-  } else {
-    COLEARN_LAUNCH(fedavg_robust_kernel<0>, grid, kThreads, 0, s, theta, slots, slot_stride, k, agg, opt, n);
-  }
-  return cudaGetLastError();
-}
 namespace {
 // one warp per 256-element block (of one row): 8 warps per CTA, at most the persistent grid
 inline int grid_for_warps(int64_t warp_tasks) {
@@ -1503,33 +1474,6 @@ inline cudaError_t launch_quantize_delta_t(const float* models, int64_t model_st
                  row_bytes, scales, n);
   return cudaGetLastError();
 }
-template <int BITS>
-inline cudaError_t launch_fedavg_q_t(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, const float* weights,
-                                     int k, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
-  const int grid = grid_for_warps(uq_nblk(n));
-  if (opt.kind == SOPT_SGD) {
-    auto kernel = fedavg_q_kernel<BITS, false>;
-    COLEARN_LAUNCH(kernel, grid, kThreads, 0, s, theta, payload, row_bytes, scales, weights, k, opt, n);
-  } else {
-    auto kernel = fedavg_q_kernel<BITS, true>;
-    COLEARN_LAUNCH(kernel, grid, kThreads, 0, s, theta, payload, row_bytes, scales, weights, k, opt, n);
-  }
-  return cudaGetLastError();
-}
-template <int BITS>
-inline cudaError_t launch_fedavg_q_robust_t(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, int k,
-                                            const AggArgs& agg, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
-  const int grid = grid_for(n, 1);
-  void (*kernel)(float*, const uint8_t*, int64_t, const float*, int, AggArgs, ServerOptArgs, int64_t);
-  // as launch_fedavg_apply_robust: the smallest register path that holds k, the general path above 32
-  if (k <= 4) kernel = fedavg_q_robust_kernel<4, BITS>;
-  else if (k <= 8) kernel = fedavg_q_robust_kernel<8, BITS>;
-  else if (k <= 16) kernel = fedavg_q_robust_kernel<16, BITS>;
-  else if (k <= 32) kernel = fedavg_q_robust_kernel<32, BITS>;
-  else kernel = fedavg_q_robust_kernel<0, BITS>;
-  COLEARN_LAUNCH(kernel, grid, kThreads, 0, s, theta, payload, row_bytes, scales, k, agg, opt, n);
-  return cudaGetLastError();
-}
 inline bool uq_layout_ok(int bits, const uint8_t* payload, int64_t row_bytes, int64_t n) {
   if (bits != 8 && bits != 4) return false;
   if (n < 1 || n >= ((int64_t)1 << 31)) return false;            // element indices are hashed as uint32
@@ -1544,20 +1488,18 @@ cudaError_t launch_quantize_delta(const float* models, int64_t model_stride, con
   return bits == 8 ? launch_quantize_delta_t<8>(models, model_stride, theta, keys, k, payload, row_bytes, scales, n, s)
                    : launch_quantize_delta_t<4>(models, model_stride, theta, keys, k, payload, row_bytes, scales, n, s);
 }
-cudaError_t launch_fedavg_apply_quantized(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales,
-                                          const float* weights, int k, int bits, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
-  if (k < 1 || !uq_layout_ok(bits, payload, row_bytes, n) || !server_opt_args_ok(opt)) return cudaErrorInvalidValue;
-  return bits == 8 ? launch_fedavg_q_t<8>(theta, payload, row_bytes, scales, weights, k, opt, n, s)
-                   : launch_fedavg_q_t<4>(theta, payload, row_bytes, scales, weights, k, opt, n, s);
-}
-cudaError_t launch_fedavg_apply_quantized_robust(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales, int k,
-                                                 int bits, const AggArgs& agg, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
-  if (k < 1 || agg.kind == AGG_MEAN || !agg_args_ok(agg) || !server_opt_args_ok(opt) || !uq_layout_ok(bits, payload, row_bytes, n))
-    return cudaErrorInvalidValue;
-  return bits == 8 ? launch_fedavg_q_robust_t<8>(theta, payload, row_bytes, scales, k, agg, opt, n, s)
-                   : launch_fedavg_q_robust_t<4>(theta, payload, row_bytes, scales, k, agg, opt, n, s);
-}
 namespace {
+// The smallest register path that holds k: f(std::integral_constant<int, KMAX>) with KMAX 4, 8, 16, 32 (LARGEST 32) or 0, the
+// general path.  A robust kind's register path costs KMAX^2 compares per element whatever k is; the geomed centre pass holds 8
+// KMAX floats of rows per lane, so LARGEST 16 is the largest that stays clear of spills.
+template <int LARGEST, class F>
+inline void with_kmax(int k, F&& f) {
+  if (k <= 4) f(std::integral_constant<int, 4>{});
+  else if (k <= 8) f(std::integral_constant<int, 8>{});
+  else if (k <= 16) f(std::integral_constant<int, 16>{});
+  else if (LARGEST >= 32 && k <= 32) f(std::integral_constant<int, (LARGEST >= 32 ? 32 : 0)>{});
+  else f(std::integral_constant<int, 0>{});
+}
 // The passes of one distance-based aggregation: the distance pass, its finalisation, then per geomed step l < L the fused centre
 // + distance pass and its finalisation, and the apply pass: 2 L + 1 launches (norm_clip: 3).  grid <= 0: one CTA per chunk up to
 // the persistent grid.
@@ -1582,13 +1524,10 @@ inline cudaError_t launch_dagg_t(const Rows& rows, float* theta, const float* al
   COLEARN_LAUNCH(dagg_finalize_kernel, k, kDaThreads, 0, s, sc, alpha, k, g, w_out, nchunks);
   const int steps = g.kind == DAGG_GEOMED ? g.iters - 1 : 0;
   for (int l = 0; l < steps; ++l) {
-    void (*kernel)(Rows, const float*, int, DistAggScratch, int64_t);
-    // the register path holds 8 KMAX floats of rows per lane: KMAX 16 is the largest that stays clear of spills
-    if (k <= 4) kernel = dagg_center_kernel<4, Rows>;
-    else if (k <= 8) kernel = dagg_center_kernel<8, Rows>;
-    else if (k <= 16) kernel = dagg_center_kernel<16, Rows>;
-    else kernel = dagg_center_kernel<0, Rows>;
-    COLEARN_LAUNCH(kernel, grid, kDaThreads, 0, s, rows, theta, k, sc, n);
+    with_kmax<16>(k, [&](auto kmax) {
+      auto kernel = dagg_center_kernel<decltype(kmax)::value, Rows>;
+      COLEARN_LAUNCH(kernel, grid, kDaThreads, 0, s, rows, theta, k, sc, n);
+    });
     COLEARN_LAUNCH(dagg_finalize_kernel, k, kDaThreads, 0, s, sc, alpha, k, g, w_out, nchunks);
   }
   const bool clip = g.kind == DAGG_NORM_CLIP, o = opt.kind != SOPT_SGD;
@@ -1598,44 +1537,14 @@ inline cudaError_t launch_dagg_t(const Rows& rows, float* theta, const float* al
   else launch_dagg_apply_t<Rows, false, false>(rows, theta, k, sc, opt, n, grid, s);
   return cudaGetLastError();
 }
-inline bool dagg_ok(int k, const DistAggArgs& g, const ServerOptArgs& opt, int64_t n, const void* scratch) {
-  return k >= 1 && n >= 1 && dist_agg_args_ok(g) && server_opt_args_ok(opt) && scratch != nullptr &&
-         (reinterpret_cast<uintptr_t>(scratch) & 15) == 0;
-}
 }  // namespace
 
-cudaError_t launch_fedavg_apply_distance(float* theta, const float* rows, int64_t row_stride, const float* weights, int k,
-                                         const DistAggArgs& g, const ServerOptArgs& opt, int64_t n, void* scratch, float* weights_out,
-                                         int grid, cudaStream_t s) {
-  if (!dagg_ok(k, g, opt, n, scratch) || row_stride < n) return cudaErrorInvalidValue;
-  const bool vec = ((uintptr_t)rows & 15) == 0 && (row_stride & 3) == 0 && (n & 3) == 0;
-  return launch_dagg_t(F32Rows{rows, row_stride, n, vec}, theta, weights, k, g, opt, n, scratch, weights_out, grid, s);
-}
-cudaError_t launch_fedavg_apply_quantized_distance(float* theta, const uint8_t* payload, int64_t row_bytes, const float* scales,
-                                                   const float* weights, int k, int bits, const DistAggArgs& g, const ServerOptArgs& opt,
-                                                   int64_t n, void* scratch, float* weights_out, int grid, cudaStream_t s) {
-  if (!dagg_ok(k, g, opt, n, scratch) || !uq_layout_ok(bits, payload, row_bytes, n)) return cudaErrorInvalidValue;
-  if (bits == 8) return launch_dagg_t(QRows<8>{payload, row_bytes, scales, uq_nblk(n), n}, theta, weights, k, g, opt, n, scratch, weights_out, grid, s);
-  return launch_dagg_t(QRows<4>{payload, row_bytes, scales, uq_nblk(n), n}, theta, weights, k, g, opt, n, scratch, weights_out, grid, s);
-}
 cudaError_t launch_topk_delta(const float* models, int64_t model_stride, const float* theta, float* residual, int64_t residual_stride,
                               int rows, int topk, uint8_t* indices, float* values, int64_t entries, int64_t n, cudaStream_t s) {
   if (rows < 1 || topk < 1 || topk > kUtMaxK || n < 1 || model_stride < n || residual_stride < n || entries < ut_entries(n, topk))
     return cudaErrorInvalidValue;
   COLEARN_LAUNCH(topk_delta_kernel, grid_for_warps(rows * uq_nblk(n)), kThreads, 0, s, models, model_stride, theta,
                  residual, residual_stride, rows, topk, indices, values, entries, n);
-  return cudaGetLastError();
-}
-cudaError_t launch_fedavg_apply_topk(float* theta, const uint8_t* indices, const float* values, int64_t entries, const float* weights,
-                                     int rows, int topk, const ServerOptArgs& opt, int64_t n, cudaStream_t s) {
-  if (rows < 1 || topk < 1 || topk > kUtMaxK || n < 1 || entries < ut_entries(n, topk) || !server_opt_args_ok(opt))
-    return cudaErrorInvalidValue;
-  const int grid = grid_for_warps(uq_nblk(n));
-  if (opt.kind == SOPT_SGD) {
-    COLEARN_LAUNCH(fedavg_topk_kernel<false>, grid, kThreads, 0, s, theta, indices, values, entries, weights, rows, topk, opt, n);
-  } else {
-    COLEARN_LAUNCH(fedavg_topk_kernel<true>, grid, kThreads, 0, s, theta, indices, values, entries, weights, rows, topk, opt, n);
-  }
   return cudaGetLastError();
 }
 cudaError_t launch_downlink_quant(const float* theta, float* replica, uint32_t key, int bits, uint8_t* payload, int64_t row_bytes,
@@ -1675,32 +1584,119 @@ cudaError_t launch_secagg_mask(const float* model, const float* theta, const uin
                  ldexpf(1.f, frac_bits), out, counts, n);
   return cudaGetLastError();
 }
-cudaError_t launch_fedavg_apply_secagg(float* theta, const uint32_t* masked, int64_t row_stride, int k, const uint32_t* keys, const int* signs,
-                                       int streams, uint32_t* workspace, int frac_bits, int n_mean, const ServerOptArgs& opt, int64_t n,
-                                       cudaStream_t s) {
-  if (k < 1 || n < 1 || n >= kSaMaxElems || row_stride < n || streams < 0 || n_mean < 1 || frac_bits < 0 || frac_bits > 64 ||
-      (reinterpret_cast<uintptr_t>(keys) & 15) != 0 || !server_opt_args_ok(opt))
-    return cudaErrorInvalidValue;
-  const int64_t cols = (n + kSaWords - 1) / kSaWords;
-  const int per = sa_streams_per_task(n, streams);
-  const uint32_t* partial = nullptr;
-  if (per > 0) {
-    if (workspace == nullptr) return cudaErrorInvalidValue;
-    cudaError_t e = cudaMemsetAsync(workspace, 0, (size_t)n * sizeof(uint32_t), s);
-    if (e != cudaSuccess) return e;
-    COLEARN_LAUNCH(secagg_streams_kernel, grid_for(cols * ((streams + per - 1) / per), 1), kThreads, 0, s, keys, signs, streams, per,
-                   workspace, n);
-    partial = workspace;
+namespace {
+inline bool is_distance_agg(int kind) { return kind == DAGG_GEOMED || kind == DAGG_NORM_CLIP; }
+// the layout checks of each row format
+inline bool rows_ok(const ClientRows& r, int64_t n) {
+  switch (r.format) {
+    case ROWS_F32: return r.stride >= n;
+    case ROWS_INT8: return uq_layout_ok(8, r.payload, r.stride, n);
+    case ROWS_INT4: return uq_layout_ok(4, r.payload, r.stride, n);
+    case ROWS_TOPK: return r.topk >= 1 && r.topk <= kUtMaxK && n >= 1 && r.stride >= ut_entries(n, r.topk);
+    case ROWS_SECAGG:
+      return n >= 1 && n < kSaMaxElems && r.stride >= n && r.streams >= 0 && r.n_mean >= 1 && r.frac_bits >= 0 && r.frac_bits <= 64 &&
+             (reinterpret_cast<uintptr_t>(r.keys) & 15) == 0;
   }
-  const float inv_scale = ldexpf(1.f, -frac_bits), nf = (float)n_mean;
-  if (opt.kind == SOPT_SGD) {
-    COLEARN_LAUNCH(fedavg_secagg_kernel<false>, grid_for(cols, 1), kThreads, 0, s, theta, masked, row_stride, k, keys, signs, streams,
-                   partial, inv_scale, nf, opt, n);
+  return false;
+}
+// Which aggregators a row format admits.  Top-k and secure-aggregation rows take only the mean: a coordinate-wise median of
+// k/256-sparse deltas is 0 wherever fewer than half the rows kept the coordinate, their distances measure which entries the
+// codec kept, and the masks leave the coordinator nothing but the sum.
+inline bool agg_admissible(int format, int kind) { return kind == AGG_MEAN || format == ROWS_F32 || format == ROWS_INT8 || format == ROWS_INT4; }
+
+template <int BITS>
+inline cudaError_t route_quantized(float* theta, const ClientRows& r, const AggArgs& agg, const DistAggArgs& g,
+                                          const ServerOptArgs& opt, int64_t n, const ApplyWork& w, cudaStream_t s) {
+  if (is_distance_agg(g.kind))
+    return launch_dagg_t(QRows<BITS>{r.payload, r.stride, r.scales, uq_nblk(n), n}, theta, r.weights, r.k, g, opt, n, w.scratch,
+                         w.weights_out, w.grid, s);
+  if (agg.kind != AGG_MEAN) {
+    with_kmax<32>(r.k, [&](auto kmax) {
+      auto kernel = fedavg_q_robust_kernel<decltype(kmax)::value, BITS>;
+      COLEARN_LAUNCH(kernel, grid_for(n, 1), kThreads, 0, s, theta, r.payload, r.stride, r.scales, r.k, agg, opt, n);
+    });
+  } else if (opt.kind == SOPT_SGD) {
+    auto kernel = fedavg_q_kernel<BITS, false>;
+    COLEARN_LAUNCH(kernel, grid_for_warps(uq_nblk(n)), kThreads, 0, s, theta, r.payload, r.stride, r.scales, r.weights, r.k, opt, n);
   } else {
-    COLEARN_LAUNCH(fedavg_secagg_kernel<true>, grid_for(cols, 1), kThreads, 0, s, theta, masked, row_stride, k, keys, signs, streams,
-                   partial, inv_scale, nf, opt, n);
+    auto kernel = fedavg_q_kernel<BITS, true>;
+    COLEARN_LAUNCH(kernel, grid_for_warps(uq_nblk(n)), kThreads, 0, s, theta, r.payload, r.stride, r.scales, r.weights, r.k, opt, n);
   }
   return cudaGetLastError();
+}
+inline cudaError_t route_secagg(float* theta, const ClientRows& r, const ServerOptArgs& opt, int64_t n, const ApplyWork& w,
+                                       cudaStream_t s) {
+  const int64_t cols = (n + kSaWords - 1) / kSaWords;
+  const int per = sa_streams_per_task(n, r.streams);
+  const uint32_t* partial = nullptr;
+  if (per > 0) {
+    uint32_t* workspace = static_cast<uint32_t*>(w.scratch);
+    cudaError_t e = cudaMemsetAsync(workspace, 0, (size_t)n * sizeof(uint32_t), s);
+    if (e != cudaSuccess) return e;
+    COLEARN_LAUNCH(secagg_streams_kernel, grid_for(cols * ((r.streams + per - 1) / per), 1), kThreads, 0, s, r.keys, r.signs, r.streams,
+                   per, workspace, n);
+    partial = workspace;
+  }
+  const float inv_scale = ldexpf(1.f, -r.frac_bits), nf = (float)r.n_mean;
+  if (opt.kind == SOPT_SGD) {
+    COLEARN_LAUNCH(fedavg_secagg_kernel<false>, grid_for(cols, 1), kThreads, 0, s, theta, r.masked, r.stride, r.k, r.keys, r.signs,
+                   r.streams, partial, inv_scale, nf, opt, n);
+  } else {
+    COLEARN_LAUNCH(fedavg_secagg_kernel<true>, grid_for(cols, 1), kThreads, 0, s, theta, r.masked, r.stride, r.k, r.keys, r.signs,
+                   r.streams, partial, inv_scale, nf, opt, n);
+  }
+  return cudaGetLastError();
+}
+// The kernel instance of each (format, aggregator, optimizer) that launch_fedavg_apply admits.
+inline cudaError_t route_fedavg_apply(float* theta, const ClientRows& r, const AggArgs& agg, const DistAggArgs& g,
+                                      const ServerOptArgs& opt, int64_t n, const ApplyWork& w, cudaStream_t s) {
+  switch (r.format) {
+    case ROWS_F32:
+      if (is_distance_agg(g.kind)) {
+        const bool vec = ((uintptr_t)r.models & 15) == 0 && (r.stride & 3) == 0 && (n & 3) == 0;
+        return launch_dagg_t(F32Rows{r.models, r.stride, n, vec}, theta, r.weights, r.k, g, opt, n, w.scratch, w.weights_out, w.grid, s);
+      }
+      if (agg.kind != AGG_MEAN) {
+        with_kmax<32>(r.k, [&](auto kmax) {
+          auto kernel = fedavg_robust_kernel<decltype(kmax)::value>;
+          COLEARN_LAUNCH(kernel, grid_for(n, 1), kThreads, 0, s, theta, r.models, r.stride, r.k, agg, opt, n);
+        });
+      } else if (opt.kind == SOPT_SGD) {
+        COLEARN_LAUNCH(fedavg_kernel<true>, grid_for(n), kThreads, 0, s, theta, r.models, r.stride, r.weights, r.k, opt.lr, n);
+      } else {
+        COLEARN_LAUNCH(fedavg_opt_kernel, grid_for(n), kThreads, 0, s, theta, r.models, r.stride, r.weights, r.k, opt, n);
+      }
+      return cudaGetLastError();
+    case ROWS_INT8: return route_quantized<8>(theta, r, agg, g, opt, n, w, s);
+    case ROWS_INT4: return route_quantized<4>(theta, r, agg, g, opt, n, w, s);
+    case ROWS_TOPK:
+      if (opt.kind == SOPT_SGD) {
+        COLEARN_LAUNCH(fedavg_topk_kernel<false>, grid_for_warps(uq_nblk(n)), kThreads, 0, s, theta, r.indices, r.values, r.stride,
+                       r.weights, r.k, r.topk, opt, n);
+      } else {
+        COLEARN_LAUNCH(fedavg_topk_kernel<true>, grid_for_warps(uq_nblk(n)), kThreads, 0, s, theta, r.indices, r.values, r.stride,
+                       r.weights, r.k, r.topk, opt, n);
+      }
+      return cudaGetLastError();
+    default: return route_secagg(theta, r, opt, n, w, s);
+  }
+}
+}  // namespace
+
+size_t fedavg_apply_work_bytes(const ClientRows& rows, const AggregatorArgs& agg, int64_t n) {
+  if (is_distance_agg(agg.kind) && agg_admissible(rows.format, agg.kind)) return (size_t)da_scratch_bytes(rows.k, n);
+  if (rows.format == ROWS_SECAGG && sa_streams_per_task(n, rows.streams) > 0) return (size_t)n * sizeof(uint32_t);
+  return 0;
+}
+cudaError_t launch_fedavg_apply(float* theta, const ClientRows& rows, const AggregatorArgs& a, const ServerOptArgs& opt, int64_t n,
+                                const ApplyWork& work, cudaStream_t s) {
+  const AggArgs agg{a.kind, a.trim};
+  const DistAggArgs g{a.kind, a.iters, a.eps, a.clip};
+  if (rows.k < 1 || !rows_ok(rows, n) || !server_opt_args_ok(opt) || !agg_admissible(rows.format, a.kind)) return cudaErrorInvalidValue;
+  if (is_distance_agg(a.kind) ? n < 1 || !dist_agg_args_ok(g) : !agg_args_ok(agg)) return cudaErrorInvalidValue;
+  if (fedavg_apply_work_bytes(rows, a, n) > 0 && (work.scratch == nullptr || (reinterpret_cast<uintptr_t>(work.scratch) & 15) != 0))
+    return cudaErrorInvalidValue;
+  return route_fedavg_apply(theta, rows, agg, g, opt, n, work, s);
 }
 cudaError_t launch_fedavg_flat(float* out, const float* slots, int64_t slot_stride, const float* weights,
                                int k, int64_t n, cudaStream_t s) {

@@ -120,58 +120,45 @@ colearn::AggArgs agg_args(int64_t kind, double trim) {
   TORCH_CHECK(colearn::agg_args_ok(g), "aggregator: unknown kind ", kind, " or trim fraction ", trim, " outside [0, 0.5)");
   return g;
 }
-// distance-based aggregator (distance_agg.cuh): kind 3 = geomed (iters, eps), 4 = norm_clip (clip); the scratch, and the
-// weights-out pointer (CPU fp32 [K] or none)
-bool is_dist_agg(int64_t kind) { return kind == colearn::DAGG_GEOMED || kind == colearn::DAGG_NORM_CLIP; }
-colearn::DistAggArgs dist_agg_args(int64_t kind, int64_t iters, double eps, double clip) {
-  colearn::DistAggArgs g;
-  memset(&g, 0, sizeof(g));
-  g.kind = (int)kind;
-  g.iters = (int)iters;
-  g.eps = (float)eps;
-  g.clip = (float)clip;
-  TORCH_CHECK(colearn::dist_agg_args_ok(g), "aggregator: kind ", kind, " with iters ", iters, ", eps ", eps, ", clip ", clip);
-  return g;
+// the trailing block of every fused FedAvg apply, as bindings.cpp::fedavg_apply_rows: CPU fp32 moments and agg_weights_out [K],
+// the work buffer in CPU memory, and the launcher's grid override of the distance-based kinds
+void fedavg_apply_rows(Tensor& theta, const colearn::ClientRows& rows, double server_lr, int64_t opt_kind, const std::vector<double>& opt_hyper,
+                       c10::optional<Tensor>& m, c10::optional<Tensor>& v, int64_t agg_kind, double trim, int64_t iters, double eps,
+                       double clip, c10::optional<Tensor>& agg_weights_out, int64_t grid) {
+  const int64_t n = theta.numel();
+  const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, n);
+  const colearn::AggregatorArgs g{(int)agg_kind, (float)trim, (int)iters, (float)eps, (float)clip};
+  colearn::ApplyWork w{nullptr, nullptr, (int)grid};
+  if (agg_weights_out.has_value()) {
+    TORCH_CHECK(agg_weights_out->numel() == rows.k, "agg_weights_out [K]");
+    w.weights_out = fmut(*agg_weights_out, "agg_weights_out");
+  }
+  Tensor scratch;
+  if (const size_t bytes = colearn::fedavg_apply_work_bytes(rows, g, n)) {
+    scratch = torch::zeros({(int64_t)(bytes + 7) / 8 + 2}, torch::kDouble);
+    w.scratch = scratch.data_ptr();
+  }
+  float* t = fmut(theta, "theta");
+  py::gil_scoped_release nogil;
+  CK(colearn::launch_fedavg_apply(t, rows, g, o, n, w, nullptr));
 }
-Tensor dist_agg_scratch(int64_t k, int64_t n) { return torch::zeros({colearn::da_scratch_bytes((int)k, n) / 8 + 2}, torch::kDouble); }
-float* dist_agg_weights_out(c10::optional<Tensor>& w, int64_t k) {
-  if (!w.has_value()) return nullptr;
-  TORCH_CHECK(w->numel() == k, "agg_weights_out [K]");
-  return fmut(*w, "agg_weights_out");
+colearn::ClientRows client_rows(int format, int64_t k, int64_t stride, const float* weights) {
+  colearn::ClientRows r{};
+  r.format = format;
+  r.k = (int)k;
+  r.stride = stride;
+  r.weights = weights;
+  return r;
 }
 void fedavg_apply(Tensor theta, Tensor slots, Tensor w, double server_lr, int64_t opt_kind, std::vector<double> opt_hyper,
                   c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind, double trim, int64_t iters, double eps, double clip,
                   c10::optional<Tensor> agg_weights_out, int64_t grid) {
-  if (is_dist_agg(agg_kind)) {
-    // (the rows may be a strided view: slot stride = slots.stride(0))
-    TORCH_CHECK(!slots.is_cuda() && slots.scalar_type() == at::kFloat && slots.dim() == 2 && slots.stride(1) == 1 && slots.size(1) >= theta.numel() &&
-                w.numel() == slots.size(0), "slots [K, >= P] (unit inner stride), weights [K]");
-    const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, theta.numel());
-    const int64_t k = slots.size(0);
-    Tensor scratch = dist_agg_scratch(k, theta.numel());
-    float* wo = dist_agg_weights_out(agg_weights_out, k);
-    float* t = fmut(theta, "theta");
-    py::gil_scoped_release nogil;
-    CK(colearn::launch_fedavg_apply_distance(t, slots.data_ptr<float>(), slots.stride(0), fptr(w, "w"), (int)k,
-                                             dist_agg_args(agg_kind, iters, eps, clip), o, theta.numel(), scratch.data_ptr(), wo, (int)grid,
-                                             nullptr));
-    return;
-  }
-  TORCH_CHECK(slots.dim() == 2 && slots.size(1) == theta.numel() && w.numel() == slots.size(0), "slots [K, P], weights [K]");
-  if (agg_kind != colearn::AGG_MEAN) {
-    const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, theta.numel());
-    CK(colearn::launch_fedavg_apply_robust(fmut(theta, "theta"), fptr(slots, "slots"), slots.size(1), (int)slots.size(0),
-                                           agg_args(agg_kind, trim), o, theta.numel(), nullptr));
-    return;
-  }
-  if (opt_kind == colearn::SOPT_SGD) {
-    CK(colearn::launch_fedavg_apply(fmut(theta, "theta"), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0),
-                                    (float)server_lr, theta.numel(), nullptr));
-    return;
-  }
-  const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, theta.numel());
-  CK(colearn::launch_fedavg_apply_opt(fmut(theta, "theta"), fptr(slots, "slots"), slots.size(1), fptr(w, "w"), (int)slots.size(0), o,
-                                      theta.numel(), nullptr));
+  // (the rows may be a strided view: slot stride = slots.stride(0))
+  TORCH_CHECK(!slots.is_cuda() && slots.scalar_type() == at::kFloat && slots.dim() == 2 && slots.stride(1) == 1 && slots.size(1) >= theta.numel() &&
+              w.numel() == slots.size(0), "slots [K, >= P] (unit inner stride), weights [K]");
+  colearn::ClientRows r = client_rows(colearn::ROWS_F32, slots.size(0), slots.stride(0), fptr(w, "w"));
+  r.models = slots.data_ptr<float>();
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, grid);
 }
 // uplink codec (uplink_quant.cuh): same shapes and row padding as bindings.cpp::quantize_delta / fedavg_apply_quantized
 std::tuple<Tensor, Tensor> quantize_delta(Tensor models, Tensor theta, Tensor keys, int64_t bits) {
@@ -194,24 +181,11 @@ void fedavg_apply_quantized(Tensor theta, Tensor payload, Tensor scales, Tensor 
   TORCH_CHECK(!payload.is_cuda() && payload.scalar_type() == at::kByte && payload.dim() == 2 && payload.stride(1) == 1, "payload uint8 [K, row]");
   const int64_t k = payload.size(0), n = theta.numel();
   TORCH_CHECK(scales.size(0) == k && scales.size(1) == (n + 255) / 256 && w.numel() == k, "scales [K, ceil(P / 256)], weights [K]");
-  const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, n);
-  if (is_dist_agg(agg_kind)) {
-    Tensor scratch = dist_agg_scratch(k, n);
-    float* wo = dist_agg_weights_out(agg_weights_out, k);
-    const colearn::DistAggArgs g = dist_agg_args(agg_kind, iters, eps, clip);
-    py::gil_scoped_release nogil;
-    CK(colearn::launch_fedavg_apply_quantized_distance(fmut(theta, "theta"), payload.data_ptr<uint8_t>(), payload.stride(0), fptr(scales, "scales"),
-                                                       fptr(w, "w"), (int)k, (int)bits, g, o, n, scratch.data_ptr(), wo, (int)grid, nullptr));
-    return;
-  }
-  py::gil_scoped_release nogil;
-  if (agg_kind != colearn::AGG_MEAN) {
-    CK(colearn::launch_fedavg_apply_quantized_robust(fmut(theta, "theta"), payload.data_ptr<uint8_t>(), payload.stride(0), fptr(scales, "scales"),
-                                                     (int)k, (int)bits, agg_args(agg_kind, trim), o, n, nullptr));
-    return;
-  }
-  CK(colearn::launch_fedavg_apply_quantized(fmut(theta, "theta"), payload.data_ptr<uint8_t>(), payload.stride(0), fptr(scales, "scales"),
-                                            fptr(w, "w"), (int)k, (int)bits, o, n, nullptr));
+  TORCH_CHECK(bits == 8 || bits == 4, "bits must be 8 or 4");
+  colearn::ClientRows r = client_rows(bits == 8 ? colearn::ROWS_INT8 : colearn::ROWS_INT4, k, payload.stride(0), fptr(w, "w"));
+  r.payload = payload.data_ptr<uint8_t>();
+  r.scales = fptr(scales, "scales");
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, grid);
 }
 // top-k uplink (uplink_topk.cuh): same shapes as bindings.cpp::topk_delta / fedavg_apply_topk; residual [K, P] updated in place
 std::tuple<Tensor, Tensor> topk_delta(Tensor models, Tensor theta, Tensor residual, int64_t topk) {
@@ -228,15 +202,17 @@ std::tuple<Tensor, Tensor> topk_delta(Tensor models, Tensor theta, Tensor residu
   return {indices, values};
 }
 void fedavg_apply_topk(Tensor theta, Tensor indices, Tensor values, Tensor w, int64_t topk, double server_lr, int64_t opt_kind,
-                       std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v) {
+                       std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind, double trim,
+                       int64_t iters, double eps, double clip, c10::optional<Tensor> agg_weights_out, int64_t grid) {
   TORCH_CHECK(!indices.is_cuda() && indices.scalar_type() == at::kByte && indices.dim() == 2 && indices.is_contiguous(), "indices uint8 [K, E]");
   const int64_t k = indices.size(0), n = theta.numel();
   TORCH_CHECK(topk >= 1 && topk <= colearn::kUtMaxK && indices.size(1) == colearn::ut_entries(n, (int)topk) &&
               values.sizes() == indices.sizes() && w.numel() == k, "indices / values [K, E(P, topk)], weights [K]");
-  const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, n);
-  py::gil_scoped_release nogil;
-  CK(colearn::launch_fedavg_apply_topk(fmut(theta, "theta"), indices.data_ptr<uint8_t>(), fptr(values, "values"), indices.size(1),
-                                       fptr(w, "w"), (int)k, (int)topk, o, n, nullptr));
+  colearn::ClientRows r = client_rows(colearn::ROWS_TOPK, k, indices.size(1), fptr(w, "w"));
+  r.indices = indices.data_ptr<uint8_t>();
+  r.values = fptr(values, "values");
+  r.topk = (int)topk;
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, grid);
 }
 // compressed downlink (downlink.cuh): same shapes and padding as bindings.cpp::downlink_quant / downlink_topk /
 // replica_apply_quant / replica_apply_topk; the replica [P] is advanced in place
@@ -298,18 +274,19 @@ std::tuple<Tensor, Tensor> secagg_mask(Tensor model, Tensor theta, Tensor keys, 
   return {out, counts};
 }
 void fedavg_apply_secagg(Tensor theta, Tensor masked, Tensor keys, Tensor signs, int64_t frac_bits, int64_t n_mean, double server_lr,
-                         int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v) {
-  const int64_t n = theta.numel();
-  TORCH_CHECK(masked.scalar_type() == at::kInt && masked.dim() == 2 && masked.stride(1) == 1 && masked.size(1) >= n, "masked int32 [K, >= P]");
+                         int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind,
+                         double trim, int64_t iters, double eps, double clip, c10::optional<Tensor> agg_weights_out, int64_t grid) {
+  TORCH_CHECK(masked.scalar_type() == at::kInt && masked.dim() == 2 && masked.stride(1) == 1 && masked.size(1) >= theta.numel(), "masked int32 [K, >= P]");
   TORCH_CHECK(keys.scalar_type() == at::kInt && keys.is_contiguous() && keys.dim() == 2 && keys.size(1) == 8, "keys int32 [S, 8]");
   TORCH_CHECK(signs.scalar_type() == at::kInt && signs.is_contiguous() && signs.numel() == keys.size(0), "signs int32 [S]");
-  const colearn::ServerOptArgs o = server_opt_args(opt_kind, server_lr, opt_hyper, m, v, n);
-  Tensor work = torch::zeros({n}, torch::kInt);
-  float* t = fmut(theta, "theta");
-  py::gil_scoped_release nogil;
-  CK(colearn::launch_fedavg_apply_secagg(t, reinterpret_cast<const uint32_t*>(masked.data_ptr<int>()), masked.stride(0), (int)masked.size(0),
-                                         reinterpret_cast<const uint32_t*>(keys.data_ptr<int>()), signs.data_ptr<int>(), (int)keys.size(0),
-                                         reinterpret_cast<uint32_t*>(work.data_ptr<int>()), (int)frac_bits, (int)n_mean, o, n, nullptr));
+  colearn::ClientRows r = client_rows(colearn::ROWS_SECAGG, masked.size(0), masked.stride(0), nullptr);
+  r.masked = reinterpret_cast<const uint32_t*>(masked.data_ptr<int>());
+  r.keys = reinterpret_cast<const uint32_t*>(keys.data_ptr<int>());
+  r.signs = signs.data_ptr<int>();
+  r.streams = (int)keys.size(0);
+  r.frac_bits = (int)frac_bits;
+  r.n_mean = (int)n_mean;
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, grid);
 }
 Tensor fedavg_flat(Tensor slots, Tensor w) {
   Tensor out = torch::zeros({slots.size(1)}, torch::kFloat);
@@ -612,7 +589,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("topk_delta", &topk_delta);
   m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("w"), py::arg("topk"),
         py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(),
-        py::arg("v") = py::none());
+        py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0, py::arg("iters") = 3, py::arg("eps") = 1e-6,
+        py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none(), py::arg("grid") = 0);
   m.def("downlink_quant", &downlink_quant);
   m.def("downlink_topk", &downlink_topk);
   m.def("replica_apply_quant", &replica_apply_quant);
@@ -625,7 +603,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("secagg_mask", &secagg_mask);
   m.def("fedavg_apply_secagg", &fedavg_apply_secagg, py::arg("theta"), py::arg("masked"), py::arg("keys"), py::arg("signs"),
         py::arg("frac_bits"), py::arg("n_mean"), py::arg("server_lr"), py::arg("opt_kind") = 0,
-        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none());
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
+        py::arg("trim") = 0.0, py::arg("iters") = 3, py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none(),
+        py::arg("grid") = 0);
   m.def("fedavg_flat", &fedavg_flat);
   m.def("sigmoid_bce", &sigmoid_bce);
   m.def("sse_loss", &sse_loss);

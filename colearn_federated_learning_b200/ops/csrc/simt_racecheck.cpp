@@ -88,24 +88,27 @@ int main() {
     std::vector<float> qtheta = randv(qn), qmodels = randv(3 * qn), qscales(3 * 4), qw(3, 1.f / 3);
     std::vector<uint32_t> qkeys = {1u, 2u, 3u};
     alignas(16) static uint8_t qpayload[3 * 1008];
+    // every fused apply below: the plain step (sgd, lr 1), the mean unless it says otherwise, no work buffer unless it needs one
+    ServerOptArgs sgd;
+    memset(&sgd, 0, sizeof(sgd));
+    sgd.lr = 1.f;
+    const AggregatorArgs mean{AGG_MEAN, 0.f, 0, 0.f, 0.f}, median{AGG_MEDIAN, 0.f, 0, 0.f, 0.f};
+    const ApplyWork nowork{nullptr, nullptr, 0};
     for (int bits : {8, 4}) {
       CK(launch_quantize_delta(qmodels.data(), qn, qtheta.data(), qkeys.data(), 3, bits, qpayload, qrow, qscales.data(), qn, nullptr));
-      ServerOptArgs qo;
-      memset(&qo, 0, sizeof(qo));
-      qo.lr = 1.f;
-      CK(launch_fedavg_apply_quantized(qtheta.data(), qpayload, qrow, qscales.data(), qw.data(), 3, bits, qo, qn, nullptr));
-      AggArgs qa{AGG_MEDIAN, 0.f};
-      CK(launch_fedavg_apply_quantized_robust(qtheta.data(), qpayload, qrow, qscales.data(), 3, bits, qa, qo, qn, nullptr));
+      ClientRows q{};
+      q.format = bits == 8 ? ROWS_INT8 : ROWS_INT4; q.k = 3; q.stride = qrow; q.weights = qw.data(); q.payload = qpayload; q.scales = qscales.data();
+      CK(launch_fedavg_apply(qtheta.data(), q, mean, sgd, qn, nowork, nullptr));
+      CK(launch_fedavg_apply(qtheta.data(), q, median, sgd, qn, nowork, nullptr));
     }
     // top-k uplink: encode 3 rows (warp select by reductions and ballots, residual written back), then the sparse decode +
     // FedAvg (per-warp shared accumulator, one __syncwarp per slot), k = 8, with a partial last block (m_last = 232)
     std::vector<float> kres(3 * qn, 0.f), kvals(3 * 32);
     std::vector<uint8_t> kidx(3 * 32);
     CK(launch_topk_delta(qmodels.data(), qn, qtheta.data(), kres.data(), qn, 3, 8, kidx.data(), kvals.data(), 32, qn, nullptr));
-    ServerOptArgs ko;
-    memset(&ko, 0, sizeof(ko));
-    ko.lr = 1.f;
-    CK(launch_fedavg_apply_topk(qtheta.data(), kidx.data(), kvals.data(), 32, qw.data(), 3, 8, ko, qn, nullptr));
+    ClientRows kr{};
+    kr.format = ROWS_TOPK; kr.k = 3; kr.stride = 32; kr.weights = qw.data(); kr.indices = kidx.data(); kr.values = kvals.data(); kr.topk = 8;
+    CK(launch_fedavg_apply(qtheta.data(), kr, mean, sgd, qn, nowork, nullptr));
     // compressed downlink: encode-and-advance of one replica (block max by shuffles / warp select, replica written in place),
     // then the device-side apply of the same wire to a second replica, int8, int4 and topk k = 8, partial last block
     std::vector<float> drep(qn, 0.f), dev_rep(qn, 0.f);
@@ -121,30 +124,34 @@ int main() {
     std::vector<int> ssigns(40), scounts(2);
     for (int i = 0; i < 40 * 8; ++i) skeys[i] = (uint32_t)rand() * 2654435761u;
     for (int i = 0; i < 40; ++i) ssigns[i] = (i & 1) ? -1 : 1;
-    std::vector<uint32_t> smasked(2 * qn), swork(qn);
+    std::vector<uint32_t> smasked(2 * qn);
+    alignas(16) static uint32_t swork[1000];
     CK(launch_secagg_mask(qmodels.data(), qtheta.data(), skeys, ssigns.data(), 3, 0.5f, 20, smasked.data(), scounts.data(), qn, nullptr));
     CK(launch_secagg_mask(qmodels.data() + qn, qtheta.data(), skeys, ssigns.data(), 3, 0.5f, 20, smasked.data() + qn, scounts.data(), qn,
                           nullptr));
-    ServerOptArgs so;
-    memset(&so, 0, sizeof(so));
-    so.lr = 1.f;
-    CK(launch_fedavg_apply_secagg(qtheta.data(), smasked.data(), qn, 2, skeys, ssigns.data(), 4, swork.data(), 20, 2, so, qn, nullptr));
-    CK(launch_fedavg_apply_secagg(qtheta.data(), smasked.data(), qn, 2, skeys, ssigns.data(), 40, swork.data(), 20, 2, so, qn, nullptr));
+    ClientRows sr{};
+    sr.format = ROWS_SECAGG; sr.k = 2; sr.stride = qn; sr.masked = smasked.data(); sr.keys = skeys; sr.signs = ssigns.data();
+    sr.frac_bits = 20; sr.n_mean = 2;
+    for (int streams : {4, 40}) {
+      sr.streams = streams;
+      CK(launch_fedavg_apply(qtheta.data(), sr, mean, sgd, qn, ApplyWork{swork, nullptr, 0}, nullptr));
+    }
     // distance-based aggregation: geomed L = 3 (distance pass, ticket finalisation by the last CTA, two fused centre passes on the
     // register path and the general one, apply) and norm_clip, fp32 and int8 rows, partial last chunk
     {
       const int64_t dn = 2100;
       std::vector<float> dtheta = randv(dn), drows = randv(40 * dn), dalpha(40, 1.f / 40), dw(40);
-      std::vector<double> dscratch(da_scratch_bytes(40, dn) / 8 + 2);
-      ServerOptArgs dopt;
-      memset(&dopt, 0, sizeof(dopt));
-      dopt.lr = 1.f;
+      const AggregatorArgs geo{DAGG_GEOMED, 0.f, 3, 1e-6f, 0.f}, clip{DAGG_NORM_CLIP, 0.f, 1, 0.f, 0.5f};
+      ClientRows fr{}, qr{};
+      fr.format = ROWS_F32; fr.k = 40; fr.stride = dn; fr.weights = dalpha.data(); fr.models = drows.data();
+      qr.format = ROWS_INT8; qr.k = 3; qr.stride = qrow; qr.weights = dalpha.data(); qr.payload = qpayload; qr.scales = qscales.data();
+      std::vector<double> dscratch(fedavg_apply_work_bytes(fr, geo, dn) / 8 + 2);
+      const ApplyWork dwork{dscratch.data(), dw.data(), 2};
       for (int dk : {5, 40}) {
-        DistAggArgs geo{DAGG_GEOMED, 3, 1e-6f, 0.f}, clip{DAGG_NORM_CLIP, 1, 0.f, 0.5f};
-        CK(launch_fedavg_apply_distance(dtheta.data(), drows.data(), dn, dalpha.data(), dk, geo, dopt, dn, dscratch.data(), dw.data(), 2, nullptr));
-        CK(launch_fedavg_apply_distance(dtheta.data(), drows.data(), dn, dalpha.data(), dk, clip, dopt, dn, dscratch.data(), dw.data(), 2, nullptr));
-        CK(launch_fedavg_apply_quantized_distance(dtheta.data(), qpayload, qrow, qscales.data(), dalpha.data(), 3, 8, geo, dopt, qn,
-                                                  dscratch.data(), dw.data(), 2, nullptr));
+        fr.k = dk;
+        CK(launch_fedavg_apply(dtheta.data(), fr, geo, sgd, dn, dwork, nullptr));
+        CK(launch_fedavg_apply(dtheta.data(), fr, clip, sgd, dn, dwork, nullptr));
+        CK(launch_fedavg_apply(dtheta.data(), qr, geo, sgd, qn, dwork, nullptr));
       }
     }
   }
