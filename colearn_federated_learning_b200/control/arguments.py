@@ -53,6 +53,11 @@ class Arguments:
     secure_agg: bool = False       # remote mode: devices send pairwise-masked fixed-point deltas, the coordinator learns only their
                                    # sum (fl/secagg.py)
     secagg_clip: float = 1.0       # secure aggregation: every coordinate of a delta is clipped to [-clip, clip] (finite, > 0)
+    fed_eval_every: int = 0        # >0: the devices score the global model on held-out rows after every N-th round and the last one
+                                   # (fl/fedeval.py); 0: no federated evaluation
+    eval_bins: int = 256           # federated evaluation: score histogram bins, a power of two in [2, 4096]
+    eval_threshold: float = 0.5    # federated evaluation: a one-column model predicts the positive class iff p > threshold
+    eval_fraction: float = 0.0     # federated evaluation, local and box mode: fraction of every device's shard held out, in (0, 1)
     backend: str = "auto"          # auto | fused | nccl | cpu
     dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the wgmma consumers)
     save_every: int = 0            # >0: checkpoint every N rounds, not only after the last one
@@ -117,6 +122,22 @@ class Arguments:
         if self.weighted:
             raise ValueError("--secure-agg does not combine with --weighted: the masked sum gives the unweighted mean")
         return clip
+
+    def fed_eval_settings(self) -> None:
+        """The checks of the federated-evaluation settings that do not depend on the mode (ValueError with the reason)."""
+        if self.fed_eval_every < 0:
+            raise ValueError(f"--fed-eval-every must be >= 0, not {self.fed_eval_every}")
+        if self.eval_bins < 2 or self.eval_bins > 4096 or self.eval_bins & (self.eval_bins - 1):
+            raise ValueError(f"--eval-bins must be a power of two in [2, 4096], not {self.eval_bins}")
+        if not 0.0 <= self.eval_threshold <= 1.0:
+            raise ValueError(f"--eval-threshold must be in [0, 1], not {self.eval_threshold}")
+        if not 0.0 <= self.eval_fraction < 1.0:
+            raise ValueError(f"--eval-fraction must be in [0, 1), not {self.eval_fraction}")
+        if self.eval_fraction > 0 and self.fed_eval_every == 0:
+            raise ValueError("--eval-fraction holds rows out for --fed-eval-every, which is not set")
+        if self.fed_eval_every > 0 and self.secure_agg:
+            raise ValueError("--fed-eval-every does not combine with --secure-agg: every device's counts (and with them the label mix "
+                             "of its data, which secure aggregation hides) would travel in the clear")
 
     def set_federated_batches(self, batches: int) -> None:
         self.federate_after_n_batches = batches

@@ -33,6 +33,7 @@ from .. import ops, settings
 from ..data import federate, synthetic_for_model, BaseDataset
 from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
+from ..fl import fedeval
 from ..fl.evaluate import evaluate
 from ..fl.secagg import check_masked_reply, check_unmask_reply, correction_streams, frac_bits, pk_from_bytes, pk_to_bytes
 from ..fl.server_opt import server_opt_state
@@ -309,6 +310,7 @@ class Coordinator(BusClient):
         log.info("Distribution data among the virtual workers")
         fed = federate(self._dataset(), list(to_train.keys()), self.device)
         log.info("Done")
+        held = self._hold_out_local(model, fed, cfg.seed)
 
         theta = flatten_params(model).to(self.device)
         model.to(self.device)
@@ -357,6 +359,10 @@ class Coordinator(BusClient):
                 rec["agg_weights"] = [0.0] * len(fed.workers)
                 for j, i in enumerate(live):
                     rec["agg_weights"][i] = agg_w[j]
+            if held is not None and self._fed_eval_round(r):
+                ex, ey, sizes = held
+                rec["fed_eval"] = result["fed_eval"] = fedeval.record(
+                    dict(zip(fed.workers, fedeval.summarize(model, theta, ex, ey, self.args.eval_bins, self.args.eval_threshold, sizes))))
             self.metrics.end_round(r, time.time() - t0, selected=fed.workers, n_k=counts, loss_k=losses, **rec)
             self._maybe_checkpoint(model, theta, r, {"workers": fed.workers, "mode": "local"})
         log.info("End training")
@@ -367,6 +373,32 @@ class Coordinator(BusClient):
         self.trainings_done += 1
         log.info("End training local")
         return result
+
+    def _fed_eval_round(self, r: int) -> bool:
+        """``--fed-eval-every N``: the global model is evaluated after every N-th round and after the last one"""
+        n = self.args.fed_eval_every
+        return n > 0 and ((r + 1) % n == 0 or r + 1 == self.enabled_round)
+
+    def _hold_out_local(self, model, fed, seed: int):
+        """``--fed-eval-every`` in local mode: every virtual worker's shard loses its ``--eval-fraction`` held-out rows
+        (``fedeval.split_eval``, keyed by the worker's position); returns ``(x, y, rows per worker)`` of the held-out rows
+        in worker order, or None without federated evaluation (the shards are left as they are)."""
+        if self.args.fed_eval_every <= 0:
+            return None
+        self.args.fed_eval_settings()
+        fedeval.check_model(model)
+        if not self.args.eval_fraction > 0:
+            raise ValueError("--fed-eval-every in local mode needs --eval-fraction > 0")
+        from ..data.federate import Shard
+        xs, ys, sizes = [], [], []
+        for i, wid in enumerate(fed.workers):
+            sh = fed[wid]
+            xt, yt, xe, ye = fedeval.split_eval(sh.x, sh.y, self.args.eval_fraction, seed + i)
+            fed.shards[wid] = Shard(wid, xt, yt)
+            xs.append(xe)
+            ys.append(ye)
+            sizes.append(int(xe.shape[0]))
+        return torch.cat(xs), torch.cat(ys), sizes
 
     # ------------------------------------------------------------------ encrypted (SMPC) mode
     def starting_training_enc(self, snapshot: "OrderedDict[str, Any]") -> Optional[Dict[str, Any]]:
@@ -397,6 +429,8 @@ class Coordinator(BusClient):
             self.args.set_federated_batches(ROUND_MODE_BATCHES)  # fc.py:533-535
         log.info("Federated batches: " + str(self.args.federate_after_n_batches))
         cfg = self._fit_config("remote")
+        if self.args.fed_eval_every > 0:
+            self.args.fed_eval_settings()
         theta = flatten_params(model).cpu()
         loop = asyncio.get_running_loop()
         # one thread per selected device: every fit RPC of a round is in flight at the same time (the default
@@ -440,6 +474,7 @@ class Coordinator(BusClient):
         codec = self.args.uplink_codec()
         down = self.args.downlink_codec()
         result["uplink"], result["downlink"] = codec.kind, down.kind
+        eval_classes = fedeval.check_model(model) if self.args.fed_eval_every > 0 else None
         # the replica of the model the devices hold, tagged "<nonce>:<round>" (a fresh nonce per training: a device cannot
         # mistake an earlier training's replica for this one's); memory only
         replica = theta.to(self.device).clone() if down.kind != "fp32" else None
@@ -533,6 +568,8 @@ class Coordinator(BusClient):
             # unmask exchange of secure aggregation
             bytes_out = sum(traffic(w)[0] - sent0[wid][0] for wid, w in to_train.items() if wid in sent0)
             bytes_in = sum(traffic(w)[1] - sent0[wid][1] for wid, w in to_train.items() if wid in sent0)
+            if self._fed_eval_round(r):
+                agg_rec["fed_eval"] = result["fed_eval"] = await self._remote_fed_eval(alive, theta, eval_classes, loop, pool)
             self.metrics.end_round(r, time.time() - t0, selected=ids, n_k=counts, bytes_out=bytes_out, bytes_in=bytes_in, **secagg_rec,
                                    **agg_rec)
             result["bytes_out"] = result.get("bytes_out", 0) + bytes_out
@@ -541,6 +578,27 @@ class Coordinator(BusClient):
             if not alive:
                 break
         return theta
+
+    async def _remote_fed_eval(self, alive, theta: torch.Tensor, classes: int, loop, pool) -> Dict[str, Any]:
+        """Federated evaluation of ``theta`` (the true global model, fp32) on every live device's evaluation data.  Every reply
+        must be the summary of ``classes`` output columns (the coordinator's model, never what the device claims) and pass
+        ``fedeval.from_wire``'s checks, or the device is listed under ``eval_excluded``; a device without evaluation data is
+        listed under ``eval_missing``."""
+        bins, thr = self.args.eval_bins, self.args.eval_threshold
+
+        async def ask(wid, worker):
+            try:
+                resp = await loop.run_in_executor(pool, lambda: worker.evaluate(theta, self.args.model, bins, thr, timeout=self.fit_timeout))
+                if not resp.get("ok", False):
+                    return wid, "missing" if resp.get("eval_missing") else "excluded"
+                return wid, fedeval.from_wire(resp, classes, bins)
+            except Exception as e:  # noqa: BLE001 - a device's reply is untrusted: it is left out of the total
+                log.info("Worker %s: evaluation reply refused: %r", wid, e)
+                return wid, "excluded"
+
+        answers = await asyncio.gather(*[ask(wid, w) for wid, w in alive.items()])
+        return fedeval.record({wid: a for wid, a in answers if isinstance(a, fedeval.Summary)},
+                              excluded=[wid for wid, a in answers if a == "excluded"], missing=[wid for wid, a in answers if a == "missing"])
 
     async def _secagg_setup(self, alive, tag: str, loop, pool, result) -> Optional[Dict[str, Any]]:
         """Secure aggregation's key agreement: every device returns a fresh public key for the training ``tag``, then every

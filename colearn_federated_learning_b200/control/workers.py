@@ -29,6 +29,7 @@ import numpy as np
 import torch
 
 from ..data import dataset_tensors
+from ..fl import fedeval
 from ..fl.trainer import FitConfig, local_fit
 from ..fl.evaluate import predict as predict_fn
 from ..fl.secagg import SecAggDevice
@@ -292,6 +293,26 @@ class WorkerServer:
                 if replica is not None:
                     reply["replica_crc"] = replica_crc(replica)
                 return reply
+        if op == "evaluate":
+            # federated evaluation (fl/fedeval.py): the model in "params" (fp32) scored on the rows hosted under "evaluation";
+            # only the summary's counts leave the device
+            held = self.datasets.get("evaluation")
+            if held is None:
+                return {"ok": False, "eval_missing": True, "error": "no evaluation data on this device"}
+            if "params" not in req:
+                return {"ok": False, "error": "evaluate request without params"}
+            with self._work_lock:
+                try:
+                    model, flat, err = self._model_and_arena(req.get("model"), req["params"])
+                    if err:
+                        return {"ok": False, "error": err}
+                    spec = getattr(model, "spec", None)
+                    if spec is not None and not spec.flatten_input and held[0].shape[1] != spec.dims[0]:
+                        return {"ok": False, "error": f"evaluation data has {held[0].shape[1]} features, {req.get('model')} wants {spec.dims[0]}"}
+                    s = fedeval.summarize(model, flat, held[0], held[1], int(req.get("bins", 256)), float(req.get("threshold", 0.5)))[0]
+                except (ValueError, TypeError) as e:
+                    return {"ok": False, "error": f"evaluation refused: {e}"}
+                return {"ok": True, **fedeval.to_wire(s)}
         if op == "predict":
             data = self.tagged.get(req.get("tag", "inference"), [])
             if not data:
@@ -368,7 +389,7 @@ class RemoteWorkerClient:
         self.bytes_sent = 0
         self.bytes_received = 0
 
-    def _call(self, req: Dict[str, Any], timeout: Optional[float] = None) -> Dict[str, Any]:
+    def _call(self, req: Dict[str, Any], timeout: Optional[float] = None, check: bool = True) -> Dict[str, Any]:
         with self._lock:
             if self._sock is None:
                 raise ConnectionError(f"worker {self.id} is closed")
@@ -386,7 +407,7 @@ class RemoteWorkerClient:
                 finally:
                     self._sock = None
                 raise
-        if not resp.get("ok", False):
+        if check and not resp.get("ok", False):
             raise RuntimeError(f"worker {self.id}: {resp.get('error')}")
         return resp
 
@@ -466,6 +487,12 @@ class RemoteWorkerClient:
         """Round ``t``'s seeds for the survivor list: the reply ``{"self_seed", "pair_seeds"}`` unchecked"""
         resp = self._call({"op": "secagg_unmask", "tag": tag, "t": t, "u2": survivors}, timeout=timeout)
         return {k: resp.get(k) for k in ("self_seed", "pair_seeds")}
+
+    def evaluate(self, flat: torch.Tensor, model_name: str, bins: int, threshold: float, timeout: Optional[float] = None) -> Dict[str, Any]:
+        """Federated evaluation of the fp32 model ``flat``: the device's reply as it came (``ok: False`` with ``eval_missing``
+        when it holds no evaluation data); ``fl.fedeval.from_wire`` checks it."""
+        return self._call({"op": "evaluate", "params": _to_bytes(flat.float()), "model": model_name, "bins": int(bins),
+                           "threshold": float(threshold)}, timeout=timeout, check=False)
 
     def search(self, tag: str) -> int:
         return int(self._call({"op": "search", "tag": tag}).get("count", 0))

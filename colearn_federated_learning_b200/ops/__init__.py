@@ -317,6 +317,30 @@ def eval_binary(p: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch.T
     return reference.eval_binary(p, y)
 
 
+def eval_summary(scores: torch.Tensor, labels: torch.Tensor, bins: int = 256, threshold: float = 0.5,
+                 segments: Optional[Sequence[int]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Detection-metrics summary of model outputs (``ops/csrc/eval_summary.cuh``): ``(counts int64 [S, L], loss_sum float64
+    [S])``, one row per segment of consecutive rows.  ``scores``: ``[N, C]`` (or ``[N]``) fp32 outputs after the output
+    activation, ``labels``: ``[N]``, ``segments``: the row count of every segment (one segment of all rows when None).  Row
+    ``s`` of ``counts`` holds ``n``, ``n_invalid``, the ``C' x C'`` confusion matrix and the ``C x 2 x bins`` score histograms
+    (``fl/fedeval.py`` reads them).  CUDA tensors: one memset and one ``eval_summary_kernel`` launch; CPU tensors:
+    ``reference.eval_summary``."""
+    scores = scores.view(-1, 1) if scores.dim() == 1 else scores
+    n = scores.shape[0]
+    sizes = [n] if segments is None else [int(s) for s in segments]
+    if any(s < 0 for s in sizes) or sum(sizes) != n or not sizes:
+        raise ValueError(f"segments {sizes} do not cover the {n} rows")
+    offsets = [0]
+    for s in sizes:
+        offsets.append(offsets[-1] + s)
+    reference.eval_summary_limits(scores.shape[1], int(bins), float(threshold), n)
+    if _cuda(scores):
+        counts, loss = _ext.require().eval_summary(scores.float().contiguous(), labels.to(scores.device, torch.float32).contiguous().view(-1),
+                                                   torch.tensor(offsets, dtype=torch.int64), int(bins), float(threshold), 0)
+        return counts, loss
+    return reference.eval_summary(scores, labels, int(bins), float(threshold), offsets)
+
+
 def argmax_rows(x: torch.Tensor) -> torch.Tensor:
     """``x.argmax(1, keepdim=True)`` (SURVEY K16; reference inference fc.py:252-256)."""
     if _cuda(x):

@@ -47,7 +47,7 @@ def _stamp(src: str, flags: List[str]) -> str:
     h = hashlib.sha1()
     with open(src, "rb") as f:
         h.update(f.read())
-    for dep in ("colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "mlp_v2.inc", "conv_ops.cuh", "conv_bindings.inc"):
+    for dep in ("colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "mlp_v2.inc", "conv_ops.cuh", "conv_bindings.inc"):
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(flags).encode())
@@ -146,7 +146,7 @@ def build_simt_emul(force: bool = False) -> str:
                                                                         f"-DTORCH_EXTENSION_NAME={SIMT_NAME}"]
     sources = ["simt_emul.cpp", "simt_mlp.cpp", "simt_elementwise.cpp", "simt_comm.cpp", "simt_convnet.cpp", "simt_gemm.cpp"]
     h = hashlib.sha1()
-    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_v2.inc", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "conv_ops.cuh"]:
+    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_v2.inc", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "conv_ops.cuh"]:
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(cxx_flags).encode())

@@ -450,6 +450,31 @@ std::vector<torch::Tensor> eval_binary(torch::Tensor p, torch::Tensor y) {
   check(launch_eval_binary(p.data_ptr<float>(), y.data_ptr<float>(), loss.data_ptr<float>(), correct.data_ptr<int>(), p.numel(), cur_stream()), "eval_binary");
   return {loss, correct};
 }
+// Detection-metrics summary (eval_summary.cuh): scores [N, C] / labels [N] contiguous CUDA fp32 (any 4-byte alignment),
+// offsets CPU int64 [S + 1]; returns (counts int64 [S, es_row_len], loss float64 [S]), views of one output block
+std::vector<torch::Tensor> eval_summary(torch::Tensor scores, torch::Tensor labels, torch::Tensor offsets, int64_t bins, double threshold,
+                                        int64_t grid) {
+  CHECK_CUDA_F32(scores); CHECK_CUDA_F32(labels);
+  TORCH_CHECK(scores.dim() == 2 && labels.dim() == 1 && labels.size(0) == scores.size(0) && labels.device() == scores.device(),
+              "scores [N, C], labels [N] on one device");
+  TORCH_CHECK(!offsets.is_cuda() && offsets.scalar_type() == at::kLong && offsets.is_contiguous() && offsets.dim() == 1 && offsets.numel() >= 2 &&
+              offsets.numel() - 1 <= INT32_MAX, "offsets: CPU int64 [S + 1]");
+  const int C = (int)scores.size(1), S = (int)offsets.numel() - 1;
+  TORCH_CHECK(eval_summary_args_ok(C, (int)bins, (float)threshold), "eval_summary: C in 1..32, bins a power of two in 2..4096 with C * 2 * bins <= 32768, "
+              "threshold in [0, 1] (C = ", C, ", bins = ", bins, ", threshold = ", threshold, ")");
+  std::vector<int64_t> table;
+  const int64_t units = es_build_table(offsets.data_ptr<int64_t>(), S, table);
+  TORCH_CHECK(units >= 0 && table[S] == scores.size(0), "offsets must rise from 0 to N");
+  TORCH_CHECK(scores.size(0) <= kEsMaxRows, "eval_summary: at most 2^32 - 1 rows per launch (uint32 shared-memory counters)");
+  c10::cuda::CUDAGuard guard(scores.device());
+  auto dev_table = torch::from_blob(table.data(), {(int64_t)table.size()}, torch::kLong).to(scores.device());
+  auto out = torch::empty({es_out_words(S, C, (int)bins, units)}, scores.options().dtype(at::kLong));
+  EvalSummaryArgs a{scores.data_ptr<float>(), labels.data_ptr<float>(), dev_table.data_ptr<int64_t>(), S, units, C, (int)bins, (float)threshold,
+                    out.data_ptr<int64_t>()};
+  check(launch_eval_summary(a, (int)grid, cur_stream()), "eval_summary");
+  const int64_t L = es_row_len(C, (int)bins);
+  return {out.narrow(0, 0, S * L).view({S, L}), out.narrow(0, S * L, S).view(at::kDouble)};
+}
 torch::Tensor argmax_rows(torch::Tensor x) {
   CHECK_CUDA_F32(x);
   TORCH_CHECK(x.dim() == 2, "2-D");
@@ -885,6 +910,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_xent", &softmax_xent);
   m.def("softmax_xent_head", &softmax_xent_head);
   m.def("eval_binary", &eval_binary);
+  m.def("eval_summary", &eval_summary);
   m.def("argmax_rows", &argmax_rows);
   m.def("minmax_scale", &minmax_scale);
   m.def("feistel_permutation", &feistel_permutation);

@@ -51,6 +51,8 @@
 #include "distance_agg.cuh"
 // secure aggregation: ChaCha20 mask streams and the fixed-point codec of the masked updates
 #include "secagg.cuh"
+// detection-metrics summary of held-out rows (federated evaluation) shared by its kernel and the reference
+#include "eval_summary.cuh"
 
 namespace colearn {
 // Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
@@ -328,6 +330,9 @@ cudaError_t launch_softmax_xent_head(const void* logits, int logits_is_bf16, int
 cudaError_t launch_eval_binary(const float* p, const float* y, float* loss_sum, int* correct,
                                int64_t n, cudaStream_t s);
 cudaError_t launch_argmax_rows(const float* x, int64_t* out, int rows, int cols, cudaStream_t s);
+// Detection-metrics summary (eval_summary.cuh): one memset of the outputs, then one launch over the (segment, chunk) units.
+// grid <= 0 picks the grid; the result does not depend on it.  cudaErrorInvalidValue outside the limits of eval_summary.cuh.
+cudaError_t launch_eval_summary(const EvalSummaryArgs& a, int grid, cudaStream_t s);
 // Column-wise min/max scaling to [0,1] (NetworkTrafficDataset preprocessing, ds.py:31-32)
 cudaError_t launch_minmax_scale(const float* x, float* out, int rows, int cols, cudaStream_t s);
 // Philox-keyed random permutation of [0, n): writes sort keys; caller argsorts? No — full device

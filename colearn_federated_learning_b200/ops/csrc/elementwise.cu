@@ -1330,6 +1330,160 @@ __global__ void argmax_rows_kernel(const float* __restrict__ x, int64_t* __restr
   }
 }
 
+// ---- detection-metrics summary (eval_summary.cuh) ---------------------------------------------------------------------------
+// One CTA per (segment, chunk) work unit at a time, one thread per row (kEsRowsPerThread rows per thread and chunk).  The counts
+// of the CTA's current segment accumulate in shared memory as uint32 and are flushed (non-zero words, 64-bit atomics) when the
+// CTA moves to another segment and at the end.  A hot bin — a trained detector puts most rows into bin 0 or B - 1 — would take
+// up to 32 shared atomics per warp on one word: the lanes with equal words are matched first and one leader adds the count.
+__device__ __forceinline__ void es_count(unsigned* __restrict__ sm, int word) {
+  const unsigned peers = __match_any_sync(0xffffffffu, word);
+  if (word >= 0 && (int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(sm + word, (unsigned)__popc(peers));
+}
+__device__ __forceinline__ void es_flush(unsigned* __restrict__ sm, int64_t len, int64_t* __restrict__ dst) {
+  __syncthreads();
+  for (int64_t i = threadIdx.x; i < len; i += kEsThreads) {
+    const unsigned v = sm[i];
+    if (v != 0u) {
+      atomicAdd(reinterpret_cast<unsigned long long*>(dst + i), (unsigned long long)v);
+      sm[i] = 0u;
+    }
+  }
+  __syncthreads();
+}
+
+// C = 1: the row's loss (0 for an invalid row), its confusion and histogram words (-1: none)
+__device__ __forceinline__ double es_row_binary(const EvalSummaryArgs& a, int64_t row, bool in, int& conf, int& hist) {
+  conf = hist = -1;
+  if (!in) return 0.0;
+  const float p = a.scores[row];
+  const int y = es_label(a.labels[row], 1);
+  if (!(p >= 0.f && p <= 1.f) || y < 0) return 0.0;            // (NaN fails the range test)
+  conf = (int)es_conf_off() + 2 * y + (p > a.threshold ? 1 : 0);
+  hist = (int)es_hist_off(1) + y * a.bins + es_bin(p, a.bins);
+  return es_bce(p, y);
+}
+
+template <bool MULTI>
+__global__ void __launch_bounds__(kEsThreads) eval_summary_kernel(const EvalSummaryArgs a) {
+  constexpr int kEsFinalTile = 1024;
+  COLEARN_DYN_SMEM(unsigned, sm);
+  __shared__ double red[kEsThreads / 32];
+  __shared__ double tile[kEsFinalTile];
+  __shared__ int s_last;
+  const int C = a.classes, B = a.bins, lane = threadIdx.x & 31;
+  const int64_t L = es_row_len(C, B);
+  const int64_t* offsets = a.table;
+  const int64_t* unit_seg = a.table + a.segments + 1;
+  const int64_t* seg_unit0 = unit_seg + a.units;
+  int64_t* counts = a.out;
+  double* loss = reinterpret_cast<double*>(a.out + (int64_t)a.segments * L);
+  unsigned* ticket = reinterpret_cast<unsigned*>(a.out + (int64_t)a.segments * L + a.segments);
+  double* partial = reinterpret_cast<double*>(a.out + (int64_t)a.segments * L + a.segments + 1);
+  for (int64_t i = threadIdx.x; i < L; i += kEsThreads) sm[i] = 0u;
+  int64_t cur = -1;
+  __syncthreads();
+  for (int64_t u = blockIdx.x; u < a.units; u += gridDim.x) {
+    const int64_t s = unit_seg[u];
+    if (s != cur) {
+      if (cur >= 0) es_flush(sm, L, counts + cur * L);
+      cur = s;
+    }
+    const int64_t r0 = offsets[s] + (u - seg_unit0[s]) * kEsChunk;
+    const int64_t r1 = r0 + kEsChunk < offsets[s + 1] ? r0 + kEsChunk : offsets[s + 1];
+    double acc = 0.0;
+    if (!MULTI) {
+      int conf[kEsRowsPerThread], hist[kEsRowsPerThread];
+      double l[kEsRowsPerThread];
+#pragma unroll
+      for (int i = 0; i < kEsRowsPerThread; ++i) {
+        const int64_t row = r0 + threadIdx.x + (int64_t)i * kEsThreads;
+        l[i] = es_row_binary(a, row, row < r1, conf[i], hist[i]);
+      }
+      int bad = 0;
+#pragma unroll
+      for (int i = 0; i < kEsRowsPerThread; ++i) {
+        acc += l[i];
+        bad += (r0 + threadIdx.x + (int64_t)i * kEsThreads < r1 && conf[i] < 0) ? 1 : 0;
+        es_count(sm, conf[i]);
+        es_count(sm, hist[i]);
+      }
+      bad = __reduce_add_sync(0xffffffffu, bad);
+      if (lane == 0 && bad != 0) atomicAdd(sm + 1, (unsigned)bad);
+    } else {
+      int bad = 0;
+      for (int i = 0; i < kEsRowsPerThread; ++i) {
+        const int64_t row = r0 + threadIdx.x + (int64_t)i * kEsThreads;
+        const bool in = row < r1;
+        const float* z = a.scores + row * C;
+        // pass 1: finite, max, argmax (on finite scores argmax_takes is v > best: the lowest index among equals)
+        int y = -1, arg = 0;
+        float m = 0.f;
+        if (in) {
+          y = es_label(a.labels[row], C);
+          bool finite = true;
+          for (int c = 0; c < C; ++c) {
+            const float v = z[c];
+            finite = finite && isfinite(v);
+            if (c == 0 || v > m) { m = v; arg = c; }
+          }
+          if (!finite) y = -1;
+          bad += y < 0 ? 1 : 0;
+        }
+        // pass 2 (from L1): the float64 softmax denominator and the loss
+        double sum = 0.0;
+        if (y >= 0) {
+          for (int c = 0; c < C; ++c) sum += exp((double)z[c] - (double)m);
+          acc += log(sum) - ((double)z[y] - (double)m);
+        }
+        es_count(sm, y >= 0 ? (int)es_conf_off() + C * y + arg : -1);
+        // pass 3 (from L1): the histogram of every class's softmax score
+        for (int c = 0; c < C; ++c) {
+          int word = -1;
+          if (y >= 0) word = (int)es_hist_off(C) + (2 * c + (y == c ? 1 : 0)) * B + es_bin(exp((double)z[c] - (double)m) / sum, B);
+          es_count(sm, word);
+        }
+      }
+      bad = __reduce_add_sync(0xffffffffu, bad);
+      if (lane == 0 && bad != 0) atomicAdd(sm + 1, (unsigned)bad);
+    }
+    acc = warp_tree_f64(acc);
+    if (lane == 0) red[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double t = red[0];
+#pragma unroll
+      for (int w = 1; w < kEsThreads / 32; ++w) t += red[w];
+      partial[u] = t;
+      sm[0] += (unsigned)(r1 - r0);
+    }
+    __syncthreads();
+  }
+  if (cur >= 0) es_flush(sm, L, counts + cur * L);
+  // the last CTA adds every segment's chunk sums in chunk order
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = atomicAdd(ticket, 1u) == gridDim.x - 1 ? 1 : 0;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  // The partials come into shared memory a tile at a time, loaded by the whole CTA (one L2 round trip per chunk in the adding
+  // thread would cost ~50 us at the full Bot-IoT set); a segment's running sum waits in loss[s] (zeroed by the launcher).
+  for (int64_t base = 0; base < a.units; base += kEsFinalTile) {
+    const int64_t n = a.units - base < kEsFinalTile ? a.units - base : kEsFinalTile;
+    for (int64_t i = threadIdx.x; i < n; i += kEsThreads) tile[i] = __ldcg(partial + base + i);
+    __syncthreads();
+    for (int64_t s = threadIdx.x; s < a.segments; s += kEsThreads) {
+      const int64_t lo = seg_unit0[s] > base ? seg_unit0[s] : base, hi = seg_unit0[s + 1] < base + n ? seg_unit0[s + 1] : base + n;
+      if (lo >= hi) continue;
+      double t = loss[s];
+      for (int64_t u = lo; u < hi; ++u) t += tile[u - base];
+      loss[s] = t;
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *ticket = 0u;
+}
+
 // MinMax: one block per column pass 1 (min/max), pass 2 scale.  cols is tiny (10).
 __global__ void minmax_scale_kernel(const float* __restrict__ x, float* __restrict__ out, int rows, int cols) {
   __shared__ float smin[32], smax[32];
@@ -1748,6 +1902,26 @@ cudaError_t launch_eval_binary(const float* p, const float* y, float* loss_sum, 
   e = cudaMemsetAsync(correct, 0, sizeof(int), s);
   if (e != cudaSuccess) return e;
   COLEARN_LAUNCH(eval_binary_kernel, grid_for(n, 1), kThreads, 0, s, p, y, loss_sum, correct, n);
+  return cudaGetLastError();
+}
+cudaError_t launch_eval_summary(const EvalSummaryArgs& a, int grid, cudaStream_t s) {
+  if (!eval_summary_args_ok(a.classes, a.bins, a.threshold) || a.segments < 1 || a.units < 0 ||
+      (reinterpret_cast<uintptr_t>(a.out) & 7) != 0)
+    return cudaErrorInvalidValue;
+  const int64_t L = es_row_len(a.classes, a.bins);
+  cudaError_t e = cudaMemsetAsync(a.out, 0, (size_t)((int64_t)a.segments * L + a.segments + 1) * sizeof(int64_t), s);
+  if (e != cudaSuccess || a.units == 0) return e;
+  const size_t smem = (size_t)L * sizeof(unsigned);
+  auto kernel = a.classes == 1 ? eval_summary_kernel<false> : eval_summary_kernel<true>;
+  e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  if (grid <= 0) {
+    int dev = 0, sms = 0;
+    if ((e = cudaGetDevice(&dev)) != cudaSuccess || (e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess)
+      return e;
+    grid = (int)(a.units < 4 * sms ? a.units : 4 * sms);
+  }
+  COLEARN_LAUNCH(kernel, grid, kEsThreads, smem, s, a);
   return cudaGetLastError();
 }
 cudaError_t launch_argmax_rows(const float* x, int64_t* out, int rows, int cols, cudaStream_t s) {

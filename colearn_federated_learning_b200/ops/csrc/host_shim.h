@@ -193,6 +193,14 @@ inline unsigned __ballot_sync(unsigned, int pred) {
   for (int i = 0; i < 32; ++i) m |= (all[i] != 0 ? 1u : 0u) << i;
   return m;
 }
+inline unsigned __match_any_sync(unsigned, int v) {
+  int all[32];
+  ::colearn_shim::warp_gather(v, all);
+  unsigned m = 0;
+  for (int i = 0; i < 32; ++i) m |= (all[i] == v ? 1u : 0u) << i;
+  return m;
+}
+inline int __ffs(unsigned v) { return __builtin_ffs((int)v); }
 template <class T>
 inline T __ldcs(const T* p) { return *p; }
 inline float __uint_as_float(unsigned u) { float f; memcpy(&f, &u, 4); return f; }

@@ -326,6 +326,26 @@ std::tuple<Tensor, Tensor> eval_binary(Tensor p, Tensor y) {
   CK(colearn::launch_eval_binary(fptr(p, "p"), fptr(y, "y"), loss.data_ptr<float>(), correct.data_ptr<int>(), p.numel(), nullptr));
   return {loss, correct};
 }
+// detection-metrics summary: same arguments and results as bindings.cpp::eval_summary on CPU tensors; grid <= 0 picks it
+std::tuple<Tensor, Tensor> eval_summary(Tensor scores, Tensor labels, Tensor offsets, int64_t bins, double threshold, int64_t grid) {
+  TORCH_CHECK(scores.dim() == 2 && labels.dim() == 1 && labels.size(0) == scores.size(0), "scores [N, C], labels [N]");
+  TORCH_CHECK(offsets.scalar_type() == at::kLong && offsets.is_contiguous() && offsets.dim() == 1 && offsets.numel() >= 2, "offsets int64 [S + 1]");
+  const int C = (int)scores.size(1), S = (int)offsets.numel() - 1;
+  TORCH_CHECK(colearn::eval_summary_args_ok(C, (int)bins, (float)threshold), "eval_summary: arguments outside the limits");
+  std::vector<int64_t> table;
+  const int64_t units = colearn::es_build_table(offsets.data_ptr<int64_t>(), S, table);
+  TORCH_CHECK(units >= 0 && table[S] == scores.size(0), "offsets must rise from 0 to N");
+  TORCH_CHECK(scores.size(0) <= colearn::kEsMaxRows, "eval_summary: at most 2^32 - 1 rows per launch (uint32 shared-memory counters)");
+  Tensor out = torch::empty({colearn::es_out_words(S, C, (int)bins, units)}, torch::kLong);
+  colearn::EvalSummaryArgs a{fptr(scores, "scores"), fptr(labels, "labels"), table.data(), S, units, C, (int)bins, (float)threshold,
+                             out.data_ptr<int64_t>()};
+  {
+    py::gil_scoped_release nogil;
+    CK(colearn::launch_eval_summary(a, (int)grid, nullptr));
+  }
+  const int64_t L = colearn::es_row_len(C, (int)bins);
+  return {out.narrow(0, 0, S * L).view({S, L}), out.narrow(0, S * L, S).view(at::kDouble)};
+}
 Tensor argmax_rows(Tensor x) {
   Tensor out = torch::zeros({x.size(0), 1}, torch::kLong);
   CK(colearn::launch_argmax_rows(fptr(x, "x"), out.data_ptr<int64_t>(), (int)x.size(0), (int)x.size(1), nullptr));
@@ -612,6 +632,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_xent", &softmax_xent);
   m.def("softmax_xent_head", &softmax_xent_head);
   m.def("eval_binary", &eval_binary);
+  m.def("eval_summary", &eval_summary);
   m.def("argmax_rows", &argmax_rows);
   m.def("minmax_scale", &minmax_scale);
   m.def("feistel_permutation", &feistel_permutation);

@@ -75,6 +75,21 @@ int main() {
     CK(launch_eval_binary(p.data(), yv.data(), loss.data(), &correct, n, nullptr));
     std::vector<int64_t> am(100);
     CK(launch_argmax_rows(logits.data(), am.data(), 100, 10, nullptr));
+    // detection-metrics summary: matched shared-memory counts, segment switches inside a CTA (flush), the ticket finalisation;
+    // C = 1 over 3 uneven segments (one empty) on 2 CTAs, then C = 10
+    {
+      const int64_t offs[4] = {0, 2100, 2100, 3000};
+      std::vector<int64_t> table;
+      const int64_t units = es_build_table(offs, 3, table);
+      std::vector<float> ylab(3000);
+      for (auto& v : ylab) v = (float)(rand() % 10);
+      std::vector<int64_t> out1(es_out_words(3, 1, 64, units)), out10(es_out_words(3, 10, 64, units));
+      EvalSummaryArgs ea{p.data(), yv.data(), table.data(), 3, units, 1, 64, 0.5f, out1.data()};
+      CK(launch_eval_summary(ea, 2, nullptr));
+      std::vector<float> z10 = randv(3000 * 10);
+      EvalSummaryArgs eb{z10.data(), ylab.data(), table.data(), 3, units, 10, 64, 0.5f, out10.data()};
+      CK(launch_eval_summary(eb, 2, nullptr));
+    }
     std::vector<float> feats = randv(200 * 10), scaled(2000);
     CK(launch_minmax_scale(feats.data(), scaled.data(), 200, 10, nullptr));
     std::vector<__nv_bfloat16> tin(70 * 45), tout(70 * 45);

@@ -747,3 +747,74 @@ def eval_binary(out: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch
 
 def argmax_rows(out: torch.Tensor) -> torch.Tensor:
     return out.argmax(1, keepdim=True)
+
+
+def eval_summary_limits(classes: int, bins: int, threshold: float, rows: int = 0) -> None:
+    """The limits of ``ops/csrc/eval_summary.cuh``: ValueError with the reason outside them"""
+    if rows >= 1 << 32:
+        raise ValueError(f"eval_summary: {rows} rows, at most 2^32 - 1 per call (the kernel counts in uint32 shared memory)")
+    if not 1 <= classes <= 32:
+        raise ValueError(f"eval_summary: {classes} output columns, the summary takes 1 to 32")
+    if bins < 2 or bins > 4096 or bins & (bins - 1):
+        raise ValueError(f"eval_summary: bins must be a power of two in [2, 4096], not {bins}")
+    if classes * 2 * bins > 32768:
+        raise ValueError(f"eval_summary: {classes} histograms of 2 x {bins} bins exceed the 32768 counters of one summary")
+    if not 0.0 <= threshold <= 1.0:
+        raise ValueError(f"eval_summary: the threshold must be in [0, 1], not {threshold}")
+
+
+def eval_summary(scores: torch.Tensor, labels: torch.Tensor, bins: int = 256, threshold: float = 0.5,
+                 offsets: Optional[Sequence[int]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """PyTorch transcription of ``ops/csrc/eval_summary.cuh``: ``(counts int64 [S, L], loss_sum float64 [S])`` of the rows
+    ``offsets[s] .. offsets[s + 1]`` of ``scores [N, C]`` / ``labels [N]`` (one segment of all rows when ``offsets`` is None).
+    The loss sums its 2048-row chunks in chunk order (inside a chunk torch's own order: equal to the kernel's to ~1e-15)."""
+    scores = scores.detach().float().cpu()
+    scores = scores.view(-1, 1) if scores.dim() == 1 else scores
+    n, c = scores.shape
+    eval_summary_limits(c, bins, threshold, n)
+    y = labels.detach().float().cpu().reshape(-1)
+    offsets = [0, n] if offsets is None else [int(o) for o in offsets]
+    cp = 2 if c == 1 else c
+    conf0, hist0 = 2, 2 + cp * cp
+    length = hist0 + c * 2 * bins
+    lab_ok = (y >= 0) & (y < cp) & (y == torch.floor(y))
+    if c == 1:
+        p = scores[:, 0]
+        valid = (p >= 0) & (p <= 1) & lab_ok
+        p = torch.where(valid, p, torch.zeros_like(p))
+        yi = torch.where(valid, y, torch.zeros_like(y)).long()
+        pd = p.double()
+        row_loss = torch.where(yi == 1, -torch.log(pd).clamp(min=-100.0), -torch.log1p(-pd).clamp(min=-100.0))
+        b = (p * float(bins)).long().clamp(max=bins - 1)
+        words = [conf0 + 2 * yi + (p > threshold).long(), hist0 + yi * bins + b]
+    else:
+        valid = torch.isfinite(scores).all(1) & lab_ok
+        z = torch.where(valid[:, None], scores, torch.zeros_like(scores))
+        yi = torch.where(valid, y, torch.zeros_like(y)).long()
+        m, arg = z.max(1).values, z.argmax(1)
+        e = torch.exp(z.double() - m.double()[:, None])
+        s = e[:, 0].clone()
+        for k in range(1, c):
+            s = s + e[:, k]
+        row_loss = torch.log(s) - (z.double().gather(1, yi[:, None])[:, 0] - m.double())
+        b = ((e / s[:, None]) * float(bins)).long().clamp(max=bins - 1)
+        cls = torch.arange(c)
+        words = [conf0 + c * yi + arg] + [hist0 + (2 * k + (yi == k).long()) * bins + b[:, k] for k in cls.tolist()]
+    row_loss = torch.where(valid, row_loss, torch.zeros_like(row_loss))
+    counts = torch.zeros(len(offsets) - 1, length, dtype=torch.int64)
+    loss = torch.zeros(len(offsets) - 1, dtype=torch.float64)
+    for s_idx, (lo, hi) in enumerate(zip(offsets[:-1], offsets[1:])):
+        if lo > hi or lo < 0 or hi > n:
+            raise ValueError("offsets must rise from 0 to N")
+        v = valid[lo:hi]
+        counts[s_idx, 0] = hi - lo
+        counts[s_idx, 1] = int((~v).sum())
+        for w in words:
+            counts[s_idx] += torch.bincount(w[lo:hi][v], minlength=length)
+        total = 0.0
+        for q in range(lo, hi, 2048):
+            total += float(row_loss[q:min(q + 2048, hi)].sum())
+        loss[s_idx] = total
+    if offsets[0] != 0 or offsets[-1] != n:
+        raise ValueError("offsets must rise from 0 to N")
+    return counts, loss

@@ -332,7 +332,10 @@ def round_record(round_idx: int, mask: int, world: int, counts: List[int], losse
 
 
 def _run_rounds_observed(engine: FederatedEngine, mask: int, rounds: int, rank: int, world: int, metrics_path: Optional[str],
-                         save_every: int, checkpoint: str, round0: int = 0) -> None:
+                         save_every: int, checkpoint: str, round0: int = 0, fed_eval=None) -> Optional[Dict[str, Any]]:
+    """``fed_eval``: ``(every, bins, threshold)`` of the federated evaluation run after every ``every``-th round and the last one
+    (a collective: every rank takes part); the last evaluation's record is returned."""
+    last_eval = None
     t0 = time.time()
     total_ms = 0.0
     for i in range(rounds):
@@ -345,6 +348,15 @@ def _run_rounds_observed(engine: FederatedEngine, mask: int, rounds: int, rank: 
             losses = rep.losses[0, :, 0].tolist() if rep.losses is not None else [0.0] * world
             rec = round_record(round0 + i, mask, world, engine.counts, losses, float(ms), rep.bytes_bcast, rep.bytes_reduce,
                                rep.launches, rep.algo, rep.extra.get("phases_ms"))
+        evaluated = fed_eval is not None and ((i + 1) % fed_eval[0] == 0 or i + 1 == rounds)
+        if evaluated:
+            from ..fl import fedeval
+            sums = engine.evaluate_federated(fed_eval[1], fed_eval[2])
+            last_eval = fedeval.record({"%s:%d" % rank_identity(k): s for k, s in enumerate(sums)})
+        if rank == 0:
+            if evaluated:
+                rec["fed_eval"] = last_eval
+                log.info("Federated evaluation round %d: %s", round0 + i, fedeval.summary_line(last_eval["total"]))
             for k, l in zip([k for k in range(world) if (mask >> k) & 1], rec["loss_k"]):
                 log.info("Loss for worker id: %s tensor(%.4f)", "%s:%d" % rank_identity(k), l)
             log.info("Time round %d : %s", i, rec["t_round_max_over_ranks_ms"] * 1e-3)
@@ -356,6 +368,7 @@ def _run_rounds_observed(engine: FederatedEngine, mask: int, rounds: int, rank: 
                 log.info("checkpoint after round %d written to %s", i + 1, checkpoint)
     if rank == 0:
         log.info("Total training time: %s (device %.3f ms for %d rounds)", time.time() - t0, total_ms, rounds)
+    return last_eval
 
 
 class BoxService:
@@ -392,7 +405,20 @@ class BoxService:
             x, y = NetworkTrafficDataset(args.test_path).tensors()
         from ..data import shard_bounds
         lo, hi = shard_bounds(len(x), world)[rank]
-        self.engine.set_local_data(x[lo:hi], y[lo:hi])
+        self.fed_eval = None
+        if args.fed_eval_every > 0:
+            # federated evaluation: every rank holds --eval-fraction of its shard out (keyed by its rank) and scores theta on it
+            from ..fl.fedeval import check_model, split_eval
+            args.fed_eval_settings()
+            check_model(self.engine.model)
+            if not args.eval_fraction > 0:
+                raise SystemExit("--box --fed-eval-every needs --eval-fraction > 0")
+            xt, yt, xe, ye = split_eval(x[lo:hi], y[lo:hi], args.eval_fraction, args.seed + rank)
+            self.engine.set_local_data(xt, yt)
+            self.engine.set_eval_data(xe, ye)
+            self.fed_eval = (args.fed_eval_every, args.eval_bins, args.eval_threshold)
+        else:
+            self.engine.set_local_data(x[lo:hi], y[lo:hi])
         self.eval_data = (x, y) if (rank == 0 and getattr(cli, "evaluate", False)) else None
         n_inf = int(getattr(cli, "box_inference_rows", 5) or 0)
         self.inference_x = x[lo:hi][:n_inf].clone()          # the device's "inference"-tagged tensors (rw.py:97-104)
@@ -421,10 +447,13 @@ class BoxService:
         t0 = time.time()
         save_every = max(0, getattr(self.args, "save_every", 0))
         metrics_path = getattr(cli, "metrics", None)
-        if metrics_path or save_every:
+        fed_eval = None
+        if metrics_path or save_every or self.fed_eval is not None:
             # observable mode: one engine call per round, so every round gets its own device time (max over ranks), traffic /
-            # link-roofline figures and, if asked for, a checkpoint.  Without these flags all rounds are enqueued in one call
-            _run_rounds_observed(self.engine, mask, rounds, rank, world, metrics_path, save_every, cli.checkpoint, self.rounds_done)
+            # link-roofline figures and, if asked for, a checkpoint and the federated evaluation.  Without these flags all rounds
+            # are enqueued in one call
+            fed_eval = _run_rounds_observed(self.engine, mask, rounds, rank, world, metrics_path, save_every, cli.checkpoint,
+                                            self.rounds_done, self.fed_eval)
             losses = None
         else:
             rep = self.engine.run_rounds(rounds, masks=mask)
@@ -438,6 +467,8 @@ class BoxService:
         self.rounds_done += rounds
         self.trainings_done += 1
         result: Dict[str, Any] = {"training": self.trainings_done, "mask": mask, "rounds": rounds}
+        if fed_eval is not None:
+            result["fed_eval"] = fed_eval
         if rank == 0:
             self.engine.save_checkpoint(cli.checkpoint)
             if losses is not None:

@@ -242,6 +242,33 @@ class FederatedEngine:
         else:
             self.counts = [self.n_local]
 
+    def set_eval_data(self, x: torch.Tensor, y: torch.Tensor) -> None:
+        """Attach this rank's held-out rows for :meth:`evaluate_federated` (device-resident from here on)."""
+        self.eval_x = x.to(self.device).float().contiguous()
+        self.eval_y = y.to(self.device).float().reshape(-1).contiguous()
+
+    def evaluate_federated(self, bins: int = 256, threshold: float = 0.5) -> List[Any]:
+        """Federated evaluation (fl/fedeval.py), a collective: theta is broadcast from the coordinator as INFERENCE does, every
+        rank summarizes its held-out rows (``set_eval_data``) and the int64 counts / float64 loss sums are all-gathered.
+        Returns every rank's :class:`fl.fedeval.Summary` in rank order (their sum is the total)."""
+        from ..fl import fedeval
+        theta = self.global_flat().detach().clone()
+        multi = _dist_ready() and self.world > 1
+        if multi:
+            dist.broadcast(theta, src=self.coord, group=self.group)
+        mine = fedeval.summarize(self.model, theta, self.eval_x, self.eval_y, bins, threshold)[0]
+        if not multi:
+            return [mine]
+        dev = self.device if self.backend != "cpu" else torch.device("cpu")
+        words = torch.tensor([mine.n, mine.n_invalid, *mine.counts.tolist()], dtype=torch.int64, device=dev)
+        loss = torch.tensor([mine.loss_sum], dtype=torch.float64, device=dev)
+        all_words = [torch.empty_like(words) for _ in range(self.world)]
+        all_loss = [torch.empty_like(loss) for _ in range(self.world)]
+        dist.all_gather(all_words, words, group=self.group)
+        dist.all_gather(all_loss, loss, group=self.group)
+        return [fedeval.Summary(mine.classes, mine.bins, int(w[0]), int(w[1]), float(l[0]), w[2:].cpu().numpy())
+                for w, l in zip(all_words, all_loss)]
+
     def server_state(self) -> Dict[str, Optional[torch.Tensor]]:
         """This rank's server optimizer moments ``{"m", "v"}`` (first P elements; None where the kind or the rank has none).
         Two-shot path: only the chunks this rank owns are ever updated."""

@@ -38,6 +38,11 @@ class PrometheusExporter:
         self.selected = Gauge("colearn_round_selected_workers", "devices that contributed to the last round", **mk)
         self.worker_loss = Gauge("colearn_worker_last_loss", "last local loss reported by a device", ["worker"], **mk)
         self.training_seconds = Gauge("colearn_last_training_seconds", "total time of the last training", **mk)
+        # federated evaluation (--fed-eval-every): the total over the devices of the last evaluated round
+        self.eval_loss = Gauge("colearn_eval_loss", "federated evaluation: mean loss of the global model on the devices' held-out rows", **mk)
+        self.eval_accuracy = Gauge("colearn_eval_accuracy", "federated evaluation: accuracy of the global model", **mk)
+        self.eval_auc = Gauge("colearn_eval_auc", "federated evaluation: ROC-AUC (macro one-vs-rest for multi-class models)", **mk)
+        self.eval_f1 = Gauge("colearn_eval_f1", "federated evaluation: F1 (macro for multi-class models)", **mk)
         self.server, self.thread = start_http_server(port, addr=addr, registry=self.registry)
         self.port = self.server.server_port
 
@@ -75,6 +80,16 @@ class RoundLogger:
 
     def end_round(self, round_idx: int, seconds: float, **fields: Any) -> Dict[str, Any]:
         self._text(f"Time round {round_idx} : {seconds}")
+        fed_eval = fields.get("fed_eval")
+        if fed_eval is not None:
+            from ..fl.fedeval import summary_line
+            total = fed_eval.get("total") or {}
+            self._text(f"Federated evaluation round {round_idx}: {summary_line(total)}")
+            if self.exporter is not None:
+                for gauge, key in ((self.exporter.eval_loss, "loss"), (self.exporter.eval_accuracy, "accuracy"),
+                                   (self.exporter.eval_auc, "auc"), (self.exporter.eval_f1, "f1")):
+                    if total.get(key) is not None:
+                        gauge.set(float(total[key]))
         rec = {"round": round_idx, "t_round_s": seconds, "ts": time.time(), **fields}
         if self.exporter is not None:
             self.exporter.rounds.inc()

@@ -111,6 +111,16 @@ def build_parser() -> argparse.ArgumentParser:
     parser.add_argument("--round-log", type=str, default=None, help="write the reference-format round log here")
     parser.add_argument("--metrics-port", type=int, default=0, help="serve Prometheus metrics (rounds, round time, losses, traffic) on this port")
     parser.add_argument("--evaluate", action="store_true", help="evaluate the global model on --test-path after training")
+    parser.add_argument("--fed-eval-every", type=int, default=d.fed_eval_every, metavar="N",
+                        help="federated evaluation: after every N-th round and after the last one the devices score the global model on "
+                             "rows they keep out of training and return counts; the round record gets fed_eval (detection rate, "
+                             "false-alarm rate, precision, F1, ROC-AUC, average precision). 0 = off")
+    parser.add_argument("--eval-bins", type=int, default=d.eval_bins, help="--fed-eval-every: score histogram bins (power of two, 2..4096)")
+    parser.add_argument("--eval-threshold", type=float, default=d.eval_threshold,
+                        help="--fed-eval-every: a one-column model flags a row as an attack iff its score is above this")
+    parser.add_argument("--eval-fraction", type=float, default=d.eval_fraction,
+                        help="--fed-eval-every in local and box mode: fraction of every device's shard held out for evaluation, in (0, 1) "
+                             "(remote devices hold theirs out themselves: remote_worker.py -de / --eval-fraction)")
     parser.add_argument("--embedded-broker", action="store_true", help="start the TCP bus broker inside this process")
     parser.add_argument("--tls-ca", default=None, help="CA bundle: verify the broker / the devices (and, with --tls-cert on the embedded broker, demand client certificates)")
     parser.add_argument("--tls-cert", default=None, help="certificate for the embedded broker / client certificate towards broker and devices")
@@ -170,6 +180,11 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
         a.n_train_items_enc = int(ns.enc_items)
     a.dtype, a.save_every = ns.dtype, max(0, ns.save_every)
     a.dataset = ns.dataset
+    a.fed_eval_every = getattr(ns, "fed_eval_every", a.fed_eval_every)
+    a.eval_bins = getattr(ns, "eval_bins", a.eval_bins)
+    a.eval_threshold = getattr(ns, "eval_threshold", a.eval_threshold)
+    a.eval_fraction = getattr(ns, "eval_fraction", a.eval_fraction)
+    a.fed_eval_settings()             # rejects bins / threshold / fraction outside their ranges and --secure-agg with it
     return a
 
 
@@ -259,6 +274,20 @@ def parse_cli(argv=None) -> argparse.Namespace:
     if ns.aggregator in ("geomed", "norm_clip") and (ns.box or ns.encryption):
         parser.error(f"--aggregator {ns.aggregator} applies to the local and remote modes only: --box reduces the models across the "
                      "GPUs in one pass (no per-step distances) and -e exchanges secret shares")
+    if ns.fed_eval_every > 0:
+        if ns.encryption:
+            parser.error("--fed-eval-every applies to the local, remote and box modes: -e exchanges secret shares")
+        if not ns.remote and not ns.eval_fraction > 0:
+            parser.error("--fed-eval-every in local and box mode needs --eval-fraction > 0: the rows every device holds out")
+        if ns.remote and ns.eval_fraction > 0:
+            parser.error("--eval-fraction applies to local and box mode: remote devices hold their evaluation rows out themselves "
+                         "(remote_worker.py -de / --eval-fraction)")
+        from colearn_federated_learning_b200.fl.fedeval import check_model
+        from colearn_federated_learning_b200.models import build_model
+        try:
+            check_model(build_model(ns.model))
+        except ValueError as e:
+            parser.error(f"--fed-eval-every with --model {ns.model}: {e}")
     if ns.secure_agg:
         if ns.box or ns.encryption or not ns.remote:
             parser.error("--secure-agg applies to remote mode (-r) only: in local mode every update is in the coordinator's process "

@@ -6,7 +6,8 @@
 
 The host MUST be given as an IP (it is what the coordinator parses out of the event).  The worker
 hosts its dataset under key ``"training"`` (rw.py:108), optional inference tensors tagged
-``"inference"`` (rw.py:102-104), announces itself on the bus after ``--wait`` seconds
+``"inference"`` (rw.py:102-104), an optional held-out set under ``"evaluation"`` (``-de`` / ``--eval-fraction``) for
+federated evaluation, announces itself on the bus after ``--wait`` seconds
 (rw.py:110-114) and then serves fit/search/predict RPCs forever (rw.py:117).
 """
 import argparse
@@ -31,6 +32,10 @@ _OPTIONS = (
     (("--training", "-dt"), dict(type=str, default=None, help="Bot-IoT CSV hosted as the private training set")),
     (("--inference", "-di"), dict(type=str, default=None, help="Bot-IoT CSV whose rows are hosted as inference tensors")),
     (("--verbose", "-v"), dict(action="store_true", help="log every RPC")),
+    (("--evaluation", "-de"), dict(type=str, default=None, help="CSV hosted as the held-out set the coordinator's federated "
+                                                                 "evaluation scores the global model on (only counts leave the device)")),
+    (("--eval-fraction",), dict(type=float, default=0.0, help="hold this fraction of the training rows out as the evaluation set "
+                                                              "(a seeded random subset, see fl/fedeval.py split_eval), in (0, 1)")),
     (("--broker-port",), dict(type=int, default=1883)),
     (("--synthetic",), dict(type=int, default=0, help="host N synthetic rows instead of --training")),
     (("--data-model",), dict(default="ffnn", help="architecture the synthetic data is shaped for (resnet18: 32x32 images, net: "
@@ -91,6 +96,15 @@ def main(args: argparse.Namespace) -> None:  # pragma: no cover - exercised by t
     server = WorkerServer(identity, args.host, args.port, device=torch.device("cuda" if on_gpu else "cpu"), verbose=args.verbose,
                           ssl_context=rpc_tls)
     server.add_dataset(pick_dataset(args), key="training")                       # rw.py:108
+    if args.evaluation and args.eval_fraction > 0:
+        raise SystemExit("-de and --eval-fraction both define the evaluation set: give one of them")
+    if args.evaluation:
+        logging.info("evaluation data: %s", args.evaluation)
+        server.add_dataset(load_dataset(args.dataset, args.evaluation), key="evaluation")
+    elif args.eval_fraction > 0:
+        from colearn_federated_learning_b200.fl.fedeval import split_eval
+        xt, yt, xe, ye = split_eval(*server.datasets["training"], args.eval_fraction, args.seed)
+        server.datasets["training"], server.datasets["evaluation"] = (xt, yt), (xe, ye)
     if args.inference:
         logging.info("inference data: %s", args.inference)
         rows = load_dataset(args.dataset, args.inference).data
