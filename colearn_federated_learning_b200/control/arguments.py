@@ -58,6 +58,11 @@ class Arguments:
     eval_bins: int = 256           # federated evaluation: score histogram bins, a power of two in [2, 4096]
     eval_threshold: float = 0.5    # federated evaluation: a one-column model predicts the positive class iff p > threshold
     eval_fraction: float = 0.0     # federated evaluation, local and box mode: fraction of every device's shard held out, in (0, 1)
+    async_buffer: int = 0          # remote mode: >0 = asynchronous buffered aggregation, one server step per K replies from devices
+                                   # that train from whatever version is current (fl/asyncagg.py); 0 = synchronous rounds
+    async_concurrency: int = 0     # asynchronous: fits in flight (0 = one per selected device)
+    max_staleness: int = 4         # asynchronous: replies trained from a model more than S versions old are dropped
+    staleness_exponent: float = 0.5  # asynchronous: a reply of staleness tau weighs (1 + tau)^-a
     backend: str = "auto"          # auto | fused | nccl | cpu
     dtype: str = "fp32"            # fp32 | bf16 (box mode: bf16 shadow of the broadcast for the wgmma consumers)
     save_every: int = 0            # >0: checkpoint every N rounds, not only after the last one
@@ -138,6 +143,19 @@ class Arguments:
         if self.fed_eval_every > 0 and self.secure_agg:
             raise ValueError("--fed-eval-every does not combine with --secure-agg: every device's counts (and with them the label mix "
                              "of its data, which secure aggregation hides) would travel in the clear")
+
+    def async_settings(self):
+        """The :class:`fl.asyncagg.AsyncSettings` of the ``async_*`` fields, None for synchronous rounds; refuses the settings it
+        cannot run with whatever the mode: secure aggregation (its masks cancel only over a synchronous cohort) and a compressed
+        downlink (one coordinator replica is only valid when every device has seen every broadcast)."""
+        from ..fl.asyncagg import optional_settings
+        st = optional_settings(self.async_buffer, self.async_concurrency, self.max_staleness, self.staleness_exponent)
+        if st is not None and self.secure_agg:
+            raise ValueError("--async-buffer does not combine with --secure-agg: the pairwise masks cancel only over a synchronous cohort")
+        if st is not None and self.downlink != "fp32":
+            raise ValueError(f"--async-buffer does not combine with --downlink-codec {self.downlink}: the coordinator's one replica is "
+                             "only valid when every device has seen every broadcast")
+        return st
 
     def set_federated_batches(self, batches: int) -> None:
         self.federate_after_n_batches = batches

@@ -33,7 +33,7 @@ from .. import ops, settings
 from ..data import federate, synthetic_for_model, BaseDataset
 from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
-from ..fl import fedeval
+from ..fl import asyncagg, fedeval
 from ..fl.evaluate import evaluate
 from ..fl.secagg import check_masked_reply, check_unmask_reply, correction_streams, frac_bits, pk_from_bytes, pk_to_bytes
 from ..fl.server_opt import server_opt_state
@@ -304,6 +304,8 @@ class Coordinator(BusClient):
         if not to_train:
             log.info("No behaviour defined for the number of devices achieved")
             return None
+        if self.args.async_buffer:
+            raise ValueError("--async-buffer applies to remote mode only: local mode trains its virtual workers in lockstep launches")
         model = self._load_model()
         cfg = self._fit_config("local")
 
@@ -440,8 +442,9 @@ class Coordinator(BusClient):
         self.metrics.start_training(cfg.max_nr_batches)
         result: Dict[str, Any] = {"workers": list(to_train.keys()), "losses": {}, "rounds": self.enabled_round, "dropped": []}
         alive = OrderedDict(to_train)
+        run = self._remote_async if self.args.async_settings() is not None else self._remote_rounds
         try:
-            theta = await self._remote_rounds(alive, to_train, theta, cfg, loop, pool, model, result)
+            theta = await run(alive, to_train, theta, cfg, loop, pool, model, result)
         finally:
             # whatever happened above, the devices' sockets are closed and they leave the registry (fc.py:573-580, 595-597)
             pool.shutdown(wait=False)
@@ -578,6 +581,141 @@ class Coordinator(BusClient):
             if not alive:
                 break
         return theta
+
+    async def _remote_async(self, alive, to_train, theta, cfg, loop, pool, model, result) -> torch.Tensor:
+        """Asynchronous buffered aggregation (``--async-buffer K``, :mod:`fl.asyncagg`): up to ``C`` fits in flight, each from
+        the global version current when it was sent; a freed device gets the current theta at once, every reply passes the
+        reply checks of its uplink codec and goes into the buffer (a failing device is dropped as in :meth:`_remote_rounds`),
+        and every ``K`` buffered replies make one server step (``-f`` of them).  fp32 replies are applied as deltas to their
+        base through the version ring (``ops.fedavg_apply_based``), codec replies are deltas already and keep their apply with
+        the staleness-scaled weights.  A ``--fed-eval-every`` step stops dispatching, drains the fits in flight into the buffer
+        and evaluates theta before it resumes.  After the last step nothing is dispatched and the fits still in flight are
+        awaited (up to ``fit_timeout``) and discarded."""
+        st = self.args.async_settings()
+        codec = self.args.uplink_codec()
+        result["uplink"], result["downlink"] = codec.kind, "fp32"
+        if any(b.is_floating_point() for b in model.buffers()):
+            raise ValueError(f"--async-buffer does not apply to {self.args.model}: averaging BatchNorm statistics across model versions "
+                             "is not defined")
+        eval_classes = fedeval.check_model(model) if self.args.fed_eval_every > 0 else None
+        th = theta.to(self.device).clone()
+        ring = asyncagg.ring_init(th, st) if not (codec.quantized or codec.sparse) else None
+        # what a fit request sends: a snapshot of theta at `version`.  A request is serialised later, in the executor thread, and
+        # the steps update th in place (th.cpu() is th itself on a CPU coordinator), so every version gets its own copy
+        current = th.detach().to("cpu", copy=True)
+        version, steps, dispatched = 0, 0, 0
+        buffer: List[asyncagg.Reply] = []
+        in_flight: Dict[Any, Any] = {}                             # task -> (device, base version)
+        idle = list(alive)
+        fitted: set = set()                                        # top-k: a device's first fit resets its residual
+        concurrency = st.concurrency or len(alive)
+        result["async_discarded"] = 0
+        traffic = lambda w: (getattr(w, "bytes_sent", 0), getattr(w, "bytes_received", 0))  # noqa: E731 - any handle type
+
+        async def fit(wid: str, worker, flat: torch.Tensor, rcfg: FitConfig, reset: bool, base: int):
+            try:
+                if codec.quantized:
+                    update, loss, n = await loop.run_in_executor(pool, lambda: worker.fit_quantized(
+                        flat, rcfg, codec, timeout=self.fit_timeout, version=base))
+                    return check_quantized_reply(update, codec, flat.numel()), loss, n
+                if codec.sparse:
+                    update, loss, n = await loop.run_in_executor(pool, lambda: worker.fit_topk(
+                        flat, rcfg, codec, ef_reset=reset, timeout=self.fit_timeout, version=base))
+                    return check_topk_reply(update, codec, flat.numel()), loss, n
+                got, loss, n = await loop.run_in_executor(pool, lambda: worker.fit(flat, rcfg, timeout=self.fit_timeout, version=base))
+                got = torch.as_tensor(got, dtype=torch.float32).reshape(-1)
+                if got.numel() != flat.numel():
+                    raise ValueError(f"model of {got.numel()} parameters returned, expected {flat.numel()}")
+                if not bool(torch.isfinite(got).all()):
+                    raise ValueError("model with non-finite parameters returned")
+                return got, loss, n
+            except Exception as e:  # noqa: BLE001 - a failing device leaves the training, the others go on
+                log.info("Worker %s failed its fit: %r", wid, e)
+                return None, None, 0
+
+        def dispatch() -> None:
+            nonlocal dispatched
+            while idle and len(in_flight) < concurrency:
+                wid = idle.pop(0)
+                rcfg = FitConfig(**{**cfg.to_dict(), "seed": cfg.seed + dispatched})
+                task = asyncio.ensure_future(fit(wid, alive[wid], current, rcfg, wid not in fitted, version))
+                in_flight[task] = (wid, version)
+                fitted.add(wid)
+                dispatched += 1
+
+        async def collect() -> List[asyncagg.Reply]:
+            """the checked replies of the fits that ended by the time the first of them did"""
+            done, _ = await asyncio.wait(list(in_flight), return_when=asyncio.FIRST_COMPLETED)
+            got = []
+            for task in done:
+                wid, base = in_flight.pop(task)
+                update, loss, n = task.result()
+                if update is None:
+                    result["dropped"].append(wid)
+                    alive.pop(wid, None)
+                    continue
+                self.metrics.worker_loss(wid, loss)
+                result["losses"][wid] = loss
+                got.append(asyncagg.Reply(wid, base, update, n, loss))
+                idle.append(wid)
+            return got
+
+        t0 = time.time()
+        sent0 = {wid: traffic(w) for wid, w in to_train.items()}
+        while steps < self.enabled_round and (in_flight or idle):
+            dispatch()
+            buffer += await collect()
+            while len(buffer) >= st.buffer and steps < self.enabled_round:
+                batch, buffer = buffer[:st.buffer], buffer[st.buffer:]
+                rec = self._async_step(th, ring, batch, version, st, codec, len(in_flight))
+                version += 1
+                current = th.detach().to("cpu", copy=True)
+                if self._fed_eval_round(steps):
+                    while in_flight:                                    # drain: the fits in flight count toward the next step
+                        buffer += await collect()
+                    rec["fed_eval"] = result["fed_eval"] = await self._remote_fed_eval(alive, current, eval_classes, loop, pool)
+                sent = {wid: traffic(w) for wid, w in to_train.items()}
+                rec["bytes_out"] = sum(sent[w][0] - sent0[w][0] for w in sent)
+                rec["bytes_in"] = sum(sent[w][1] - sent0[w][1] for w in sent)
+                result["bytes_out"] = result.get("bytes_out", 0) + rec["bytes_out"]
+                result["bytes_in"] = result.get("bytes_in", 0) + rec["bytes_in"]
+                sent0 = sent
+                self.metrics.end_round(steps, time.time() - t0, **rec)
+                self._maybe_checkpoint(model, current, steps, {"workers": list(to_train.keys()), "mode": "remote"})
+                steps += 1
+                t0 = time.time()
+        # after the last step: nothing new is dispatched; what is still in flight is awaited, then discarded with the buffer
+        left = len(in_flight)
+        if in_flight:
+            _, late = await asyncio.wait(list(in_flight), timeout=self.fit_timeout)
+            for task in late:
+                task.cancel()
+        result["async_discarded"] = left + len(buffer)
+        result["async_steps"] = steps
+        return current
+
+    def _async_step(self, th: torch.Tensor, ring: Optional[torch.Tensor], batch, version: int, st, codec: UplinkCodec,
+                    in_flight: int) -> Dict[str, Any]:
+        """One asynchronous server step on ``th`` at global ``version`` with the buffered replies ``batch``: returns the step's
+        record (``selected``, ``n_k`` and ``async``, plus ``agg_weights`` under a distance-based aggregator)."""
+        plan = asyncagg.plan_step(batch, version, st, self.args.weighted)
+        rec: Dict[str, Any] = {"selected": [r.device for r in plan.kept], "n_k": [r.n for r in plan.kept]}
+        if plan.kept:
+            w = torch.tensor(plan.weights, dtype=torch.float32, device=self.device)
+            if ring is None:
+                wire = [torch.stack(field).to(self.device) for field in zip(*[r.update for r in plan.kept])]
+                apply = ops.fedavg_apply_topk if codec.sparse else ops.fedavg_apply_quantized
+                agg_w = self._server_update(th, partial(apply, th, *wire, w, codec), len(plan.kept))
+            else:
+                models = torch.stack([r.update for r in plan.kept]).to(self.device)
+                agg_w = self._server_update(th, partial(ops.fedavg_apply_based, th, models, ring, [st.slot(r.base) for r in plan.kept], w,
+                                                        st.slot(version + 1)), len(plan.kept))
+            if agg_w is not None:
+                rec["agg_weights"] = agg_w
+        elif ring is not None:
+            ring[st.slot(version + 1)].copy_(th)                   # nothing applied: version + 1 is the same model
+        rec["async"] = {"version": version, "replies": plan.record, "stale_dropped": plan.stale_dropped, "in_flight": in_flight}
+        return rec
 
     async def _remote_fed_eval(self, alive, theta: torch.Tensor, classes: int, loop, pool) -> Dict[str, Any]:
         """Federated evaluation of ``theta`` (the true global model, fp32) on every live device's evaluation data.  Every reply

@@ -292,6 +292,8 @@ class WorkerServer:
                     reply["buffers"] = _to_bytes(torch.cat(bufs))
                 if replica is not None:
                     reply["replica_crc"] = replica_crc(replica)
+                if "version" in req:                      # asynchronous aggregation: the global version this fit started from
+                    reply["version"] = req["version"]
                 return reply
         if op == "evaluate":
             # federated evaluation (fl/fedeval.py): the model in "params" (fp32) scored on the rows hosted under "evaluation";
@@ -415,10 +417,13 @@ class RemoteWorkerClient:
         return bool(self._call({"op": "ping"}, timeout=5.0).get("ok"))
 
     def fit(self, flat: torch.Tensor, cfg: FitConfig, dataset_key: str = "training",
-            timeout: Optional[float] = None) -> Tuple[torch.Tensor, float, int]:
-        """Broadcast leg + remote local-SGD + gather leg (cf.py:209-211) in one RPC."""
-        resp = self._call({"op": "fit", "config": cfg.to_dict(), "params": _to_bytes(flat),
-                           "dataset_key": dataset_key}, timeout=timeout)
+            timeout: Optional[float] = None, version: Optional[int] = None) -> Tuple[torch.Tensor, float, int]:
+        """Broadcast leg + remote local-SGD + gather leg (cf.py:209-211) in one RPC.  ``version``: the global version of
+        ``flat`` under asynchronous aggregation (the device echoes it; None sends no version field)."""
+        req = {"op": "fit", "config": cfg.to_dict(), "params": _to_bytes(flat), "dataset_key": dataset_key}
+        if version is not None:
+            req["version"] = int(version)
+        resp = self._call(req, timeout=timeout)
         self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None     # BatchNorm statistics, if any
         return _from_bytes(resp["params"]), float(resp["loss"]), int(resp["n"])
 
@@ -433,12 +438,15 @@ class RemoteWorkerClient:
         return req
 
     def fit_quantized(self, flat: torch.Tensor, cfg: FitConfig, codec: UplinkCodec, dataset_key: str = "training",
-                      timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None) -> Tuple[Dict[str, Any], float, int]:
+                      timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None,
+                      version: Optional[int] = None) -> Tuple[Dict[str, Any], float, int]:
         """:meth:`fit` asking the device for its quantized delta (``codec``): returns the reply's ``{"uplink", "payload",
         "scales"}`` (and ``"replica_crc"`` with a ``downlink``) unchecked (it is untrusted input: the coordinator validates
-        it), the loss and the sample count."""
+        it), the loss and the sample count.  ``version`` as in :meth:`fit`."""
         req = self._fit_request(flat, cfg, dataset_key, downlink)
         req["uplink"] = codec.kind
+        if version is not None:
+            req["version"] = int(version)
         resp = self._call({**req, **(downlink or {})}, timeout=timeout)
         self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None
         update = {"uplink": resp.get("uplink"), "payload": resp.get("payload"), "scales": resp.get("scales")}
@@ -447,12 +455,16 @@ class RemoteWorkerClient:
         return update, float(resp["loss"]), int(resp["n"])
 
     def fit_topk(self, flat: torch.Tensor, cfg: FitConfig, codec: UplinkCodec, ef_reset: bool, dataset_key: str = "training",
-                 timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None) -> Tuple[Dict[str, Any], float, int]:
+                 timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None,
+                 version: Optional[int] = None) -> Tuple[Dict[str, Any], float, int]:
         """:meth:`fit` asking the device for the top-k entries of its delta plus residual (``codec``), after zeroing that
         residual if ``ef_reset``: returns the reply's ``{"uplink", "topk", "indices", "values"}`` (and ``"replica_crc"`` with a
-        ``downlink``) unchecked (it is untrusted input: the coordinator validates it), the loss and the sample count."""
+        ``downlink``) unchecked (it is untrusted input: the coordinator validates it), the loss and the sample count.
+        ``version`` as in :meth:`fit`."""
         req = self._fit_request(flat, cfg, dataset_key, downlink)
         req.update({"uplink": codec.kind, "topk": codec.k, "ef_reset": bool(ef_reset)})
+        if version is not None:
+            req["version"] = int(version)
         resp = self._call({**req, **(downlink or {})}, timeout=timeout)
         self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None
         update = {k: resp.get(k) for k in ("uplink", "topk", "indices", "values")}

@@ -102,6 +102,34 @@ def fedavg_apply(theta: torch.Tensor, models: torch.Tensor, weights: torch.Tenso
                         lambda: (models, weights, theta))
 
 
+def fedavg_apply_based(theta: torch.Tensor, models: torch.Tensor, ring: torch.Tensor, base_slot, weights: torch.Tensor, write_slot: int,
+                       server_lr: float = 1.0, opt=None, aggregator=None, agg_weights_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """:func:`fedavg_apply` on models trained from older global versions (asynchronous buffered aggregation, ``fl/asyncagg.py``):
+    ``ring`` (fp32 ``[slots, P]``, contiguous; ``S + 2`` slots under ``--max-staleness S``) holds the recent versions of
+    theta and row ``k`` of ``models [K, >= P]`` counts as its delta ``models[k] - ring[base_slot[k]]``.  ``a = theta + sum_k w_k d_k`` (``fedavg_based_kernel``, fmaf in row
+    order), or ``theta +`` the robust aggregate of the deltas (coordinate-wise: unweighted; distance-based: from 0 with
+    ``weights`` as alpha), then the server step of ``server_lr`` / ``opt`` as in :func:`fedavg_apply`; the new theta is also
+    written to ``ring[write_slot]`` in the same pass.  ``write_slot`` must not be any row's base.  CPU tensors:
+    ``reference.fedavg_apply_based``."""
+    slots = [int(b) for b in (base_slot.tolist() if isinstance(base_slot, torch.Tensor) else base_slot)]
+    if ring.dim() != 2 or ring.shape[1] != theta.numel() or not ring.is_contiguous() or ring.dtype != torch.float32:
+        raise ValueError("ring must be a contiguous float32 [slots, P] tensor (it is written in place)")
+    if len(slots) != models.shape[0]:
+        raise ValueError(f"one base slot per row: {len(slots)} for {models.shape[0]} rows")
+    if not 0 <= int(write_slot) < ring.shape[0] or any(not 0 <= b < ring.shape[0] or b == int(write_slot) for b in slots):
+        raise ValueError(f"base slots {slots} and write slot {write_slot} must lie in [0, {ring.shape[0]}) and differ")
+
+    def launch(*tail):
+        dev = theta.device
+        _ext.require().fedavg_apply_based(theta, models.to(dev, torch.float32).contiguous(), ring, torch.tensor(slots, dtype=torch.int32),
+                                          weights.to(dev, torch.float32).contiguous(), int(write_slot), *tail)
+
+    return _fused_apply(
+        "fp32_based", theta, models.shape[0], server_lr, opt, aggregator, agg_weights_out, launch,
+        lambda: reference.fedavg_apply_based(theta, models, ring, slots, weights, write_slot, server_lr, opt=opt, aggregator=aggregator),
+        lambda: (reference.based_deltas(models, ring, slots), weights, torch.zeros(theta.numel())))
+
+
 def _keys_i32(keys, device) -> torch.Tensor:
     """uint32 keys as the int32 tensor (same bits) the kernels take"""
     k = torch.tensor([int(x) & 0xFFFFFFFF for x in keys], dtype=torch.int64)

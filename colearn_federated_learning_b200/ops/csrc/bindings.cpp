@@ -186,6 +186,33 @@ void fedavg_apply(torch::Tensor theta, torch::Tensor slots, torch::Tensor weight
   r.models = slots.data_ptr<float>();
   fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, "fedavg_apply");
 }
+// Asynchronous buffered aggregation: theta += step towards theta + aggregate of the K deltas models[k] - ring[base_slot[k]]
+// (models fp32 [K, >= P], ring fp32 [slots, P] contiguous, S + 2 slots under --max-staleness S; base_slot int32 [K] on the CPU:
+// the launcher checks it before it launches), the new theta also stored to ring[write_slot]; the server optimizer / aggregator
+// arguments as in fedavg_apply_rows.  The slots reach the device through pinned memory without a host synchronisation.
+void fedavg_apply_based(torch::Tensor theta, torch::Tensor models, torch::Tensor ring, torch::Tensor base_slot, torch::Tensor weights,
+                        int64_t write_slot, double server_lr, int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<torch::Tensor> m,
+                        c10::optional<torch::Tensor> v, int64_t agg_kind, double trim, int64_t iters, double eps, double clip,
+                        c10::optional<torch::Tensor> agg_weights_out) {
+  CHECK_CUDA_F32(theta); CHECK_CUDA_F32(models); CHECK_CUDA_F32(ring); CHECK_CUDA_F32(weights);
+  const int64_t n = theta.numel();
+  TORCH_CHECK(models.dim() == 2 && models.stride(1) == 1 && models.size(1) >= n && weights.numel() == models.size(0) &&
+              models.device() == theta.device() && weights.device() == theta.device(), "models [K, >= P], weights [K] on theta's device");
+  TORCH_CHECK(ring.dim() == 2 && ring.size(1) == n && ring.is_contiguous() && ring.device() == theta.device(),
+              "ring: contiguous [slots, P] on theta's device");
+  TORCH_CHECK(!base_slot.is_cuda() && base_slot.scalar_type() == at::kInt && base_slot.is_contiguous() && base_slot.numel() == models.size(0),
+              "base_slot: CPU int32 [K]");
+  c10::cuda::CUDAGuard guard(theta.device());
+  const torch::Tensor base_dev = base_slot.pin_memory().to(theta.device(), /*non_blocking=*/true);
+  ClientRows r = client_rows(ROWS_F32_BASED, models.size(0), models.stride(0), weights.data_ptr<float>());
+  r.models = models.data_ptr<float>();
+  r.ring = ring.data_ptr<float>();
+  r.ring_slots = (int)ring.size(0);
+  r.write_slot = (int)write_slot;
+  r.base_slot = base_dev.data_ptr<int>();
+  r.base_slot_host = base_slot.data_ptr<int>();
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, "fedavg_apply_based");
+}
 // ---- uplink codec (uplink_quant.cuh) ------------------------------------------------------------------------------------------
 // (payload uint8 [K, row_bytes], scales fp32 [K, ceil(P / 256)]) of models [K, P] - theta [P] with keys int32 [K] (uint32 bits);
 // row_bytes = the packed codes (P bytes for bits 8, ceil(P / 2) for bits 4) rounded up to 16 bytes
@@ -885,6 +912,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
         py::arg("trim") = 0.0, py::arg("iters") = 3,
         py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none());
+  m.def("fedavg_apply_based", &fedavg_apply_based, py::arg("theta"), py::arg("models"), py::arg("ring"), py::arg("base_slot"),
+        py::arg("weights"), py::arg("write_slot"), py::arg("server_lr"), py::arg("opt_kind") = 0,
+        py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
+        py::arg("trim") = 0.0, py::arg("iters") = 3, py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none());
   m.def("topk_delta", &topk_delta);
   m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("weights"),
         py::arg("topk"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},

@@ -246,7 +246,12 @@ cudaError_t launch_sgd_step_bf16grad(float* param, const void* grad_bf16, float 
 //   ROWS_SECAGG  secure aggregation (secagg.cuh), n < 2^36: masked [k][stride] uint32 words, keys [streams][8] uint32 (16-byte
 //                aligned), signs [streams] (< 0 subtracts the stream); z = sum of the k rows + the streams, a = theta +
 //                sa_decode(z) / n_mean with 2^frac_bits (0 <= frac_bits <= 64)
-enum RowFormat : int { ROWS_F32 = 0, ROWS_INT8 = 1, ROWS_INT4 = 2, ROWS_TOPK = 3, ROWS_SECAGG = 4 };
+//   ROWS_F32_BASED  fp32 models [k][stride] trained from older global versions (asynchronous buffered aggregation): ring
+//                [ring_slots][n] fp32 (16-byte aligned) holds the last ring_slots versions, row r is the delta models[r] -
+//                ring[base_slot[r]]; a = theta + aggregate of the deltas (the mean: fmaf in slot order from +0).  The step also
+//                writes the new theta into ring[write_slot] in the same pass, so no base_slot may equal write_slot
+//                (base_slot: device [k] for the kernels, base_slot_host the same values on the host for the launcher's check)
+enum RowFormat : int { ROWS_F32 = 0, ROWS_INT8 = 1, ROWS_INT4 = 2, ROWS_TOPK = 3, ROWS_SECAGG = 4, ROWS_F32_BASED = 5 };
 struct ClientRows {
   int format;                // RowFormat
   int k;                     // rows, >= 1
@@ -262,10 +267,15 @@ struct ClientRows {
   const uint32_t* keys;
   const int* signs;
   int streams, frac_bits, n_mean;
+  float* ring;               // ROWS_F32_BASED (models as for ROWS_F32)
+  int ring_slots, write_slot;
+  const int* base_slot;
+  const int* base_slot_host;
 };
 // The aggregator: kind AGG_MEAN (the weighted mean), AGG_MEDIAN / AGG_TRIMMED_MEAN (robust_agg.cuh: coordinate-wise,
 // unweighted, any k) or DAGG_GEOMED / DAGG_NORM_CLIP (distance_agg.cuh: the rows weighted by their L2 distance from a centre,
-// start point theta for fp32 models and 0 for deltas).  Top-k and secure-aggregation rows admit only the mean.
+// start point theta for fp32 models and 0 for deltas, ROWS_F32_BASED included).  Top-k and secure-aggregation rows admit only
+// the mean.
 struct AggregatorArgs {
   int kind;
   float trim;      // trimmed mean: fraction trimmed at each end, in [0, 0.5)

@@ -176,6 +176,14 @@ __global__ void fedavg_opt_kernel(float* __restrict__ theta, const float* __rest
   }
 }
 
+// Whether a row loader also names a second destination of the new theta (the version ring of ROWS_F32_BASED): the store of
+// the step writes it in the same pass.  Off for every other loader.
+template <class Rows>
+struct RingWrite {
+  static constexpr bool kOn = false;
+  __device__ __forceinline__ static float* out(const Rows&) { return nullptr; }
+};
+
 // Slot loaders of the robust FedAvg body.  stream(c, j) / cached(c, j): value j of slot c, read once (register path) or
 // reread through L1 / L2 (general path); average(a, t): the a the server step moves towards, from the aggregate of the slots.
 // fp32 slots hold the client models themselves.
@@ -232,7 +240,9 @@ __device__ __forceinline__ void fedavg_robust_body(float* __restrict__ theta, co
     }
     const float t = theta[j];
     a = slots.average(a, t);
-    theta[j] = (opt.kind == SOPT_SGD) ? fmaf(opt.lr, a - t, t) : server_opt_step(opt, j, t, a);
+    const float r = (opt.kind == SOPT_SGD) ? fmaf(opt.lr, a - t, t) : server_opt_step(opt, j, t, a);
+    theta[j] = r;
+    if constexpr (RingWrite<Slots>::kOn) RingWrite<Slots>::out(slots)[j] = r;
   }
 }
 
@@ -358,10 +368,11 @@ struct StagedWeights {
 };
 
 // theta[e0 .. e0 + 7] (none past n) moved towards a = theta + acc: theta += opt.lr (a - theta) (OPT false) or the server
-// optimizer step (OPT true); 16-byte accesses of theta and the moments per 4 elements inside n when vec
-template <bool OPT>
+// optimizer step (OPT true); 16-byte accesses of theta and the moments per 4 elements inside n when vec.  RING: the new values
+// are also stored to ring (16-byte stores when vec)
+template <bool OPT, bool RING = false>
 __device__ __forceinline__ void apply8(float* __restrict__ theta, int64_t e0, int64_t n, bool vec, const float (&acc)[8],
-                                       const ServerOptArgs& opt) {
+                                       const ServerOptArgs& opt, float* __restrict__ ring = nullptr) {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int64_t e = e0 + 4 * h;
@@ -376,12 +387,15 @@ __device__ __forceinline__ void apply8(float* __restrict__ theta, int64_t e0, in
         t.z = fmaf(opt.lr, a.z - t.z, t.z); t.w = fmaf(opt.lr, a.w - t.w, t.w);
       }
       *t4 = t;
+      if constexpr (RING) *reinterpret_cast<float4*>(ring + e) = t;
     } else {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         if (e + i < n) {
           const float t = theta[e + i], a = t + acc[4 * h + i];
-          theta[e + i] = OPT ? server_opt_step(opt, e + i, t, a) : fmaf(opt.lr, a - t, t);
+          const float r = OPT ? server_opt_step(opt, e + i, t, a) : fmaf(opt.lr, a - t, t);
+          theta[e + i] = r;
+          if constexpr (RING) ring[e + i] = r;
         }
       }
     }
@@ -492,6 +506,36 @@ struct QRows {
     for (int i = 0; i < 8; ++i) x[i] = e0 + i < n ? uq_decode(q[i], step) : 0.f;   // codes past n are padding
   }
 };
+// ROWS_F32_BASED: fp32 models trained from older global versions, each read as its delta to its own base, the ring slot
+// base[k] (ring [slots][n]).  The loader of the robust body (stream / cached / average), of the distance passes (load8) and of
+// fedavg_based_kernel; ring_out = ring + write_slot n receives the new theta.  vec: models, ring and n allow 16-byte loads.
+struct BasedRows {
+  static constexpr bool kDelta = true;
+  const float* p;
+  int64_t stride;
+  const float* ring;
+  const int* base;
+  float* ring_out;
+  int64_t n;
+  bool vec;
+  __device__ __forceinline__ const float* base_row(int k) const { return ring + (int64_t)__ldg(base + k) * n; }
+  template <LdHint HINT>
+  __device__ __forceinline__ void load8(int k, int64_t e0, float (&x)[8]) const {
+    float b[8];
+    lane_load8<HINT>(p + k * stride, e0, n, vec, x);
+    lane_load8<kLdReadOnly>(base_row(k), e0, n, vec, b);   // a base is shared by every row trained from that version
+#pragma unroll
+    for (int i = 0; i < 8; ++i) x[i] = x[i] - b[i];
+  }
+  __device__ __forceinline__ float stream(int c, int64_t j) const { return __ldcs(p + c * stride + j) - __ldg(base_row(c) + j); }
+  __device__ __forceinline__ float cached(int c, int64_t j) const { return __ldg(p + c * stride + j) - __ldg(base_row(c) + j); }
+  __device__ __forceinline__ float average(float a, float t) const { return t + a; }
+};
+template <>
+struct RingWrite<BasedRows> {
+  static constexpr bool kOn = true;
+  __device__ __forceinline__ static float* out(const BasedRows& r) { return r.ring_out; }
+};
 
 __device__ __forceinline__ double warp_tree_f64(double v) {
 #pragma unroll
@@ -532,8 +576,7 @@ __device__ __forceinline__ void da_start8(const float* __restrict__ theta, int64
 
 // Distance pass of the first step: the chunk sums of (x_k - c^0)^2 for every row
 template <class Rows>
-__global__ void __launch_bounds__(kDaThreads)
-dagg_dist_kernel(Rows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
+__device__ __forceinline__ void dagg_dist_body(Rows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
   __shared__ double red[kDaThreads / 32][32];
   const DaRowSums sums{red};
   const int64_t nchunks = da_chunks(n);
@@ -553,13 +596,17 @@ dagg_dist_kernel(Rows rows, const float* __restrict__ theta, int k, DistAggScrat
     }
   }
 }
+template <class Rows>
+__global__ void __launch_bounds__(kDaThreads)
+dagg_dist_kernel(Rows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
+  dagg_dist_body(rows, theta, k, sc, n);
+}
 
 // A geomed step l < L fused with the next distance pass: the lane forms c^l for its 8 elements from the current weights (c^0
 // when no row is left), then the chunk sums of (x_k - c^l)^2, in one read of the rows.  KMAX > 0: k <= KMAX, the rows' 8 values
 // stay in registers between the two loops; KMAX = 0: any k, the second loop rereads them through L1 / L2.
 template <int KMAX, class Rows>
-__global__ void __launch_bounds__(kDaThreads, 1)
-dagg_center_kernel(Rows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
+__device__ __forceinline__ void dagg_center_body(Rows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
   __shared__ double red[kDaThreads / 32][32];
   __shared__ float sw[StagedWeights::kSw];
   const StagedWeights staged(sw, sc.w, k);
@@ -619,6 +666,11 @@ dagg_center_kernel(Rows rows, const float* __restrict__ theta, int k, DistAggScr
     }
   }
 }
+template <int KMAX, class Rows>
+__global__ void __launch_bounds__(kDaThreads, 1)
+dagg_center_kernel(Rows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
+  dagg_center_body<KMAX>(rows, theta, k, sc, n);
+}
 
 // Finalisation of one step: CTA r adds row r's chunk sums (distance_agg.cuh order) into d_r; the last CTA to take a ticket
 // forms the raw weights in parallel, their sum in row order (thread 0) and the weights, and leaves the ticket at 0.
@@ -670,10 +722,11 @@ dagg_finalize_kernel(DistAggScratch sc, const float* __restrict__ alpha, int k, 
 }
 
 // theta[e0 .. e0 + 7] (t, none past n) moved towards a: theta += opt.lr (a - theta) (OPT false) or the server optimizer step
-// (OPT true); 16-byte accesses of theta and the moments per 4 elements inside n when vec
-template <bool OPT>
+// (OPT true); 16-byte accesses of theta and the moments per 4 elements inside n when vec.  RING: the new values are also stored
+// to ring
+template <bool OPT, bool RING = false>
 __device__ __forceinline__ void step_to8(float* __restrict__ theta, int64_t e0, int64_t n, bool vec, const float (&t)[8],
-                                         const float (&a)[8], const ServerOptArgs& opt) {
+                                         const float (&a)[8], const ServerOptArgs& opt, float* __restrict__ ring = nullptr) {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int64_t e = e0 + 4 * h;
@@ -687,12 +740,15 @@ __device__ __forceinline__ void step_to8(float* __restrict__ theta, int64_t e0, 
         tt.z = fmaf(opt.lr, aa.z - tt.z, tt.z); tt.w = fmaf(opt.lr, aa.w - tt.w, tt.w);
       }
       *reinterpret_cast<float4*>(theta + e) = tt;
+      if constexpr (RING) *reinterpret_cast<float4*>(ring + e) = tt;
     } else {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         if (e + i < n) {
           const float tv = t[4 * h + i], av = a[4 * h + i];
-          theta[e + i] = OPT ? server_opt_step(opt, e + i, tv, av) : fmaf(opt.lr, av - tv, tv);
+          const float r = OPT ? server_opt_step(opt, e + i, tv, av) : fmaf(opt.lr, av - tv, tv);
+          theta[e + i] = r;
+          if constexpr (RING) ring[e + i] = r;
         }
       }
     }
@@ -702,8 +758,7 @@ __device__ __forceinline__ void step_to8(float* __restrict__ theta, int64_t e0, 
 // Last pass: the aggregate from the final weights (geomed: c^L, or c^0 when no row is left; norm_clip: c^0 + the clipped sum),
 // theta + it for deltas, and the server step on theta with the moments in place.
 template <class Rows, bool CLIP, bool OPT>
-__global__ void __launch_bounds__(kDaThreads)
-dagg_apply_kernel(Rows rows, float* __restrict__ theta, int k, DistAggScratch sc, ServerOptArgs opt, int64_t n) {
+__device__ __forceinline__ void dagg_apply_body(Rows rows, float* __restrict__ theta, int k, DistAggScratch sc, ServerOptArgs opt, int64_t n) {
   __shared__ float sw[StagedWeights::kSw];
   const StagedWeights staged(sw, sc.w, k);
   const bool live = *sc.live > 0;
@@ -732,9 +787,76 @@ dagg_apply_kernel(Rows rows, float* __restrict__ theta, int k, DistAggScratch sc
       a[i] = CLIP ? c0[i] + acc[i] : (live ? acc[i] : c0[i]);
       if (Rows::kDelta) a[i] = t[i] + a[i];
     }
-    step_to8<OPT>(theta, e0, n, vec, t, a, opt);
+    step_to8<OPT, RingWrite<Rows>::kOn>(theta, e0, n, vec, t, a, opt, RingWrite<Rows>::out(rows));
   }
 }
+template <class Rows, bool CLIP, bool OPT>
+__global__ void __launch_bounds__(kDaThreads)
+dagg_apply_kernel(Rows rows, float* __restrict__ theta, int k, DistAggScratch sc, ServerOptArgs opt, int64_t n) {
+  dagg_apply_body<Rows, CLIP, OPT>(rows, theta, k, sc, opt, n);
+}
+
+// ---- asynchronous buffered aggregation (ROWS_F32_BASED) -------------------------------------------------------------------------
+// The fp32 twin of fedavg_q_kernel on rows of mixed base versions: per element acc = fmaf(w_k, x_k - ring[base_k], acc) in slot
+// order from +0, a = theta + acc, the step of apply8, and the new theta stored to theta and ring_out in the same pass.  One warp
+// per 256 elements, lane l holding 8 of them.
+template <bool OPT>
+__global__ void __launch_bounds__(256)
+fedavg_based_kernel(float* __restrict__ theta, BasedRows rows, const float* __restrict__ weights, int k, ServerOptArgs opt, int64_t n) {
+  __shared__ float sw[StagedWeights::kSw];
+  const StagedWeights staged(sw, weights, k);
+  const int lane = threadIdx.x & 31;
+  const int64_t nblk = uq_nblk(n);
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const bool vec = rows.vec && (((uintptr_t)theta | (uintptr_t)opt.m | (uintptr_t)opt.v) & 15) == 0;
+  for (int64_t blk = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < nblk; blk += warps) {
+    const int64_t e0 = blk * kUqBlock + lane * 8;
+    if (e0 >= n) continue;
+    float acc[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+#pragma unroll 2
+    for (int c = 0; c < k; ++c) {
+      const float w = staged.wt(c);
+      float d[8];
+      rows.load8<kLdStream>(c, e0, d);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] = fmaf(w, d[i], acc[i]);
+    }
+    apply8<OPT, true>(theta, e0, n, vec, acc, opt, rows.ring_out);
+  }
+}
+
+// robust aggregate of the deltas to their bases: the body of fedavg_robust_kernel with the based loader (and its ring store)
+template <int KMAX>
+__global__ void __launch_bounds__(256)
+fedavg_based_robust_kernel(float* __restrict__ theta, BasedRows rows, int k, AggArgs agg, ServerOptArgs opt, int64_t n) {
+  fedavg_robust_body<KMAX>(theta, rows, k, agg, opt, n);
+}
+
+// the distance passes on based rows: the bodies of dagg_dist_kernel / dagg_center_kernel / dagg_apply_kernel under their own
+// kernel names
+__global__ void __launch_bounds__(kDaThreads)
+dagg_based_dist_kernel(BasedRows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
+  dagg_dist_body(rows, theta, k, sc, n);
+}
+template <int KMAX>
+__global__ void __launch_bounds__(kDaThreads, 1)
+dagg_based_center_kernel(BasedRows rows, const float* __restrict__ theta, int k, DistAggScratch sc, int64_t n) {
+  dagg_center_body<KMAX>(rows, theta, k, sc, n);
+}
+template <bool CLIP, bool OPT>
+__global__ void __launch_bounds__(kDaThreads)
+dagg_based_apply_kernel(BasedRows rows, float* __restrict__ theta, int k, DistAggScratch sc, ServerOptArgs opt, int64_t n) {
+  dagg_apply_body<BasedRows, CLIP, OPT>(rows, theta, k, sc, opt, n);
+}
+// the kernel of each distance pass for a row loader
+template <class Rows> inline auto dagg_dist_for(const Rows&) { return dagg_dist_kernel<Rows>; }
+inline auto dagg_dist_for(const BasedRows&) { return dagg_based_dist_kernel; }
+template <int KMAX, class Rows> inline auto dagg_center_for(const Rows&) { return dagg_center_kernel<KMAX, Rows>; }
+template <int KMAX> inline auto dagg_center_for(const BasedRows&) { return dagg_based_center_kernel<KMAX>; }
+template <bool CLIP, bool OPT, class Rows> inline auto dagg_apply_for(const Rows&) { return dagg_apply_kernel<Rows, CLIP, OPT>; }
+template <bool CLIP, bool OPT> inline auto dagg_apply_for(const BasedRows&) { return dagg_based_apply_kernel<CLIP, OPT>; }
 
 // ---- top-k uplink with error feedback (uplink_topk.cuh) -----------------------------------------------------------------------
 // exclusive prefix over the lower lanes of x in [0, 15], one ballot per bit
@@ -1660,7 +1782,7 @@ inline void with_kmax(int k, F&& f) {
 template <class Rows, bool CLIP, bool OPT>
 inline void launch_dagg_apply_t(Rows rows, float* theta, int k, const DistAggScratch& sc, const ServerOptArgs& opt, int64_t n, int grid,
                                 cudaStream_t s) {
-  auto kernel = dagg_apply_kernel<Rows, CLIP, OPT>;
+  auto kernel = dagg_apply_for<CLIP, OPT>(rows);
   COLEARN_LAUNCH(kernel, grid, kDaThreads, 0, s, rows, theta, k, sc, opt, n);
 }
 template <class Rows>
@@ -1672,14 +1794,14 @@ inline cudaError_t launch_dagg_t(const Rows& rows, float* theta, const float* al
   cudaError_t e = cudaMemsetAsync(sc.ticket, 0, sizeof(unsigned), s);
   if (e != cudaSuccess) return e;
   {
-    auto kernel = dagg_dist_kernel<Rows>;
+    auto kernel = dagg_dist_for(rows);
     COLEARN_LAUNCH(kernel, grid, kDaThreads, 0, s, rows, theta, k, sc, n);
   }
   COLEARN_LAUNCH(dagg_finalize_kernel, k, kDaThreads, 0, s, sc, alpha, k, g, w_out, nchunks);
   const int steps = g.kind == DAGG_GEOMED ? g.iters - 1 : 0;
   for (int l = 0; l < steps; ++l) {
     with_kmax<16>(k, [&](auto kmax) {
-      auto kernel = dagg_center_kernel<decltype(kmax)::value, Rows>;
+      auto kernel = dagg_center_for<decltype(kmax)::value>(rows);
       COLEARN_LAUNCH(kernel, grid, kDaThreads, 0, s, rows, theta, k, sc, n);
     });
     COLEARN_LAUNCH(dagg_finalize_kernel, k, kDaThreads, 0, s, sc, alpha, k, g, w_out, nchunks);
@@ -1750,13 +1872,43 @@ inline bool rows_ok(const ClientRows& r, int64_t n) {
     case ROWS_SECAGG:
       return n >= 1 && n < kSaMaxElems && r.stride >= n && r.streams >= 0 && r.n_mean >= 1 && r.frac_bits >= 0 && r.frac_bits <= 64 &&
              (reinterpret_cast<uintptr_t>(r.keys) & 15) == 0;
+    case ROWS_F32_BASED: {
+      // the ring slot the step writes must not be a base of any row: the pass reads the bases while it stores the new theta
+      if (r.stride < n || r.ring == nullptr || (reinterpret_cast<uintptr_t>(r.ring) & 15) != 0 || r.ring_slots < 2 ||
+          r.write_slot < 0 || r.write_slot >= r.ring_slots || r.base_slot == nullptr || r.base_slot_host == nullptr)
+        return false;
+      for (int i = 0; i < r.k; ++i) {
+        const int b = r.base_slot_host[i];
+        if (b < 0 || b >= r.ring_slots || b == r.write_slot) return false;
+      }
+      return true;
+    }
   }
   return false;
 }
 // Which aggregators a row format admits.  Top-k and secure-aggregation rows take only the mean: a coordinate-wise median of
 // k/256-sparse deltas is 0 wherever fewer than half the rows kept the coordinate, their distances measure which entries the
 // codec kept, and the masks leave the coordinator nothing but the sum.
-inline bool agg_admissible(int format, int kind) { return kind == AGG_MEAN || format == ROWS_F32 || format == ROWS_INT8 || format == ROWS_INT4; }
+inline bool agg_admissible(int format, int kind) {
+  return kind == AGG_MEAN || format == ROWS_F32 || format == ROWS_INT8 || format == ROWS_INT4 || format == ROWS_F32_BASED;
+}
+inline cudaError_t route_based(float* theta, const ClientRows& r, const AggArgs& agg, const DistAggArgs& g, const ServerOptArgs& opt,
+                               int64_t n, const ApplyWork& w, cudaStream_t s) {
+  const bool vec = (((uintptr_t)r.models | (uintptr_t)r.ring) & 15) == 0 && (r.stride & 3) == 0 && (n & 3) == 0;
+  const BasedRows rows{r.models, r.stride, r.ring, r.base_slot, r.ring + (int64_t)r.write_slot * n, n, vec};
+  if (is_distance_agg(g.kind)) return launch_dagg_t(rows, theta, r.weights, r.k, g, opt, n, w.scratch, w.weights_out, w.grid, s);
+  if (agg.kind != AGG_MEAN) {
+    with_kmax<32>(r.k, [&](auto kmax) {
+      auto kernel = fedavg_based_robust_kernel<decltype(kmax)::value>;
+      COLEARN_LAUNCH(kernel, grid_for(n, 1), kThreads, 0, s, theta, rows, r.k, agg, opt, n);
+    });
+  } else if (opt.kind == SOPT_SGD) {
+    COLEARN_LAUNCH(fedavg_based_kernel<false>, grid_for_warps(uq_nblk(n)), kThreads, 0, s, theta, rows, r.weights, r.k, opt, n);
+  } else {
+    COLEARN_LAUNCH(fedavg_based_kernel<true>, grid_for_warps(uq_nblk(n)), kThreads, 0, s, theta, rows, r.weights, r.k, opt, n);
+  }
+  return cudaGetLastError();
+}
 
 template <int BITS>
 inline cudaError_t route_quantized(float* theta, const ClientRows& r, const AggArgs& agg, const DistAggArgs& g,
@@ -1832,6 +1984,7 @@ inline cudaError_t route_fedavg_apply(float* theta, const ClientRows& r, const A
                        r.weights, r.k, r.topk, opt, n);
       }
       return cudaGetLastError();
+    case ROWS_F32_BASED: return route_based(theta, r, agg, g, opt, n, w, s);
     default: return route_secagg(theta, r, opt, n, w, s);
   }
 }

@@ -160,6 +160,23 @@ void fedavg_apply(Tensor theta, Tensor slots, Tensor w, double server_lr, int64_
   r.models = slots.data_ptr<float>();
   fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, grid);
 }
+// asynchronous buffered aggregation: same shapes as bindings.cpp::fedavg_apply_based (base_slot is read by the launcher and the
+// kernels alike)
+void fedavg_apply_based(Tensor theta, Tensor models, Tensor ring, Tensor base_slot, Tensor w, int64_t write_slot, double server_lr,
+                        int64_t opt_kind, std::vector<double> opt_hyper, c10::optional<Tensor> m, c10::optional<Tensor> v, int64_t agg_kind,
+                        double trim, int64_t iters, double eps, double clip, c10::optional<Tensor> agg_weights_out, int64_t grid) {
+  TORCH_CHECK(!models.is_cuda() && models.scalar_type() == at::kFloat && models.dim() == 2 && models.stride(1) == 1 &&
+              models.size(1) >= theta.numel() && w.numel() == models.size(0), "models [K, >= P] (unit inner stride), weights [K]");
+  TORCH_CHECK(ring.dim() == 2 && ring.size(1) == theta.numel() && ring.is_contiguous(), "ring: contiguous [slots, P]");
+  TORCH_CHECK(base_slot.scalar_type() == at::kInt && base_slot.is_contiguous() && base_slot.numel() == models.size(0), "base_slot int32 [K]");
+  colearn::ClientRows r = client_rows(colearn::ROWS_F32_BASED, models.size(0), models.stride(0), fptr(w, "w"));
+  r.models = models.data_ptr<float>();
+  r.ring = fmut(ring, "ring");
+  r.ring_slots = (int)ring.size(0);
+  r.write_slot = (int)write_slot;
+  r.base_slot = r.base_slot_host = base_slot.data_ptr<int>();
+  fedavg_apply_rows(theta, r, server_lr, opt_kind, opt_hyper, m, v, agg_kind, trim, iters, eps, clip, agg_weights_out, grid);
+}
 // uplink codec (uplink_quant.cuh): same shapes and row padding as bindings.cpp::quantize_delta / fedavg_apply_quantized
 std::tuple<Tensor, Tensor> quantize_delta(Tensor models, Tensor theta, Tensor keys, int64_t bits) {
   TORCH_CHECK(models.dim() == 2 && models.size(1) == theta.numel(), "models [K, P], theta [P]");
@@ -605,6 +622,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fedavg_apply", &fedavg_apply, py::arg("theta"), py::arg("slots"), py::arg("w"), py::arg("server_lr"), py::arg("opt_kind") = 0,
         py::arg("opt_hyper") = std::vector<double>{}, py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0,
         py::arg("trim") = 0.0, py::arg("iters") = 3,
+        py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none(), py::arg("grid") = 0);
+  m.def("fedavg_apply_based", &fedavg_apply_based, py::arg("theta"), py::arg("models"), py::arg("ring"), py::arg("base_slot"), py::arg("w"),
+        py::arg("write_slot"), py::arg("server_lr"), py::arg("opt_kind") = 0, py::arg("opt_hyper") = std::vector<double>{},
+        py::arg("m") = py::none(), py::arg("v") = py::none(), py::arg("agg_kind") = 0, py::arg("trim") = 0.0, py::arg("iters") = 3,
         py::arg("eps") = 1e-6, py::arg("clip") = 0.0, py::arg("agg_weights_out") = py::none(), py::arg("grid") = 0);
   m.def("topk_delta", &topk_delta);
   m.def("fedavg_apply_topk", &fedavg_apply_topk, py::arg("theta"), py::arg("indices"), py::arg("values"), py::arg("w"), py::arg("topk"),

@@ -168,6 +168,16 @@ int main() {
         CK(launch_fedavg_apply(dtheta.data(), fr, clip, sgd, dn, dwork, nullptr));
         CK(launch_fedavg_apply(dtheta.data(), qr, geo, sgd, qn, dwork, nullptr));
       }
+      // asynchronous buffered aggregation: fp32 rows read as deltas to ring slots, the new theta stored to the write slot by the
+      // mean (weights in shared memory), the robust body and the distance passes
+      alignas(16) static float ring[3 * 2100];
+      std::vector<int> bases = {0, 2, 0, 2, 0};
+      ClientRows br{};
+      br.format = ROWS_F32_BASED; br.k = 5; br.stride = dn; br.weights = dalpha.data(); br.models = drows.data();
+      br.ring = ring; br.ring_slots = 3; br.write_slot = 1; br.base_slot = br.base_slot_host = bases.data();
+      CK(launch_fedavg_apply(dtheta.data(), br, mean, sgd, dn, nowork, nullptr));
+      CK(launch_fedavg_apply(dtheta.data(), br, median, sgd, dn, nowork, nullptr));
+      CK(launch_fedavg_apply(dtheta.data(), br, geo, sgd, dn, dwork, nullptr));
     }
   }
   printf("elementwise kernels ok\n");

@@ -685,7 +685,8 @@ def secagg_decode(z: np.ndarray, frac_bits: int, n: int) -> np.ndarray:
 
 def _fmaf(a, b, c) -> np.ndarray:
     """float32 fused multiply-add: the float32 product is exact in float64, then one float64 add and the float32 rounding"""
-    return (np.float64(a) * np.float64(b) + np.float64(c)).astype(np.float32)
+    f = lambda x: np.asarray(x, dtype=np.float64)  # noqa: E731 - (a one-element array stays an array)
+    return (f(a) * f(b) + f(c)).astype(np.float32)
 
 
 def _server_opt_np(t: np.ndarray, a: np.ndarray, opt, server_lr: float) -> np.ndarray:
@@ -728,6 +729,38 @@ def fedavg_apply_secagg(theta: torch.Tensor, masked: torch.Tensor, keys, signs, 
     with np.errstate(over="ignore", invalid="ignore"):
         out = _server_opt_np(t, t + mean, opt, server_lr)
     return theta.copy_(torch.from_numpy(out).view_as(theta))
+
+
+def based_deltas(models: torch.Tensor, ring: torch.Tensor, base_slot) -> torch.Tensor:
+    """float32 ``[K, P]``: ``models[k] - ring[base_slot[k]]``, every row's delta to the global version it was trained from"""
+    r = ring.detach().to("cpu", torch.float32)
+    x = models.detach().to("cpu", torch.float32)[:, :r.shape[1]]
+    return x - r[torch.as_tensor([int(b) for b in base_slot], dtype=torch.long)]
+
+
+def fedavg_apply_based(theta: torch.Tensor, models: torch.Tensor, ring: torch.Tensor, base_slot, weights: torch.Tensor, write_slot: int,
+                       server_lr: float = 1.0, opt=None, aggregator=None) -> torch.Tensor:
+    """Asynchronous buffered aggregation's apply (``ROWS_F32_BASED``): the deltas ``d_k = models[k] - ring[base_slot[k]]``,
+    ``a = theta + acc`` with ``acc = sum_k fmaf(w_k, d_k, acc)`` in row order from +0 (or the robust aggregate of the deltas:
+    coordinate-wise unweighted, distance-based from 0 with ``weights`` as alpha), then ``theta += server_lr (a - theta)`` or
+    the server optimizer step of ``opt``, in place; the new theta is also written to ``ring[write_slot]``.  The float32
+    roundings of ``fedavg_based_kernel`` / the robust body: bit for bit what they write (the distance-based kinds within
+    the tolerance of :func:`distance_aggregate`)."""
+    d = based_deltas(models, ring, base_slot)
+    t = theta.detach().to("cpu", torch.float32).reshape(-1).numpy()
+    if aggregator is None or not aggregator.robust:
+        w = weights.detach().to("cpu", torch.float32).numpy()
+        acc = np.zeros_like(t)
+        for k, dk in enumerate(d.numpy()):
+            acc = _fmaf(w[k], dk, acc)
+    elif aggregator.distance_based:
+        acc = distance_aggregate(d, weights, aggregator, torch.zeros(d.shape[1]))[0].numpy()
+    else:
+        acc = robust_aggregate(d, None, aggregator.kind, aggregator.trim).numpy()
+    with np.errstate(over="ignore", invalid="ignore"):
+        out = torch.from_numpy(_server_opt_np(t, t + acc, opt, server_lr))
+    ring[int(write_slot)].copy_(out.to(ring.device))
+    return theta.copy_(out.view_as(theta).to(theta.device))
 
 
 def linear_bias_relu(x, w, b, relu=True):

@@ -43,6 +43,8 @@ class PrometheusExporter:
         self.eval_accuracy = Gauge("colearn_eval_accuracy", "federated evaluation: accuracy of the global model", **mk)
         self.eval_auc = Gauge("colearn_eval_auc", "federated evaluation: ROC-AUC (macro one-vs-rest for multi-class models)", **mk)
         self.eval_f1 = Gauge("colearn_eval_f1", "federated evaluation: F1 (macro for multi-class models)", **mk)
+        self.async_staleness = Gauge("colearn_async_staleness", "asynchronous buffered aggregation: mean staleness (versions) of the "
+                                     "replies in the last server step", **mk)
         self.server, self.thread = start_http_server(port, addr=addr, registry=self.registry)
         self.port = self.server.server_port
 
@@ -92,6 +94,9 @@ class RoundLogger:
                         gauge.set(float(total[key]))
         rec = {"round": round_idx, "t_round_s": seconds, "ts": time.time(), **fields}
         if self.exporter is not None:
+            if fields.get("async") is not None and fields["async"]["replies"]:
+                taus = [r[2] for r in fields["async"]["replies"]]
+                self.exporter.async_staleness.set(sum(taus) / len(taus))
             self.exporter.rounds.inc()
             self.exporter.round_seconds.observe(float(seconds))
             self.exporter.bytes_out.inc(float(fields.get("bytes_out", 0) or 0))

@@ -121,6 +121,17 @@ def build_parser() -> argparse.ArgumentParser:
     parser.add_argument("--eval-fraction", type=float, default=d.eval_fraction,
                         help="--fed-eval-every in local and box mode: fraction of every device's shard held out for evaluation, in (0, 1) "
                              "(remote devices hold theirs out themselves: remote_worker.py -de / --eval-fraction)")
+    parser.add_argument("--async-buffer", type=int, default=d.async_buffer, metavar="K",
+                        help="remote mode: asynchronous buffered aggregation (FedBuff): devices train whenever they are free, from the "
+                             "current global version, and the server steps once K replies are buffered, each weighted by (1 + "
+                             "staleness)^-a; -f then counts server steps. 0 = synchronous rounds (not with --secure-agg, a compressed "
+                             "--downlink-codec, --box, -e, local mode or models with BatchNorm buffers)")
+    parser.add_argument("--async-concurrency", type=int, default=d.async_concurrency, metavar="C",
+                        help="--async-buffer: fits in flight at once (0 = one per selected device)")
+    parser.add_argument("--max-staleness", type=int, default=d.max_staleness, metavar="S",
+                        help="--async-buffer: a reply trained from a model more than S versions old is dropped")
+    parser.add_argument("--staleness-exponent", type=float, default=d.staleness_exponent, metavar="A",
+                        help="--async-buffer: a reply of staleness tau weighs (1 + tau)^-A (0.5 = FedBuff's 1/sqrt(1 + tau))")
     parser.add_argument("--embedded-broker", action="store_true", help="start the TCP bus broker inside this process")
     parser.add_argument("--tls-ca", default=None, help="CA bundle: verify the broker / the devices (and, with --tls-cert on the embedded broker, demand client certificates)")
     parser.add_argument("--tls-cert", default=None, help="certificate for the embedded broker / client certificate towards broker and devices")
@@ -185,6 +196,11 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.eval_threshold = getattr(ns, "eval_threshold", a.eval_threshold)
     a.eval_fraction = getattr(ns, "eval_fraction", a.eval_fraction)
     a.fed_eval_settings()             # rejects bins / threshold / fraction outside their ranges and --secure-agg with it
+    a.async_buffer = getattr(ns, "async_buffer", a.async_buffer)
+    a.async_concurrency = getattr(ns, "async_concurrency", a.async_concurrency)
+    a.max_staleness = getattr(ns, "max_staleness", a.max_staleness)
+    a.staleness_exponent = getattr(ns, "staleness_exponent", a.staleness_exponent)
+    a.async_settings()                # rejects negative settings and --async-buffer with --secure-agg or a compressed downlink
     return a
 
 
@@ -296,6 +312,14 @@ def parse_cli(argv=None) -> argparse.Namespace:
         if any(b.is_floating_point() for b in build_model(ns.model).buffers()):
             parser.error(f"--secure-agg does not apply to --model {ns.model}: its floating-point buffers (BatchNorm running "
                          "statistics) would travel in the clear")
+    if ns.async_buffer:
+        if ns.box or ns.encryption or not ns.remote:
+            parser.error("--async-buffer applies to remote mode (-r) only: local mode and --box train their workers in lockstep "
+                         "launches and -e exchanges secret shares")
+        from colearn_federated_learning_b200.models import build_model
+        if any(b.is_floating_point() for b in build_model(ns.model).buffers()):
+            parser.error(f"--async-buffer does not apply to --model {ns.model}: averaging its BatchNorm statistics across model "
+                         "versions is not defined")
     return ns
 
 
