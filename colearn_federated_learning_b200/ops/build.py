@@ -47,7 +47,7 @@ def _stamp(src: str, flags: List[str]) -> str:
     h = hashlib.sha1()
     with open(src, "rb") as f:
         h.update(f.read())
-    for dep in ("colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "mlp_v2.inc", "conv_ops.cuh", "conv_bindings.inc"):
+    for dep in ("colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "mlp_v2.cuh", "conv_ops.cuh", "conv_bindings.inc"):
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(flags).encode())
@@ -135,7 +135,7 @@ def simt_path() -> str:
 
 
 def build_simt_emul(force: bool = False) -> str:
-    """g++ build of ``csrc/simt_emul.cpp``: ``mlp_persistent.cu`` + ``mlp_v2.inc`` — the kernel sources themselves —
+    """g++ build of ``csrc/simt_emul.cpp``: ``mlp_persistent.cu`` + ``mlp_v2.cuh`` — the kernel sources themselves —
     compiled for the CPU with one OS thread per CUDA thread (``csrc/host_shim.h``).  Needs C++20 (``std::barrier``) and
     the CUDA headers, no GPU and no CUDA libraries."""
     ce, cuda_home, inc, flags = _cxx_setup()
@@ -146,7 +146,7 @@ def build_simt_emul(force: bool = False) -> str:
                                                                         f"-DTORCH_EXTENSION_NAME={SIMT_NAME}"]
     sources = ["simt_emul.cpp", "simt_mlp.cpp", "simt_elementwise.cpp", "simt_comm.cpp", "simt_convnet.cpp", "simt_gemm.cpp"]
     h = hashlib.sha1()
-    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_v2.inc", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "conv_ops.cuh"]:
+    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_v2.cuh", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "conv_ops.cuh"]:
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(cxx_flags).encode())

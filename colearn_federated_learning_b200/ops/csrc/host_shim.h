@@ -1,4 +1,4 @@
-// SIMT-on-CPU shim: compiles the warp-synchronous CUDA kernels of this directory (mlp_persistent.cu + mlp_v2.inc) with
+// SIMT-on-CPU shim: compiles the warp-synchronous CUDA kernels of this directory (mlp_persistent.cu + mlp_v2.cuh) with
 // g++ and runs them with one OS thread per CUDA thread, so that the CPU test-suite executes the *same source* the GPU
 // runs — the flagship persistent-MLP kernel included (tests only; never used to train).
 //

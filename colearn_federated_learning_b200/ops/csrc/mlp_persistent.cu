@@ -437,23 +437,23 @@ mlp_local_sgd_kernel(const ClientDesc* __restrict__ descs, SgdHyper hp) {
 // =====================================================================================================
 #define V2_NS v2_128
 #define V2_NT 128
-#include "mlp_v2.inc"
+#include "mlp_v2.cuh"
 #undef V2_NS
 #undef V2_NT
-// 128 threads, blocked reduction slices + pre-scaled dz (see the V2_BLOCKED comment in mlp_v2.inc)
+// 128 threads, blocked reduction slices + pre-scaled dz (see the V2_BLOCKED comment in mlp_v2.cuh)
 #define V2_NS v2_128b
 #define V2_NT 128
 #define V2_BLOCKED 1
-#include "mlp_v2.inc"
+#include "mlp_v2.cuh"
 #undef V2_BLOCKED
 #undef V2_NS
 #undef V2_NT
-// the blocked kernel with its FMAs written in pairs (see the V2_PACKED comment in mlp_v2.inc)
+// the blocked kernel with its FMAs written in pairs (see the V2_PACKED comment in mlp_v2.cuh)
 #define V2_NS v2_128p
 #define V2_NT 128
 #define V2_BLOCKED 1
 #define V2_PACKED 1
-#include "mlp_v2.inc"
+#include "mlp_v2.cuh"
 #undef V2_PACKED
 #undef V2_BLOCKED
 #undef V2_NS

@@ -1,4 +1,4 @@
-// Python face of the SIMT-on-CPU build: mlp_persistent.cu (+ mlp_v2.inc), elementwise.cu and comm.cu — the kernel
+// Python face of the SIMT-on-CPU build: mlp_persistent.cu (+ mlp_v2.cuh), elementwise.cu and comm.cu — the kernel
 // sources themselves — are compiled with g++ through host_shim.h (simt_mlp.cpp / simt_elementwise.cpp / simt_comm.cpp,
 // one OS thread per CUDA thread) and driven here through the same launch_* entry points bindings.cpp uses on a GPU.
 // Tests only (ops/build.py::build_simt_emul, tests/test_simt_emul.py).

@@ -1,4 +1,4 @@
-// mlp_persistent.cu (+ mlp_v2.inc) compiled for the CPU through host_shim.h — see simt_emul.cpp
+// mlp_persistent.cu (+ mlp_v2.cuh) compiled for the CPU through host_shim.h — see simt_emul.cpp
 #define COLEARN_HOST_SHIM 1
 #include "host_shim.h"
 
