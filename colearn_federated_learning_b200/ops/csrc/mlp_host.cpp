@@ -88,7 +88,7 @@ __attribute__((always_inline)) inline void forward_one(const Net& net, const flo
 #pragma omp simd reduction(+ : s)
       for (int i = 0; i < k; ++i) s += wr[i] * in[i];
       s += b[j];
-      if (l < L - 1) s = s > 0.f ? s : 0.f;
+      if (l < L - 1) s = s <= 0.f ? 0.f : s;   // ReLU that keeps NaN, like torch.relu
       else if (net.sigmoid_out) s = 1.f / (1.f + std::exp(-s));
       out[j] = s;
     }
@@ -187,7 +187,7 @@ void run_fit(const Net& net, Task& t, const Hyper& hp, Scratch& sc) {
               for (int i = 0; i < k; ++i) dp[i] += g * wr[i];
             }
             for (int i = 0; i < k; ++i)
-              if (!(a[i] > 0.f)) dp[i] = 0.f;
+              if (a[i] <= 0.f) dp[i] = 0.f;   // threshold_backward: a NaN activation passes the gradient
           }
           if (B == 1) {   // batch-1 (the reference's Arguments): apply the update right away, no gradient arena
             for (int j = 0; j < n; ++j) {
@@ -256,7 +256,7 @@ __attribute__((always_inline)) inline void fixed_forward(const float* theta, flo
 #pragma omp simd reduction(+ : s)
       for (int i = 0; i < K; ++i) s += wr[i] * in[i];
       s += b[j];
-      if (l < S::L - 1) s = s > 0.f ? s : 0.f;
+      if (l < S::L - 1) s = s <= 0.f ? 0.f : s;   // (keeps NaN)
       else if (sigmoid_out) s = 1.f / (1.f + std::exp(-s));
       out[j] = s;
     }
@@ -280,7 +280,7 @@ __attribute__((always_inline)) inline void fixed_backward(float* theta, const fl
         for (int i = 0; i < K; ++i) dprev[i] += g * wr[i];
       }
       for (int i = 0; i < K; ++i)
-        if (!(a[i] > 0.f)) dprev[i] = 0.f;
+        if (a[i] <= 0.f) dprev[i] = 0.f;
     }
     for (int j = 0; j < N; ++j) {
       const float g = lr * dz[j];

@@ -97,6 +97,22 @@ __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {
 }
 #endif
 
+// max that keeps NaN, like torch.relu / torch.clamp: fmaxf(NaN, 0) is 0, which let a NaN sample train the rest of the model
+// on zeros and report a finite loss.  max.NaN.f32 is still one FMNMX; without a NaN operand it gives the bits of fmaxf.
+#ifdef COLEARN_HOST_SHIM
+inline float fmax_nan(float a, float b) { return a != a ? a : (b != b ? b : fmaxf(a, b)); }
+#else
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+#endif
+__device__ __forceinline__ float relu_nan(float z) { return fmax_nan(z, 0.f); }
+// ReLU backward as threshold_backward computes it: the gradient passes unless the activation is <= 0, so a NaN activation
+// passes it on (`a > 0 ? g : 0` would zero it)
+__device__ __forceinline__ float relu_grad(float a, float g) { return a <= 0.f ? 0.f : g; }
+
 // ---- per-layer device functions ----------------------------------------------------------------
 // OWN_ONLY (the training kernel): threads past the last (neuron, lane) pair skip the weight reads instead of shadowing
 // the last neuron's row — their result was always discarded, but in the training loop those reads raced with the owner
@@ -125,7 +141,7 @@ __device__ __forceinline__ void fwd_layer(const float* __restrict__ sP, const fl
   for (int o = T / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   if (valid && t == 0) {
     const float z = acc + sP[Offs<N, LI>::smem + NO * KP + n];
-    a_out[n] = RELU ? fmaxf(z, 0.f) : z;
+    a_out[n] = RELU ? relu_nan(z) : z;
   }
 }
 
@@ -148,7 +164,7 @@ __device__ __forceinline__ void bwd_dh(const float* __restrict__ sP, const float
   float acc = acc0 + acc1;
 #pragma unroll
   for (int o = TB / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if (valid && t == 0) dz_in[k] = a_in[k] > 0.f ? acc : 0.f;
+  if (valid && t == 0) dz_in[k] = relu_grad(a_in[k], acc);
 }
 
 // P[n][k] += scale * dz_out[n] * a_in[k];  bias[n] += scale * dz_out[n]
@@ -222,7 +238,7 @@ __device__ __forceinline__ float loss_and_dz(float* aL, float* dzL, const float*
       float out = z, dact = 1.f;
       if (N::kSigmoid) { out = 1.f / (1.f + __expf(-z)); dact = out * (1.f - out); aL[lane] = out; }
       if (loss == LOSS_BCE) {
-        const float lp = fmaxf(__logf(out), -100.f), l1p = fmaxf(log1pf(-out), -100.f);
+        const float lp = fmax_nan(__logf(out), -100.f), l1p = fmax_nan(log1pf(-out), -100.f);
         contrib = -(y * lp + (1.f - y) * l1p) * (1.f / DO);
         dzL[lane] = (out - y) * inv_b * (1.f / DO);
       } else {  // SSE / MSE
@@ -312,7 +328,7 @@ mlp_local_sgd_kernel(const ClientDesc* __restrict__ descs, SgdHyper hp) {
   const int n = d.n;
   const int ydim = d.y_dim;
   const int row = DIN + ydim;
-  const int spe = (n + B - 1) / B;  // steps per epoch
+  const int spe = ((n > 0 ? n : 1) + B - 1) / B;  // steps per epoch (an empty shard: Q = 0 below, see the v2 kernel)
   long long total_steps = (long long)hp.epochs * spe;
   if (hp.max_steps > 0 && hp.max_steps < total_steps) total_steps = hp.max_steps;
   // total samples consumed by those steps

@@ -254,7 +254,7 @@ __device__ __forceinline__ void fwd(AllRegs<N, 0, ACC>& all, const float* __rest
   for (int o = R::T / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   if (valid && t == 0) {
     const float z = BLK ? acc : acc + r.br;
-    a_out[n] = RELU ? fmaxf(z, 0.f) : z;
+    a_out[n] = RELU ? relu_nan(z) : z;
   }
 }
 
@@ -374,7 +374,7 @@ __device__ __forceinline__ float bwd(AllRegs<N, 0, ACC>& all, const float* __res
 #pragma unroll
     for (int o = R::TB / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
     ak = a_in[k];
-    dz_mine = ak > 0.f ? acc : 0.f;
+    dz_mine = relu_grad(ak, acc);
     if (WRITE_SMEM && valid && t == 0) {
       dz_in[k] = dz_mine;
       if constexpr (BLK && !ACC) dz_in[k + ATot<N>::v] = scale * dz_mine;
@@ -640,7 +640,7 @@ __device__ __forceinline__ void head_backward(AllRegs<N, 0, ACC>& all, HeadRegs<
   for (int o = R::TB / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   const float ak = a_in[k];
   if (valid && t == 0) {
-    const float dzk = ak > 0.f ? acc : 0.f;
+    const float dzk = relu_grad(ak, acc);
     dz_in[k] = dzk;
     if constexpr (BLK && !ACC) dz_in[k + ATot<N>::v] = scale * dzk;   // see bwd(): SIN
   }
@@ -782,7 +782,10 @@ mlp_local_sgd_kernel_v2(const ClientDesc* __restrict__ descs, SgdHyper hp) {
   int* sIdx = reinterpret_cast<int*>(sMisc + 8);   // RING: 2 x CHUNK sample indices
 
   const int n = d.n, ydim = d.y_dim, row = DIN + ydim;
-  const int spe = (n + B - 1) / B;
+  // An empty shard (trailing virtual clients of a short one, see shard_bounds) gets Q = 0 (spe counts it as one step per
+  // epoch of 0 samples): no steps and no loads from x, y or perm; the write-out stores out_scale * theta_in (0 in delta
+  // mode), the losses are {0, 0}, the flags work as usual.
+  const int spe = ((n > 0 ? n : 1) + B - 1) / B;
   long long total_steps = (long long)hp.epochs * spe;
   if (hp.max_steps > 0 && hp.max_steps < total_steps) total_steps = hp.max_steps;
   long long Q;

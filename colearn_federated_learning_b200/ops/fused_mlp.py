@@ -52,7 +52,11 @@ def _ptr(t: PtrLike) -> int:
 
 @dataclass
 class ClientTask:
-    """Everything one client CTA needs.  Pointers may be tensors or raw ints (peer memory)."""
+    """Everything one client CTA needs.  Pointers may be tensors or raw ints (peer memory).
+
+    An empty shard (``x`` with 0 rows, e.g. a trailing virtual client of a short shard) is a valid task: the kernel runs no
+    step and reads nothing from ``x``, ``y`` or ``perm``, writes ``out_scale * theta_in`` (0 in delta mode) to ``theta_out``
+    and ``{0, 0}`` to ``loss_out``, and still waits on ``wait_flag`` and raises ``signal_flag``."""
 
     x: torch.Tensor                      # [n, d_in] fp32 CUDA
     y: torch.Tensor                      # [n, y_dim] fp32 CUDA (xent: class index as float)

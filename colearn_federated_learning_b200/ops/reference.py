@@ -102,7 +102,8 @@ def mlp_backward(flat: torch.Tensor, dims: Sequence[int], acts: List[torch.Tenso
         gw.copy_(dz.t() @ a)
         gb.copy_(dz.sum(0))
         if li > 0:
-            dz = (dz @ w) * (a > 0).to(dz.dtype)  # a = relu(z_{li-1})
+            # a = relu(z_{li-1}); ReLU's backward as autograd computes it: 0 where a <= 0, so a NaN activation passes dz on
+            dz = torch.ops.aten.threshold_backward(dz @ w, a, 0)
     return grad
 
 
