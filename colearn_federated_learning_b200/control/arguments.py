@@ -58,6 +58,8 @@ class Arguments:
     eval_bins: int = 256           # federated evaluation: score histogram bins, a power of two in [2, 4096]
     eval_threshold: float = 0.5    # federated evaluation: a one-column model predicts the positive class iff p > threshold
     eval_fraction: float = 0.0     # federated evaluation, local and box mode: fraction of every device's shard held out, in (0, 1)
+    alarm_fpr: float = 0.01        # autoencoder: the alarm threshold lets at most this fraction of the held-out benign rows raise an
+                                   # alarm, in (0, 1) (fl/anomaly.py)
     async_buffer: int = 0          # remote mode: >0 = asynchronous buffered aggregation, one server step per K replies from devices
                                    # that train from whatever version is current (fl/asyncagg.py); 0 = synchronous rounds
     async_concurrency: int = 0     # asynchronous: fits in flight (0 = one per selected device)
@@ -138,6 +140,8 @@ class Arguments:
             raise ValueError(f"--eval-threshold must be in [0, 1], not {self.eval_threshold}")
         if not 0.0 <= self.eval_fraction < 1.0:
             raise ValueError(f"--eval-fraction must be in [0, 1), not {self.eval_fraction}")
+        if not 0.0 < self.alarm_fpr < 1.0:
+            raise ValueError(f"--alarm-fpr must be in (0, 1), not {self.alarm_fpr}")
         if self.eval_fraction > 0 and self.fed_eval_every == 0:
             raise ValueError("--eval-fraction holds rows out for --fed-eval-every, which is not set")
         if self.fed_eval_every > 0 and self.secure_agg:

@@ -29,7 +29,7 @@ import numpy as np
 import torch
 
 from ..data import dataset_tensors
-from ..fl import fedeval
+from ..fl import anomaly, fedeval
 from ..fl.trainer import FitConfig, local_fit
 from ..fl.evaluate import predict as predict_fn
 from ..fl.secagg import SecAggDevice
@@ -238,6 +238,8 @@ class WorkerServer:
                 spec = getattr(model, "spec", None)
                 if spec is not None and not spec.flatten_input and x.shape[1] != spec.dims[0]:
                     return {"ok": False, "error": f"dataset has {x.shape[1]} features, {cfg.model} wants {spec.dims[0]}"}
+                if anomaly.is_autoencoder(model):
+                    x, y = anomaly.training_rows(x, y)       # the benign rows, the input as the target; n = their count
                 if sa is not None:
                     if any(b.is_floating_point() for b in model.buffers()):
                         return {"ok": False, "error": f"secure aggregation refused: {cfg.model}'s floating-point buffers would travel in the clear"}
@@ -311,6 +313,8 @@ class WorkerServer:
                     spec = getattr(model, "spec", None)
                     if spec is not None and not spec.flatten_input and held[0].shape[1] != spec.dims[0]:
                         return {"ok": False, "error": f"evaluation data has {held[0].shape[1]} features, {req.get('model')} wants {spec.dims[0]}"}
+                    if anomaly.is_autoencoder(model):
+                        return {"ok": True, **anomaly.to_wire(anomaly.summarize(model, flat, held[0], held[1], int(req.get("bins", 256)))[0])}
                     s = fedeval.summarize(model, flat, held[0], held[1], int(req.get("bins", 256)), float(req.get("threshold", 0.5)))[0]
                 except (ValueError, TypeError) as e:
                     return {"ok": False, "error": f"evaluation refused: {e}"}
@@ -326,6 +330,16 @@ class WorkerServer:
                 spec = getattr(model, "spec", None)
                 keep_shape = spec is None                       # conv nets take [C, H, W] samples as they are
                 x = torch.stack([d if keep_shape else d.reshape(-1) for d in data]).float()
+                if anomaly.is_autoencoder(model):
+                    # per-row alarms at the federated threshold the request carries ("alarm_bin" of "bins" error bins)
+                    j, bins = req.get("alarm_bin"), req.get("bins")
+                    if not isinstance(j, int) or not isinstance(bins, int) or isinstance(j, bool) or isinstance(bins, bool):
+                        return {"ok": False, "error": f"{req['model']} predicts alarms: the request needs an integer alarm_bin and bins"}
+                    try:
+                        pred = anomaly.predict(model, flat, x, j, bins)
+                    except ValueError as e:
+                        return {"ok": False, "error": f"prediction refused: {e}"}
+                    return {"ok": True, "pred": pred.reshape(-1).tolist(), "count": len(data)}
                 pred = predict_fn(model, x, flat)
                 return {"ok": True, "pred": pred.reshape(-1).tolist(), "count": len(data)}
         return {"ok": False, "error": f"unknown op {op!r}"}
@@ -509,8 +523,13 @@ class RemoteWorkerClient:
     def search(self, tag: str) -> int:
         return int(self._call({"op": "search", "tag": tag}).get("count", 0))
 
-    def predict(self, flat: torch.Tensor, model_name: str, tag: str = "inference") -> List[int]:
-        return list(self._call({"op": "predict", "params": _to_bytes(flat), "model": model_name, "tag": tag})["pred"])
+    def predict(self, flat: torch.Tensor, model_name: str, tag: str = "inference", alarm: Optional[Dict[str, Any]] = None) -> List[int]:
+        """The device's predictions on its ``tag`` rows; an autoencoder needs ``alarm`` (``alarm_bin`` and ``bins`` of the
+        checkpoint's federated threshold) and returns 0 / 1 alarms"""
+        req = {"op": "predict", "params": _to_bytes(flat), "model": model_name, "tag": tag}
+        if alarm is not None:
+            req.update(alarm_bin=int(alarm["alarm_bin"]), bins=int(alarm["bins"]))
+        return list(self._call(req)["pred"])
 
     def close(self) -> None:
         with self._lock:

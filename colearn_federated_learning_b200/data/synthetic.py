@@ -30,6 +30,29 @@ def synthetic_unsw(n: int, seed: int = 0, n_features: int = 10, noise: float = 0
     return x, y
 
 
+def synthetic_anomaly(n: int, seed: int = 0, attack_fraction: float = 0.1,
+                      device: Optional[torch.device] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Traffic for the anomaly detector (``--model autoencoder``): ``(X[n, 10] in [0, 1], y[n, 1])``, deterministic in
+    ``seed``.  A benign row (y = 0) lies near a 3-dimensional manifold: the sigmoid of a standard-normal latent through a
+    fixed 10 x 3 map (the same for every seed), plus N(0, 0.01^2) noise.  An attack row (y = 1, each row with probability
+    ``attack_fraction``) is uniform in [0, 1]^10, off the manifold almost surely."""
+    if not 0.0 <= attack_fraction <= 1.0:
+        raise ValueError(f"attack_fraction must be in [0, 1], not {attack_fraction}")
+    fixed = torch.Generator().manual_seed(20190718)
+    w = torch.randn(10, 3, generator=fixed) * 1.5
+    b = torch.randn(10, generator=fixed) * 0.5
+    g = torch.Generator().manual_seed(seed)
+    z = torch.randn(n, 3, generator=g)
+    benign = (torch.sigmoid(z @ w.t() + b) + 0.01 * torch.randn(n, 10, generator=g)).clamp(0.0, 1.0)
+    attack = torch.rand(n, 10, generator=g)
+    y = (torch.rand(n, generator=g) < attack_fraction).view(n, 1)
+    x = torch.where(y, attack, benign)
+    y = y.float()
+    if device is not None:
+        x, y = x.to(device), y.to(device)
+    return x, y
+
+
 def synthetic_images(n: int, seed: int = 0, size: int = 32, classes: int = 10,
                      device: Optional[torch.device] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Synthetic ``[n,3,size,size]`` images with class-dependent mean (BASELINE config 4)."""
@@ -46,7 +69,8 @@ def synthetic_for_model(model: str, n: int, seed: int = 0,
                         device: Optional[torch.device] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Synthetic data of the shape ``model`` consumes (``--synthetic N`` on the CLIs): 32x32 images with 10 classes
     for ``resnet18``, 28x28 single-channel digits-shaped inputs for ``net`` (784-128-64-10), two XOR-like features
-    for ``testing_remote``, the ten UNSW-IoT features otherwise.  Labels are ``[n, 1]`` floats (class index for the
+    for ``testing_remote``, benign rows on a manifold with 10 % attacks off it for ``autoencoder``, the ten UNSW-IoT features
+    otherwise.  Labels are ``[n, 1]`` floats (class index for the
     cross-entropy models), which is what every fit executor accepts."""
     if model == "resnet18":
         x, y = synthetic_images(n, seed=seed)
@@ -56,6 +80,8 @@ def synthetic_for_model(model: str, n: int, seed: int = 0,
         x, y = x[:, :1].contiguous(), y.float().view(n, 1)
     elif model == "testing_remote":
         x, y = synthetic_unsw(n, seed=seed, n_features=2)
+    elif model == "autoencoder":
+        x, y = synthetic_anomaly(n, seed=seed)
     else:
         x, y = synthetic_unsw(n, seed=seed)
     if device is not None:

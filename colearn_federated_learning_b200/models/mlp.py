@@ -25,8 +25,9 @@ import torch.nn.functional as F
 class MLPSpec:
     dims: Tuple[int, ...]          # (in, h1, ..., out)
     out_activation: str = "none"   # none | sigmoid
-    default_loss: str = "xent"     # bce | sse | xent
+    default_loss: str = "xent"     # bce | sse | xent | mse
     flatten_input: bool = False
+    target: str = "label"          # label: trained on the dataset's labels; input: trained to reconstruct its input (fl/anomaly.py)
 
     @property
     def n_layers(self) -> int:
@@ -85,6 +86,7 @@ TESTING_REMOTE_SPEC = MLPSpec((2, 50, 10, 1), "none", "sse")
 NET_SPEC = MLPSpec((784, 128, 64, 10), "none", "xent", flatten_input=True)
 MLP_SPEC = MLPSpec((10, 64, 64, 2), "none", "xent")
 WIDE_MLP_SPEC = MLPSpec((10, 4096, 4096, 4096, 4096, 2), "none", "xent")
+AE_SPEC = MLPSpec((10, 32, 4, 32, 10), "none", "mse", target="input")
 
 
 class FFNN(MLPNet):
@@ -115,6 +117,16 @@ class MLP(MLPNet):
 
     def __init__(self) -> None:
         super().__init__(MLP_SPEC)
+
+
+class Autoencoder(MLPNet):
+    """Anomaly detector: 10-32-4-32-10 trained on benign rows to reconstruct its input (974 params); a row whose
+    reconstruction error passes the federated alarm threshold is an alarm (fl/anomaly.py)."""
+
+    spec = AE_SPEC                  # on the class too: the CLI tells an autoencoder from its registry entry without building it
+
+    def __init__(self) -> None:
+        super().__init__(AE_SPEC)
 
 
 class WideMLP(MLPNet):

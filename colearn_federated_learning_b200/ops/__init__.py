@@ -369,6 +369,33 @@ def eval_summary(scores: torch.Tensor, labels: torch.Tensor, bins: int = 256, th
     return reference.eval_summary(scores, labels, int(bins), float(threshold), offsets)
 
 
+def recon_summary(xhat: torch.Tensor, x: torch.Tensor, labels: Optional[torch.Tensor] = None, bins: int = 256,
+                  segments: Optional[Sequence[int]] = None, alarm_bin: Optional[int] = None):
+    """Reconstruction-error summary of an autoencoder's outputs (``ops/csrc/recon_summary.cuh``): ``(counts int64 [S, 2 + 2 B],
+    err_sum float64 [S], err fp32 [N] or None, flag uint8 [N] or None)``, one row per segment of consecutive rows.  ``xhat``:
+    the model's output ``[N, D]``, ``x``: its input, ``labels``: ``[N]`` 0 / 1 or None, ``segments``: the row count of every
+    segment (one segment of all rows when None).  Row ``s`` of ``counts`` holds ``n``, ``n_invalid`` and the error
+    histograms of label 0 and label 1 (``fl/anomaly.py`` reads them).  With ``alarm_bin`` also the per-row error and alarm
+    flag.  CUDA tensors: one memset and one ``recon_summary_kernel`` launch; CPU tensors: ``reference.recon_summary``."""
+    n = x.shape[0]
+    sizes = [n] if segments is None else [int(s) for s in segments]
+    if any(s < 0 for s in sizes) or sum(sizes) != n or not sizes:
+        raise ValueError(f"segments {sizes} do not cover the {n} rows")
+    offsets = [0]
+    for s in sizes:
+        offsets.append(offsets[-1] + s)
+    if xhat.dim() != 2 or tuple(xhat.shape) != tuple(x.shape):
+        raise ValueError(f"xhat {tuple(xhat.shape)} and x {tuple(x.shape)} must both be [N, D]")
+    reference.recon_summary_limits(int(x.shape[1]), int(bins), n, alarm_bin)
+    if _cuda(x):
+        lab = None if labels is None else labels.to(x.device, torch.float32).contiguous().view(-1)
+        counts, total, err, flag = _ext.require().recon_summary(xhat.to(x.device).float().contiguous(), x.float().contiguous(), lab,
+                                                                torch.tensor(offsets, dtype=torch.int64), int(bins),
+                                                                -1 if alarm_bin is None else int(alarm_bin), 0)
+        return counts, total, (err if alarm_bin is not None else None), (flag if alarm_bin is not None else None)
+    return reference.recon_summary(xhat, x, labels, int(bins), offsets, alarm_bin)
+
+
 def argmax_rows(x: torch.Tensor) -> torch.Tensor:
     """``x.argmax(1, keepdim=True)`` (SURVEY K16; reference inference fc.py:252-256)."""
     if _cuda(x):

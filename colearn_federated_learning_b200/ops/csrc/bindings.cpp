@@ -65,6 +65,7 @@ void set_spin_limit(double seconds) {
   const unsigned long long ns = seconds <= 0 ? 0ull : (unsigned long long)(seconds * 1e9);
   check(set_spin_limit_comm(ns), "set_spin_limit (comm)");
   check(set_spin_limit_mlp(ns), "set_spin_limit (mlp)");
+  check(set_spin_limit_mlp_ae(ns), "set_spin_limit (mlp, autoencoder)");
   check(set_spin_limit_gemm(ns), "set_spin_limit (gemm)");
   check(preload_comm_kernels(), "preload_comm_kernels");     // same call site: once per device, before any round
 }
@@ -501,6 +502,40 @@ std::vector<torch::Tensor> eval_summary(torch::Tensor scores, torch::Tensor labe
   check(launch_eval_summary(a, (int)grid, cur_stream()), "eval_summary");
   const int64_t L = es_row_len(C, (int)bins);
   return {out.narrow(0, 0, S * L).view({S, L}), out.narrow(0, S * L, S).view(at::kDouble)};
+}
+// Reconstruction-error summary (recon_summary.cuh): xhat / x [N, D] contiguous CUDA fp32, labels [N] CUDA fp32 or none, offsets
+// CPU int64 [S + 1]; alarm_bin >= 0 also writes the per-row error and alarm flag.  Returns (counts int64 [S, 2 + 2 B],
+// err_sum float64 [S], err fp32 [N] and flag uint8 [N], both empty without alarm_bin).  Limits are checked before the launch.
+std::vector<torch::Tensor> recon_summary(torch::Tensor xhat, torch::Tensor x, c10::optional<torch::Tensor> labels, torch::Tensor offsets,
+                                         int64_t bins, int64_t alarm_bin, int64_t grid) {
+  CHECK_CUDA_F32(xhat); CHECK_CUDA_F32(x);
+  TORCH_CHECK(xhat.dim() == 2 && x.sizes() == xhat.sizes() && x.device() == xhat.device(), "xhat and x: [N, D] on one device");
+  if (labels.has_value()) {
+    CHECK_CUDA_F32((*labels));
+    TORCH_CHECK(labels->dim() == 1 && labels->size(0) == x.size(0) && labels->device() == x.device(), "labels [N] on the device of x");
+  }
+  TORCH_CHECK(!offsets.is_cuda() && offsets.scalar_type() == at::kLong && offsets.is_contiguous() && offsets.dim() == 1 && offsets.numel() >= 2 &&
+              offsets.numel() - 1 <= INT32_MAX, "offsets: CPU int64 [S + 1]");
+  TORCH_CHECK(x.size(1) <= kRsMaxDim && recon_summary_args_ok((int)x.size(1), (int)bins) && bins <= kRsMaxBins,
+              "recon_summary: D in 1..1024, bins a power of two in 32..4096 (D = ", x.size(1), ", bins = ", bins, ")");
+  TORCH_CHECK(alarm_bin < 0 || alarm_bin <= bins, "recon_summary: the alarm bin must be in [0, bins]");
+  const int S = (int)offsets.numel() - 1;
+  std::vector<int64_t> table;
+  const int64_t units = es_build_table(offsets.data_ptr<int64_t>(), S, table);
+  TORCH_CHECK(units >= 0 && table[S] == x.size(0), "offsets must rise from 0 to N");
+  TORCH_CHECK(x.size(0) <= kEsMaxRows, "recon_summary: at most 2^32 - 1 rows per launch (uint32 shared-memory counters)");
+  c10::cuda::CUDAGuard guard(x.device());
+  auto dev_table = torch::from_blob(table.data(), {(int64_t)table.size()}, torch::kLong).to(x.device());
+  auto out = torch::empty({rs_out_words(S, (int)bins, units)}, x.options().dtype(at::kLong));
+  const bool rows = alarm_bin >= 0;
+  auto err = torch::empty({rows ? x.size(0) : 0}, x.options());
+  auto flag = torch::empty({rows ? x.size(0) : 0}, x.options().dtype(at::kByte));
+  ReconSummaryArgs a{xhat.data_ptr<float>(), x.data_ptr<float>(), labels.has_value() ? labels->data_ptr<float>() : nullptr,
+                     dev_table.data_ptr<int64_t>(), S, units, (int)x.size(1), (int)bins, rows ? (int)alarm_bin : 0,
+                     rows ? err.data_ptr<float>() : nullptr, rows ? flag.data_ptr<uint8_t>() : nullptr, out.data_ptr<int64_t>()};
+  check(launch_recon_summary(a, (int)grid, cur_stream()), "recon_summary");
+  const int64_t L = rs_row_len((int)bins);
+  return {out.narrow(0, 0, S * L).view({S, L}), out.narrow(0, S * L, S).view(at::kDouble), err, flag};
 }
 torch::Tensor argmax_rows(torch::Tensor x) {
   CHECK_CUDA_F32(x);
@@ -942,6 +977,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_xent_head", &softmax_xent_head);
   m.def("eval_binary", &eval_binary);
   m.def("eval_summary", &eval_summary);
+  m.def("recon_summary", &recon_summary);
   m.def("argmax_rows", &argmax_rows);
   m.def("minmax_scale", &minmax_scale);
   m.def("feistel_permutation", &feistel_permutation);

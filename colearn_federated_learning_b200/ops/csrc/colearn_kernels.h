@@ -53,6 +53,8 @@
 #include "secagg.cuh"
 // detection-metrics summary of held-out rows (federated evaluation) shared by its kernel and the reference
 #include "eval_summary.cuh"
+// reconstruction-error summary of an autoencoder on held-out rows (federated anomaly detection)
+#include "recon_summary.cuh"
 
 namespace colearn {
 // Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
@@ -132,6 +134,7 @@ inline void spin_wait_ge(const uint32_t* p, uint32_t want, unsigned, const char*
 cudaError_t set_spin_limit_comm(unsigned long long ns);
 cudaError_t preload_comm_kernels();   // force the lazy loader for every kernel of comm.cu (see there)
 cudaError_t set_spin_limit_mlp(unsigned long long ns);
+cudaError_t set_spin_limit_mlp_ae(unsigned long long ns);   // mlp_persistent_ae.cu: its own copy of the limit
 cudaError_t set_spin_limit_gemm(unsigned long long ns);
 
 // ---------------------------------------------------------------------------------------------
@@ -179,7 +182,7 @@ COLEARN_HD uint32_t feistel_index(uint32_t v, uint32_t n, FeistelDomain dom, uin
 // Persistent whole-network local SGD (mlp_persistent.cu)
 // ---------------------------------------------------------------------------------------------
 enum LossKind : int { LOSS_BCE = 0, LOSS_SSE = 1, LOSS_XENT = 2, LOSS_MSE = 3 };
-enum NetKind : int { NET_FFNN = 0, NET_MLP64 = 1, NET_TESTING_REMOTE = 2 };
+enum NetKind : int { NET_FFNN = 0, NET_MLP64 = 1, NET_TESTING_REMOTE = 2, NET_AE = 3 };
 
 // One descriptor per client (= one CTA).  A "client" is a federated worker: it starts from
 // theta_in, runs its local SGD over its private shard and emits out_scale * theta_k (or the
@@ -343,6 +346,9 @@ cudaError_t launch_argmax_rows(const float* x, int64_t* out, int rows, int cols,
 // Detection-metrics summary (eval_summary.cuh): one memset of the outputs, then one launch over the (segment, chunk) units.
 // grid <= 0 picks the grid; the result does not depend on it.  cudaErrorInvalidValue outside the limits of eval_summary.cuh.
 cudaError_t launch_eval_summary(const EvalSummaryArgs& a, int grid, cudaStream_t s);
+// Reconstruction-error summary (recon_summary.cuh): one memset of the outputs, then one launch; the same work units and grid
+// rule as launch_eval_summary.  cudaErrorInvalidValue outside the limits of recon_summary.cuh.
+cudaError_t launch_recon_summary(const ReconSummaryArgs& a, int grid, cudaStream_t s);
 // Column-wise min/max scaling to [0,1] (NetworkTrafficDataset preprocessing, ds.py:31-32)
 cudaError_t launch_minmax_scale(const float* x, float* out, int rows, int cols, cudaStream_t s);
 // Philox-keyed random permutation of [0, n): writes sort keys; caller argsorts? No — full device

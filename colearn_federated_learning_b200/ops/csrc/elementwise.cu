@@ -1606,6 +1606,114 @@ __global__ void __launch_bounds__(kEsThreads) eval_summary_kernel(const EvalSumm
   if (threadIdx.x == 0) *ticket = 0u;
 }
 
+// ---- reconstruction-error summary (recon_summary.cuh) -----------------------------------------------------------------------
+// The work units, shared-memory counts (es_count / es_flush) and the chunk-order float64 sum of eval_summary_kernel; one thread
+// per row computes the row's error over its D columns.
+constexpr int kRsFinalTile = 1024;
+
+// After every CTA flushed: the last CTA (by ticket) adds every segment's chunk sums in chunk order into sum[s] (zeroed by the
+// launcher) and re-arms the ticket.  tile: kRsFinalTile doubles of shared memory.
+__device__ __forceinline__ void rs_sum_chunks_in_order(const double* partial, unsigned* ticket, double* sum, const int64_t* seg_unit0,
+                                                       int64_t segments, int64_t units, double* tile, int* s_last) {
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) *s_last = atomicAdd(ticket, 1u) == gridDim.x - 1 ? 1 : 0;
+  __syncthreads();
+  if (!*s_last) return;
+  __threadfence();
+  for (int64_t base = 0; base < units; base += kRsFinalTile) {
+    const int64_t n = units - base < kRsFinalTile ? units - base : kRsFinalTile;
+    for (int64_t i = threadIdx.x; i < n; i += kEsThreads) tile[i] = __ldcg(partial + base + i);
+    __syncthreads();
+    for (int64_t s = threadIdx.x; s < segments; s += kEsThreads) {
+      const int64_t lo = seg_unit0[s] > base ? seg_unit0[s] : base, hi = seg_unit0[s + 1] < base + n ? seg_unit0[s + 1] : base + n;
+      if (lo >= hi) continue;
+      double t = sum[s];
+      for (int64_t u = lo; u < hi; ++u) t += tile[u - base];
+      sum[s] = t;
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *ticket = 0u;
+}
+
+__global__ void __launch_bounds__(kEsThreads) recon_summary_kernel(const ReconSummaryArgs a) {
+  COLEARN_DYN_SMEM(unsigned, sm);
+  __shared__ double red[kEsThreads / 32];
+  __shared__ double tile[kRsFinalTile];
+  __shared__ int s_last;
+  const int B = a.bins, D = a.dim, lane = threadIdx.x & 31, sub = rs_sub_log2(B);
+  const int64_t L = rs_row_len(B);
+  const int64_t* offsets = a.table;
+  const int64_t* unit_seg = a.table + a.segments + 1;
+  const int64_t* seg_unit0 = unit_seg + a.units;
+  int64_t* counts = a.out;
+  double* sum = reinterpret_cast<double*>(a.out + (int64_t)a.segments * L);
+  unsigned* ticket = reinterpret_cast<unsigned*>(a.out + (int64_t)a.segments * L + a.segments);
+  double* partial = reinterpret_cast<double*>(a.out + (int64_t)a.segments * L + a.segments + 1);
+  for (int64_t i = threadIdx.x; i < L; i += kEsThreads) sm[i] = 0u;
+  int64_t cur = -1;
+  __syncthreads();
+  for (int64_t u = blockIdx.x; u < a.units; u += gridDim.x) {
+    const int64_t s = unit_seg[u];
+    if (s != cur) {
+      if (cur >= 0) es_flush(sm, L, counts + cur * L);
+      cur = s;
+    }
+    const int64_t r0 = offsets[s] + (u - seg_unit0[s]) * kEsChunk;
+    const int64_t r1 = r0 + kEsChunk < offsets[s + 1] ? r0 + kEsChunk : offsets[s + 1];
+    double acc = 0.0;
+    int bad = 0;
+    for (int i = 0; i < kEsRowsPerThread; ++i) {
+      const int64_t row = r0 + threadIdx.x + (int64_t)i * kEsThreads;
+      int word = -1;
+      if (row < r1) {
+        const float* ph = a.xhat + row * D;
+        const float* px = a.x + row * D;
+        double e = 0.0;
+        bool finite = true;
+        for (int c = 0; c < D; ++c) {
+          const float h = ph[c], v = px[c];
+          finite = finite && isfinite(h) && isfinite(v);
+          const double d = (double)(h - v);
+          e += d * d;
+        }
+        int y = 0;
+        if (a.labels != nullptr) {
+          const float l = a.labels[row];
+          y = l == 0.f ? 0 : (l == 1.f ? 1 : -1);
+        }
+        const bool valid = finite && y >= 0;
+        const int b = rs_bin(e, sub);
+        if (a.err != nullptr) a.err[row] = (float)e;
+        if (a.flag != nullptr) a.flag[row] = (!valid || b >= a.alarm_bin) ? 1 : 0;
+        if (valid) {
+          acc += e;
+          word = 2 + y * B + b;
+        } else {
+          ++bad;
+        }
+      }
+      es_count(sm, word);
+    }
+    bad = __reduce_add_sync(0xffffffffu, bad);
+    if (lane == 0 && bad != 0) atomicAdd(sm + 1, (unsigned)bad);
+    acc = warp_tree_f64(acc);
+    if (lane == 0) red[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double t = red[0];
+#pragma unroll
+      for (int w = 1; w < kEsThreads / 32; ++w) t += red[w];
+      partial[u] = t;
+      sm[0] += (unsigned)(r1 - r0);
+    }
+    __syncthreads();
+  }
+  if (cur >= 0) es_flush(sm, L, counts + cur * L);
+  rs_sum_chunks_in_order(partial, ticket, sum, seg_unit0, a.segments, a.units, tile, &s_last);
+}
+
 // MinMax: one block per column pass 1 (min/max), pass 2 scale.  cols is tiny (10).
 __global__ void minmax_scale_kernel(const float* __restrict__ x, float* __restrict__ out, int rows, int cols) {
   __shared__ float smin[32], smax[32];
@@ -2075,6 +2183,25 @@ cudaError_t launch_eval_summary(const EvalSummaryArgs& a, int grid, cudaStream_t
     grid = (int)(a.units < 4 * sms ? a.units : 4 * sms);
   }
   COLEARN_LAUNCH(kernel, grid, kEsThreads, smem, s, a);
+  return cudaGetLastError();
+}
+cudaError_t launch_recon_summary(const ReconSummaryArgs& a, int grid, cudaStream_t s) {
+  if (!recon_summary_args_ok(a.dim, a.bins) || a.segments < 1 || a.units < 0 || (reinterpret_cast<uintptr_t>(a.out) & 7) != 0 ||
+      (a.flag != nullptr && (a.alarm_bin < 0 || a.alarm_bin > a.bins)))
+    return cudaErrorInvalidValue;
+  const int64_t L = rs_row_len(a.bins);
+  cudaError_t e = cudaMemsetAsync(a.out, 0, (size_t)((int64_t)a.segments * L + a.segments + 1) * sizeof(int64_t), s);
+  if (e != cudaSuccess || a.units == 0) return e;
+  const size_t smem = (size_t)L * sizeof(unsigned);
+  e = cudaFuncSetAttribute(recon_summary_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  if (grid <= 0) {
+    int dev = 0, sms = 0;
+    if ((e = cudaGetDevice(&dev)) != cudaSuccess || (e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess)
+      return e;
+    grid = (int)(a.units < 4 * sms ? a.units : 4 * sms);
+  }
+  COLEARN_LAUNCH(recon_summary_kernel, grid, kEsThreads, smem, s, a);
   return cudaGetLastError();
 }
 cudaError_t launch_argmax_rows(const float* x, int64_t* out, int rows, int cols, cudaStream_t s) {

@@ -363,6 +363,33 @@ std::tuple<Tensor, Tensor> eval_summary(Tensor scores, Tensor labels, Tensor off
   const int64_t L = colearn::es_row_len(C, (int)bins);
   return {out.narrow(0, 0, S * L).view({S, L}), out.narrow(0, S * L, S).view(at::kDouble)};
 }
+// reconstruction-error summary: same arguments and results as bindings.cpp::recon_summary on CPU tensors; grid <= 0 picks it
+std::vector<Tensor> recon_summary(Tensor xhat, Tensor x, c10::optional<Tensor> labels, Tensor offsets, int64_t bins, int64_t alarm_bin,
+                                  int64_t grid) {
+  TORCH_CHECK(xhat.dim() == 2 && x.sizes() == xhat.sizes(), "xhat and x: [N, D]");
+  TORCH_CHECK(!labels.has_value() || (labels->dim() == 1 && labels->size(0) == x.size(0)), "labels [N]");
+  TORCH_CHECK(offsets.scalar_type() == at::kLong && offsets.is_contiguous() && offsets.dim() == 1 && offsets.numel() >= 2, "offsets int64 [S + 1]");
+  TORCH_CHECK(x.size(1) <= colearn::kRsMaxDim && colearn::recon_summary_args_ok((int)x.size(1), (int)bins) && bins <= colearn::kRsMaxBins,
+              "recon_summary: arguments outside the limits");
+  TORCH_CHECK(alarm_bin < 0 || alarm_bin <= bins, "recon_summary: the alarm bin must be in [0, bins]");
+  const int S = (int)offsets.numel() - 1;
+  std::vector<int64_t> table;
+  const int64_t units = colearn::es_build_table(offsets.data_ptr<int64_t>(), S, table);
+  TORCH_CHECK(units >= 0 && table[S] == x.size(0), "offsets must rise from 0 to N");
+  TORCH_CHECK(x.size(0) <= colearn::kEsMaxRows, "recon_summary: at most 2^32 - 1 rows per launch (uint32 shared-memory counters)");
+  Tensor out = torch::empty({colearn::rs_out_words(S, (int)bins, units)}, torch::kLong);
+  const bool rows = alarm_bin >= 0;
+  Tensor err = torch::empty({rows ? x.size(0) : 0}, torch::kFloat), flag = torch::empty({rows ? x.size(0) : 0}, torch::kUInt8);
+  colearn::ReconSummaryArgs a{fptr(xhat, "xhat"), fptr(x, "x"), labels.has_value() ? fptr(*labels, "labels") : nullptr, table.data(), S, units,
+                              (int)x.size(1), (int)bins, rows ? (int)alarm_bin : 0, rows ? err.data_ptr<float>() : nullptr,
+                              rows ? flag.data_ptr<uint8_t>() : nullptr, out.data_ptr<int64_t>()};
+  {
+    py::gil_scoped_release nogil;
+    CK(colearn::launch_recon_summary(a, (int)grid, nullptr));
+  }
+  const int64_t L = colearn::rs_row_len((int)bins);
+  return {out.narrow(0, 0, S * L).view({S, L}), out.narrow(0, S * L, S).view(at::kDouble), err, flag};
+}
 Tensor argmax_rows(Tensor x) {
   Tensor out = torch::zeros({x.size(0), 1}, torch::kLong);
   CK(colearn::launch_argmax_rows(fptr(x, "x"), out.data_ptr<int64_t>(), (int)x.size(0), (int)x.size(1), nullptr));
@@ -654,6 +681,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_xent_head", &softmax_xent_head);
   m.def("eval_binary", &eval_binary);
   m.def("eval_summary", &eval_summary);
+  m.def("recon_summary", &recon_summary);
   m.def("argmax_rows", &argmax_rows);
   m.def("minmax_scale", &minmax_scale);
   m.def("feistel_permutation", &feistel_permutation);

@@ -33,9 +33,9 @@ int main() {
   using namespace colearn;
   srand(1);
   // ---- persistent MLP: every net x variant, batch 1 and batch 3 (gradient-accumulation path), two clients ----------------
-  const int din[3] = {10, 10, 2}, dout[3] = {1, 2, 1};
-  const int losses[3] = {LOSS_BCE, LOSS_XENT, LOSS_SSE};
-  for (int kind = 0; kind < 3; ++kind)
+  const int din[4] = {10, 10, 2, 10}, dout[4] = {1, 2, 1, 10};
+  const int losses[4] = {LOSS_BCE, LOSS_XENT, LOSS_SSE, LOSS_MSE};
+  for (int kind = 0; kind < 4; ++kind)
     for (int variant : {1, 3, 5, 6})
       for (int batch : {1, 3}) {
         const int P = mlp_net_num_params(kind), n = 7;
@@ -89,6 +89,12 @@ int main() {
       std::vector<float> z10 = randv(3000 * 10);
       EvalSummaryArgs eb{z10.data(), ylab.data(), table.data(), 3, units, 10, 64, 0.5f, out10.data()};
       CK(launch_eval_summary(eb, 2, nullptr));
+      // reconstruction-error summary: the same segments on 2 CTAs, labels and per-row outputs
+      std::vector<float> xh = randv(3000 * 10), xr = randv(3000 * 10), err(3000);
+      std::vector<uint8_t> flag(3000);
+      std::vector<int64_t> outr(rs_out_words(3, 64, units));
+      ReconSummaryArgs ra{xh.data(), xr.data(), yv.data(), table.data(), 3, units, 10, 64, 40, err.data(), flag.data(), outr.data()};
+      CK(launch_recon_summary(ra, 2, nullptr));
     }
     std::vector<float> feats = randv(200 * 10), scaled(2000);
     CK(launch_minmax_scale(feats.data(), scaled.data(), 200, 10, nullptr));

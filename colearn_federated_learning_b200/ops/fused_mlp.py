@@ -4,7 +4,7 @@ One launch runs the *entire* local fit of one or many federated clients (one CTA
 reference's per-batch ``zero_grad → forward → loss → backward → step`` loop
 (``client_federated.py:101-120`` locally; PySyft ``_fit`` remotely, SURVEY C27) never returns to
 the host.  Supported architectures are the compile-time instantiations FFNN (10-50-30-10-1,
-sigmoid), MLP (10-64-64-2) and TestingRemote (2-50-10-1); anything else goes through the
+sigmoid), MLP (10-64-64-2), TestingRemote (2-50-10-1) and the autoencoder (10-32-4-32-10, MSE on its input); anything else goes through the
 layer-wise trainer (``fl/layerwise.py``).
 """
 from __future__ import annotations
@@ -20,6 +20,7 @@ NET_KINDS = {
     ((10, 50, 30, 10, 1), "sigmoid"): 0,
     ((10, 64, 64, 2), "none"): 1,
     ((2, 50, 10, 1), "none"): 2,
+    ((10, 32, 4, 32, 10), "none"): 3,     # the anomaly detector's autoencoder (models/mlp.py AE_SPEC)
 }
 LOSS_CODES = {"bce": 0, "sse": 1, "xent": 2, "mse": 3}
 # Kernel variants: 5 = register-resident weights, 128-thread CTA, blocked reduction slices (LDS.128) + pre-scaled dz;
@@ -27,7 +28,7 @@ LOSS_CODES = {"bce": 0, "sse": 1, "xent": 2, "mse": 3}
 # (the round-1 default); 1 = smem-resident weights (first version).
 # 0 (default) picks variant 5 for every net.
 KERNEL_VARIANT = int(__import__("os").environ.get("COLEARN_MLP_VARIANT", "0"))
-BEST_VARIANT = {0: 5, 1: 5, 2: 5}          # net kind (NET_KINDS values) -> variant
+BEST_VARIANT = {0: 5, 1: 5, 2: 5, 3: 5}          # net kind (NET_KINDS values) -> variant
 
 
 def resolve_variant(kind: int, variant: Optional[int] = None) -> int:

@@ -852,3 +852,88 @@ def eval_summary(scores: torch.Tensor, labels: torch.Tensor, bins: int = 256, th
     if offsets[0] != 0 or offsets[-1] != n:
         raise ValueError("offsets must rise from 0 to N")
     return counts, loss
+
+
+def recon_summary_limits(dim: int, bins: int, rows: int = 0, alarm_bin: Optional[int] = None) -> None:
+    """The limits of ``ops/csrc/recon_summary.cuh``: ValueError with the reason outside them"""
+    if rows >= 1 << 32:
+        raise ValueError(f"recon_summary: {rows} rows, at most 2^32 - 1 per call (the kernel counts in uint32 shared memory)")
+    if not 1 <= dim <= 1024:
+        raise ValueError(f"recon_summary: {dim} columns, the summary takes 1 to 1024")
+    if bins < 32 or bins > 4096 or bins & (bins - 1):
+        raise ValueError(f"recon_summary: bins must be a power of two in [32, 4096], not {bins}")
+    if alarm_bin is not None and not 0 <= alarm_bin <= bins:
+        raise ValueError(f"recon_summary: the alarm bin must be in [0, {bins}], not {alarm_bin}")
+
+
+def recon_bin(e: torch.Tensor, bins: int) -> torch.Tensor:
+    """``rs_bin`` of ``recon_summary.cuh``: the bin of every float64 error, from the bits of ``(float)e`` (int64)"""
+    sub = (bins // 32).bit_length() - 1
+    u = e.float().view(torch.int32).long() & 0xFFFFFFFF
+    b = (((u >> 23) - 103) << sub) + ((u & 0x7FFFFF) >> (23 - sub))
+    return torch.where(u < 0x33800000, torch.zeros_like(b), torch.where(u >= 0x43800000, torch.full_like(b, bins - 1), b))
+
+
+def recon_summary(xhat: torch.Tensor, x: torch.Tensor, labels: Optional[torch.Tensor] = None, bins: int = 256,
+                  offsets: Optional[Sequence[int]] = None, alarm_bin: Optional[int] = None):
+    """PyTorch transcription of ``ops/csrc/recon_summary.cuh``, equal to the kernel bit for bit: ``(counts int64 [S, 2 + 2 B],
+    err_sum float64 [S], err fp32 [N] or None, flag uint8 [N] or None)`` of the rows ``offsets[s] .. offsets[s + 1]`` (one
+    segment of all rows when ``offsets`` is None); the per-row outputs only with ``alarm_bin``.  The error sum follows the
+    kernel's order exactly: 2048-row chunks, thread t adding rows t, t + 256, ..., t + 1792, a xor butterfly over each warp's
+    32 lanes, the 8 warp sums in order, the chunk sums in order."""
+    xhat = xhat.detach().float().cpu()
+    x = x.detach().float().cpu()
+    if xhat.dim() != 2 or xhat.shape != x.shape:
+        raise ValueError("xhat and x must both be [N, D]")
+    n, d = x.shape
+    recon_summary_limits(d, bins, n, alarm_bin)
+    offsets = [0, n] if offsets is None else [int(o) for o in offsets]
+    if len(offsets) < 2 or offsets[0] != 0 or offsets[-1] != n or any(b < a for a, b in zip(offsets[:-1], offsets[1:])):
+        raise ValueError("offsets must rise from 0 to N")
+    dd = (xhat - x).double()                                        # d formed in fp32, d^2 exact in float64
+    sq = dd * dd
+    e = torch.zeros(n, dtype=torch.float64)
+    for c in range(d):
+        e = e + sq[:, c]
+    valid = torch.isfinite(xhat).all(1) & torch.isfinite(x).all(1)
+    y = torch.zeros(n, dtype=torch.int64)
+    if labels is not None:
+        lab = labels.detach().float().cpu().reshape(-1)
+        y = torch.where(lab == 0, 0, torch.where(lab == 1, 1, -1)).long()
+        valid &= y >= 0
+    b = recon_bin(e, bins)
+    words = torch.where(valid, 2 + y.clamp(min=0) * bins + b, torch.zeros_like(b))
+    ev = torch.where(valid, e, torch.zeros_like(e))
+    length = 2 + 2 * bins
+    counts = torch.zeros(len(offsets) - 1, length, dtype=torch.int64)
+    total = torch.zeros(len(offsets) - 1, dtype=torch.float64)
+    for s_idx, (lo, hi) in enumerate(zip(offsets[:-1], offsets[1:])):
+        v = valid[lo:hi]
+        counts[s_idx, 0] = hi - lo
+        counts[s_idx, 1] = int((~v).sum())
+        counts[s_idx] += torch.bincount(words[lo:hi][v], minlength=length)
+        chunks = (hi - lo + 2047) // 2048
+        if chunks == 0:
+            continue
+        pad = torch.zeros(chunks * 2048, dtype=torch.float64)
+        pad[:hi - lo] = ev[lo:hi]
+        rows = pad.view(chunks, 8, 256)                              # [chunk, i, thread]
+        acc = rows[:, 0]
+        for i in range(1, 8):
+            acc = acc + rows[:, i]
+        lanes = acc.view(chunks, 8, 32)                              # [chunk, warp, lane]
+        for o in (16, 8, 4, 2, 1):
+            lanes = lanes[..., :o] + lanes[..., o:2 * o]
+        warps = lanes[..., 0]
+        part = warps[:, 0]
+        for w in range(1, 8):
+            part = part + warps[:, w]
+        t = torch.zeros((), dtype=torch.float64)
+        for q in range(chunks):
+            t = t + part[q]
+        total[s_idx] = t
+    err = flag = None
+    if alarm_bin is not None:
+        err = e.float()
+        flag = ((~valid) | (b >= alarm_bin)).to(torch.uint8)
+    return counts, total, err, flag

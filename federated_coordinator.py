@@ -121,6 +121,9 @@ def build_parser() -> argparse.ArgumentParser:
     parser.add_argument("--eval-fraction", type=float, default=d.eval_fraction,
                         help="--fed-eval-every in local and box mode: fraction of every device's shard held out for evaluation, in (0, 1) "
                              "(remote devices hold theirs out themselves: remote_worker.py -de / --eval-fraction)")
+    parser.add_argument("--alarm-fpr", type=float, default=d.alarm_fpr,
+                        help="--model autoencoder: the federated alarm threshold is the lowest error bin at which at most this fraction "
+                             "of the devices' held-out benign rows raise an alarm, in (0, 1)")
     parser.add_argument("--async-buffer", type=int, default=d.async_buffer, metavar="K",
                         help="remote mode: asynchronous buffered aggregation (FedBuff): devices train whenever they are free, from the "
                              "current global version, and the server steps once K replies are buffered, each weighted by (1 + "
@@ -195,6 +198,7 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.eval_bins = getattr(ns, "eval_bins", a.eval_bins)
     a.eval_threshold = getattr(ns, "eval_threshold", a.eval_threshold)
     a.eval_fraction = getattr(ns, "eval_fraction", a.eval_fraction)
+    a.alarm_fpr = getattr(ns, "alarm_fpr", a.alarm_fpr)
     a.fed_eval_settings()             # rejects bins / threshold / fraction outside their ranges and --secure-agg with it
     a.async_buffer = getattr(ns, "async_buffer", a.async_buffer)
     a.async_concurrency = getattr(ns, "async_concurrency", a.async_concurrency)
@@ -304,6 +308,12 @@ def parse_cli(argv=None) -> argparse.Namespace:
             check_model(build_model(ns.model))
         except ValueError as e:
             parser.error(f"--fed-eval-every with --model {ns.model}: {e}")
+    from colearn_federated_learning_b200.fl import anomaly
+    if anomaly.is_autoencoder(MODEL_REGISTRY.get(ns.model)):
+        try:
+            anomaly.check_settings(ns, box=ns.box, encryption=ns.encryption)
+        except ValueError as e:
+            parser.error(str(e))
     if ns.secure_agg:
         if ns.box or ns.encryption or not ns.remote:
             parser.error("--secure-agg applies to remote mode (-r) only: in local mode every update is in the coordinator's process "
