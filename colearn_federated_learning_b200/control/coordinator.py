@@ -33,7 +33,7 @@ from .. import ops, settings
 from ..data import federate, synthetic_for_model, BaseDataset
 from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
-from ..fl import anomaly, asyncagg, fedeval
+from ..fl import anomaly, asyncagg, fedeval, uplink
 from ..fl.evaluate import evaluate
 from ..fl.secagg import check_masked_reply, check_unmask_reply, correction_streams, frac_bits, pk_from_bytes, pk_to_bytes
 from ..fl.server_opt import server_opt_state
@@ -54,6 +54,11 @@ log = logging.getLogger(__name__)
 
 def default_device() -> torch.device:
     return torch.device("cuda" if torch.cuda.is_available() else "cpu")
+
+
+def traffic(handle) -> tuple:
+    """(bytes sent, bytes received) so far over a device handle (0 for handles that do not count)"""
+    return getattr(handle, "bytes_sent", 0), getattr(handle, "bytes_received", 0)
 
 
 class Coordinator(BusClient):
@@ -344,21 +349,13 @@ class Coordinator(BusClient):
             agg_w = None
             if live:
                 w = normalized_weights([counts[i] for i in live] if self.args.weighted else None, len(live), device=self.device)
-                if codec.quantized:
-                    # every worker's delta through the uplink codec (one batched encode), as a device would send it
-                    keys = [uplink_key(fed.workers[i], cfg.seed + r) for i in live]
-                    payload, scales = ops.encode_delta(flats[live], replica, codec, keys)
-                    agg_w = self._server_update(theta, partial(ops.fedavg_apply_quantized, theta, payload, scales, w, codec), len(live))
-                elif codec.sparse:
-                    # the live workers' deltas plus residuals through the top-k encode (one batched launch); a worker that
-                    # did not train this round keeps its residual
-                    res = residual if len(live) == len(fed.workers) else residual[live]
-                    indices, values = ops.encode_topk_delta(flats[live], replica, res, codec)
-                    if res is not residual:
-                        residual[live] = res
-                    self._server_update(theta, partial(ops.fedavg_apply_topk, theta, indices, values, w, codec), len(live))
-                else:
-                    agg_w = self._server_update(theta, partial(ops.fedavg_apply, theta, flats[live].contiguous(), w), len(live))
+                # every live worker's update through the uplink codec (one batched encode), as a device would send it; topk: a
+                # worker that did not train this round keeps its residual
+                res = residual if residual is None or len(live) == len(fed.workers) else residual[live]
+                wire = uplink.encode(codec, flats[live], replica, [uplink_key(fed.workers[i], cfg.seed + r) for i in live], res)
+                if res is not residual:
+                    residual[live] = res
+                agg_w = self._server_update(theta, partial(uplink.server_apply, theta, wire, w, codec), len(live))
             for wid, l in zip(fed.workers, losses):
                 self.metrics.worker_loss(wid, l)
                 result["losses"][wid] = l
@@ -487,6 +484,31 @@ class Coordinator(BusClient):
         self.trainings_done += 1
         return result
 
+    async def _fit(self, loop, pool, wid: str, worker, flat: torch.Tensor, rcfg: FitConfig, codec: UplinkCodec, *, ef_reset: bool = False,
+                   secagg: Optional[Dict[str, Any]] = None, downlink: Optional[Dict[str, Any]] = None, version: Optional[int] = None,
+                   crc: Optional[int] = None):
+        """One device's fit RPC, run in ``pool`` (the fields as in :meth:`RemoteWorkerClient.fit_update`): ``(checked update,
+        loss, n)``, or ``(None, None, 0)`` when the RPC failed or the reply failed the checks of its format, or did not echo
+        the replica crc ``crc``.  A device's reply is untrusted input: a malformed update would poison (or abort) the whole
+        average, so such a device counts as failed."""
+        try:
+            if codec.kind == "fp32" and secagg is None:
+                # the fp32 model (never with a compressed downlink): `fit` is every handle's verb for it
+                kw = {} if version is None else {"version": version}
+                got, loss, n = await loop.run_in_executor(pool, lambda: worker.fit(flat, rcfg, timeout=self.fit_timeout, **kw))
+                update = {"params": got}
+            else:
+                update, loss, n = await loop.run_in_executor(pool, lambda: worker.fit_update(
+                    flat, rcfg, codec, ef_reset=ef_reset, secagg=secagg, downlink=downlink, version=version, timeout=self.fit_timeout))
+            if crc is not None and update.get("replica_crc") != crc:
+                raise ValueError(f"replica crc {update.get('replica_crc')!r} returned, the coordinator's is {crc}")
+            if secagg is not None:
+                return check_masked_reply(update, flat.numel()), loss, n
+            return uplink.check_reply(update, codec, flat.numel()), loss, n
+        except Exception as e:  # noqa: BLE001 - a failing device must not sink the round or the training
+            log.info("Worker %s failed its fit: %r", wid, e)
+            return None, None, 0
+
     async def _remote_rounds(self, alive, to_train, theta, cfg, loop, pool, model, result) -> torch.Tensor:
         """The round loop of ``training_remote`` (fc.py:540-568): fan the fit RPC out to every live device, FedAvg what came
         back, repeat.  Returns the final global parameters.  With a quantized ``--uplink-codec`` the devices send their deltas
@@ -513,54 +535,16 @@ class Coordinator(BusClient):
         for r in range(self.enabled_round):
             log.info("\n\n#### ROUND {} #####".format(r))
             t0 = time.time()
-            rcfg = FitConfig(**{**cfg.to_dict(), "seed": cfg.seed + r})
+            rcfg = cfg.with_seed(cfg.seed + r)
             downlink = self._downlink_fields(down, theta, replica, nonce, r, rcfg.seed) if replica is not None else None
             crc = replica_crc(replica) if replica is not None else None
-
-            def same_replica(update):
-                if crc is not None and update.get("replica_crc") != crc:
-                    raise ValueError(f"replica crc {update.get('replica_crc')!r} returned, the coordinator's is {crc}")
-                return update
-
             u1 = list(alive)                                          # secure aggregation: this round's participants
-
-            async def one(wid: str, worker: RemoteWorkerClient):
-                try:
-                    if sa is not None:
-                        fields = {"tag": sa["tag"], "t": r, "u1": u1, "clip": sa["clip"], "frac_bits": sa["frac_bits"]}
-                        fut = loop.run_in_executor(pool, lambda: worker.fit_secagg(theta, rcfg, fields, timeout=self.fit_timeout,
-                                                                                  downlink=downlink))
-                        update, loss, n = await fut
-                        return wid, check_masked_reply(same_replica(update), theta.numel()), loss, n
-                    if codec.quantized:
-                        fut = loop.run_in_executor(pool, lambda: worker.fit_quantized(theta, rcfg, codec, timeout=self.fit_timeout,
-                                                                                     downlink=downlink))
-                        update, loss, n = await fut
-                        return wid, check_quantized_reply(same_replica(update), codec, theta.numel()), loss, n
-                    if codec.sparse:
-                        fut = loop.run_in_executor(pool, lambda: worker.fit_topk(theta, rcfg, codec, ef_reset=r == 0, timeout=self.fit_timeout,
-                                                                                downlink=downlink))
-                        update, loss, n = await fut
-                        return wid, check_topk_reply(same_replica(update), codec, theta.numel()), loss, n
-                    fut = loop.run_in_executor(pool, lambda: worker.fit(theta, rcfg, timeout=self.fit_timeout))
-                    flat, loss, n = await fut
-                    # a device's reply is untrusted input: a wrong-length or non-finite model would poison (or abort) the
-                    # whole average, so such a device counts as failed for this round
-                    flat = torch.as_tensor(flat, dtype=torch.float32).reshape(-1)
-                    if flat.numel() != theta.numel():
-                        raise ValueError(f"model of {flat.numel()} parameters returned, expected {theta.numel()}")
-                    if not bool(torch.isfinite(flat).all()):
-                        raise ValueError("model with non-finite parameters returned")
-                    return wid, flat, loss, n
-                except Exception as e:  # noqa: BLE001 - a failing worker must not sink the round
-                    log.info("Worker %s failed this round: %r", wid, e)
-                    return wid, None, None, 0
-
-            traffic = lambda w: (getattr(w, "bytes_sent", 0), getattr(w, "bytes_received", 0))  # noqa: E731 - any handle type
+            fields = None if sa is None else {"tag": sa["tag"], "t": r, "u1": u1, "clip": sa["clip"], "frac_bits": sa["frac_bits"]}
             sent0 = {wid: traffic(w) for wid, w in alive.items()}
-            results = await asyncio.gather(*[one(wid, w) for wid, w in alive.items()])
+            results = await asyncio.gather(*[self._fit(loop, pool, wid, w, theta, rcfg, codec, ef_reset=r == 0, secagg=fields,
+                                                       downlink=downlink, crc=crc) for wid, w in alive.items()])
             flats, counts, ids = [], [], []
-            for wid, flat, loss, n in results:
+            for wid, (flat, loss, n) in zip(u1, results):
                 if flat is not None:
                     flats.append(flat)
                     counts.append(n)
@@ -577,13 +561,8 @@ class Coordinator(BusClient):
             elif flats:
                 w = normalized_weights(counts if self.args.weighted else None, len(flats), device=self.device)
                 th = theta.to(self.device)
-                if codec.quantized or codec.sparse:
-                    # the checked replies' (payload, scales) or (indices, values), one [K, ...] tensor per field
-                    wire = [torch.stack(field).to(self.device) for field in zip(*flats)]
-                    apply = ops.fedavg_apply_topk if codec.sparse else ops.fedavg_apply_quantized
-                    agg_w = self._server_update(th, partial(apply, th, *wire, w, codec), len(flats))
-                else:
-                    agg_w = self._server_update(th, partial(ops.fedavg_apply, th, torch.stack(flats).to(self.device), w), len(flats))
+                wire = uplink.stack(flats, codec, self.device)
+                agg_w = self._server_update(th, partial(uplink.server_apply, th, wire, w, codec), len(flats))
                 if agg_w is not None:
                     agg_rec["agg_weights"] = agg_w       # the final weight of every device in `ids` (distance-based aggregator)
                 theta = th.cpu()
@@ -620,7 +599,7 @@ class Coordinator(BusClient):
                              "is not defined")
         eval_classes = fedeval.check_model(model) if self.args.fed_eval_every > 0 else None
         th = theta.to(self.device).clone()
-        ring = asyncagg.ring_init(th, st) if not (codec.quantized or codec.sparse) else None
+        ring = asyncagg.ring_init(th, st) if codec.kind == "fp32" else None
         # what a fit request sends: a snapshot of theta at `version`.  A request is serialised later, in the executor thread, and
         # the steps update th in place (th.cpu() is th itself on a CPU coordinator), so every version gets its own copy
         current = th.detach().to("cpu", copy=True)
@@ -631,35 +610,13 @@ class Coordinator(BusClient):
         fitted: set = set()                                        # top-k: a device's first fit resets its residual
         concurrency = st.concurrency or len(alive)
         result["async_discarded"] = 0
-        traffic = lambda w: (getattr(w, "bytes_sent", 0), getattr(w, "bytes_received", 0))  # noqa: E731 - any handle type
-
-        async def fit(wid: str, worker, flat: torch.Tensor, rcfg: FitConfig, reset: bool, base: int):
-            try:
-                if codec.quantized:
-                    update, loss, n = await loop.run_in_executor(pool, lambda: worker.fit_quantized(
-                        flat, rcfg, codec, timeout=self.fit_timeout, version=base))
-                    return check_quantized_reply(update, codec, flat.numel()), loss, n
-                if codec.sparse:
-                    update, loss, n = await loop.run_in_executor(pool, lambda: worker.fit_topk(
-                        flat, rcfg, codec, ef_reset=reset, timeout=self.fit_timeout, version=base))
-                    return check_topk_reply(update, codec, flat.numel()), loss, n
-                got, loss, n = await loop.run_in_executor(pool, lambda: worker.fit(flat, rcfg, timeout=self.fit_timeout, version=base))
-                got = torch.as_tensor(got, dtype=torch.float32).reshape(-1)
-                if got.numel() != flat.numel():
-                    raise ValueError(f"model of {got.numel()} parameters returned, expected {flat.numel()}")
-                if not bool(torch.isfinite(got).all()):
-                    raise ValueError("model with non-finite parameters returned")
-                return got, loss, n
-            except Exception as e:  # noqa: BLE001 - a failing device leaves the training, the others go on
-                log.info("Worker %s failed its fit: %r", wid, e)
-                return None, None, 0
 
         def dispatch() -> None:
             nonlocal dispatched
             while idle and len(in_flight) < concurrency:
                 wid = idle.pop(0)
-                rcfg = FitConfig(**{**cfg.to_dict(), "seed": cfg.seed + dispatched})
-                task = asyncio.ensure_future(fit(wid, alive[wid], current, rcfg, wid not in fitted, version))
+                task = asyncio.ensure_future(self._fit(loop, pool, wid, alive[wid], current, cfg.with_seed(cfg.seed + dispatched), codec,
+                                                       ef_reset=wid not in fitted, version=version))
                 in_flight[task] = (wid, version)
                 fitted.add(wid)
                 dispatched += 1
@@ -724,9 +681,8 @@ class Coordinator(BusClient):
         if plan.kept:
             w = torch.tensor(plan.weights, dtype=torch.float32, device=self.device)
             if ring is None:
-                wire = [torch.stack(field).to(self.device) for field in zip(*[r.update for r in plan.kept])]
-                apply = ops.fedavg_apply_topk if codec.sparse else ops.fedavg_apply_quantized
-                agg_w = self._server_update(th, partial(apply, th, *wire, w, codec), len(plan.kept))
+                wire = uplink.stack([r.update for r in plan.kept], codec, self.device)
+                agg_w = self._server_update(th, partial(uplink.server_apply, th, wire, w, codec), len(plan.kept))
             else:
                 models = torch.stack([r.update for r in plan.kept]).to(self.device)
                 agg_w = self._server_update(th, partial(ops.fedavg_apply_based, th, models, ring, [st.slot(r.base) for r in plan.kept], w,
@@ -770,7 +726,6 @@ class Coordinator(BusClient):
         the training.  Returns ``{"tag", "order", "clip", "frac_bits"}`` (``frac_bits`` for the devices left, see
         :func:`fl.secagg.frac_bits`), or None when fewer than two are left."""
         clip = self.args.secagg_clip_value()
-        traffic = lambda w: (getattr(w, "bytes_sent", 0), getattr(w, "bytes_received", 0))  # noqa: E731
         before = {wid: traffic(w) for wid, w in alive.items()}
         handles = dict(alive)
 
@@ -843,16 +798,14 @@ class Coordinator(BusClient):
         fields: Dict[str, Any] = {"downlink": down.kind, "downlink_topk": down.k, "replica": f"{nonce}:{r}"}
         if r == 0:
             return fields
-        a, b = ops.encode_downlink(theta.to(replica.device), replica, down, downlink_key(seed))
+        wire = ops.encode_downlink(theta.to(replica.device), replica, down, downlink_key(seed))
         fields["replica_base"] = f"{nonce}:{r - 1}"
-        names = ("dpayload", "dscales") if down.quantized else ("dindices", "dvalues")
-        fields[names[0]] = a.cpu().numpy().tobytes()
-        fields[names[1]] = b.cpu().numpy().astype("<f4").tobytes()
+        fields.update(uplink.wire_fields(down, wire, prefix="d"))
         return fields
 
     def _server_update(self, theta: torch.Tensor, apply, k: int) -> Optional[List[float]]:
         """One server step on ``theta`` in place: ``apply`` is a fused FedAvg apply of :mod:`ops` bound to theta and the round's
-        ``k`` rows (``partial(ops.fedavg_apply_quantized, theta, payload, scales, w, codec)`` and the like); it gets the
+        ``k`` rows (``partial(uplink.server_apply, theta, wire, w, codec)`` and the like); it gets the
         aggregate of ``--aggregator`` (mean, median / trimmed mean, geometric median / norm-bounded mean) and the step of
         ``--server-opt``.  Returns the final weight of every row under a distance-based aggregator (0 for a row it excluded),
         None otherwise."""
@@ -935,7 +888,7 @@ def train_virtual_workers(theta: torch.Tensor, model, fed, cfg: FitConfig, round
             sh = fed[wid]
             if len(sh) == 0:
                 continue
-            perm = make_perm(len(sh), FitConfig(**{**cfg.to_dict(), "seed": cfg.seed + 31 * i}), device, round_idx)
+            perm = make_perm(len(sh), cfg.with_seed(cfg.seed + 31 * i), device, round_idx)
             x = sh.x.view(len(sh), -1).contiguous().float()
             y = sh.y.contiguous().float().view(len(sh), -1)
             tasks.append(ops.ClientTask(x=x, y=y, theta_in=theta, theta_out=flats[i], perm=perm, loss_out=loss_out[i]))
@@ -953,7 +906,7 @@ def train_virtual_workers(theta: torch.Tensor, model, fed, cfg: FitConfig, round
         idx = [i for i, wid in enumerate(fed.workers) if len(fed[wid]) > 0]
         if idx:
             shards = [fed[fed.workers[i]] for i in idx]
-            perms = [make_perm(len(sh), FitConfig(**{**cfg.to_dict(), "seed": cfg.seed + 31 * i}), device, round_idx)
+            perms = [make_perm(len(sh), cfg.with_seed(cfg.seed + 31 * i), device, round_idx)
                      for i, sh in zip(idx, shards)]
             res = ops.host.mlp_local_sgd_multi(spec.dims, spec.out_activation, [flats[i] for i in idx], [sh.x for sh in shards],
                                                [sh.y for sh in shards], perms, cfg.batch_size, cfg.lr, cfg.epochs,
@@ -965,7 +918,7 @@ def train_virtual_workers(theta: torch.Tensor, model, fed, cfg: FitConfig, round
         sh = fed[wid]
         if len(sh) == 0:
             continue
-        wcfg = FitConfig(**{**cfg.to_dict(), "seed": cfg.seed + 31 * i})
+        wcfg = cfg.with_seed(cfg.seed + 31 * i)
         last, _ = local_fit(flats[i], model, sh.x, sh.y, wcfg, round_idx)
         losses[i] = float(last)
     return flats, losses, counts

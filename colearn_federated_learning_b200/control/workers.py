@@ -33,7 +33,7 @@ from ..fl import anomaly, fedeval
 from ..fl.trainer import FitConfig, local_fit
 from ..fl.evaluate import predict as predict_fn
 from ..fl.secagg import SecAggDevice
-from ..fl.uplink import UplinkCodec, check_quantized_reply, check_topk_reply, uplink_key
+from ..fl.uplink import FIELDS, UplinkCodec, check_reply, device_reply, echo, request_fields, uplink_key
 from ..models import build_model, num_params
 
 log = logging.getLogger(__name__)
@@ -109,6 +109,11 @@ def _from_bytes(b: bytes, device=None) -> torch.Tensor:
 def replica_crc(replica: torch.Tensor) -> int:
     """crc32 of a downlink replica's fp32 bytes: a device reports it after every fit, the coordinator compares it with its own"""
     return zlib.crc32(_to_bytes(replica))
+
+
+def _codec(kind: str, k: Any) -> UplinkCodec:
+    """The codec a fit request names; ``k`` only counts for topk"""
+    return UplinkCodec(kind, k=k) if kind == "topk" else UplinkCodec(kind)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -208,95 +213,7 @@ class WorkerServer:
             except ValueError as e:
                 return {"ok": False, "error": f"secure aggregation refused: {e}"}
         if op == "fit":
-            cfg = FitConfig.from_dict(req["config"])
-            x, y = self.datasets[req.get("dataset_key", "training")]
-            # "uplink": send the quantized or top-k delta instead of the model (fl/uplink.py); absent = the fp32 model.
-            # topk carries "topk" (k in 1..32, anything else is refused before the fit) and "ef_reset" (zero the residual)
-            kind = req.get("uplink", "fp32")
-            codec = UplinkCodec(kind, k=req.get("topk")) if kind == "topk" else UplinkCodec(kind)
-            # "downlink": the model arrives as a compressed delta to the replica this device keeps (fl/uplink.py); absent = fp32
-            dkind = req.get("downlink", "fp32")
-            down = UplinkCodec(dkind, k=req.get("downlink_topk")) if dkind == "topk" else UplinkCodec(dkind)
-            if down.kind != "fp32" and not isinstance(req.get("replica"), str):
-                return {"ok": False, "error": "a compressed downlink needs the replica's tag"}
-            # "secagg": send the masked fixed-point delta (fl/secagg.py) instead of the model; absent = no secure aggregation
-            sa = req.get("secagg")
-            if sa is not None and (not isinstance(sa, dict) or codec.kind != "fp32"):
-                return {"ok": False, "error": "secure aggregation takes a dict of fields and no uplink codec"}
-            with self._work_lock:
-                if down.kind != "fp32" and "replica_base" in req:
-                    model, flat, err = self._model_and_arena(cfg.model, None)
-                    wire = None if err else self._downlink_wire(req, down, cfg.model, flat.numel())
-                    if isinstance(wire, str):
-                        err = wire
-                elif "params" in req:
-                    model, flat, err = self._model_and_arena(cfg.model, req["params"])
-                else:
-                    err = "fit request without params"
-                if err:
-                    return {"ok": False, "error": err}
-                spec = getattr(model, "spec", None)
-                if spec is not None and not spec.flatten_input and x.shape[1] != spec.dims[0]:
-                    return {"ok": False, "error": f"dataset has {x.shape[1]} features, {cfg.model} wants {spec.dims[0]}"}
-                if anomaly.is_autoencoder(model):
-                    x, y = anomaly.training_rows(x, y)       # the benign rows, the input as the target; n = their count
-                if sa is not None:
-                    if any(b.is_floating_point() for b in model.buffers()):
-                        return {"ok": False, "error": f"secure aggregation refused: {cfg.model}'s floating-point buffers would travel in the clear"}
-                    try:
-                        with self._secagg_lock:
-                            sa_keys, sa_signs = self._secagg.begin_round(sa.get("tag"), sa.get("t"), sa.get("u1"), sa.get("clip"),
-                                                                         sa.get("frac_bits"))
-                    except ValueError as e:
-                        return {"ok": False, "error": f"secure aggregation refused: {e}"}
-                replica = None
-                if down.kind != "fp32":
-                    if "replica_base" in req:             # round t >= 1: advance the replica by the wire, train from it
-                        from .. import ops
-                        replica = self._replicas[cfg.model][1]
-                        ops.apply_downlink(replica, wire[0].to(replica.device), wire[1].to(replica.device), down)
-                        flat.copy_(replica)
-                    else:                                 # round 0: the fp32 model is the replica
-                        replica = flat.clone()
-                    self._replicas[cfg.model] = (str(req.get("replica")), replica)
-                # the theta the coordinator decodes against
-                received = flat.clone() if codec.quantized or codec.sparse or sa is not None else None
-                from ..utils.threads import small_model_threads
-                with small_model_threads(flat.numel(), flat.device):   # tiny models on a CPU device: no OpenMP fork/join
-                    loss, path = local_fit(flat, model, x, y, cfg, round_idx=self._round)
-                self._round += 1
-                self.fits_served += 1
-                if sa is not None:
-                    from .. import ops
-                    masked, clipped, nonfinite = ops.secagg_mask(flat, received, sa_keys, sa_signs, sa["clip"], sa["frac_bits"])
-                    reply = {"ok": True, "secagg": "masked", "masked": masked.cpu().numpy().astype("<u4").tobytes(), "clipped": clipped,
-                             "nonfinite": nonfinite, "loss": float(loss), "n": int(x.shape[0]), "path": path}
-                elif codec.quantized:
-                    from .. import ops
-                    payload, scales = ops.encode_delta(flat.unsqueeze(0), received, codec, [uplink_key(self.id, cfg.seed)])
-                    reply = {"ok": True, "uplink": codec.kind, "payload": payload.cpu().numpy().tobytes(), "scales": _to_bytes(scales),
-                             "loss": float(loss), "n": int(x.shape[0]), "path": path}
-                elif codec.sparse:
-                    from .. import ops
-                    res = self._residuals.get(cfg.model)
-                    if req.get("ef_reset") or res is None or res.numel() != flat.numel() or res.device != flat.device:
-                        res = self._residuals[cfg.model] = torch.zeros(1, flat.numel(), device=flat.device)
-                    indices, values = ops.encode_topk_delta(flat.unsqueeze(0), received, res, codec)
-                    reply = {"ok": True, "uplink": codec.kind, "topk": codec.k, "indices": indices.cpu().numpy().tobytes(),
-                             "values": _to_bytes(values), "loss": float(loss), "n": int(x.shape[0]), "path": path}
-                else:
-                    reply = {"ok": True, "params": _to_bytes(flat), "loss": float(loss), "n": int(x.shape[0]), "path": path}
-                # floating-point buffers the fit updated on this device (BatchNorm running statistics): the flat arena holds
-                # named_parameters only, so without them the coordinator would save trained weights next to the INITIAL running
-                # stats and every eval-mode use of the checkpoint would be meaningless (FFNN / MLPs have none: nothing is sent)
-                bufs = [b.detach().reshape(-1).float() for b in model.buffers() if b.is_floating_point()]
-                if bufs:
-                    reply["buffers"] = _to_bytes(torch.cat(bufs))
-                if replica is not None:
-                    reply["replica_crc"] = replica_crc(replica)
-                if "version" in req:                      # asynchronous aggregation: the global version this fit started from
-                    reply["version"] = req["version"]
-                return reply
+            return self._fit(req)
         if op == "evaluate":
             # federated evaluation (fl/fedeval.py): the model in "params" (fp32) scored on the rows hosted under "evaluation";
             # only the summary's counts leave the device
@@ -344,6 +261,90 @@ class WorkerServer:
                 return {"ok": True, "pred": pred.reshape(-1).tolist(), "count": len(data)}
         return {"ok": False, "error": f"unknown op {op!r}"}
 
+    def _fit(self, req: Dict[str, Any]) -> Dict[str, Any]:
+        """A fit request: its refusals, the model it trains (the fp32 ``params`` or the downlink replica), the fit and the
+        reply with the update in the format the request asks for.  A refused request trains nothing and is not counted."""
+        cfg = FitConfig.from_dict(req["config"])
+        x, y = self.datasets[req.get("dataset_key", "training")]
+        # "uplink": send the quantized or top-k delta instead of the model (fl/uplink.py); absent = the fp32 model.
+        # topk carries "topk" (k in 1..32, anything else is refused before the fit) and "ef_reset" (zero the residual)
+        codec = _codec(req.get("uplink", "fp32"), req.get("topk"))
+        # "downlink": the model arrives as a compressed delta to the replica this device keeps (fl/uplink.py); absent = fp32
+        down = _codec(req.get("downlink", "fp32"), req.get("downlink_topk"))
+        if down.kind != "fp32" and not isinstance(req.get("replica"), str):
+            return {"ok": False, "error": "a compressed downlink needs the replica's tag"}
+        # "secagg": send the masked fixed-point delta (fl/secagg.py) instead of the model; absent = no secure aggregation
+        sa = req.get("secagg")
+        if sa is not None and (not isinstance(sa, dict) or codec.kind != "fp32"):
+            return {"ok": False, "error": "secure aggregation takes a dict of fields and no uplink codec"}
+        with self._work_lock:
+            model, flat, wire = self._restore(req, cfg.model, down)
+            if model is None:
+                return {"ok": False, "error": wire}
+            spec = getattr(model, "spec", None)
+            if spec is not None and not spec.flatten_input and x.shape[1] != spec.dims[0]:
+                return {"ok": False, "error": f"dataset has {x.shape[1]} features, {cfg.model} wants {spec.dims[0]}"}
+            if anomaly.is_autoencoder(model):
+                x, y = anomaly.training_rows(x, y)       # the benign rows, the input as the target; n = their count
+            if sa is not None:
+                if any(b.is_floating_point() for b in model.buffers()):
+                    return {"ok": False, "error": f"secure aggregation refused: {cfg.model}'s floating-point buffers would travel in the clear"}
+                try:
+                    with self._secagg_lock:
+                        sa_keys, sa_signs = self._secagg.begin_round(sa.get("tag"), sa.get("t"), sa.get("u1"), sa.get("clip"),
+                                                                     sa.get("frac_bits"))
+                except ValueError as e:
+                    return {"ok": False, "error": f"secure aggregation refused: {e}"}
+            replica = None
+            if down.kind != "fp32":
+                if wire is not None:                  # round t >= 1: advance the replica by the wire, train from it
+                    from .. import ops
+                    replica = self._replicas[cfg.model][1]
+                    ops.apply_downlink(replica, wire[0].to(replica.device), wire[1].to(replica.device), down)
+                    flat.copy_(replica)
+                else:                                 # round 0: the fp32 model is the replica
+                    replica = flat.clone()
+                self._replicas[cfg.model] = (str(req.get("replica")), replica)
+            # the theta the coordinator decodes against
+            received = flat.clone() if codec.kind != "fp32" or sa is not None else None
+            from ..utils.threads import small_model_threads
+            with small_model_threads(flat.numel(), flat.device):   # tiny models on a CPU device: no OpenMP fork/join
+                loss, path = local_fit(flat, model, x, y, cfg, round_idx=self._round)
+            self._round += 1
+            self.fits_served += 1
+            if sa is not None:
+                from .. import ops
+                masked, clipped, nonfinite = ops.secagg_mask(flat, received, sa_keys, sa_signs, sa["clip"], sa["frac_bits"])
+                update = {"secagg": "masked", "masked": masked.cpu().numpy().astype("<u4").tobytes(), "clipped": clipped,
+                          "nonfinite": nonfinite}
+            else:
+                update = device_reply(codec, flat, received, uplink_key(self.id, cfg.seed), self._residuals, cfg.model,
+                                      bool(req.get("ef_reset")))
+            reply = {"ok": True, **update, "loss": float(loss), "n": int(x.shape[0]), "path": path}
+            # floating-point buffers the fit updated on this device (BatchNorm running statistics): the flat arena holds
+            # named_parameters only, so without them the coordinator would save trained weights next to the INITIAL running
+            # stats and every eval-mode use of the checkpoint would be meaningless (FFNN / MLPs have none: nothing is sent)
+            bufs = [b.detach().reshape(-1).float() for b in model.buffers() if b.is_floating_point()]
+            if bufs:
+                reply["buffers"] = _to_bytes(torch.cat(bufs))
+            if replica is not None:
+                reply["replica_crc"] = replica_crc(replica)
+            if "version" in req:                      # asynchronous aggregation: the global version this fit started from
+                reply["version"] = req["version"]
+            return reply
+
+    def _restore(self, req: Dict[str, Any], name: str, down: UplinkCodec):
+        """``(model, arena, downlink wire)`` a fit request trains from, or ``(None, None, reason)``: the fp32 ``params`` (wire
+        None), or from round t >= 1 of a compressed downlink the arena as it is plus the checked wire that advances the
+        replica (the caller applies it once nothing else refuses the request)."""
+        if down.kind != "fp32" and "replica_base" in req:
+            model, flat, _ = self._model_and_arena(name, None)
+            wire = self._downlink_wire(req, down, name, flat.numel())
+            return (None, None, wire) if isinstance(wire, str) else (model, flat, wire)
+        if "params" not in req:
+            return None, None, "fit request without params"
+        return self._model_and_arena(name, req["params"])
+
     def _downlink_wire(self, req: Dict[str, Any], codec: UplinkCodec, model: str, p: int):
         """The two wire tensors of a round t >= 1 downlink, or the reason it is refused: this device must hold the replica
         of ``model`` tagged ``replica_base``, and the wire must pass the checks the coordinator runs on replies."""
@@ -351,10 +352,7 @@ class WorkerServer:
         if held is None or held[0] != req.get("replica_base") or held[1].numel() != p:
             return f"no replica {req.get('replica_base')!r} of {model} on this device (it holds {held[0] if held else None!r})"
         try:
-            if codec.quantized:
-                return check_quantized_reply({"uplink": codec.kind, "payload": req.get("dpayload"), "scales": req.get("dscales")}, codec, p)
-            return check_topk_reply({"uplink": codec.kind, "topk": codec.k, "indices": req.get("dindices"), "values": req.get("dvalues")},
-                                    codec, p)
+            return check_reply({**echo(codec), **{name: req.get("d" + name) for name in FIELDS[codec.kind]}}, codec, p)
         except ValueError as e:
             return f"downlink refused: {e}"
 
@@ -432,71 +430,37 @@ class RemoteWorkerClient:
 
     def fit(self, flat: torch.Tensor, cfg: FitConfig, dataset_key: str = "training",
             timeout: Optional[float] = None, version: Optional[int] = None) -> Tuple[torch.Tensor, float, int]:
-        """Broadcast leg + remote local-SGD + gather leg (cf.py:209-211) in one RPC.  ``version``: the global version of
-        ``flat`` under asynchronous aggregation (the device echoes it; None sends no version field)."""
-        req = {"op": "fit", "config": cfg.to_dict(), "params": _to_bytes(flat), "dataset_key": dataset_key}
-        if version is not None:
-            req["version"] = int(version)
-        resp = self._call(req, timeout=timeout)
-        self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None     # BatchNorm statistics, if any
-        return _from_bytes(resp["params"]), float(resp["loss"]), int(resp["n"])
+        """Broadcast leg + remote local-SGD + gather leg (cf.py:209-211) in one RPC: the trained fp32 model (unchecked), the
+        loss and the sample count.  ``version`` as in :meth:`fit_update`."""
+        update, loss, n = self.fit_update(flat, cfg, UplinkCodec(), version=version, dataset_key=dataset_key, timeout=timeout)
+        return update["params"], loss, n
 
-    @staticmethod
-    def _fit_request(flat: torch.Tensor, cfg: FitConfig, dataset_key: str, downlink: Optional[Dict[str, Any]]) -> Dict[str, Any]:
-        """the fit request up to the uplink fields: the fp32 model, unless ``downlink`` (the compressed downlink's fields,
-        :meth:`Coordinator._downlink_fields`) replaces it by a wire to the device's replica"""
+    def fit_update(self, flat: torch.Tensor, cfg: FitConfig, codec: UplinkCodec, *, ef_reset: bool = False,
+                   secagg: Optional[Dict[str, Any]] = None, downlink: Optional[Dict[str, Any]] = None, version: Optional[int] = None,
+                   dataset_key: str = "training", timeout: Optional[float] = None) -> Tuple[Dict[str, Any], float, int]:
+        """One fit RPC from ``flat``: the reply's update fields unchecked (untrusted input: the coordinator checks them; an fp32
+        model is decoded to a tensor), the loss and the sample count.  ``codec``: the update's format (topk: ``ef_reset`` zeroes
+        the device's residual first); ``secagg``: the round's ``{"tag", "t", "u1", "clip", "frac_bits"}``, for a masked delta;
+        ``downlink``: :meth:`Coordinator._downlink_fields`, which from round 1 on replace ``flat`` by a wire to the device's
+        replica and add ``replica_crc`` to the update; ``version``: the global version of ``flat`` under asynchronous
+        aggregation (the device echoes it; None sends no version field)."""
         req: Dict[str, Any] = {"op": "fit", "config": cfg.to_dict()}
         if downlink is None or "replica_base" not in downlink:
             req["params"] = _to_bytes(flat)
         req["dataset_key"] = dataset_key
-        return req
-
-    def fit_quantized(self, flat: torch.Tensor, cfg: FitConfig, codec: UplinkCodec, dataset_key: str = "training",
-                      timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None,
-                      version: Optional[int] = None) -> Tuple[Dict[str, Any], float, int]:
-        """:meth:`fit` asking the device for its quantized delta (``codec``): returns the reply's ``{"uplink", "payload",
-        "scales"}`` (and ``"replica_crc"`` with a ``downlink``) unchecked (it is untrusted input: the coordinator validates
-        it), the loss and the sample count.  ``version`` as in :meth:`fit`."""
-        req = self._fit_request(flat, cfg, dataset_key, downlink)
-        req["uplink"] = codec.kind
+        req.update(request_fields(codec, ef_reset))
+        if secagg is not None:
+            req["secagg"] = secagg
         if version is not None:
             req["version"] = int(version)
         resp = self._call({**req, **(downlink or {})}, timeout=timeout)
-        self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None
-        update = {"uplink": resp.get("uplink"), "payload": resp.get("payload"), "scales": resp.get("scales")}
-        if downlink is not None:
-            update["replica_crc"] = resp.get("replica_crc")
-        return update, float(resp["loss"]), int(resp["n"])
-
-    def fit_topk(self, flat: torch.Tensor, cfg: FitConfig, codec: UplinkCodec, ef_reset: bool, dataset_key: str = "training",
-                 timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None,
-                 version: Optional[int] = None) -> Tuple[Dict[str, Any], float, int]:
-        """:meth:`fit` asking the device for the top-k entries of its delta plus residual (``codec``), after zeroing that
-        residual if ``ef_reset``: returns the reply's ``{"uplink", "topk", "indices", "values"}`` (and ``"replica_crc"`` with a
-        ``downlink``) unchecked (it is untrusted input: the coordinator validates it), the loss and the sample count.
-        ``version`` as in :meth:`fit`."""
-        req = self._fit_request(flat, cfg, dataset_key, downlink)
-        req.update({"uplink": codec.kind, "topk": codec.k, "ef_reset": bool(ef_reset)})
-        if version is not None:
-            req["version"] = int(version)
-        resp = self._call({**req, **(downlink or {})}, timeout=timeout)
-        self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None
-        update = {k: resp.get(k) for k in ("uplink", "topk", "indices", "values")}
-        if downlink is not None:
-            update["replica_crc"] = resp.get("replica_crc")
-        return update, float(resp["loss"]), int(resp["n"])
-
-    def fit_secagg(self, flat: torch.Tensor, cfg: FitConfig, fields: Dict[str, Any], dataset_key: str = "training",
-                   timeout: Optional[float] = None, downlink: Optional[Dict[str, Any]] = None) -> Tuple[Dict[str, Any], float, int]:
-        """:meth:`fit` asking the device for its masked update (secure aggregation, ``fields`` = the round's ``{"tag", "t",
-        "u1", "clip", "frac_bits"}``): returns the reply's ``{"secagg", "masked", "clipped", "nonfinite"}`` (and
-        ``"replica_crc"`` with a ``downlink``) unchecked (it is untrusted input: the coordinator validates it), the loss and the
-        sample count."""
-        req = self._fit_request(flat, cfg, dataset_key, downlink)
-        req["secagg"] = fields
-        resp = self._call({**req, **(downlink or {})}, timeout=timeout)
-        self.last_buffers = None
-        update = {k: resp.get(k) for k in ("secagg", "masked", "clipped", "nonfinite")}
+        self.last_buffers = _from_bytes(resp["buffers"]) if resp.get("buffers") else None     # BatchNorm statistics, if any
+        if secagg is not None:
+            update = {k: resp.get(k) for k in ("secagg", "masked", "clipped", "nonfinite")}
+        elif codec.kind == "fp32":
+            update = {"params": _from_bytes(resp["params"])}
+        else:
+            update = {k: resp.get(k) for k in (*echo(codec), *FIELDS[codec.kind])}
         if downlink is not None:
             update["replica_crc"] = resp.get("replica_crc")
         return update, float(resp["loss"]), int(resp["n"])

@@ -18,7 +18,7 @@ from __future__ import annotations
 
 import logging
 import os
-from dataclasses import dataclass, asdict
+from dataclasses import dataclass, asdict, replace
 from typing import Any, Dict, Optional, Tuple
 
 import torch
@@ -50,6 +50,10 @@ class FitConfig:
     @classmethod
     def from_dict(cls, d: Dict[str, Any]) -> "FitConfig":
         return cls(**{k: v for k, v in d.items() if k in cls.__dataclass_fields__})
+
+    def with_seed(self, seed: int) -> "FitConfig":
+        """This config with another ``seed`` (one per round, device or dispatch)"""
+        return replace(self, seed=seed)
 
 
 # Which executor trains conv nets on a GPU: "native" = fl/convnet.py (this repo's kernels), "torch" = autograd over

@@ -35,13 +35,17 @@ r`` once (int8 / int4 rounded with :func:`downlink_key`, or its top-k entries), 
 both sides advance ``r`` by what was sent, bit for bit alike.  Devices train from ``r`` and send their deltas to ``r``; what
 was not delivered yet stays in ``theta - r`` and goes out in later rounds.  Defined in ``ops/csrc/downlink.cuh``;
 ``ops.reference.encode_downlink`` / ``apply_downlink`` transcribe it.
+
+Each format's wire is defined here alone: the request fields (:func:`request_fields`, :func:`echo`), the update fields
+(:data:`FIELDS`), the device's encode (:func:`device_reply`, :func:`encode`), the coordinator's reply check
+(:func:`check_reply`) and its server step over K checked replies (:func:`stack`, :func:`server_apply`).
 """
 from __future__ import annotations
 
 import math
 import zlib
 from dataclasses import dataclass
-from typing import Any, ClassVar, Dict
+from typing import Any, ClassVar, Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -128,6 +132,69 @@ class UplinkCodec:
         return float(x)
 
 
+# ---- the wire of each format ------------------------------------------------------------------------------------------------------
+# the update fields of a reply, in wire order; the compressed downlink sends its wire under the same names with a "d" prefix
+FIELDS = {"fp32": ("params",), "int8": ("payload", "scales"), "int4": ("payload", "scales"), "topk": ("indices", "values")}
+
+
+def echo(codec: UplinkCodec) -> Dict[str, Any]:
+    """The fields that name the format: a fit request carries them and the device's reply echoes them (none for fp32)"""
+    if codec.kind == "fp32":
+        return {}
+    return {"uplink": codec.kind, "topk": codec.k} if codec.sparse else {"uplink": codec.kind}
+
+
+def request_fields(codec: UplinkCodec, ef_reset: bool = False) -> Dict[str, Any]:
+    """The uplink fields of a fit request: :func:`echo`, and for topk whether the device zeroes its residual first"""
+    return {**echo(codec), "ef_reset": bool(ef_reset)} if codec.sparse else echo(codec)
+
+
+def wire_fields(codec: UplinkCodec, wire: Sequence[torch.Tensor], prefix: str = "") -> Dict[str, bytes]:
+    """The wire tensors of one update (or of the downlink, ``prefix`` "d") as the fields of :data:`FIELDS`"""
+    return {prefix + name: t.detach().cpu().contiguous().numpy().tobytes() for name, t in zip(FIELDS[codec.kind], wire)}
+
+
+def encode(codec: UplinkCodec, flats: torch.Tensor, base: Optional[torch.Tensor], keys: Sequence[int],
+           residual: Optional[torch.Tensor] = None):
+    """The wire tensors of K trained models ``flats`` [K, P]: their deltas to ``base`` as ``(payload, scales)`` rounded with
+    ``keys`` (one per row) or as ``(indices, values)`` plus ``residual`` [K, P], which keeps what was not sent; fp32 ``(flats,)``"""
+    from .. import ops
+    if codec.quantized:
+        return ops.encode_delta(flats, base, codec, keys)
+    if codec.sparse:
+        return ops.encode_topk_delta(flats, base, residual, codec)
+    return (flats,)
+
+
+def device_reply(codec: UplinkCodec, flat: torch.Tensor, received: Optional[torch.Tensor], key: int,
+                 residuals: Dict[str, torch.Tensor], model: str, ef_reset: bool) -> Dict[str, Any]:
+    """A device's reply fields for ``flat`` trained from ``received``: :func:`echo` and the update.  topk keeps its residual
+    [1, P] in ``residuals[model]``, zeroed on ``ef_reset`` and whenever the model's size or device changed."""
+    res = None
+    if codec.sparse:
+        res = residuals.get(model)
+        if ef_reset or res is None or res.numel() != flat.numel() or res.device != flat.device:
+            res = residuals[model] = torch.zeros(1, flat.numel(), device=flat.device)
+    return {**echo(codec), **wire_fields(codec, encode(codec, flat.unsqueeze(0), received, [key], res))}
+
+
+def stack(updates: List[Any], codec: UplinkCodec, device) -> List[torch.Tensor]:
+    """K checked replies (:func:`check_reply`) as one [K, ...] tensor per field on ``device``"""
+    rows = [(u,) for u in updates] if codec.kind == "fp32" else updates
+    return [torch.stack(field).to(device) for field in zip(*rows)]
+
+
+def server_apply(theta: torch.Tensor, wire: Sequence[torch.Tensor], w: torch.Tensor, codec: UplinkCodec, **server):
+    """One server step on ``theta`` in place from K updates, ``wire`` (:func:`encode` or :func:`stack`), weighted by ``w``:
+    the fused FedAvg apply of the format; ``server`` are its aggregator and server-optimizer keywords."""
+    from .. import ops
+    if codec.quantized:
+        return ops.fedavg_apply_quantized(theta, *wire, w, codec, **server)
+    if codec.sparse:
+        return ops.fedavg_apply_topk(theta, *wire, w, codec, **server)
+    return ops.fedavg_apply(theta, *wire, w, **server)
+
+
 # ---- checks of untrusted wire bytes: a device's reply on the coordinator, the coordinator's downlink on a device ----------------
 def check_quantized_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
     """``(payload uint8 [codec.payload_bytes(p)], scales fp32 [codec.scale_count(p)])`` of a device's quantized reply, or
@@ -169,3 +236,19 @@ def check_topk_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
     if not bool(torch.isfinite(v).all()):
         raise ValueError("non-finite value returned")
     return torch.from_numpy(idx.astype(np.uint8)), v
+
+
+def check_reply(update: Dict[str, Any], codec: UplinkCodec, p: int):
+    """The checked update of a device's reply in the format ``codec``, or ValueError: :func:`check_quantized_reply`,
+    :func:`check_topk_reply`, or for fp32 the model ``update["params"]`` (as ``RemoteWorkerClient`` decodes it) as a flat
+    fp32 tensor of ``p`` finite parameters: a wrong-length or non-finite model would poison (or abort) the whole average."""
+    if codec.quantized:
+        return check_quantized_reply(update, codec, p)
+    if codec.sparse:
+        return check_topk_reply(update, codec, p)
+    flat = torch.as_tensor(update.get("params"), dtype=torch.float32).reshape(-1)
+    if flat.numel() != p:
+        raise ValueError(f"model of {flat.numel()} parameters returned, expected {p}")
+    if not bool(torch.isfinite(flat).all()):
+        raise ValueError("model with non-finite parameters returned")
+    return flat

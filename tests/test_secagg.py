@@ -533,6 +533,7 @@ def one_device():
     """a worker, a client to it and two in-process peers, through the setup of training "T" """
     from colearn_federated_learning_b200.control.workers import RemoteWorkerClient
     from colearn_federated_learning_b200.fl.trainer import FitConfig
+    from colearn_federated_learning_b200.fl.uplink import UplinkCodec
     from colearn_federated_learning_b200.models import FFNN, flatten_params
 
     w = _worker(1)
@@ -549,7 +550,7 @@ def one_device():
     f = sa.frac_bits(0.5, 3)
 
     def fit(t, u1, frac=f):
-        return client.fit_secagg(theta, cfg, {"tag": "T", "t": t, "u1": u1, "clip": 0.5, "frac_bits": frac})
+        return client.fit_update(theta, cfg, UplinkCodec(), secagg={"tag": "T", "t": t, "u1": u1, "clip": 0.5, "frac_bits": frac})
     yield client, ids, fit, w
     client.close()
     w.stop()

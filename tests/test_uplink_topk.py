@@ -437,7 +437,7 @@ def test_worker_residual_lifetime():
         cfg = FitConfig(model="ffnn", loss="bce", batch_size=16, epochs=1, max_nr_batches=5, lr=0.1, shuffle=True, seed=1)
 
         def fit(reset):
-            update, _, _ = client.fit_topk(theta, cfg, codec, ef_reset=reset)
+            update, _, _ = client.fit_update(theta, cfg, codec, ef_reset=reset)
             from colearn_federated_learning_b200.control.coordinator import check_topk_reply
             idx, val = check_topk_reply(update, codec, theta.numel())
             sent = reference.decode_topk_delta(idx.view(1, -1), val.view(1, -1), 4, theta.numel())
