@@ -33,13 +33,13 @@ from .. import ops, settings
 from ..data import federate, synthetic_for_model, BaseDataset
 from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
-from ..fl import anomaly, asyncagg, fedeval, uplink
+from ..fl import anomaly, asyncagg, category, fedeval, uplink
 from ..fl.evaluate import evaluate
 from ..fl.secagg import check_masked_reply, check_unmask_reply, correction_streams, frac_bits, pk_from_bytes, pk_to_bytes
 from ..fl.server_opt import server_opt_state
 # the reply checks live next to the codec (the workers run them on the downlink wire too) and are exported from here as before
 from ..fl.uplink import UplinkCodec, check_quantized_reply, check_topk_reply, downlink_key, uplink_key  # noqa: F401
-from ..models import MLPNet, build_model, flatten_params, unflatten_params
+from ..models import MODEL_REGISTRY, MLPNet, build_model, flatten_params, unflatten_params
 from ..utils.checkpoint import DEFAULT_PATH, checkpoint_compatible, load_or_init, save_model
 from ..utils.metrics import RoundLogger
 from .arguments import Arguments, ROUND_MODE_BATCHES
@@ -269,7 +269,10 @@ class Coordinator(BusClient):
             x, y = synthetic_for_model(self.args.model, self.args.synthetic, seed=self.args.seed)
             return BaseDataset(x, y)
         from ..data import load_dataset
-        return load_dataset(getattr(self.args, "dataset", "unsw"), self.args.test_path)
+        ds = load_dataset(getattr(self.args, "dataset", "unsw"), self.args.test_path)
+        if category.is_category(MODEL_REGISTRY.get(self.args.model)):
+            return BaseDataset(*category.labels(ds))     # the rows' attack categories are the labels
+        return ds
 
     def _fit_config(self, mode: str) -> FitConfig:
         loss = self.args.loss
@@ -372,14 +375,15 @@ class Coordinator(BusClient):
                         dict(zip(fed.workers, anomaly.summarize(model, theta, ex, ey, self.args.eval_bins, sizes))), self.args.alarm_fpr,
                         self.args.eval_bins)
                 else:
-                    rec["fed_eval"] = result["fed_eval"] = fedeval.record(
+                    make = category.record if category.is_category(model) else fedeval.record
+                    rec["fed_eval"] = result["fed_eval"] = make(
                         dict(zip(fed.workers, fedeval.summarize(model, theta, ex, ey, self.args.eval_bins, self.args.eval_threshold, sizes))))
             self.metrics.end_round(r, time.time() - t0, selected=fed.workers, n_k=counts, loss_k=losses, **rec)
-            self._maybe_checkpoint(model, theta, r, {"workers": fed.workers, "mode": "local", **self._anomaly_meta(model, result)})
+            self._maybe_checkpoint(model, theta, r, {"workers": fed.workers, "mode": "local", **self._model_meta(model, result)})
         log.info("End training")
         unflatten_params(model, theta)
         save_model(model.cpu(), self.path, meta={"model": self.args.model, "rounds": self.enabled_round, "workers": fed.workers, "mode": "local",
-                                                 **self._anomaly_meta(model, result)})
+                                                 **self._model_meta(model, result)})
         self._deregister(to_train.keys())
         self.metrics.end_training()
         self.trainings_done += 1
@@ -387,9 +391,12 @@ class Coordinator(BusClient):
         return result
 
     @staticmethod
-    def _anomaly_meta(model, result: Dict[str, Any]) -> Dict[str, Any]:
-        """An autoencoder's checkpoint sidecar carries the alarm threshold of its last federated evaluation"""
-        return {"anomaly": anomaly.checkpoint_meta(result.get("fed_eval"))} if anomaly.is_autoencoder(model) else {}
+    def _model_meta(model, result: Dict[str, Any]) -> Dict[str, Any]:
+        """An autoencoder's checkpoint sidecar carries the alarm threshold of its last federated evaluation, a category
+        model's the names of its classes"""
+        if anomaly.is_autoencoder(model):
+            return {"anomaly": anomaly.checkpoint_meta(result.get("fed_eval"))}
+        return {"classes": list(category.CATEGORIES)} if category.is_category(model) else {}
 
     def _fed_eval_round(self, r: int) -> bool:
         """``--fed-eval-every N``: the global model is evaluated after every N-th round and after the last one"""
@@ -472,7 +479,7 @@ class Coordinator(BusClient):
             self._deregister(to_train.keys())
         unflatten_params(model, theta)
         save_model(model, self.path, meta={"model": self.args.model, "rounds": self.enabled_round, "workers": list(to_train.keys()), "mode": "remote",
-                                           **self._anomaly_meta(model, result)})
+                                           **self._model_meta(model, result)})
         eval_loss = None
         if self.evaluate_after:
             ds = self._dataset()
@@ -577,7 +584,7 @@ class Coordinator(BusClient):
                                    **agg_rec)
             result["bytes_out"] = result.get("bytes_out", 0) + bytes_out
             result["bytes_in"] = result.get("bytes_in", 0) + bytes_in
-            self._maybe_checkpoint(model, theta, r, {"workers": list(to_train.keys()), "mode": "remote", **self._anomaly_meta(model, result)})
+            self._maybe_checkpoint(model, theta, r, {"workers": list(to_train.keys()), "mode": "remote", **self._model_meta(model, result)})
             if not alive:
                 break
         return theta
@@ -659,7 +666,7 @@ class Coordinator(BusClient):
                 result["bytes_in"] = result.get("bytes_in", 0) + rec["bytes_in"]
                 sent0 = sent
                 self.metrics.end_round(steps, time.time() - t0, **rec)
-                self._maybe_checkpoint(model, current, steps, {"workers": list(to_train.keys()), "mode": "remote", **self._anomaly_meta(model, result)})
+                self._maybe_checkpoint(model, current, steps, {"workers": list(to_train.keys()), "mode": "remote", **self._model_meta(model, result)})
                 steps += 1
                 t0 = time.time()
         # after the last step: nothing new is dispatched; what is still in flight is awaited, then discarded with the buffer
@@ -718,6 +725,8 @@ class Coordinator(BusClient):
         excluded, missing = [wid for wid, a in answers if a == "excluded"], [wid for wid, a in answers if a == "missing"]
         if ae:
             return anomaly.record(good, self.args.alarm_fpr, bins, excluded=excluded, missing=missing)
+        if category.is_category(MODEL_REGISTRY.get(self.args.model)):
+            return category.record(good, excluded=excluded, missing=missing)
         return fedeval.record(good, excluded=excluded, missing=missing)
 
     async def _secagg_setup(self, alive, tag: str, loop, pool, result) -> Optional[Dict[str, Any]]:
@@ -859,6 +868,8 @@ class Coordinator(BusClient):
                 pred = worker.predict(flat, self.args.model, alarm=alarm)
                 self.last_predictions = pred
                 log.info(pred)
+                if category.is_category(model):
+                    log.info("attack categories: %s", [category.CATEGORIES[i] if 0 <= i < len(category.CATEGORIES) else i for i in pred])
             else:
                 log.info("Inference data not found!")
         finally:

@@ -29,7 +29,7 @@ import numpy as np
 import torch
 
 from ..data import dataset_tensors
-from ..fl import anomaly, fedeval
+from ..fl import anomaly, category, fedeval
 from ..fl.trainer import FitConfig, local_fit
 from ..fl.evaluate import predict as predict_fn
 from ..fl.secagg import SecAggDevice
@@ -127,6 +127,8 @@ class WorkerServer:
         self.device = device or torch.device("cuda" if torch.cuda.is_available() else "cpu")
         self.verbose = verbose
         self.datasets: Dict[str, Tuple[torch.Tensor, torch.Tensor]] = {}
+        # attack-category class indices [N, 1] of a hosted dataset that has them (fl/category.py), under the same key
+        self.categories: Dict[str, torch.Tensor] = {}
         self.tagged: Dict[str, List[torch.Tensor]] = {}
         self.fits_served = 0
         self._round = 0
@@ -184,6 +186,30 @@ class WorkerServer:
     # -- data hosting (rw.py:97-108) -------------------------------------------------------
     def add_dataset(self, dataset, key: str = "training") -> None:
         self.datasets[key] = dataset_tensors(dataset, self.device)
+        self.categories.pop(key, None)
+        if getattr(dataset, "categories", None) is not None:
+            self.categories[key] = category.labels(dataset, self.device)[1]
+
+    def hold_out_evaluation(self, fraction: float, seed: int) -> None:
+        """Move a seeded ``fraction`` of the training rows to the evaluation set (``fedeval.split_eval``), their attack
+        categories with them when the training data has some"""
+        x, y = self.datasets["training"]
+        xt, yt, xe, ye = fedeval.split_eval(x, y, fraction, seed)
+        self.datasets["training"], self.datasets["evaluation"] = (xt, yt), (xe, ye)
+        self.categories.pop("evaluation", None)
+        if "training" in self.categories:           # the same rows: the split depends on n and the seed only
+            _, ct, _, ce = fedeval.split_eval(x, self.categories["training"], fraction, seed)
+            self.categories["training"], self.categories["evaluation"] = ct, ce
+
+    def _labels(self, model, key: str, y: torch.Tensor) -> Tuple[Optional[torch.Tensor], Optional[str]]:
+        """``(labels, None)`` the model trains and is scored on: the attack categories for a category model, ``y`` otherwise;
+        ``(None, reason)`` when this device's ``key`` data has no categories"""
+        if not category.is_category(model):
+            return y, None
+        codes = self.categories.get(key)
+        if codes is None:
+            return None, f"{model.__class__.__name__} trains on attack categories: this device's {key} data has none"
+        return codes, None
 
     def load_data(self, tensors: List[torch.Tensor], tag: str = "inference") -> None:
         self.tagged.setdefault(tag, []).extend(t.to(self.device) for t in tensors)
@@ -232,7 +258,10 @@ class WorkerServer:
                         return {"ok": False, "error": f"evaluation data has {held[0].shape[1]} features, {req.get('model')} wants {spec.dims[0]}"}
                     if anomaly.is_autoencoder(model):
                         return {"ok": True, **anomaly.to_wire(anomaly.summarize(model, flat, held[0], held[1], int(req.get("bins", 256)))[0])}
-                    s = fedeval.summarize(model, flat, held[0], held[1], int(req.get("bins", 256)), float(req.get("threshold", 0.5)))[0]
+                    ey, why = self._labels(model, "evaluation", held[1])
+                    if why:
+                        return {"ok": False, "error": f"evaluation refused: {why}"}
+                    s = fedeval.summarize(model, flat, held[0], ey, int(req.get("bins", 256)), float(req.get("threshold", 0.5)))[0]
                 except (ValueError, TypeError) as e:
                     return {"ok": False, "error": f"evaluation refused: {e}"}
                 return {"ok": True, **fedeval.to_wire(s)}
@@ -265,7 +294,8 @@ class WorkerServer:
         """A fit request: its refusals, the model it trains (the fp32 ``params`` or the downlink replica), the fit and the
         reply with the update in the format the request asks for.  A refused request trains nothing and is not counted."""
         cfg = FitConfig.from_dict(req["config"])
-        x, y = self.datasets[req.get("dataset_key", "training")]
+        key = req.get("dataset_key", "training")
+        x, y = self.datasets[key]
         # "uplink": send the quantized or top-k delta instead of the model (fl/uplink.py); absent = the fp32 model.
         # topk carries "topk" (k in 1..32, anything else is refused before the fit) and "ef_reset" (zero the residual)
         codec = _codec(req.get("uplink", "fp32"), req.get("topk"))
@@ -286,6 +316,9 @@ class WorkerServer:
                 return {"ok": False, "error": f"dataset has {x.shape[1]} features, {cfg.model} wants {spec.dims[0]}"}
             if anomaly.is_autoencoder(model):
                 x, y = anomaly.training_rows(x, y)       # the benign rows, the input as the target; n = their count
+            y, why = self._labels(model, key, y)
+            if why:
+                return {"ok": False, "error": why}
             if sa is not None:
                 if any(b.is_floating_point() for b in model.buffers()):
                     return {"ok": False, "error": f"secure aggregation refused: {cfg.model}'s floating-point buffers would travel in the clear"}

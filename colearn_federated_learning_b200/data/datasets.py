@@ -21,6 +21,9 @@ from torch.utils.data import Dataset
 FEATURE_COLUMNS = ["seq", "stddev", "N_IN_Conn_P_SrcIP", "min", "state_number", "mean",
                    "N_IN_Conn_P_DstIP", "drate", "srate", "max"]
 LABEL_COLUMN = "attack"
+CATEGORY_COLUMN = "category"
+# The attack categories of Bot-IoT, in class-index order.  Index 0 is Normal, so "any attack" is class != 0.
+CATEGORIES = ("Normal", "DDoS", "DoS", "Reconnaissance", "Theft")
 CSV_HEADER = ["pkSeqID", "proto", "saddr", "sport", "daddr", "dport", "seq", "stddev",
               "N_IN_Conn_P_SrcIP", "min", "state_number", "mean", "N_IN_Conn_P_DstIP", "drate",
               "srate", "max", "attack", "category", "subcategory"]
@@ -77,6 +80,8 @@ class NetworkTrafficDataset(Dataset):
         self.data = minmax_scale(self.df.values[:, 1:])
         self.targets = self.df.iloc[:, 0]
         self.transform = transform
+        # class index (CATEGORIES) of every row, None for a CSV without the column
+        self.categories = _category_codes(df, csv_file) if CATEGORY_COLUMN in df.columns else None
 
     def __len__(self) -> int:
         return len(self.df)
@@ -99,6 +104,37 @@ class NetworkTrafficDataset(Dataset):
         return x, y
 
 
+def _category_codes(df, csv_file: str) -> np.ndarray:
+    """int64 [N] class indices of the ``category`` column.  ValueError naming the CSV line (header = line 1) and the value
+    for a category outside CATEGORIES, or for a row whose ``attack`` disagrees with it (attack == 0 exactly when Normal)."""
+    index = {name: i for i, name in enumerate(CATEGORIES)}
+    names = df[CATEGORY_COLUMN].astype(str).str.strip()
+    codes = names.map(index)
+    bad = codes.isna().to_numpy()
+    if bad.any():
+        i = int(np.flatnonzero(bad)[0])
+        raise ValueError(f"{csv_file}:{i + 2}: category {df[CATEGORY_COLUMN].iloc[i]!r} is not one of {', '.join(CATEGORIES)}")
+    codes = codes.to_numpy(dtype=np.int64)
+    attack = df[LABEL_COLUMN].to_numpy()
+    bad = (attack == 0) != (codes == 0)
+    if bad.any():
+        i = int(np.flatnonzero(bad)[0])
+        raise ValueError(f"{csv_file}:{i + 2}: attack {attack[i].item()!r} disagrees with category {names.iloc[i]!r} "
+                         "(attack is 0 exactly for Normal rows)")
+    return codes
+
+
+def category_tensors(ds, device: Optional[torch.device] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``(X[N, F], class index[N, 1] float)`` of a dataset that carries attack categories (``ds.categories``).  ValueError for
+    one that does not (a CSV without the column, a plugin dataset, the XOR toy)."""
+    codes = getattr(ds, "categories", None)
+    if codes is None:
+        raise ValueError(f"the {type(ds).__name__} has no attack categories (a '{CATEGORY_COLUMN}' column)")
+    x = dataset_tensors(ds, device)[0]
+    y = torch.from_numpy(np.array(codes, dtype=np.float32)).view(-1, 1).to(x.device)
+    return x, y
+
+
 class BaseDataset(Dataset):
     """In-memory ``(data, targets)`` dataset (the PySyft ``sy.BaseDataset`` used at rw.py:80)."""
 
@@ -119,6 +155,16 @@ class BaseDataset(Dataset):
         if device is not None:
             x, y = x.to(device), y.to(device)
         return x, y
+
+
+def category_dataset(x: torch.Tensor, codes: torch.Tensor) -> BaseDataset:
+    """Rows whose attack categories are known (class indices into CATEGORIES, e.g. ``synthetic_category``'s labels) as a
+    dataset shaped like the CSV adapter's: the binary ``attack`` label (category != Normal) as targets, the class indices as
+    ``categories``"""
+    codes = codes.reshape(-1).long()
+    ds = BaseDataset(x, (codes != 0).float().view(-1, 1))
+    ds.categories = codes.cpu().numpy()
+    return ds
 
 
 def xor_toy_dataset() -> BaseDataset:

@@ -13,7 +13,7 @@ from typing import Optional, Tuple
 import numpy as np
 import torch
 
-from .datasets import CSV_HEADER, FEATURE_COLUMNS
+from .datasets import CATEGORIES, CSV_HEADER, FEATURE_COLUMNS
 
 
 def synthetic_unsw(n: int, seed: int = 0, n_features: int = 10, noise: float = 0.05,
@@ -53,6 +53,23 @@ def synthetic_anomaly(n: int, seed: int = 0, attack_fraction: float = 0.1,
     return x, y
 
 
+def synthetic_category(n: int, seed: int = 0, device: Optional[torch.device] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Traffic for the attack classifier (``--model ffnn_category``): ``(X[n, 10] in [0, 1], y[n, 1])`` with ``y`` the class
+    index into CATEGORIES, deterministic in ``seed``.  Each class is a Gaussian blob (sd 0.08) around its own fixed centre in
+    [0.2, 0.8]^10 (the same for every seed), clipped to [0, 1]; the classes are drawn with probabilities 40 / 20 / 20 / 10 / 10 %,
+    so Normal is the majority class at 40 %."""
+    fixed = torch.Generator().manual_seed(20181105)
+    centres = 0.2 + 0.6 * torch.rand(len(CATEGORIES), 10, generator=fixed)
+    g = torch.Generator().manual_seed(seed)
+    probs = torch.tensor([0.4, 0.2, 0.2, 0.1, 0.1])
+    y = torch.multinomial(probs, n, replacement=True, generator=g) if n > 0 else torch.zeros(0, dtype=torch.long)
+    x = (centres[y] + 0.08 * torch.randn(n, 10, generator=g)).clamp(0.0, 1.0)
+    y = y.float().view(n, 1)
+    if device is not None:
+        x, y = x.to(device), y.to(device)
+    return x, y
+
+
 def synthetic_images(n: int, seed: int = 0, size: int = 32, classes: int = 10,
                      device: Optional[torch.device] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Synthetic ``[n,3,size,size]`` images with class-dependent mean (BASELINE config 4)."""
@@ -69,8 +86,8 @@ def synthetic_for_model(model: str, n: int, seed: int = 0,
                         device: Optional[torch.device] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Synthetic data of the shape ``model`` consumes (``--synthetic N`` on the CLIs): 32x32 images with 10 classes
     for ``resnet18``, 28x28 single-channel digits-shaped inputs for ``net`` (784-128-64-10), two XOR-like features
-    for ``testing_remote``, benign rows on a manifold with 10 % attacks off it for ``autoencoder``, the ten UNSW-IoT features
-    otherwise.  Labels are ``[n, 1]`` floats (class index for the
+    for ``testing_remote``, benign rows on a manifold with 10 % attacks off it for ``autoencoder``, five attack categories for
+    ``ffnn_category``, the ten UNSW-IoT features otherwise.  Labels are ``[n, 1]`` floats (class index for the
     cross-entropy models), which is what every fit executor accepts."""
     if model == "resnet18":
         x, y = synthetic_images(n, seed=seed)
@@ -82,6 +99,8 @@ def synthetic_for_model(model: str, n: int, seed: int = 0,
         x, y = synthetic_unsw(n, seed=seed, n_features=2)
     elif model == "autoencoder":
         x, y = synthetic_anomaly(n, seed=seed)
+    elif model == "ffnn_category":
+        x, y = synthetic_category(n, seed=seed)
     else:
         x, y = synthetic_unsw(n, seed=seed)
     if device is not None:

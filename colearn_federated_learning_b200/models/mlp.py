@@ -27,7 +27,8 @@ class MLPSpec:
     out_activation: str = "none"   # none | sigmoid
     default_loss: str = "xent"     # bce | sse | xent | mse
     flatten_input: bool = False
-    target: str = "label"          # label: trained on the dataset's labels; input: trained to reconstruct its input (fl/anomaly.py)
+    target: str = "label"          # label: trained on the dataset's labels; input: trained to reconstruct its input (fl/anomaly.py);
+                                   # category: trained on the attack category of every row (data.CATEGORIES, fl/category.py)
 
     @property
     def n_layers(self) -> int:
@@ -87,6 +88,7 @@ NET_SPEC = MLPSpec((784, 128, 64, 10), "none", "xent", flatten_input=True)
 MLP_SPEC = MLPSpec((10, 64, 64, 2), "none", "xent")
 WIDE_MLP_SPEC = MLPSpec((10, 4096, 4096, 4096, 4096, 2), "none", "xent")
 AE_SPEC = MLPSpec((10, 32, 4, 32, 10), "none", "mse", target="input")
+FFNN_CAT_SPEC = MLPSpec((10, 50, 30, 10, 5), "none", "xent", target="category")
 
 
 class FFNN(MLPNet):
@@ -127,6 +129,16 @@ class Autoencoder(MLPNet):
 
     def __init__(self) -> None:
         super().__init__(AE_SPEC)
+
+
+class FFNNCategory(MLPNet):
+    """Attack classifier: the FFNN's 10-50-30-10 body with a 5-way head (2 445 params), trained with softmax cross-entropy on
+    the ``category`` column (Normal, DDoS, DoS, Reconnaissance, Theft; data.CATEGORIES)."""
+
+    spec = FFNN_CAT_SPEC            # on the class too: the CLI tells a category model from its registry entry without building it
+
+    def __init__(self) -> None:
+        super().__init__(FFNN_CAT_SPEC)
 
 
 class WideMLP(MLPNet):

@@ -13,7 +13,7 @@ from typing import Callable, Dict, List, Optional, Tuple
 import torch
 import torch.nn as nn
 
-from .mlp import FFNN, MLP, Autoencoder, MLPNet, MLPSpec, Net, TestingRemote, WideMLP
+from .mlp import FFNN, MLP, Autoencoder, FFNNCategory, MLPNet, MLPSpec, Net, TestingRemote, WideMLP
 from .resnet import ResNet18
 
 MODEL_REGISTRY: Dict[str, Callable[[], nn.Module]] = {
@@ -24,10 +24,12 @@ MODEL_REGISTRY: Dict[str, Callable[[], nn.Module]] = {
     "wide_mlp": WideMLP,
     "resnet18": ResNet18,
     "autoencoder": Autoencoder,
+    "ffnn_category": FFNNCategory,
 }
 
 DEFAULT_LOSS = {"ffnn": "bce", "testing_remote": "sse", "net": "xent", "mlp": "xent",
-                "wide_mlp": "xent", "resnet18": "xent", "autoencoder": "mse"}
+                "wide_mlp": "xent", "resnet18": "xent", "autoencoder": "mse",
+                "ffnn_category": "xent"}
 
 
 def register_model(name: str, factory: Callable[..., nn.Module], default_loss: str = "xent", overwrite: bool = False) -> None:

@@ -24,7 +24,7 @@ EMUL_NAME = "_colearn_emul"     # CPU emulator of the conv kernels (tests on box
 HOST_NAME = "_colearn_host"     # native CPU executor of the MLP local fit (devices / boxes without a GPU)
 SIMT_NAME = "_colearn_simt"     # the persistent-MLP CUDA kernels compiled for the CPU through csrc/host_shim.h (tests)
 
-CU_SOURCES = ["mlp_persistent.cu", "mlp_persistent_ae.cu", "elementwise.cu", "comm.cu", "gemm_wgmma.cu", "convnet.cu"]
+CU_SOURCES = ["mlp_persistent.cu", "mlp_persistent_ae.cu", "mlp_persistent_cat.cu", "elementwise.cu", "comm.cu", "gemm_wgmma.cu", "convnet.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo",
@@ -144,9 +144,9 @@ def build_simt_emul(force: bool = False) -> str:
     src = os.path.join(CSRC, "simt_emul.cpp")
     cxx_flags = [f for f in flags if f not in ("-O2", "-std=c++17")] + ["-O1", "-std=c++20", "-pthread", "-Wno-unknown-pragmas",
                                                                         f"-DTORCH_EXTENSION_NAME={SIMT_NAME}"]
-    sources = ["simt_emul.cpp", "simt_mlp.cpp", "simt_mlp_ae.cpp", "simt_elementwise.cpp", "simt_comm.cpp", "simt_convnet.cpp", "simt_gemm.cpp"]
+    sources = ["simt_emul.cpp", "simt_mlp.cpp", "simt_mlp_ae.cpp", "simt_mlp_cat.cpp", "simt_elementwise.cpp", "simt_comm.cpp", "simt_convnet.cpp", "simt_gemm.cpp"]
     h = hashlib.sha1()
-    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_persistent_ae.cu", "mlp_v2.cuh", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "conv_ops.cuh"]:
+    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_persistent_ae.cu", "mlp_persistent_cat.cu", "mlp_v2.cuh", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "conv_ops.cuh"]:
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(cxx_flags).encode())

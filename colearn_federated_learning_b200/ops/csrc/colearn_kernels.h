@@ -135,6 +135,7 @@ cudaError_t set_spin_limit_comm(unsigned long long ns);
 cudaError_t preload_comm_kernels();   // force the lazy loader for every kernel of comm.cu (see there)
 cudaError_t set_spin_limit_mlp(unsigned long long ns);
 cudaError_t set_spin_limit_mlp_ae(unsigned long long ns);   // mlp_persistent_ae.cu: its own copy of the limit
+cudaError_t set_spin_limit_mlp_cat(unsigned long long ns);  // mlp_persistent_cat.cu: likewise
 cudaError_t set_spin_limit_gemm(unsigned long long ns);
 
 // ---------------------------------------------------------------------------------------------
@@ -182,7 +183,7 @@ COLEARN_HD uint32_t feistel_index(uint32_t v, uint32_t n, FeistelDomain dom, uin
 // Persistent whole-network local SGD (mlp_persistent.cu)
 // ---------------------------------------------------------------------------------------------
 enum LossKind : int { LOSS_BCE = 0, LOSS_SSE = 1, LOSS_XENT = 2, LOSS_MSE = 3 };
-enum NetKind : int { NET_FFNN = 0, NET_MLP64 = 1, NET_TESTING_REMOTE = 2, NET_AE = 3 };
+enum NetKind : int { NET_FFNN = 0, NET_MLP64 = 1, NET_TESTING_REMOTE = 2, NET_AE = 3, NET_FFNN_CAT = 4 };
 
 // One descriptor per client (= one CTA).  A "client" is a federated worker: it starts from
 // theta_in, runs its local SGD over its private shard and emits out_scale * theta_k (or the

@@ -508,6 +508,9 @@ using TestingRemoteNet = Net<false, 2, 50, 10, 1>;
 // autoencoder of the anomaly detector (models/mlp.py AE_SPEC): trained to reconstruct its input, MSE head.  Its instances
 // are compiled in mlp_persistent_ae.cu, not here (see there).
 using AENet = Net<false, 10, 32, 4, 32, 10>;
+// attack-category classifier (models/mlp.py FFNN_CAT_SPEC): the FFNN's body with a 5-way linear head and softmax
+// cross-entropy.  Its instances are compiled in mlp_persistent_cat.cu, for the reason mlp_persistent_ae.cu gives.
+using CatNet = Net<false, 10, 50, 30, 10, 5>;
 
 template <class N>
 int smem_bytes(int batch_size) {
@@ -557,10 +560,16 @@ cudaError_t launch_mlp_local_sgd_ae(const ClientDesc* descs, int n_clients, SgdH
 int mlp_local_sgd_smem_bytes_ae(int batch_size);
 int mlp_net_num_params_ae();
 cudaError_t launch_mlp_forward_ae(const float* theta, const float* x, float* out, int n, cudaStream_t stream);
+// the attack-category FFNN's instances (mlp_persistent_cat.cu): variants 1, 3, 5 and 6, the batched forward
+cudaError_t launch_mlp_local_sgd_cat(const ClientDesc* descs, int n_clients, SgdHyper hp, cudaStream_t stream);
+int mlp_local_sgd_smem_bytes_cat(int batch_size);
+int mlp_net_num_params_cat();
+cudaError_t launch_mlp_forward_cat(const float* theta, const float* x, float* out, int n, cudaStream_t stream);
 
 cudaError_t launch_mlp_local_sgd(int net_kind, const ClientDesc* descs, int n_clients, SgdHyper hp,
                                  cudaStream_t stream) {
   if (net_kind == NET_AE) return launch_mlp_local_sgd_ae(descs, n_clients, hp, stream);
+  if (net_kind == NET_FFNN_CAT) return launch_mlp_local_sgd_cat(descs, n_clients, hp, stream);
   // variant 5 (default, set by ops/fused_mlp.py): register-resident weights, 128-thread CTA, blocked reduction slices
   // (LDS.128) + pre-scaled dz; 6: the same with its FMAs written in pairs; 3: the same kernel with strided slices;
   // 1: first version with smem-resident weights.
@@ -603,6 +612,7 @@ int mlp_local_sgd_smem_bytes(int net_kind, int batch_size) {
     case NET_MLP64: return smem_bytes<MLP64Net>(batch_size);
     case NET_TESTING_REMOTE: return smem_bytes<TestingRemoteNet>(batch_size);
     case NET_AE: return mlp_local_sgd_smem_bytes_ae(batch_size);
+    case NET_FFNN_CAT: return mlp_local_sgd_smem_bytes_cat(batch_size);
     default: return -1;
   }
 }
@@ -613,6 +623,7 @@ int mlp_net_num_params(int net_kind) {
     case NET_MLP64: return Totals<MLP64Net>::flat_params;
     case NET_TESTING_REMOTE: return Totals<TestingRemoteNet>::flat_params;
     case NET_AE: return mlp_net_num_params_ae();
+    case NET_FFNN_CAT: return mlp_net_num_params_cat();
     default: return -1;
   }
 }
@@ -624,6 +635,7 @@ cudaError_t launch_mlp_forward(int net_kind, const float* theta, const float* x,
     case NET_MLP64: return forward_t<MLP64Net>(theta, x, out, n, stream);
     case NET_TESTING_REMOTE: return forward_t<TestingRemoteNet>(theta, x, out, n, stream);
     case NET_AE: return launch_mlp_forward_ae(theta, x, out, n, stream);
+    case NET_FFNN_CAT: return launch_mlp_forward_cat(theta, x, out, n, stream);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -59,15 +59,28 @@ __host__ __device__ constexpr int gsize(int n_out, int k_in) {
 }
 __host__ __device__ constexpr int align4(int x) { return (x + 3) / 4 * 4; }
 
+// Widest head that every warp replicates and fuses with its loss (HeadCfg::kFused, RL::REP).  The batch-1 instances hold such
+// a head whole in every lane (HeadCfg::ht): DOUT x K weights, K inputs and DOUT biases, plus DOUT logits, exponentials and dz_L
+// around the softmax, next to the row and column slices of the body.  On the FFNN body (10-50-30-10-C) ptxas fits every
+// instance into its 255 registers without a spill up to C = 7; at C = 8 the batch-1 instances of variants 3, 5 and 6 spill.
+// Hence 7: it covers the 5 attack categories with room, and the autoencoder's 10-wide head stays on the block-wide path.
+constexpr int kFusedHeadMax = 7;
+
 // Lanes per neuron of the set "outputs of layer LI" (LI <= L-2).  The SAME group size is used when that set is
 // written (forward / row update of layer LI: T) and when its gradient is produced (dgrad of layer LI+1: TB),
 // so thread (n, t) of layer LI's row copy is also the thread that holds dz for neuron n after the dgrad
 // butterfly — the layer-0 update can take dz from a register instead of shared memory + a barrier.
 template <class N, int LI>
 __host__ __device__ constexpr int pair_group() {
-  int g = pow2_floor(NT2 / N::template dim<LI + 1>());
+  const int no = N::template dim<LI + 1>();
+  int g = pow2_floor(NT2 / no);
   if (g > 8) g = 8;
   while (g > 1 && (g > N::template dim<LI>() || g > N::template dim<LI + 2>())) g /= 2;
+  // In front of a fused softmax head (3 .. kFusedHeadMax classes) the group is capped so that a layer of <= 32 outputs fits
+  // into one warp (RL::REP), as the loop above already does for heads of 1 or 2 outputs.  10-50-30-10-5: 2 lanes per neuron
+  // of the 30 -> 10 layer, and 2 per input of the head's dgrad (one lane each needs 30 more registers for the row slices, and
+  // the accumulating instances spill).
+  if (LI == N::L - 2 && N::DOUT >= 3 && N::DOUT <= kFusedHeadMax && no <= 32 && g * no > 32) g = pow2_floor(32 / no);
   return g;
 }
 template <class N, int LI, bool HEAD = (LI == N::L - 1)>
@@ -95,7 +108,7 @@ struct RL {
   // memory, so the hop to the (per-warp) head needs __syncwarp instead of a block barrier: one of the step's barrier-separated
   // hops less, and no warp waits at a barrier for the one that used to do this layer alone.  The replicas stay identical: every
   // warp applies the same rank-1 update to its copy (same dz from shared memory, same inputs).
-  static constexpr bool REP = (N::DOUT <= 2) && (N::L >= 3) && (LI == N::L - 2) && (NO * T <= 32);
+  static constexpr bool REP = (N::DOUT <= kFusedHeadMax) && (N::L >= 3) && (LI == N::L - 2) && (NO * T <= 32);
   static constexpr int RSTRIDE = (NO + 3) / 4 * 4;        // floats between the warps' output slots
   static __host__ __device__ constexpr int row_thread(int tid) { return REP ? (tid & 31) : tid; }
   // element i of lane t's row slice (reduction index k) / column slice (output index n)
@@ -134,7 +147,7 @@ template <class N> struct HeadCfg {
   template <bool ACC> static constexpr int kh() { return (K + ht<ACC>() - 1) / ht<ACC>(); }
   static constexpr int FW = Offs<N, LI>::flat;
   static constexpr int FB = Offs<N, LI>::flat + DO * K;
-  static constexpr bool kFused = (N::DOUT <= 2) && (N::L >= 2);
+  static constexpr bool kFused = (N::DOUT <= kFusedHeadMax) && (N::L >= 2);
 };
 
 template <class N, int LI, bool ACC>
@@ -433,7 +446,7 @@ __device__ __forceinline__ void apply_grads(AllRegs<N, 0, ACC>& all, float neg_l
 }
 
 
-// ---- replicated head (DOUT <= 2) ----------------------------------------------------------------------
+// ---- replicated head (DOUT <= kFusedHeadMax) ---------------------------------------------------------------------
 // Every warp keeps its own copy of the head layer (HeadCfg::ht lanes per dot product).  After the
 // barrier that publishes a_{L-1}, each warp computes the logits itself (register FMAs + a short butterfly), so
 // every thread knows dz_L in registers: the "head -> loss -> barrier -> dgrad" hop of the step disappears
@@ -490,19 +503,20 @@ __device__ __forceinline__ void head_store(const HeadRegs<N, ACC>& H, const floa
   }
 }
 
-// exp(x) for x <= 0 and 1 / x for x in [1, 2] as single MUFU instructions (ex2.approx.ftz, rcp.approx.ftz: 2 ulp / 1 ulp).  The
-// sigmoid of the head sits on the step's dependent chain: __expf adds a range fix-up around MUFU.EX2, __frcp_rn a Newton step and
-// a slow-path branch around MUFU.RCP — neither can trigger for these arguments.
+// exp(x) for x <= 0 and 1 / x for a normal x > 0 as single MUFU instructions (ex2.approx.ftz, rcp.approx.ftz: 2 ulp / 1 ulp, the
+// latter over every normal argument).  The heads call them on the step's dependent chain with x in [1, 2] (the sigmoid's 1 + e)
+// and in [1, C] (the softmax sum of a C-class head): __expf adds a range fix-up around MUFU.EX2, __frcp_rn a Newton step and a
+// slow-path branch around MUFU.RCP — neither can trigger for these arguments.
 #ifdef COLEARN_HOST_SHIM
 inline float exp_nonpos(float x) { return expf(x); }
-inline float rcp_1to2(float x) { return 1.0f / x; }
+inline float rcp_approx(float x) { return 1.0f / x; }
 #else
 __device__ __forceinline__ float exp_nonpos(float x) {
   float r;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x * 1.4426950408889634f));
   return r;
 }
-__device__ __forceinline__ float rcp_1to2(float x) {
+__device__ __forceinline__ float rcp_approx(float x) {
   float r;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
   return r;
@@ -561,16 +575,36 @@ __device__ __forceinline__ float head_forward_loss(HeadRegs<N, ACC>& H, const fl
   float value = 0.f;
   if (loss == LOSS_XENT) {
     const int label = (int)yrow[0];
-    const float d = (C::DO == 2) ? z[C::DO - 1] - z[0] : 0.f;
-    const float e = exp_nonpos(-fabsf(d));
-    const float r1 = rcp_1to2(1.f + e);
-    const float p1 = d >= 0.f ? r1 : e * r1;
-    dzh[0] = ((1.f - p1) - (label == 0 ? 1.f : 0.f)) * inv_b;
-    if (C::DO == 2) dzh[C::DO - 1] = (p1 - (label == 1 ? 1.f : 0.f)) * inv_b;
-    {  // (every thread, no branch: the value only feeds the loss statistics, so it schedules off the dependent chain, while an
-       //  `if (tid == 0)` made warp 0 run MUFU.LG2 + a reconvergence point in front of the barrier the other warps wait at)
-      const float margin = (label == 0) ? d : -d;
-      value = fmaxf(margin, 0.f) + __logf(1.f + e);
+    if constexpr (C::DO >= 3) {
+      // softmax cross-entropy, in every thread's registers: m = max z, e_c = exp(z_c - m), s = sum e_c in [1, DO],
+      // dz_c = (e_c / s - [c == y]) / B, loss log(s) + m - z_y.  z_y by compare-and-select over the compile-time class
+      // index (a dynamically indexed register array would go to local memory).
+      float m = z[0];
+#pragma unroll
+      for (int c = 1; c < C::DO; ++c) m = fmaxf(m, z[c]);
+      float e[C::DO], s = 0.f, zy = 0.f;
+#pragma unroll
+      for (int c = 0; c < C::DO; ++c) {
+        e[c] = exp_nonpos(z[c] - m);
+        s += e[c];
+        zy = (label == c) ? z[c] : zy;
+      }
+      const float r = rcp_approx(s);   // s in [1, DO]
+#pragma unroll
+      for (int c = 0; c < C::DO; ++c) dzh[c] = (e[c] * r - (label == c ? 1.f : 0.f)) * inv_b;
+      value = (__logf(s) + m) - zy;   // (every thread: see below)
+    } else {
+      const float d = (C::DO == 2) ? z[C::DO - 1] - z[0] : 0.f;
+      const float e = exp_nonpos(-fabsf(d));
+      const float r1 = rcp_approx(1.f + e);
+      const float p1 = d >= 0.f ? r1 : e * r1;
+      dzh[0] = ((1.f - p1) - (label == 0 ? 1.f : 0.f)) * inv_b;
+      if (C::DO == 2) dzh[C::DO - 1] = (p1 - (label == 1 ? 1.f : 0.f)) * inv_b;
+      {  // (every thread, no branch: the value only feeds the loss statistics, so it schedules off the dependent chain, while an
+         //  `if (tid == 0)` made warp 0 run MUFU.LG2 + a reconvergence point in front of the barrier the other warps wait at)
+        const float margin = (label == 0) ? d : -d;
+        value = fmaxf(margin, 0.f) + __logf(1.f + e);
+      }
     }
   } else {
 #pragma unroll
@@ -578,7 +612,7 @@ __device__ __forceinline__ float head_forward_loss(HeadRegs<N, ACC>& H, const fl
       const float y = yrow[c], zz = z[c];
       if (N::kSigmoid) {
         const float e = exp_nonpos(-fabsf(zz));
-        const float r1 = rcp_1to2(1.f + e);
+        const float r1 = rcp_approx(1.f + e);
         const float out = zz >= 0.f ? r1 : e * r1;
         if (loss == LOSS_BCE) {
           dzh[c] = (out - y) * inv_b * (1.f / C::DO);
@@ -633,7 +667,14 @@ __device__ __forceinline__ void head_backward(AllRegs<N, 0, ACC>& all, HeadRegs<
 #pragma unroll
   for (int i = 0; i < R::NC; ++i) {
     const int n = R::nidx(i, t);
-    dzv[i] = (n == 0) ? dzh[0] : ((C::DO == 2 && n == 1) ? dzh[C::DO - 1] : 0.f);
+    if constexpr (C::DO >= 3) {   // dz_n by compare-and-select over the class index (n >= DO: a padding slot, 0)
+      float v = 0.f;
+#pragma unroll
+      for (int c = 0; c < C::DO; ++c) v = (n == c) ? dzh[c] : v;
+      dzv[i] = v;
+    } else {
+      dzv[i] = (n == 0) ? dzh[0] : ((C::DO == 2 && n == 1) ? dzh[C::DO - 1] : 0.f);
+    }
     acc = fmaf(r.wt[i], dzv[i], acc);
   }
 #pragma unroll

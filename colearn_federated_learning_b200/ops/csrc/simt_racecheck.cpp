@@ -33,13 +33,13 @@ int main() {
   using namespace colearn;
   srand(1);
   // ---- persistent MLP: every net x variant, batch 1 and batch 3 (gradient-accumulation path), two clients ----------------
-  const int din[4] = {10, 10, 2, 10}, dout[4] = {1, 2, 1, 10};
-  const int losses[4] = {LOSS_BCE, LOSS_XENT, LOSS_SSE, LOSS_MSE};
-  for (int kind = 0; kind < 4; ++kind)
+  const int din[5] = {10, 10, 2, 10, 10}, dout[5] = {1, 2, 1, 10, 5};
+  const int losses[5] = {LOSS_BCE, LOSS_XENT, LOSS_SSE, LOSS_MSE, LOSS_XENT};
+  for (int kind = 0; kind < 5; ++kind)
     for (int variant : {1, 3, 5, 6})
       for (int batch : {1, 3}) {
         const int P = mlp_net_num_params(kind), n = 7;
-        std::vector<float> theta = randv(P, 0.3f), x = randv((size_t)n * din[kind]), y((size_t)n * (kind == 1 ? 1 : dout[kind]));
+        std::vector<float> theta = randv(P, 0.3f), x = randv((size_t)n * din[kind]), y((size_t)n * (losses[kind] == LOSS_XENT ? 1 : dout[kind]));
         for (auto& v : y) v = (float)(rand() % 2);
         std::vector<float> out0(P), out1(P), loss(4);
         std::vector<ClientDesc> d(2);
@@ -47,7 +47,7 @@ int main() {
           memset(&d[c], 0, sizeof(ClientDesc));
           d[c].x = x.data(); d[c].y = y.data(); d[c].theta_in = theta.data();
           d[c].theta_out = c ? out1.data() : out0.data(); d[c].loss_out = loss.data() + 2 * c;
-          d[c].n = n; d[c].perm_rows = 1; d[c].y_dim = kind == 1 ? 1 : dout[kind]; d[c].out_scale = 0.5f;
+          d[c].n = n; d[c].perm_rows = 1; d[c].y_dim = losses[kind] == LOSS_XENT ? 1 : dout[kind]; d[c].out_scale = 0.5f;
         }
         SgdHyper hp{batch, 2, -1, losses[kind], 0.05f, variant};
         CK(launch_mlp_local_sgd(kind, d.data(), 2, hp, nullptr));

@@ -4,7 +4,8 @@ One launch runs the *entire* local fit of one or many federated clients (one CTA
 reference's per-batch ``zero_grad → forward → loss → backward → step`` loop
 (``client_federated.py:101-120`` locally; PySyft ``_fit`` remotely, SURVEY C27) never returns to
 the host.  Supported architectures are the compile-time instantiations FFNN (10-50-30-10-1,
-sigmoid), MLP (10-64-64-2), TestingRemote (2-50-10-1) and the autoencoder (10-32-4-32-10, MSE on its input); anything else goes through the
+sigmoid), MLP (10-64-64-2), TestingRemote (2-50-10-1), the autoencoder (10-32-4-32-10, MSE on its input) and the attack-category
+FFNN (10-50-30-10-5, softmax cross-entropy); anything else goes through the
 layer-wise trainer (``fl/layerwise.py``).
 """
 from __future__ import annotations
@@ -21,14 +22,16 @@ NET_KINDS = {
     ((10, 64, 64, 2), "none"): 1,
     ((2, 50, 10, 1), "none"): 2,
     ((10, 32, 4, 32, 10), "none"): 3,     # the anomaly detector's autoencoder (models/mlp.py AE_SPEC)
+    ((10, 50, 30, 10, 5), "none"): 4,     # the attack-category FFNN (models/mlp.py FFNN_CAT_SPEC)
 }
+NET_FFNN_CAT = 4
 LOSS_CODES = {"bce": 0, "sse": 1, "xent": 2, "mse": 3}
 # Kernel variants: 5 = register-resident weights, 128-thread CTA, blocked reduction slices (LDS.128) + pre-scaled dz;
 # 6 = 5 with its FMAs written in pairs (Hopper has no packed fp32 FMA: the same FFMA sequence as 5); 3 = strided slices
 # (the round-1 default); 1 = smem-resident weights (first version).
 # 0 (default) picks variant 5 for every net.
 KERNEL_VARIANT = int(__import__("os").environ.get("COLEARN_MLP_VARIANT", "0"))
-BEST_VARIANT = {0: 5, 1: 5, 2: 5, 3: 5}          # net kind (NET_KINDS values) -> variant
+BEST_VARIANT = {0: 5, 1: 5, 2: 5, 3: 5, 4: 5}    # net kind (NET_KINDS values) -> variant
 
 
 def resolve_variant(kind: int, variant: Optional[int] = None) -> int:
@@ -111,7 +114,12 @@ def _prep_xy(x: torch.Tensor, y: torch.Tensor, loss: str) -> Tuple[torch.Tensor,
 def mlp_local_sgd_multi(dims: Sequence[int], out_activation: str, descs: torch.Tensor, n_clients: int,
                         batch_size: int = 1, lr: float = 0.01, epochs: int = 1, max_nr_batches: int = -1,
                         loss: str = "xent", desc_offset: int = 0, variant: Optional[int] = None) -> None:
-    """Launch ``n_clients`` CTAs from a packed descriptor tensor (see :func:`build_client_descs`)."""
+    """Launch ``n_clients`` CTAs from a packed descriptor tensor (see :func:`build_client_descs`).
+
+    The labels behind the descriptors are not checked here (they are device memory the caller packed).  For the
+    attack-category net they must be class indices in [0, 5): the kernel stays memory-safe for any other value (its heads
+    select z_y by compare-and-select or ``label & 31``), but trains on a wrong gradient.  Every data path that feeds this
+    (the CSV adapter, ``synthetic_category``) validates its codes when it loads them; :func:`mlp_local_sgd` checks them."""
     kind = net_kind_for(dims, out_activation)
     if kind is None:
         raise ValueError(f"no persistent-kernel instantiation for dims={tuple(dims)} act={out_activation}")
@@ -129,7 +137,10 @@ def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: t
     """Single-client in-place local SGD on ``flat``; returns the last batch loss (0-dim tensor).
 
     CPU tensors run ``reference.mlp_local_sgd`` (identical semantics); CUDA tensors run the
-    persistent kernel — there is no silent fallback on CUDA."""
+    persistent kernel — there is no silent fallback on CUDA.  The attack-category net refuses, before any launch, a label that
+    is not a class index in [0, 5): the kernel's head selects z_y by that index."""
+    if net_kind_for(dims, out_activation) == NET_FFNN_CAT:
+        check_class_labels(y, int(dims[-1]))
     if not flat.is_cuda:
         # CPU devices: the native host executor (csrc/mlp_host.cpp) when it is built and the arena can be trained in
         # place, else the PyTorch definitions (identical semantics; the executor is tested against them)
@@ -149,6 +160,15 @@ def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: t
     descs = build_client_descs([task], flat.device)
     mlp_local_sgd_multi(dims, out_activation, descs, 1, batch_size, lr, epochs, max_nr_batches, loss, variant=variant)
     return loss_out[1 if return_mean else 0]
+
+
+def check_class_labels(y: torch.Tensor, classes: int) -> None:
+    """ValueError unless every label is an integer class index in [0, classes)"""
+    v = y.detach().reshape(-1).double()
+    bad = ~((v == v.floor()) & (v >= 0) & (v < classes))
+    if bool(bad.any()):
+        i = int(bad.nonzero()[0, 0])
+        raise ValueError(f"label {float(v[i])!r} of row {i} is not a class index in [0, {classes})")
 
 
 def mlp_forward(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, out_activation: str = "none") -> torch.Tensor:

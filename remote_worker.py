@@ -39,7 +39,8 @@ _OPTIONS = (
     (("--broker-port",), dict(type=int, default=1883)),
     (("--synthetic",), dict(type=int, default=0, help="host N synthetic rows instead of --training")),
     (("--data-model",), dict(default="ffnn", help="architecture the synthetic data is shaped for (resnet18: 32x32 images, net: "
-                                                  "28x28, testing_remote: 2 features, otherwise the ten UNSW-IoT features)")),
+                                                  "28x28, testing_remote: 2 features, ffnn_category: five attack categories, "
+                                                  "otherwise the ten UNSW-IoT features)")),
     (("--seed",), dict(type=int, default=0)),
     (("--dataset",), dict(default="unsw", help="dataset adapter that reads -dt / -di (data.register_dataset; default: the Bot-IoT CSV adapter)")),
     (("--plugin",), dict(action="append", default=[], metavar="MODULE_OR_FILE",
@@ -66,11 +67,18 @@ def build_parser() -> argparse.ArgumentParser:
 
 
 def pick_dataset(args):
-    """--synthetic N > the CSV given with -dt > the reference's XOR toy set (rw.py:75-80)."""
-    from colearn_federated_learning_b200.data import BaseDataset, load_dataset, synthetic_for_model, xor_toy_dataset
+    """--synthetic N > the CSV given with -dt > the reference's XOR toy set (rw.py:75-80).  Synthetic rows made for an
+    attack-category model (--data-model ffnn_category) keep their class indices as the dataset's categories, next to the
+    binary attack label, like a Bot-IoT CSV."""
+    from colearn_federated_learning_b200.data import BaseDataset, category_dataset, load_dataset, synthetic_for_model, xor_toy_dataset
+    from colearn_federated_learning_b200.fl import category
+    from colearn_federated_learning_b200.models import MODEL_REGISTRY
 
     if args.synthetic > 0:
-        return BaseDataset(*synthetic_for_model(args.data_model, args.synthetic, seed=args.seed))
+        x, y = synthetic_for_model(args.data_model, args.synthetic, seed=args.seed)
+        if category.is_category(MODEL_REGISTRY.get(args.data_model)):
+            return category_dataset(x, y)
+        return BaseDataset(x, y)
     if args.training:
         logging.info("training data: %s", args.training)
         return load_dataset(args.dataset, args.training)
@@ -102,9 +110,7 @@ def main(args: argparse.Namespace) -> None:  # pragma: no cover - exercised by t
         logging.info("evaluation data: %s", args.evaluation)
         server.add_dataset(load_dataset(args.dataset, args.evaluation), key="evaluation")
     elif args.eval_fraction > 0:
-        from colearn_federated_learning_b200.fl.fedeval import split_eval
-        xt, yt, xe, ye = split_eval(*server.datasets["training"], args.eval_fraction, args.seed)
-        server.datasets["training"], server.datasets["evaluation"] = (xt, yt), (xe, ye)
+        server.hold_out_evaluation(args.eval_fraction, args.seed)
     if args.inference:
         logging.info("inference data: %s", args.inference)
         rows = load_dataset(args.dataset, args.inference).data

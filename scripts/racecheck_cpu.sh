@@ -9,9 +9,9 @@ OUT=${1:-/tmp/colearn_racecheck}
 mkdir -p "$OUT"
 CUDA_INC=${CUDA_HOME:-/usr/local/cuda}/include
 FLAGS="-std=c++20 -O1 -g -fsanitize=thread -pthread -Wno-unknown-pragmas -Wno-tsan -DCOLEARN_HOST_SHIM=1 -I$CSRC -I$CUDA_INC"
-for f in simt_mlp simt_mlp_ae simt_elementwise simt_comm simt_convnet simt_gemm simt_racecheck; do
+for f in simt_mlp simt_mlp_ae simt_mlp_cat simt_elementwise simt_comm simt_convnet simt_gemm simt_racecheck; do
   g++ $FLAGS -c "$CSRC/$f.cpp" -o "$OUT/$f.o" &
 done
 wait
-g++ -fsanitize=thread -pthread "$OUT"/simt_mlp.o "$OUT"/simt_mlp_ae.o "$OUT"/simt_elementwise.o "$OUT"/simt_comm.o "$OUT"/simt_convnet.o "$OUT"/simt_gemm.o "$OUT"/simt_racecheck.o -o "$OUT/racecheck"
+g++ -fsanitize=thread -pthread "$OUT"/simt_mlp.o "$OUT"/simt_mlp_ae.o "$OUT"/simt_mlp_cat.o "$OUT"/simt_elementwise.o "$OUT"/simt_comm.o "$OUT"/simt_convnet.o "$OUT"/simt_gemm.o "$OUT"/simt_racecheck.o -o "$OUT/racecheck"
 TSAN_OPTIONS="halt_on_error=0 exitcode=66 second_deadlock_stack=1" "$OUT/racecheck"
