@@ -30,16 +30,16 @@ import numpy as np
 import torch
 
 from .. import ops, settings
-from ..data import federate, synthetic_for_model, BaseDataset
+from ..data import federate
 from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
-from ..fl import anomaly, asyncagg, category, fedeval, uplink
+from ..fl import asyncagg, fedeval, targets, uplink
 from ..fl.evaluate import evaluate
 from ..fl.secagg import check_masked_reply, check_unmask_reply, correction_streams, frac_bits, pk_from_bytes, pk_to_bytes
 from ..fl.server_opt import server_opt_state
 # the reply checks live next to the codec (the workers run them on the downlink wire too) and are exported from here as before
 from ..fl.uplink import UplinkCodec, check_quantized_reply, check_topk_reply, downlink_key, uplink_key  # noqa: F401
-from ..models import MODEL_REGISTRY, MLPNet, build_model, flatten_params, unflatten_params
+from ..models import MLPNet, build_model, flatten_params, unflatten_params
 from ..utils.checkpoint import DEFAULT_PATH, checkpoint_compatible, load_or_init, save_model
 from ..utils.metrics import RoundLogger
 from .arguments import Arguments, ROUND_MODE_BATCHES
@@ -266,13 +266,11 @@ class Coordinator(BusClient):
 
     def _dataset(self):
         if self.args.synthetic and self.args.synthetic > 0:
-            x, y = synthetic_for_model(self.args.model, self.args.synthetic, seed=self.args.seed)
-            return BaseDataset(x, y)
-        from ..data import load_dataset
-        ds = load_dataset(getattr(self.args, "dataset", "unsw"), self.args.test_path)
-        if category.is_category(MODEL_REGISTRY.get(self.args.model)):
-            return BaseDataset(*category.labels(ds))     # the rows' attack categories are the labels
-        return ds
+            ds = targets.synthetic_dataset(self.args.model, self.args.synthetic, seed=self.args.seed)
+        else:
+            from ..data import load_dataset
+            ds = load_dataset(getattr(self.args, "dataset", "unsw"), self.args.test_path)
+        return targets.of(self.args.model).dataset(ds)
 
     def _fit_config(self, mode: str) -> FitConfig:
         loss = self.args.loss
@@ -316,18 +314,16 @@ class Coordinator(BusClient):
             raise ValueError("--async-buffer applies to remote mode only: local mode trains its virtual workers in lockstep launches")
         model = self._load_model()
         cfg = self._fit_config("local")
-        ae = anomaly.is_autoencoder(model)
-        if ae:
-            anomaly.check_settings(self.args)
+        tgt = targets.of(model)
+        tgt.check_settings(self.args)
 
         log.info("Distribution data among the virtual workers")
         fed = federate(self._dataset(), list(to_train.keys()), self.device)
         log.info("Done")
         held = self._hold_out_local(model, fed, cfg.seed)
-        if ae:
-            from ..data.federate import Shard
-            for wid in fed.workers:
-                fed.shards[wid] = Shard(wid, *anomaly.training_rows(fed[wid].x, fed[wid].y))
+        from ..data.federate import Shard
+        for wid in fed.workers:
+            fed.shards[wid] = Shard(wid, *tgt.training_rows(fed[wid].x, fed[wid].y))
 
         theta = flatten_params(model).to(self.device)
         model.to(self.device)
@@ -370,33 +366,19 @@ class Coordinator(BusClient):
                     rec["agg_weights"][i] = agg_w[j]
             if held is not None and self._fed_eval_round(r):
                 ex, ey, sizes = held
-                if ae:
-                    rec["fed_eval"] = result["fed_eval"] = anomaly.record(
-                        dict(zip(fed.workers, anomaly.summarize(model, theta, ex, ey, self.args.eval_bins, sizes))), self.args.alarm_fpr,
-                        self.args.eval_bins)
-                else:
-                    make = category.record if category.is_category(model) else fedeval.record
-                    rec["fed_eval"] = result["fed_eval"] = make(
-                        dict(zip(fed.workers, fedeval.summarize(model, theta, ex, ey, self.args.eval_bins, self.args.eval_threshold, sizes))))
+                summaries = tgt.summarize(model, theta, ex, ey, self.args.eval_bins, self.args.eval_threshold, sizes)
+                rec["fed_eval"] = result["fed_eval"] = tgt.record(dict(zip(fed.workers, summaries)), self.args)
             self.metrics.end_round(r, time.time() - t0, selected=fed.workers, n_k=counts, loss_k=losses, **rec)
-            self._maybe_checkpoint(model, theta, r, {"workers": fed.workers, "mode": "local", **self._model_meta(model, result)})
+            self._maybe_checkpoint(model, theta, r, {"workers": fed.workers, "mode": "local", **tgt.checkpoint_meta(result.get("fed_eval"))})
         log.info("End training")
         unflatten_params(model, theta)
         save_model(model.cpu(), self.path, meta={"model": self.args.model, "rounds": self.enabled_round, "workers": fed.workers, "mode": "local",
-                                                 **self._model_meta(model, result)})
+                                                 **tgt.checkpoint_meta(result.get("fed_eval"))})
         self._deregister(to_train.keys())
         self.metrics.end_training()
         self.trainings_done += 1
         log.info("End training local")
         return result
-
-    @staticmethod
-    def _model_meta(model, result: Dict[str, Any]) -> Dict[str, Any]:
-        """An autoencoder's checkpoint sidecar carries the alarm threshold of its last federated evaluation, a category
-        model's the names of its classes"""
-        if anomaly.is_autoencoder(model):
-            return {"anomaly": anomaly.checkpoint_meta(result.get("fed_eval"))}
-        return {"classes": list(category.CATEGORIES)} if category.is_category(model) else {}
 
     def _fed_eval_round(self, r: int) -> bool:
         """``--fed-eval-every N``: the global model is evaluated after every N-th round and after the last one"""
@@ -455,8 +437,7 @@ class Coordinator(BusClient):
         cfg = self._fit_config("remote")
         if self.args.fed_eval_every > 0:
             self.args.fed_eval_settings()
-        if anomaly.is_autoencoder(model):
-            anomaly.check_settings(self.args)
+        targets.of(model).check_settings(self.args)
         theta = flatten_params(model).cpu()
         loop = asyncio.get_running_loop()
         # one thread per selected device: every fit RPC of a round is in flight at the same time (the default
@@ -479,7 +460,7 @@ class Coordinator(BusClient):
             self._deregister(to_train.keys())
         unflatten_params(model, theta)
         save_model(model, self.path, meta={"model": self.args.model, "rounds": self.enabled_round, "workers": list(to_train.keys()), "mode": "remote",
-                                           **self._model_meta(model, result)})
+                                           **targets.of(model).checkpoint_meta(result.get("fed_eval"))})
         eval_loss = None
         if self.evaluate_after:
             ds = self._dataset()
@@ -579,12 +560,13 @@ class Coordinator(BusClient):
             bytes_out = sum(traffic(w)[0] - sent0[wid][0] for wid, w in to_train.items() if wid in sent0)
             bytes_in = sum(traffic(w)[1] - sent0[wid][1] for wid, w in to_train.items() if wid in sent0)
             if self._fed_eval_round(r):
-                agg_rec["fed_eval"] = result["fed_eval"] = await self._remote_fed_eval(alive, theta, eval_classes, loop, pool, ae=anomaly.is_autoencoder(model))
+                agg_rec["fed_eval"] = result["fed_eval"] = await self._remote_fed_eval(alive, theta, eval_classes, loop, pool)
             self.metrics.end_round(r, time.time() - t0, selected=ids, n_k=counts, bytes_out=bytes_out, bytes_in=bytes_in, **secagg_rec,
                                    **agg_rec)
             result["bytes_out"] = result.get("bytes_out", 0) + bytes_out
             result["bytes_in"] = result.get("bytes_in", 0) + bytes_in
-            self._maybe_checkpoint(model, theta, r, {"workers": list(to_train.keys()), "mode": "remote", **self._model_meta(model, result)})
+            self._maybe_checkpoint(model, theta, r, {"workers": list(to_train.keys()), "mode": "remote",
+                                                     **targets.of(model).checkpoint_meta(result.get("fed_eval"))})
             if not alive:
                 break
         return theta
@@ -658,7 +640,7 @@ class Coordinator(BusClient):
                 if self._fed_eval_round(steps):
                     while in_flight:                                    # drain: the fits in flight count toward the next step
                         buffer += await collect()
-                    rec["fed_eval"] = result["fed_eval"] = await self._remote_fed_eval(alive, current, eval_classes, loop, pool, ae=anomaly.is_autoencoder(model))
+                    rec["fed_eval"] = result["fed_eval"] = await self._remote_fed_eval(alive, current, eval_classes, loop, pool)
                 sent = {wid: traffic(w) for wid, w in to_train.items()}
                 rec["bytes_out"] = sum(sent[w][0] - sent0[w][0] for w in sent)
                 rec["bytes_in"] = sum(sent[w][1] - sent0[w][1] for w in sent)
@@ -666,7 +648,8 @@ class Coordinator(BusClient):
                 result["bytes_in"] = result.get("bytes_in", 0) + rec["bytes_in"]
                 sent0 = sent
                 self.metrics.end_round(steps, time.time() - t0, **rec)
-                self._maybe_checkpoint(model, current, steps, {"workers": list(to_train.keys()), "mode": "remote", **self._model_meta(model, result)})
+                self._maybe_checkpoint(model, current, steps, {"workers": list(to_train.keys()), "mode": "remote",
+                                                               **targets.of(model).checkpoint_meta(result.get("fed_eval"))})
                 steps += 1
                 t0 = time.time()
         # after the last step: nothing new is dispatched; what is still in flight is awaited, then discarded with the buffer
@@ -701,33 +684,28 @@ class Coordinator(BusClient):
         rec["async"] = {"version": version, "replies": plan.record, "stale_dropped": plan.stale_dropped, "in_flight": in_flight}
         return rec
 
-    async def _remote_fed_eval(self, alive, theta: torch.Tensor, classes: int, loop, pool, ae: bool = False) -> Dict[str, Any]:
+    async def _remote_fed_eval(self, alive, theta: torch.Tensor, classes: int, loop, pool) -> Dict[str, Any]:
         """Federated evaluation of ``theta`` (the true global model, fp32) on every live device's evaluation data.  Every reply
         must be the summary of ``classes`` output columns (the coordinator's model, never what the device claims) and pass
-        ``fedeval.from_wire``'s checks, or the device is listed under ``eval_excluded``; a device without evaluation data is
-        listed under ``eval_missing``.  ``ae``: the model is an autoencoder, the replies are reconstruction-error summaries
-        (``anomaly.from_wire``) and the record carries the federated alarm threshold (``anomaly.record``)."""
+        the ``from_wire`` checks of the model's target (fl/targets.py), or the device is listed under ``eval_excluded``; a device
+        without evaluation data is listed under ``eval_missing``."""
         bins, thr = self.args.eval_bins, self.args.eval_threshold
-        decode = (lambda resp: anomaly.from_wire(resp, bins)) if ae else (lambda resp: fedeval.from_wire(resp, classes, bins))
+        tgt = targets.of(self.args.model)
 
         async def ask(wid, worker):
             try:
                 resp = await loop.run_in_executor(pool, lambda: worker.evaluate(theta, self.args.model, bins, thr, timeout=self.fit_timeout))
                 if not resp.get("ok", False):
                     return wid, "missing" if resp.get("eval_missing") else "excluded"
-                return wid, decode(resp)
+                return wid, tgt.from_wire(resp, classes, bins)
             except Exception as e:  # noqa: BLE001 - a device's reply is untrusted: it is left out of the total
                 log.info("Worker %s: evaluation reply refused: %r", wid, e)
                 return wid, "excluded"
 
         answers = await asyncio.gather(*[ask(wid, w) for wid, w in alive.items()])
-        good = {wid: a for wid, a in answers if isinstance(a, (fedeval.Summary, anomaly.ReconSummary))}
+        good = {wid: a for wid, a in answers if not isinstance(a, str)}
         excluded, missing = [wid for wid, a in answers if a == "excluded"], [wid for wid, a in answers if a == "missing"]
-        if ae:
-            return anomaly.record(good, self.args.alarm_fpr, bins, excluded=excluded, missing=missing)
-        if category.is_category(MODEL_REGISTRY.get(self.args.model)):
-            return category.record(good, excluded=excluded, missing=missing)
-        return fedeval.record(good, excluded=excluded, missing=missing)
+        return tgt.record(good, self.args, excluded=excluded, missing=missing)
 
     async def _secagg_setup(self, alive, tag: str, loop, pool, result) -> Optional[Dict[str, Any]]:
         """Secure aggregation's key agreement: every device returns a fresh public key for the training ``tag``, then every
@@ -850,17 +828,14 @@ class Coordinator(BusClient):
     def _inference(self, worker: RemoteWorkerClient) -> None:
         model = self._load_model()
         flat = flatten_params(model)
-        alarm = None
-        if anomaly.is_autoencoder(model):
-            # the alarm threshold travels with the checkpoint (its JSON sidecar); without one an autoencoder flags nothing
-            from ..utils.checkpoint import load_meta
-            alarm = (load_meta(self.path).get("anomaly") or {}) if os.path.exists(self.path) else {}
-            if alarm.get("alarm_bin") is None or alarm.get("bins") is None:
-                log.info("Inference refused: the autoencoder checkpoint at %s has no alarm threshold (train it with --fed-eval-every)",
-                         self.path)
-                self.known_workers.pop(worker.id, None)
-                worker.close()
-                return
+        tgt = targets.of(model)
+        try:
+            alarm = tgt.inference_alarm(self.path)
+        except ValueError as e:
+            log.info("Inference refused: %s", e)
+            self.known_workers.pop(worker.id, None)
+            worker.close()
+            return
         try:
             count = worker.search("inference")
             log.info("inference tensors found: %d", count)
@@ -868,8 +843,7 @@ class Coordinator(BusClient):
                 pred = worker.predict(flat, self.args.model, alarm=alarm)
                 self.last_predictions = pred
                 log.info(pred)
-                if category.is_category(model):
-                    log.info("attack categories: %s", [category.CATEGORIES[i] if 0 <= i < len(category.CATEGORIES) else i for i in pred])
+                tgt.log_predictions(pred)
             else:
                 log.info("Inference data not found!")
         finally:

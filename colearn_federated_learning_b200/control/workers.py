@@ -28,10 +28,9 @@ import msgpack
 import numpy as np
 import torch
 
-from ..data import dataset_tensors
-from ..fl import anomaly, category, fedeval
+from ..data import category_tensors, dataset_tensors
+from ..fl import fedeval, targets
 from ..fl.trainer import FitConfig, local_fit
-from ..fl.evaluate import predict as predict_fn
 from ..fl.secagg import SecAggDevice
 from ..fl.uplink import FIELDS, UplinkCodec, check_reply, device_reply, echo, request_fields, uplink_key
 from ..models import build_model, num_params
@@ -127,7 +126,7 @@ class WorkerServer:
         self.device = device or torch.device("cuda" if torch.cuda.is_available() else "cpu")
         self.verbose = verbose
         self.datasets: Dict[str, Tuple[torch.Tensor, torch.Tensor]] = {}
-        # attack-category class indices [N, 1] of a hosted dataset that has them (fl/category.py), under the same key
+        # attack-category class indices [N, 1] of a hosted dataset that has them (fl/targets.py), under the same key
         self.categories: Dict[str, torch.Tensor] = {}
         self.tagged: Dict[str, List[torch.Tensor]] = {}
         self.fits_served = 0
@@ -188,7 +187,7 @@ class WorkerServer:
         self.datasets[key] = dataset_tensors(dataset, self.device)
         self.categories.pop(key, None)
         if getattr(dataset, "categories", None) is not None:
-            self.categories[key] = category.labels(dataset, self.device)[1]
+            self.categories[key] = category_tensors(dataset, self.device)[1]
 
     def hold_out_evaluation(self, fraction: float, seed: int) -> None:
         """Move a seeded ``fraction`` of the training rows to the evaluation set (``fedeval.split_eval``), their attack
@@ -200,16 +199,6 @@ class WorkerServer:
         if "training" in self.categories:           # the same rows: the split depends on n and the seed only
             _, ct, _, ce = fedeval.split_eval(x, self.categories["training"], fraction, seed)
             self.categories["training"], self.categories["evaluation"] = ct, ce
-
-    def _labels(self, model, key: str, y: torch.Tensor) -> Tuple[Optional[torch.Tensor], Optional[str]]:
-        """``(labels, None)`` the model trains and is scored on: the attack categories for a category model, ``y`` otherwise;
-        ``(None, reason)`` when this device's ``key`` data has no categories"""
-        if not category.is_category(model):
-            return y, None
-        codes = self.categories.get(key)
-        if codes is None:
-            return None, f"{model.__class__.__name__} trains on attack categories: this device's {key} data has none"
-        return codes, None
 
     def load_data(self, tensors: List[torch.Tensor], tag: str = "inference") -> None:
         self.tagged.setdefault(tag, []).extend(t.to(self.device) for t in tensors)
@@ -256,15 +245,12 @@ class WorkerServer:
                     spec = getattr(model, "spec", None)
                     if spec is not None and not spec.flatten_input and held[0].shape[1] != spec.dims[0]:
                         return {"ok": False, "error": f"evaluation data has {held[0].shape[1]} features, {req.get('model')} wants {spec.dims[0]}"}
-                    if anomaly.is_autoencoder(model):
-                        return {"ok": True, **anomaly.to_wire(anomaly.summarize(model, flat, held[0], held[1], int(req.get("bins", 256)))[0])}
-                    ey, why = self._labels(model, "evaluation", held[1])
-                    if why:
-                        return {"ok": False, "error": f"evaluation refused: {why}"}
-                    s = fedeval.summarize(model, flat, held[0], ey, int(req.get("bins", 256)), float(req.get("threshold", 0.5)))[0]
+                    tgt = targets.of(model)
+                    ex, ey = tgt.device_rows(model, "evaluation", *held, self.categories.get("evaluation"))
+                    s = tgt.summarize(model, flat, ex, ey, int(req.get("bins", 256)), float(req.get("threshold", 0.5)))[0]
+                    return {"ok": True, **tgt.to_wire(s)}
                 except (ValueError, TypeError) as e:
                     return {"ok": False, "error": f"evaluation refused: {e}"}
-                return {"ok": True, **fedeval.to_wire(s)}
         if op == "predict":
             data = self.tagged.get(req.get("tag", "inference"), [])
             if not data:
@@ -276,17 +262,10 @@ class WorkerServer:
                 spec = getattr(model, "spec", None)
                 keep_shape = spec is None                       # conv nets take [C, H, W] samples as they are
                 x = torch.stack([d if keep_shape else d.reshape(-1) for d in data]).float()
-                if anomaly.is_autoencoder(model):
-                    # per-row alarms at the federated threshold the request carries ("alarm_bin" of "bins" error bins)
-                    j, bins = req.get("alarm_bin"), req.get("bins")
-                    if not isinstance(j, int) or not isinstance(bins, int) or isinstance(j, bool) or isinstance(bins, bool):
-                        return {"ok": False, "error": f"{req['model']} predicts alarms: the request needs an integer alarm_bin and bins"}
-                    try:
-                        pred = anomaly.predict(model, flat, x, j, bins)
-                    except ValueError as e:
-                        return {"ok": False, "error": f"prediction refused: {e}"}
-                    return {"ok": True, "pred": pred.reshape(-1).tolist(), "count": len(data)}
-                pred = predict_fn(model, x, flat)
+                try:
+                    pred = targets.of(model).predict(model, flat, x, req)
+                except ValueError as e:
+                    return {"ok": False, "error": str(e)}
                 return {"ok": True, "pred": pred.reshape(-1).tolist(), "count": len(data)}
         return {"ok": False, "error": f"unknown op {op!r}"}
 
@@ -314,11 +293,11 @@ class WorkerServer:
             spec = getattr(model, "spec", None)
             if spec is not None and not spec.flatten_input and x.shape[1] != spec.dims[0]:
                 return {"ok": False, "error": f"dataset has {x.shape[1]} features, {cfg.model} wants {spec.dims[0]}"}
-            if anomaly.is_autoencoder(model):
-                x, y = anomaly.training_rows(x, y)       # the benign rows, the input as the target; n = their count
-            y, why = self._labels(model, key, y)
-            if why:
-                return {"ok": False, "error": why}
+            tgt = targets.of(model)
+            try:
+                x, y = tgt.training_rows(*tgt.device_rows(model, key, x, y, self.categories.get(key)))    # n = their count
+            except ValueError as e:
+                return {"ok": False, "error": str(e)}
             if sa is not None:
                 if any(b.is_floating_point() for b in model.buffers()):
                     return {"ok": False, "error": f"secure aggregation refused: {cfg.model}'s floating-point buffers would travel in the clear"}

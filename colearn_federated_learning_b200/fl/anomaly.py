@@ -1,9 +1,9 @@
-"""Federated anomaly detection: an autoencoder (a model whose ``spec.target`` is ``"input"``) is trained on every device's
-benign rows to reconstruct them; a row whose reconstruction error lies at or above the federated alarm threshold is an
+"""Federated anomaly detection: an autoencoder (the target :data:`fl.targets.INPUT`) is trained on every device's benign rows
+to reconstruct them; a row whose reconstruction error lies at or above the federated alarm threshold is an
 alarm.  The devices agree on the threshold without pooling their data: each returns an additive summary of its held-out
 rows, and the coordinator picks the threshold from the sum.
 
-This is the only module that knows these rules:
+This is the only module that knows these rules (:mod:`fl.targets` calls them for an autoencoder):
 
 * **Training rows.**  A device trains on its rows labelled 0 (benign), with the input itself as the target: the kernel's
   ``y`` is the shard's ``x`` (``y_dim`` = D), so nothing is copied twice.  ``n_k`` of ``--weighted`` is the benign count.
@@ -35,12 +35,6 @@ from .fedeval import _auc_ap, _div
 MIN_BINS = 32
 
 
-def is_autoencoder(model) -> bool:
-    """True for a model trained to reconstruct its input (``MLPSpec.target == "input"``)"""
-    spec = getattr(model, "spec", None)
-    return spec is not None and getattr(spec, "target", "label") == "input"
-
-
 def training_rows(x: torch.Tensor, y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """``(x_benign, x_benign)``: the rows labelled 0 as input and target (one tensor, passed twice)"""
     xb = x[y.reshape(-1) == 0].contiguous()
@@ -67,7 +61,8 @@ def summarize(model, flat: torch.Tensor, x: torch.Tensor, y: Optional[torch.Tens
     """One :class:`ReconSummary` per segment of consecutive rows of ``x`` (all rows when ``segments`` is None) of the
     autoencoder whose parameters are ``flat``: one forward (``ops.mlp_forward``), one ``ops.recon_summary`` launch."""
     from .evaluate import forward_flat
-    if not is_autoencoder(model):
+    from .targets import INPUT, of
+    if of(model) is not INPUT:
         raise ValueError("the reconstruction summary needs an autoencoder (a model trained on its input)")
     x = x.to(flat.device).float()
     xhat = forward_flat(model, flat, x)

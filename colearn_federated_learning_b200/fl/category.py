@@ -1,31 +1,17 @@
-"""Attack categorisation: a model whose ``spec.target`` is ``"category"`` (``ffnn_category``) is trained and evaluated on the
-attack category of every row (``data.CATEGORIES``: Normal, DDoS, DoS, Reconnaissance, Theft) instead of the binary ``attack``
-label.  This module holds the rules every mode shares:
-
-* which labels such a model takes (:func:`labels`: the dataset's category codes; a dataset without them is refused);
-* what its federated-evaluation record adds to the usual per-class and macro metrics (:func:`record`): the class names and
-  the binary detection view of the same summed summary, so that its numbers compare line for line with the binary FFNN's.
+"""Attack categorisation: a model of the target :data:`fl.targets.CATEGORY` (``ffnn_category``) is trained and evaluated on
+the attack category of every row (``data.CATEGORIES``: Normal, DDoS, DoS, Reconnaissance, Theft) instead of the binary
+``attack`` label; :mod:`fl.targets` picks those labels (``data.category_tensors``: the dataset's category codes; a dataset
+without them is refused).  This module holds what its federated-evaluation record adds to the usual per-class and macro
+metrics (:func:`record`): the class names and the binary detection view of the same summed summary, so that its numbers
+compare line for line with the binary FFNN's.
 """
 from __future__ import annotations
 
-from typing import Any, Dict, Optional, Sequence, Tuple
+from typing import Any, Dict, Optional, Sequence
 
-import torch
-
-from ..data.datasets import CATEGORIES, category_tensors
+from ..data.datasets import CATEGORIES
 from . import fedeval
 from .fedeval import _auc_ap, _div
-
-
-def is_category(model) -> bool:
-    """True for a model trained on the attack category (``MLPSpec.target == "category"``); takes a model or its class"""
-    spec = getattr(model, "spec", None)
-    return spec is not None and getattr(spec, "target", "label") == "category"
-
-
-def labels(ds, device: Optional[torch.device] = None) -> Tuple[torch.Tensor, torch.Tensor]:
-    """``(X[N, F], class index[N, 1])`` of a dataset with attack categories; ValueError with the reason for one without"""
-    return category_tensors(ds, device)
 
 
 def attack_view(s: fedeval.Summary) -> Dict[str, Any]:

@@ -308,18 +308,11 @@ def parse_cli(argv=None) -> argparse.Namespace:
             check_model(build_model(ns.model))
         except ValueError as e:
             parser.error(f"--fed-eval-every with --model {ns.model}: {e}")
-    from colearn_federated_learning_b200.fl import anomaly
-    if anomaly.is_autoencoder(MODEL_REGISTRY.get(ns.model)):
-        try:
-            anomaly.check_settings(ns, box=ns.box, encryption=ns.encryption)
-        except ValueError as e:
-            parser.error(str(e))
-    from colearn_federated_learning_b200.fl import category
-    if category.is_category(MODEL_REGISTRY.get(ns.model)):
-        if ns.box:
-            parser.error(f"--model {ns.model} does not run in box mode (--box): box mode trains on the binary attack label")
-        if ns.encryption:
-            parser.error(f"--model {ns.model} does not run with -e: the secret-shared training takes the binary attack label")
+    from colearn_federated_learning_b200.fl import targets
+    try:
+        targets.of(ns.model).check_settings(ns, box=ns.box, encryption=ns.encryption)
+    except ValueError as e:
+        parser.error(str(e))
     if ns.secure_agg:
         if ns.box or ns.encryption or not ns.remote:
             parser.error("--secure-agg applies to remote mode (-r) only: in local mode every update is in the coordinator's process "

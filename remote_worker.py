@@ -70,15 +70,11 @@ def pick_dataset(args):
     """--synthetic N > the CSV given with -dt > the reference's XOR toy set (rw.py:75-80).  Synthetic rows made for an
     attack-category model (--data-model ffnn_category) keep their class indices as the dataset's categories, next to the
     binary attack label, like a Bot-IoT CSV."""
-    from colearn_federated_learning_b200.data import BaseDataset, category_dataset, load_dataset, synthetic_for_model, xor_toy_dataset
-    from colearn_federated_learning_b200.fl import category
-    from colearn_federated_learning_b200.models import MODEL_REGISTRY
+    from colearn_federated_learning_b200.data import load_dataset, xor_toy_dataset
+    from colearn_federated_learning_b200.fl import targets
 
     if args.synthetic > 0:
-        x, y = synthetic_for_model(args.data_model, args.synthetic, seed=args.seed)
-        if category.is_category(MODEL_REGISTRY.get(args.data_model)):
-            return category_dataset(x, y)
-        return BaseDataset(x, y)
+        return targets.synthetic_dataset(args.data_model, args.synthetic, seed=args.seed)
     if args.training:
         logging.info("training data: %s", args.training)
         return load_dataset(args.dataset, args.training)

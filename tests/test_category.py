@@ -335,6 +335,18 @@ def test_attack_view_is_the_collapsed_matrix():
     assert math.isclose(v["auc"], fedeval._auc_ap(hist[0, 0], hist[0, 1])[0])
 
 
+def test_target_lookup():
+    """targets.of takes a registry name, a model class or a built model; LABEL for a model without a spec and for any other
+    target value"""
+    from types import SimpleNamespace
+    from colearn_federated_learning_b200.fl import targets
+    from colearn_federated_learning_b200.models import MODEL_REGISTRY, build_model
+    assert targets.of(CAT) is targets.of(MODEL_REGISTRY[CAT]) is targets.of(build_model(CAT)) is targets.CATEGORY
+    assert targets.of("autoencoder") is targets.of(build_model("autoencoder")) is targets.INPUT
+    for other in ("ffnn", "resnet18", "no_such_model", lambda: None, SimpleNamespace(spec=SimpleNamespace(target="other"))):
+        assert targets.of(other) is targets.LABEL, other
+
+
 def local_run(tmp_path, device=torch.device("cpu"), **kw):
     """A 4-worker local training on synthetic_category with a federated evaluation after every round (test_anomaly.local_run)"""
     from colearn_federated_learning_b200.control.arguments import Arguments
