@@ -9,7 +9,7 @@ as a CLI flag by ``federated_coordinator.py`` with the reference value as defaul
 from __future__ import annotations
 
 from dataclasses import dataclass, asdict
-from typing import Any, Dict
+from typing import Any, Dict, Optional
 
 DEFAULT_TEST_PATH = "./dataset_example/UNSW_2018_IoT_Botnet_Final_10_best_Training_1_1.csv"
 ROUND_MODE_BATCHES = 1000  # reference: ``round > 1`` forces 1000 local batches (fc.py:533-535)
@@ -60,6 +60,9 @@ class Arguments:
     eval_fraction: float = 0.0     # federated evaluation, local and box mode: fraction of every device's shard held out, in (0, 1)
     alarm_fpr: float = 0.01        # autoencoder: the alarm threshold lets at most this fraction of the held-out benign rows raise an
                                    # alarm, in (0, 1) (fl/anomaly.py)
+    class_weight: Optional[str] = None   # class-weighted local fits (fl/classweight.py): "balanced" (from the federated class
+                                   # counts) or C comma-separated weights; None: unweighted
+    class_weight_max: float = 10.0  # balanced class weights: the cap of every weight (> 0)
     async_buffer: int = 0          # remote mode: >0 = asynchronous buffered aggregation, one server step per K replies from devices
                                    # that train from whatever version is current (fl/asyncagg.py); 0 = synchronous rounds
     async_concurrency: int = 0     # asynchronous: fits in flight (0 = one per selected device)

@@ -23,6 +23,7 @@ import secrets
 import time
 import zlib
 from collections import OrderedDict
+from dataclasses import replace
 from functools import partial
 from typing import Any, Dict, List, Optional
 
@@ -33,7 +34,7 @@ from .. import ops, settings
 from ..data import federate
 from ..fl.fedavg import normalized_weights
 from ..fl.trainer import FitConfig, local_fit, make_perm, resolve_loss
-from ..fl import asyncagg, fedeval, targets, uplink
+from ..fl import asyncagg, classweight, fedeval, targets, uplink
 from ..fl.evaluate import evaluate
 from ..fl.secagg import check_masked_reply, check_unmask_reply, correction_streams, frac_bits, pk_from_bytes, pk_to_bytes
 from ..fl.server_opt import server_opt_state
@@ -324,12 +325,17 @@ class Coordinator(BusClient):
         from ..data.federate import Shard
         for wid in fed.workers:
             fed.shards[wid] = Shard(wid, *tgt.training_rows(fed[wid].x, fed[wid].y))
+        cw = classweight.setting(self.args, tgt.classes(model))
+        result: Dict[str, Any] = {"workers": list(to_train.keys()), "losses": {}, "rounds": self.enabled_round}
+        if cw is not None:
+            # one weight vector for the training, from every virtual worker's training rows (balanced) or as given
+            result["class_weights"] = classweight.local(cw, [fed[wid].y for wid in fed.workers])
+            cfg = replace(cfg, class_weights=result["class_weights"]["weights"])
 
         theta = flatten_params(model).to(self.device)
         model.to(self.device)
         log.info("Start training")
         self.metrics.start_training(cfg.max_nr_batches)
-        result: Dict[str, Any] = {"workers": list(to_train.keys()), "losses": {}, "rounds": self.enabled_round}
         codec = self.args.uplink_codec()
         result["uplink"] = codec.kind
         # topk: every device's error-feedback residual, zero at the start of the training (memory only, not checkpointed)
@@ -358,7 +364,7 @@ class Coordinator(BusClient):
             for wid, l in zip(fed.workers, losses):
                 self.metrics.worker_loss(wid, l)
                 result["losses"][wid] = l
-            rec = {}
+            rec = self._training_fields(result, r)
             if agg_w is not None:
                 # distance-based aggregator: the final weight of every worker in the order of `selected` (0: excluded or not trained)
                 rec["agg_weights"] = [0.0] * len(fed.workers)
@@ -449,7 +455,13 @@ class Coordinator(BusClient):
         alive = OrderedDict(to_train)
         run = self._remote_async if self.args.async_settings() is not None else self._remote_rounds
         try:
+            cw = await self._class_weights(model, alive, loop, pool)
+            if cw is not None:
+                result["class_weights"] = cw
+                cfg = replace(cfg, class_weights=cw["weights"])      # every fit request carries them
             theta = await run(alive, to_train, theta, cfg, loop, pool, model, result)
+        except classweight.NoCounts as e:
+            log.info("Class weights: %s: no rounds", e)
         finally:
             # whatever happened above, the devices' sockets are closed and they leave the registry (fc.py:573-580, 595-597)
             pool.shutdown(wait=False)
@@ -562,7 +574,7 @@ class Coordinator(BusClient):
             if self._fed_eval_round(r):
                 agg_rec["fed_eval"] = result["fed_eval"] = await self._remote_fed_eval(alive, theta, eval_classes, loop, pool)
             self.metrics.end_round(r, time.time() - t0, selected=ids, n_k=counts, bytes_out=bytes_out, bytes_in=bytes_in, **secagg_rec,
-                                   **agg_rec)
+                                   **agg_rec, **self._training_fields(result, r))
             result["bytes_out"] = result.get("bytes_out", 0) + bytes_out
             result["bytes_in"] = result.get("bytes_in", 0) + bytes_in
             self._maybe_checkpoint(model, theta, r, {"workers": list(to_train.keys()), "mode": "remote",
@@ -647,7 +659,7 @@ class Coordinator(BusClient):
                 result["bytes_out"] = result.get("bytes_out", 0) + rec["bytes_out"]
                 result["bytes_in"] = result.get("bytes_in", 0) + rec["bytes_in"]
                 sent0 = sent
-                self.metrics.end_round(steps, time.time() - t0, **rec)
+                self.metrics.end_round(steps, time.time() - t0, **rec, **self._training_fields(result, steps))
                 self._maybe_checkpoint(model, current, steps, {"workers": list(to_train.keys()), "mode": "remote",
                                                                **targets.of(model).checkpoint_meta(result.get("fed_eval"))})
                 steps += 1
@@ -706,6 +718,32 @@ class Coordinator(BusClient):
         good = {wid: a for wid, a in answers if not isinstance(a, str)}
         excluded, missing = [wid for wid, a in answers if a == "excluded"], [wid for wid, a in answers if a == "missing"]
         return tgt.record(good, self.args, excluded=excluded, missing=missing)
+
+    @staticmethod
+    def _training_fields(result: Dict[str, Any], r: int) -> Dict[str, Any]:
+        """What the first round record of a training carries besides its own fields: the ``class_weights`` block"""
+        return {"class_weights": result["class_weights"]} if r == 0 and "class_weights" in result else {}
+
+    async def _class_weights(self, model, alive, loop, pool) -> Optional[Dict[str, Any]]:
+        """The ``class_weights`` block of a remote training (fl/classweight.py), None without ``--class-weight``.  ``balanced``
+        asks every device in ``alive`` for the class counts of its training rows once (the ``class_counts`` request); a device
+        whose request fails or whose reply fails the checks is left out of the sum and listed under ``excluded`` (it still
+        trains).  :class:`classweight.NoCounts` when no device answered usable counts."""
+        st = classweight.setting(self.args, targets.of(model).classes(model))
+        if st is None or st.mode == "given":
+            return None if st is None else classweight.record(st, st.given)
+
+        async def ask(wid, worker):
+            try:
+                return wid, await loop.run_in_executor(pool, lambda: worker.class_counts(self.args.model, timeout=self.fit_timeout))
+            except Exception as e:  # noqa: BLE001 - the device is excluded from the counts, not from the training
+                return wid, {"ok": False, "error": repr(e)}
+
+        replies = dict(await asyncio.gather(*[ask(wid, w) for wid, w in alive.items()]))
+        rec = classweight.weights_from(st, replies)
+        if rec["excluded"]:
+            log.info("Class weights: no usable counts from %s", ", ".join(rec["excluded"]))
+        return rec
 
     async def _secagg_setup(self, alive, tag: str, loop, pool, result) -> Optional[Dict[str, Any]]:
         """Secure aggregation's key agreement: every device returns a fresh public key for the training ``tag``, then every
@@ -881,7 +919,7 @@ def train_virtual_workers(theta: torch.Tensor, model, fed, cfg: FitConfig, round
         if tasks:
             descs = ops.build_client_descs(tasks, device)
             ops.mlp_local_sgd_multi(spec.dims, spec.out_activation, descs, len(tasks), cfg.batch_size, cfg.lr,
-                                    cfg.epochs, cfg.max_nr_batches, resolve_loss(cfg.model, cfg.loss))
+                                    cfg.epochs, cfg.max_nr_batches, resolve_loss(cfg.model, cfg.loss), class_weights=cfg.class_weights)
             vals = loss_out[:, 0].tolist()
             for i in idx:
                 losses[i] = vals[i]
@@ -895,7 +933,8 @@ def train_virtual_workers(theta: torch.Tensor, model, fed, cfg: FitConfig, round
                      for i, sh in zip(idx, shards)]
             res = ops.host.mlp_local_sgd_multi(spec.dims, spec.out_activation, [flats[i] for i in idx], [sh.x for sh in shards],
                                                [sh.y for sh in shards], perms, cfg.batch_size, cfg.lr, cfg.epochs,
-                                               cfg.max_nr_batches, resolve_loss(cfg.model, cfg.loss))
+                                               cfg.max_nr_batches, resolve_loss(cfg.model, cfg.loss),
+                                               class_weights=cfg.class_weights)
             for j, i in enumerate(idx):
                 losses[i] = float(res[j, 0])
         return flats, losses, counts

@@ -29,11 +29,11 @@ import numpy as np
 import torch
 
 from ..data import category_tensors, dataset_tensors
-from ..fl import fedeval, targets
+from ..fl import classweight, fedeval, targets
 from ..fl.trainer import FitConfig, local_fit
 from ..fl.secagg import SecAggDevice
 from ..fl.uplink import FIELDS, UplinkCodec, check_reply, device_reply, echo, request_fields, uplink_key
-from ..models import build_model, num_params
+from ..models import MODEL_REGISTRY, build_model, num_params
 
 log = logging.getLogger(__name__)
 
@@ -227,6 +227,8 @@ class WorkerServer:
                     return {"ok": True, "pk": self._secagg.setup(req.get("tag"))}
             except ValueError as e:
                 return {"ok": False, "error": f"secure aggregation refused: {e}"}
+        if op == "class_counts":
+            return self._class_counts(req)
         if op == "fit":
             return self._fit(req)
         if op == "evaluate":
@@ -296,6 +298,11 @@ class WorkerServer:
             tgt = targets.of(model)
             try:
                 x, y = tgt.training_rows(*tgt.device_rows(model, key, x, y, self.categories.get(key)))    # n = their count
+                if cfg.class_weights is not None:
+                    classes = tgt.classes(model)
+                    if classes is None:
+                        raise ValueError(f"class weights refused: {cfg.model} has no class-weighted fit")
+                    cfg.class_weights = classweight.check_weights(cfg.class_weights, classes, "class weights refused")
             except ValueError as e:
                 return {"ok": False, "error": str(e)}
             if sa is not None:
@@ -344,6 +351,25 @@ class WorkerServer:
             if "version" in req:                      # asynchronous aggregation: the global version this fit started from
                 reply["version"] = req["version"]
             return reply
+
+    def _class_counts(self, req: Dict[str, Any]) -> Dict[str, Any]:
+        """A ``class_counts`` request (fl/classweight.py): the class counts of the rows a fit of ``model`` would train on"""
+        name, key = req.get("model"), req.get("dataset_key", "training")
+        if not isinstance(name, str) or name not in MODEL_REGISTRY:
+            return {"ok": False, "error": f"unknown model {name!r}"}
+        if key not in self.datasets:
+            return {"ok": False, "error": f"no {key} data on this device"}
+        with self._work_lock:
+            model = self._model_and_arena(name, None)[0]
+            tgt = targets.of(model)
+            classes = tgt.classes(model)
+            if classes is None:
+                return {"ok": False, "error": f"{name} has no classes to count"}
+            try:
+                _, y = tgt.training_rows(*tgt.device_rows(model, key, *self.datasets[key], self.categories.get(key)))
+                return {"ok": True, "counts": classweight.count(y, classes)}
+            except ValueError as e:
+                return {"ok": False, "error": str(e)}
 
     def _restore(self, req: Dict[str, Any], name: str, down: UplinkCodec):
         """``(model, arena, downlink wire)`` a fit request trains from, or ``(None, None, reason)``: the fp32 ``params`` (wire
@@ -495,6 +521,10 @@ class RemoteWorkerClient:
         when it holds no evaluation data); ``fl.fedeval.from_wire`` checks it."""
         return self._call({"op": "evaluate", "params": _to_bytes(flat.float()), "model": model_name, "bins": int(bins),
                            "threshold": float(threshold)}, timeout=timeout, check=False)
+
+    def class_counts(self, model_name: str, timeout: Optional[float] = None) -> Dict[str, Any]:
+        """The device's reply to a ``class_counts`` request, unchecked (fl/classweight.py checks it)"""
+        return self._call({"op": "class_counts", "model": model_name}, timeout=timeout, check=False)
 
     def search(self, tag: str) -> int:
         return int(self._call({"op": "search", "tag": tag}).get("count", 0))

@@ -8,7 +8,7 @@ training path is exercised (reference example file: ``dataset_example/*.csv``).
 """
 from __future__ import annotations
 
-from typing import Optional, Tuple
+from typing import Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -53,15 +53,16 @@ def synthetic_anomaly(n: int, seed: int = 0, attack_fraction: float = 0.1,
     return x, y
 
 
-def synthetic_category(n: int, seed: int = 0, device: Optional[torch.device] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+def synthetic_category(n: int, seed: int = 0, device: Optional[torch.device] = None,
+                       probs: Optional[Sequence[float]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Traffic for the attack classifier (``--model ffnn_category``): ``(X[n, 10] in [0, 1], y[n, 1])`` with ``y`` the class
     index into CATEGORIES, deterministic in ``seed``.  Each class is a Gaussian blob (sd 0.08) around its own fixed centre in
-    [0.2, 0.8]^10 (the same for every seed), clipped to [0, 1]; the classes are drawn with probabilities 40 / 20 / 20 / 10 / 10 %,
-    so Normal is the majority class at 40 %."""
+    [0.2, 0.8]^10 (the same for every seed), clipped to [0, 1]; the classes are drawn with probabilities ``probs`` (one per
+    class, in CATEGORIES order), by default 40 / 20 / 20 / 10 / 10 %, so Normal is the majority class at 40 %."""
     fixed = torch.Generator().manual_seed(20181105)
     centres = 0.2 + 0.6 * torch.rand(len(CATEGORIES), 10, generator=fixed)
     g = torch.Generator().manual_seed(seed)
-    probs = torch.tensor([0.4, 0.2, 0.2, 0.1, 0.1])
+    probs = torch.tensor([0.4, 0.2, 0.2, 0.1, 0.1] if probs is None else [float(p) for p in probs])
     y = torch.multinomial(probs, n, replacement=True, generator=g) if n > 0 else torch.zeros(0, dtype=torch.long)
     x = (centres[y] + 0.08 * torch.randn(n, 10, generator=g)).clamp(0.0, 1.0)
     y = y.float().view(n, 1)

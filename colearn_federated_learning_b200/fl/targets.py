@@ -20,7 +20,8 @@ import torch
 from ..data.datasets import CATEGORIES, BaseDataset, category_dataset, category_tensors
 from ..data.synthetic import synthetic_for_model
 from ..models import MODEL_REGISTRY
-from . import anomaly, category, fedeval
+from ..ops.fused_mlp import NET_FFNN, net_kind_for
+from . import anomaly, category, classweight, fedeval
 from .evaluate import predict as classify
 
 log = logging.getLogger(__name__)
@@ -31,6 +32,16 @@ class Target:
 
     def check_settings(self, args, box: bool = False, encryption: bool = False) -> None:
         """ValueError with the reason when the settings cannot train a model of this target"""
+        classweight.setting(args, self.classes(args.model), box, encryption)
+
+    def classes(self, model) -> Optional[int]:
+        """How many classes a class-weighted fit of ``model`` (a built model, a model class or a registry name) weighs, None when
+        it cannot be class-weighted: 2 (the 0 / 1 label) for the sigmoid FFNN, the one net of this target with class-weighted
+        kernels"""
+        if isinstance(model, str):
+            model = MODEL_REGISTRY.get(model)
+        spec = getattr(model, "spec", None)
+        return 2 if spec is not None and net_kind_for(spec.dims, spec.out_activation) == NET_FFNN else None
 
     def dataset(self, ds):
         """The dataset the coordinator trains on, from the loaded CSV or synthetic dataset"""
@@ -80,6 +91,10 @@ class Target:
 class _Input(Target):
     def check_settings(self, args, box: bool = False, encryption: bool = False) -> None:
         anomaly.check_settings(args, box, encryption)
+        super().check_settings(args, box, encryption)
+
+    def classes(self, model) -> Optional[int]:
+        return None                 # trained on its input: no classes
 
     def training_rows(self, x, y):
         return anomaly.training_rows(x, y)
@@ -124,6 +139,10 @@ class _Category(Target):
             raise ValueError(f"--model {args.model} does not run in box mode (--box): box mode trains on the binary attack label")
         if encryption:
             raise ValueError(f"--model {args.model} does not run with -e: the secret-shared training takes the binary attack label")
+        super().check_settings(args, box, encryption)
+
+    def classes(self, model) -> Optional[int]:
+        return len(CATEGORIES)
 
     def dataset(self, ds):
         return BaseDataset(*category_tensors(ds))     # the rows' attack categories are the labels

@@ -19,7 +19,7 @@ from __future__ import annotations
 import logging
 import os
 from dataclasses import dataclass, asdict, replace
-from typing import Any, Dict, Optional, Tuple
+from typing import Any, Dict, List, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -43,9 +43,13 @@ class FitConfig:
     shuffle: bool = True
     seed: int = 1
     optimizer: str = "SGD"
+    class_weights: Optional[List[float]] = None   # a class-weighted fit (fl/classweight.py); None: unweighted
 
     def to_dict(self) -> Dict[str, Any]:
-        return asdict(self)
+        d = asdict(self)
+        if d["class_weights"] is None:
+            del d["class_weights"]                # an unweighted request is the one it was before class weights existed
+        return d
 
     @classmethod
     def from_dict(cls, d: Dict[str, Any]) -> "FitConfig":
@@ -140,13 +144,16 @@ def local_fit(flat: torch.Tensor, model: nn.Module, x: torch.Tensor, y: torch.Te
     cfg = FitConfig(**{**cfg.to_dict(), "loss": loss})
     if perm is None:
         perm = make_perm(x.shape[0], cfg, flat.device, round_idx)
+    if cfg.class_weights is not None and not isinstance(model, MLPNet):
+        raise ValueError(f"class weights: {cfg.model} has no class-weighted fit")
     if isinstance(model, MLPNet):
         spec = model.spec
         xx = x.view(x.shape[0], -1) if spec.flatten_input else x
         has_kernel = ops.net_kind_for(spec.dims, spec.out_activation) is not None
-        if not flat.is_cuda or has_kernel:
+        # a class-weighted fit goes nowhere else: ops.mlp_local_sgd refuses a net without class-weighted kernels
+        if not flat.is_cuda or has_kernel or cfg.class_weights is not None:
             last = ops.mlp_local_sgd(flat, spec.dims, xx, y, perm, cfg.batch_size, cfg.lr, cfg.epochs,
-                                     cfg.max_nr_batches, loss, spec.out_activation)
+                                     cfg.max_nr_batches, loss, spec.out_activation, class_weights=cfg.class_weights)
             LAST_FIT_LAUNCHES = 1 if flat.is_cuda else 0
             return last, ("persistent" if flat.is_cuda else "reference")
         if flat.is_cuda:

@@ -94,6 +94,8 @@ FFNN_CAT_SPEC = MLPSpec((10, 50, 30, 10, 5), "none", "xent", target="category")
 class FFNN(MLPNet):
     """Simple binary feed-forward network (reference ``client_federated.py:50-69``)."""
 
+    spec = FFNN_SPEC                # on the class too: the CLI tells whether it has class-weighted kernels without building it
+
     def __init__(self) -> None:
         super().__init__(FFNN_SPEC)
 

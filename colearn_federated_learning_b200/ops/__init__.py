@@ -13,7 +13,7 @@ import torch
 from . import reference
 from . import _ext
 from . import host  # noqa: F401  (native CPU executor of the MLP local fit)
-from .fused_mlp import (NET_KINDS, LOSS_CODES, net_kind_for, mlp_local_sgd, mlp_local_sgd_multi,  # noqa: F401
+from .fused_mlp import (NET_KINDS, LOSS_CODES, net_kind_for, mlp_local_sgd, mlp_local_sgd_multi, check_class_weights,  # noqa: F401
                         mlp_forward, ClientTask, build_client_descs)
 from .reference import make_permutation, total_steps  # noqa: F401
 

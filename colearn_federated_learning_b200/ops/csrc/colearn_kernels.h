@@ -136,6 +136,7 @@ cudaError_t preload_comm_kernels();   // force the lazy loader for every kernel 
 cudaError_t set_spin_limit_mlp(unsigned long long ns);
 cudaError_t set_spin_limit_mlp_ae(unsigned long long ns);   // mlp_persistent_ae.cu: its own copy of the limit
 cudaError_t set_spin_limit_mlp_cat(unsigned long long ns);  // mlp_persistent_cat.cu: likewise
+cudaError_t set_spin_limit_mlp_cw(unsigned long long ns);   // mlp_persistent_cw.cu: likewise
 cudaError_t set_spin_limit_gemm(unsigned long long ns);
 
 // ---------------------------------------------------------------------------------------------
@@ -226,6 +227,16 @@ cudaError_t launch_mlp_local_sgd(int net_kind, const ClientDesc* descs, int n_cl
                                  SgdHyper hp, cudaStream_t stream);
 int mlp_local_sgd_smem_bytes(int net_kind, int batch_size);
 int mlp_net_num_params(int net_kind);
+
+// Per-class loss weights of a class-weighted fit (mlp_persistent_cw.cu): w[c] for the classes c < 2 of the FFNN (its 0 / 1 label)
+// or c < 5 of the attack-category net (its class index); every value finite and >= 0 (checked by the caller).  Row i's gradient
+// and loss carry w[c_i] * (1 / batch) where the unweighted fit has 1 / batch (sse: w[c_i] where it has 1).
+struct ClassWeights {
+  float w[8];
+};
+// Variant 5 only, NET_FFNN with bce / sse / mse and NET_FFNN_CAT with xent; anything else: cudaErrorInvalidValue, no launch.
+cudaError_t launch_mlp_local_sgd_cw(int net_kind, const ClientDesc* descs, int n_clients, SgdHyper hp, ClassWeights cw,
+                                    cudaStream_t stream);
 
 // Forward-only batched inference/eval for the small nets: out[n, d_out] (post-activation).
 cudaError_t launch_mlp_forward(int net_kind, const float* theta, const float* x, float* out,

@@ -60,6 +60,7 @@ struct Task {
 struct Hyper {
   int batch, epochs, max_steps, loss;
   float lr;
+  const float* cw = nullptr;   // a class-weighted fit: w[class of the row] (its label y[0]) scales the row's loss and gradient
 };
 
 // Per-thread scratch: activations of every layer for every sample of the batch, dz ping-pong, gradient arena (B > 1)
@@ -95,15 +96,17 @@ __attribute__((always_inline)) inline void forward_one(const Net& net, const flo
   }
 }
 
-// loss value of the batch and dL/d(pre-activation of the last layer) per sample (ops/reference.py::loss_and_dz)
+// loss value of the batch and dL/d(pre-activation of the last layer) per sample (ops/reference.py::loss_and_dz); cw: class
+// weights (nullptr: none)
 __attribute__((always_inline)) inline float loss_and_dout(const Net& net, int loss, const float* acts, int stride_b, int stride_l, const float* const* ys, int y_dim,
-                           int bsz, float* dout) {
+                           int bsz, float* dout, const float* cw) {
   const int L = net.layers(), d = net.dims[L];
   double value = 0.0;
   for (int s = 0; s < bsz; ++s) {
     const float* out = acts + (int64_t)s * stride_b + (int64_t)L * stride_l;
     float* dz = dout + (int64_t)s * d;
     const float* y = ys[s];
+    const float r = cw ? cw[(int)y[0]] : 1.f;
     if (loss == XENT) {
       const int label = (int)y[0];
       float mx = out[0];
@@ -111,17 +114,21 @@ __attribute__((always_inline)) inline float loss_and_dout(const Net& net, int lo
       float se = 0.f;
       for (int j = 0; j < d; ++j) se += std::exp(out[j] - mx);
       const float lse = mx + std::log(se);
-      value += (double)(lse - out[label >= 0 && label < d ? label : 0]);
-      for (int j = 0; j < d; ++j) dz[j] = (std::exp(out[j] - lse) - (j == label ? 1.f : 0.f)) / (float)bsz;
+      const float term = lse - out[label >= 0 && label < d ? label : 0];
+      value += (double)(cw ? r * term : term);
+      for (int j = 0; j < d; ++j) {
+        const float g = (std::exp(out[j] - lse) - (j == label ? 1.f : 0.f)) / (float)bsz;
+        dz[j] = cw ? g * r : g;
+      }
     } else if (loss == BCE) {
-      const float inv = 1.f / (float)(bsz * d);
+      const float inv0 = 1.f / (float)(bsz * d), inv = cw ? inv0 * r : inv0;
       for (int j = 0; j < d; ++j) {
         const float p = out[j], t = y_dim >= d ? y[j] : y[0];
         value -= (double)(t * clamp_log(std::log(p)) + (1.f - t) * clamp_log(std::log1p(-p))) * inv;
         dz[j] = (p - t) * inv;
       }
     } else {   // SSE / MSE
-      const float scale = loss == SSE ? 1.f : 1.f / (float)bsz;
+      const float scale0 = loss == SSE ? 1.f : 1.f / (float)bsz, scale = cw ? scale0 * r : scale0;
       for (int j = 0; j < d; ++j) {
         const float diff = out[j] - (y_dim >= d ? y[j] : y[0]);
         value += (double)(diff * diff * scale);
@@ -166,7 +173,7 @@ void run_fit(const Net& net, Task& t, const Hyper& hp, Scratch& sc) {
         forward_one(net, theta, t.x + (int64_t)idx * net.dims[0], sc.acts.data() + (int64_t)s * stride_b, stride_l);
         ys[s] = t.y + (int64_t)idx * t.y_dim;
       }
-      t.last = loss_and_dout(net, hp.loss, sc.acts.data(), stride_b, stride_l, ys.data(), t.y_dim, bsz, sc.dout.data());
+      t.last = loss_and_dout(net, hp.loss, sc.acts.data(), stride_b, stride_l, ys.data(), t.y_dim, bsz, sc.dout.data(), hp.cw);
       loss_sum += t.last;
       if (B > 1) std::fill(sc.grad.begin(), sc.grad.end(), 0.f);
       for (int s = 0; s < bsz; ++s) {
@@ -310,7 +317,7 @@ COLEARN_CLONES void run_fit_fixed(const Net& net, Task& t, const Hyper& hp, Scra
       std::memcpy(acts[0], t.x + (int64_t)idx * S::dims[0], sizeof(float) * S::dims[0]);
       fixed_forward<S, 0>(theta, acts, net.sigmoid_out);
       const float* y = t.y + (int64_t)idx * t.y_dim;
-      t.last = loss_and_dout(net, hp.loss, &acts[0][0], (L + 1) * MD, MD, &y, t.y_dim, 1, sc.dout.data());
+      t.last = loss_and_dout(net, hp.loss, &acts[0][0], (L + 1) * MD, MD, &y, t.y_dim, 1, sc.dout.data(), hp.cw);
       loss_sum += t.last;
       std::memcpy(dz, sc.dout.data(), sizeof(float) * S::dims[L]);
       fixed_backward<S, L - 1>(theta, acts, dz, dprev, hp.lr);
@@ -360,10 +367,11 @@ Task make_task(const Net& net, const torch::Tensor& theta, const torch::Tensor& 
 }
 
 // K clients, each trained in place on its own arena, min(K, threads) at a time.  Returns [K, 2] = {last, mean} losses.
-torch::Tensor mlp_local_sgd_host(std::vector<int64_t> dims, bool sigmoid_out, std::vector<torch::Tensor> thetas,
-                                 std::vector<torch::Tensor> xs, std::vector<torch::Tensor> ys,
-                                 std::vector<c10::optional<torch::Tensor>> perms, int64_t batch_size, int64_t epochs,
-                                 int64_t max_nr_batches, int64_t loss, double lr, int64_t threads) {
+// class_weights (mlp_local_sgd_cw): one weight per class; every row's label y[0] must be a class index below their count.
+torch::Tensor fit_host(std::vector<int64_t> dims, bool sigmoid_out, std::vector<torch::Tensor> thetas,
+                       std::vector<torch::Tensor> xs, std::vector<torch::Tensor> ys,
+                       std::vector<c10::optional<torch::Tensor>> perms, int64_t batch_size, int64_t epochs,
+                       int64_t max_nr_batches, int64_t loss, double lr, int64_t threads, const std::vector<double>* class_weights) {
   const Net net(dims, sigmoid_out);
   const size_t K = thetas.size();
   TORCH_CHECK(K >= 1 && xs.size() == K && ys.size() == K && perms.size() == K, "one theta / x / y / perm per client");
@@ -374,7 +382,17 @@ torch::Tensor mlp_local_sgd_host(std::vector<int64_t> dims, bool sigmoid_out, st
     tasks.push_back(make_task(net, thetas[i], xs[i], ys[i], perms[i]));
     if (loss == XENT) TORCH_CHECK(tasks.back().y_dim >= 1, "xent needs a label column");
   }
-  const Hyper hp{(int)batch_size, (int)epochs, (int)max_nr_batches, (int)loss, (float)lr};
+  std::vector<float> cw;
+  if (class_weights != nullptr) {
+    for (double w : *class_weights) cw.push_back((float)w);
+    TORCH_CHECK(!cw.empty(), "no class weights");
+    for (const Task& t : tasks)
+      for (int i = 0; i < t.n; ++i) {
+        const float c = t.y[(int64_t)i * t.y_dim];
+        TORCH_CHECK(c >= 0.f && c < (float)cw.size() && c == (float)(int)c, "label of row ", i, " is not a class index below ", cw.size());
+      }
+  }
+  const Hyper hp{(int)batch_size, (int)epochs, (int)max_nr_batches, (int)loss, (float)lr, class_weights ? cw.data() : nullptr};
   int nthreads = threads > 0 ? (int)threads : (int)std::thread::hardware_concurrency();
   nthreads = std::max(1, std::min<int>(nthreads, (int)K));
   {
@@ -399,6 +417,18 @@ torch::Tensor mlp_local_sgd_host(std::vector<int64_t> dims, bool sigmoid_out, st
     o[2 * i + 1] = tasks[i].mean;
   }
   return out;
+}
+torch::Tensor mlp_local_sgd_host(std::vector<int64_t> dims, bool sigmoid_out, std::vector<torch::Tensor> thetas,
+                                 std::vector<torch::Tensor> xs, std::vector<torch::Tensor> ys,
+                                 std::vector<c10::optional<torch::Tensor>> perms, int64_t batch_size, int64_t epochs,
+                                 int64_t max_nr_batches, int64_t loss, double lr, int64_t threads) {
+  return fit_host(dims, sigmoid_out, thetas, xs, ys, perms, batch_size, epochs, max_nr_batches, loss, lr, threads, nullptr);
+}
+torch::Tensor mlp_local_sgd_cw_host(std::vector<int64_t> dims, bool sigmoid_out, std::vector<torch::Tensor> thetas,
+                                    std::vector<torch::Tensor> xs, std::vector<torch::Tensor> ys,
+                                    std::vector<c10::optional<torch::Tensor>> perms, int64_t batch_size, int64_t epochs,
+                                    int64_t max_nr_batches, int64_t loss, double lr, int64_t threads, std::vector<double> class_weights) {
+  return fit_host(dims, sigmoid_out, thetas, xs, ys, perms, batch_size, epochs, max_nr_batches, loss, lr, threads, &class_weights);
 }
 
 // Batched forward (inference / evaluation): out [n, d_out], post output-activation
@@ -425,5 +455,6 @@ torch::Tensor mlp_forward_host(std::vector<int64_t> dims, bool sigmoid_out, torc
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "colearn host executor: MLP local SGD / forward on CPU devices (no CUDA dependency)";
   m.def("mlp_local_sgd", &mlp_local_sgd_host);
+  m.def("mlp_local_sgd_cw", &mlp_local_sgd_cw_host);
   m.def("mlp_forward", &mlp_forward_host);
 }

@@ -148,6 +148,8 @@ template <class N> struct HeadCfg {
   static constexpr int FW = Offs<N, LI>::flat;
   static constexpr int FB = Offs<N, LI>::flat + DO * K;
   static constexpr bool kFused = (N::DOUT <= kFusedHeadMax) && (N::L >= 2);
+  // classes of a class-weighted fit (CW): the label 0 / 1 of a one-output sigmoid head, the class index of a softmax head
+  static constexpr int NCW = (DO == 1) ? 2 : DO;
 };
 
 template <class N, int LI, bool ACC>
@@ -523,12 +525,41 @@ __device__ __forceinline__ float rcp_approx(float x) {
 }
 #endif
 
+// CW: the weight of the row's class (its label yrow[0]: the FFNN's 0 / 1, the class index of a softmax head), by compare-and-select
+// over the compile-time class index (a dynamically indexed register array would go to local memory).  The kernel calls it at the
+// top of the step, as soon as the row is in shared memory, so that nothing of the step's forward pass waits for it.
+template <class N>
+__device__ __forceinline__ float class_weight(const float* cw, const float* yrow) {
+  const int cls = (int)yrow[0];
+  float wc = cw[0];
+#pragma unroll
+  for (int c = 1; c < HeadCfg<N>::NCW; ++c) wc = (cls == c) ? cw[c] : wc;
+  return wc;
+}
+// a * b rounded to fp32 before any add: the loss statistics of the class-weighted kernels add the product the way the unweighted
+// ones add v * inv_b (which the compiler does not fuse into an FMA), so that w = 1 gives their bits
+#ifdef COLEARN_HOST_SHIM
+inline float mul_rn(float a, float b) { return a * b; }
+#else
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+#endif
+
 // logits (all-reduced inside every warp) -> dz_L in registers of every thread; returns the loss (valid on tid 0)
-template <class N, bool ACC>
+// CW (class-weighted fit, docs/KERNELS.md §5d): the row's factor s = wc * inv_b (sse: wc), wc = class_weight(), stands where inv_b
+// (sse: the implicit 1) stands without weights, in dz_L and — through *s_out, which the caller multiplies the returned loss with —
+// in the loss statistics.  Without CW, sc = inv_b and sc1 = 1: the expressions of the unweighted kernels.
+template <class N, bool ACC, bool CW = false>
 __device__ __forceinline__ float head_forward_loss(HeadRegs<N, ACC>& H, const float* __restrict__ a_in,
                                                    const float* __restrict__ yrow, int loss, float inv_b,
-                                                   float (&dzh)[HeadCfg<N>::DO], int lane, int tid) {
+                                                   float (&dzh)[HeadCfg<N>::DO], int lane, int tid,
+                                                   float wc = 1.f, float* s_out = nullptr) {
   using C = HeadCfg<N>;
+  float sc = inv_b, sc1 = 1.f;
+  if constexpr (CW) {
+    sc = wc * inv_b;
+    sc1 = wc;
+    *s_out = (loss == LOSS_SSE) ? wc : sc;
+  }
   float z[C::DO];
 #pragma unroll
   for (int c = 0; c < C::DO; ++c) z[c] = 0.f;
@@ -591,7 +622,7 @@ __device__ __forceinline__ float head_forward_loss(HeadRegs<N, ACC>& H, const fl
       }
       const float r = rcp_approx(s);   // s in [1, DO]
 #pragma unroll
-      for (int c = 0; c < C::DO; ++c) dzh[c] = (e[c] * r - (label == c ? 1.f : 0.f)) * inv_b;
+      for (int c = 0; c < C::DO; ++c) dzh[c] = (e[c] * r - (label == c ? 1.f : 0.f)) * sc;
       value = (__logf(s) + m) - zy;   // (every thread: see below)
     } else {
       const float d = (C::DO == 2) ? z[C::DO - 1] - z[0] : 0.f;
@@ -615,16 +646,16 @@ __device__ __forceinline__ float head_forward_loss(HeadRegs<N, ACC>& H, const fl
         const float r1 = rcp_approx(1.f + e);
         const float out = zz >= 0.f ? r1 : e * r1;
         if (loss == LOSS_BCE) {
-          dzh[c] = (out - y) * inv_b * (1.f / C::DO);
+          dzh[c] = (out - y) * sc * (1.f / C::DO);
           value += (fmaxf(zz, 0.f) + __logf(1.f + e) - y * zz) * (1.f / C::DO);
         } else {
           const float df = out - y;
-          dzh[c] = 2.f * df * out * (1.f - out) * ((loss == LOSS_MSE) ? inv_b : 1.f);
+          dzh[c] = 2.f * df * out * (1.f - out) * ((loss == LOSS_MSE) ? sc : sc1);
           value += df * df;
         }
       } else {
         const float df = zz - y;
-        dzh[c] = 2.f * df * ((loss == LOSS_MSE) ? inv_b : 1.f);
+        dzh[c] = 2.f * df * ((loss == LOSS_MSE) ? inv_b : 1.f);   // (no weighted instance has this head)
         value += df * df;
       }
     }
@@ -800,267 +831,28 @@ __host__ __device__ constexpr int stage_offset2() {
   return (((BLK ? 4 : 3) * ATot<N>::v + 2 * CHUNK * Totals<N>::ROW_MAX + 8 + 2 * CHUNK) + 3) / 4 * 4;
 }
 
+// The local fit of one client per CTA.  Its body (mlp_v2_fit.inc) is spelled out in each kernel rather than called as an inline
+// function: inlined from a function, the accumulating MLP64 instances get other PTX register numbers, and with them other
+// SASS.  CW: class-weighted fit, only in mlp_persistent_cw.cu (see head_forward_loss).
 template <class N, bool ACC>
 __global__ void __launch_bounds__(NT2, 1)
 mlp_local_sgd_kernel_v2(const ClientDesc* __restrict__ descs, SgdHyper hp) {
-  using Tot = Totals<N>;
-  constexpr int DIN = N::DIN, ROWM = Tot::ROW_MAX;
-  constexpr int EPT2 = (CHUNK * ROWM + NT2 - 1) / NT2;
-  constexpr int ACTS = ATot<N>::v;
-  COLEARN_DYN_SMEM(float, smem);
-  const ClientDesc d = descs[blockIdx.x];
-  const int tid = threadIdx.x;
-  const int B = hp.batch_size < 1 ? 1 : hp.batch_size;
-
-  float* sAct = smem;                       // 2 x ACTS (double buffered by step parity)
-  float* sDz = sAct + 2 * ACTS;             // ACTS (blocked variant: + ACTS of scale * dz right behind)
-  float* sData = sDz + (BLK ? 2 : 1) * ACTS;   // 2 x CHUNK x ROWM
-  float* sMisc = sData + 2 * CHUNK * ROWM;  // [0] last loss, [1] loss sum
-  // Two forms of the gather's index lookup, chosen per net (docs/KERNELS.md §2): RING = one thread per sample resolves the
-  // index two chunks ahead into a shared-memory ring (the 4-layer nets, with the keyed order computed right there); otherwise
-  // every gathering thread reads the order table itself (the 64-wide MLP)
-  constexpr bool RING = (N::L >= 4);
-  int* sIdx = reinterpret_cast<int*>(sMisc + 8);   // RING: 2 x CHUNK sample indices
-
-  const int n = d.n, ydim = d.y_dim, row = DIN + ydim;
-  // An empty shard (trailing virtual clients of a short one, see shard_bounds) gets Q = 0 (spe counts it as one step per
-  // epoch of 0 samples): no steps and no loads from x, y or perm; the write-out stores out_scale * theta_in (0 in delta
-  // mode), the losses are {0, 0}, the flags work as usual.
-  const int spe = ((n > 0 ? n : 1) + B - 1) / B;
-  long long total_steps = (long long)hp.epochs * spe;
-  if (hp.max_steps > 0 && hp.max_steps < total_steps) total_steps = hp.max_steps;
-  long long Q;
-  {
-    const long long full_epochs = total_steps / spe;
-    long long rem_samples = (total_steps - full_epochs * spe) * B;
-    if (rem_samples > n) rem_samples = n;
-    Q = full_epochs * (long long)n + rem_samples;
-  }
-  const int n_chunks = (int)((Q + CHUNK - 1) / CHUNK);
-
-  // Sample order.  d.perm: a caller-made table.  d.perm_seed: the kernel makes the table ITSELF, right here — all threads
-  // fill d.perm_scratch with the keyed Feistel bijection of every epoch this fit will touch (the shuffle of the reference's
-  // loaders: no separate launch, no host round trip, and it runs while the broadcast this client waits for is still in
-  // flight).  The gather below then reads either table with plain (coherent) loads.
-  const int* perm_tab = d.perm;
-  int perm_rows = d.perm_rows;
-  const FeistelDomain fdom = feistel_domain((uint32_t)(n > 0 ? n : 1));
-  if (!RING && d.perm == nullptr && d.perm_seed != 0 && d.perm_scratch != nullptr && n > 0) {
-    const int rows = (int)((Q + n - 1) / n);
-    const long long total = (long long)rows * n;
-    for (long long e = tid; e < total; e += NT2) {
-      const int r = (int)(e / n);
-      d.perm_scratch[e] = (int)feistel_index((uint32_t)(e - (long long)r * n), (uint32_t)n, fdom, d.perm_seed, d.perm_row0 + r);
-    }
-    __syncthreads();
-    perm_tab = d.perm_scratch;
-    perm_rows = rows > 0 ? rows : 1;
-  }
-  // only now wait for this round's broadcast and pull the model into registers
-  if (d.wait_flag != nullptr) {
-    if (tid == 0) spin_wait_ge(d.wait_flag, d.wait_value, 32, "mlp_local_sgd: broadcast flag of this round");
-    __syncthreads();
-  }
-  AllRegs<N, 0, ACC> W;
-  load_regs<N, 0, ACC>(W, d.theta_in, tid);
-  HeadRegs<N, ACC> H;
-  if constexpr (HeadCfg<N>::kFused) head_load<N, ACC>(H, d.theta_in, tid & 31);
-  if (tid < 2) sMisc[tid] = 0.f;
-  float last_loss = 0.f, loss_sum = 0.f;   // blocked variant and batch 1: thread 0 keeps the loss statistics in registers (it is their only reader)
-  auto sample_index = [&](long long q) -> int {
-    const int ep = (int)(q / n);
-    const int pos = (int)(q - (long long)ep * n);
-    if (perm_tab) return __ldcg(perm_tab + (size_t)(ep % perm_rows) * n + pos);
-    if (RING && d.perm_seed) return (int)feistel_index((uint32_t)pos, (uint32_t)n, fdom, d.perm_seed, d.perm_row0 + ep);
-    return pos;
-  };
-  auto compute_indices = [&](int chunk) {      // RING only: threads 0 .. CHUNK-1, one sample each
-    if (tid < CHUNK) {
-      const long long q = (long long)chunk * CHUNK + tid;
-      sIdx[(chunk & 1) * CHUNK + tid] = q < Q ? sample_index(q) : 0;
-    }
-  };
-  float pre[EPT2];
-  auto issue_loads = [&](int chunk) {
-    const int* order = sIdx + (chunk & 1) * CHUNK;
+  constexpr bool CW = false;
+  const float* const cw = nullptr;
+#include "mlp_v2_fit.inc"
+}
+// The class-weighted instances: the weights travel by value as a kernel argument of their own and are held in registers for the
+// whole fit.
+template <class N, bool ACC>
+__global__ void __launch_bounds__(NT2, 1)
+mlp_local_sgd_kernel_v2_cw(const ClientDesc* __restrict__ descs, SgdHyper hp, ClassWeights cwa) {
+  static_assert(HeadCfg<N>::kFused, "class weights act in the fused head");
+  constexpr bool CW = true;
+  float cwr[HeadCfg<N>::NCW];
 #pragma unroll
-    for (int j = 0; j < EPT2; ++j) {
-      const int e = tid + j * NT2;
-      pre[j] = 0.f;
-      if (e < CHUNK * row) {
-        const int i = e / row, c = e - i * row;
-        const long long q = (long long)chunk * CHUNK + i;
-        if (q < Q) {
-          const int idx = RING ? order[i] : sample_index(q);
-          pre[j] = (c < DIN) ? __ldg(d.x + (size_t)idx * DIN + c) : __ldg(d.y + (size_t)idx * ydim + (c - DIN));
-        }
-      }
-    }
-  };
-  auto store_loads = [&](int buf) {
-    float* dst = sData + buf * (CHUNK * ROWM);
-#pragma unroll
-    for (int j = 0; j < EPT2; ++j) {
-      const int e = tid + j * NT2;
-      if (e < CHUNK * row) dst[e] = pre[j];
-    }
-  };
-  if constexpr (RING) {
-    if (n_chunks > 0) compute_indices(0);
-    if (n_chunks > 1) compute_indices(1);
-    __syncthreads();
-  }
-  if (n_chunks > 0) { issue_loads(0); store_loads(0); }
-  __syncthreads();
-
-  long long step = 0;
-  int pos_in_epoch = 0, in_batch = 0;
-  int cur_batch = (n < B) ? n : B;
-  float batch_loss = 0.f;
-  int parity = 0;
-  const float neg_lr = -hp.lr;
-  // Batch 1 (ACC == false): every sample is an SGD step, so the step body carries none of the batch bookkeeping, and the rank-1
-  // updates that nothing on the dependent chain waits for — both copies of layer 1 and the head — move out of the tail of their
-  // step, where they stood in-order between dz_1 and the next step's first loads (docs/KERNELS.md §2):
-  //   * the row copy of layer 1 and the head go to the top of the next step, in one basic block with the layer-0 forward, and
-  //     fill the latency of its sample loads (layer 1's forward reads the row copy right after the first barrier);
-  //   * the column copy of layer 1 goes behind that barrier, where its loads and FMAs fill the latency of the layer-1 forward
-  //     and the head (its first reader is the dgrad of layer 1).
-  // Same operands, same FMA per weight: the model is bit-identical.  The first step of a chunk has nothing pending; the last
-  // one's updates are issued after the chunk's steps.
-  constexpr bool DEFER = !ACC && HeadCfg<N>::kFused && N::L >= 3;
-  float dzh_last[HeadCfg<N>::DO];   // batch 1: dz_L of the last step (DEFER: its head update is pending)
-#pragma unroll
-  for (int j = 0; j < HeadCfg<N>::DO; ++j) dzh_last[j] = 0.f;
-  float ak1_last = 0.f;              // DEFER: a_1[k] of the last step, input of the pending column-copy update
-  auto deferred_before_fwd0 = [&]() {
-    if constexpr (DEFER) {
-      bwd1_deferred<N, false, true>(W, 0.f, sDz, neg_lr, tid);
-      head_update<N, ACC>(H, dzh_last, neg_lr);
-    }
-  };
-  auto deferred_after_fwd0 = [&]() {
-    if constexpr (DEFER) bwd1_deferred<N, true, false>(W, ak1_last, sDz, neg_lr, tid);
-  };
-
-  for (int c = 0; c < n_chunks; ++c) {
-    if (c + 1 < n_chunks) issue_loads(c + 1);
-    if constexpr (RING) {
-      if (c + 2 < n_chunks) compute_indices(c + 2);      // slot c & 1: chunk c's indices were consumed one iteration ago
-    }
-    const float* chunk = sData + (c & 1) * (CHUNK * ROWM);
-    const long long q0 = (long long)c * CHUNK;
-    const int cnt = (int)((Q - q0) < CHUNK ? (Q - q0) : CHUNK);
-    if constexpr (!ACC) {
-      auto train_step = [&](auto pending, int i) {
-        if constexpr (decltype(pending)::value) deferred_before_fwd0();
-        const float* a0 = chunk + i * row;
-        float* acts = sAct + parity * ACTS;
-        static_assert(!RL<N, 0>::REP, "layer 0 publishes its outputs through a block barrier");
-        fwd<N, 0, ACC>(W, a0, acts + AOff<N, 0>::v, tid);
-        __syncthreads();
-        if constexpr (decltype(pending)::value) deferred_after_fwd0();
-        Fwd2<N, 1, ACC>::run(W, a0, acts, tid);
-        float v = 0.f;
-        if constexpr (HeadCfg<N>::kFused) {
-          constexpr int LH = N::L - 1;
-          const float* a_head = acts + AOff<N, LH - 1>::v + (RL<N, LH - 1>::REP ? (tid >> 5) * RL<N, LH - 1>::RSTRIDE : 0);
-          v = head_forward_loss<N, ACC>(H, a_head, a0 + DIN, hp.loss, 1.f, dzh_last, tid & 31, tid);
-          head_backward<N, ACC, !DEFER>(W, H, dzh_last, a_head, sDz + AOff<N, LH - 1>::v, neg_lr, tid);
-          if constexpr (RL<N, LH - 1>::REP) __syncwarp();
-          else __syncthreads();
-          Bwd2<N, LH - 1, ACC, DEFER>::run(W, a0, acts, sDz, neg_lr, tid, &ak1_last);
-        } else {
-          if (tid < 32) v = loss_and_dz<N>(acts + AOff<N, N::L - 1>::v, sDz + AOff<N, N::L - 1>::v, a0 + DIN, hp.loss, 1.f, tid);
-          __syncthreads();
-          Bwd2<N, N::L - 1, ACC>::run(W, a0, acts, sDz, neg_lr, tid);
-        }
-        parity ^= 1;
-        const float step_loss = 0.f + v;   // the sum the batch path forms (a -0 loss reports as +0); thread 0's copy is reported
-        last_loss = step_loss;
-        loss_sum += step_loss;
-      };
-      if constexpr (DEFER) {
-        train_step(std::false_type{}, 0);
-        for (int i = 1; i < cnt; ++i) train_step(std::true_type{}, i);
-        deferred_before_fwd0();
-        deferred_after_fwd0();
-      } else {
-        for (int i = 0; i < cnt; ++i) train_step(std::false_type{}, i);
-      }
-    } else for (int i = 0; i < cnt; ++i) {
-      const float* a0 = chunk + i * row;
-      float* acts = sAct + parity * ACTS;
-      const float inv_b = 1.f / (float)cur_batch;
-
-      Fwd2<N, 0, ACC>::run(W, a0, acts, tid);
-      if constexpr (HeadCfg<N>::kFused) {
-        constexpr int LH = N::L - 1;
-        // a_{L-1}, published by the last barrier (or by this warp itself: RL::REP)
-        const float* a_head = acts + AOff<N, LH - 1>::v + (RL<N, LH - 1>::REP ? (tid >> 5) * RL<N, LH - 1>::RSTRIDE : 0);
-        float dzh[HeadCfg<N>::DO];
-        const float v = head_forward_loss<N, ACC>(H, a_head, a0 + DIN, hp.loss, inv_b, dzh, tid & 31, tid);
-        batch_loss += (hp.loss == LOSS_SSE) ? v : v * inv_b;     // (all threads: thread 0's copy is the one that is reported)
-        head_backward<N, ACC>(W, H, dzh, a_head, sDz + AOff<N, LH - 1>::v, neg_lr, tid);
-        if constexpr (RL<N, LH - 1>::REP) __syncwarp();            // dz_{L-1}: this warp's slot, read back by this warp
-        else __syncthreads();                                      // dz_{L-1} visible
-        Bwd2<N, LH - 1, ACC>::run(W, a0, acts, sDz, neg_lr, tid);
-      } else {
-        if (tid < 32) {
-          const float v = loss_and_dz<N>(acts + AOff<N, N::L - 1>::v, sDz + AOff<N, N::L - 1>::v, a0 + DIN, hp.loss, inv_b, tid);
-          if (tid == 0) batch_loss += (hp.loss == LOSS_SSE) ? v : v * inv_b;
-        }
-        __syncthreads();
-        Bwd2<N, N::L - 1, ACC>::run(W, a0, acts, sDz, neg_lr, tid);
-      }
-      parity ^= 1;
-
-      ++in_batch;
-      ++pos_in_epoch;
-      if (in_batch == cur_batch) {
-        if (ACC) { apply_grads<N, 0, ACC>(W, neg_lr); if constexpr (HeadCfg<N>::kFused) head_apply_grads<N, ACC>(H, neg_lr); }
-        if (BLK) { last_loss = batch_loss; loss_sum += batch_loss; batch_loss = 0.f; }
-        else if (tid == 0) { sMisc[0] = batch_loss; sMisc[1] += batch_loss; batch_loss = 0.f; }
-        ++step;
-        in_batch = 0;
-        if (pos_in_epoch >= n) pos_in_epoch = 0;
-        const int left = n - pos_in_epoch;
-        cur_batch = left < B ? left : B;
-      }
-    }
-    __syncthreads();
-    if (c + 1 < n_chunks) store_loads((c + 1) & 1);
-    __syncthreads();
-  }
-  if constexpr (!ACC) step = Q;
-  __syncthreads();
-  // Write-out.  The registers hold the model in the layers' lane mappings (lane t of a row owns a blocked or strided slice of
-  // it): stored from there, every 4-byte store is its own 32-byte NVLink packet when theta_out is a coordinator's slot on
-  // another GPU.  STAGED: the same stores (scale and delta included) target a staging area in shared memory — a generic
-  // pointer, same ST.E instructions — and the model leaves as 16-byte vectors, 512 contiguous bytes per warp instruction.
-  // ptxas schedules the training loop of the 64-wide MLP differently as soon as this epilogue changes, so the 3-layer nets
-  // keep the direct stores.
-  constexpr bool STAGED = (N::L >= 4);
-  if constexpr (STAGED) {
-    float* sOut = smem + stage_offset2<N>();
-    store_regs<N, 0, ACC>(W, d.theta_in, sOut, d.out_scale, d.delta_mode, tid);
-    if constexpr (HeadCfg<N>::kFused) head_store<N, ACC>(H, d.theta_in, sOut, d.out_scale, d.delta_mode, tid);
-    __syncthreads();
-    write_out_staged(sOut, d.theta_out, Tot::flat_params, tid);
-  } else {
-    store_regs<N, 0, ACC>(W, d.theta_in, d.theta_out, d.out_scale, d.delta_mode, tid);
-    if constexpr (HeadCfg<N>::kFused) head_store<N, ACC>(H, d.theta_in, d.theta_out, d.out_scale, d.delta_mode, tid);
-  }
-  if (tid == 0 && d.loss_out != nullptr) {
-    constexpr bool REG = BLK || !ACC;   // loss statistics kept in registers
-    d.loss_out[0] = REG ? last_loss : sMisc[0];
-    d.loss_out[1] = step > 0 ? (REG ? loss_sum : sMisc[1]) / (float)step : 0.f;
-  }
-  __syncthreads();
-  if (tid == 0 && d.signal_flag != nullptr) {
-    __threadfence_system();
-    st_release_sys(d.signal_flag, d.signal_value);
-  }
+  for (int c = 0; c < HeadCfg<N>::NCW; ++c) cwr[c] = cwa.w[c];
+  const float* const cw = cwr;
+#include "mlp_v2_fit.inc"
 }
 
 template <class N>
@@ -1073,6 +865,14 @@ cudaError_t launch2(const ClientDesc* descs, int n_clients, SgdHyper hp, cudaStr
   // (launched through a pointer: a template-id with a comma cannot travel through the launch macro)
   void (*kern)(const ClientDesc*, SgdHyper) = hp.batch_size > 1 ? mlp_local_sgd_kernel_v2<N, true> : mlp_local_sgd_kernel_v2<N, false>;
   COLEARN_LAUNCH(kern, n_clients, NT2, bytes, stream, descs, hp);
+  return cudaGetLastError();
+}
+template <class N>
+cudaError_t launch2_cw(const ClientDesc* descs, int n_clients, SgdHyper hp, ClassWeights cw, cudaStream_t stream) {
+  const int bytes = smem_bytes2<N>();
+  void (*kern)(const ClientDesc*, SgdHyper, ClassWeights) =
+      hp.batch_size > 1 ? mlp_local_sgd_kernel_v2_cw<N, true> : mlp_local_sgd_kernel_v2_cw<N, false>;
+  COLEARN_LAUNCH(kern, n_clients, NT2, bytes, stream, descs, hp, cw);
   return cudaGetLastError();
 }
 

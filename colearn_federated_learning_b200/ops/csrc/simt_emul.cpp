@@ -19,10 +19,11 @@ const float* fptr(const Tensor& t, const char* name) {
 
 // K clients (one emulated CTA each, run one after the other).  theta_outs[i] may alias theta_in.
 // Returns losses [K, 2] = {last, mean}; flags (int32 [K], optional) receive signal_value = 7 + i.
-Tensor mlp_local_sgd(int64_t net_kind, Tensor theta_in, std::vector<Tensor> theta_outs, std::vector<Tensor> xs, std::vector<Tensor> ys,
-                     std::vector<c10::optional<Tensor>> perms, int64_t batch_size, int64_t epochs, int64_t max_steps, int64_t loss,
-                     double lr, int64_t variant, std::vector<double> out_scales, bool delta_mode, c10::optional<Tensor> flags,
-                     int64_t perm_seed, int64_t perm_row0, c10::optional<Tensor> perm_scratch) {
+// class_weights (mlp_local_sgd_cw): the class-weighted instances of mlp_persistent_cw.cu; nullptr: the unweighted ones.
+Tensor mlp_fit(int64_t net_kind, Tensor theta_in, std::vector<Tensor> theta_outs, std::vector<Tensor> xs, std::vector<Tensor> ys,
+               std::vector<c10::optional<Tensor>> perms, int64_t batch_size, int64_t epochs, int64_t max_steps, int64_t loss,
+               double lr, int64_t variant, std::vector<double> out_scales, bool delta_mode, c10::optional<Tensor> flags,
+               int64_t perm_seed, int64_t perm_row0, c10::optional<Tensor> perm_scratch, const std::vector<double>* class_weights) {
   const size_t K = xs.size();
   TORCH_CHECK(K >= 1 && ys.size() == K && perms.size() == K && theta_outs.size() == K && out_scales.size() == K, "one entry per client");
   const int P = colearn::mlp_net_num_params((int)net_kind);
@@ -73,10 +74,31 @@ Tensor mlp_local_sgd(int64_t net_kind, Tensor theta_in, std::vector<Tensor> thet
   hp.variant = (int)variant;
   {
     py::gil_scoped_release nogil;
-    cudaError_t e = colearn::launch_mlp_local_sgd((int)net_kind, descs.data(), (int)K, hp, nullptr);
+    cudaError_t e;
+    if (class_weights != nullptr) {
+      colearn::ClassWeights cw{};
+      TORCH_CHECK(class_weights->size() <= 8, "at most 8 class weights");
+      for (size_t c = 0; c < class_weights->size(); ++c) cw.w[c] = (float)(*class_weights)[c];
+      e = colearn::launch_mlp_local_sgd_cw((int)net_kind, descs.data(), (int)K, hp, cw, nullptr);
+    } else {
+      e = colearn::launch_mlp_local_sgd((int)net_kind, descs.data(), (int)K, hp, nullptr);
+    }
     TORCH_CHECK(e == cudaSuccess, "launch_mlp_local_sgd (host shim) failed");
   }
   return losses;
+}
+Tensor mlp_local_sgd(int64_t net_kind, Tensor theta_in, std::vector<Tensor> theta_outs, std::vector<Tensor> xs, std::vector<Tensor> ys,
+                     std::vector<c10::optional<Tensor>> perms, int64_t batch_size, int64_t epochs, int64_t max_steps, int64_t loss,
+                     double lr, int64_t variant, std::vector<double> out_scales, bool delta_mode, c10::optional<Tensor> flags,
+                     int64_t perm_seed, int64_t perm_row0, c10::optional<Tensor> perm_scratch) {
+  return mlp_fit(net_kind, theta_in, theta_outs, xs, ys, perms, batch_size, epochs, max_steps, loss, lr, variant, out_scales, delta_mode,
+                 flags, perm_seed, perm_row0, perm_scratch, nullptr);
+}
+Tensor mlp_local_sgd_cw(int64_t net_kind, Tensor theta_in, std::vector<Tensor> theta_outs, std::vector<Tensor> xs, std::vector<Tensor> ys,
+                        std::vector<c10::optional<Tensor>> perms, int64_t batch_size, int64_t epochs, int64_t max_steps, int64_t loss,
+                        double lr, int64_t variant, std::vector<double> out_scales, std::vector<double> class_weights) {
+  return mlp_fit(net_kind, theta_in, theta_outs, xs, ys, perms, batch_size, epochs, max_steps, loss, lr, variant, out_scales, false,
+                 c10::nullopt, 0, 0, c10::nullopt, &class_weights);
 }
 
 Tensor mlp_forward(int64_t net_kind, Tensor theta, Tensor x, int64_t d_out) {
@@ -642,6 +664,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mlp_local_sgd", &mlp_local_sgd, py::arg("net_kind"), py::arg("theta_in"), py::arg("theta_outs"), py::arg("xs"), py::arg("ys"), py::arg("perms"),
         py::arg("batch_size"), py::arg("epochs"), py::arg("max_steps"), py::arg("loss"), py::arg("lr"), py::arg("variant"), py::arg("out_scales"),
         py::arg("delta_mode"), py::arg("flags"), py::arg("perm_seed") = 0, py::arg("perm_row0") = 0, py::arg("perm_scratch") = py::none());
+  m.def("mlp_local_sgd_cw", &mlp_local_sgd_cw);
   m.def("mlp_forward", &mlp_forward);
   m.def("mlp_net_params", [](int64_t kind) { return (int64_t)colearn::mlp_net_num_params((int)kind); });
   m.def("sgd_step", &sgd_step);

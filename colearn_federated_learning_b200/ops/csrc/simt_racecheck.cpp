@@ -55,6 +55,24 @@ int main() {
         CK(launch_mlp_forward(kind, theta.data(), x.data(), o.data(), n, nullptr));
       }
   printf("mlp kernels ok\n");
+  // ---- class-weighted instances (mlp_persistent_cw.cu): FFNN (bce) and the category net (xent), variant 5, batch 1 and 3 ----
+  for (int kind : {0, 4})
+    for (int batch : {1, 3}) {
+      const int P = mlp_net_num_params(kind), n = 7;
+      std::vector<float> theta = randv(P, 0.3f), x = randv((size_t)n * 10), y(n), out0(P), out1(P), loss(4);
+      for (auto& v : y) v = (float)(rand() % (kind == 0 ? 2 : 5));
+      std::vector<ClientDesc> d(2);
+      for (int c = 0; c < 2; ++c) {
+        memset(&d[c], 0, sizeof(ClientDesc));
+        d[c].x = x.data(); d[c].y = y.data(); d[c].theta_in = theta.data();
+        d[c].theta_out = c ? out1.data() : out0.data(); d[c].loss_out = loss.data() + 2 * c;
+        d[c].n = n; d[c].perm_rows = 1; d[c].y_dim = 1; d[c].out_scale = 0.5f;
+      }
+      const ClassWeights cw{{2.f, 0.5f, 1.f, 3.f, 0.f, 0.f, 0.f, 0.f}};
+      SgdHyper hp{batch, 2, -1, kind == 0 ? LOSS_BCE : LOSS_XENT, 0.05f, 5};
+      CK(launch_mlp_local_sgd_cw(kind, d.data(), 2, hp, cw, nullptr));
+    }
+  printf("class-weighted mlp kernels ok\n");
   // ---- elementwise (the ones with shared memory / shuffles / atomics) ----------------------------------------------------------
   {
     const int64_t n = 3000;

@@ -10,6 +10,7 @@ layer-wise trainer (``fl/layerwise.py``).
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass, field
 from typing import Optional, Sequence, Tuple, Union
 
@@ -24,7 +25,11 @@ NET_KINDS = {
     ((10, 32, 4, 32, 10), "none"): 3,     # the anomaly detector's autoencoder (models/mlp.py AE_SPEC)
     ((10, 50, 30, 10, 5), "none"): 4,     # the attack-category FFNN (models/mlp.py FFNN_CAT_SPEC)
 }
-NET_FFNN_CAT = 4
+NET_FFNN, NET_FFNN_CAT = 0, 4
+# Class-weighted fits (csrc/mlp_persistent_cw.cu): net kind -> (classes, losses).  The FFNN's class is its 0 / 1 label, the
+# category net's its class index; the weighted instances exist for variant 5 only.
+CLASS_WEIGHTED = {NET_FFNN: (2, ("bce", "sse", "mse")), NET_FFNN_CAT: (5, ("xent",))}
+CLASS_WEIGHTED_VARIANT = 5
 LOSS_CODES = {"bce": 0, "sse": 1, "xent": 2, "mse": 3}
 # Kernel variants: 5 = register-resident weights, 128-thread CTA, blocked reduction slices (LDS.128) + pre-scaled dz;
 # 6 = 5 with its FMAs written in pairs (Hopper has no packed fp32 FMA: the same FFMA sequence as 5); 3 = strided slices
@@ -111,35 +116,74 @@ def _prep_xy(x: torch.Tensor, y: torch.Tensor, loss: str) -> Tuple[torch.Tensor,
     return x, y
 
 
+def check_class_weights(kind: Optional[int], loss: str, class_weights: Sequence[float], variant: Optional[int] = None,
+                        cuda: bool = True) -> list:
+    """The weights as a list of floats, or ValueError: a class-weighted fit needs a net and loss with weighted instances
+    (:data:`CLASS_WEIGHTED`), on CUDA kernel variant 5 (``variant`` / ``COLEARN_MLP_VARIANT``), and one finite weight >= 0 per
+    class."""
+    if kind not in CLASS_WEIGHTED:
+        raise ValueError("class weights: only the FFNN and the attack-category net have class-weighted kernels")
+    classes, losses = CLASS_WEIGHTED[kind]
+    if loss not in losses:
+        raise ValueError(f"class weights: loss {loss!r} not supported for this net (use {', '.join(losses)})")
+    if cuda and resolve_variant(kind, variant) != CLASS_WEIGHTED_VARIANT:
+        raise ValueError(f"class weights: only kernel variant {CLASS_WEIGHTED_VARIANT} has class-weighted instances, "
+                         f"not {resolve_variant(kind, variant)}")
+    w = [float(v) for v in class_weights]
+    if len(w) != classes:
+        raise ValueError(f"class weights: {len(w)} values for {classes} classes")
+    for c, v in enumerate(w):
+        if not (math.isfinite(v) and v >= 0.0):
+            raise ValueError(f"class weights: weight {v!r} of class {c} is not a finite number >= 0")
+    return w
+
+
 def mlp_local_sgd_multi(dims: Sequence[int], out_activation: str, descs: torch.Tensor, n_clients: int,
                         batch_size: int = 1, lr: float = 0.01, epochs: int = 1, max_nr_batches: int = -1,
-                        loss: str = "xent", desc_offset: int = 0, variant: Optional[int] = None) -> None:
+                        loss: str = "xent", desc_offset: int = 0, variant: Optional[int] = None,
+                        class_weights: Optional[Sequence[float]] = None) -> None:
     """Launch ``n_clients`` CTAs from a packed descriptor tensor (see :func:`build_client_descs`).
 
     The labels behind the descriptors are not checked here (they are device memory the caller packed).  For the
     attack-category net they must be class indices in [0, 5): the kernel stays memory-safe for any other value (its heads
     select z_y by compare-and-select or ``label & 31``), but trains on a wrong gradient.  Every data path that feeds this
-    (the CSV adapter, ``synthetic_category``) validates its codes when it loads them; :func:`mlp_local_sgd` checks them."""
+    (the CSV adapter, ``synthetic_category``) validates its codes when it loads them; :func:`mlp_local_sgd` checks them.  The
+    same holds for the 0 / 1 labels of a class-weighted FFNN fit.
+
+    ``class_weights``: a class-weighted fit (``reference.loss_and_dz``), launched on the weighted instances; the weights, net,
+    loss and variant are checked before the launch (:func:`check_class_weights`)."""
     kind = net_kind_for(dims, out_activation)
     if kind is None:
         raise ValueError(f"no persistent-kernel instantiation for dims={tuple(dims)} act={out_activation}")
     if loss == "bce" and out_activation != "sigmoid":
         raise ValueError("bce needs a sigmoid head")
-    _ext.require().mlp_local_sgd(kind, descs, int(desc_offset), int(n_clients), int(batch_size), int(epochs),
-                                 int(max_nr_batches if max_nr_batches is not None else -1), LOSS_CODES[loss], float(lr),
-                                 resolve_variant(kind, variant))
+    args = (kind, descs, int(desc_offset), int(n_clients), int(batch_size), int(epochs),
+            int(max_nr_batches if max_nr_batches is not None else -1), LOSS_CODES[loss], float(lr), resolve_variant(kind, variant))
+    if class_weights is None:
+        _ext.require().mlp_local_sgd(*args)
+    else:
+        w = check_class_weights(kind, loss, class_weights, variant)
+        _ext.require().mlp_local_sgd_cw(*args, w)
 
 
 def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: torch.Tensor,
                   perm: Optional[torch.Tensor], batch_size: int = 1, lr: float = 0.01, epochs: int = 1,
                   max_nr_batches: int = -1, loss: str = "xent", out_activation: str = "none",
-                  return_mean: bool = False, variant: Optional[int] = None) -> torch.Tensor:
+                  return_mean: bool = False, variant: Optional[int] = None,
+                  class_weights: Optional[Sequence[float]] = None) -> torch.Tensor:
     """Single-client in-place local SGD on ``flat``; returns the last batch loss (0-dim tensor).
 
     CPU tensors run ``reference.mlp_local_sgd`` (identical semantics); CUDA tensors run the
     persistent kernel — there is no silent fallback on CUDA.  The attack-category net refuses, before any launch, a label that
-    is not a class index in [0, 5): the kernel's head selects z_y by that index."""
-    if net_kind_for(dims, out_activation) == NET_FFNN_CAT:
+    is not a class index in [0, 5): the kernel's head selects z_y by that index.
+
+    ``class_weights``: a class-weighted fit (FFNN: 2 weights, for labels 0 and 1; attack-category net: 5), refused before any
+    launch unless :func:`check_class_weights` accepts it and every label is a class index."""
+    kind = net_kind_for(dims, out_activation)
+    if class_weights is not None:
+        class_weights = check_class_weights(kind, loss, class_weights, variant, cuda=flat.is_cuda)
+        check_class_labels(y, len(class_weights))
+    elif kind == NET_FFNN_CAT:
         check_class_labels(y, int(dims[-1]))
     if not flat.is_cuda:
         # CPU devices: the native host executor (csrc/mlp_host.cpp) when it is built and the arena can be trained in
@@ -147,18 +191,20 @@ def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: t
         if (host.available() and flat.dtype == torch.float32 and flat.is_contiguous() and not flat.requires_grad
                 and out_activation in ("none", "sigmoid")):
             res = host.mlp_local_sgd_multi(dims, out_activation, [flat], [x], [y], [perm], batch_size, lr, epochs,
-                                           max_nr_batches, loss, threads=1)
+                                           max_nr_batches, loss, threads=1, class_weights=class_weights)
             return res[0, 1 if return_mean else 0].clone()
         if perm is None:
             perm = reference.make_permutation(x.shape[0], epochs, 0, shuffle=False)
-        return reference.mlp_local_sgd(flat, dims, x, y, perm, batch_size, lr, epochs, max_nr_batches, loss, out_activation)
+        cw = None if class_weights is None else torch.tensor(class_weights, dtype=torch.float32).to(flat.dtype)
+        return reference.mlp_local_sgd(flat, dims, x, y, perm, batch_size, lr, epochs, max_nr_batches, loss, out_activation, cw)
     x, y = _prep_xy(x, y, loss)
     loss_out = torch.zeros(2, device=flat.device, dtype=torch.float32)
     if perm is not None:
         perm = perm.to(flat.device, torch.int32).contiguous()
     task = ClientTask(x=x, y=y, theta_in=flat, theta_out=flat, perm=perm, loss_out=loss_out)
     descs = build_client_descs([task], flat.device)
-    mlp_local_sgd_multi(dims, out_activation, descs, 1, batch_size, lr, epochs, max_nr_batches, loss, variant=variant)
+    mlp_local_sgd_multi(dims, out_activation, descs, 1, batch_size, lr, epochs, max_nr_batches, loss, variant=variant,
+                        class_weights=class_weights)
     return loss_out[1 if return_mean else 0]
 
 

@@ -52,9 +52,13 @@ def mlp_forward(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor,
     return h, acts
 
 
-def loss_and_dz(out: torch.Tensor, y: torch.Tensor, loss: str, out_activation: str
-                ) -> Tuple[torch.Tensor, torch.Tensor]:
+def loss_and_dz(out: torch.Tensor, y: torch.Tensor, loss: str, out_activation: str,
+                class_weights: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Loss value and gradient w.r.t. the last layer's *pre-activation*.
+
+    ``class_weights`` (a class-weighted fit): row i's loss term and its gradient are multiplied by ``w[c_i]``, its class being
+    the label (``y[:, 0]``: the class index for xent, the 0 / 1 label otherwise).  The batch reductions stay what they are
+    (means divide by the batch, not by the sum of the weights), so ``w = 1`` is the unweighted fit.
 
     bce  : mean binary cross-entropy on probabilities (reference remote mode, cf.py:76-79).
            Needs a sigmoid head; log terms are clamped at -100 like ``F.binary_cross_entropy``.
@@ -63,26 +67,35 @@ def loss_and_dz(out: torch.Tensor, y: torch.Tensor, loss: str, out_activation: s
     xent : softmax cross-entropy, integer labels in ``y[:, 0]``, mean over the batch.
     """
     bsz = out.shape[0]
+    r = None                  # [bsz, 1]: the weight of every row's class
+    if class_weights is not None:
+        r = class_weights.to(out.dtype)[y.reshape(bsz, -1)[:, 0].long()].view(bsz, 1)
     if loss == "xent":
         labels = y.reshape(bsz).long()
         lse = torch.logsumexp(out, dim=1)
-        value = (lse - out.gather(1, labels.view(-1, 1)).squeeze(1)).mean()
+        terms = lse - out.gather(1, labels.view(-1, 1)).squeeze(1)
         p = torch.softmax(out, dim=1)
         p = p - torch.nn.functional.one_hot(labels, out.shape[1]).to(p.dtype)
-        return value, p / bsz
+        if r is not None:
+            terms, p = terms * r.view(bsz), p * r
+        return terms.mean(), p / bsz
     y = y.reshape(out.shape).to(out.dtype)
     if loss == "bce":
         if out_activation != "sigmoid":
             raise ValueError("bce needs a sigmoid head")
         logp = torch.clamp(torch.log(out), min=-100.0)
         log1mp = torch.clamp(torch.log1p(-out), min=-100.0)
-        value = -(y * logp + (1 - y) * log1mp).mean()
-        return value, (out - y) / out.numel()
+        terms, dz = -(y * logp + (1 - y) * log1mp), out - y
+        if r is not None:
+            terms, dz = terms * r, dz * r
+        return terms.mean(), dz / out.numel()
     if loss in ("sse", "mse"):
         diff = out - y
         scale = 1.0 if loss == "sse" else 1.0 / bsz
-        value = (diff * diff).sum() * scale
-        dz = 2.0 * diff * scale
+        sq, dz = diff * diff, 2.0 * diff * scale
+        if r is not None:
+            sq, dz = sq * r, dz * r
+        value = sq.sum() * scale
         if out_activation == "sigmoid":
             dz = dz * out * (1 - out)
         return value, dz
@@ -107,9 +120,9 @@ def mlp_backward(flat: torch.Tensor, dims: Sequence[int], acts: List[torch.Tenso
     return grad
 
 
-def mlp_grad(flat, dims, x, y, loss="xent", out_activation="none"):
+def mlp_grad(flat, dims, x, y, loss="xent", out_activation="none", class_weights=None):
     out, acts = mlp_forward(flat, dims, x, out_activation)
-    value, dz = loss_and_dz(out, y, loss, out_activation)
+    value, dz = loss_and_dz(out, y, loss, out_activation, class_weights)
     return value, mlp_backward(flat, dims, acts, dz)
 
 
@@ -134,9 +147,11 @@ def total_steps(n: int, batch_size: int, epochs: int, max_nr_batches: int = -1) 
 
 def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: torch.Tensor,
                   perm: torch.Tensor, batch_size: int = 1, lr: float = 0.01, epochs: int = 1,
-                  max_nr_batches: int = -1, loss: str = "xent", out_activation: str = "none"
-                  ) -> torch.Tensor:
+                  max_nr_batches: int = -1, loss: str = "xent", out_activation: str = "none",
+                  class_weights: Optional[torch.Tensor] = None) -> torch.Tensor:
     """In-place local SGD on the flat arena; returns the last batch's loss (0-dim tensor).
+
+    ``class_weights``: a class-weighted fit (see :func:`loss_and_dz`), the definition the kernels and the host executor follow.
 
     ``max_nr_batches``: PySyft stops when ``it >= max_nr_batches >= 0`` *after* a step, so 0
     behaves like "one step"; negative means unlimited.  We normalise: <= 0 → unlimited except
@@ -149,7 +164,7 @@ def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: t
         order = perm[e % perm.shape[0]].long()
         for lo in range(0, n, batch_size):
             idx = order[lo:lo + batch_size]
-            last, g = mlp_grad(flat, dims, x[idx], y[idx], loss, out_activation)
+            last, g = mlp_grad(flat, dims, x[idx], y[idx], loss, out_activation, class_weights)
             flat.sub_(lr * g)
             it += 1
             if limit is not None and it >= limit:

@@ -96,6 +96,12 @@ def build_parser() -> argparse.ArgumentParser:
                         help="import this module / .py file first: it may call models.register_model / data.register_dataset "
                              "(the reference's 'use your own model/dataset' without editing sources; repeatable)")
     parser.add_argument("--weighted", action="store_true", help="sample-count weighted FedAvg (default: uniform, like the reference)")
+    parser.add_argument("--class-weight", default=d.class_weight, metavar="SPEC",
+                        help="class-weighted local fits of ffnn (2 classes: label 0, 1) and ffnn_category (5 categories): 'balanced' = "
+                             "min(M, N / (C * N_c)) from the class counts of every device's training rows, or C comma-separated "
+                             "weights >= 0 (local and remote mode; balanced not with --secure-agg)")
+    parser.add_argument("--class-weight-max", type=float, default=d.class_weight_max, metavar="M",
+                        help="--class-weight balanced: the cap of every class weight (> 0)")
     parser.add_argument("--select", type=int, default=None, help="train at most k of the collected workers")
     parser.add_argument("--selection", choices=["all", "first", "random"], default="all")
     parser.add_argument("--checkpoint", type=str, default="./test.pth")
@@ -205,6 +211,8 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.max_staleness = getattr(ns, "max_staleness", a.max_staleness)
     a.staleness_exponent = getattr(ns, "staleness_exponent", a.staleness_exponent)
     a.async_settings()                # rejects negative settings and --async-buffer with --secure-agg or a compressed downlink
+    a.class_weight = getattr(ns, "class_weight", a.class_weight)
+    a.class_weight_max = getattr(ns, "class_weight_max", a.class_weight_max)
     return a
 
 
