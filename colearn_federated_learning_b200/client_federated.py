@@ -52,11 +52,14 @@ def encrypted_training(args, model, private_train_loader, optimizer=None, epoch:
 
 
 async def train_remote(worker: RemoteWorkerClient, traced_model, batch_size: int, optimizer: str, max_nr_batches: int,
-                       epochs: int, lr: float, model_name: str = "ffnn", loss: str = "bce"):
+                       epochs: int, lr: float, model_name: str = "ffnn", loss: str = "bce", optimizer_args=None):
     """Send the model to ``worker``, fit remotely, get it back (reference cf.py:175-213: TrainConfig.send →
-    async_fit → model_ptr.get).  Returns ``(worker.id, model, loss)``; one RPC carries all three legs."""
+    async_fit → model_ptr.get).  Returns ``(worker.id, model, loss)``; one RPC carries all three legs.  ``optimizer`` /
+    ``optimizer_args`` name the device's local optimizer as ``torch.optim`` does (fl/local_opt.py); they are checked here,
+    before the request leaves."""
     cfg = FitConfig(model=model_name, loss=loss, batch_size=batch_size, epochs=epochs, max_nr_batches=max_nr_batches,
                     lr=lr, optimizer=optimizer)
+    cfg = cfg.with_local_opt(FitConfig(optimizer=optimizer, optimizer_args=optimizer_args).local_opt())
     flat = flatten_params(traced_model).cpu()
     loop = asyncio.get_running_loop()
     new_flat, last, _n = await loop.run_in_executor(None, lambda: worker.fit(flat, cfg))

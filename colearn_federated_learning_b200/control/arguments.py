@@ -9,7 +9,7 @@ as a CLI flag by ``federated_coordinator.py`` with the reference value as defaul
 from __future__ import annotations
 
 from dataclasses import dataclass, asdict
-from typing import Any, Dict, Optional
+from typing import Any, Dict, Optional, Tuple
 
 DEFAULT_TEST_PATH = "./dataset_example/UNSW_2018_IoT_Botnet_Final_10_best_Training_1_1.csv"
 ROUND_MODE_BATCHES = 1000  # reference: ``round > 1`` forces 1000 local batches (fc.py:533-535)
@@ -63,6 +63,12 @@ class Arguments:
     class_weight: Optional[str] = None   # class-weighted local fits (fl/classweight.py): "balanced" (from the federated class
                                    # counts) or C comma-separated weights; None: unweighted
     class_weight_max: float = 10.0  # balanced class weights: the cap of every weight (> 0)
+    local_optimizer: str = "SGD"   # the devices' local optimizer (fl/local_opt.py): "SGD" or "Adam"
+    local_momentum: float = 0.0    # SGD momentum in [0, 1) (not `momentum` above: the reference's 0.5 there was never applied)
+    local_nesterov: bool = False   # SGD: nesterov momentum
+    local_weight_decay: float = 0.0  # SGD / Adam: L2 weight decay (>= 0)
+    local_betas: Tuple[float, float] = (0.9, 0.999)  # Adam: (beta1, beta2), each in [0, 1)
+    local_eps: float = 1e-8        # Adam: eps (> 0)
     async_buffer: int = 0          # remote mode: >0 = asynchronous buffered aggregation, one server step per K replies from devices
                                    # that train from whatever version is current (fl/asyncagg.py); 0 = synchronous rounds
     async_concurrency: int = 0     # asynchronous: fits in flight (0 = one per selected device)
@@ -75,6 +81,20 @@ class Arguments:
     dataset: str = "unsw"          # data.DATASET_REGISTRY entry that reads test_path (user datasets: data.register_dataset)
     n_train_items_enc: int = 1000  # fc.py:432
     precision_fractional: int = 3  # fc.py:433
+
+    def local_opt(self):
+        """The :class:`fl.local_opt.LocalOpt` of every device's fit.  ValueError for settings out of range, and for a setting of
+        the other optimizer (momentum or nesterov with Adam, betas or eps with SGD) rather than ignoring it."""
+        from ..fl.local_opt import LocalOpt
+        other = {"SGD": ("local_betas", "local_eps"), "Adam": ("local_momentum", "local_nesterov")}.get(self.local_optimizer, ())
+        default = Arguments()
+        for name in other:
+            if getattr(self, name) != getattr(default, name):
+                flag = "--" + name.replace("_", "-")
+                raise ValueError(f"{flag} does not apply to --local-optimizer {self.local_optimizer}")
+        if self.local_optimizer == "SGD":
+            return LocalOpt("SGD", momentum=self.local_momentum, nesterov=self.local_nesterov, weight_decay=self.local_weight_decay)
+        return LocalOpt(self.local_optimizer, weight_decay=self.local_weight_decay, betas=tuple(self.local_betas), eps=self.local_eps)
 
     def server_optimizer(self):
         """The :class:`fl.server_opt.ServerOpt` these arguments describe (``server_lr`` is its learning rate)."""

@@ -278,9 +278,10 @@ class Coordinator(BusClient):
         if loss in ("auto", "", None):
             # reference: local mode trains with sum-squared-error (cf.py:112), remote with BCE (cf.py:79)
             loss = "sse" if (mode == "local" and self.args.model in ("ffnn", "testing_remote")) else resolve_loss(self.args.model, "auto")
-        return FitConfig(model=self.args.model, loss=loss, batch_size=self.args.batch_size, epochs=self.args.epochs,
-                         max_nr_batches=self.args.federate_after_n_batches, lr=self.args.lr, shuffle=True,
-                         seed=self.args.seed)
+        cfg = FitConfig(model=self.args.model, loss=loss, batch_size=self.args.batch_size, epochs=self.args.epochs,
+                        max_nr_batches=self.args.federate_after_n_batches, lr=self.args.lr, shuffle=True,
+                        seed=self.args.seed)
+        return cfg.with_local_opt(self.args.local_opt())
 
     def _maybe_checkpoint(self, model, theta: torch.Tensor, round_idx: int, meta: Dict[str, Any]) -> None:
         """``--save-every N``: durable progress inside a long training (the reference only saves after the last
@@ -327,6 +328,7 @@ class Coordinator(BusClient):
             fed.shards[wid] = Shard(wid, *tgt.training_rows(fed[wid].x, fed[wid].y))
         cw = classweight.setting(self.args, tgt.classes(model))
         result: Dict[str, Any] = {"workers": list(to_train.keys()), "losses": {}, "rounds": self.enabled_round}
+        result.update(_local_opt_field(cfg, self.args.class_weight))
         if cw is not None:
             # one weight vector for the training, from every virtual worker's training rows (balanced) or as given
             result["class_weights"] = classweight.local(cw, [fed[wid].y for wid in fed.workers])
@@ -452,6 +454,7 @@ class Coordinator(BusClient):
         pool = ThreadPoolExecutor(max_workers=max(1, len(to_train)), thread_name_prefix="fit-rpc")
         self.metrics.start_training(cfg.max_nr_batches)
         result: Dict[str, Any] = {"workers": list(to_train.keys()), "losses": {}, "rounds": self.enabled_round, "dropped": []}
+        result.update(_local_opt_field(cfg, self.args.class_weight))
         alive = OrderedDict(to_train)
         run = self._remote_async if self.args.async_settings() is not None else self._remote_rounds
         try:
@@ -721,8 +724,9 @@ class Coordinator(BusClient):
 
     @staticmethod
     def _training_fields(result: Dict[str, Any], r: int) -> Dict[str, Any]:
-        """What the first round record of a training carries besides its own fields: the ``class_weights`` block"""
-        return {"class_weights": result["class_weights"]} if r == 0 and "class_weights" in result else {}
+        """What the first round record of a training carries besides its own fields: the ``class_weights`` and ``local_opt``
+        blocks"""
+        return {key: result[key] for key in ("class_weights", "local_opt") if r == 0 and key in result}
 
     async def _class_weights(self, model, alive, loop, pool) -> Optional[Dict[str, Any]]:
         """The ``class_weights`` block of a remote training (fl/classweight.py), None without ``--class-weight``.  ``balanced``
@@ -890,6 +894,16 @@ class Coordinator(BusClient):
 
 
 # --------------------------------------------------------------------------------------------------
+def _local_opt_field(cfg: FitConfig, class_weight: Optional[str]) -> Dict[str, Any]:
+    """``{"local_opt": {kind, ...}}`` for a training whose devices fit with anything but plain SGD, else nothing.  ValueError
+    before any round for such an optimizer next to class weights (``class_weight``: the ``--class-weight`` setting)."""
+    from ..fl.local_opt import resolve
+    lo = resolve(cfg.local_opt())
+    if lo is not None and class_weight is not None:
+        raise ValueError("class weights together with a local optimizer other than plain SGD are not supported")
+    return {} if lo is None else {"local_opt": lo.record()}
+
+
 def train_virtual_workers(theta: torch.Tensor, model, fed, cfg: FitConfig, round_idx: int):
     """One round of local training for every virtual worker, each starting from ``theta``.
 
@@ -903,6 +917,10 @@ def train_virtual_workers(theta: torch.Tensor, model, fed, cfg: FitConfig, round
     counts = [len(fed[w]) for w in fed.workers]
     losses = [0.0] * k
     spec = model.spec if isinstance(model, MLPNet) else None
+    from ..fl.local_opt import resolve
+    lopt = resolve(cfg.local_opt())
+    if lopt is not None and cfg.class_weights is not None:
+        raise ValueError("class weights together with a local optimizer are not supported")
     fused = (spec is not None and device.type == "cuda" and ops.net_kind_for(spec.dims, spec.out_activation) is not None)
     if fused:
         loss_out = torch.zeros(k, 2, device=device)
@@ -919,7 +937,8 @@ def train_virtual_workers(theta: torch.Tensor, model, fed, cfg: FitConfig, round
         if tasks:
             descs = ops.build_client_descs(tasks, device)
             ops.mlp_local_sgd_multi(spec.dims, spec.out_activation, descs, len(tasks), cfg.batch_size, cfg.lr,
-                                    cfg.epochs, cfg.max_nr_batches, resolve_loss(cfg.model, cfg.loss), class_weights=cfg.class_weights)
+                                    cfg.epochs, cfg.max_nr_batches, resolve_loss(cfg.model, cfg.loss), class_weights=cfg.class_weights,
+                                    local_opt=lopt)
             vals = loss_out[:, 0].tolist()
             for i in idx:
                 losses[i] = vals[i]
@@ -934,7 +953,7 @@ def train_virtual_workers(theta: torch.Tensor, model, fed, cfg: FitConfig, round
             res = ops.host.mlp_local_sgd_multi(spec.dims, spec.out_activation, [flats[i] for i in idx], [sh.x for sh in shards],
                                                [sh.y for sh in shards], perms, cfg.batch_size, cfg.lr, cfg.epochs,
                                                cfg.max_nr_batches, resolve_loss(cfg.model, cfg.loss),
-                                               class_weights=cfg.class_weights)
+                                               class_weights=cfg.class_weights, local_opt=lopt)
             for j, i in enumerate(idx):
                 losses[i] = float(res[j, 0])
         return flats, losses, counts

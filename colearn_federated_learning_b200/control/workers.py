@@ -303,6 +303,10 @@ class WorkerServer:
                     if classes is None:
                         raise ValueError(f"class weights refused: {cfg.model} has no class-weighted fit")
                     cfg.class_weights = classweight.check_weights(cfg.class_weights, classes, "class weights refused")
+                # the local optimizer the request names (fl/local_opt.py): an unknown name or argument is refused, not trained
+                # as SGD
+                if not cfg.local_opt().is_plain() and cfg.class_weights is not None:
+                    raise ValueError("class weights together with a local optimizer are not supported")
             except ValueError as e:
                 return {"ok": False, "error": str(e)}
             if sa is not None:

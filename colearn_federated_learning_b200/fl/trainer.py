@@ -44,12 +44,25 @@ class FitConfig:
     seed: int = 1
     optimizer: str = "SGD"
     class_weights: Optional[List[float]] = None   # a class-weighted fit (fl/classweight.py); None: unweighted
+    optimizer_args: Optional[Dict[str, Any]] = None   # the local optimizer's arguments (fl/local_opt.py); None: its defaults
 
     def to_dict(self) -> Dict[str, Any]:
         d = asdict(self)
-        if d["class_weights"] is None:
-            del d["class_weights"]                # an unweighted request is the one it was before class weights existed
+        for key in ("class_weights", "optimizer_args"):
+            if d[key] is None:
+                del d[key]                        # an unset option leaves the request as it was before the option existed
         return d
+
+    def local_opt(self):
+        """The :class:`fl.local_opt.LocalOpt` this fit names (ValueError with the reason for a name or argument it refuses)"""
+        from .local_opt import from_request
+        return from_request(self.optimizer, self.optimizer_args)
+
+    def with_local_opt(self, local_opt) -> "FitConfig":
+        """This config naming ``local_opt`` (None or plain SGD: ``optimizer="SGD"`` and no arguments)"""
+        from .local_opt import wire
+        name, args = wire(local_opt)
+        return replace(self, optimizer=name, optimizer_args=args)
 
     @classmethod
     def from_dict(cls, d: Dict[str, Any]) -> "FitConfig":
@@ -105,9 +118,13 @@ def _loss_torch(out: torch.Tensor, y: torch.Tensor, loss: str) -> torch.Tensor:
 
 def torch_fit(model: nn.Module, x: torch.Tensor, y: torch.Tensor, cfg: FitConfig, perm: Optional[torch.Tensor],
               autocast_bf16: bool = False) -> torch.Tensor:
-    """Generic autograd fit (library conv/BN kernels) with a flat in-place SGD step."""
+    """Generic autograd fit (library conv/BN kernels) with a flat in-place SGD step, or the ``torch.optim`` optimizer the
+    config names when it is not plain SGD (fresh for this fit)."""
     model.train()
     params = [p for p in model.parameters()]
+    from .local_opt import resolve
+    lopt = resolve(cfg.local_opt())
+    opt = lopt.torch_optimizer(params, cfg.lr) if lopt is not None else None
     n = x.shape[0]
     it = 0
     limit = cfg.max_nr_batches if cfg.max_nr_batches and cfg.max_nr_batches > 0 else None
@@ -122,13 +139,16 @@ def torch_fit(model: nn.Module, x: torch.Tensor, y: torch.Tensor, cfg: FitConfig
                 out = model(x[idx])
             last = _loss_torch(out, y[idx], cfg.loss)
             last.backward()
-            with torch.no_grad():
-                for p in params:
-                    if p.grad is not None:
-                        if p.is_cuda and p.dtype == torch.float32 and p.is_contiguous() and p.grad.is_contiguous():
-                            ops.sgd_step(p.data.view(-1), p.grad.view(-1), cfg.lr)
-                        else:
-                            p.sub_(p.grad, alpha=cfg.lr)
+            if opt is not None:
+                opt.step()
+            else:
+                with torch.no_grad():
+                    for p in params:
+                        if p.grad is not None:
+                            if p.is_cuda and p.dtype == torch.float32 and p.is_contiguous() and p.grad.is_contiguous():
+                                ops.sgd_step(p.data.view(-1), p.grad.view(-1), cfg.lr)
+                            else:
+                                p.sub_(p.grad, alpha=cfg.lr)
             it += 1
             if limit is not None and it >= limit:
                 return last.detach()
@@ -146,6 +166,10 @@ def local_fit(flat: torch.Tensor, model: nn.Module, x: torch.Tensor, y: torch.Te
         perm = make_perm(x.shape[0], cfg, flat.device, round_idx)
     if cfg.class_weights is not None and not isinstance(model, MLPNet):
         raise ValueError(f"class weights: {cfg.model} has no class-weighted fit")
+    from .local_opt import refuse_non_plain, resolve
+    lopt = resolve(cfg.local_opt())
+    if lopt is not None and cfg.class_weights is not None:
+        raise ValueError("class weights together with a local optimizer are not supported")
     if isinstance(model, MLPNet):
         spec = model.spec
         xx = x.view(x.shape[0], -1) if spec.flatten_input else x
@@ -153,12 +177,14 @@ def local_fit(flat: torch.Tensor, model: nn.Module, x: torch.Tensor, y: torch.Te
         # a class-weighted fit goes nowhere else: ops.mlp_local_sgd refuses a net without class-weighted kernels
         if not flat.is_cuda or has_kernel or cfg.class_weights is not None:
             last = ops.mlp_local_sgd(flat, spec.dims, xx, y, perm, cfg.batch_size, cfg.lr, cfg.epochs,
-                                     cfg.max_nr_batches, loss, spec.out_activation, class_weights=cfg.class_weights)
+                                     cfg.max_nr_batches, loss, spec.out_activation, class_weights=cfg.class_weights,
+                                     local_opt=lopt)
             LAST_FIT_LAUNCHES = 1 if flat.is_cuda else 0
             return last, ("persistent" if flat.is_cuda else "reference")
         if flat.is_cuda:
             from .layerwise import LayerwiseMLPTrainer
             if LayerwiseMLPTrainer.supports(spec, cfg):
+                refuse_non_plain(lopt, f"the layer-wise trainer of {cfg.model} (MLP {tuple(spec.dims)})")
                 tr = LayerwiseMLPTrainer.cached(spec, flat, cfg.batch_size)
                 before = tr.launches
                 last = tr.fit(flat, xx, y, cfg, perm)
@@ -167,6 +193,7 @@ def local_fit(flat: torch.Tensor, model: nn.Module, x: torch.Tensor, y: torch.Te
     if conv_path(flat.device) == "native":
         from .convnet import ConvNetTrainer
         if ConvNetTrainer.supports(model, cfg, x):
+            refuse_non_plain(lopt, f"the conv-net trainer of {cfg.model}")
             tr = ConvNetTrainer.cached(model, flat, cfg.batch_size, tuple(x.shape[2:]))
             before = tr.launches
             last = tr.fit(flat, model, x, y, cfg, perm)

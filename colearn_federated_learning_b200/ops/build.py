@@ -24,7 +24,7 @@ EMUL_NAME = "_colearn_emul"     # CPU emulator of the conv kernels (tests on box
 HOST_NAME = "_colearn_host"     # native CPU executor of the MLP local fit (devices / boxes without a GPU)
 SIMT_NAME = "_colearn_simt"     # the persistent-MLP CUDA kernels compiled for the CPU through csrc/host_shim.h (tests)
 
-CU_SOURCES = ["mlp_persistent.cu", "mlp_persistent_ae.cu", "mlp_persistent_cat.cu", "mlp_persistent_cw.cu", "elementwise.cu", "comm.cu", "gemm_wgmma.cu", "convnet.cu"]
+CU_SOURCES = ["mlp_persistent.cu", "mlp_persistent_ae.cu", "mlp_persistent_cat.cu", "mlp_persistent_cw.cu", "mlp_persistent_opt.cu", "elementwise.cu", "comm.cu", "gemm_wgmma.cu", "convnet.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo",
@@ -47,7 +47,7 @@ def _stamp(src: str, flags: List[str]) -> str:
     h = hashlib.sha1()
     with open(src, "rb") as f:
         h.update(f.read())
-    for dep in ("colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "mlp_v2.cuh", "mlp_v2_fit.inc", "mlp_persistent.cu", "conv_ops.cuh", "conv_bindings.inc"):
+    for dep in ("colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "mlp_v2.cuh", "mlp_v2_fit.inc", "mlp_v1_fit.inc", "local_opt.cuh", "mlp_persistent.cu", "conv_ops.cuh", "conv_bindings.inc"):
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(flags).encode())
@@ -114,7 +114,8 @@ def build_host(force: bool = False) -> str:
     out = host_path()
     src = os.path.join(CSRC, "mlp_host.cpp")
     cxx_flags = [f for f in flags if f != "-O2"] + ["-O3", "-fno-math-errno", "-fopenmp-simd", f"-DTORCH_EXTENSION_NAME={HOST_NAME}"]
-    h = hashlib.sha1(open(src, "rb").read() + " ".join(cxx_flags).encode()).hexdigest()[:16]
+    h = hashlib.sha1(open(src, "rb").read() + open(os.path.join(CSRC, "local_opt.cuh"), "rb").read()
+                     + " ".join(cxx_flags).encode()).hexdigest()[:16]
     obj = os.path.join(OBJ, f"mlp_host.cpp.{h}.o")
     if force or not os.path.exists(obj) or not os.path.exists(out):
         for name in os.listdir(OBJ):
@@ -144,9 +145,9 @@ def build_simt_emul(force: bool = False) -> str:
     src = os.path.join(CSRC, "simt_emul.cpp")
     cxx_flags = [f for f in flags if f not in ("-O2", "-std=c++17")] + ["-O1", "-std=c++20", "-pthread", "-Wno-unknown-pragmas",
                                                                         f"-DTORCH_EXTENSION_NAME={SIMT_NAME}"]
-    sources = ["simt_emul.cpp", "simt_mlp.cpp", "simt_mlp_ae.cpp", "simt_mlp_cat.cpp", "simt_mlp_cw.cpp", "simt_elementwise.cpp", "simt_comm.cpp", "simt_convnet.cpp", "simt_gemm.cpp"]
+    sources = ["simt_emul.cpp", "simt_mlp.cpp", "simt_mlp_ae.cpp", "simt_mlp_cat.cpp", "simt_mlp_cw.cpp", "simt_mlp_opt.cpp", "simt_elementwise.cpp", "simt_comm.cpp", "simt_convnet.cpp", "simt_gemm.cpp"]
     h = hashlib.sha1()
-    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_persistent_ae.cu", "mlp_persistent_cat.cu", "mlp_persistent_cw.cu", "mlp_v2.cuh", "mlp_v2_fit.inc", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "conv_ops.cuh"]:
+    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_persistent_ae.cu", "mlp_persistent_cat.cu", "mlp_persistent_cw.cu", "mlp_persistent_opt.cu", "mlp_v2.cuh", "mlp_v2_fit.inc", "mlp_v1_fit.inc", "local_opt.cuh", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "conv_ops.cuh"]:
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(cxx_flags).encode())

@@ -67,6 +67,7 @@ void set_spin_limit(double seconds) {
   check(set_spin_limit_mlp(ns), "set_spin_limit (mlp)");
   check(set_spin_limit_mlp_ae(ns), "set_spin_limit (mlp, autoencoder)");
   check(set_spin_limit_mlp_cw(ns), "set_spin_limit (mlp, class-weighted)");
+  check(set_spin_limit_mlp_opt(ns), "set_spin_limit (mlp, local optimizer)");
   check(set_spin_limit_gemm(ns), "set_spin_limit (gemm)");
   check(preload_comm_kernels(), "preload_comm_kernels");     // same call site: once per device, before any round
 }
@@ -96,6 +97,21 @@ void mlp_local_sgd_cw(int64_t net_kind, torch::Tensor descs, int64_t desc_offset
   hp.loss = (int)loss; hp.lr = (float)lr; hp.variant = (int)variant;
   const ClientDesc* d = reinterpret_cast<const ClientDesc*>(descs.data_ptr<uint8_t>()) + desc_offset;
   check(launch_mlp_local_sgd_cw((int)net_kind, d, (int)n_clients, hp, cw, cur_stream()), "mlp_local_sgd_cw launch");
+}
+// the local optimizer instances (mlp_persistent_opt.cu); opt: {kind, nesterov, momentum, weight_decay, beta1, beta2, eps}, checked
+// by the caller (fl/local_opt.py)
+void mlp_local_sgd_opt(int64_t net_kind, torch::Tensor descs, int64_t desc_offset, int64_t n_clients, int64_t batch_size,
+                       int64_t epochs, int64_t max_steps, int64_t loss, double lr, std::vector<double> opt) {
+  TORCH_CHECK(descs.is_cuda() && descs.scalar_type() == at::kByte && descs.is_contiguous(), "descs must be CUDA uint8");
+  TORCH_CHECK((desc_offset + n_clients) * (int64_t)sizeof(ClientDesc) <= descs.numel(), "descs too small");
+  TORCH_CHECK(opt.size() == 7, "local optimizer: 7 values");
+  const LocalOptArgs lo{(int)opt[0], (int)opt[1], (float)opt[2], (float)opt[3], (float)opt[4], (float)opt[5], (float)opt[6]};
+  c10::cuda::CUDAGuard guard(descs.device());
+  SgdHyper hp;
+  hp.batch_size = (int)batch_size; hp.epochs = (int)epochs; hp.max_steps = (int)max_steps;
+  hp.loss = (int)loss; hp.lr = (float)lr; hp.variant = 1;
+  const ClientDesc* d = reinterpret_cast<const ClientDesc*>(descs.data_ptr<uint8_t>()) + desc_offset;
+  check(launch_mlp_local_sgd_opt((int)net_kind, d, (int)n_clients, hp, lo, cur_stream()), "mlp_local_sgd_opt launch");
 }
 int64_t mlp_net_params(int64_t net_kind) { return mlp_net_num_params((int)net_kind); }
 int64_t mlp_smem_bytes(int64_t net_kind, int64_t batch) { return mlp_local_sgd_smem_bytes((int)net_kind, (int)batch); }
@@ -954,6 +970,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("client_desc_size", &client_desc_size);
   m.def("mlp_local_sgd", &mlp_local_sgd);
   m.def("mlp_local_sgd_cw", &mlp_local_sgd_cw);
+  m.def("mlp_local_sgd_opt", &mlp_local_sgd_opt);
   m.def("mlp_net_params", &mlp_net_params);
   m.def("mlp_smem_bytes", &mlp_smem_bytes);
   m.def("mlp_forward", &mlp_forward);

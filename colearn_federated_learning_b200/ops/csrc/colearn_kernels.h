@@ -55,6 +55,8 @@
 #include "eval_summary.cuh"
 // reconstruction-error summary of an autoencoder on held-out rows (federated anomaly detection)
 #include "recon_summary.cuh"
+// per-element local optimizer step of a device's fit (SGD with momentum / weight decay, Adam)
+#include "local_opt.cuh"
 
 namespace colearn {
 // Programmatic dependent launch is ON unless COLEARN_PDL=0 (bit-identical results)
@@ -137,6 +139,7 @@ cudaError_t set_spin_limit_mlp(unsigned long long ns);
 cudaError_t set_spin_limit_mlp_ae(unsigned long long ns);   // mlp_persistent_ae.cu: its own copy of the limit
 cudaError_t set_spin_limit_mlp_cat(unsigned long long ns);  // mlp_persistent_cat.cu: likewise
 cudaError_t set_spin_limit_mlp_cw(unsigned long long ns);   // mlp_persistent_cw.cu: likewise
+cudaError_t set_spin_limit_mlp_opt(unsigned long long ns);  // mlp_persistent_opt.cu: likewise
 cudaError_t set_spin_limit_gemm(unsigned long long ns);
 
 // ---------------------------------------------------------------------------------------------
@@ -237,6 +240,12 @@ struct ClassWeights {
 // Variant 5 only, NET_FFNN with bce / sse / mse and NET_FFNN_CAT with xent; anything else: cudaErrorInvalidValue, no launch.
 cudaError_t launch_mlp_local_sgd_cw(int net_kind, const ClientDesc* descs, int n_clients, SgdHyper hp, ClassWeights cw,
                                     cudaStream_t stream);
+
+// Local optimizer instances (mlp_persistent_opt.cu): variant 1 with the local_opt.cuh step (LocalOptArgs::kind LOCAL_OPT_SGD or
+// LOCAL_OPT_ADAM, hyper-parameters checked by the caller) for every net kind; hp.variant is not read.  Anything else:
+// cudaErrorInvalidValue, no launch.
+cudaError_t launch_mlp_local_sgd_opt(int net_kind, const ClientDesc* descs, int n_clients, SgdHyper hp, LocalOptArgs lo,
+                                     cudaStream_t stream);
 
 // Forward-only batched inference/eval for the small nets: out[n, d_out] (post-activation).
 cudaError_t launch_mlp_forward(int net_kind, const float* theta, const float* x, float* out,

@@ -17,6 +17,8 @@
 #include <thread>
 #include <vector>
 
+#include "local_opt.cuh"
+
 namespace py = pybind11;
 
 namespace {
@@ -61,13 +63,15 @@ struct Hyper {
   int batch, epochs, max_steps, loss;
   float lr;
   const float* cw = nullptr;   // a class-weighted fit: w[class of the row] (its label y[0]) scales the row's loss and gradient
+  const colearn::LocalOptArgs* opt = nullptr;   // a local optimizer (local_opt.cuh) instead of plain SGD: the generic loop only
 };
 
 // Per-thread scratch: activations of every layer for every sample of the batch, dz ping-pong, gradient arena (B > 1)
 struct Scratch {
   std::vector<float> acts;       // [layers + 1][B][max_dim]
   std::vector<float> dz, dprev;  // [max_dim]
-  std::vector<float> grad;       // [n_params] (only used when B > 1)
+  std::vector<float> grad;       // [n_params] (used when B > 1 or with a local optimizer)
+  std::vector<float> m, v;       // [n_params] the local optimizer's moments (this fit's)
   std::vector<float> dout;       // [B][d_out]: dL/d(pre-activation of the last layer)
 };
 
@@ -158,7 +162,13 @@ void run_fit(const Net& net, Task& t, const Hyper& hp, Scratch& sc) {
   sc.dz.assign(md, 0.f);
   sc.dprev.assign(md, 0.f);
   sc.dout.assign((size_t)B * net.dims[L], 0.f);
-  if (B > 1) sc.grad.assign((size_t)net.n_params, 0.f);
+  const bool acc = B > 1 || hp.opt != nullptr;   // accumulate the batch gradient, then step
+  if (acc) sc.grad.assign((size_t)net.n_params, 0.f);
+  colearn::LocalOptStep ost = colearn::local_opt_start();
+  if (hp.opt != nullptr) {
+    sc.m.assign((size_t)net.n_params, 0.f);
+    sc.v.assign((size_t)net.n_params, 0.f);
+  }
   std::vector<const float*> ys(B);
   float* theta = t.theta;
   double loss_sum = 0.0;
@@ -175,7 +185,7 @@ void run_fit(const Net& net, Task& t, const Hyper& hp, Scratch& sc) {
       }
       t.last = loss_and_dout(net, hp.loss, sc.acts.data(), stride_b, stride_l, ys.data(), t.y_dim, bsz, sc.dout.data(), hp.cw);
       loss_sum += t.last;
-      if (B > 1) std::fill(sc.grad.begin(), sc.grad.end(), 0.f);
+      if (acc) std::fill(sc.grad.begin(), sc.grad.end(), 0.f);
       for (int s = 0; s < bsz; ++s) {
         const float* acts = sc.acts.data() + (int64_t)s * stride_b;
         std::memcpy(sc.dz.data(), sc.dout.data() + (int64_t)s * net.dims[L], sizeof(float) * net.dims[L]);
@@ -196,7 +206,7 @@ void run_fit(const Net& net, Task& t, const Hyper& hp, Scratch& sc) {
             for (int i = 0; i < k; ++i)
               if (a[i] <= 0.f) dp[i] = 0.f;   // threshold_backward: a NaN activation passes the gradient
           }
-          if (B == 1) {   // batch-1 (the reference's Arguments): apply the update right away, no gradient arena
+          if (!acc) {   // batch-1 plain SGD (the reference's Arguments): apply the update right away, no gradient arena
             for (int j = 0; j < n; ++j) {
               const float g = hp.lr * dz[j];
               float* wr = w + (int64_t)j * k;
@@ -216,7 +226,10 @@ void run_fit(const Net& net, Task& t, const Hyper& hp, Scratch& sc) {
           if (l > 0) std::swap(sc.dz, sc.dprev);
         }
       }
-      if (B > 1) {
+      if (hp.opt != nullptr) {
+        const float* g = sc.grad.data();
+        colearn::local_opt_pass(*hp.opt, ost, hp.lr, theta, g, sc.m.data(), sc.v.data(), net.n_params);
+      } else if (B > 1) {
         const float* g = sc.grad.data();
         for (int64_t i = 0; i < net.n_params; ++i) theta[i] -= hp.lr * g[i];
       }
@@ -333,10 +346,10 @@ using ShapeMLP64 = Shape<10, 64, 64, 2>;         // BASELINE MLP
 using ShapeFFNN = Shape<10, 50, 30, 10, 1>;      // the reference's FFNN (cf.py:22-44)
 using ShapeTestingRemote = Shape<2, 50, 10, 1>;  // the reference's TestingRemote (cf.py:46-55)
 
-// one local fit: the fixed-shape path for the known networks at batch 1, the generic loop otherwise
+// one local fit: the fixed-shape path for the known networks at batch-1 plain SGD, the generic loop otherwise
 inline void run_fit_any(const Net& net, Task& t, const Hyper& hp, Scratch& sc) {
   static const bool generic_only = std::getenv("COLEARN_HOST_GENERIC") != nullptr;
-  if (hp.batch == 1 && !generic_only) {
+  if (hp.batch == 1 && hp.opt == nullptr && !generic_only) {
     if (ShapeMLP64::matches(net)) return run_fit_fixed<ShapeMLP64>(net, t, hp, sc);
     if (ShapeFFNN::matches(net)) return run_fit_fixed<ShapeFFNN>(net, t, hp, sc);
     if (ShapeTestingRemote::matches(net)) return run_fit_fixed<ShapeTestingRemote>(net, t, hp, sc);
@@ -371,7 +384,8 @@ Task make_task(const Net& net, const torch::Tensor& theta, const torch::Tensor& 
 torch::Tensor fit_host(std::vector<int64_t> dims, bool sigmoid_out, std::vector<torch::Tensor> thetas,
                        std::vector<torch::Tensor> xs, std::vector<torch::Tensor> ys,
                        std::vector<c10::optional<torch::Tensor>> perms, int64_t batch_size, int64_t epochs,
-                       int64_t max_nr_batches, int64_t loss, double lr, int64_t threads, const std::vector<double>* class_weights) {
+                       int64_t max_nr_batches, int64_t loss, double lr, int64_t threads, const std::vector<double>* class_weights,
+                       const std::vector<double>* local_opt = nullptr) {
   const Net net(dims, sigmoid_out);
   const size_t K = thetas.size();
   TORCH_CHECK(K >= 1 && xs.size() == K && ys.size() == K && perms.size() == K, "one theta / x / y / perm per client");
@@ -392,7 +406,15 @@ torch::Tensor fit_host(std::vector<int64_t> dims, bool sigmoid_out, std::vector<
         TORCH_CHECK(c >= 0.f && c < (float)cw.size() && c == (float)(int)c, "label of row ", i, " is not a class index below ", cw.size());
       }
   }
-  const Hyper hp{(int)batch_size, (int)epochs, (int)max_nr_batches, (int)loss, (float)lr, class_weights ? cw.data() : nullptr};
+  colearn::LocalOptArgs lo{};
+  if (local_opt != nullptr) {
+    TORCH_CHECK(local_opt->size() == 7, "local optimizer: 7 values");
+    const std::vector<double>& o = *local_opt;
+    lo = colearn::LocalOptArgs{(int)o[0], (int)o[1], (float)o[2], (float)o[3], (float)o[4], (float)o[5], (float)o[6]};
+    TORCH_CHECK(lo.kind == colearn::LOCAL_OPT_SGD || lo.kind == colearn::LOCAL_OPT_ADAM, "unknown local optimizer kind");
+  }
+  const Hyper hp{(int)batch_size, (int)epochs, (int)max_nr_batches, (int)loss, (float)lr, class_weights ? cw.data() : nullptr,
+                 local_opt ? &lo : nullptr};
   int nthreads = threads > 0 ? (int)threads : (int)std::thread::hardware_concurrency();
   nthreads = std::max(1, std::min<int>(nthreads, (int)K));
   {
@@ -430,6 +452,14 @@ torch::Tensor mlp_local_sgd_cw_host(std::vector<int64_t> dims, bool sigmoid_out,
                                     int64_t max_nr_batches, int64_t loss, double lr, int64_t threads, std::vector<double> class_weights) {
   return fit_host(dims, sigmoid_out, thetas, xs, ys, perms, batch_size, epochs, max_nr_batches, loss, lr, threads, &class_weights);
 }
+// the generic loop with a local optimizer's step (local_opt.cuh); local_opt: {kind, nesterov, momentum, weight_decay, beta1,
+// beta2, eps}, checked by the caller (fl/local_opt.py)
+torch::Tensor mlp_local_sgd_opt_host(std::vector<int64_t> dims, bool sigmoid_out, std::vector<torch::Tensor> thetas,
+                                     std::vector<torch::Tensor> xs, std::vector<torch::Tensor> ys,
+                                     std::vector<c10::optional<torch::Tensor>> perms, int64_t batch_size, int64_t epochs,
+                                     int64_t max_nr_batches, int64_t loss, double lr, int64_t threads, std::vector<double> local_opt) {
+  return fit_host(dims, sigmoid_out, thetas, xs, ys, perms, batch_size, epochs, max_nr_batches, loss, lr, threads, nullptr, &local_opt);
+}
 
 // Batched forward (inference / evaluation): out [n, d_out], post output-activation
 torch::Tensor mlp_forward_host(std::vector<int64_t> dims, bool sigmoid_out, torch::Tensor theta, torch::Tensor x) {
@@ -456,5 +486,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "colearn host executor: MLP local SGD / forward on CPU devices (no CUDA dependency)";
   m.def("mlp_local_sgd", &mlp_local_sgd_host);
   m.def("mlp_local_sgd_cw", &mlp_local_sgd_cw_host);
+  m.def("mlp_local_sgd_opt", &mlp_local_sgd_opt_host);
   m.def("mlp_forward", &mlp_forward_host);
 }

@@ -293,149 +293,20 @@ struct ParamIO {
 template <class N>
 __global__ void __launch_bounds__(NT, 1)
 mlp_local_sgd_kernel(const ClientDesc* __restrict__ descs, SgdHyper hp) {
-  using Tot = Totals<N>;
-  constexpr int SP = Tot::smem_params;
-  constexpr int DIN = N::DIN, DOUT = N::DOUT, ROWM = Tot::ROW_MAX, EPT = Tot::EPT;
-  COLEARN_DYN_SMEM(float, smem);
+  constexpr int kOpt = 0;
+  const LocalOptArgs lo{};   // (read by the optimizer instances only)
+#include "mlp_v1_fit.inc"
+}
 
-  const ClientDesc d = descs[blockIdx.x];
-  const int tid = threadIdx.x;
-  const int B = hp.batch_size < 1 ? 1 : hp.batch_size;
-  const bool accumulate = B > 1;
-
-  float* sP = smem;                              // padded params
-  float* sG = sP + SP;                           // gradient accumulator (only touched if B > 1)
-  float* sAct = sG + (accumulate ? SP : 0);      // 2 x acts (double buffered by step parity)
-  float* sDz = sAct + 2 * Tot::acts;             // dz_1..dz_L
-  float* sData = sDz + Tot::acts;                // 2 x CHUNK x ROWM sample ring
-  float* sMisc = sData + 2 * CHUNK * ROWM;       // [0] last loss, [1] loss sum
-
-  // (1) wait for the broadcast of this round's global model to land (SURVEY K1/K4)
-  if (d.wait_flag != nullptr) {
-    if (tid == 0) {
-      spin_wait_ge(d.wait_flag, d.wait_value, 32, "mlp_local_sgd: broadcast flag of this round");
-    }
-    __syncthreads();
-  }
-
-  // (2) global arena -> padded smem layout (L1 bypass: the arena may be peer-written)
-  ParamIO<N, 0>::template load<true>(sP, d.theta_in, tid);
-  if (accumulate)
-    for (int i = tid; i < SP; i += NT) sG[i] = 0.f;
-  if (tid < 2) sMisc[tid] = 0.f;
-
-  // (3) step bookkeeping
-  const int n = d.n;
-  const int ydim = d.y_dim;
-  const int row = DIN + ydim;
-  const int spe = ((n > 0 ? n : 1) + B - 1) / B;  // steps per epoch (an empty shard: Q = 0 below, see the v2 kernel)
-  long long total_steps = (long long)hp.epochs * spe;
-  if (hp.max_steps > 0 && hp.max_steps < total_steps) total_steps = hp.max_steps;
-  // total samples consumed by those steps
-  long long Q;
-  {
-    const long long full_epochs = total_steps / spe;
-    const long long rem_steps = total_steps - full_epochs * spe;
-    long long rem_samples = rem_steps * B;
-    if (rem_samples > n) rem_samples = n;
-    Q = full_epochs * (long long)n + rem_samples;
-  }
-  const int n_chunks = (int)((Q + CHUNK - 1) / CHUNK);
-
-  const FeistelDomain fdom = feistel_domain((uint32_t)(n > 0 ? n : 1));   // in-kernel shuffle (ClientDesc::perm_seed)
-  float pre[EPT];
-  auto issue_loads = [&](int chunk) {
-#pragma unroll
-    for (int j = 0; j < EPT; ++j) {
-      const int e = tid + j * NT;
-      pre[j] = 0.f;
-      if (e < CHUNK * row) {
-        const int i = e / row, c = e - i * row;
-        const long long q = (long long)chunk * CHUNK + i;
-        if (q < Q) {
-          const int ep = (int)(q / n);
-          const int pos = (int)(q - (long long)ep * n);
-          const int idx = d.perm ? __ldg(d.perm + (size_t)(ep % d.perm_rows) * n + pos)
-                                 : (d.perm_seed ? (int)feistel_index((uint32_t)pos, (uint32_t)n, fdom, d.perm_seed, d.perm_row0 + ep) : pos);
-          pre[j] = (c < DIN) ? __ldg(d.x + (size_t)idx * DIN + c) : __ldg(d.y + (size_t)idx * ydim + (c - DIN));
-        }
-      }
-    }
-  };
-  auto store_loads = [&](int buf) {
-    float* dst = sData + buf * (CHUNK * ROWM);
-#pragma unroll
-    for (int j = 0; j < EPT; ++j) {
-      const int e = tid + j * NT;
-      if (e < CHUNK * row) dst[e] = pre[j];
-    }
-  };
-
-  if (n_chunks > 0) { issue_loads(0); store_loads(0); }
-  __syncthreads();
-
-  long long step = 0;
-  int pos_in_epoch = 0;   // samples consumed in the current epoch
-  int in_batch = 0;       // samples accumulated in the current batch
-  int cur_batch = (n < B) ? n : B;
-  float batch_loss = 0.f;  // only meaningful on tid 0
-  int parity = 0;
-
-  for (int c = 0; c < n_chunks; ++c) {
-    if (c + 1 < n_chunks) issue_loads(c + 1);  // next chunk's gathers fly during this chunk's math
-    const float* chunk = sData + (c & 1) * (CHUNK * ROWM);
-    const long long q0 = (long long)c * CHUNK;
-    const int cnt = (int)((Q - q0) < CHUNK ? (Q - q0) : CHUNK);
-    for (int i = 0; i < cnt; ++i) {
-      const float* a0 = chunk + i * row;
-      const float* yrow = a0 + DIN;
-      float* acts = sAct + parity * Tot::acts;
-      const float inv_b = 1.f / (float)cur_batch;
-
-      FwdChain<N, 0, true>::run(sP, a0, acts, tid);
-      if (tid < 32) {
-        const float v = loss_and_dz<N>(acts + Offs<N, N::L - 1>::act, sDz + Offs<N, N::L - 1>::act,
-                                       yrow, hp.loss, inv_b, tid);
-        if (tid == 0) batch_loss += (hp.loss == LOSS_SSE) ? v : v * inv_b;
-      }
-      __syncthreads();
-      BwdChain<N, N::L - 1>::run(sP, accumulate ? sG : sP, a0, acts, sDz,
-                                 accumulate ? 1.f : -hp.lr, tid);
-      parity ^= 1;
-
-      ++in_batch;
-      ++pos_in_epoch;
-      if (in_batch == cur_batch) {  // batch closes -> SGD step
-        if (accumulate) {
-          __syncthreads();
-          for (int k = tid; k < SP; k += NT) { sP[k] = fmaf(-hp.lr, sG[k], sP[k]); sG[k] = 0.f; }
-          __syncthreads();
-        }
-        if (tid == 0) { sMisc[0] = batch_loss; sMisc[1] += batch_loss; batch_loss = 0.f; }
-        ++step;
-        in_batch = 0;
-        if (pos_in_epoch >= n) pos_in_epoch = 0;
-        const int left = n - pos_in_epoch;
-        cur_batch = left < B ? left : B;
-      }
-    }
-    __syncthreads();                 // everyone is done reading chunk buffers of this parity
-    if (c + 1 < n_chunks) store_loads((c + 1) & 1);
-    __syncthreads();
-  }
-  __syncthreads();
-
-  // (4) epilogue: out_scale * theta_k (or scaled delta) -> theta_out (possibly a peer GPU)
-  ParamIO<N, 0>::store(sP, d.theta_in, d.theta_out, d.out_scale, d.delta_mode, tid);
-  if (tid == 0 && d.loss_out != nullptr) {
-    d.loss_out[0] = sMisc[0];
-    d.loss_out[1] = step > 0 ? sMisc[1] / (float)step : 0.f;
-  }
-  __syncthreads();
-  if (tid == 0 && d.signal_flag != nullptr) {
-    __threadfence_system();
-    st_release_sys(d.signal_flag, d.signal_value);
-  }
+// The same fit with a local optimizer's step (SGD with momentum / weight decay, or Adam: local_opt.cuh) in place of plain SGD.
+// Its instances are compiled in mlp_persistent_opt.cu.
+template <class N, int OPT>
+__global__ void __launch_bounds__(NT, 1)
+mlp_local_sgd_opt_kernel(const ClientDesc* __restrict__ descs, SgdHyper hp, LocalOptArgs lo_arg) {
+  constexpr int kOpt = OPT;
+  LocalOptArgs lo = lo_arg;
+  lo.kind = OPT;             // a compile-time kind: the other optimizer's branches are pruned
+#include "mlp_v1_fit.inc"
 }
 
 
@@ -532,6 +403,36 @@ cudaError_t launch_t(const ClientDesc* descs, int n_clients, SgdHyper hp, cudaSt
   }
   COLEARN_LAUNCH(mlp_local_sgd_kernel<N>, n_clients, NT, bytes, stream, descs, hp);
   return cudaGetLastError();
+}
+
+// the optimizer instances: sG at every batch size, then one (SGD) or two (Adam) moment arrays of the same padded size
+template <class N, int OPT>
+int smem_bytes_opt() {
+  using Tot = Totals<N>;
+  int f = Tot::smem_params * (OPT == LOCAL_OPT_ADAM ? 4 : 3) + 3 * Tot::acts + 2 * CHUNK * Tot::ROW_MAX + 8;
+  return f * (int)sizeof(float);
+}
+
+template <class N, int OPT>
+cudaError_t launch_opt_t(const ClientDesc* descs, int n_clients, SgdHyper hp, LocalOptArgs lo, cudaStream_t stream) {
+  const int bytes = smem_bytes_opt<N, OPT>();
+  static bool configured[64] = {false};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (!configured[dev & 63]) {
+    cudaError_t e = cudaFuncSetAttribute(mlp_local_sgd_opt_kernel<N, OPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e != cudaSuccess) return e;
+    configured[dev & 63] = true;
+  }
+  COLEARN_LAUNCH((mlp_local_sgd_opt_kernel<N, OPT>), n_clients, NT, bytes, stream, descs, hp, lo);
+  return cudaGetLastError();
+}
+
+template <class N>
+cudaError_t launch_opt_n(const ClientDesc* descs, int n_clients, SgdHyper hp, LocalOptArgs lo, cudaStream_t stream) {
+  if (lo.kind == LOCAL_OPT_SGD) return launch_opt_t<N, LOCAL_OPT_SGD>(descs, n_clients, hp, lo, stream);
+  if (lo.kind == LOCAL_OPT_ADAM) return launch_opt_t<N, LOCAL_OPT_ADAM>(descs, n_clients, hp, lo, stream);
+  return cudaErrorInvalidValue;
 }
 
 template <class N>

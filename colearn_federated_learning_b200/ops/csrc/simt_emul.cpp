@@ -23,7 +23,8 @@ const float* fptr(const Tensor& t, const char* name) {
 Tensor mlp_fit(int64_t net_kind, Tensor theta_in, std::vector<Tensor> theta_outs, std::vector<Tensor> xs, std::vector<Tensor> ys,
                std::vector<c10::optional<Tensor>> perms, int64_t batch_size, int64_t epochs, int64_t max_steps, int64_t loss,
                double lr, int64_t variant, std::vector<double> out_scales, bool delta_mode, c10::optional<Tensor> flags,
-               int64_t perm_seed, int64_t perm_row0, c10::optional<Tensor> perm_scratch, const std::vector<double>* class_weights) {
+               int64_t perm_seed, int64_t perm_row0, c10::optional<Tensor> perm_scratch, const std::vector<double>* class_weights,
+               const std::vector<double>* local_opt = nullptr) {
   const size_t K = xs.size();
   TORCH_CHECK(K >= 1 && ys.size() == K && perms.size() == K && theta_outs.size() == K && out_scales.size() == K, "one entry per client");
   const int P = colearn::mlp_net_num_params((int)net_kind);
@@ -75,7 +76,12 @@ Tensor mlp_fit(int64_t net_kind, Tensor theta_in, std::vector<Tensor> theta_outs
   {
     py::gil_scoped_release nogil;
     cudaError_t e;
-    if (class_weights != nullptr) {
+    if (local_opt != nullptr) {
+      TORCH_CHECK(local_opt->size() == 7, "local optimizer: 7 values");
+      const std::vector<double>& o = *local_opt;
+      const colearn::LocalOptArgs lo{(int)o[0], (int)o[1], (float)o[2], (float)o[3], (float)o[4], (float)o[5], (float)o[6]};
+      e = colearn::launch_mlp_local_sgd_opt((int)net_kind, descs.data(), (int)K, hp, lo, nullptr);
+    } else if (class_weights != nullptr) {
       colearn::ClassWeights cw{};
       TORCH_CHECK(class_weights->size() <= 8, "at most 8 class weights");
       for (size_t c = 0; c < class_weights->size(); ++c) cw.w[c] = (float)(*class_weights)[c];
@@ -99,6 +105,29 @@ Tensor mlp_local_sgd_cw(int64_t net_kind, Tensor theta_in, std::vector<Tensor> t
                         double lr, int64_t variant, std::vector<double> out_scales, std::vector<double> class_weights) {
   return mlp_fit(net_kind, theta_in, theta_outs, xs, ys, perms, batch_size, epochs, max_steps, loss, lr, variant, out_scales, false,
                  c10::nullopt, 0, 0, c10::nullopt, &class_weights);
+}
+// the local optimizer instances of mlp_persistent_opt.cu; local_opt: {kind, nesterov, momentum, weight_decay, beta1, beta2, eps}
+Tensor mlp_local_sgd_opt(int64_t net_kind, Tensor theta_in, std::vector<Tensor> theta_outs, std::vector<Tensor> xs, std::vector<Tensor> ys,
+                         std::vector<c10::optional<Tensor>> perms, int64_t batch_size, int64_t epochs, int64_t max_steps, int64_t loss,
+                         double lr, std::vector<double> out_scales, bool delta_mode, c10::optional<Tensor> flags, int64_t perm_seed,
+                         int64_t perm_row0, std::vector<double> local_opt) {
+  return mlp_fit(net_kind, theta_in, theta_outs, xs, ys, perms, batch_size, epochs, max_steps, loss, lr, 1, out_scales, delta_mode,
+                 flags, perm_seed, perm_row0, c10::nullopt, nullptr, &local_opt);
+}
+
+// local_opt.cuh's per-element step over arrays, in place: g [steps, n] holds the gradient of every step, m and v the moments
+void local_opt_steps(Tensor theta, Tensor g, Tensor m, Tensor v, double lr, std::vector<double> o) {
+  TORCH_CHECK(o.size() == 7, "local optimizer: 7 values");
+  const int64_t n = theta.numel();
+  TORCH_CHECK(g.dim() == 2 && g.size(1) == n && m.numel() == n && v.numel() == n, "theta, m, v [n], g [steps, n]");
+  const int64_t steps = g.size(0);
+  float* t = const_cast<float*>(fptr(theta, "theta"));
+  const float* gp = fptr(g, "g");
+  float* mp = const_cast<float*>(fptr(m, "m"));
+  float* vp = const_cast<float*>(fptr(v, "v"));
+  const colearn::LocalOptArgs lo{(int)o[0], (int)o[1], (float)o[2], (float)o[3], (float)o[4], (float)o[5], (float)o[6]};
+  colearn::LocalOptStep st = colearn::local_opt_start();
+  for (int64_t s = 0; s < steps; ++s) colearn::local_opt_pass(lo, st, (float)lr, t, gp + s * n, mp, vp, n);
 }
 
 Tensor mlp_forward(int64_t net_kind, Tensor theta, Tensor x, int64_t d_out) {
@@ -665,6 +694,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("batch_size"), py::arg("epochs"), py::arg("max_steps"), py::arg("loss"), py::arg("lr"), py::arg("variant"), py::arg("out_scales"),
         py::arg("delta_mode"), py::arg("flags"), py::arg("perm_seed") = 0, py::arg("perm_row0") = 0, py::arg("perm_scratch") = py::none());
   m.def("mlp_local_sgd_cw", &mlp_local_sgd_cw);
+  m.def("mlp_local_sgd_opt", &mlp_local_sgd_opt);
+  m.def("local_opt_steps", &local_opt_steps);
   m.def("mlp_forward", &mlp_forward);
   m.def("mlp_net_params", [](int64_t kind) { return (int64_t)colearn::mlp_net_num_params((int)kind); });
   m.def("sgd_step", &sgd_step);

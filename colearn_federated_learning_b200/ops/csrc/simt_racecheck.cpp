@@ -73,6 +73,27 @@ int main() {
       CK(launch_mlp_local_sgd_cw(kind, d.data(), 2, hp, cw, nullptr));
     }
   printf("class-weighted mlp kernels ok\n");
+  // ---- local optimizer instances (mlp_persistent_opt.cu): every net, SGD with nesterov momentum and weight decay, and Adam --------
+  for (int kind = 0; kind < 5; ++kind)
+    for (int opt : {LOCAL_OPT_SGD, LOCAL_OPT_ADAM}) {
+      const int din = kind == 2 ? 2 : 10, dout = kind == 0 || kind == 2 ? 1 : (kind == 1 ? 2 : (kind == 3 ? 10 : 5));
+      const int loss = kind == 0 ? LOSS_BCE : (kind == 2 ? LOSS_SSE : (kind == 3 ? LOSS_MSE : LOSS_XENT));
+      const int ydim = loss == LOSS_XENT ? 1 : dout;
+      const int P = mlp_net_num_params(kind), n = 7;
+      std::vector<float> theta = randv(P, 0.3f), x = randv((size_t)n * din), y((size_t)n * ydim), out0(P), out1(P), lossv(4);
+      for (auto& v : y) v = (float)(rand() % 2);
+      std::vector<ClientDesc> d(2);
+      for (int c = 0; c < 2; ++c) {
+        memset(&d[c], 0, sizeof(ClientDesc));
+        d[c].x = x.data(); d[c].y = y.data(); d[c].theta_in = theta.data();
+        d[c].theta_out = c ? out1.data() : out0.data(); d[c].loss_out = lossv.data() + 2 * c;
+        d[c].n = n; d[c].perm_rows = 1; d[c].y_dim = ydim; d[c].out_scale = 0.5f;
+      }
+      const LocalOptArgs lo{opt, opt == LOCAL_OPT_SGD, opt == LOCAL_OPT_SGD ? 0.9f : 0.f, 0.01f, 0.9f, 0.999f, 1e-8f};
+      SgdHyper hp{3, 2, -1, loss, 0.05f, 1};
+      CK(launch_mlp_local_sgd_opt(kind, d.data(), 2, hp, lo, nullptr));
+    }
+  printf("local optimizer mlp kernels ok\n");
   // ---- elementwise (the ones with shared memory / shuffles / atomics) ----------------------------------------------------------
   {
     const int64_t n = 3000;

@@ -138,10 +138,26 @@ def check_class_weights(kind: Optional[int], loss: str, class_weights: Sequence[
     return w
 
 
+def check_local_opt(local_opt, class_weights=None):
+    """The optimizer to launch on the optimizer instances (``csrc/mlp_persistent_opt.cu``), or None for plain SGD (``None`` or
+    a plain ``LocalOpt``: the kernels of before optimizers existed).  ValueError for anything but a ``fl.local_opt.LocalOpt``
+    and for class weights next to an optimizer (the weighted instances are variant 5's, the optimizer instances variant 1's)."""
+    from ..fl.local_opt import LocalOpt
+    if local_opt is None:
+        return None
+    if not isinstance(local_opt, LocalOpt):
+        raise ValueError(f"local_opt must be a fl.local_opt.LocalOpt, got {type(local_opt).__name__}")
+    if local_opt.is_plain():
+        return None
+    if class_weights is not None:
+        raise ValueError("class weights together with a local optimizer are not supported")
+    return local_opt
+
+
 def mlp_local_sgd_multi(dims: Sequence[int], out_activation: str, descs: torch.Tensor, n_clients: int,
                         batch_size: int = 1, lr: float = 0.01, epochs: int = 1, max_nr_batches: int = -1,
                         loss: str = "xent", desc_offset: int = 0, variant: Optional[int] = None,
-                        class_weights: Optional[Sequence[float]] = None) -> None:
+                        class_weights: Optional[Sequence[float]] = None, local_opt=None) -> None:
     """Launch ``n_clients`` CTAs from a packed descriptor tensor (see :func:`build_client_descs`).
 
     The labels behind the descriptors are not checked here (they are device memory the caller packed).  For the
@@ -151,12 +167,22 @@ def mlp_local_sgd_multi(dims: Sequence[int], out_activation: str, descs: torch.T
     same holds for the 0 / 1 labels of a class-weighted FFNN fit.
 
     ``class_weights``: a class-weighted fit (``reference.loss_and_dz``), launched on the weighted instances; the weights, net,
-    loss and variant are checked before the launch (:func:`check_class_weights`)."""
+    loss and variant are checked before the launch (:func:`check_class_weights`).
+
+    ``local_opt``: a ``fl.local_opt.LocalOpt``.  None or plain SGD launches what it always launched; any other optimizer
+    launches the optimizer instances (variant 1's shared-memory kernel with the ``local_opt.cuh`` step), whatever ``variant``
+    says."""
     kind = net_kind_for(dims, out_activation)
     if kind is None:
         raise ValueError(f"no persistent-kernel instantiation for dims={tuple(dims)} act={out_activation}")
     if loss == "bce" and out_activation != "sigmoid":
         raise ValueError("bce needs a sigmoid head")
+    lo = check_local_opt(local_opt, class_weights)
+    if lo is not None:
+        _ext.require().mlp_local_sgd_opt(kind, descs, int(desc_offset), int(n_clients), int(batch_size), int(epochs),
+                                         int(max_nr_batches if max_nr_batches is not None else -1), LOSS_CODES[loss], float(lr),
+                                         lo.launch_args())
+        return
     args = (kind, descs, int(desc_offset), int(n_clients), int(batch_size), int(epochs),
             int(max_nr_batches if max_nr_batches is not None else -1), LOSS_CODES[loss], float(lr), resolve_variant(kind, variant))
     if class_weights is None:
@@ -170,7 +196,7 @@ def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: t
                   perm: Optional[torch.Tensor], batch_size: int = 1, lr: float = 0.01, epochs: int = 1,
                   max_nr_batches: int = -1, loss: str = "xent", out_activation: str = "none",
                   return_mean: bool = False, variant: Optional[int] = None,
-                  class_weights: Optional[Sequence[float]] = None) -> torch.Tensor:
+                  class_weights: Optional[Sequence[float]] = None, local_opt=None) -> torch.Tensor:
     """Single-client in-place local SGD on ``flat``; returns the last batch loss (0-dim tensor).
 
     CPU tensors run ``reference.mlp_local_sgd`` (identical semantics); CUDA tensors run the
@@ -178,7 +204,11 @@ def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: t
     is not a class index in [0, 5): the kernel's head selects z_y by that index.
 
     ``class_weights``: a class-weighted fit (FFNN: 2 weights, for labels 0 and 1; attack-category net: 5), refused before any
-    launch unless :func:`check_class_weights` accepts it and every label is a class index."""
+    launch unless :func:`check_class_weights` accepts it and every label is a class index.
+
+    ``local_opt``: the fit's ``fl.local_opt.LocalOpt`` (see :func:`mlp_local_sgd_multi`); on CPU the host executor's generic
+    loop or ``reference.mlp_local_sgd`` takes its step."""
+    local_opt = check_local_opt(local_opt, class_weights)
     kind = net_kind_for(dims, out_activation)
     if class_weights is not None:
         class_weights = check_class_weights(kind, loss, class_weights, variant, cuda=flat.is_cuda)
@@ -191,12 +221,13 @@ def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: t
         if (host.available() and flat.dtype == torch.float32 and flat.is_contiguous() and not flat.requires_grad
                 and out_activation in ("none", "sigmoid")):
             res = host.mlp_local_sgd_multi(dims, out_activation, [flat], [x], [y], [perm], batch_size, lr, epochs,
-                                           max_nr_batches, loss, threads=1, class_weights=class_weights)
+                                           max_nr_batches, loss, threads=1, class_weights=class_weights, local_opt=local_opt)
             return res[0, 1 if return_mean else 0].clone()
         if perm is None:
             perm = reference.make_permutation(x.shape[0], epochs, 0, shuffle=False)
         cw = None if class_weights is None else torch.tensor(class_weights, dtype=torch.float32).to(flat.dtype)
-        return reference.mlp_local_sgd(flat, dims, x, y, perm, batch_size, lr, epochs, max_nr_batches, loss, out_activation, cw)
+        return reference.mlp_local_sgd(flat, dims, x, y, perm, batch_size, lr, epochs, max_nr_batches, loss, out_activation, cw,
+                                       local_opt)
     x, y = _prep_xy(x, y, loss)
     loss_out = torch.zeros(2, device=flat.device, dtype=torch.float32)
     if perm is not None:
@@ -204,7 +235,7 @@ def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: t
     task = ClientTask(x=x, y=y, theta_in=flat, theta_out=flat, perm=perm, loss_out=loss_out)
     descs = build_client_descs([task], flat.device)
     mlp_local_sgd_multi(dims, out_activation, descs, 1, batch_size, lr, epochs, max_nr_batches, loss, variant=variant,
-                        class_weights=class_weights)
+                        class_weights=class_weights, local_opt=local_opt)
     return loss_out[1 if return_mean else 0]
 
 

@@ -69,10 +69,12 @@ def _f32(t: torch.Tensor) -> torch.Tensor:
 def mlp_local_sgd_multi(dims: Sequence[int], out_activation: str, thetas: List[torch.Tensor], xs: List[torch.Tensor],
                         ys: List[torch.Tensor], perms: List[Optional[torch.Tensor]], batch_size: int = 1, lr: float = 0.01,
                         epochs: int = 1, max_nr_batches: int = -1, loss: str = "xent", threads: int = 0,
-                        class_weights: Optional[Sequence[float]] = None) -> torch.Tensor:
+                        class_weights: Optional[Sequence[float]] = None, local_opt=None) -> torch.Tensor:
     """Train K clients concurrently, each in place on its own flat fp32 arena (``thetas[i]`` must be contiguous CPU
     fp32 — a row of a ``[K, P]`` matrix is fine).  Returns ``[K, 2]`` = (last batch loss, mean loss over the steps).
-    ``class_weights``: a class-weighted fit (``reference.loss_and_dz``), checked by the caller (``fused_mlp.check_class_weights``)."""
+    ``class_weights``: a class-weighted fit (``reference.loss_and_dz``), checked by the caller (``fused_mlp.check_class_weights``).
+    ``local_opt``: a ``fl.local_opt.LocalOpt`` other than plain SGD, run by the generic loop (the caller refuses it together
+    with class weights)."""
     mod = load()
     if mod is None:
         raise RuntimeError(f"_colearn_host is not built (colearn-build-kernels --host): {last_error()}")
@@ -84,6 +86,10 @@ def mlp_local_sgd_multi(dims: Sequence[int], out_activation: str, thetas: List[t
     perms2 = [None if p is None else p.detach().to(torch.int32).contiguous().view(-1, x.shape[0]) for p, x in zip(perms, xs2)]
     args = ([int(d) for d in dims], out_activation == "sigmoid", list(thetas), xs2, ys2, perms2, int(batch_size), int(epochs),
             int(max_nr_batches if max_nr_batches is not None else -1), LOSS_CODES[loss], float(lr), int(threads))
+    if local_opt is not None and not local_opt.is_plain():
+        if class_weights is not None:
+            raise ValueError("class weights together with a local optimizer are not supported")
+        return mod.mlp_local_sgd_opt(*args, local_opt.launch_args())
     if class_weights is None:
         return mod.mlp_local_sgd(*args)
     return mod.mlp_local_sgd_cw(*args, [float(w) for w in class_weights])

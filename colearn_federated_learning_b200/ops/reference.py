@@ -145,13 +145,58 @@ def total_steps(n: int, batch_size: int, epochs: int, max_nr_batches: int = -1) 
     return steps
 
 
+def _sqrt_rn(t: torch.Tensor) -> torch.Tensor:
+    """Correctly rounded square root: torch's vectorised float32 sqrt is not (it can be 1 ulp off), the float64 one rounded
+    to float32 is (53 >= 2 * 24 + 2 bits)"""
+    return torch.sqrt(t.double()).float() if t.dtype == torch.float32 else torch.sqrt(t)
+
+
+def local_opt_state(flat: torch.Tensor) -> dict:
+    """Fresh state of a local optimizer for one fit: step count 0, moments 0, Adam's running products 1"""
+    one = torch.ones((), dtype=flat.dtype)
+    return {"t": 0, "m": torch.zeros_like(flat), "v": torch.zeros_like(flat), "p1": one, "p2": one.clone()}
+
+
+def local_opt_step(flat: torch.Tensor, g: torch.Tensor, local_opt, lr: float, state: dict) -> None:
+    """One step of a local optimizer (``fl/local_opt.py``) on ``flat`` in place, from the batch gradient ``g``: the
+    operation order of ``csrc/local_opt.cuh``, one rounding per operation in ``flat``'s dtype (every scalar is cast to it
+    first)."""
+    dt = flat.dtype
+    c = lambda v: torch.tensor(v, dtype=torch.float32).to(dt)            # noqa: E731  the fp32 hyper-parameter the kernel holds
+    lr_t = c(lr)
+    state["t"] += 1
+    if local_opt.weight_decay != 0.0:
+        g = g + c(local_opt.weight_decay) * flat
+    m, v = state["m"], state["v"]
+    if local_opt.kind == "Adam":
+        b1, b2 = c(local_opt.betas[0]), c(local_opt.betas[1])
+        one = torch.ones((), dtype=dt)
+        state["p1"] = state["p1"] * b1
+        state["p2"] = state["p2"] * b2
+        s = lr_t / (one - state["p1"])
+        r = _sqrt_rn(one - state["p2"])
+        m.copy_(b1 * m + (one - b1) * g)
+        v.copy_(b2 * v + (one - b2) * (g * g))
+        flat.copy_(flat - (s * m) / (_sqrt_rn(v) / r + c(local_opt.eps)))
+        return
+    d = g
+    if local_opt.momentum != 0.0:
+        mu = c(local_opt.momentum)
+        m.copy_(g if state["t"] == 1 else mu * m + g)
+        d = g + mu * m if local_opt.nesterov else m
+    flat.copy_(flat - lr_t * d)
+
+
 def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: torch.Tensor,
                   perm: torch.Tensor, batch_size: int = 1, lr: float = 0.01, epochs: int = 1,
                   max_nr_batches: int = -1, loss: str = "xent", out_activation: str = "none",
-                  class_weights: Optional[torch.Tensor] = None) -> torch.Tensor:
+                  class_weights: Optional[torch.Tensor] = None, local_opt=None) -> torch.Tensor:
     """In-place local SGD on the flat arena; returns the last batch's loss (0-dim tensor).
 
     ``class_weights``: a class-weighted fit (see :func:`loss_and_dz`), the definition the kernels and the host executor follow.
+
+    ``local_opt``: a ``fl.local_opt.LocalOpt`` other than plain SGD takes :func:`local_opt_step` per batch, with state that
+    starts fresh for this fit; None (or plain SGD) is ``flat -= lr * g``.
 
     ``max_nr_batches``: PySyft stops when ``it >= max_nr_batches >= 0`` *after* a step, so 0
     behaves like "one step"; negative means unlimited.  We normalise: <= 0 → unlimited except
@@ -160,12 +205,18 @@ def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: t
     it = 0
     last = torch.zeros((), dtype=flat.dtype, device=flat.device)
     limit = max_nr_batches if (max_nr_batches is not None and max_nr_batches > 0) else None
+    if local_opt is not None and local_opt.is_plain():
+        local_opt = None
+    state = local_opt_state(flat) if local_opt is not None else None
     for e in range(epochs):
         order = perm[e % perm.shape[0]].long()
         for lo in range(0, n, batch_size):
             idx = order[lo:lo + batch_size]
             last, g = mlp_grad(flat, dims, x[idx], y[idx], loss, out_activation, class_weights)
-            flat.sub_(lr * g)
+            if state is None:
+                flat.sub_(lr * g)
+            else:
+                local_opt_step(flat, g, local_opt, lr, state)
             it += 1
             if limit is not None and it >= limit:
                 return last

@@ -391,7 +391,7 @@ class BoxService:
                                       local_epochs=args.epochs, max_batches=max_batches, loss=args.loss, weighted=args.weighted,
                                       server_lr=args.server_lr if sgd else 1.0, seed=args.seed,
                                       server_opt=None if sgd else args.server_optimizer(),
-                                      aggregator=args.client_aggregator(),
+                                      aggregator=args.client_aggregator(), local_opt=args.local_opt(),
                                       bf16_shadow=on_gpu and getattr(args, "dtype", "fp32") == "bf16",
                                       clients_per_rank=getattr(cli, "clients_per_gpu", 1) if on_gpu else 1,
                                       round_deadline_ms=float(getattr(cli, "round_deadline_ms", 0.0) or 0.0))

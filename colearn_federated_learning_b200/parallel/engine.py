@@ -36,6 +36,7 @@ from .. import ops
 from ..fl.aggregate import Aggregator
 from ..fl.fedavg import normalized_weights
 from ..fl.server_opt import ServerOpt, resolve_server_opt
+from ..fl.local_opt import LocalOpt, refuse_non_plain, resolve as resolve_local_opt
 from ..fl.trainer import FitConfig, local_fit, resolve_loss
 from ..models import MLPNet, build_model, flatten_params, num_params, state_dict_from_flat
 from ..utils.checkpoint import save_state_dict
@@ -71,8 +72,11 @@ class FederatedEngine:
                  round_deadline_ms: float = 0.0, clients_per_rank: int = 1,
                  model_kwargs: Optional[Dict[str, Any]] = None, overlap_reduce: Optional[bool] = None,
                  phase_timing: Optional[bool] = None, server_opt: Optional[ServerOpt] = None,
-                 aggregator: Optional[Aggregator] = None) -> None:
-        """``aggregator``: how the client models become the average the server steps towards (``fl/aggregate.py``):
+                 aggregator: Optional[Aggregator] = None, local_opt: Optional[LocalOpt] = None) -> None:
+        """``local_opt``: the clients' local optimizer (``fl/local_opt.py``); anything but plain SGD trains on the persistent
+        kernel's optimizer instances and needs the star path (a persistent-kernel model).
+
+        ``aggregator``: how the client models become the average the server steps towards (``fl/aggregate.py``):
         the weighted FedAvg mean (default) or the coordinate-wise ``median`` / ``trimmed_mean``.  The robust kinds are
         unweighted, so ``weighted`` does not apply to them; they need one client per rank (``clients_per_rank == 1``) and take
         the P2P path of the two-shot kernel (no NVLS)."""
@@ -98,7 +102,8 @@ class FederatedEngine:
         self.P = num_params(self.model)
         self.P4 = (self.P + 3) // 4 * 4
         self.cfg = FitConfig(model=model, loss=resolve_loss(model, loss), batch_size=batch_size, epochs=local_epochs,
-                             max_nr_batches=max_batches, lr=lr, shuffle=shuffle, seed=seed)
+                             max_nr_batches=max_batches, lr=lr, shuffle=shuffle, seed=seed).with_local_opt(local_opt)
+        self.local_opt = resolve_local_opt(local_opt)
         self.weighted = weighted
         # server optimizer (fl/server_opt.py): plain FedAvg with server_lr unless a ServerOpt is given (it carries its own lr)
         self.server_opt = resolve_server_opt(server_opt, server_lr)
@@ -110,6 +115,8 @@ class FederatedEngine:
         if algo == "star" and backend == "fused" and not persistent:
             raise ValueError(f"algo 'star' needs a persistent-kernel model, got {model}")
         self.algo = algo
+        if algo == "twoshot":
+            refuse_non_plain(self.local_opt, f"the two-shot / layer-wise engine path of {model}")
         if algo == "twoshot" and round_deadline_ms > 0 and self.server_opt.kind != "sgd":
             raise ValueError(f"server_opt={self.server_opt.kind!r} cannot run on the two-shot path with a round deadline: the "
                              "optimizer moments are sharded by chunk owner, and with a deadline chunk ownership moves with the set "
@@ -410,7 +417,7 @@ class FederatedEngine:
                 row0 = self.rounds_done * cfg.epochs
                 perm = ops.device_permutation(self.n_local, row0 + cfg.epochs, pseed, dev)[row0:].contiguous()
             ops.mlp_local_sgd(local, self.spec.dims, self.x, self.y, perm, cfg.batch_size, cfg.lr, cfg.epochs, cfg.max_nr_batches,
-                              cfg.loss, self.spec.out_activation)
+                              cfg.loss, self.spec.out_activation, local_opt=self.local_opt)
             contrib = local * w
         if self.aggregator.robust:
             avg = self._robust_average(contrib, mask)                                     # K2 + K3, library form (gather)
@@ -571,7 +578,8 @@ class FederatedEngine:
             if (masks[i] >> r) & 1:
                 with self._phase("local_fit"):
                     ops.mlp_local_sgd_multi(self.spec.dims, self.spec.out_activation, descs, C, cfg.batch_size, cfg.lr,
-                                            cfg.epochs, cfg.max_nr_batches, cfg.loss, desc_offset=desc_base + i * C)
+                                            cfg.epochs, cfg.max_nr_batches, cfg.loss, desc_offset=desc_base + i * C,
+                                            local_opt=self.local_opt)
                     launches += 1
                     if C > 1:
                         ext.reduce_push(self.client_slots.data_ptr(), C, P4, P4, coord_slots, self.client_losses.data_ptr(),

@@ -102,6 +102,16 @@ def build_parser() -> argparse.ArgumentParser:
                              "weights >= 0 (local and remote mode; balanced not with --secure-agg)")
     parser.add_argument("--class-weight-max", type=float, default=d.class_weight_max, metavar="M",
                         help="--class-weight balanced: the cap of every class weight (> 0)")
+    parser.add_argument("--local-optimizer", choices=["SGD", "Adam"], default=d.local_optimizer,
+                        help="the devices' local optimizer, as torch.optim names it; fresh moments every fit (default SGD: the "
+                             "plain step of the reference).  Anything but plain SGD trains the persistent-kernel MLPs only, not "
+                             "with -e or --class-weight")
+    parser.add_argument("--local-momentum", type=float, default=d.local_momentum, help="--local-optimizer SGD: momentum in [0, 1)")
+    parser.add_argument("--local-nesterov", action="store_true", help="--local-optimizer SGD: nesterov momentum (needs momentum > 0)")
+    parser.add_argument("--local-weight-decay", type=float, default=d.local_weight_decay, help="local optimizer: L2 weight decay (>= 0)")
+    parser.add_argument("--local-betas", default=",".join(str(b) for b in d.local_betas), metavar="B1,B2",
+                        help="--local-optimizer Adam: beta1,beta2, each in [0, 1)")
+    parser.add_argument("--local-eps", type=float, default=d.local_eps, help="--local-optimizer Adam: eps (> 0)")
     parser.add_argument("--select", type=int, default=None, help="train at most k of the collected workers")
     parser.add_argument("--selection", choices=["all", "first", "random"], default="all")
     parser.add_argument("--checkpoint", type=str, default="./test.pth")
@@ -213,6 +223,18 @@ def arguments_from_cli(ns: argparse.Namespace) -> Arguments:
     a.async_settings()                # rejects negative settings and --async-buffer with --secure-agg or a compressed downlink
     a.class_weight = getattr(ns, "class_weight", a.class_weight)
     a.class_weight_max = getattr(ns, "class_weight_max", a.class_weight_max)
+    a.local_optimizer = getattr(ns, "local_optimizer", a.local_optimizer)
+    a.local_momentum = getattr(ns, "local_momentum", a.local_momentum)
+    a.local_nesterov = getattr(ns, "local_nesterov", a.local_nesterov)
+    a.local_weight_decay = getattr(ns, "local_weight_decay", a.local_weight_decay)
+    betas = getattr(ns, "local_betas", None)
+    if betas is not None:
+        try:
+            a.local_betas = tuple(float(b) for b in str(betas).split(","))
+        except ValueError:
+            raise ValueError(f"--local-betas takes two numbers b1,b2, got {betas!r}") from None
+    a.local_eps = getattr(ns, "local_eps", a.local_eps)
+    a.local_opt()                     # rejects settings out of range (momentum, betas in [0, 1), eps > 0, weight decay >= 0)
     return a
 
 
@@ -316,6 +338,13 @@ def parse_cli(argv=None) -> argparse.Namespace:
             check_model(build_model(ns.model))
         except ValueError as e:
             parser.error(f"--fed-eval-every with --model {ns.model}: {e}")
+    lopt = arguments_from_cli(ns).local_opt()
+    if not lopt.is_plain():
+        if ns.encryption:
+            parser.error(f"--local-optimizer {lopt.kind} {lopt.args()} does not apply to -e: the SMPC trainer is fixed-point SGD")
+        if ns.class_weight is not None:
+            parser.error("--class-weight together with a local optimizer other than plain SGD is not supported: the class-weighted "
+                         "kernels are the register-resident ones, the optimizer kernels keep their weights in shared memory")
     from colearn_federated_learning_b200.fl import targets
     try:
         targets.of(ns.model).check_settings(ns, box=ns.box, encryption=ns.encryption)
