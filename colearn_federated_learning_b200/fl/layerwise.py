@@ -15,6 +15,12 @@ averages); bf16 shadows of the three 4096×4096 layers are *views into the bf16 
 the two-shot FedAvg kernel fills over NVLink, so the first forward GEMM of a round can poll the
 per-chunk ready flags and start on the rows that have landed (fused broadcast → GEMM, SURVEY K1).
 The 10-wide input and 2-wide head are zero-padded to tile multiples (128).
+
+A local optimizer other than plain SGD (``fl/local_opt.py``: momentum, nesterov, weight decay, Adam) takes its step wherever the
+plain fit applies ``lr``: in the wgrad epilogue of the exact layers (``gemm_wgmma_opt_kernel``, still no dW), and through
+``ops.local_opt_apply`` on the padded edge layers' fp32 dW, the head bias and the hidden biases' epilogue partials.  Its moments
+are arena-shaped (``m``, and ``v`` for Adam), allocated on the first such fit and zeroed at the start of every fit; the step
+scalars run over the fit's batches on the host.
 """
 from __future__ import annotations
 
@@ -25,6 +31,7 @@ import torch
 
 from .. import ops
 from ..ops import conv as conv_ops
+from ..ops import reference
 from ..models import MLPSpec
 
 PAD = 128
@@ -125,6 +132,10 @@ class LayerwiseMLPTrainer:
         self.dw_edge = {l: torch.zeros(self.kp[l + 1], self.kp[l], device=dev) for l in range(self.L) if not self.exact[l]}
         self.launches = 0
         self._wt_fresh = [False] * self.L                     # W_l^T matches the bf16 shadow W_l
+        # local optimizer moments, arena-shaped over the parameters (allocated by the first fit that needs them)
+        self.n_params = self.offsets[self.L - 1][1] + self.dims[self.L]
+        self.opt_m: Optional[torch.Tensor] = None
+        self.opt_v: Optional[torch.Tensor] = None
 
     # -- parameter views -----------------------------------------------------------------------------
     def _w(self, flat: torch.Tensor, l: int) -> torch.Tensor:
@@ -233,14 +244,26 @@ class LayerwiseMLPTrainer:
         self.launches += L + 1 + (0 if self.wgrad_mn else 2)       # own kernels: L GEMMs, the loss, two transposes
         return loss_val
 
-    def backward(self, flat: torch.Tensor, lr: float, produced=None) -> None:
+    def _opt(self, opt, lo: int, shape) -> Tuple:
+        """``ops`` argument of a local-optimizer step on the parameters at arena elements ``[lo, lo + numel)`` viewed as
+        ``shape``: ``(LocalOpt, step state, m, v)`` with the moments' views of the same elements (None where not kept)"""
+        n = 1
+        for d in shape:
+            n *= d
+        view = lambda t: None if t is None else t[lo:lo + n].view(shape)   # noqa: E731
+        return (opt[0], opt[1], view(self.opt_m), view(self.opt_v))
+
+    def backward(self, flat: torch.Tensor, lr: float, produced=None, opt=None) -> None:
         """dgrad with the old weights first, then the (fused) update of layer l.
 
         ``produced`` (:class:`ops.produced.ProducedSpec`, last step of a round only): fused wgrad → FedAvg reduce.  The
         fused-SGD epilogues report the blocks of final parameters they wrote and everything else that finalises a piece
         of the arena is followed by ``produced.mark`` — every arena element exactly once — so that the overlapped
         two-shot kernel reduces layer ``l`` while layers ``l-1 … 0`` are still in their backward pass.  Wᵀ is not
-        rebuilt on that step (the next round derives it from the broadcast)."""
+        rebuilt on that step (the next round derives it from the broadcast).
+
+        ``opt = (LocalOpt, step state)`` (from :meth:`fit`, never next to ``produced``): the local optimizer's step replaces every
+        ``lr`` update, with the moments of this trainer."""
         L = self.L
         end = self.offsets[L - 1][1] + self.dims[L]              # first element after the parameters (arena tail)
         if produced is not None:
@@ -252,7 +275,12 @@ class LayerwiseMLPTrainer:
                 ops.gemm_bf16(self.dz[l], self.Ws[l] if self.dgrad_kn else self.WsT[l], b_kn=self.dgrad_kn, relu_mask=self.a[l],
                               out_bf16=self.dz[l - 1], out_bf16_t=self.dzT[l - 1], colsum=self.dbp[l - 1],
                               max_ctas=produced.max_ctas if produced is not None else 0)
-            if self.exact[l]:
+            wshape = (self.dims[l + 1], self.dims[l])
+            if self.exact[l] and opt is not None:
+                self._wgrad(l, sgd_master=self._w(flat, l), sgd_lr=lr, sgd_shadow=self.Ws[l],
+                            opt=self._opt(opt, self.offsets[l][0], wshape))
+                self._wt_fresh[l] = False
+            elif self.exact[l]:
                 # fused SGD on the fp32 master + bf16 shadow; W^T is rebuilt by the coalesced transpose kernel
                 # (2-byte transposed stores from the epilogue cost more than a separate 64 MB pass)
                 self._wgrad(l, sgd_master=self._w(flat, l), sgd_lr=lr, sgd_shadow=self.Ws[l],
@@ -261,14 +289,22 @@ class LayerwiseMLPTrainer:
             else:
                 self._wgrad(l, out_f32=self.dw_edge[l])
                 w = self._w(flat, l)
-                w.sub_(self.dw_edge[l][: w.shape[0], : w.shape[1]], alpha=lr)
+                if opt is not None:
+                    ops.local_opt_apply(w, self.dw_edge[l][: w.shape[0]], self._opt(opt, self.offsets[l][0], wshape), lr)
+                else:
+                    w.sub_(self.dw_edge[l][: w.shape[0], : w.shape[1]], alpha=lr)
                 self.Ws[l][: w.shape[0], : w.shape[1]].copy_(w)
                 self._wt_fresh[l] = False
                 if produced is not None:
                     produced.mark(self.offsets[l][0], self.offsets[l][0] + w.numel())
             b = self._b(flat, l)
-            if l == L - 1:
+            bopt = self._opt(opt, self.offsets[l][1], (1, b.shape[0])) if opt is not None else None
+            if l == L - 1 and opt is not None:
+                ops.local_opt_apply(b.view(1, -1), self.db[l].view(1, -1), bopt, lr)
+            elif l == L - 1:
                 b.sub_(self.db[l][: b.shape[0]], alpha=lr)          # head: gradient came from the loss kernel
+            elif opt is not None:                                    # hidden: the epilogue partials, summed as below
+                ops.local_opt_apply(b.view(1, -1), self.dbp[l], bopt, lr, g_rows=self.dbp[l].shape[0])
             else:
                 ops.bias_sgd_from_partials(b, self.dbp[l], lr)       # hidden: reduce the epilogue partials + SGD
             if not self.exact[l]:
@@ -276,6 +312,8 @@ class LayerwiseMLPTrainer:
             if produced is not None:
                 produced.mark(self.offsets[l][1], self.offsets[l][1] + b.shape[0])
         self.launches += 2 * L + 4
+        if opt is not None:                                          # the edge layers' and the head bias's steps
+            self.launches += sum(1 for e in self.exact if not e) + 1
 
     def _wgrad(self, l: int, **epilogue) -> None:
         """``dW_l = dz_lᵀ · a_l`` with the given epilogue: K-major operands from the transposed copies, or the MN-major form."""
@@ -296,8 +334,21 @@ class LayerwiseMLPTrainer:
             steps = min(steps, cfg.max_nr_batches)
         return steps
 
+    def _start_opt(self, local_opt) -> None:
+        """Moments of a fresh fit: allocated on first use (plain SGD allocates nothing), zeroed at the start of every fit"""
+        need_m = local_opt.kind == "Adam" or local_opt.momentum != 0.0
+        need_v = local_opt.kind == "Adam"
+        if need_m and self.opt_m is None:
+            self.opt_m = torch.zeros(self.n_params, device=self.dev)
+        if need_v and self.opt_v is None:
+            self.opt_v = torch.zeros(self.n_params, device=self.dev)
+        for t, need in ((self.opt_m, need_m), (self.opt_v, need_v)):
+            if need:
+                t.zero_()
+
     def fit(self, flat: torch.Tensor, x: torch.Tensor, y: torch.Tensor, cfg, perm: Optional[torch.Tensor],
-            ready: Optional[ReadySpec] = None, wait_chunks=None, produced=None, before_last_backward=None) -> torch.Tensor:
+            ready: Optional[ReadySpec] = None, wait_chunks=None, produced=None, before_last_backward=None,
+            local_opt=None) -> torch.Tensor:
         """Local SGD in place on ``flat`` (full batches only; a tail < batch_size is dropped).
 
         With ``ready`` (fused broadcast consumption) the order is: wait only for the chunks of the
@@ -307,7 +358,20 @@ class LayerwiseMLPTrainer:
 
         ``produced`` + ``before_last_backward`` (fused wgrad → FedAvg reduce): the backward of the round's LAST step
         reports what it finalises (:meth:`backward`); the callback runs right before it is queued — the engine launches
-        the overlapped two-shot kernel on its side stream there."""
+        the overlapped two-shot kernel on its side stream there.
+
+        ``local_opt`` (``fl/local_opt.LocalOpt``): the fit's optimizer; None or plain SGD runs the kernels of the plain fit.  Its
+        state lives for this fit (moments 0, step count over the fit's batches across its epochs).  It is refused next to
+        ``ready`` / ``produced`` / ``before_last_backward`` (the engine's fused round trains with plain SGD)."""
+        from .local_opt import resolve
+        lopt = resolve(local_opt)
+        if lopt is not None and (ready is not None or produced is not None or before_last_backward is not None):
+            raise ValueError(f"local optimizer {lopt.kind}: the fused-broadcast / fused-reduce round of the layer-wise trainer "
+                             "trains with plain SGD only")
+        opt = None
+        if lopt is not None:
+            self._start_opt(lopt)
+            opt = (lopt, reference.local_opt_clock())
         n, b = x.shape[0], self.b
         total = self.n_steps(n, cfg)
         if ready is not None and wait_chunks is not None:
@@ -335,7 +399,9 @@ class LayerwiseMLPTrainer:
                 final = produced is not None and it == total - 1
                 if final and before_last_backward is not None:
                     before_last_backward()
-                self.backward(flat, cfg.lr, produced if final else None)
+                if opt is not None:
+                    reference.local_opt_next(opt[1], lopt, cfg.lr)
+                self.backward(flat, cfg.lr, produced if final else None, opt)
                 it += 1
                 if limit is not None and it >= limit:
                     return last

@@ -16,7 +16,8 @@ gradient ``g`` the kernels form (the mean over the batch; a sum for ``sse``)::
 
 ``ops/csrc/local_opt.cuh`` writes that operation order down for the kernels and the host executor, and
 ``ops.reference.local_opt_step`` for PyTorch.  Plain SGD (no momentum, no weight decay) is today's fit and runs the kernels it
-always ran; any other optimizer trains on the persistent kernel's optimizer instances (``ops.mlp_local_sgd(local_opt=...)``).
+always ran; any other optimizer trains on the persistent kernel's optimizer instances (``ops.mlp_local_sgd(local_opt=...)``), or on
+the layer-wise wgmma trainer's optimizer epilogue (``fl/layerwise.py``) for the MLPs that have no persistent kernel.
 """
 from __future__ import annotations
 
@@ -153,4 +154,4 @@ def refuse_non_plain(local_opt: Optional[LocalOpt], what: str) -> None:
     """ValueError when a trainer without optimizer instances is asked for anything but plain SGD"""
     if resolve(local_opt) is not None:
         raise ValueError(f"local optimizer {local_opt.kind} {local_opt.args()}: {what} trains with plain SGD only "
-                         "(momentum, weight decay and Adam run on the persistent-kernel MLPs)")
+                         "(momentum, weight decay and Adam run on the persistent-kernel MLPs and the layer-wise MLP trainer)")

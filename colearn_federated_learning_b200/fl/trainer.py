@@ -184,10 +184,9 @@ def local_fit(flat: torch.Tensor, model: nn.Module, x: torch.Tensor, y: torch.Te
         if flat.is_cuda:
             from .layerwise import LayerwiseMLPTrainer
             if LayerwiseMLPTrainer.supports(spec, cfg):
-                refuse_non_plain(lopt, f"the layer-wise trainer of {cfg.model} (MLP {tuple(spec.dims)})")
                 tr = LayerwiseMLPTrainer.cached(spec, flat, cfg.batch_size)
                 before = tr.launches
-                last = tr.fit(flat, xx, y, cfg, perm)
+                last = tr.fit(flat, xx, y, cfg, perm, local_opt=lopt)
                 LAST_FIT_LAUNCHES = tr.launches - before
                 return last, "layerwise"
     if conv_path(flat.device) == "native":

@@ -441,4 +441,4 @@ def l2_flush(buf: torch.Tensor) -> None:
         buf.fill_(1.0)
 
 
-from .linear import gemm_bf16, linear_forward, transpose_bf16, bias_sgd_from_partials  # noqa: E402,F401
+from .linear import gemm_bf16, linear_forward, transpose_bf16, bias_sgd_from_partials, local_opt_apply  # noqa: E402,F401

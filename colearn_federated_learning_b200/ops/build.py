@@ -47,7 +47,7 @@ def _stamp(src: str, flags: List[str]) -> str:
     h = hashlib.sha1()
     with open(src, "rb") as f:
         h.update(f.read())
-    for dep in ("colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "mlp_v2.cuh", "mlp_v2_fit.inc", "mlp_v1_fit.inc", "local_opt.cuh", "mlp_persistent.cu", "conv_ops.cuh", "conv_bindings.inc"):
+    for dep in ("colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "mlp_v2.cuh", "mlp_v2_fit.inc", "mlp_v1_fit.inc", "local_opt.cuh", "mlp_persistent.cu", "conv_ops.cuh", "conv_bindings.inc", "gemm_wgmma_body.inc"):
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(flags).encode())
@@ -147,7 +147,7 @@ def build_simt_emul(force: bool = False) -> str:
                                                                         f"-DTORCH_EXTENSION_NAME={SIMT_NAME}"]
     sources = ["simt_emul.cpp", "simt_mlp.cpp", "simt_mlp_ae.cpp", "simt_mlp_cat.cpp", "simt_mlp_cw.cpp", "simt_mlp_opt.cpp", "simt_elementwise.cpp", "simt_comm.cpp", "simt_convnet.cpp", "simt_gemm.cpp"]
     h = hashlib.sha1()
-    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_persistent_ae.cu", "mlp_persistent_cat.cu", "mlp_persistent_cw.cu", "mlp_persistent_opt.cu", "mlp_v2.cuh", "mlp_v2_fit.inc", "mlp_v1_fit.inc", "local_opt.cuh", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "conv_ops.cuh"]:
+    for dep in sources + ["host_shim.h", "mlp_persistent.cu", "mlp_persistent_ae.cu", "mlp_persistent_cat.cu", "mlp_persistent_cw.cu", "mlp_persistent_opt.cu", "mlp_v2.cuh", "mlp_v2_fit.inc", "mlp_v1_fit.inc", "local_opt.cuh", "elementwise.cu", "comm.cu", "convnet.cu", "gemm_wgmma.cu", "gemm_wgmma_body.inc", "gemm_host_model.h", "conv_bindings.inc", "colearn_kernels.h", "server_opt.cuh", "robust_agg.cuh", "uplink_quant.cuh", "uplink_topk.cuh", "downlink.cuh", "secagg.cuh", "distance_agg.cuh", "eval_summary.cuh", "recon_summary.cuh", "conv_ops.cuh"]:
         with open(os.path.join(CSRC, dep), "rb") as f:
             h.update(f.read())
     h.update(" ".join(cxx_flags).encode())

@@ -113,6 +113,42 @@ void mlp_local_sgd_opt(int64_t net_kind, torch::Tensor descs, int64_t desc_offse
   const ClientDesc* d = reinterpret_cast<const ClientDesc*>(descs.data_ptr<uint8_t>()) + desc_offset;
   check(launch_mlp_local_sgd_opt((int)net_kind, d, (int)n_clients, hp, lo, cur_stream()), "mlp_local_sgd_opt launch");
 }
+// the local optimizer of the layer-wise trainer: opt as above, step = {t, p1, p2, s, r} (LocalOptStep) of the current step,
+// advanced on the host (reference.local_opt_next)
+static LocalOptArgs local_opt_args(const std::vector<double>& opt) {
+  TORCH_CHECK(opt.size() == 7, "local optimizer: 7 values");
+  TORCH_CHECK((int)opt[0] == LOCAL_OPT_SGD || (int)opt[0] == LOCAL_OPT_ADAM, "local optimizer: unknown kind");
+  return LocalOptArgs{(int)opt[0], (int)opt[1], (float)opt[2], (float)opt[3], (float)opt[4], (float)opt[5], (float)opt[6]};
+}
+static LocalOptStep local_opt_step_of(const std::vector<double>& step) {
+  TORCH_CHECK(step.size() == 5 && step[0] >= 1, "local optimizer step: {t >= 1, p1, p2, s, r}");
+  LocalOptStep st;
+  st.t = (int)step[0]; st.p1 = (float)step[1]; st.p2 = (float)step[2]; st.s = (float)step[3]; st.r = (float)step[4];
+  return st;
+}
+// m / v of a parameter block: CUDA fp32 with the parameter's sizes and strides; required where the optimizer keeps them
+static float* local_opt_moment(const c10::optional<torch::Tensor>& t, const torch::Tensor& param, bool needed, const char* name) {
+  TORCH_CHECK(t.has_value() || !needed, name, ": this optimizer keeps it, pass the buffer");
+  if (!t.has_value()) return nullptr;
+  TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->sizes() == param.sizes() && t->strides() == param.strides(),
+              name, ": CUDA fp32 with the parameter's sizes and strides");
+  return t->data_ptr<float>();
+}
+// theta [rows, cols] (unit column stride) takes the local optimizer step from grad [rows * g_rows, >= cols] (unit column stride),
+// g_rows consecutive gradient rows summed per parameter row (the dgrad epilogue's bias-gradient partials)
+void local_opt_apply(torch::Tensor theta, torch::Tensor grad, int64_t g_rows, c10::optional<torch::Tensor> m, c10::optional<torch::Tensor> v,
+                     double lr, std::vector<double> opt, std::vector<double> step) {
+  TORCH_CHECK(theta.is_cuda() && theta.scalar_type() == at::kFloat && theta.dim() == 2 && theta.stride(1) == 1, "theta: CUDA fp32 [rows, cols]");
+  TORCH_CHECK(grad.is_cuda() && grad.scalar_type() == at::kFloat && grad.dim() == 2 && grad.stride(1) == 1 && g_rows >= 1 &&
+              grad.size(0) == theta.size(0) * g_rows && grad.size(1) >= theta.size(1), "grad: CUDA fp32 [rows * g_rows, >= cols]");
+  const LocalOptArgs a = local_opt_args(opt);
+  float* mp = local_opt_moment(m, theta, a.kind == LOCAL_OPT_ADAM || a.momentum != 0.f, "m");
+  float* vp = local_opt_moment(v, theta, a.kind == LOCAL_OPT_ADAM, "v");
+  c10::cuda::CUDAGuard guard(theta.device());
+  check(launch_local_opt_apply(theta.data_ptr<float>(), theta.stride(0), grad.data_ptr<float>(), grad.stride(0), (int)g_rows, mp, vp,
+                               (int)theta.size(0), (int)theta.size(1), a, local_opt_step_of(step), (float)lr, cur_stream()),
+        "local_opt_apply");
+}
 int64_t mlp_net_params(int64_t net_kind) { return mlp_net_num_params((int)net_kind); }
 int64_t mlp_smem_bytes(int64_t net_kind, int64_t batch) { return mlp_local_sgd_smem_bytes((int)net_kind, (int)batch); }
 
@@ -845,15 +881,15 @@ void produced_mark(int64_t sig, int64_t chunk_elems, int64_t lo, int64_t hi) {
 }
 
 // ---- wgmma GEMM ------------------------------------------------------------------------------------------
-void gemm_tcgen05(torch::Tensor A, torch::Tensor B, c10::optional<torch::Tensor> bias, bool relu,
-                  c10::optional<torch::Tensor> relu_mask, c10::optional<torch::Tensor> out_bf16,
-                  c10::optional<torch::Tensor> out_f32, c10::optional<torch::Tensor> out_bf16_t,
-                  c10::optional<torch::Tensor> sgd_master, double sgd_lr, c10::optional<torch::Tensor> sgd_shadow,
-                  c10::optional<torch::Tensor> sgd_shadow_t, c10::optional<torch::Tensor> colsum,
-                  int64_t ready_flags, int64_t ready_epoch, int64_t ready_chunk_elems, int64_t ready_elem_offset, int64_t tile_n,
-                  int64_t ready_epoch_ptr, int64_t cluster, int64_t split_k, c10::optional<torch::Tensor> split_out,
-                  int64_t mn_m, bool b_kn, c10::optional<torch::Tensor> addend, std::vector<int64_t> conv,
-                  std::vector<int64_t> produced) {
+static void gemm_run(torch::Tensor A, torch::Tensor B, c10::optional<torch::Tensor> bias, bool relu,
+                     c10::optional<torch::Tensor> relu_mask, c10::optional<torch::Tensor> out_bf16,
+                     c10::optional<torch::Tensor> out_f32, c10::optional<torch::Tensor> out_bf16_t,
+                     c10::optional<torch::Tensor> sgd_master, double sgd_lr, c10::optional<torch::Tensor> sgd_shadow,
+                     c10::optional<torch::Tensor> sgd_shadow_t, c10::optional<torch::Tensor> colsum,
+                     int64_t ready_flags, int64_t ready_epoch, int64_t ready_chunk_elems, int64_t ready_elem_offset, int64_t tile_n,
+                     int64_t ready_epoch_ptr, int64_t cluster, int64_t split_k, c10::optional<torch::Tensor> split_out,
+                     int64_t mn_m, bool b_kn, c10::optional<torch::Tensor> addend, std::vector<int64_t> conv,
+                     std::vector<int64_t> produced, const GemmOptEpilogue* lopt) {
   TORCH_CHECK(A.is_cuda() && B.is_cuda() && A.scalar_type() == at::kBFloat16 && B.scalar_type() == at::kBFloat16, "A,B must be CUDA bf16");
   TORCH_CHECK(A.dim() == 2 && B.dim() == 2 && A.is_contiguous() && B.is_contiguous(), "A, B must be contiguous matrices");
   // mn_m > 0: "MN-major" operands A[K, a_cols], B[K, N] (C = A^T B, M = mn_m >= a_cols);
@@ -911,6 +947,7 @@ void gemm_tcgen05(torch::Tensor A, torch::Tensor B, c10::optional<torch::Tensor>
     ep.split_out = split_out->data_ptr<float>();
   }
   ep.addend = chk(addend, at::kBFloat16, M, N, "addend");
+  if (lopt != nullptr) ep.lopt = *lopt;
   if (is_conv) {
     convops::ConvAddr& g = ep.conv;
     g.mode = (int)conv[0]; g.flip = (int)conv[1]; g.C = (int)conv[2]; g.KH = (int)conv[3]; g.KW = (int)conv[4]; g.pad = (int)conv[5];
@@ -936,6 +973,43 @@ void gemm_tcgen05(torch::Tensor A, torch::Tensor B, c10::optional<torch::Tensor>
   }
   cudaError_t e = launch_gemm_tcgen05(A.data_ptr(), B.data_ptr(), M, N, K, ep, cur_stream());
   TORCH_CHECK(e == cudaSuccess, "gemm_tcgen05: ", cudaGetErrorString(e), " (", gemm_tcgen05_last_error(), ")");
+}
+void gemm_tcgen05(torch::Tensor A, torch::Tensor B, c10::optional<torch::Tensor> bias, bool relu,
+                  c10::optional<torch::Tensor> relu_mask, c10::optional<torch::Tensor> out_bf16,
+                  c10::optional<torch::Tensor> out_f32, c10::optional<torch::Tensor> out_bf16_t,
+                  c10::optional<torch::Tensor> sgd_master, double sgd_lr, c10::optional<torch::Tensor> sgd_shadow,
+                  c10::optional<torch::Tensor> sgd_shadow_t, c10::optional<torch::Tensor> colsum,
+                  int64_t ready_flags, int64_t ready_epoch, int64_t ready_chunk_elems, int64_t ready_elem_offset, int64_t tile_n,
+                  int64_t ready_epoch_ptr, int64_t cluster, int64_t split_k, c10::optional<torch::Tensor> split_out,
+                  int64_t mn_m, bool b_kn, c10::optional<torch::Tensor> addend, std::vector<int64_t> conv,
+                  std::vector<int64_t> produced) {
+  gemm_run(A, B, bias, relu, relu_mask, out_bf16, out_f32, out_bf16_t, sgd_master, sgd_lr, sgd_shadow, sgd_shadow_t, colsum, ready_flags,
+           ready_epoch, ready_chunk_elems, ready_elem_offset, tile_n, ready_epoch_ptr, cluster, split_k, split_out, mn_m, b_kn, addend, conv,
+           produced, nullptr);
+}
+// The local optimizer of the wgrad (GemmEpilogue::lopt): gemm_tcgen05's arguments, then the moments m and v (fp32 like sgd_master,
+// None where the optimizer keeps none), opt = {kind, nesterov, momentum, weight_decay, beta1, beta2, eps} and the step scalars
+// step = {t, p1, p2, s, r} of this step.  The launcher refuses every other epilogue option next to it.
+void gemm_tcgen05_opt(torch::Tensor A, torch::Tensor B, c10::optional<torch::Tensor> bias, bool relu,
+                      c10::optional<torch::Tensor> relu_mask, c10::optional<torch::Tensor> out_bf16,
+                      c10::optional<torch::Tensor> out_f32, c10::optional<torch::Tensor> out_bf16_t,
+                      c10::optional<torch::Tensor> sgd_master, double sgd_lr, c10::optional<torch::Tensor> sgd_shadow,
+                      c10::optional<torch::Tensor> sgd_shadow_t, c10::optional<torch::Tensor> colsum,
+                      int64_t ready_flags, int64_t ready_epoch, int64_t ready_chunk_elems, int64_t ready_elem_offset, int64_t tile_n,
+                      int64_t ready_epoch_ptr, int64_t cluster, int64_t split_k, c10::optional<torch::Tensor> split_out,
+                      int64_t mn_m, bool b_kn, c10::optional<torch::Tensor> addend, std::vector<int64_t> conv,
+                      std::vector<int64_t> produced, c10::optional<torch::Tensor> m, c10::optional<torch::Tensor> v,
+                      std::vector<double> opt, std::vector<double> step) {
+  TORCH_CHECK(sgd_master.has_value(), "the local optimizer epilogue updates sgd_master");
+  GemmOptEpilogue lo;
+  std::memset(&lo, 0, sizeof(lo));
+  lo.args = local_opt_args(opt);
+  lo.step = local_opt_step_of(step);
+  lo.m = local_opt_moment(m, *sgd_master, lo.args.kind == LOCAL_OPT_ADAM || lo.args.momentum != 0.f, "m");
+  lo.v = local_opt_moment(v, *sgd_master, lo.args.kind == LOCAL_OPT_ADAM, "v");
+  gemm_run(A, B, bias, relu, relu_mask, out_bf16, out_f32, out_bf16_t, sgd_master, sgd_lr, sgd_shadow, sgd_shadow_t, colsum, ready_flags,
+           ready_epoch, ready_chunk_elems, ready_elem_offset, tile_n, ready_epoch_ptr, cluster, split_k, split_out, mn_m, b_kn, addend, conv,
+           produced, &lo);
 }
 
 // ---- NHWC conv / BatchNorm / pooling (convnet.cu); wrappers shared with the host emulator ------------------
@@ -1056,5 +1130,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("enable_peer_access", &enable_peer_access);
   m.def("tensor_from_ptr", &tensor_from_ptr);
   m.def("gemm_tcgen05", &gemm_tcgen05);
+  m.def("gemm_tcgen05_opt", &gemm_tcgen05_opt);
+  m.def("local_opt_apply", &local_opt_apply);
   convbind::register_ops<ConvCudaExec>(m);
 }

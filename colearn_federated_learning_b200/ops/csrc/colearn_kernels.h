@@ -379,6 +379,11 @@ cudaError_t launch_feistel_permutation(int* out, int n, int rows, uint64_t seed,
 cudaError_t launch_fp32_to_bf16(const float* in, void* out, int64_t n, cudaStream_t s);
 cudaError_t launch_l2_flush(float* buf, int64_t n, cudaStream_t s);
 // bias[n] -= lr * sum_r partials[r, n]   (also writes the summed gradient to grad_out if non-null)
+// Local-optimizer step of a strided block (the layer-wise trainer's padded edge layers and biases): theta[r * ld + c] for
+// r < rows, c < cols takes local_opt_elem with the gradient sum_{p < g_rows} grad[(r * g_rows + p) * g_ld + c], added in
+// order of p from 0 as bias_sgd_from_partials_kernel does; m and v (nullptr when the optimizer keeps none) share theta's ld.
+cudaError_t launch_local_opt_apply(float* theta, int64_t ld, const float* grad, int64_t g_ld, int g_rows, float* m, float* v,
+                                   int rows, int cols, LocalOptArgs a, LocalOptStep st, float lr, cudaStream_t s);
 cudaError_t launch_bias_sgd_from_partials(float* bias, const float* partials, int rows, int n, int64_t row_stride,
                                           float lr, float* grad_out, int n_bias, cudaStream_t s);
 // SMPC ring ops (int64, arithmetic mod 2^64)
@@ -518,6 +523,15 @@ cudaError_t launch_p2p_copy(float* dst, const float* src, int64_t n, uint32_t* f
 // ---------------------------------------------------------------------------------------------
 // wgmma GEMM family (gemm_wgmma.cu):  C[M,N] = A[M,K] * B[N,K]^T  (both operands K-major bf16)
 // ---------------------------------------------------------------------------------------------
+// Local optimizer of the layer-wise trainer's wgrad (GemmEpilogue::lopt, read only by gemm_wgmma_opt_kernel): args.kind = 0 is
+// off; LOCAL_OPT_SGD / LOCAL_OPT_ADAM replace the fused SGD of sgd_master by local_opt_elem (local_opt.cuh) with the moments
+// m (SGD with momentum, Adam) and v (Adam), fp32 [M, N] like the master, and the step scalars of this step (advanced on the host)
+struct GemmOptEpilogue {
+  float* m;
+  float* v;
+  LocalOptArgs args;
+  LocalOptStep step;
+};
 struct GemmEpilogue {
   const float* bias;        // [N] or nullptr
   int relu;                 // apply max(0, .)
@@ -562,6 +576,7 @@ struct GemmEpilogue {
   int max_ctas;             // > 0: cap the persistent grid (leave SMs to a communication kernel running next to the GEMM)
   int pdl;                  // 1: launched with the programmatic-dependent-launch attribute; the kernel runs COLEARN_PDL_PROLOGUE
                             // after its own set-up (barrier init and tensor-map prefetch overlap the predecessor)
+  GemmOptEpilogue lopt;     // local-optimizer wgrad (needs sgd_master; no other output, no split_k / cluster / ready / produced)
 };
 // A: [M,K] bf16 row-major, B: [N,K] bf16 row-major.  M%128==0, N%128==0, K%64==0.
 cudaError_t launch_gemm_tcgen05(const void* A, const void* B, int M, int N, int K,

@@ -1823,6 +1823,23 @@ __global__ void bias_sgd_from_partials_kernel(float* __restrict__ bias, const fl
   if (bias && c < n_bias) bias[c] = fmaf(-lr, g, bias[c]);
 }
 
+// local-optimizer step of a strided block (launch_local_opt_apply): one element per thread, grid-stride
+__global__ void local_opt_apply_kernel(float* __restrict__ theta, int64_t ld, const float* __restrict__ grad, int64_t g_ld, int g_rows,
+                                       float* __restrict__ m, float* __restrict__ v, int rows, int cols, LocalOptArgs a, LocalOptStep st,
+                                       float lr) {
+  const int64_t n = (int64_t)rows * cols, stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int64_t r = i / cols, c = i - r * cols;
+    float g = 0.f;
+    for (int p = 0; p < g_rows; ++p) g += grad[(r * g_rows + p) * g_ld + c];
+    const int64_t e = r * ld + c;
+    float mm = m != nullptr ? m[e] : 0.f, vv = v != nullptr ? v[e] : 0.f;
+    local_opt_elem(a, st, lr, theta[e], g, mm, vv);
+    if (m != nullptr) m[e] = mm;
+    if (v != nullptr) v[e] = vv;
+  }
+}
+
 __global__ void l2_flush_kernel(float* __restrict__ buf, int64_t n) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) buf[i] = (float)i;
@@ -2246,6 +2263,13 @@ cudaError_t launch_ring_matmul(const long long* A, const long long* B, long long
 cudaError_t launch_bias_sgd_from_partials(float* bias, const float* partials, int rows, int n, int64_t row_stride, float lr,
                                           float* grad_out, int n_bias, cudaStream_t s) {
   COLEARN_LAUNCH(bias_sgd_from_partials_kernel, (n + 255) / 256, 256, 0, s, bias, partials, rows, n, row_stride, lr, grad_out, n_bias);
+  return cudaGetLastError();
+}
+cudaError_t launch_local_opt_apply(float* theta, int64_t ld, const float* grad, int64_t g_ld, int g_rows, float* m, float* v,
+                                   int rows, int cols, LocalOptArgs a, LocalOptStep st, float lr, cudaStream_t s) {
+  if (rows <= 0 || cols <= 0) return cudaSuccess;
+  COLEARN_LAUNCH(local_opt_apply_kernel, grid_for((int64_t)rows * cols, 1), kThreads, 0, s, theta, ld, grad, g_ld, g_rows, m, v, rows,
+                 cols, a, st, lr);
   return cudaGetLastError();
 }
 cudaError_t launch_l2_flush(float* buf, int64_t n, cudaStream_t s) {

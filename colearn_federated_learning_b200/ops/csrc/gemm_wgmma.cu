@@ -336,6 +336,42 @@ __device__ __forceinline__ void epilogue_chunk(const uint32_t (&v)[32], const Ge
   }
 }
 
+// Local-optimizer epilogue (gemm_wgmma_opt_kernel, OPT = LOCAL_OPT_SGD / LOCAL_OPT_ADAM): the accumulator is the gradient g of
+// master[row, col .. col+31]; every element takes local_opt_elem (local_opt.cuh) on master, its momentum m (SGD with momentum,
+// Adam) and v (Adam), all [M, N] fp32, then the bf16 shadow gets the new weights.  dW is never stored.
+template <int OPT>
+__device__ __forceinline__ void epilogue_opt_chunk(const uint32_t (&v)[32], const GemmEpilogue& ep, int row, int col, int N) {
+  LocalOptArgs a = ep.lopt.args;
+  a.kind = OPT;                                      // the optimizer branch of local_opt_elem folds at compile time
+  const LocalOptStep st = ep.lopt.step;
+  const bool use_m = OPT == LOCAL_OPT_ADAM || a.momentum != 0.f;
+  const size_t base = (size_t)row * N + col;
+  float4* wp = reinterpret_cast<float4*>(ep.sgd_master + base);
+  float4* mp = reinterpret_cast<float4*>(ep.lopt.m + base);
+  float4* vp = reinterpret_cast<float4*>(ep.lopt.v + base);
+  uint4* sp = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(ep.sgd_shadow) + base);
+#pragma unroll
+  for (int h = 0; h < 4; ++h) {            // 8 columns at a time: two float4 of master / moments, one uint4 of shadow
+    float f[8];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int g = h * 2 + q;
+      float4 w = wp[g];
+      float4 m = use_m ? mp[g] : make_float4(0.f, 0.f, 0.f, 0.f);
+      float4 s = OPT == LOCAL_OPT_ADAM ? vp[g] : make_float4(0.f, 0.f, 0.f, 0.f);
+      local_opt_elem(a, st, ep.sgd_lr, w.x, __uint_as_float(v[g * 4 + 0]), m.x, s.x);
+      local_opt_elem(a, st, ep.sgd_lr, w.y, __uint_as_float(v[g * 4 + 1]), m.y, s.y);
+      local_opt_elem(a, st, ep.sgd_lr, w.z, __uint_as_float(v[g * 4 + 2]), m.z, s.z);
+      local_opt_elem(a, st, ep.sgd_lr, w.w, __uint_as_float(v[g * 4 + 3]), m.w, s.w);
+      wp[g] = w;
+      if (use_m) mp[g] = m;
+      if (OPT == LOCAL_OPT_ADAM) vp[g] = s;
+      f[q * 4 + 0] = w.x; f[q * 4 + 1] = w.y; f[q * 4 + 2] = w.z; f[q * 4 + 3] = w.w;
+    }
+    if (ep.sgd_shadow != nullptr) sp[h] = make_uint4(pack2(f[0], f[1]), pack2(f[2], f[3]), pack2(f[4], f[5]), pack2(f[6], f[7]));
+  }
+}
+
 
 // CL = 2: thread-block cluster of two CTAs working on vertically adjacent tiles (same n-block).  Each CTA fetches
 // its own A tile and HALF of the shared B tile, multicasting that half into both CTAs' shared memory, which cuts
@@ -351,208 +387,21 @@ template <int BN, int CL, bool MN = false, bool BMN = MN>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   int M, int N, int K, GemmEpilogue ep) {
-  using C = Cfg<BN>;
-  const uint32_t crank = (CL == 2) ? cluster_ctarank() : 0u;
-  constexpr int kStages = C::kStages;
-  constexpr uint32_t kStageBytesA = C::kStageBytesA, kStageBytesB = C::kStageBytesB, kStageBytes = C::kStageBytes;
-  COLEARN_DYN_SMEM_UNALIGNED(uint8_t, smem_raw);
-  // SWIZZLE_128B operands need 1024-byte alignment
-  uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * kStageBytesA;
-  SharedBarriers* bars = reinterpret_cast<SharedBarriers*>(smem + kStages * kStageBytes);
-  float* staging = reinterpret_cast<float*>(smem + kStages * kStageBytes + 256);
+  constexpr int OPT = 0;
+#include "gemm_wgmma_body.inc"
+}
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int wg = threadIdx.x >> 7;
-  const int m_tiles = M / BM, n_tiles = N / BN, num_kb = K / BK;
-  // work unit = one tile (CL == 1) or a vertical pair of tiles handled by the two CTAs of a cluster (CL == 2)
-  const int m_units = m_tiles / CL;
-  // split-K (CL == 1 only): work unit = (output tile, K slice); slices of one tile are adjacent work units, so they
-  // run concurrently on different SMs and each stores a raw fp32 partial (see GemmEpilogue::split_k)
-  const int S = (CL == 1 && ep.split_k > 1) ? ep.split_k : 1;
-  const int total_work = m_units * n_tiles * S;
-  const int work0 = blockIdx.x / CL, work_stride = gridDim.x / CL;
-
-  if (warp == 0 && lane == 0) {
-    tmap_prefetch(&tmap_a);
-    tmap_prefetch(&tmap_b);
-    for (int i = 0; i < kStages; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], kConsumers * CL); }
-    fence_mbarrier_init();
-  }
-  __syncthreads();
-  if (CL == 2) cluster_sync_all();   // the peer may multicast into my smem / arrive on my barriers from now on
-  // programmatic dependent launch: everything above overlapped the predecessor's tail; nothing below may touch global
-  // memory before the grids this launch depends on have completed
-  if (ep.pdl) COLEARN_PDL_PROLOGUE();
-
-  if (wg == 0) {
-    // ===== TMA producer =====
-    set_max_regs<40>();
-    if (warp == 0 && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = work0; tile < total_work; tile += work_stride) {
-        int mu, nb;
-        work_to_tile(tile / S, m_units, n_tiles, mu, nb);
-        const int ks = tile % S;
-        const int kb_lo = split_kb(num_kb, ks, S), kb_hi = split_kb(num_kb, ks + 1, S);
-        const int m0 = (mu * CL + (int)crank) * BM, n0 = nb * BN;
-        if (ep.ready_flags != nullptr) {
-          const uint32_t want = ep.ready_epoch_ptr ? ld_acquire_sys(ep.ready_epoch_ptr) : ep.ready_epoch;
-          // wait for the peer-written weight rows [n0, n0+BN) of this round, then make them
-          // visible to the async proxy before TMA touches them
-          const int64_t c_lo = (ep.ready_elem_offset + (int64_t)n0 * K) / ep.ready_chunk_elems;
-          const int64_t c_hi = (ep.ready_elem_offset + (int64_t)(n0 + BN) * K - 1) / ep.ready_chunk_elems;
-          for (int64_t c = c_lo; c <= c_hi; ++c)
-            ready_wait_ge(ep.ready_flags + c, want);
-          if (ep.bias != nullptr) {  // the layer's fp32 bias directly follows its weight in the flat arena
-            const int64_t b_lo = (ep.ready_elem_offset + (int64_t)N * K + n0) / ep.ready_chunk_elems;
-            const int64_t b_hi = (ep.ready_elem_offset + (int64_t)N * K + n0 + BN - 1) / ep.ready_chunk_elems;
-            for (int64_t c = b_lo; c <= b_hi; ++c)
-              ready_wait_ge(ep.ready_flags + c, want);
-          }
-          fence_proxy_async();
-        }
-        for (int kb = kb_lo; kb < kb_hi; ++kb) {
-          mbar_wait(&bars->empty[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&bars->full[stage], kStageBytes);
-          if (CL == 1 && !MN && ep.conv.mode == 1) {
-            // implicit-GEMM convolution, forward / dgrad: the A tile is the activation box of this tap (conv_ops.cuh)
-            const convops::ConvBox bx = convops::conv_kblock(ep.conv, kb, m0, n0);
-            tma_load_4d(smem_a + stage * kStageBytesA, &tmap_a, bx.c, bx.w, bx.h, bx.n, &bars->full[stage]);
-            if (BMN) {
-              // dgrad against the packed weights Wp[co, (tap, ci)] themselves (MN-major B): the K index (co) runs over
-              // ROWS, the N index over the columns of this tap — the same two numbers with their roles swapped
-#pragma unroll
-              for (int j = 0; j < BN / 64; ++j)
-                tma_load_2d(smem_b + stage * kStageBytesB + j * kMnBoxBytes, &tmap_b, bx.b_row + j * 64, bx.b_col, &bars->full[stage]);
-            } else {
-              tma_load_2d(smem_b + stage * kStageBytesB, &tmap_b, bx.b_col, bx.b_row, &bars->full[stage]);
-            }
-            if (++stage == kStages) { stage = 0; phase ^= 1; }
-            continue;
-          }
-          if (MN) {
-#pragma unroll
-            for (int j = 0; j < BM / 64; ++j)
-              tma_load_2d(smem_a + stage * kStageBytesA + j * kMnBoxBytes, &tmap_a, m0 + j * 64, kb * BK, &bars->full[stage]);
-          } else {
-            tma_load_2d(smem_a + stage * kStageBytesA, &tmap_a, kb * BK, m0, &bars->full[stage]);
-          }
-          if (BMN && ep.conv.mode == 2) {
-            // implicit-GEMM convolution, wgrad: every 64-column block (tap, 64 channels) of the B tile is an activation box
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j) {
-              const convops::ConvBox bx = convops::conv_nblock(ep.conv, n0 / 64 + j, kb);
-              tma_load_4d(smem_b + stage * kStageBytesB + j * kMnBoxBytes, &tmap_b, bx.c, bx.w, bx.h, bx.n, &bars->full[stage]);
-            }
-          } else if (BMN) {
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j)
-              tma_load_2d(smem_b + stage * kStageBytesB + j * kMnBoxBytes, &tmap_b, n0 + j * 64, kb * BK, &bars->full[stage]);
-          } else if (CL == 2) {
-            // my half of the shared B tile -> both CTAs (tmap_b's box is BN/2 rows in this mode)
-            tma_load_2d_mcast(smem_b + stage * kStageBytesB + crank * (kStageBytesB / 2), &tmap_b, kb * BK,
-                              n0 + (int)crank * (BN / 2), &bars->full[stage], (uint16_t)0x3);
-          } else {
-            tma_load_2d(smem_b + stage * kStageBytesB, &tmap_b, kb * BK, n0, &bars->full[stage]);
-          }
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ===== consumer warpgroup g: tile rows [64 g, 64 g + 64) =====
-    set_max_regs<232>();
-    const int g = wg - 1;
-    const int t = threadIdx.x & 127, w = t >> 5;
-    const uint32_t mn_lbo = ep.mn_lbo ? (uint32_t)ep.mn_lbo : kMnBoxBytes, mn_sbo = ep.mn_sbo ? (uint32_t)ep.mn_sbo : 1024u;
-    float* stg = staging + g * 64 * kEpiStride;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = work0; tile < total_work; tile += work_stride) {
-      int mu, nb;
-      work_to_tile(tile / S, m_units, n_tiles, mu, nb);
-      const int m0 = (mu * CL + (int)crank) * BM, n0 = nb * BN;
-      const int ks = tile % S;
-      const int kb_lo = split_kb(num_kb, ks, S), kb_hi = split_kb(num_kb, ks + 1, S);
-      float acc[BN / 2];
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      int prev = -1;
-      for (int kb = kb_lo; kb < kb_hi; ++kb) {
-        mbar_wait(&bars->full[stage], phase);
-        // K-major operand: +16 bf16 = 32 bytes inside the 128B swizzle atom per wgmma K step (+2 in addr>>4 units);
-        // MN-major operand: +16 reduction rows = 16 lines of 128 bytes = two whole swizzle atoms (+128).  This
-        // warpgroup's 64 A rows start 8 KB into the stage in both layouts (64 K-major lines / the second 64-column box).
-        const uint32_t sa = smem_u32(smem_a + stage * kStageBytesA + g * 8192), sb = smem_u32(smem_b + stage * kStageBytesB);
-        const uint64_t da = MN ? make_smem_desc_mn(sa, mn_lbo, mn_sbo) : make_smem_desc(sa);
-        const uint64_t db = BMN ? make_smem_desc_mn(sb, mn_lbo, mn_sbo) : make_smem_desc(sb);
-        constexpr uint32_t kStepA = MN ? 128 : 2, kStepB = BMN ? 128 : 2;
-        acc_fence(acc);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / WG_K; ++k) wgmma_bf16<MN ? 1 : 0, BMN ? 1 : 0>(acc, da + kStepA * k, db + kStepB * k);
-        wgmma_commit();
-        acc_fence(acc);
-        // the previous stage's wgmmas have completed once at most this stage's group is in flight: release it
-        wgmma_wait<1>();
-        if (prev >= 0 && t == 0) {
-          for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&bars->empty[prev], (uint32_t)r);
-        }
-        prev = stage;
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      acc_fence(acc);
-      if (prev >= 0 && t == 0) {
-        for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&bars->empty[prev], (uint32_t)r);
-      }
-      // epilogue, 64 columns at a time: fragment -> staging (thread t holds rows 16 w + t%32/4 (+8), columns
-      // 8 i + 2 (t%4) (+1)), then warp w takes the 32-row half (w & 1) and the 32-column half (w >> 1) of the chunk
-      const int rl = (w & 1) * 32 + lane;
-      const int row = m0 + g * 64 + rl;
-      const int q = g * 2 + (w & 1);
-      // split-K: this work unit's raw accumulator goes to slice ks of the fp32 partial buffer
-      float* part = (S > 1) ? ep.split_out + ((size_t)ks * M + row) * N + n0 : nullptr;
-#pragma unroll
-      for (int c = 0; c < BN / 64; ++c) {
-        wg_bar_sync(1 + g);                           // the previous chunk's reads are done
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-#pragma unroll
-          for (int r = 0; r < 4; ++r)
-            stg[(16 * w + lane / 4 + 8 * (r >> 1)) * kEpiStride + 8 * i + 2 * (lane % 4) + (r & 1)] = acc[(8 * c + i) * 4 + r];
-        wg_bar_sync(1 + g);
-        const int c0 = c * 64 + (w >> 1) * 32;
-        uint32_t v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(stg[rl * kEpiStride + (w >> 1) * 32 + j]);
-        if (S > 1) {
-          float4* op = reinterpret_cast<float4*>(part + c0);
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            op[j] = make_float4(__uint_as_float(v[j * 4]), __uint_as_float(v[j * 4 + 1]), __uint_as_float(v[j * 4 + 2]),
-                                __uint_as_float(v[j * 4 + 3]));
-        } else {
-          epilogue_chunk(v, ep, row, n0 + c0, lane, q, m0, M, N);
-        }
-      }
-      // fused wgrad -> FedAvg reduce: this warpgroup's 64 x BN block of the master matrix is final (the barrier orders
-      // the 128 threads' stores before thread 0's fence)
-      if (ep.produced != nullptr) {
-        wg_bar_sync(1 + g);
-        if (t == 0) {
-          __threadfence_system();
-          produced_block(ep.produced, ep.produced_elem_offset, m0 + g * 64, 64, N, n0, BN);
-        }
-      }
-    }
-  }
-
-  __syncthreads();
-  if (CL == 2) cluster_sync_all();   // nobody may still multicast into / arrive on a CTA that exits
+// The wgrad dW = dz^T a of the layer-wise trainer with the local-optimizer epilogue (epilogue_opt_chunk): 1-CTA, both
+// operands K-major (MN = false: the transposed copies dz^T, a^T) or both MN-major (MN = true: dz and a read in place).
+// OPT = LOCAL_OPT_SGD or LOCAL_OPT_ADAM.  Same body as gemm_wgmma_kernel; only these instances read ep.lopt.
+template <int BN, bool MN, int OPT_>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_wgmma_opt_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                      int M, int N, int K, GemmEpilogue ep) {
+  constexpr int CL = 1;
+  constexpr bool BMN = MN;
+  constexpr int OPT = OPT_;
+#include "gemm_wgmma_body.inc"
 }
 
 // ---- host side: tensor maps ---------------------------------------------------------------------------
@@ -754,6 +603,61 @@ cudaError_t launch_mn(const void* A, int a_cols, const void* B, int b_rows, int 
   return launch_1cta(gemm_wgmma_kernel<BN, 1, AMN, true>, units, C::kSmemBytes, s, ta, tb, M, N, K, ep);
 }
 
+// gemm_wgmma_opt_kernel: MN = false: A [M, K], B [N, K]; MN = true: A [K, a_cols], B [K, N] (as launch_mn with a_mn = 1)
+template <int BN, bool MN, int OPT>
+cudaError_t launch_opt_t(const void* A, int a_cols, const void* B, int M, int N, int K, const GemmEpilogue& ep, cudaStream_t s) {
+  using C = Cfg<BN>;
+  CUtensorMap ta, tb;
+  if (!(MN ? make_tmap(A, K, a_cols, 64, &ta) && make_tmap(B, K, N, 64, &tb) : make_tmap(A, M, K, BM, &ta) && make_tmap(B, N, K, BN, &tb)))
+    return cudaErrorInvalidValue;
+  static bool configured[64] = {false};
+  static int num_sms[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (!configured[dev & 63]) {
+    cudaError_t e = configure_smem(reinterpret_cast<const void*>(gemm_wgmma_opt_kernel<BN, MN, OPT>), C::kSmemBytes, dev);
+    if (e != cudaSuccess) { g_last_error = "cudaFuncSetAttribute(smem, local optimizer) failed"; return e; }
+    cudaDeviceGetAttribute(&num_sms[dev & 63], cudaDevAttrMultiProcessorCount, dev);
+    configured[dev & 63] = true;
+  }
+  const int work = (M / BM) * (N / BN);
+  int units = num_sms[dev & 63];
+  if (ep.max_ctas > 0 && ep.max_ctas < units) units = ep.max_ctas;
+  if (work < units) units = work;
+  if (units < 1) units = 1;
+  return launch_1cta(gemm_wgmma_opt_kernel<BN, MN, OPT>, units, C::kSmemBytes, s, ta, tb, M, N, K, ep);
+}
+
+// The local-optimizer epilogue (ep.lopt.args.kind != 0) is the fused-SGD wgrad with another update: it takes sgd_master,
+// sgd_lr, sgd_shadow and the moments, and nothing else.  The tile width follows the rule of the plain launchers (so that it
+// walks the tiles the fused-SGD wgrad of the same layer walks).
+cudaError_t launch_opt(const void* A, bool mn, int a_cols, const void* B, int M, int N, int K, const GemmEpilogue& ep, cudaStream_t s) {
+  const LocalOptArgs& o = ep.lopt.args;
+  const char* why = nullptr;
+  if (o.kind != LOCAL_OPT_SGD && o.kind != LOCAL_OPT_ADAM) why = "local optimizer: kind must be LOCAL_OPT_SGD or LOCAL_OPT_ADAM";
+  else if (ep.split_k > 1 || ep.cluster != 0 || ep.ready_flags != nullptr || ep.produced != nullptr || ep.colsum != nullptr ||
+           ep.out_f32 != nullptr || ep.out_bf16 != nullptr || ep.out_bf16_t != nullptr || ep.conv.mode != 0)
+    why = "local optimizer epilogue: no split_k, cluster, ready_flags, produced, colsum, out_* or conv";
+  else if (ep.bias != nullptr || ep.relu || ep.relu_mask != nullptr || ep.addend != nullptr || ep.sgd_shadow_t != nullptr)
+    why = "local optimizer epilogue: no bias, relu, relu_mask, addend or sgd_shadow_t (it is the wgrad's update)";
+  else if (ep.sgd_master == nullptr || ((o.kind == LOCAL_OPT_ADAM || o.momentum != 0.f) && ep.lopt.m == nullptr) ||
+           (o.kind == LOCAL_OPT_ADAM && ep.lopt.v == nullptr))
+    why = "local optimizer epilogue: needs sgd_master, m (momentum / Adam) and v (Adam)";
+  else if ((((uintptr_t)ep.sgd_master) | ((uintptr_t)ep.lopt.m) | ((uintptr_t)ep.lopt.v) | ((uintptr_t)ep.sgd_shadow)) & 15)
+    why = "local optimizer epilogue: master, m, v and shadow must be 16-byte aligned";
+  else if (ep.tile_n == 256 && (N % 256))
+    why = "tile_n=256 needs N%256==0";
+  if (why != nullptr) { g_last_error = why; return cudaErrorInvalidValue; }
+  const bool adam = o.kind == LOCAL_OPT_ADAM;
+  const bool wide = (N % 256 == 0) && ep.tile_n != 128 && (ep.tile_n == 256 || (int64_t)(M / BM) * (N / 256) >= 120);
+  if (mn) {
+    if (wide) return adam ? launch_opt_t<256, true, LOCAL_OPT_ADAM>(A, a_cols, B, M, N, K, ep, s) : launch_opt_t<256, true, LOCAL_OPT_SGD>(A, a_cols, B, M, N, K, ep, s);
+    return adam ? launch_opt_t<128, true, LOCAL_OPT_ADAM>(A, a_cols, B, M, N, K, ep, s) : launch_opt_t<128, true, LOCAL_OPT_SGD>(A, a_cols, B, M, N, K, ep, s);
+  }
+  if (wide) return adam ? launch_opt_t<256, false, LOCAL_OPT_ADAM>(A, 0, B, M, N, K, ep, s) : launch_opt_t<256, false, LOCAL_OPT_SGD>(A, 0, B, M, N, K, ep, s);
+  return adam ? launch_opt_t<128, false, LOCAL_OPT_ADAM>(A, 0, B, M, N, K, ep, s) : launch_opt_t<128, false, LOCAL_OPT_SGD>(A, 0, B, M, N, K, ep, s);
+}
+
 }  // namespace
 
 const char* gemm_tcgen05_last_error() { return g_last_error.c_str(); }
@@ -812,6 +716,7 @@ cudaError_t launch_gemm_tcgen05_conv(const void* act, int n_images, int H, int W
   }
   if ((((uintptr_t)act) | ((uintptr_t)other)) & 15) { g_last_error = "operands must be 16-byte aligned"; return cudaErrorInvalidValue; }
   if (ep.cluster != 0 || ep.ready_flags != nullptr) { g_last_error = "implicit conv GEMM has no cluster / ready-flag variant"; return cudaErrorInvalidValue; }
+  if (ep.lopt.args.kind != 0) { g_last_error = "implicit conv GEMM has no local-optimizer epilogue"; return cudaErrorInvalidValue; }
   if (g.mode == 1) {
     // M = pixels (whole images per 128-row tile), K = taps * C
     if (M != n_images * HW || K != g.KH * g.KW * g.C) { g_last_error = "implicit conv GEMM (A): M = N*H*W, K = KH*KW*C"; return cudaErrorInvalidValue; }
@@ -871,6 +776,10 @@ cudaError_t launch_gemm_tcgen05_mn(const void* A, int a_mn, int a_cols, const vo
   }
   if ((((uintptr_t)A) | ((uintptr_t)B)) & 15) { g_last_error = "operands must be 16-byte aligned"; return cudaErrorInvalidValue; }
   if (ep.cluster != 0 || ep.ready_flags != nullptr) { g_last_error = "mn-major mode has no cluster / ready-flag variant"; return cudaErrorInvalidValue; }
+  if (ep.lopt.args.kind != 0) {
+    if (!a_mn) { g_last_error = "local optimizer epilogue: the mn-major form is the wgrad's (a_mn = 1)"; return cudaErrorInvalidValue; }
+    return launch_opt(A, true, a_cols, B, M, N, K, ep, s);
+  }
   if (ep.split_k > 1) {
     if (ep.split_out == nullptr || K / BK < ep.split_k || (((uintptr_t)ep.split_out) & 15)) {
       g_last_error = "split_k needs a 16-byte aligned split_out and K/64 >= split_k";
@@ -898,6 +807,7 @@ cudaError_t launch_gemm_tcgen05(const void* A, const void* B, int M, int N, int 
     return cudaErrorInvalidValue;
   }
   if ((((uintptr_t)A) | ((uintptr_t)B)) & 15) { g_last_error = "operands must be 16-byte aligned"; return cudaErrorInvalidValue; }
+  if (ep.lopt.args.kind != 0) return launch_opt(A, false, 0, B, M, N, K, ep, s);
   if (ep.produced != nullptr && (ep.sgd_master == nullptr || ep.split_k > 1)) {
     g_last_error = "produced reports come from the fused-SGD epilogue (needs sgd_master, no split_k)";
     return cudaErrorInvalidValue;

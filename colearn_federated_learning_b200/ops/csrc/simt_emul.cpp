@@ -601,11 +601,11 @@ void produced_mark(int64_t sig, int64_t chunk_elems, int64_t lo, int64_t hi) {
 
 // ---- gemm_wgmma.cu on the functional wgmma / TMA / mbarrier model (gemm_host_model.h) -------------------------------------
 // Same argument meaning as bindings.cpp::gemm_tcgen05 (minus the cross-GPU ready flags and the cluster modes).
-void gemm_tcgen05(Tensor A, Tensor B, c10::optional<Tensor> bias, bool relu, c10::optional<Tensor> relu_mask, c10::optional<Tensor> out_bf16,
-                  c10::optional<Tensor> out_f32, c10::optional<Tensor> out_bf16_t, c10::optional<Tensor> sgd_master, double sgd_lr,
-                  c10::optional<Tensor> sgd_shadow, c10::optional<Tensor> sgd_shadow_t, c10::optional<Tensor> colsum, int64_t tile_n,
-                  int64_t split_k, c10::optional<Tensor> split_out, int64_t mn_m, bool b_kn, c10::optional<Tensor> addend,
-                  std::vector<int64_t> conv, std::vector<int64_t> produced) {
+static void gemm_run(Tensor A, Tensor B, c10::optional<Tensor> bias, bool relu, c10::optional<Tensor> relu_mask, c10::optional<Tensor> out_bf16,
+                     c10::optional<Tensor> out_f32, c10::optional<Tensor> out_bf16_t, c10::optional<Tensor> sgd_master, double sgd_lr,
+                     c10::optional<Tensor> sgd_shadow, c10::optional<Tensor> sgd_shadow_t, c10::optional<Tensor> colsum, int64_t tile_n,
+                     int64_t split_k, c10::optional<Tensor> split_out, int64_t mn_m, bool b_kn, c10::optional<Tensor> addend,
+                     std::vector<int64_t> conv, std::vector<int64_t> produced, const colearn::GemmOptEpilogue* lopt) {
   TORCH_CHECK(!A.is_cuda() && !B.is_cuda() && A.scalar_type() == at::kBFloat16 && B.scalar_type() == at::kBFloat16 && A.is_contiguous() &&
               B.is_contiguous() && A.dim() == 2 && B.dim() == 2, "A, B: contiguous CPU bf16 matrices");
   const bool mn = mn_m > 0, is_conv = !conv.empty();
@@ -632,6 +632,7 @@ void gemm_tcgen05(Tensor A, Tensor B, c10::optional<Tensor> bias, bool relu, c10
   ep.sgd_shadow_t = ptr(sgd_shadow_t, at::kBFloat16, (int64_t)M * N, "sgd_shadow_t");
   ep.colsum = (float*)ptr(colsum, at::kFloat, (int64_t)(M / 32) * N, "colsum");
   ep.addend = ptr(addend, at::kBFloat16, (int64_t)M * N, "addend");
+  if (lopt != nullptr) ep.lopt = *lopt;
   ep.ready_chunk_elems = 1;
   ep.tile_n = (int)tile_n;
   if (!produced.empty()) {
@@ -662,6 +663,65 @@ void gemm_tcgen05(Tensor A, Tensor B, c10::optional<Tensor> bias, bool relu, c10
   }
   TORCH_CHECK(e == cudaSuccess, "gemm_tcgen05 (host model): ", colearn::gemm_tcgen05_last_error());
 }
+void gemm_tcgen05(Tensor A, Tensor B, c10::optional<Tensor> bias, bool relu, c10::optional<Tensor> relu_mask, c10::optional<Tensor> out_bf16,
+                  c10::optional<Tensor> out_f32, c10::optional<Tensor> out_bf16_t, c10::optional<Tensor> sgd_master, double sgd_lr,
+                  c10::optional<Tensor> sgd_shadow, c10::optional<Tensor> sgd_shadow_t, c10::optional<Tensor> colsum, int64_t tile_n,
+                  int64_t split_k, c10::optional<Tensor> split_out, int64_t mn_m, bool b_kn, c10::optional<Tensor> addend,
+                  std::vector<int64_t> conv, std::vector<int64_t> produced) {
+  gemm_run(A, B, bias, relu, relu_mask, out_bf16, out_f32, out_bf16_t, sgd_master, sgd_lr, sgd_shadow, sgd_shadow_t, colsum, tile_n, split_k,
+           split_out, mn_m, b_kn, addend, conv, produced, nullptr);
+}
+
+// the local optimizer of the layer-wise trainer (bindings.cpp): opt = {kind, nesterov, momentum, weight_decay, beta1, beta2, eps},
+// step = {t, p1, p2, s, r}; m / v: fp32 with the parameter's sizes and strides, None where the optimizer keeps none
+static colearn::LocalOptArgs local_opt_args(const std::vector<double>& o) {
+  TORCH_CHECK(o.size() == 7, "local optimizer: 7 values");
+  TORCH_CHECK((int)o[0] == colearn::LOCAL_OPT_SGD || (int)o[0] == colearn::LOCAL_OPT_ADAM, "local optimizer: unknown kind");
+  return colearn::LocalOptArgs{(int)o[0], (int)o[1], (float)o[2], (float)o[3], (float)o[4], (float)o[5], (float)o[6]};
+}
+static colearn::LocalOptStep local_opt_step_of(const std::vector<double>& step) {
+  TORCH_CHECK(step.size() == 5 && step[0] >= 1, "local optimizer step: {t >= 1, p1, p2, s, r}");
+  colearn::LocalOptStep st;
+  st.t = (int)step[0]; st.p1 = (float)step[1]; st.p2 = (float)step[2]; st.s = (float)step[3]; st.r = (float)step[4];
+  return st;
+}
+static float* local_opt_moment(const c10::optional<Tensor>& t, const Tensor& param, bool needed, const char* name) {
+  TORCH_CHECK(t.has_value() || !needed, name, ": this optimizer keeps it, pass the buffer");
+  if (!t.has_value()) return nullptr;
+  TORCH_CHECK(!t->is_cuda() && t->scalar_type() == at::kFloat && t->sizes() == param.sizes() && t->strides() == param.strides(),
+              name, ": CPU fp32 with the parameter's sizes and strides");
+  return t->data_ptr<float>();
+}
+void gemm_tcgen05_opt(Tensor A, Tensor B, c10::optional<Tensor> bias, bool relu, c10::optional<Tensor> relu_mask, c10::optional<Tensor> out_bf16,
+                      c10::optional<Tensor> out_f32, c10::optional<Tensor> out_bf16_t, c10::optional<Tensor> sgd_master, double sgd_lr,
+                      c10::optional<Tensor> sgd_shadow, c10::optional<Tensor> sgd_shadow_t, c10::optional<Tensor> colsum, int64_t tile_n,
+                      int64_t split_k, c10::optional<Tensor> split_out, int64_t mn_m, bool b_kn, c10::optional<Tensor> addend,
+                      std::vector<int64_t> conv, std::vector<int64_t> produced, c10::optional<Tensor> m, c10::optional<Tensor> v,
+                      std::vector<double> opt, std::vector<double> step) {
+  TORCH_CHECK(sgd_master.has_value(), "the local optimizer epilogue updates sgd_master");
+  colearn::GemmOptEpilogue lo;
+  memset(&lo, 0, sizeof(lo));
+  lo.args = local_opt_args(opt);
+  lo.step = local_opt_step_of(step);
+  lo.m = local_opt_moment(m, *sgd_master, lo.args.kind == colearn::LOCAL_OPT_ADAM || lo.args.momentum != 0.f, "m");
+  lo.v = local_opt_moment(v, *sgd_master, lo.args.kind == colearn::LOCAL_OPT_ADAM, "v");
+  gemm_run(A, B, bias, relu, relu_mask, out_bf16, out_f32, out_bf16_t, sgd_master, sgd_lr, sgd_shadow, sgd_shadow_t, colsum, tile_n, split_k,
+           split_out, mn_m, b_kn, addend, conv, produced, &lo);
+}
+// local_opt_apply_kernel of elementwise.cu (bindings.cpp::local_opt_apply)
+void local_opt_apply(Tensor theta, Tensor grad, int64_t g_rows, c10::optional<Tensor> m, c10::optional<Tensor> v, double lr,
+                     std::vector<double> opt, std::vector<double> step) {
+  TORCH_CHECK(!theta.is_cuda() && theta.scalar_type() == at::kFloat && theta.dim() == 2 && theta.stride(1) == 1, "theta: CPU fp32 [rows, cols]");
+  TORCH_CHECK(!grad.is_cuda() && grad.scalar_type() == at::kFloat && grad.dim() == 2 && grad.stride(1) == 1 && g_rows >= 1 &&
+              grad.size(0) == theta.size(0) * g_rows && grad.size(1) >= theta.size(1), "grad: CPU fp32 [rows * g_rows, >= cols]");
+  const colearn::LocalOptArgs a = local_opt_args(opt);
+  float* mp = local_opt_moment(m, theta, a.kind == colearn::LOCAL_OPT_ADAM || a.momentum != 0.f, "m");
+  float* vp = local_opt_moment(v, theta, a.kind == colearn::LOCAL_OPT_ADAM, "v");
+  const colearn::LocalOptStep st = local_opt_step_of(step);
+  py::gil_scoped_release nogil;
+  CK(colearn::launch_local_opt_apply(theta.data_ptr<float>(), theta.stride(0), grad.data_ptr<float>(), grad.stride(0), (int)g_rows, mp, vp,
+                                     (int)theta.size(0), (int)theta.size(1), a, st, (float)lr, nullptr));
+}
 
 // ---- convnet.cu: the launchers themselves (grid mapping, two-phase blocks, the ticket-counter BatchNorm reduction) behind the
 // torch-facing wrappers of conv_bindings.inc — a third instantiation next to the GPU one and the body emulator ----------------
@@ -690,6 +750,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "the CUDA kernels of mlp_persistent.cu / elementwise.cu / comm.cu / convnet.cu compiled for the CPU through a SIMT shim (tests only)";
   convbind::register_ops<ConvSimtExec>(m);
   m.def("gemm_tcgen05", &gemm_tcgen05);
+  m.def("gemm_tcgen05_opt", &gemm_tcgen05_opt);
+  m.def("local_opt_apply", &local_opt_apply);
   m.def("mlp_local_sgd", &mlp_local_sgd, py::arg("net_kind"), py::arg("theta_in"), py::arg("theta_outs"), py::arg("xs"), py::arg("ys"), py::arg("perms"),
         py::arg("batch_size"), py::arg("epochs"), py::arg("max_steps"), py::arg("loss"), py::arg("lr"), py::arg("variant"), py::arg("out_scales"),
         py::arg("delta_mode"), py::arg("flags"), py::arg("perm_seed") = 0, py::arg("perm_row0") = 0, py::arg("perm_scratch") = py::none());

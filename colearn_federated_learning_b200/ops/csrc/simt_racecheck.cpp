@@ -335,6 +335,17 @@ int main() {
       std::vector<__nv_bfloat16> shadow((size_t)M * N);
       memset(&ep, 0, sizeof(ep)); ep.ready_chunk_elems = 1; ep.sgd_master = master.data(); ep.sgd_lr = 0.1f; ep.sgd_shadow = shadow.data();
       CK(launch_gemm_tcgen05_mn(a.data(), 1, ac, b.data(), Kd, M, N, Kd, ep, nullptr));
+      // the same wgrad with the local-optimizer epilogue (Adam: master, m, v and the shadow per element), then its apply kernel
+      // on a strided block with bias-style partial rows
+      std::vector<float> m((size_t)M * N, 0.f), v((size_t)M * N, 0.f);
+      ep.lopt.args = LocalOptArgs{LOCAL_OPT_ADAM, 0, 0.f, 0.01f, 0.9f, 0.999f, 1e-8f};
+      ep.lopt.step = local_opt_start();
+      local_opt_next(ep.lopt.step, ep.lopt.args, 0.1f);
+      ep.lopt.m = m.data(); ep.lopt.v = v.data();
+      CK(launch_gemm_tcgen05_mn(a.data(), 1, ac, b.data(), Kd, M, N, Kd, ep, nullptr));
+      std::vector<float> partials((size_t)2 * 64 * N, 0.25f);
+      CK(launch_local_opt_apply(master.data(), N, partials.data(), N, 2, m.data(), v.data(), 64, 300, ep.lopt.args, ep.lopt.step, 0.1f,
+                                nullptr));
     }
     // implicit-GEMM forward: 4 images of 8x8, 64 -> 64 channels
     {

@@ -11,7 +11,7 @@ from typing import Optional
 
 import torch
 
-from . import _ext
+from . import _ext, reference
 
 
 def gemm_bf16(a: torch.Tensor, b: torch.Tensor, *, bias: Optional[torch.Tensor] = None, relu: bool = False,
@@ -23,7 +23,7 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, *, bias: Optional[torch.Tensor] 
               ready_chunk_elems: int = 1, ready_elem_offset: int = 0, tile_n: int = 0,
               ready_epoch_ptr: int = 0, cluster: int = 0, split_k: int = 0,
               split_out: Optional[torch.Tensor] = None, mn_m: int = 0, b_kn: bool = False,
-              addend: Optional[torch.Tensor] = None, produced=None, max_ctas: int = 0) -> None:
+              addend: Optional[torch.Tensor] = None, produced=None, max_ctas: int = 0, opt=None) -> None:
     """Launch the wgmma GEMM; results land in the provided output tensors.
 
     ``mn_m = M > 0`` selects the "MN-major" form ``C[M, N] = Aᵀ·B`` for ``a[K, a_cols]`` (``a_cols <= M``, the missing
@@ -43,7 +43,13 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, *, bias: Optional[torch.Tensor] 
     ``elem_offset``): fused wgrad → FedAvg reduce — each epilogue warp reports the block of final parameters it wrote
     (``ops.produced``), and ``ProducedSpec.max_ctas`` caps the persistent grid so that the overlapped two-shot kernel
     keeps its SMs; ``max_ctas`` alone caps the grid of a GEMM that only runs next to that kernel (the dgrads of the
-    last backward)."""
+    last backward).
+
+    ``opt = (LocalOpt, state, m, v)`` (``fl/local_opt.py``; not plain SGD): the fused-SGD wgrad with the local optimizer's step
+    instead of ``master -= lr * acc`` (``gemm_wgmma_opt_kernel``).  ``state`` holds this step's scalars, already advanced by
+    ``reference.local_opt_next``; ``m`` / ``v`` are fp32 like ``sgd_master`` (None where the optimizer keeps none) and are
+    updated in place.  It takes ``sgd_master``, ``sgd_lr``, ``sgd_shadow``, ``tile_n`` and ``mn_m`` and no other option; dW is
+    never stored.  CPU tensors: the fp32 product, then ``reference.local_opt_apply``."""
     prod_arg = [0, 0, int(max_ctas)] if max_ctas else []
     if produced is not None:
         assert sgd_master is not None and not (split_k and split_k > 1), "produced reports come from the fused-SGD epilogue"
@@ -71,6 +77,16 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, *, bias: Optional[torch.Tensor] 
         assert (bias is None and not relu and relu_mask is None and out_bf16 is None and out_f32 is None and out_bf16_t is None
                 and sgd_master is None and colsum is None and not ready_flags and addend is None), "split-K stores raw partials only"
         assert k_red // 64 >= split_k, "split_k must not exceed K/64"
+    opt_arg = []
+    if opt is not None:
+        lo, state, m, v = opt
+        assert sgd_master is not None, "the local optimizer epilogue updates sgd_master"
+        opt_arg = [m, v, lo.launch_args(), reference.local_opt_scalars(state)]
+    if simt_mod is not None and opt is not None:
+        simt_mod.gemm_tcgen05_opt(a.contiguous(), b.contiguous(), bias, bool(relu), relu_mask, out_bf16, out_f32, out_bf16_t, sgd_master,
+                                  float(sgd_lr), sgd_shadow, sgd_shadow_t, colsum, int(tile_n), int(split_k or 0), split_out, int(mn_m or 0),
+                                  bool(b_kn), addend, [], prod_arg, *opt_arg)
+        return
     if simt_mod is not None:
         simt_mod.gemm_tcgen05(a.contiguous(), b.contiguous(), bias, bool(relu), relu_mask, out_bf16, out_f32, out_bf16_t, sgd_master,
                               float(sgd_lr), sgd_shadow, sgd_shadow_t, colsum, int(tile_n), int(split_k or 0), split_out, int(mn_m or 0),
@@ -95,6 +111,11 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, *, bias: Optional[torch.Tensor] 
             acc = acc + addend.float()
         if colsum is not None:   # [M/32, N] per-32-row-block partial column sums
             colsum.copy_(acc.view(acc.shape[0] // 32, 32, acc.shape[1]).sum(1))
+        if opt is not None:
+            reference.local_opt_apply(sgd_master, acc, lo, sgd_lr, state, m, v)
+            if sgd_shadow is not None:
+                sgd_shadow.copy_(sgd_master)
+            return
         if sgd_master is not None:
             sgd_master.sub_(sgd_lr * acc)
             if sgd_shadow is not None:
@@ -110,6 +131,12 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, *, bias: Optional[torch.Tensor] 
             out_bf16.copy_(acc)
         if out_bf16_t is not None:
             out_bf16_t.copy_(acc.t())
+        return
+    if opt is not None:
+        _ext.require().gemm_tcgen05_opt(a, b, bias, bool(relu), relu_mask, out_bf16, out_f32, out_bf16_t, sgd_master,
+                                        float(sgd_lr), sgd_shadow, sgd_shadow_t, colsum, int(ready_flags), int(ready_epoch),
+                                        int(ready_chunk_elems), int(ready_elem_offset), int(tile_n), int(ready_epoch_ptr), int(cluster),
+                                        int(split_k or 0), split_out, int(mn_m or 0), bool(b_kn), addend, [], prod_arg, *opt_arg)
         return
     _ext.require().gemm_tcgen05(a, b, bias, bool(relu), relu_mask, out_bf16, out_f32, out_bf16_t, sgd_master,
                                 float(sgd_lr), sgd_shadow, sgd_shadow_t, colsum, int(ready_flags), int(ready_epoch),
@@ -149,3 +176,26 @@ def bias_sgd_from_partials(bias: Optional[torch.Tensor], partials: torch.Tensor,
             bias.sub_(g[: bias.numel()], alpha=lr)
         return g
     return _ext.require().bias_sgd_from_partials(bias, partials.contiguous(), float(lr))
+
+
+def local_opt_apply(theta: torch.Tensor, grad: torch.Tensor, opt, lr: float, g_rows: int = 1) -> torch.Tensor:
+    """The local optimizer's step on a parameter block in place (the layer-wise trainer's padded edge layers and biases):
+    ``theta [rows, cols]`` (unit column stride, any row stride) takes ``reference.local_opt_apply`` with the gradient
+    ``sum_{p < g_rows} grad[r * g_rows + p, :cols]``, the rows added in order from 0 as ``bias_sgd_from_partials`` does.  ``opt``
+    as in :func:`gemm_bf16`; ``m`` / ``v`` have the sizes and strides of ``theta``.  CUDA tensors: ``local_opt_apply_kernel``;
+    CPU tensors: the SIMT build inside ``ops.conv.simt()``, else the PyTorch definition."""
+    lo, state, m, v = opt
+    from . import conv as _conv
+    simt_mod = (_conv._EMUL["mod"] if (not theta.is_cuda and _conv._EMUL["on"] and hasattr(_conv._EMUL["mod"], "local_opt_apply"))
+                else None)
+    if theta.is_cuda or simt_mod is not None:
+        mod = _ext.require() if theta.is_cuda else simt_mod
+        mod.local_opt_apply(theta, grad, int(g_rows), m, v, float(lr), lo.launch_args(), reference.local_opt_scalars(state))
+        return theta
+    rows, cols = theta.shape
+    g = torch.zeros(rows, cols, dtype=theta.dtype)
+    gv = grad[:, :cols].reshape(rows, int(g_rows), cols)
+    for p in range(int(g_rows)):
+        g = g + gv[:, p]
+    reference.local_opt_apply(theta, g, lo, lr, state, m, v)
+    return theta

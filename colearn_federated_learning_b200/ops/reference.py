@@ -151,40 +151,68 @@ def _sqrt_rn(t: torch.Tensor) -> torch.Tensor:
     return torch.sqrt(t.double()).float() if t.dtype == torch.float32 else torch.sqrt(t)
 
 
+def local_opt_clock(dtype: torch.dtype = torch.float32) -> dict:
+    """The per-step scalars of a fresh fit (``LocalOptStep`` of ``csrc/local_opt.cuh``): step count 0, Adam's running products 1,
+    ``s`` 0 and ``r`` 1, in ``dtype``"""
+    one = torch.ones((), dtype=dtype)
+    return {"t": 0, "p1": one, "p2": one.clone(), "s": torch.zeros((), dtype=dtype), "r": one.clone()}
+
+
 def local_opt_state(flat: torch.Tensor) -> dict:
-    """Fresh state of a local optimizer for one fit: step count 0, moments 0, Adam's running products 1"""
-    one = torch.ones((), dtype=flat.dtype)
-    return {"t": 0, "m": torch.zeros_like(flat), "v": torch.zeros_like(flat), "p1": one, "p2": one.clone()}
+    """Fresh state of a local optimizer for one fit: the scalars of :func:`local_opt_clock` in ``flat``'s dtype, moments 0"""
+    return {**local_opt_clock(flat.dtype), "m": torch.zeros_like(flat), "v": torch.zeros_like(flat)}
 
 
-def local_opt_step(flat: torch.Tensor, g: torch.Tensor, local_opt, lr: float, state: dict) -> None:
-    """One step of a local optimizer (``fl/local_opt.py``) on ``flat`` in place, from the batch gradient ``g``: the
-    operation order of ``csrc/local_opt.cuh``, one rounding per operation in ``flat``'s dtype (every scalar is cast to it
-    first)."""
-    dt = flat.dtype
+def local_opt_next(state: dict, local_opt, lr: float) -> None:
+    """Advance the per-step scalars to the next step (``local_opt_next`` of ``csrc/local_opt.cuh``): ``t``, and for Adam
+    ``p1 = p1 * b1``, ``p2 = p2 * b2``, ``s = lr / (1 - p1)``, ``r = sqrt(1 - p2)``, one rounding per operation in the
+    scalars' dtype.  The layer-wise trainer runs this once per step on the host and passes the values to its kernels."""
+    dt = state["p1"].dtype
     c = lambda v: torch.tensor(v, dtype=torch.float32).to(dt)            # noqa: E731  the fp32 hyper-parameter the kernel holds
-    lr_t = c(lr)
     state["t"] += 1
+    if local_opt.kind == "Adam":
+        one = torch.ones((), dtype=dt)
+        state["p1"] = state["p1"] * c(local_opt.betas[0])
+        state["p2"] = state["p2"] * c(local_opt.betas[1])
+        state["s"] = c(lr) / (one - state["p1"])
+        state["r"] = _sqrt_rn(one - state["p2"])
+
+
+def local_opt_scalars(state: dict) -> List[float]:
+    """``[t, p1, p2, s, r]``: the ``LocalOptStep`` the bindings take (float32 values are exact as Python floats)"""
+    return [float(state["t"])] + [float(state[k]) for k in ("p1", "p2", "s", "r")]
+
+
+def local_opt_apply(theta: torch.Tensor, g: torch.Tensor, local_opt, lr: float, state: dict, m: Optional[torch.Tensor],
+                    v: Optional[torch.Tensor]) -> None:
+    """The per-element step of ``csrc/local_opt.cuh`` (``local_opt_elem``) on ``theta`` in place, from the gradient ``g``, with the
+    step scalars of ``state`` (already advanced by :func:`local_opt_next`) and the moments ``m`` / ``v`` (updated in place; None
+    where the optimizer keeps none)."""
+    dt = theta.dtype
+    c = lambda v_: torch.tensor(v_, dtype=torch.float32).to(dt)          # noqa: E731
     if local_opt.weight_decay != 0.0:
-        g = g + c(local_opt.weight_decay) * flat
-    m, v = state["m"], state["v"]
+        g = g + c(local_opt.weight_decay) * theta
     if local_opt.kind == "Adam":
         b1, b2 = c(local_opt.betas[0]), c(local_opt.betas[1])
         one = torch.ones((), dtype=dt)
-        state["p1"] = state["p1"] * b1
-        state["p2"] = state["p2"] * b2
-        s = lr_t / (one - state["p1"])
-        r = _sqrt_rn(one - state["p2"])
         m.copy_(b1 * m + (one - b1) * g)
         v.copy_(b2 * v + (one - b2) * (g * g))
-        flat.copy_(flat - (s * m) / (_sqrt_rn(v) / r + c(local_opt.eps)))
+        theta.copy_(theta - (state["s"] * m) / (_sqrt_rn(v) / state["r"] + c(local_opt.eps)))
         return
     d = g
     if local_opt.momentum != 0.0:
         mu = c(local_opt.momentum)
         m.copy_(g if state["t"] == 1 else mu * m + g)
         d = g + mu * m if local_opt.nesterov else m
-    flat.copy_(flat - lr_t * d)
+    theta.copy_(theta - c(lr) * d)
+
+
+def local_opt_step(flat: torch.Tensor, g: torch.Tensor, local_opt, lr: float, state: dict) -> None:
+    """One step of a local optimizer (``fl/local_opt.py``) on ``flat`` in place, from the batch gradient ``g``: the
+    operation order of ``csrc/local_opt.cuh``, one rounding per operation in ``flat``'s dtype (every scalar is cast to it
+    first).  :func:`local_opt_next`, then :func:`local_opt_apply` with the moments of ``state``."""
+    local_opt_next(state, local_opt, lr)
+    local_opt_apply(flat, g, local_opt, lr, state, state["m"], state["v"])
 
 
 def mlp_local_sgd(flat: torch.Tensor, dims: Sequence[int], x: torch.Tensor, y: torch.Tensor,
